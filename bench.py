@@ -27,6 +27,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import time
 
 import numpy as np
@@ -38,14 +39,6 @@ if ROOT not in sys.path:
 METRIC = "candidate-evals/sec (GP+sort+HV) pop=65536 dim=30 obj=3"
 UNIT = "candidates/s"
 REF_DIR = os.environ.get("DMOSOPT_REF") or os.path.join(ROOT, "baseline", "_ref")
-
-# DRAM bytes of one gp_var launch from the committed `ncu --set full` captures (profiles/), keyed by
-# (kernel version, pop, d, M, N); null for anything else -- the number is not re-measured inside the timed run
-# (a run under ncu is never a bench value).
-NCU_TRAFFIC = {
-    ("v3", 65536, 30, 3, 4096): ("profiles/r2_gp_var_tc3_kernel_details.txt", 5.134091e9 + 16.331008e6),
-    ("v2", 65536, 30, 3, 4096): ("profiles/r1_gp_var_tc2_kernel_details.txt", 22.553779e9 + 7.566592e6),
-}
 
 
 def workload(pop, d, M, N, seed=20260921 + 2):
@@ -78,11 +71,12 @@ def load_peaks():
         with open(p) as f:
             d = json.load(f)
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA's H100 SXM data sheet (700 W): HBM3 bandwidth and dense BF16 tensor-core rate; not a measured rate
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md).
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region.
 
     The sampler is started before the warm-up steps (spawning nvidia-smi takes longer than a short timed region) and
     writes time-stamped rows every 50 ms; ``stop`` keeps the rows that fall inside the marked region.  If the region was
@@ -97,11 +91,10 @@ class ClockSampler:
         self.device = device
         self.proc = None
         self.t0 = self.t1 = None
-        self.path = os.path.join(ROOT, "gpurun_out", f"clocks_bench_{os.getpid()}.csv")
+        self.path = os.path.join(tempfile.gettempdir(), f"dmosopt_clocks_bench_{os.getpid()}.csv")
 
     def start(self):
         try:
-            os.makedirs(os.path.dirname(self.path), exist_ok=True)
             self.f = open(self.path, "w")
             self.proc = subprocess.Popen(["nvidia-smi", f"--query-gpu={self.Q}", "--format=csv,noheader,nounits", "-lms", "50", "-i", str(self.device)],
                                          stdout=self.f, stderr=subprocess.DEVNULL)
@@ -131,9 +124,11 @@ class ClockSampler:
         except Exception:
             self.proc.kill()
         self.f.close()
+        rows_text = open(self.path).read().splitlines()
+        os.remove(self.path)
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         rows = []
-        for line in open(self.path):
+        for line in rows_text:
             parts = [p.strip() for p in line.split(",")]
             if len(parts) < 10:
                 continue
@@ -427,6 +422,16 @@ def sort_hv_legs(L, pop, M, y_gp_merged, ref_gp):
     return out
 
 
+def dump_outputs(out_dir, rs):
+    """What the last timed step handed back to its caller: the surviving population (parameters, objectives, ranks), its
+    hypervolume and the number of offspring, as float64 .npy files (about 17 MB at the default sizes)."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"population_x": rs.pop_x.download(), "population_y": rs.pop_y.download(), "rank": rs.rank.download(),
+              "hypervolume": np.array([rs.hv]), "n_children": np.array([rs.nch[0]])}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.asarray(a, dtype=np.float64))
+
+
 def run_ours(args):
     import dmosopt_b200 as b2
     from dmosopt_b200 import _lib as L
@@ -531,23 +536,23 @@ def run_ours(args):
     clk = clocks.stop() if rank == 0 else {}
     value = n_val / t_val
     refined = sm._gp.auto_info()["last_refined"] if prec == L.GP_AUTO else 0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, rs)
 
     # ------------------------------------------------------------------ roofline of the dominant kernel (GP variance)
     var_ms, var_cnt = prof.get("gp_var", (0.0, 0))
     P_local = (n_val / args.steps) / world
     flops_per_launch = 2.0 * N * N * M * P_local  # SURVEY section 8d: GEMM form 2 N^2 M per candidate
     tensor_path = prec == L.GP_TENSOR or (prec == L.GP_AUTO and auto["var_tensor"])
-    version = "v2" if os.environ.get("DMO_GP_TC") == "2" else "v3"
     roof = None
     if var_cnt:
         avg_s = var_ms * 1e-3 / var_cnt
         ach = flops_per_launch / avg_s / 1e12
         peak = peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops"))
-        tr = NCU_TRAFFIC.get((version, pop, d, M, N)) if (tensor_path and world == 1) else None
         roof = {"bound": "tensor", "kernel": "gp_var (V = L^-1 K_*^T, column sums of V^2)", "achieved": ach, "peak": peak, "unit": "TFLOP/s",
-                "frac": ach / peak, "traffic": tr[1] if tr else None, "traffic_source": tr[0] if tr else None,
-                "peak_kind": f"bf16 dense, sustained, {peak_kind}", "avg_launch_ms": avg_s * 1e3, "flops_per_launch": flops_per_launch,
-                "arithmetic": "tcgen05 split-fp16" if tensor_path else "float64 CUDA cores"}
+                "frac": ach / peak,
+                "peak_kind": f"bf16 dense, {'sustained' if 'bf16_tflops_sustained' in peaks else 'peak'}, {peak_kind}", "avg_launch_ms": avg_s * 1e3, "flops_per_launch": flops_per_launch,
+                "arithmetic": "wgmma split-fp16" if tensor_path else "float64 CUDA cores"}
     shares = {k: v[0] / (ms_dev if ms_dev > 0 else 1.0) for k, v in prof.items()}
 
     if rank != 0:
@@ -618,7 +623,7 @@ def run_ours(args):
     if prec == L.GP_FP64:
         dtype = "f64"
     elif tensor_path:
-        dtype = ("f64 results; GP variance contraction in split-fp16 tcgen05 with fp32 accumulation"
+        dtype = ("f64 results; GP variance contraction in split-fp16 wgmma with fp32 accumulation"
                  + (f" (precision=auto: calibrated against the float64 path, {refined} of {int(P_local)} rows of the last step recomputed in float64)" if auto else "")
                  + "; ranks on u32 ids")
     else:
@@ -654,7 +659,7 @@ def main():
     ap.add_argument("--obj", type=int, default=3)
     ap.add_argument("--ntrain", type=int, default=4096)
     # auto = the plugin default: tensor path where the per-model calibration admits it, float64 rows where it does not;
-    # tensor = the tcgen05 split-fp16 variance kernel unconditionally (<= 1e-5 of the prior variance); fp64 = the float64
+    # tensor = the wgmma split-fp16 variance kernel unconditionally (<= 1e-5 of the prior variance); fp64 = the float64
     # CUDA-core path that matches scikit-learn to 1e-8 (parity anchor, ~15x slower)
     ap.add_argument("--precision", default=os.environ.get("DMOSOPT_B200_GP", "auto"), choices=["auto", "fp64", "tensor"])
     # MOASMO.epoch constructs its optimizer with distance_metric=None (dmosopt/MOASMO.py:365-373): rank ties keep
@@ -666,6 +671,8 @@ def main():
     ap.add_argument("--e2e-warmup", type=int, default=None)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-sort-hv", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the outputs of the last one to DIR/<name>.npy (float64)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

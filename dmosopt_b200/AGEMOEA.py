@@ -1,4 +1,4 @@
-"""AGE-MOEA optimizer plugin on the B200 path.
+"""AGE-MOEA optimizer plugin on the GPU path.
 
 Drop-in for ``dmosopt.AGEMOEA.AGEMOEA`` (dmosopt/AGEMOEA.py:24-501), selected by
 ``optimizer_name="dmosopt_b200.AGEMOEA"``.

@@ -1,4 +1,4 @@
-"""MO-CMA-ES optimizer plugin on the B200 path.
+"""MO-CMA-ES optimizer plugin on the GPU path.
 
 Drop-in for ``dmosopt.CMAES.CMAES`` (dmosopt/CMAES.py:26-537), selected by ``optimizer_name="dmosopt_b200.CMAES"``.
 

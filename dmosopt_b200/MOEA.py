@@ -82,7 +82,7 @@ def _initial_design(n, d, local_random, method=None):
 
 
 class MOEA(object):
-    """Base class of the B200 optimizer plugins; same contract as dmosopt.MOEA.MOEA (MOEA.py:55-188)."""
+    """Base class of the GPU optimizer plugins; same contract as dmosopt.MOEA.MOEA (MOEA.py:55-188)."""
 
     def __init__(self, name: str, popsize: int, nInput: int, nOutput: int, **kwargs):
         doubled = bool(kwargs.pop("optimize_mean_variance", False))  # not an optimizer parameter: only sizes the check below

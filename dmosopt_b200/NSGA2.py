@@ -1,4 +1,4 @@
-"""NSGA-II optimizer plugin on the B200 path.
+"""NSGA-II optimizer plugin on the GPU path.
 
 Drop-in for ``dmosopt.NSGA2.NSGA2`` (dmosopt/NSGA2.py:18-316): same constructor, parameters, state
 fields and ``generate / update`` contract, selected in dmosopt by

@@ -1,4 +1,4 @@
-"""SMPSO optimizer plugin on the B200 path.
+"""SMPSO optimizer plugin on the GPU path.
 
 Drop-in for ``dmosopt.SMPSO.SMPSO`` (dmosopt/SMPSO.py:19-348), selected by
 ``optimizer_name="dmosopt_b200.SMPSO"``.  ``swarm_size`` independent swarms of ``popsize`` particles:

@@ -1,4 +1,4 @@
-"""Trust-region search optimizer plugin on the B200 path (SURVEY.md section 8f row N4).
+"""Trust-region search optimizer plugin on the GPU path (SURVEY.md section 8f row N4).
 
 Drop-in for ``dmosopt.TRS.TRS`` (dmosopt/TRS.py:36-322), selected by ``optimizer_name="dmosopt_b200.TRS"``.
 

@@ -1,4 +1,4 @@
-"""dmosopt_b200 -- B200-native surrogate-generation hot path for dmosopt.
+"""dmosopt_b200 -- H100-native surrogate-generation hot path for dmosopt.
 
 Plugin import paths (dmosopt resolves them with ``config.import_object_by_path``):
 

@@ -111,7 +111,7 @@ def load_library(path=None):
     if not os.path.exists(path):
         raise DmoError(
             f"dmosopt_b200: CUDA library {path} not found. Build it with `python -m dmosopt_b200.build` "
-            "(nvcc, sm_100a). There is no CPU fallback."
+            "(nvcc, sm_90a). There is no CPU fallback."
         )
     lib = ctypes.CDLL(path)
     for name, (res, args) in _SIGNATURES.items():
@@ -141,7 +141,7 @@ def context(device=None):
         h = _vp()
         st = lib.dmo_create(dev, ctypes.byref(h))
         if st != 0 or not h.value:
-            raise DmoError(f"dmosopt_b200: dmo_create(device={dev}) failed with status {st}: no usable CUDA device (B200 required)")
+            raise DmoError(f"dmosopt_b200: dmo_create(device={dev}) failed with status {st}: no usable CUDA device (H100 required)")
         if _ctx is not None:
             lib.dmo_destroy(_ctx)
         _ctx, _ctx_device = h, dev

@@ -1,10 +1,9 @@
-"""Build libdmosopt_b200.so in-tree with nvcc for sm_100a.
+"""Build libdmosopt_b200.so in-tree with nvcc for sm_90a (H100).
 
     python -m dmosopt_b200.build            # incremental
     python -m dmosopt_b200.build --force    # rebuild everything
 
-nvcc cross-compiles without a GPU; the resulting .so sits next to this file
-(git-ignored, but shipped to the GPU box by gpurun).
+nvcc cross-compiles without a GPU; the resulting .so sits next to this file (git-ignored).
 """
 
 import hashlib
@@ -22,7 +21,7 @@ SOURCES = ["ctx.cu", "prims.cu", "rank.cu", "sortmo.cu", "variation.cu", "gp.cu"
 
 NVCC_FLAGS = [
     "-gencode",
-    "arch=compute_100a,code=sm_100a",
+    "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "-O3",
     "-std=c++17",
@@ -83,7 +82,7 @@ def build(force=False, verbose=True):
     objs = [o for o, _ in res]
     changed = any(c for _, c in res)
     if changed or not os.path.exists(LIB):
-        cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -1,4 +1,4 @@
-// Shared plumbing for the dmosopt_b200 CUDA library (sm_100a).
+// Shared plumbing for the dmosopt_b200 CUDA library (sm_90a).
 // Context, stream-ordered scratch buffers, host/device pointer staging,
 // launch accounting, order-preserving float transforms and Philox4x32-10.
 #pragma once
@@ -20,7 +20,7 @@ struct dmo_ctx {
   cudaMemPool_t pool = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;  // stream <-> aux ordering
-  int sm_count = 148;
+  int sm_count = 132;  // H100 SXM; replaced by the device's count in dmo_create
   int64_t launches = 0;
   std::string err;
   void* flush_buf = nullptr;

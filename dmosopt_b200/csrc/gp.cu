@@ -8,7 +8,7 @@
 // final subtraction from the prior variance.
 //
 // This file holds the float64 CUDA-core path (DMO_GP_FP64, the parity anchor, ~1e-10 of sklearn) and the object
-// management; the tcgen05 split-precision path lives in gp_tensor.cu.
+// management; the wgmma split-precision path lives in gp_tensor.cu.
 #include "gp.cuh"
 
 namespace {

@@ -1,4 +1,4 @@
-// GP posterior state shared by gp.cu (float64 path) and gp_tensor.cu (tcgen05 path).
+// GP posterior state shared by gp.cu (float64 path) and gp_tensor.cu (wgmma path).
 #pragma once
 #include <vector>
 

@@ -1,22 +1,22 @@
-// GP posterior variance on the 5th-generation tensor cores (DMO_GP_TENSOR, and the fast leg of DMO_GP_AUTO).
+// GP posterior variance on the Hopper tensor cores (DMO_GP_TENSOR, and the fast leg of DMO_GP_AUTO).
 //
 //   ||L^-1 K_*^T||^2 per candidate  ==  row sums of  D^2,   D[p][i] = sum_k K_*[p][k] * Linv[i][k]
 //
-// D is a dense (candidates x N_train) x N_train contraction, both operands k-contiguous ("TN").  It runs as
-// tcgen05.mma kind::f16 with the accumulator in TMEM:
+// D is a dense (candidates x N_train) x N_train contraction, both operands k-contiguous ("TN").  It runs as warpgroup
+// MMAs (wgmma.mma_async m64n256k16, fp16 inputs, fp32 accumulators in registers):
 //   * split precision: every float operand x is carried as two fp16 numbers hi + lo (22 significand bits) after an
 //     exact power-of-two scaling (per Linv row, per objective for K_*) that keeps both halves in fp16's normal range;
 //     D accumulates hi*hi + hi*lo + lo*hi in fp32 (three MMAs per product, the lo*lo term is below fp32 resolution);
-//   * A operand = K_* tile (2 x 128 candidates x 32 k), B operand = Linv tile (256 rows x 32 k), so one TMEM lane is
-//     one candidate and the epilogue's sum of squares is a private per-thread accumulation (no cross-lane reduction);
+//   * a work item is 128 candidates (two consumer warpgroups x 64 rows) against 256-row blocks of Linv; each thread's
+//     accumulators hold two candidate rows, so the epilogue's sum of squares is per thread plus a reduction over the
+//     four lanes that share a row;
 //   * Linv is lower triangular: the row block [256 j, 256 j + 256) only needs k < 256 (j + 1) -- half the MMAs skipped;
-//   * operand tiles arrive by TMA (cp.async.bulk.tensor, SWIZZLE_64B) into a 3-stage shared-memory ring, completion
-//     on mbarriers; one elected thread issues the MMAs; tcgen05.commit releases the ring slots and publishes the
-//     accumulator; four epilogue warps drain TMEM with tcgen05.ld;
-//   * persistent CTAs (one per SM) walk a list of equal-cost work items in an L2-friendly order (version 3, below).
+//   * operand tiles arrive by TMA (cp.async.bulk.tensor, SWIZZLE_64B) into a 4-stage shared-memory ring, completion on
+//     mbarriers; one producer warp issues the loads, each consumer warp releases a slot once its MMAs have read it;
+//   * persistent CTAs (one per SM) walk a list of equal-cost work items in an L2-friendly order (see below).
 //
 // K_* itself is produced in fp32 (relative error ~1e-6 on K_*) by kstar_mean_kernel, which accumulates the mean from the same
-// kernel values (packed fp32 over 16 training points, then float64, slices added in a fixed order: deterministic);
+// kernel values (fp32 over 16 training points, then float64, slices added in a fixed order: deterministic);
 // kstar_tensor_kernel + mean_split_kernel are the fallback for shapes that kernel does not take.  Predicts without
 // variance never write K_*: gp_mean_direct_kernel.
 //
@@ -32,10 +32,16 @@
 
 namespace {
 
-constexpr int TM = 128;      // candidates per UMMA tile  (UMMA M, TMEM lanes)
-constexpr int TN = 256;      // Linv rows per tile        (UMMA N, TMEM columns per accumulator)
-constexpr int UK = 16;       // UMMA K for 16-bit inputs
-constexpr int NTHREADS = 192;  // warp 0: TMA producer, warp 1: MMA issuer, warps 2..5: epilogue
+constexpr int TN = 256;       // Linv rows per tile (wgmma N); Npad is a multiple of it
+constexpr int TMV = 128;      // candidates per work item: two consumer warpgroups x wgmma M = 64
+constexpr int TK = 32;        // k per pipeline stage: 64-byte rows, SWIZZLE_64B
+constexpr int UK = 16;        // wgmma K for 16-bit inputs
+constexpr int STAGES = 4;
+constexpr int A_BYTES = TMV * TK * 2;                          // 8 KiB: K_* hi or lo
+constexpr int B_BYTES = TN * TK * 2;                           // 16 KiB: Linv hi or lo
+constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;         // 48 KiB
+constexpr size_t GEMM_SMEM = (size_t)STAGES * STAGE_BYTES + 1024 + 256;
+constexpr int NTHREADS = 384;  // warpgroups 0, 1: consumers; warpgroup 2: TMA producer (one thread issues the loads)
 
 // ------------------------------------------------------------------------------------------------ PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -85,256 +91,72 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* ba
       : "memory");
 }
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// K-major SWIZZLE_64B shared-memory matrix descriptor (wgmma): [0,14) start address >> 4 | [16,30) leading byte
+// offset >> 4 (unused for swizzled K-major: 1) | [32,46) stride byte offset >> 4 (8 rows x 64 B = 512 B between 8-row
+// groups) | [62,64) layout type = 2 (SWIZZLE_64B)
+__device__ __forceinline__ uint64_t make_sdesc64(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(512 >> 4) << 32) | (2ull << 62);
 }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                           uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+
+// d (+)= A[smem desc] (64 x 16) * B[smem desc]^T (256 x 16), fp16 inputs, fp32 accumulators; accumulate = 0 overwrites d.
+// Thread t of the warpgroup holds rows 16 (t / 32) + (t % 32) / 4 (+ 8) and columns 8 i + 2 (t % 4) (+ 1):
+// d[4 i] = (row, col), d[4 i + 1] = (row, col + 1), d[4 i + 2] = (row + 8, col), d[4 i + 3] = (row + 8, col + 1).
+__device__ __forceinline__ void wgmma_f16_m64n256(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+      "setp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
       : "memory");
 }
 
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread
-__device__ __forceinline__ void tc_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, mma_sm100_desc.hpp):
-//   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 (unused for swizzled K-major: 1)
-//   [32,46) stride byte offset >> 4 (8 rows x 128 B = 1024 B between 8-row groups) | [46,48) version = 1
-//   [61,64) layout type = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t make_sdesc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) |
-         (2ull << 61);
-}
-
-// kind::f16 instruction descriptor (cute::UMMA::InstrDescriptor): fp16 A/B (format 0), fp32 accumulate (c_format 1),
-// both K-major, N >> 3 at [17,23), M >> 4 at [24,29)
-constexpr uint32_t IDESC = (1u << 4) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-
-// ------------------------------------------------------------------------------------------------ the GEMM, version 2
-// Same contraction, 1.5x less L2 -> shared-memory traffic per MMA: a work item owns 256 candidates (two M = 128
-// sub-tiles that share every Linv tile), k is staged 32 elements at a time (64-byte rows, SWIZZLE_64B) so that three
-// 64 KiB stages fit, both TMEM accumulators (2 x 256 columns) belong to the two sub-tiles, and the Linv row blocks of a
-// candidate block are split into two halves of equal MMA count (two work items, partial sums added in a fixed order)
-// to keep the tail of the persistent schedule short.
-namespace v2 {
-constexpr int TM2 = 256, TN2 = 256, TK2 = 32, STAGES2 = 3;
-constexpr int TILE_BYTES2 = 256 * TK2 * 2;             // 16 KiB: 256 rows x 64 B
-constexpr int STAGE_BYTES2 = 4 * TILE_BYTES2;          // K* hi/lo + Linv hi/lo
-constexpr size_t GEMM_SMEM2 = (size_t)STAGES2 * STAGE_BYTES2 + 1024 + 256;
-
-// K-major SWIZZLE_64B descriptor: 8-row groups are 512 B apart, layout type 4
-__device__ __forceinline__ uint64_t make_sdesc64(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(512 >> 4) << 32) | (1ull << 46) | (4ull << 61);
-}
-
-struct GemmParams2 {
-  int M, n_pb, n_jt, j_split;  // row blocks [0, j_split) belong to half 0, [j_split, n_jt) to half 1
-  int64_t k_rows, l_rows;
-  const float* inv_scale;
-  double* vnorm;  // [2][M][vn_ld]
-  int64_t vn_ld;
-  int* abort_flag;
-};
-
-__global__ void __launch_bounds__(NTHREADS, 1)
-    gp_var_tc2_kernel(const __grid_constant__ CUtensorMap map_kh, const __grid_constant__ CUtensorMap map_kl,
-                      const __grid_constant__ CUtensorMap map_lh, const __grid_constant__ CUtensorMap map_ll,
-                      const GemmParams2 prm) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* tiles = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  uint64_t* bars = (uint64_t*)(tiles + (size_t)STAGES2 * STAGE_BYTES2);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + STAGES2;
-  uint64_t* acc_full = bars + 2 * STAGES2;
-  uint64_t* acc_empty = bars + 2 * STAGES2 + 1;
-  uint32_t* tmem_slot = (uint32_t*)(bars + 2 * STAGES2 + 2);
-  volatile int* abort_flag = prm.abort_flag;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES2; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    mbar_init(acc_full, 1);
-    mbar_init(acc_empty, 4);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const int n_work = prm.M * prm.n_pb * 2;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      uint32_t stage = 0, phase = 0;
-      for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
-        const int z = w & 1, wp = w >> 1;
-        const int m = wp / prm.n_pb, pb = wp - m * prm.n_pb;
-        const int a_row = (int)(m * prm.k_rows + (int64_t)pb * TM2);
-        const int j0 = z ? prm.j_split : 0, j1 = z ? prm.n_jt : prm.j_split;
-        for (int jt = j0; jt < j1; ++jt) {
-          const int b_row = (int)(m * prm.l_rows + (int64_t)jt * TN2);
-          const int nkc = (jt + 1) * (TN2 / TK2);
-          for (int kc = 0; kc < nkc; ++kc) {
-            mbar_wait(&empty[stage], phase ^ 1u, abort_flag);
-            uint8_t* st = tiles + (size_t)stage * STAGE_BYTES2;
-            mbar_expect_tx(&full[stage], STAGE_BYTES2);
-            tma_load_2d(&map_kh, &full[stage], st, kc * TK2, a_row);
-            tma_load_2d(&map_kl, &full[stage], st + TILE_BYTES2, kc * TK2, a_row);
-            tma_load_2d(&map_lh, &full[stage], st + 2 * TILE_BYTES2, kc * TK2, b_row);
-            tma_load_2d(&map_ll, &full[stage], st + 3 * TILE_BYTES2, kc * TK2, b_row);
-            if (++stage == STAGES2) {
-              stage = 0;
-              phase ^= 1u;
-            }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      uint32_t stage = 0, phase = 0, acc_phase = 0;
-      for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
-        const int z = w & 1;
-        const int j0 = z ? prm.j_split : 0, j1 = z ? prm.n_jt : prm.j_split;
-        for (int jt = j0; jt < j1; ++jt) {
-          mbar_wait(acc_empty, acc_phase ^ 1u, abort_flag);
-          tc_fence_after();
-          const int nkc = (jt + 1) * (TN2 / TK2);
-          for (int kc = 0; kc < nkc; ++kc) {
-            mbar_wait(&full[stage], phase, abort_flag);
-            tc_fence_after();
-            const uint32_t sa = smem_u32(tiles + (size_t)stage * STAGE_BYTES2);
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const uint32_t d_tmem = tmem_base + h * TN2;
-              const uint32_t a_off = h * (128 * TK2 * 2);  // second sub-tile: rows 128..255 of the K* boxes
-              const uint64_t a_hi = make_sdesc64(sa + a_off), a_lo = make_sdesc64(sa + TILE_BYTES2 + a_off);
-              const uint64_t b_hi = make_sdesc64(sa + 2 * TILE_BYTES2), b_lo = make_sdesc64(sa + 3 * TILE_BYTES2);
-#pragma unroll
-              for (int ks = 0; ks < TK2 / UK; ++ks) {
-                const uint64_t adv = (uint64_t)((ks * UK * 2) >> 4);
-                tc_mma_f16(d_tmem, a_hi + adv, b_hi + adv, IDESC, (kc | ks) ? 1u : 0u);
-                tc_mma_f16(d_tmem, a_hi + adv, b_lo + adv, IDESC, 1u);
-                tc_mma_f16(d_tmem, a_lo + adv, b_hi + adv, IDESC, 1u);
-              }
-            }
-            tc_commit(&empty[stage]);
-            if (++stage == STAGES2) {
-              stage = 0;
-              phase ^= 1u;
-            }
-          }
-          tc_commit(acc_full);
-          acc_phase ^= 1u;
-        }
-      }
-    }
-  } else {
-    const int quarter = warp & 3;
-    uint32_t acc_phase = 0;
-    for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
-      const int z = w & 1, wp = w >> 1;
-      const int m = wp / prm.n_pb, pb = wp - m * prm.n_pb;
-      const float* isc = prm.inv_scale + (int64_t)m * prm.l_rows;
-      const int j0 = z ? prm.j_split : 0, j1 = z ? prm.n_jt : prm.j_split;
-      double total0 = 0.0, total1 = 0.0;
-      for (int jt = j0; jt < j1; ++jt) {
-        mbar_wait(acc_full, acc_phase, abort_flag);
-        tc_fence_after();
-        float part0 = 0.f, part1 = 0.f;
-#pragma unroll 1
-        for (int c0 = 0; c0 < TN2; c0 += 32) {
-          uint32_t r0[32], r1[32];
-          const uint32_t t_addr = tmem_base + ((uint32_t)(quarter * 32) << 16) + c0;
-          tc_ld_32x32(t_addr, r0);
-          tc_ld_32x32(t_addr + TN2, r1);
-          tc_wait_ld();
-          const float* sc = isc + jt * TN2 + c0;
-#pragma unroll
-          for (int e = 0; e < 32; ++e) {
-            const float s = __ldg(sc + e);
-            const float t0 = __uint_as_float(r0[e]) * s, t1 = __uint_as_float(r1[e]) * s;
-            part0 = fmaf(t0, t0, part0);
-            part1 = fmaf(t1, t1, part1);
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(acc_empty);
-        total0 += (double)part0;
-        total1 += (double)part1;
-        acc_phase ^= 1u;
-      }
-      double* out = prm.vnorm + ((int64_t)z * prm.M + m) * prm.vn_ld + (int64_t)pb * TM2 + quarter * 32 + lane;
-      out[0] = total0;
-      out[128] = total1;
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
-  }
-}
-}  // namespace v2
-
-// ------------------------------------------------------------------------------------------------ the GEMM, version 3
-// Same tiles and pipeline as version 2; what changes is the work list and where K_* comes from.
-//   * A work item is (objective, 256 candidates, PAIR of Linv row blocks {q, n_jt - 1 - q}): every item costs the same
-//     n_jt + 1 k-blocks, so a static round-robin over the persistent CTAs has a tail of at most one item in
-//     M * n_pb * ceil(n_jt / 2) (6144 at the BASELINE shape, 41.5 rounds on 148 SMs).
-//   * Items are ordered (objective, candidate block, pair): the ceil(n_jt / 2) CTAs that hold the same candidate block
-//     start together at k = 0 and walk k at the same (MMA-bound) rate, so one of them pulls a K_* tile from DRAM and the
-//     others hit it in L2; version 2 ran 148 different candidate blocks at once and re-read every K_* tile from DRAM
-//     once per row block (22.6 GB per launch for 3.2 GB of operands).
-//   * Optional (DMO_GP_OVERLAP=1, off by default -- measured slower under the 1 kW power cap, see gp_predict_tensor): the
-//     kernel can be launched while the K_* producer (kstar_tensor_kernel, on the context's second stream) is still
-//     running; the TMA thread then waits for the producer's per-candidate-block completion counter before the first
-//     load of an item (ld.acquire.gpu + fence.proxy.async).
-namespace v3 {
-using v2::make_sdesc64;
-using v2::STAGE_BYTES2;
-using v2::STAGES2;
-using v2::TILE_BYTES2;
-using v2::TK2;
-using v2::TM2;
-using v2::TN2;
-using v2::GEMM_SMEM2;
-
-struct GemmParams3 {
-  int M, n_pb, n_jt, n_q;
+// ------------------------------------------------------------------------------------------------ the contraction
+// Work items and their order.  An item is (objective, 128 candidates, item q of the candidate block); the q of a
+// candidate block are adjacent in the list, so the CTAs that share a K_* tile start together at k = 0 and walk k at the
+// same (MMA-bound) rate: one of them pulls the tile from DRAM and the others hit it in L2.
+//   * paired (default): item q owns the Linv row blocks {q, n_jt - 1 - q}, so every item costs the same n_jt + 1
+//     k-blocks and a static round-robin over the persistent CTAs has a tail of at most one item;
+//   * halves (DMO_GP_TC=2, the previous schedule): item 0 owns row blocks [0, j_split), item 1 [j_split, n_jt).
+// Each item writes its partial sums to its own plane q of vnorm (and mnorm); var_finish_tc_kernel adds the planes in
+// a fixed order.
+struct GemmParams {
+  int M, n_pb, n_jt, n_q;  // n_q items per candidate block
+  int paired, j_split;
   int64_t k_rows, l_rows;
   const float* inv_scale;
   double* vnorm;  // [n_q][M][vn_ld]
@@ -342,10 +164,21 @@ struct GemmParams3 {
   int* abort_flag;
   const float* zf;        // [M][l_rows] whitened targets (nullptr: the mean is not taken from this contraction)
   double* mnorm;          // [n_q][M][vn_ld] partial sums of D z
-  const unsigned* ready;  // [n_pb] completion counters of the K_* producer (nullptr: K_* is complete at launch)
+  const unsigned* ready;  // [n_pb / 2] completion counters of the K_* producer (nullptr: K_* is complete at launch)
   unsigned ready_target;
   int dbg;  // DMO_GP_DBG bits (diagnostics): 1 = no proxy fence, 2 = no nanosleep in the wait loop
 };
+
+__device__ __forceinline__ int item_blocks(const GemmParams& p, int q) {
+  if (p.paired) return q == p.n_jt - 1 - q ? 1 : 2;
+  return q ? p.n_jt - p.j_split : p.j_split;
+}
+// s-th row block of item q; in the paired schedule the short one comes first: its K_* tiles are read again right away
+// by the long one
+__device__ __forceinline__ int item_row_block(const GemmParams& p, int q, int s) {
+  if (p.paired) return s ? p.n_jt - 1 - q : q;
+  return (q ? p.j_split : 0) + s;
+}
 
 __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
   unsigned v;
@@ -354,50 +187,39 @@ __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
 }
 
 __global__ void __launch_bounds__(NTHREADS, 1)
-    gp_var_tc3_kernel(const __grid_constant__ CUtensorMap map_kh, const __grid_constant__ CUtensorMap map_kl,
-                      const __grid_constant__ CUtensorMap map_lh, const __grid_constant__ CUtensorMap map_ll,
-                      const GemmParams3 prm) {
+    gp_var_wgmma_kernel(const __grid_constant__ CUtensorMap map_kh, const __grid_constant__ CUtensorMap map_kl,
+                        const __grid_constant__ CUtensorMap map_lh, const __grid_constant__ CUtensorMap map_ll,
+                        const GemmParams prm) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* tiles = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  uint64_t* bars = (uint64_t*)(tiles + (size_t)STAGES2 * STAGE_BYTES2);
+  uint64_t* bars = (uint64_t*)(tiles + (size_t)STAGES * STAGE_BYTES);
   uint64_t* full = bars;
-  uint64_t* empty = bars + STAGES2;
-  uint64_t* acc_full = bars + 2 * STAGES2;
-  uint64_t* acc_empty = bars + 2 * STAGES2 + 1;
-  uint32_t* tmem_slot = (uint32_t*)(bars + 2 * STAGES2 + 2);
+  uint64_t* empty = bars + STAGES;
   volatile int* abort_flag = prm.abort_flag;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES2; ++s) {
+    for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 8);  // one arrival per consumer warp
     }
-    mbar_init(acc_full, 1);
-    mbar_init(acc_empty, 4);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int per_m = prm.n_pb * prm.n_q;
   const int n_work = prm.M * per_m;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  // registers move from the producer warpgroup to the consumers (128 accumulators each): 40 + 2 x 232 per sub-partition
+  if (warp >= 8) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+    if (warp == 8 && lane == 0) {
       uint32_t stage = 0, phase = 0;
       for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
         const int m = w / per_m, r = w - m * per_m;
         const int pb = r / prm.n_q, q = r - pb * prm.n_q;
         if (prm.ready) {  // the K_* rows of this candidate block must have been written (by another kernel, generic proxy)
           uint32_t spins = 0;
-          while (ld_acquire_u32(prm.ready + pb) < prm.ready_target) {
+          while (ld_acquire_u32(prm.ready + (pb >> 1)) < prm.ready_target) {
             if (!(prm.dbg & 2)) __nanosleep(256);
             if ((++spins & 0xFFu) == 0u) {
               if (*abort_flag) break;
@@ -409,22 +231,21 @@ __global__ void __launch_bounds__(NTHREADS, 1)
           }
           if (!(prm.dbg & 1)) asm volatile("fence.proxy.async;" ::: "memory");  // order the TMA (async proxy) reads after the acquire
         }
-        const int a_row = (int)(m * prm.k_rows + (int64_t)pb * TM2);
-        const int jhi = prm.n_jt - 1 - q;
-        for (int s = 0; s < 2; ++s) {  // short row block first: its K_* tiles are read again right away by the long one
-          const int jt = s ? jhi : q;
-          if (s && q == jhi) break;
-          const int b_row = (int)(m * prm.l_rows + (int64_t)jt * TN2);
-          const int nkc = (jt + 1) * (TN2 / TK2);
+        const int a_row = (int)(m * prm.k_rows + (int64_t)pb * TMV);
+        const int nb = item_blocks(prm, q);
+        for (int s = 0; s < nb; ++s) {
+          const int jt = item_row_block(prm, q, s);
+          const int b_row = (int)(m * prm.l_rows + (int64_t)jt * TN);
+          const int nkc = (jt + 1) * (TN / TK);
           for (int kc = 0; kc < nkc; ++kc) {
             mbar_wait(&empty[stage], phase ^ 1u, abort_flag);
-            uint8_t* st = tiles + (size_t)stage * STAGE_BYTES2;
-            mbar_expect_tx(&full[stage], STAGE_BYTES2);
-            tma_load_2d(&map_kh, &full[stage], st, kc * TK2, a_row);
-            tma_load_2d(&map_kl, &full[stage], st + TILE_BYTES2, kc * TK2, a_row);
-            tma_load_2d(&map_lh, &full[stage], st + 2 * TILE_BYTES2, kc * TK2, b_row);
-            tma_load_2d(&map_ll, &full[stage], st + 3 * TILE_BYTES2, kc * TK2, b_row);
-            if (++stage == STAGES2) {
+            uint8_t* st = tiles + (size_t)stage * STAGE_BYTES;
+            mbar_expect_tx(&full[stage], STAGE_BYTES);
+            tma_load_2d(&map_kh, &full[stage], st, kc * TK, a_row);
+            tma_load_2d(&map_kl, &full[stage], st + A_BYTES, kc * TK, a_row);
+            tma_load_2d(&map_lh, &full[stage], st + 2 * A_BYTES, kc * TK, b_row);
+            tma_load_2d(&map_ll, &full[stage], st + 2 * A_BYTES + B_BYTES, kc * TK, b_row);
+            if (++stage == STAGES) {
               stage = 0;
               phase ^= 1u;
             }
@@ -432,122 +253,103 @@ __global__ void __launch_bounds__(NTHREADS, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      uint32_t stage = 0, phase = 0, acc_phase = 0;
-      for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
-        const int r = w % per_m;
-        const int q = r % prm.n_q;
-        const int jhi = prm.n_jt - 1 - q;
-        for (int s = 0; s < 2; ++s) {
-          const int jt = s ? jhi : q;
-          if (s && q == jhi) break;
-          mbar_wait(acc_empty, acc_phase ^ 1u, abort_flag);
-          tc_fence_after();
-          const int nkc = (jt + 1) * (TN2 / TK2);
-          for (int kc = 0; kc < nkc; ++kc) {
-            mbar_wait(&full[stage], phase, abort_flag);
-            tc_fence_after();
-            const uint32_t sa = smem_u32(tiles + (size_t)stage * STAGE_BYTES2);
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const uint32_t d_tmem = tmem_base + h * TN2;
-              const uint32_t a_off = h * (128 * TK2 * 2);
-              const uint64_t a_hi = make_sdesc64(sa + a_off), a_lo = make_sdesc64(sa + TILE_BYTES2 + a_off);
-              const uint64_t b_hi = make_sdesc64(sa + 2 * TILE_BYTES2), b_lo = make_sdesc64(sa + 3 * TILE_BYTES2);
-#pragma unroll
-              for (int ks = 0; ks < TK2 / UK; ++ks) {
-                const uint64_t adv = (uint64_t)((ks * UK * 2) >> 4);
-                tc_mma_f16(d_tmem, a_hi + adv, b_hi + adv, IDESC, (kc | ks) ? 1u : 0u);
-                tc_mma_f16(d_tmem, a_hi + adv, b_lo + adv, IDESC, 1u);
-                tc_mma_f16(d_tmem, a_lo + adv, b_hi + adv, IDESC, 1u);
-              }
-            }
-            tc_commit(&empty[stage]);
-            if (++stage == STAGES2) {
-              stage = 0;
-              phase ^= 1u;
-            }
-          }
-          tc_commit(acc_full);
-          acc_phase ^= 1u;
-        }
-      }
-    }
-  } else {
-    const int quarter = warp & 3;
-    uint32_t acc_phase = 0;
-    for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
-      const int m = w / per_m, r = w - m * per_m;
-      const int pb = r / prm.n_q, q = r - pb * prm.n_q;
-      const float* isc = prm.inv_scale + (int64_t)m * prm.l_rows;
-      const float* zf = prm.zf ? prm.zf + (int64_t)m * prm.l_rows : nullptr;
-      const int jhi = prm.n_jt - 1 - q;
-      double total0 = 0.0, total1 = 0.0, mtot0 = 0.0, mtot1 = 0.0;
-      for (int s = 0; s < 2; ++s) {
-        const int jt = s ? jhi : q;
-        if (s && q == jhi) break;
-        mbar_wait(acc_full, acc_phase, abort_flag);
-        tc_fence_after();
-#pragma unroll 1
-        for (int c0 = 0; c0 < TN2; c0 += 32) {
-          uint32_t r0[32], r1[32];
-          const uint32_t t_addr = tmem_base + ((uint32_t)(quarter * 32) << 16) + c0;
-          tc_ld_32x32(t_addr, r0);
-          tc_ld_32x32(t_addr + TN2, r1);
-          tc_wait_ld();
-          const float* sc = isc + jt * TN2 + c0;
-          // four independent fp32 partial sums per sub-tile over 8 squares each, folded into float64 every 32 columns:
-          // the rounding of the sum of squares stays at the 2^-24 * sqrt(8) level instead of growing with N
-          float p0[4] = {0.f, 0.f, 0.f, 0.f}, p1[4] = {0.f, 0.f, 0.f, 0.f};
-          if (zf) {  // posterior mean = D z out of the same accumulator (z = L^-1 y_n): one more FMA per element
-            const float* zc = zf + jt * TN2 + c0;
-            float q0[4] = {0.f, 0.f, 0.f, 0.f}, q1[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-            for (int e = 0; e < 32; ++e) {
-              const float sv = __ldg(sc + e), zv = __ldg(zc + e);
-              const float t0 = __uint_as_float(r0[e]) * sv, t1 = __uint_as_float(r1[e]) * sv;
-              p0[e & 3] = fmaf(t0, t0, p0[e & 3]);
-              p1[e & 3] = fmaf(t1, t1, p1[e & 3]);
-              q0[e & 3] = fmaf(t0, zv, q0[e & 3]);
-              q1[e & 3] = fmaf(t1, zv, q1[e & 3]);
-            }
-            mtot0 += ((double)q0[0] + (double)q0[1]) + ((double)q0[2] + (double)q0[3]);
-            mtot1 += ((double)q1[0] + (double)q1[1]) + ((double)q1[2] + (double)q1[3]);
-          } else {
-#pragma unroll
-            for (int e = 0; e < 32; ++e) {
-              const float sv = __ldg(sc + e);
-              const float t0 = __uint_as_float(r0[e]) * sv, t1 = __uint_as_float(r1[e]) * sv;
-              p0[e & 3] = fmaf(t0, t0, p0[e & 3]);
-              p1[e & 3] = fmaf(t1, t1, p1[e & 3]);
-            }
-          }
-          total0 += ((double)p0[0] + (double)p0[1]) + ((double)p0[2] + (double)p0[3]);
-          total1 += ((double)p1[0] + (double)p1[1]) + ((double)p1[2] + (double)p1[3]);
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(acc_empty);
-        acc_phase ^= 1u;
-      }
-      if (zf) {
-        double* mo = prm.mnorm + ((int64_t)q * prm.M + m) * prm.vn_ld + (int64_t)pb * TM2 + quarter * 32 + lane;
-        mo[0] = mtot0;
-        mo[128] = mtot1;
-      }
-      double* out = prm.vnorm + ((int64_t)q * prm.M + m) * prm.vn_ld + (int64_t)pb * TM2 + quarter * 32 + lane;
-      out[0] = total0;
-      out[128] = total1;
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
+
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+  // consumers: warpgroup wg owns candidate rows [64 wg, 64 wg + 64) of the item
+  const int wg = warp >> 2;
+  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // and row0 + 8
+  const int col0 = 2 * (lane & 3);
+  float acc[128];
+  uint32_t stage = 0, phase = 0;
+  for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
+    const int m = w / per_m, r = w - m * per_m;
+    const int pb = r / prm.n_q, q = r - pb * prm.n_q;
+    const float* isc = prm.inv_scale + (int64_t)m * prm.l_rows;
+    const float* zf = prm.zf ? prm.zf + (int64_t)m * prm.l_rows : nullptr;
+    double total0 = 0.0, total1 = 0.0, mtot0 = 0.0, mtot1 = 0.0;
+    const int nb = item_blocks(prm, q);
+    for (int s = 0; s < nb; ++s) {
+      const int jt = item_row_block(prm, q, s);
+      const int nkc = (jt + 1) * (TN / TK);
+      uint32_t prev = 0;
+      for (int kc = 0; kc < nkc; ++kc) {
+        mbar_wait(&full[stage], phase, abort_flag);
+        const uint32_t sa = smem_u32(tiles + (size_t)stage * STAGE_BYTES);
+        const uint32_t a_off = wg * (64 * TK * 2);
+        const uint64_t a_hi = make_sdesc64(sa + a_off), a_lo = make_sdesc64(sa + A_BYTES + a_off);
+        const uint64_t b_hi = make_sdesc64(sa + 2 * A_BYTES), b_lo = make_sdesc64(sa + 2 * A_BYTES + B_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < TK / UK; ++ks) {
+          const uint64_t adv = (uint64_t)((ks * UK * 2) >> 4);
+          wgmma_f16_m64n256(acc, a_hi + adv, b_hi + adv, (kc | ks) ? 1u : 0u);
+          wgmma_f16_m64n256(acc, a_hi + adv, b_lo + adv, 1u);
+          wgmma_f16_m64n256(acc, a_lo + adv, b_hi + adv, 1u);
+        }
+        wgmma_commit();
+        if (kc > 0) {  // the previous k-block's MMAs are done with their slot: hand it back to the producer
+          wgmma_wait<1>();
+          if (lane == 0) mbar_arrive(&empty[prev]);
+        }
+        prev = stage;
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1u;
+        }
+      }
+      wgmma_wait<0>();
+      if (lane == 0) mbar_arrive(&empty[prev]);
+      // per 32 columns a thread holds 8 squares of each of its rows, in four fp32 partial sums folded into float64: the
+      // rounding of the sum of squares stays at the 2^-24 level instead of growing with N
+      const float* sc = isc + jt * TN + col0;
+      const float* zc = zf ? zf + jt * TN + col0 : nullptr;
+#pragma unroll
+      for (int g = 0; g < TN / 32; ++g) {
+        float p0[4] = {0.f, 0.f, 0.f, 0.f}, p1[4] = {0.f, 0.f, 0.f, 0.f};
+        float q0[4] = {0.f, 0.f, 0.f, 0.f}, q1[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const int i = 4 * g + u;
+          const float2 sv = __ldg(reinterpret_cast<const float2*>(sc + 8 * i));
+          const float t00 = acc[4 * i] * sv.x, t01 = acc[4 * i + 1] * sv.y;
+          const float t10 = acc[4 * i + 2] * sv.x, t11 = acc[4 * i + 3] * sv.y;
+          p0[u] = fmaf(t01, t01, t00 * t00);
+          p1[u] = fmaf(t11, t11, t10 * t10);
+          if (zc) {  // posterior mean = D z out of the same accumulator (z = L^-1 y_n)
+            const float2 zv = __ldg(reinterpret_cast<const float2*>(zc + 8 * i));
+            q0[u] = fmaf(t01, zv.y, t00 * zv.x);
+            q1[u] = fmaf(t11, zv.y, t10 * zv.x);
+          }
+        }
+        total0 += ((double)p0[0] + (double)p0[1]) + ((double)p0[2] + (double)p0[3]);
+        total1 += ((double)p1[0] + (double)p1[1]) + ((double)p1[2] + (double)p1[3]);
+        if (zc) {
+          mtot0 += ((double)q0[0] + (double)q0[1]) + ((double)q0[2] + (double)q0[3]);
+          mtot1 += ((double)q1[0] + (double)q1[1]) + ((double)q1[2] + (double)q1[3]);
+        }
+      }
+    }
+    // the four lanes of a quad hold disjoint columns of the same two rows
+#pragma unroll
+    for (int o = 1; o < 4; o <<= 1) {
+      total0 += __shfl_xor_sync(0xffffffffu, total0, o);
+      total1 += __shfl_xor_sync(0xffffffffu, total1, o);
+      mtot0 += __shfl_xor_sync(0xffffffffu, mtot0, o);
+      mtot1 += __shfl_xor_sync(0xffffffffu, mtot1, o);
+    }
+    if ((lane & 3) == 0) {
+      const int64_t o = ((int64_t)q * prm.M + m) * prm.vn_ld + (int64_t)pb * TMV + row0;
+      prm.vnorm[o] = total0;
+      prm.vnorm[o + 8] = total1;
+      if (zf) {
+        prm.mnorm[o] = mtot0;
+        prm.mnorm[o + 8] = mtot1;
+      }
+    }
   }
 }
-}  // namespace v3
 
 // ------------------------------------------------------------------------------------------------ operand preparation
 // Linv row -> scaled fp16 hi / lo.  One block per (objective, row).
@@ -593,22 +395,30 @@ __device__ __forceinline__ float stationary_f(float s2, int kind) {
   return __expf(-0.5f * s2);
 }
 
-// the same for a pair of squared distances, on the packed fp32 pipe (FMUL2 / FFMA2); the two MUFU ops per value stay scalar
+// fp32 pairs: one correctly rounded operation per component (no FMA contraction), so a pair gives exactly what two
+// scalar operations give
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+
+// the same for a pair of squared distances
 __device__ __forceinline__ float2 stationary2_f(float2 s2, int kind) {
   float2 e;
   if (kind == DMO_KERNEL_MATERN52) {
     float2 r;
     asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(r.x) : "f"(s2.x));
     asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(r.y) : "f"(s2.y));
-    const float2 K = __fmul2_rn(r, make_float2(2.2360679774997896f, 2.2360679774997896f));
+    const float2 K = fmul2(r, make_float2(2.2360679774997896f, 2.2360679774997896f));
     const float2 one = make_float2(1.0f, 1.0f);
-    const float2 p = __ffma2_rn(K, __ffma2_rn(K, make_float2(1.0f / 3.0f, 1.0f / 3.0f), one), one);
-    const float2 t = __fmul2_rn(K, make_float2(-1.4426950408889634f, -1.4426950408889634f));  // exp(-K) = 2^(-K log2 e)
+    const float2 p = ffma2(K, ffma2(K, make_float2(1.0f / 3.0f, 1.0f / 3.0f), one), one);
+    const float2 t = fmul2(K, make_float2(-1.4426950408889634f, -1.4426950408889634f));  // exp(-K) = 2^(-K log2 e)
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.x) : "f"(t.x));
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.y) : "f"(t.y));
-    return __fmul2_rn(p, e);
+    return fmul2(p, e);
   }
-  const float2 t = __fmul2_rn(s2, make_float2(-0.5f * 1.4426950408889634f, -0.5f * 1.4426950408889634f));
+  const float2 t = fmul2(s2, make_float2(-0.5f * 1.4426950408889634f, -0.5f * 1.4426950408889634f));
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.x) : "f"(t.x));
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.y) : "f"(t.y));
   return e;
@@ -640,8 +450,7 @@ __global__ void __launch_bounds__(KT_TN)
     s_il[t] = j < d ? (float)inv_ls[m * d + j] : 0.f;
   }
   if (threadIdx.x < M) s_c[threadIdx.x] = scalbnf((float)constant[threadIdx.x], k_exp[threadIdx.x]);
-  // training coordinates as packed pairs (two coordinates per 64-bit register pair): the distance loop runs on the
-  // packed fp32 pipe, FADD2 + FFMA2 per two coordinates and point instead of 2 FADD + 2 FFMA
+  // training coordinates as pairs (two coordinates per 64-bit register pair)
   float2 xa[DMAX / 2], xb[DMAX / 2];
 #pragma unroll
   for (int j = 0; j < DMAX / 2; ++j) {
@@ -665,14 +474,14 @@ __global__ void __launch_bounds__(KT_TN)
       for (int j = 0; j < DMAX / 4; ++j) {
         const float4 c = xc[j];
         const float2 c01 = make_float2(c.x, c.y), c23 = make_float2(c.z, c.w);
-        const float2 da0 = __fadd2_rn(c01, make_float2(-xa[2 * j].x, -xa[2 * j].y));
-        const float2 db0 = __fadd2_rn(c01, make_float2(-xb[2 * j].x, -xb[2 * j].y));
-        const float2 da1 = __fadd2_rn(c23, make_float2(-xa[2 * j + 1].x, -xa[2 * j + 1].y));
-        const float2 db1 = __fadd2_rn(c23, make_float2(-xb[2 * j + 1].x, -xb[2 * j + 1].y));
-        acc_a0 = __ffma2_rn(da0, da0, acc_a0);
-        acc_b0 = __ffma2_rn(db0, db0, acc_b0);
-        acc_a1 = __ffma2_rn(da1, da1, acc_a1);
-        acc_b1 = __ffma2_rn(db1, db1, acc_b1);
+        const float2 da0 = fadd2(c01, make_float2(-xa[2 * j].x, -xa[2 * j].y));
+        const float2 db0 = fadd2(c01, make_float2(-xb[2 * j].x, -xb[2 * j].y));
+        const float2 da1 = fadd2(c23, make_float2(-xa[2 * j + 1].x, -xa[2 * j + 1].y));
+        const float2 db1 = fadd2(c23, make_float2(-xb[2 * j + 1].x, -xb[2 * j + 1].y));
+        acc_a0 = ffma2(da0, da0, acc_a0);
+        acc_b0 = ffma2(db0, db0, acc_b0);
+        acc_a1 = ffma2(da1, da1, acc_a1);
+        acc_b1 = ffma2(db1, db1, acc_b1);
       }
       sa = (acc_a0.x + acc_a0.y) + (acc_a1.x + acc_a1.y);
       sb = (acc_b0.x + acc_b0.y) + (acc_b1.x + acc_b1.y);
@@ -682,7 +491,7 @@ __global__ void __launch_bounds__(KT_TN)
       if (ISO) {
         const float il = s_il[m * DMAX];
         const float il2 = il * il;
-        rr = __fmul2_rn(make_float2(sa, sb), make_float2(il2, il2));
+        rr = fmul2(make_float2(sa, sb), make_float2(il2, il2));
       } else {
         const float4* il4 = reinterpret_cast<const float4*>(s_il + m * DMAX);
         float2 acc_a = make_float2(0.f, 0.f), acc_b = acc_a;
@@ -691,19 +500,19 @@ __global__ void __launch_bounds__(KT_TN)
           const float4 c = xc[j], il = il4[j];
           const float2 c01 = make_float2(c.x, c.y), c23 = make_float2(c.z, c.w);
           const float2 i01 = make_float2(il.x, il.y), i23 = make_float2(il.z, il.w);
-          const float2 da0 = __fmul2_rn(__fadd2_rn(c01, make_float2(-xa[2 * j].x, -xa[2 * j].y)), i01);
-          const float2 db0 = __fmul2_rn(__fadd2_rn(c01, make_float2(-xb[2 * j].x, -xb[2 * j].y)), i01);
-          const float2 da1 = __fmul2_rn(__fadd2_rn(c23, make_float2(-xa[2 * j + 1].x, -xa[2 * j + 1].y)), i23);
-          const float2 db1 = __fmul2_rn(__fadd2_rn(c23, make_float2(-xb[2 * j + 1].x, -xb[2 * j + 1].y)), i23);
-          acc_a = __ffma2_rn(da0, da0, acc_a);
-          acc_b = __ffma2_rn(db0, db0, acc_b);
-          acc_a = __ffma2_rn(da1, da1, acc_a);
-          acc_b = __ffma2_rn(db1, db1, acc_b);
+          const float2 da0 = fmul2(fadd2(c01, make_float2(-xa[2 * j].x, -xa[2 * j].y)), i01);
+          const float2 db0 = fmul2(fadd2(c01, make_float2(-xb[2 * j].x, -xb[2 * j].y)), i01);
+          const float2 da1 = fmul2(fadd2(c23, make_float2(-xa[2 * j + 1].x, -xa[2 * j + 1].y)), i23);
+          const float2 db1 = fmul2(fadd2(c23, make_float2(-xb[2 * j + 1].x, -xb[2 * j + 1].y)), i23);
+          acc_a = ffma2(da0, da0, acc_a);
+          acc_b = ffma2(db0, db0, acc_b);
+          acc_a = ffma2(da1, da1, acc_a);
+          acc_b = ffma2(db1, db1, acc_b);
         }
         rr = make_float2(acc_a.x + acc_a.y, acc_b.x + acc_b.y);
       }
       const float sc = s_c[m];
-      const float2 kk = __fmul2_rn(stationary2_f(rr, kind), make_float2(sc, sc));  // c * k(r), scaled by 2^kexp (exact)
+      const float2 kk = fmul2(stationary2_f(rr, kind), make_float2(sc, sc));  // c * k(r), scaled by 2^kexp (exact)
       const float ka = live_a ? kk.x : 0.f;
       const float kb = live_b ? kk.y : 0.f;
       const __half2 h = __floats2half2_rn(ka, kb);
@@ -727,8 +536,8 @@ __global__ void __launch_bounds__(KT_TN)
 
 // Mean-only posterior (what MOASMO.optimize asks for every generation: model.evaluate -> mean, MOASMO.py:107-108): K_* is
 // never written.  A thread owns two candidates (coordinates in registers), the block walks its share of the training
-// points through a shared-memory tile (16-byte broadcast reads, packed fp32 distance loops as in kstar_tensor_kernel),
-// k(x, x_n) * (c alpha_n) is accumulated with packed FFMA over 32 training points and then folded into float64; the
+// points through a shared-memory tile (16-byte broadcast reads, paired fp32 distance loops as in kstar_tensor_kernel),
+// k(x, x_n) * (c alpha_n) is accumulated in fp32 over 32 training points and then folded into float64; the
 // partial sums of the blockIdx.x slices are added in a fixed order by mean_finish_tc_kernel (deterministic).
 constexpr int KM_T = 128, KM_Q = 256, KM_NS = 32, KM_D = 32;
 
@@ -806,14 +615,14 @@ __global__ void __launch_bounds__(KM_T, 4)
         for (int j = 0; j < NJ; ++j) {
           const float4 c = xr[j];
           const float2 c01 = make_float2(c.x, c.y), c23 = make_float2(c.z, c.w);
-          const float2 da0 = __fadd2_rn(c01, make_float2(-ca[2 * j].x, -ca[2 * j].y));
-          const float2 db0 = __fadd2_rn(c01, make_float2(-cb[2 * j].x, -cb[2 * j].y));
-          const float2 da1 = __fadd2_rn(c23, make_float2(-ca[2 * j + 1].x, -ca[2 * j + 1].y));
-          const float2 db1 = __fadd2_rn(c23, make_float2(-cb[2 * j + 1].x, -cb[2 * j + 1].y));
-          a0 = __ffma2_rn(da0, da0, a0);
-          b0 = __ffma2_rn(db0, db0, b0);
-          a1 = __ffma2_rn(da1, da1, a1);
-          b1 = __ffma2_rn(db1, db1, b1);
+          const float2 da0 = fadd2(c01, make_float2(-ca[2 * j].x, -ca[2 * j].y));
+          const float2 db0 = fadd2(c01, make_float2(-cb[2 * j].x, -cb[2 * j].y));
+          const float2 da1 = fadd2(c23, make_float2(-ca[2 * j + 1].x, -ca[2 * j + 1].y));
+          const float2 db1 = fadd2(c23, make_float2(-cb[2 * j + 1].x, -cb[2 * j + 1].y));
+          a0 = ffma2(da0, da0, a0);
+          b0 = ffma2(db0, db0, b0);
+          a1 = ffma2(da1, da1, a1);
+          b1 = ffma2(db1, db1, b1);
         }
         const float2 r2 = make_float2((a0.x + a0.y) + (a1.x + a1.y), (b0.x + b0.y) + (b1.x + b1.y));
 #pragma unroll
@@ -821,7 +630,7 @@ __global__ void __launch_bounds__(KM_T, 4)
           const float il = s_il[m * KM_D];
           const float il2 = il * il;
           const float al = s_al[m * KM_NS + i];
-          acc[m] = __ffma2_rn(stationary2_f(__fmul2_rn(r2, make_float2(il2, il2)), kind), make_float2(al, al), acc[m]);
+          acc[m] = ffma2(stationary2_f(fmul2(r2, make_float2(il2, il2)), kind), make_float2(al, al), acc[m]);
         }
       }
 #pragma unroll
@@ -843,17 +652,17 @@ __global__ void __launch_bounds__(KM_T, 4)
             const float4 c = xr[j], il = il4[j];
             const float2 c01 = make_float2(c.x, c.y), c23 = make_float2(c.z, c.w);
             const float2 i01 = make_float2(il.x, il.y), i23 = make_float2(il.z, il.w);
-            const float2 da0 = __fmul2_rn(__fadd2_rn(c01, make_float2(-ca[2 * j].x, -ca[2 * j].y)), i01);
-            const float2 db0 = __fmul2_rn(__fadd2_rn(c01, make_float2(-cb[2 * j].x, -cb[2 * j].y)), i01);
-            const float2 da1 = __fmul2_rn(__fadd2_rn(c23, make_float2(-ca[2 * j + 1].x, -ca[2 * j + 1].y)), i23);
-            const float2 db1 = __fmul2_rn(__fadd2_rn(c23, make_float2(-cb[2 * j + 1].x, -cb[2 * j + 1].y)), i23);
-            aa = __ffma2_rn(da0, da0, aa);
-            bb = __ffma2_rn(db0, db0, bb);
-            aa = __ffma2_rn(da1, da1, aa);
-            bb = __ffma2_rn(db1, db1, bb);
+            const float2 da0 = fmul2(fadd2(c01, make_float2(-ca[2 * j].x, -ca[2 * j].y)), i01);
+            const float2 db0 = fmul2(fadd2(c01, make_float2(-cb[2 * j].x, -cb[2 * j].y)), i01);
+            const float2 da1 = fmul2(fadd2(c23, make_float2(-ca[2 * j + 1].x, -ca[2 * j + 1].y)), i23);
+            const float2 db1 = fmul2(fadd2(c23, make_float2(-cb[2 * j + 1].x, -cb[2 * j + 1].y)), i23);
+            aa = ffma2(da0, da0, aa);
+            bb = ffma2(db0, db0, bb);
+            aa = ffma2(da1, da1, aa);
+            bb = ffma2(db1, db1, bb);
           }
           const float al = s_al[m * KM_NS + i];
-          acc = __ffma2_rn(stationary2_f(make_float2(aa.x + aa.y, bb.x + bb.y), kind), make_float2(al, al), acc);
+          acc = ffma2(stationary2_f(make_float2(aa.x + aa.y, bb.x + bb.y), kind), make_float2(al, al), acc);
         }
         sum_a[m] += (double)acc.x;
         sum_b[m] += (double)acc.y;
@@ -948,14 +757,14 @@ __global__ void __launch_bounds__(KM_T, 3)
             for (int j = 0; j < KM_D / 4; ++j) {
               const float4 c = xr[j];
               const float2 c01 = make_float2(c.x, c.y), c23 = make_float2(c.z, c.w);
-              const float2 da0 = __fadd2_rn(c01, make_float2(-ca[2 * j].x, -ca[2 * j].y));
-              const float2 db0 = __fadd2_rn(c01, make_float2(-cb[2 * j].x, -cb[2 * j].y));
-              const float2 da1 = __fadd2_rn(c23, make_float2(-ca[2 * j + 1].x, -ca[2 * j + 1].y));
-              const float2 db1 = __fadd2_rn(c23, make_float2(-cb[2 * j + 1].x, -cb[2 * j + 1].y));
-              a0 = __ffma2_rn(da0, da0, a0);
-              b0 = __ffma2_rn(db0, db0, b0);
-              a1 = __ffma2_rn(da1, da1, a1);
-              b1 = __ffma2_rn(db1, db1, b1);
+              const float2 da0 = fadd2(c01, make_float2(-ca[2 * j].x, -ca[2 * j].y));
+              const float2 db0 = fadd2(c01, make_float2(-cb[2 * j].x, -cb[2 * j].y));
+              const float2 da1 = fadd2(c23, make_float2(-ca[2 * j + 1].x, -ca[2 * j + 1].y));
+              const float2 db1 = fadd2(c23, make_float2(-cb[2 * j + 1].x, -cb[2 * j + 1].y));
+              a0 = ffma2(da0, da0, a0);
+              b0 = ffma2(db0, db0, b0);
+              a1 = ffma2(da1, da1, a1);
+              b1 = ffma2(db1, db1, b1);
             }
             r2 = make_float2((a0.x + a0.y) + (a1.x + a1.y), (b0.x + b0.y) + (b1.x + b1.y));
           }
@@ -966,7 +775,7 @@ __global__ void __launch_bounds__(KM_T, 3)
             if (ISO) {
               const float il = s_il[m * KM_D];
               const float il2 = il * il;
-              rr = __fmul2_rn(r2, make_float2(il2, il2));
+              rr = fmul2(r2, make_float2(il2, il2));
             } else {
               const float4* il4 = reinterpret_cast<const float4*>(s_il + m * KM_D);
               float2 aa = make_float2(0.f, 0.f), bb = aa;
@@ -975,22 +784,22 @@ __global__ void __launch_bounds__(KM_T, 3)
                 const float4 c = xr[j], il = il4[j];
                 const float2 c01 = make_float2(c.x, c.y), c23 = make_float2(c.z, c.w);
                 const float2 i01 = make_float2(il.x, il.y), i23 = make_float2(il.z, il.w);
-                const float2 da0 = __fmul2_rn(__fadd2_rn(c01, make_float2(-ca[2 * j].x, -ca[2 * j].y)), i01);
-                const float2 db0 = __fmul2_rn(__fadd2_rn(c01, make_float2(-cb[2 * j].x, -cb[2 * j].y)), i01);
-                const float2 da1 = __fmul2_rn(__fadd2_rn(c23, make_float2(-ca[2 * j + 1].x, -ca[2 * j + 1].y)), i23);
-                const float2 db1 = __fmul2_rn(__fadd2_rn(c23, make_float2(-cb[2 * j + 1].x, -cb[2 * j + 1].y)), i23);
-                aa = __ffma2_rn(da0, da0, aa);
-                bb = __ffma2_rn(db0, db0, bb);
-                aa = __ffma2_rn(da1, da1, aa);
-                bb = __ffma2_rn(db1, db1, bb);
+                const float2 da0 = fmul2(fadd2(c01, make_float2(-ca[2 * j].x, -ca[2 * j].y)), i01);
+                const float2 db0 = fmul2(fadd2(c01, make_float2(-cb[2 * j].x, -cb[2 * j].y)), i01);
+                const float2 da1 = fmul2(fadd2(c23, make_float2(-ca[2 * j + 1].x, -ca[2 * j + 1].y)), i23);
+                const float2 db1 = fmul2(fadd2(c23, make_float2(-cb[2 * j + 1].x, -cb[2 * j + 1].y)), i23);
+                aa = ffma2(da0, da0, aa);
+                bb = ffma2(db0, db0, bb);
+                aa = ffma2(da1, da1, aa);
+                bb = ffma2(db1, db1, bb);
               }
               rr = make_float2(aa.x + aa.y, bb.x + bb.y);
             }
             const float2 k0 = stationary2_f(rr, kind);
             const float al = s_al[m * KF_NS + i];
-            acc[m] = __ffma2_rn(k0, make_float2(al, al), acc[m]);
+            acc[m] = ffma2(k0, make_float2(al, al), acc[m]);
             const float sc = s_c[m] * live;
-            kv[u][m] = __fmul2_rn(k0, make_float2(sc, sc));  // c * k(r), scaled by 2^kexp (exact); padding columns: 0
+            kv[u][m] = fmul2(k0, make_float2(sc, sc));  // c * k(r), scaled by 2^kexp (exact); padding columns: 0
           }
         }
 #pragma unroll
@@ -1249,27 +1058,25 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
   if (!d_var && d <= KM_D && M <= 6 && !(getenv("DMO_GP_MEAN_DIRECT") && atoi(getenv("DMO_GP_MEAN_DIRECT")) == 0))
     return gp_mean_direct(ctx, gp, dXn, P, d_mean);  // nothing but the mean is wanted: K_* stays in registers
   DMO_TRY(prepare_tensor_state(ctx, gp));
-  // kernel version: 3 (default) = equal-cost paired row blocks in L2-friendly order, overlapped with the K_* producer;
-  // 2 = previous schedule, K_* / mean / variance back to back on one stream (DMO_GP_TC=2, kept for comparison)
+  // work schedule of the contraction: 3 (default) = equal-cost paired row blocks, optionally overlapped with the K_*
+  // producer; 2 = the previous schedule, two halves of the row blocks per candidate block (DMO_GP_TC=2, kept for comparison)
   int version = 3;
   if (const char* e = getenv("DMO_GP_TC")) version = atoi(e) == 2 ? 2 : 3;
   // DMO_GP_OVERLAP=1 (experimental, off by default): launch the contraction while the K_* producer is still running on
-  // the context's second stream and let its TMA thread wait on per-candidate-block completion counters.  Measured on
-  // B200 (profiles/README.md, round 2): no gain -- the contraction is power-capped, co-running FP32 work lowers its clock
-  // by what the overlap hides (10.35 ms vs 9.98 ms per predict at P = 65 536) -- and the co-residency of the two kernels
-  // is not guaranteed by the hardware scheduler (a launch at P = 4608 failed), so the in-line order is the product path.
+  // the context's second stream and let its TMA thread wait on per-candidate-block completion counters.  The
+  // co-residency of the two kernels is not guaranteed by the hardware scheduler, so the in-line order is the product path.
   const bool overlap = version == 3 && getenv("DMO_GP_OVERLAP") && atoi(getenv("DMO_GP_OVERLAP"));
   const int dbg = getenv("DMO_GP_DBG") ? atoi(getenv("DMO_GP_DBG")) : 0;  // 4: event instead of flags, 8: mean after var
   const bool use_flags = overlap && !(dbg & 4);
   // mean from the contraction (D z) instead of the K_* alpha pass: only with the variance, version 3 and a model created from L
   mean_from_d = mean_from_d && d_var != nullptr && version == 3 && gp->z_ready;
-  constexpr int64_t TMv = v2::TM2;
+  constexpr int64_t TMv = KM_Q;  // candidate padding: the K_* producers write 256-candidate blocks
   // candidate chunk: K_* hi/lo (2 x M x Pc x Npad fp16) within ~6 GiB
   int64_t Pc_max = ((int64_t)6 << 30) / ((int64_t)M * Npad * 4);
   Pc_max = (Pc_max / TMv) * TMv;
   if (Pc_max < TMv) Pc_max = TMv;
   const int64_t Pc_alloc = P < Pc_max ? ceil_div(P, TMv) * TMv : Pc_max;
-  const int n_jt = (int)(Npad / v2::TN2);
+  const int n_jt = (int)(Npad / TN);
   const int n_q = version == 3 ? (n_jt + 1) / 2 : 2;
   const int64_t n_chunks = ceil_div(P, Pc_alloc);
   const int n_pb_alloc = (int)(Pc_alloc / TMv);
@@ -1287,12 +1094,11 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
   DMO_CUDA(cudaMemsetAsync(abort_flag.p, 0, sizeof(int), ctx->stream));
   DMO_CUDA(cudaMemsetAsync(ready.p, 0, (size_t)n_chunks * n_pb_alloc * sizeof(unsigned), ctx->stream));
   CUtensorMap map_kh, map_kl, map_lh, map_ll;
-  DMO_TRY(make_map(ctx, &map_kh, Kh.p, (uint64_t)M * Pc_alloc, (uint64_t)Npad, 256, v2::TK2, CU_TENSOR_MAP_SWIZZLE_64B));
-  DMO_TRY(make_map(ctx, &map_kl, Kl.p, (uint64_t)M * Pc_alloc, (uint64_t)Npad, 256, v2::TK2, CU_TENSOR_MAP_SWIZZLE_64B));
-  DMO_TRY(make_map(ctx, &map_lh, gp->Lhi.p, (uint64_t)M * Npad, (uint64_t)Npad, 256, v2::TK2, CU_TENSOR_MAP_SWIZZLE_64B));
-  DMO_TRY(make_map(ctx, &map_ll, gp->Llo.p, (uint64_t)M * Npad, (uint64_t)Npad, 256, v2::TK2, CU_TENSOR_MAP_SWIZZLE_64B));
-  DMO_CUDA(cudaFuncSetAttribute(v2::gp_var_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)v2::GEMM_SMEM2));
-  DMO_CUDA(cudaFuncSetAttribute(v3::gp_var_tc3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)v2::GEMM_SMEM2));
+  DMO_TRY(make_map(ctx, &map_kh, Kh.p, (uint64_t)M * Pc_alloc, (uint64_t)Npad, TMV, TK, CU_TENSOR_MAP_SWIZZLE_64B));
+  DMO_TRY(make_map(ctx, &map_kl, Kl.p, (uint64_t)M * Pc_alloc, (uint64_t)Npad, TMV, TK, CU_TENSOR_MAP_SWIZZLE_64B));
+  DMO_TRY(make_map(ctx, &map_lh, gp->Lhi.p, (uint64_t)M * Npad, (uint64_t)Npad, TN, TK, CU_TENSOR_MAP_SWIZZLE_64B));
+  DMO_TRY(make_map(ctx, &map_ll, gp->Llo.p, (uint64_t)M * Npad, (uint64_t)Npad, TN, TK, CU_TENSOR_MAP_SWIZZLE_64B));
+  DMO_CUDA(cudaFuncSetAttribute(gp_var_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GEMM_SMEM));
   const int64_t kplane = Pc_alloc * Npad;
   // K_* producer fused with the mean (d <= 32, M <= 6; DMO_GP_FUSED=0 keeps kstar_tensor_kernel + mean_split_kernel)
   // (per-dimension length scales with more than two objectives spill in the fused kernel: they keep the two-kernel route)
@@ -1384,12 +1190,26 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
       }
 }
     if (overlap) DMO_CUDA(cudaEventRecord(ctx->ev_join, ctx->aux));
-    if (d_var && version == 3) {
-      v3::GemmParams3 prm;
+    if (d_var) {
+      GemmParams prm;
       prm.M = M;
-      prm.n_pb = (int)(Pcpad / TMv);
+      prm.n_pb = (int)(Pcpad / TMV);
       prm.n_jt = n_jt;
       prm.n_q = n_q;
+      prm.paired = version == 3;
+      // halves: split the row blocks where the cumulative MMA count sum_{j < J} (j + 1) is closest to half of the total
+      prm.j_split = n_jt;
+      if (!prm.paired) {
+        const int64_t tot = (int64_t)n_jt * (n_jt + 1) / 2;
+        int64_t best_d = tot;
+        for (int J = 0; J <= n_jt; ++J) {
+          const int64_t dlt = llabs(2 * ((int64_t)J * (J + 1) / 2) - tot);
+          if (dlt < best_d) {
+            best_d = dlt;
+            prm.j_split = J;
+          }
+        }
+      }
       prm.k_rows = Pc_alloc;
       prm.l_rows = Npad;
       prm.inv_scale = gp->Lscale.p;
@@ -1405,46 +1225,13 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
       const int grid = n_work < ctx->sm_count ? n_work : ctx->sm_count;
       {
         ProfileScope ps_(ctx, "gp_var");
-        DMO_LAUNCH(v3::gp_var_tc3_kernel, grid, NTHREADS, v2::GEMM_SMEM2, map_kh, map_kl, map_lh, map_ll, prm);
+        DMO_LAUNCH(gp_var_wgmma_kernel, grid, NTHREADS, GEMM_SMEM, map_kh, map_kl, map_lh, map_ll, prm);
       }
       DMO_LAUNCH(var_finish_tc_kernel, (unsigned)ceil_div(Pc * M, 256), 256, 0, vnorm.p, n_q, Pc, Pc_alloc, M,
                  gp->constant.p, gp->noise.p, gp->ystd.p, p_base, d_var);
       if (mean_from_d)
         DMO_LAUNCH(mean_finish_tc_kernel, (unsigned)ceil_div(Pc * M, 256), 256, 0, mnorm.p, n_q, Pc, Pc_alloc, M, gp->ymean.p,
                    gp->ystd.p, p_base, d_mean);
-    } else if (d_var) {
-      v2::GemmParams2 prm;
-      prm.M = M;
-      prm.n_pb = (int)(Pcpad / v2::TM2);
-      prm.n_jt = n_jt;
-      // split the row blocks where the cumulative MMA count sum_{j < J} (j + 1) is closest to half of the total
-      {
-        const int64_t tot = (int64_t)prm.n_jt * (prm.n_jt + 1) / 2;
-        int best_j = prm.n_jt;
-        int64_t best_d = tot;
-        for (int J = 0; J <= prm.n_jt; ++J) {
-          const int64_t dlt = llabs(2 * ((int64_t)J * (J + 1) / 2) - tot);
-          if (dlt < best_d) {
-            best_d = dlt;
-            best_j = J;
-          }
-        }
-        prm.j_split = best_j;
-      }
-      prm.k_rows = Pc_alloc;
-      prm.l_rows = Npad;
-      prm.inv_scale = gp->Lscale.p;
-      prm.vnorm = vnorm.p;
-      prm.vn_ld = Pc_alloc;
-      prm.abort_flag = abort_flag.p;
-      const int n_work = prm.M * prm.n_pb * 2;
-      const int grid = n_work < ctx->sm_count ? n_work : ctx->sm_count;
-      {
-        ProfileScope ps_(ctx, "gp_var");
-        DMO_LAUNCH(v2::gp_var_tc2_kernel, grid, NTHREADS, v2::GEMM_SMEM2, map_kh, map_kl, map_lh, map_ll, prm);
-      }
-      DMO_LAUNCH(var_finish_tc_kernel, (unsigned)ceil_div(Pc * M, 256), 256, 0, vnorm.p, 2, Pc, Pc_alloc, M,
-                 gp->constant.p, gp->noise.p, gp->ystd.p, p_base, d_var);
     }
     if (overlap) DMO_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));  // mean (and K_*) of this chunk done
     if ((dbg & 8) && !mean_from_d) {

@@ -1,4 +1,4 @@
-"""Exact-GP surrogates on the B200 path: drop-ins for ``dmosopt.model.GPR_Matern`` / ``GPR_RBF``.
+"""Exact-GP surrogates on the GPU path: drop-ins for ``dmosopt.model.GPR_Matern`` / ``GPR_RBF``.
 
 Reference: dmosopt/model.py:1182-1275 (GPR_Matern) and :1278-1364 (GPR_RBF); selected in dmosopt by
 ``surrogate_method_name="dmosopt_b200.GPR_Matern"`` (dmosopt/MOASMO.py:516-530).  The constructor
@@ -79,7 +79,7 @@ class _GPRBase:
         self.xrg = self.xub - self.xlb
         self.logger = logger
         self.return_mean_variance = return_mean_variance
-        # "auto" (default): the tcgen05 path wherever a per-model calibration against the float64 path holds the
+        # "auto" (default): the tensor-core path wherever a per-model calibration against the float64 path holds the
         # 1e-5 bar, float64 for the rest (csrc/gp.cu, DMO_GP_AUTO); "tensor" / "fp64" force one arithmetic
         codes = {"auto": _lib.GP_AUTO, "tensor": _lib.GP_TENSOR, "fp64": _lib.GP_FP64,
                  _lib.GP_AUTO: _lib.GP_AUTO, _lib.GP_TENSOR: _lib.GP_TENSOR, _lib.GP_FP64: _lib.GP_FP64}

@@ -1,4 +1,4 @@
-"""gpytorch exact-GP surrogate on the B200 path: ``EGP_Matern`` (row A19).
+"""gpytorch exact-GP surrogate on the GPU path: ``EGP_Matern`` (row A19).
 
 Drop-in for ``dmosopt.model_gpytorch.EGP_Matern`` (dmosopt/model_gpytorch.py:1927-2235), selected in dmosopt by
 ``surrogate_method_name="dmosopt_b200.model_gpytorch.EGP_Matern"``.  As with the scikit-learn surrogates, *fitting*

@@ -1,5 +1,5 @@
 /*
- * dmosopt_b200 -- C ABI of the B200-native surrogate-generation hot path.
+ * dmosopt_b200 -- C ABI of the H100-native surrogate-generation hot path.
  *
  * The reference (dmosopt @ 5cd63e4c) is pure Python and has NO foreign-function
  * interface; this header is new surface that sits directly under the Python
@@ -51,7 +51,7 @@ extern "C" {
 
 /* arithmetic used for the GP posterior variance contraction */
 #define DMO_GP_FP64 0   /* CUDA-core float64 everywhere: matches sklearn to ~1e-10               */
-#define DMO_GP_TENSOR 1 /* tcgen05 split-fp16 (3 MMAs / product), fp32 accumulate in TMEM        */
+#define DMO_GP_TENSOR 1 /* wgmma split-fp16 (3 MMAs / product), fp32 accumulate in registers     */
 #define DMO_GP_AUTO 2   /* tensor path where a per-model calibration against the float64 path   *
                          * holds 1e-5, float64 for the rest (rows with small variance, badly   *
                          * conditioned models): see dmo_gp_auto_info                            */
@@ -218,7 +218,7 @@ int dmo_gp_predict(dmo_ctx* ctx, dmo_gp* gp, const double* X, int64_t P, double*
  * both arithmetic paths predict 512 probe candidates; mean_tensor bit 0 = the fp32-K_* alpha pass is
  * admitted (predicts with variance), bit 1 = the mean is taken from the variance contraction (D z, predicts with
  * variance), bit 2 = the mean-only kernel (K_* never written, fp32 kernel values, float64 partial sums) is admitted
- * for predicts without variance; var_tensor = 1 when the tcgen05 variance is admitted; errors relative to max(|mean|, y_std) and to
+ * for predicts without variance; var_tensor = 1 when the wgmma variance is admitted; errors relative to max(|mean|, y_std) and to
  * the prior variance, margins documented in csrc/gp.cu; theta: rows whose tensor variance is
  * below theta * prior are recomputed in float64; last_refined: rows the last AUTO predict recomputed
  * (= P when the whole call ran in float64).  Any output pointer may be NULL. */

@@ -77,7 +77,7 @@ def gp_sweep():
 def stream_sweep():
     """The HBM-bound kernels at the BASELINE shape: crowding / euclidean distance (n = 131072, M = 3), SBX + mutation
     (pop 65536, d 30), mean kernel's neighbours, hypervolume of a 65536-point 3-D front.  Prints time and the achieved
-    fraction of the algorithmic bytes; run under ncu for the DRAM counters (profiles/README.md)."""
+    fraction of the algorithmic bytes."""
     L.context()
     rng = np.random.default_rng(2)
     lib, ctx = L.load_library(), L.context()

@@ -1,15 +1,15 @@
 #!/usr/bin/env python
 """Generate golden input/output vectors from the *reference itself*.
 
-Run in the build container, where the reference checkout is mounted read-only:
+Run with the reference package importable (a checkout of dmosopt on PYTHONPATH):
 
-    PYTHONPATH=/root/reference PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
+    PYTHONPATH=<dmosopt checkout> PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py [name ...]
 
 It imports dmosopt's own modules (dda, indicators, MOEA, NSGA2, AGEMOEA, SMPSO,
 CMAES, hv, hv_box_decomposition, model + scikit-learn) and records seeded
 inputs together with the outputs the reference produces, as small ``.npz``
-files next to this script.  The reference cannot travel to the GPU box, the
-fixtures do; ``tests/test_oracle_golden.py`` pins the oracle to them and the
+files next to this script.  The tests need only the fixtures, not the
+reference; ``tests/test_oracle_golden.py`` pins the oracle to them and the
 ``-m gpu`` tests pin the CUDA path to the same files.
 
 Nothing outside ``tests/golden/`` is written.
@@ -798,8 +798,30 @@ def gen_trs(rng):
     save("trs", **out)
 
 
+def gen_helpers(rng):
+    """The controller helpers dmosopt_b200.install() routes to the GPU, on the inputs of
+    tests/test_gpu_reference_loop.py::test_install_routes_controller_helpers_to_the_gpu_with_identical_results
+    (MOEA.get_duplicates, MOEA.sortMO, MOEA.crowding_distance_metric, hv.AdaptiveHyperVolume.compute_hypervolume)."""
+    rng = np.random.default_rng(21)
+    n, d, M = 700, 9, 3
+    x = rng.random((n, d))
+    y = np.column_stack((x[:, 0] + 0.1, (1.1 - x[:, 0]) * (1 + x[:, 1]), 0.2 + x[:, 2] ** 2 + x[:, 1]))
+    y[50] = y[3]
+    y[400] = y[3]
+    x0 = rng.random((300, d))
+    x0[:40] = x[100:140]
+    ref_pt = y.max(axis=0) + 0.1
+    y_tf = y[np.r_[0:50, 51:400, 401:n]]  # tie-free columns: with exact ties the reference's own crowding depends on argsort's order
+    dup_y = MOEA.get_duplicates(y)
+    xs, ys, rank, _, perm = MOEA.sortMO(x[~dup_y], y[~dup_y], return_perm=True)
+    assert np.array_equal(xs, x[~dup_y][perm]) and np.array_equal(ys, y[~dup_y][perm])  # the test checks the order via perm
+    # outputs only: the test regenerates the inputs from the same seed
+    save("helpers", dup_x=MOEA.get_duplicates(x, x0), dup_y=dup_y, sort_rank=np.asarray(rank), sort_perm=np.asarray(perm),
+         cd=MOEA.crowding_distance_metric(y_tf), hv=np.array(hv_mod.AdaptiveHyperVolume(ref_pt).compute_hypervolume(y[:300])))
+
+
 def main():
-    which = sys.argv[1:] or ["dda", "distance", "sortmo", "variation", "tournament", "duplicates", "gp", "hv", "ehvi", "nsga2", "agemoea", "smpso", "cmaes", "plugins", "trs", "adaptive", "hv_many"]
+    which = sys.argv[1:] or ["dda", "distance", "sortmo", "variation", "tournament", "duplicates", "gp", "hv", "ehvi", "nsga2", "agemoea", "smpso", "cmaes", "plugins", "trs", "adaptive", "hv_many", "helpers"]
     gens = {
         "dda": gen_dda,
         "distance": gen_distance,
@@ -818,6 +840,7 @@ def main():
         "trs": gen_trs,
         "adaptive": gen_adaptive,
         "hv_many": gen_hv_many,
+        "helpers": gen_helpers,
     }
     for i, name in enumerate(which):
         gens[name](np.random.default_rng(20260921 + i * 0 + sum(map(ord, name))))

@@ -3,6 +3,7 @@
 import ctypes
 import os
 import re
+import shutil
 import subprocess
 
 import pytest
@@ -46,9 +47,11 @@ def test_python_binding_covers_every_header_symbol(lib_path):
     _lib.load_library()  # declares all prototypes; raises if a symbol is missing
 
 
-def test_library_is_built_for_sm_100a(lib_path):
-    out = subprocess.run(["cuobjdump", "-lelf", lib_path], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+def test_library_is_built_for_sm_90a(lib_path):
+    cuobjdump = shutil.which("cuobjdump") or os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "cuobjdump")
+    out = subprocess.run([cuobjdump, "-lelf", lib_path], capture_output=True, text=True).stdout
+    cubins = re.findall(r"\.(sm_\w+)\.cubin", out)
+    assert cubins and set(cubins) == {"sm_90a"}, out
 
 
 def test_no_gpu_means_loud_failure(lib_path):

@@ -324,7 +324,7 @@ def _handle_from_state(L, st, d):
 
 @pytest.mark.parametrize("N,d,M,P", [(300, 30, 3, 200), (1000, 12, 2, 517), (2048, 30, 3, 1500), (600, 22, 5, 700)])
 def test_gp_predict_tensor_path(L, N, d, M, P):
-    """tcgen05 split-fp16 path: |var - var_ref| <= 1e-5 * prior variance, |mean - mean_ref| <= 1e-5 * max(|mean|, y_std)."""
+    """wgmma split-fp16 path: |var - var_ref| <= 1e-5 * prior variance, |mean - mean_ref| <= 1e-5 * max(|mean|, y_std)."""
     rng, xlb, xub, Xtr, st = _baseline_gp(N, d, M, 100 + N)
     X = rng.random((P, d))
     X[:6] = np.clip(Xtr[:6] + 2e-3 * rng.standard_normal((6, d)), 0, 1)  # small posterior variance rows

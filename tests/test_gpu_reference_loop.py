@@ -1,9 +1,9 @@
 """The real thing on hardware: the UNMODIFIED reference controller loop (dmosopt/MOASMO.py:196-470, MOASMO.epoch) driving
-the B200 plugins by import path on the GPU, and the plain-C host of include/dmosopt_b200.h executed on the GPU.
+the GPU plugins by import path, the controller helpers routed to the GPU by install(), and the plain-C host of
+include/dmosopt_b200.h executed on the GPU.
 
-The reference package is taken from ``baseline/_ref`` (the unmodified dmosopt modules installed there by pip from a copy
-of /root/reference, git-ignored, shipped to the GPU box by gpurun) or from ``$DMOSOPT_REF``; /root/reference itself is
-never read at run time.
+The tests that run the reference's own code take the dmosopt package that build() compiles into ``oracle/_ref``
+(git-ignored; oracle/reference_build.py), ``$DMOSOPT_REF`` or ``baseline/_ref``, and skip without one; the install() test compares with stored reference results (tests/golden/helpers.npz).
 """
 
 import os
@@ -20,10 +20,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _reference_path():
-    for p in (os.environ.get("DMOSOPT_REF"), os.path.join(ROOT, "baseline", "_ref")):
-        if p and os.path.isdir(os.path.join(p, "dmosopt")):
-            return p
-    return None
+    from oracle import reference_build
+
+    return reference_build.reference_path()
 
 
 def _zdt1(x):
@@ -32,7 +31,7 @@ def _zdt1(x):
     return np.column_stack((x[:, 0], g * (1.0 - np.sqrt(x[:, 0] / g))))
 
 
-@pytest.mark.skipif(_reference_path() is None, reason="reference package not shipped (baseline/_ref or $DMOSOPT_REF)")
+@pytest.mark.skipif(_reference_path() is None, reason="reference package not built (oracle/_ref) nor given ($DMOSOPT_REF)")
 @pytest.mark.parametrize("optimizer,kwargs", [("dmosopt_b200.NSGA2", {}), ("dmosopt_b200.AGEMOEA", {}), ("dmosopt_b200.SMPSO", {}), ("dmosopt_b200.CMAES", {})])
 def test_unmodified_moasmo_epoch_drives_the_gpu_plugins(optimizer, kwargs):
     """MOASMO.epoch resolves optimizer_name / surrogate_method_name by import path (config.py:5-11), fits the surrogate
@@ -138,24 +137,34 @@ def test_plain_c_host_runs_the_resident_step_on_the_gpu(tmp_path):
     assert all(b >= a - 1e-12 for a, b in zip(hv, hv[1:])), hv  # elitist survival: the hypervolume never shrinks
 
 
-@pytest.mark.skipif(_reference_path() is None, reason="reference package not shipped")
-def test_install_routes_controller_helpers_to_the_gpu_with_identical_results():
-    """dmosopt_b200.install(): MOASMO.get_best (duplicates + sortMO, MOASMO.py:581-639), the resample helpers
-    (MOASMO.py:441-448) and the termination hypervolume (hv.py:123-189) give the reference's own results -- computed
-    first with the untouched reference, then again after the routing hook."""
-    ref = _reference_path()
-    sys.path.insert(0, ref)
-    try:
-        import dmosopt.hv as rhv
-        import dmosopt.MOASMO as rMOASMO
-        import dmosopt.MOEA as rMOEA
-    finally:
-        sys.path.remove(ref)
+_STUB_MODULES = {
+    "MOEA": "def _absent(*a, **k):\n    raise AssertionError('not routed')\n\n"
+            + "".join(f"{n} = _absent\n" for n in ("get_duplicates", "remove_duplicates", "sortMO", "orderMO", "remove_worst",
+                                                    "crowding_distance_metric", "euclidean_distance_metric", "dda_ens")),
+    "indicators": "def crowding_distance_metric(*a, **k):\n    raise AssertionError('not routed')\n",
+    "dda": "def dda_ens(*a, **k):\n    raise AssertionError('not routed')\n",
+    "hv": ("class AdaptiveHyperVolume:\n    dimension_threshold_exact = 6\n\n    def __init__(self, ref_point):\n"
+           "        self.ref_point = ref_point\n        self.n_objectives = len(ref_point)\n\n"
+           "    def compute_hypervolume(self, pareto_front, algorithm=None, verbose=False):\n        raise AssertionError('not routed')\n"),
+}
+
+
+def test_install_routes_controller_helpers_to_the_gpu_with_identical_results(golden, tmp_path):
+    """dmosopt_b200.install(): the helpers the reference controller calls on its own modules -- MOEA.get_duplicates and
+    MOEA.sortMO (MOASMO.get_best, MOASMO.py:581-639), MOEA.crowding_distance_metric (resample step, MOASMO.py:441-448)
+    and the termination hypervolume (hv.py:123-189) -- are rebound to the GPU and give the reference's own results
+    (tests/golden/helpers.npz).  The rebinding is exercised on a stand-in package with the reference's module layout."""
     import dmosopt_b200 as b2
     from dmosopt_b200 import _lib
 
-    rng = np.random.default_rng(21)
-    n, d, M = 700, 9, 3
+    pkg = tmp_path / "refstub"
+    pkg.mkdir()
+    (pkg / "__init__.py").write_text("")
+    for name, src in _STUB_MODULES.items():
+        (pkg / f"{name}.py").write_text(src)
+    g = golden("helpers")
+    rng = np.random.default_rng(21)  # the inputs tests/golden/make_golden.py (gen_helpers) gave the reference
+    n, d = 700, 9
     x = rng.random((n, d))
     y = np.column_stack((x[:, 0] + 0.1, (1.1 - x[:, 0]) * (1 + x[:, 1]), 0.2 + x[:, 2] ** 2 + x[:, 1]))
     y[50] = y[3]
@@ -163,26 +172,31 @@ def test_install_routes_controller_helpers_to_the_gpu_with_identical_results():
     x0 = rng.random((300, d))
     x0[:40] = x[100:140]
     ref_pt = y.max(axis=0) + 0.1
-    # reference results, untouched
-    best_ref = rMOASMO.get_best(x, y, None, None, d, M, return_perm=True)
-    dup_ref = rMOEA.get_duplicates(x, x0)
-    y_tf = y[np.r_[0:50, 51:400, 401:n]]  # tie-free columns: with exact ties the reference's own crowding depends on argsort's order
-    cd_ref = rMOEA.crowding_distance_metric(y_tf)
-    hv_ref = rhv.AdaptiveHyperVolume(ref_pt).compute_hypervolume(y[:300])
-    launches0 = _lib.launch_count()
-    patched = b2.install()
+    sys.path.insert(0, str(tmp_path))
     try:
-        assert any(name.endswith("get_duplicates") for name in patched)
-        best_gpu = rMOASMO.get_best(x, y, None, None, d, M, return_perm=True)
-        dup_gpu = rMOEA.get_duplicates(x, x0)
-        cd_gpu = rMOEA.crowding_distance_metric(y_tf)
-        hv_gpu = rhv.AdaptiveHyperVolume(ref_pt).compute_hypervolume(y[:300])
+        import refstub.hv as rhv
+        import refstub.MOEA as rMOEA
+
+        launches0 = _lib.launch_count()
+        patched = b2.install(package="refstub")
+        try:
+            assert any(name.endswith("get_duplicates") for name in patched)
+            dup_x = rMOEA.get_duplicates(x, x0)
+            dup_y = rMOEA.get_duplicates(y)
+            xs, ys, rank, _, perm = rMOEA.sortMO(x[~dup_y], y[~dup_y], return_perm=True)
+            cd = rMOEA.crowding_distance_metric(y[np.r_[0:50, 51:400, 401:n]])
+            hv = rhv.AdaptiveHyperVolume(ref_pt).compute_hypervolume(y[:300])
+        finally:
+            b2.uninstall()
+        assert _lib.launch_count() > launches0
+        assert rMOEA.get_duplicates.__module__ == "refstub.MOEA"  # restored
     finally:
-        b2.uninstall()
-    assert _lib.launch_count() > launches0
-    assert rMOEA.get_duplicates.__module__.startswith("dmosopt.")  # restored
-    for a, b in zip(best_ref, best_gpu):
-        assert (a is None and b is None) or np.array_equal(np.asarray(a), np.asarray(b))
-    assert np.array_equal(dup_ref, dup_gpu) and dup_ref.sum() == 40
-    assert np.array_equal(cd_ref, cd_gpu)  # float64 bit-exact crowding (tie-free columns)
-    assert abs(hv_gpu - hv_ref) <= 1e-9 * abs(hv_ref)
+        sys.path.remove(str(tmp_path))
+        for m in [m for m in sys.modules if m == "refstub" or m.startswith("refstub.")]:
+            del sys.modules[m]
+    assert np.array_equal(dup_x, g["dup_x"]) and dup_x.sum() == 40
+    assert np.array_equal(dup_y, g["dup_y"])
+    assert np.array_equal(np.asarray(rank), g["sort_rank"]) and np.array_equal(np.asarray(perm), g["sort_perm"])
+    assert np.array_equal(xs, x[~dup_y][g["sort_perm"]]) and np.array_equal(ys, y[~dup_y][g["sort_perm"]])
+    assert np.array_equal(cd, g["cd"])  # float64 bit-exact crowding (tie-free columns)
+    assert abs(hv - float(g["hv"])) <= 1e-9 * abs(float(g["hv"]))

@@ -1,7 +1,7 @@
 """Host-side logic of the plugins (no GPU): the ``_lib`` calls are replaced by the oracle-backed test seam.
 
 Checks the state handling / dtype flow of dmosopt_b200.NSGA2 and GPR_Matern against golden vectors recorded
-from the reference plugin, and -- when the reference checkout is present (build container) -- drives the plugins
+from the reference plugin, and -- with the reference package that build() compiles into oracle/_ref -- drives the plugins
 from the reference's own, unmodified ``MOASMO.epoch``.
 """
 
@@ -13,8 +13,9 @@ import pytest
 
 import fake_backend
 from conftest import load_golden
+from oracle import reference_build
 
-REFERENCE = "/root/reference"
+REFERENCE = reference_build.reference_path()  # the compiled reference package (oracle/_ref), or $DMOSOPT_REF
 
 
 @pytest.fixture
@@ -186,7 +187,6 @@ def test_age_smpso_cmaes_plugins_reproduce_reference(fake):
     _run_plugin_goldens(b2)
 
 
-@pytest.mark.skipif(not os.path.isdir(os.path.join(REFERENCE, "dmosopt")), reason="reference checkout not present")
 def test_adaptive_helpers_reproduce_reference(fake):
     """update_population_size (NSGA2 / AGEMOEA / SMPSO / CMAES / TRS) and update_operator_rates (NSGA2 / SMPSO) against
     the reference's own results on crafted states (tests/golden/adaptive.npz): host control logic of the plugin contract."""
@@ -241,6 +241,7 @@ def test_adaptive_helpers_reproduce_reference(fake):
             np.testing.assert_allclose(got, g[f"smpso_rates{k}"][rnd], rtol=1e-15, atol=0, err_msg=str((k, rnd)))
 
 
+@pytest.mark.skipif(REFERENCE is None, reason="reference package not built (oracle/_ref) nor given ($DMOSOPT_REF)")
 def test_plugins_drop_into_unmodified_moasmo_epoch(fake):
     """The reference's own MOASMO.epoch (dmosopt/MOASMO.py:196-470) drives the plugins by import path."""
     sys.path.insert(0, REFERENCE)
