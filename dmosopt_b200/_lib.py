@@ -71,6 +71,10 @@ _SIGNATURES = {
     "dmo_gp_predict": (_c_int, [_vp, _vp, _vp, _c_i64, _vp, _vp, _c_int]),
     "dmo_gp_auto_info": (_c_int, [_vp, _vp, ctypes.POINTER(_c_int), ctypes.POINTER(_c_int), ctypes.POINTER(_c_dbl), ctypes.POINTER(_c_dbl),
                                   ctypes.POINTER(_c_dbl), ctypes.POINTER(_c_i64)]),
+    "dmo_mtgp_create": (_c_int, [_vp, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.POINTER(_c_dbl),
+                                 ctypes.POINTER(_vp)]),
+    "dmo_mtgp_predict": (_c_int, [_vp, _vp, _vp, _c_i64, _vp, _vp, _c_int]),
+    "dmo_mtgp_destroy": (_c_int, [_vp, _vp]),
     "dmo_nsga2_step": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_i64, _c_int, _c_int, _c_dbl, _c_dbl, _c_dbl, _vp, _vp, _vp, _vp, _c_u64, _c_u64,
                                 _c_int, _c_int, _c_int, _c_int, _vp, _vp, _vp]),
     "dmo_hypervolume": (_c_int, [_vp, _vp, _c_i64, _c_int, _vp, ctypes.POINTER(_c_dbl)]),
@@ -736,6 +740,54 @@ class GPHandle:
     def close(self):
         if getattr(self, "_h", None) is not None and _lib is not None and _ctx is not None:
             _lib.dmo_gp_destroy(_ctx, self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+# --------------------------------------------------------------------------- A19: multitask exact GP (MEGP_Matern)
+class MTGPHandle:
+    """Owns a dmo_mtgp object: the multitask posterior (covariance K_x (x) B + I (x) diag(D), linear mean per task)
+    resident in HBM.  ``lml`` is the exact log marginal likelihood of the normalised targets."""
+
+    def __init__(self, X_train, Y, length_scale, B, D, weight, bias, y_mean, y_std, xlb, xub):
+        lib = load_library()
+        X_train, Y = _f64(X_train), _f64(Y)
+        N, d = X_train.shape
+        if Y.ndim == 1:
+            Y = Y.reshape(-1, 1)
+        M = Y.shape[1]
+        assert Y.shape == (N, M), Y.shape
+        ls, Bm, Dv = _f64(np.broadcast_to(np.asarray(length_scale, dtype=np.float64).reshape(-1), (d,))), _f64(B).reshape(M, M), _f64(D).reshape(M)
+        w, b = _f64(weight).reshape(M, d), _f64(bias).reshape(M)
+        ym, ys, lb, ub = _f64(y_mean).reshape(M), _f64(y_std).reshape(M), _f64(xlb).reshape(d), _f64(xub).reshape(d)
+        self.N, self.d, self.M = N, d, M
+        h, lml = _vp(), _c_dbl(0.0)
+        _check(
+            lib.dmo_mtgp_create(context(), N, d, M, _ptr(X_train), _ptr(Y), _ptr(ls), _ptr(Bm), _ptr(Dv), _ptr(w), _ptr(b), _ptr(ym), _ptr(ys),
+                                _ptr(lb), _ptr(ub), ctypes.byref(lml), ctypes.byref(h)),
+            "dmo_mtgp_create",
+        )
+        self._h = h
+        self.lml = float(lml.value)
+
+    def predict(self, X, return_var=True, precision=GP_FP64):
+        X = _f64(X)
+        if X.ndim == 1:
+            X = X.reshape(1, -1)
+        P = X.shape[0]
+        mean = pinned_empty((P, self.M), np.float64)
+        var = pinned_empty((P, self.M), np.float64) if return_var else None
+        _check(load_library().dmo_mtgp_predict(context(), self._h, _in(X), P, _ptr(mean), _ptr(var), int(precision)), "dmo_mtgp_predict")
+        return mean, var
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and _lib is not None and _ctx is not None:
+            _lib.dmo_mtgp_destroy(_ctx, self._h)
             self._h = None
 
     def __del__(self):

@@ -340,6 +340,44 @@ __global__ void var_finish_kernel(const double* __restrict__ vnorm, int nplanes,
 
 }  // namespace
 
+int gp_linv_from_factor(dmo_ctx* ctx, const double* L, int64_t N, int64_t ldo, double* dst) {
+  int64_t Np = TRI_B;
+  while (Np < N) Np *= 2;
+  DevBuf<double> Lp, X, T;
+  DMO_TRY(Lp.alloc(ctx, (size_t)Np * Np));
+  DMO_TRY(X.alloc(ctx, (size_t)Np * Np));
+  DMO_TRY(T.alloc(ctx, (size_t)Np * Np / 2));
+  DMO_CUDA(cudaMemsetAsync(X.p, 0, (size_t)Np * Np * sizeof(double), ctx->stream));
+  DMO_LAUNCH(tri_embed_kernel, (unsigned)ceil_div(Np * Np, 256), 256, 0, L, N, Np, Lp.p);
+  DMO_LAUNCH(tri_diag_inverse_kernel, (unsigned)(Np / TRI_B), TRI_B, 0, Lp.p, Np, X.p);
+  for (int64_t sz = TRI_B; sz < Np; sz *= 2) {
+    const int64_t pairs = Np / (2 * sz);
+    const int64_t stride = 2 * sz * Np + 2 * sz;  // next diagonal 2s x 2s block
+    dim3 grid((unsigned)(sz / 64), (unsigned)(sz / 64), (unsigned)pairs);
+    // T = C * A^-1        (C = Lp[s:2s, 0:s], A^-1 = X[0:s, 0:s])
+    DMO_LAUNCH(gemm_nn_f64_kernel, grid, 256, 0, Lp.p + sz * Np, Np, stride, X.p, Np, stride, T.p, sz, sz * sz, sz, sz,
+               sz, 1.0);
+    // X[s:2s, 0:s] = -B^-1 * T   (B^-1 = X[s:2s, s:2s])
+    DMO_LAUNCH(gemm_nn_f64_kernel, grid, 256, 0, X.p + sz * Np + sz, Np, stride, T.p, sz, sz * sz, X.p + sz * Np, Np,
+               stride, sz, sz, sz, -1.0);
+  }
+  DMO_LAUNCH(tri_extract_kernel, (unsigned)ceil_div(N * N, 256), 256, 0, X.p, Np, N, ldo, dst);
+  DMO_CUDA(cudaGetLastError());
+  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  return DMO_OK;
+}
+
+static_assert(VB == GP_F64_TILE, "gp.cuh exports the float64 variance tile edge");
+
+int gp_var_contract_fp64(dmo_ctx* ctx, const dmo_gp* gp, const double* Ks, int64_t kplane, int64_t Pcpad, int nsplit,
+                         double* vnorm, int64_t vn_ld) {
+  dim3 gv((unsigned)(Pcpad / VB), (unsigned)gp->M, (unsigned)nsplit);
+  DMO_CUDA(cudaFuncSetAttribute(var_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)VAR_SMEM));
+  DMO_LAUNCH(var_kernel, gv, 256, VAR_SMEM, gp->Linv.p, gp->Npad, gp->Npad * gp->Npad, Ks, gp->Npad, kplane, gp->Npad, vnorm,
+             vn_ld);
+  return DMO_OK;
+}
+
 int gp_predict_fp64(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var) {
   const int64_t N = gp->N, Npad = gp->Npad;
   const int M = gp->M, d = gp->d;
@@ -659,29 +697,7 @@ int dmo_gp_create(dmo_ctx* ctx, int64_t N, int d, int M, int kernel, const doubl
                      gp->Zf.p + (size_t)m * Npad);
           gp->z_ready = true;
         }
-        int64_t Np = TRI_B;
-        while (Np < N) Np *= 2;
-        DevBuf<double> Lp, X, T;
-        GP_TRY(Lp.alloc(ctx, (size_t)Np * Np));
-        GP_TRY(X.alloc(ctx, (size_t)Np * Np));
-        GP_TRY(T.alloc(ctx, (size_t)Np * Np / 2));
-        GP_CUDA(cudaMemsetAsync(X.p, 0, (size_t)Np * Np * sizeof(double), ctx->stream));
-        DMO_LAUNCH(tri_embed_kernel, (unsigned)ceil_div(Np * Np, 256), 256, 0, src, N, Np, Lp.p);
-        DMO_LAUNCH(tri_diag_inverse_kernel, (unsigned)(Np / TRI_B), TRI_B, 0, Lp.p, Np, X.p);
-        for (int64_t sz = TRI_B; sz < Np; sz *= 2) {
-          const int64_t pairs = Np / (2 * sz);
-          const int64_t stride = 2 * sz * Np + 2 * sz;  // next diagonal 2s x 2s block
-          dim3 grid((unsigned)(sz / 64), (unsigned)(sz / 64), (unsigned)pairs);
-          // T = C * A^-1        (C = Lp[s:2s, 0:s], A^-1 = X[0:s, 0:s])
-          DMO_LAUNCH(gemm_nn_f64_kernel, grid, 256, 0, Lp.p + sz * Np, Np, stride, X.p, Np, stride, T.p, sz, sz * sz, sz, sz,
-                     sz, 1.0);
-          // X[s:2s, 0:s] = -B^-1 * T   (B^-1 = X[s:2s, s:2s])
-          DMO_LAUNCH(gemm_nn_f64_kernel, grid, 256, 0, X.p + sz * Np + sz, Np, stride, T.p, sz, sz * sz, X.p + sz * Np, Np,
-                     stride, sz, sz, sz, -1.0);
-        }
-        DMO_LAUNCH(tri_extract_kernel, (unsigned)ceil_div(N * N, 256), 256, 0, X.p, Np, N, Npad, dst);
-        GP_CUDA(cudaGetLastError());
-        GP_CUDA(cudaStreamSynchronize(ctx->stream));
+        GP_TRY(gp_linv_from_factor(ctx, src, N, Npad, dst));
       }
     }
     GP_CUDA(cudaGetLastError());

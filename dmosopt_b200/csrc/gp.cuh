@@ -44,5 +44,25 @@ struct dmo_gp {
 };
 
 int gp_predict_fp64(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var);
+
+// Building blocks shared with the multitask posterior (gp_multitask.cu).  All pointers are device pointers.
+// L^-1 of the lower Cholesky factor L (N, N) into dst (rows of ldo doubles, lower triangle; the rest is left untouched)
+int gp_linv_from_factor(dmo_ctx* ctx, const double* L, int64_t N, int64_t ldo, double* dst);
+// float64 variance contraction (var_kernel): vnorm[z][m][p] = partial sums over the row blocks z (mod nsplit) of
+// ||Linv_m Ks_m[p]||^2, Ks_m = Ks + m * kplane with rows of gp->Npad doubles (kplane = 0: one K_* plane for every m);
+// Pcpad is a multiple of GP_F64_TILE
+constexpr int GP_F64_TILE = 128;
+int gp_var_contract_fp64(dmo_ctx* ctx, const dmo_gp* gp, const double* Ks, int64_t kplane, int64_t Pcpad, int nsplit,
+                         double* vnorm, int64_t vn_ld);
+// the fp16 hi / lo split of L^-1 and its row scales (built once per model; gp->Kexp holds the K_* scaling exponents)
+int gp_prepare_tensor(dmo_ctx* ctx, dmo_gp* gp);
+// wgmma variance contraction (gp_var_wgmma_kernel, paired schedule) over K_* hi / lo rows of gp->Npad fp16 values:
+// k_alloc rows are allocated, objective m reads rows m * k_rows + [0, Pcpad) (k_rows = 0: one plane for every m);
+// Pcpad is a multiple of GP_TC_TILE.  vnorm[q][m][p], q < gp_tensor_var_planes(gp->Npad), holds the partial sums.
+// abort_flag (device int, zeroed by the caller) is set when the pipeline watchdog trips.
+constexpr int GP_TC_TILE = 128;
+int gp_tensor_var_planes(int64_t Npad);
+int gp_var_contract_tensor(dmo_ctx* ctx, dmo_gp* gp, const uint16_t* Kh, const uint16_t* Kl, int64_t k_alloc, int64_t k_rows,
+                           int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag);
 // mean_from_d: take the mean from the variance contraction (needs d_var and gp->z_ready), else from the K_* alpha pass
 int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var, bool mean_from_d = false);

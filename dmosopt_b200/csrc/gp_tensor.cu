@@ -1049,6 +1049,46 @@ int gp_mean_direct(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, doubl
 
 }  // namespace
 
+int gp_prepare_tensor(dmo_ctx* ctx, dmo_gp* gp) { return prepare_tensor_state(ctx, gp); }
+
+static_assert(TMV == GP_TC_TILE, "gp.cuh exports the wgmma candidate tile");
+
+int gp_tensor_var_planes(int64_t Npad) { return (int)((Npad / TN + 1) / 2); }
+
+int gp_var_contract_tensor(dmo_ctx* ctx, dmo_gp* gp, const uint16_t* Kh, const uint16_t* Kl, int64_t k_alloc, int64_t k_rows,
+                           int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag) {
+  const int64_t Npad = gp->Npad;
+  DMO_REQUIRE(Npad % TN == 0 && Pcpad % TMV == 0, "gp_var_contract_tensor: internal padding error");
+  CUtensorMap map_kh, map_kl, map_lh, map_ll;
+  DMO_TRY(make_map(ctx, &map_kh, Kh, (uint64_t)k_alloc, (uint64_t)Npad, TMV, TK, CU_TENSOR_MAP_SWIZZLE_64B));
+  DMO_TRY(make_map(ctx, &map_kl, Kl, (uint64_t)k_alloc, (uint64_t)Npad, TMV, TK, CU_TENSOR_MAP_SWIZZLE_64B));
+  DMO_TRY(make_map(ctx, &map_lh, gp->Lhi.p, (uint64_t)gp->M * Npad, (uint64_t)Npad, TN, TK, CU_TENSOR_MAP_SWIZZLE_64B));
+  DMO_TRY(make_map(ctx, &map_ll, gp->Llo.p, (uint64_t)gp->M * Npad, (uint64_t)Npad, TN, TK, CU_TENSOR_MAP_SWIZZLE_64B));
+  DMO_CUDA(cudaFuncSetAttribute(gp_var_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GEMM_SMEM));
+  GemmParams prm;
+  prm.M = gp->M;
+  prm.n_pb = (int)(Pcpad / TMV);
+  prm.n_jt = (int)(Npad / TN);
+  prm.n_q = gp_tensor_var_planes(Npad);
+  prm.paired = 1;
+  prm.j_split = prm.n_jt;
+  prm.k_rows = k_rows;
+  prm.l_rows = Npad;
+  prm.inv_scale = gp->Lscale.p;
+  prm.vnorm = vnorm;
+  prm.vn_ld = vn_ld;
+  prm.abort_flag = abort_flag;
+  prm.zf = nullptr;
+  prm.mnorm = nullptr;
+  prm.ready = nullptr;
+  prm.ready_target = 0;
+  prm.dbg = 0;
+  const int n_work = prm.M * prm.n_pb * prm.n_q;
+  const int grid = n_work < ctx->sm_count ? n_work : ctx->sm_count;
+  DMO_LAUNCH(gp_var_wgmma_kernel, grid, NTHREADS, GEMM_SMEM, map_kh, map_kl, map_lh, map_ll, prm);
+  return DMO_OK;
+}
+
 int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var, bool mean_from_d) {
   const int64_t N = gp->N, Npad = gp->Npad;
   const int M = gp->M, d = gp->d;

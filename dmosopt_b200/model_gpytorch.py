@@ -1,19 +1,23 @@
-"""gpytorch exact-GP surrogate on the GPU path: ``EGP_Matern`` (row A19).
+"""gpytorch exact-GP surrogates on the GPU path: ``EGP_Matern`` and ``MEGP_Matern`` (row A19).
 
-Drop-in for ``dmosopt.model_gpytorch.EGP_Matern`` (dmosopt/model_gpytorch.py:1927-2235), selected in dmosopt by
-``surrogate_method_name="dmosopt_b200.model_gpytorch.EGP_Matern"``.  As with the scikit-learn surrogates, *fitting*
-stays with the host library -- here the reference class itself, which needs gpytorch -- and only the posterior is
-taken over: after training, the hyper-parameters (ARD length scales, output scale, noise, linear-mean weights / bias)
-and the model's own normalised training tensors are read out, K + sigma^2 I is factorised once in float64, and every
-``predict`` / ``evaluate`` runs on the GPU through ``dmo_gp_create`` / ``dmo_gp_set_linear_mean`` / ``dmo_gp_predict``.
+Drop-ins for ``dmosopt.model_gpytorch.EGP_Matern`` (dmosopt/model_gpytorch.py:1927-2235) and
+``dmosopt.model_gpytorch.MEGP_Matern`` (:1623-1926), selected in dmosopt by
+``surrogate_method_name="dmosopt_b200.model_gpytorch.EGP_Matern"`` (or ``.MEGP_Matern``).  As with the scikit-learn
+surrogates, *fitting* stays with the host library -- here the reference class itself, which needs gpytorch -- and only
+the posterior is taken over: after training, the hyper-parameters and the model's own normalised training tensors are
+read out, the posterior is factorised once in float64, and every ``predict`` / ``evaluate`` runs on the GPU.
 
-The predictive variance is the exact one (gpytorch's ``fast_pred_var=False``); the reference's default
-``fast_pred_var=True`` (LOVE) is a low-rank approximation of it.  gpytorch is not part of this image, so the
-extraction from a trained gpytorch model is untested here; the posterior arithmetic is tested against oracle/egp.py
-through the ``hyperparameters=`` constructor path (tests/test_gpu_parity.py::test_egp_linear_mean_*).
+* ``EGP_Matern``: M independent GPs (ARD length scales, output scale, noise, linear-mean weights / bias per objective);
+  ``dmo_gp_create`` / ``dmo_gp_set_linear_mean`` / ``dmo_gp_predict``.
+* ``MEGP_Matern``: one multitask GP over all objectives, covariance K_x (x) B + I (x) D (shared ARD Matern-5/2 K_x,
+  rank-1 IndexKernel B, task + global noise D, linear mean per task); ``dmo_mtgp_create`` / ``dmo_mtgp_predict``.  The
+  (N*M) x (N*M) system splits exactly into M single-output blocks that share one K_* (csrc/gp_multitask.cu).
 
-``MEGP_Matern`` (multitask Kronecker model, model_gpytorch.py:1872-1919) couples the objectives in one (N*M) x (N*M)
-system and is not covered.
+The predictive variance is the exact one (gpytorch's ``fast_pred_var=False``); ``fast_pred_var=True`` (LOVE) is a
+low-rank approximation of it.  gpytorch is not part of this image, so training through the reference classes is
+untested here; the read-out of a trained model is tested on a stand-in with gpytorch's attribute names, and the
+posterior arithmetic against oracle/egp.py and oracle/megp.py through the ``hyperparameters=`` constructor path
+(tests/test_gpu_parity.py::test_egp_linear_mean_*, tests/test_gpu_megp.py).
 """
 
 import numpy as np
@@ -111,5 +115,148 @@ class EGP_Matern:
 
     def evaluate(self, x):
         """model_gpytorch.py:2230-2235."""
+        mean, var = self.predict(x)
+        return (mean, var) if self.return_mean_variance else mean
+
+
+# ----------------------------------------------------------------------------------------------------------- MEGP
+def filter_samples(y, x, nan="remove"):
+    """MOEA.filter_samples (dmosopt/MOEA.py:445-467) for the ``nan=`` modes: "remove" drops rows with a NaN objective,
+    "max" replaces NaNs by max(1e3 * column max, 1e5), a number replaces them by that number."""
+    y = np.array(y, dtype=np.float64)
+    x = np.asarray(x, dtype=np.float64)
+    if nan == "max":
+        m = np.max(np.nan_to_num(y), axis=0)
+        for c in range(y.shape[1]):
+            y[:, c] = np.nan_to_num(y[:, c], nan=max(1e3 * m[c], 1e5))
+        return y, x
+    if nan == "remove":
+        keep = ~np.any(np.isnan(y), axis=1)
+        return y[keep], x[keep]
+    return np.nan_to_num(y, nan=nan), x
+
+
+def normalise_targets(yin):
+    """model_gpytorch.py:1686-1703: float32 per-task mean and standard deviation (a zero deviation becomes 1), then
+    (y - mean) / (std + 1e-12)."""
+    yin = np.asarray(yin, dtype=np.float64)
+    ymean = np.asarray([np.mean(yin[:, i]) for i in range(yin.shape[1])], dtype=np.float32)
+    ystd = np.asarray([np.std(yin[:, i]) for i in range(yin.shape[1])], dtype=np.float32)
+    ystd[ystd == 0.0] = 1.0
+    yn = (yin - ymean.astype(np.float64)) / (ystd.astype(np.float64) + 1e-12)
+    return yn, ymean.astype(np.float64), ystd.astype(np.float64)
+
+
+def megp_hyperparameters(gp_model):
+    """Read a trained ``GPyTorchMultitaskExactGPModelMatern`` (dmosopt/model_gpytorch.py:510-571) out into
+    (xn (N,d), yn (N,M), hyperparameters): its own normalised training tensors and the ``hyperparameters=`` dict of
+    ``MEGP_Matern`` -- ARD length scales of the shared Matern kernel, the IndexKernel's covar_factor (M, rank) and var (M,),
+    the likelihood's task_noises (M,) and global noise, and the LinearMean weights (M,d) / biases (M,) of every task."""
+
+    def arr(t):
+        return t.detach().cpu().numpy().astype(np.float64)
+
+    cm = getattr(gp_model.covar_module, "module", gp_model.covar_module)  # MultiDeviceKernel wraps the MultitaskKernel
+    task = cm.task_covar_module
+    lik = gp_model.likelihood
+    M = int(task.covar_factor.shape[-2])
+    weights, biases = [], []
+    for m in gp_model.mean_module.base_means:
+        if hasattr(m, "weights"):
+            weights.append(arr(m.weights).reshape(-1))
+            biases.append(float(arr(m.bias).reshape(-1)[0]))
+        else:  # ConstantMean (linear_mean=False)
+            weights.append(None)
+            biases.append(float(arr(m.constant).reshape(-1)[0]))
+    xn = arr(gp_model.train_inputs[0])
+    N, d = xn.shape
+    hp = {
+        "lengthscale": arr(cm.data_covar_module.lengthscale).reshape(-1),
+        "covar_factor": arr(task.covar_factor).reshape(M, -1),
+        "var": arr(task.var).reshape(M),
+        "task_noises": arr(lik.task_noises).reshape(M) if getattr(lik, "has_task_noise", True) else np.zeros(M),
+        "noise": float(arr(lik.noise).reshape(-1)[0]) if getattr(lik, "has_global_noise", True) else 0.0,
+        "weights": np.stack([np.zeros(d) if w is None else w for w in weights]),
+        "biases": np.asarray(biases, dtype=np.float64),
+    }
+    return xn, arr(gp_model.train_targets).reshape(N, M), hp
+
+
+class MEGP_Matern:
+    """Multitask exact-GP surrogate; the reference constructor signature (model_gpytorch.py:1624-1647) plus
+    ``precision`` ("fp64", the default, or "tensor"; there is no "auto" calibration for this model) and
+    ``hyperparameters`` (dict with lengthscale (d,), covar_factor (M, rank), var (M,), task_noises (M,), noise, weights
+    (M,d), biases (M,)): when given, training is skipped.  ``log_marginal_likelihood_value`` is the exact log marginal
+    likelihood of the normalised targets under the model."""
+
+    def __init__(self, xin, yin, nInput, nOutput, xlb, xub, seed=None, gp_lengthscale_bounds=None, gp_likelihood_sigma=None,
+                 batch_size=None, preconditioner_size=100, adam_lr=0.01, fast_pred_var=False, n_iter=5000,
+                 min_loss_pct_change=0.1, return_mean_variance=False, use_cuda=False, nan="remove", top_k=None, logger=None,
+                 precision="fp64", hyperparameters=None, **kwargs):
+        codes = {"fp64": _lib.GP_FP64, "tensor": _lib.GP_TENSOR, _lib.GP_FP64: _lib.GP_FP64, _lib.GP_TENSOR: _lib.GP_TENSOR}
+        if precision not in codes:
+            raise ValueError(f"MEGP_Matern: precision must be 'fp64' or 'tensor' (got {precision!r})")
+        self.precision = codes[precision]
+        self.nInput, self.nOutput = nInput, nOutput
+        self.xlb = np.asarray(xlb, dtype=np.float64)
+        xub = np.asarray(xub, dtype=np.float64)
+        self.xrng = np.where(np.isclose(xub - self.xlb, 0.0, rtol=1e-6, atol=1e-6), 1.0, xub - self.xlb)  # model_gpytorch.py:1662-1664
+        self.return_mean_variance = return_mean_variance
+        self.logger = logger
+        if hyperparameters is None:
+            ref_kwargs = dict(seed=seed, gp_lengthscale_bounds=gp_lengthscale_bounds, gp_likelihood_sigma=gp_likelihood_sigma,
+                              batch_size=batch_size, preconditioner_size=preconditioner_size, adam_lr=adam_lr,
+                              fast_pred_var=fast_pred_var, n_iter=n_iter, min_loss_pct_change=min_loss_pct_change,
+                              use_cuda=use_cuda, nan=nan, top_k=top_k, **kwargs)
+            xn, yn, ymean, ystd, hyperparameters = self._fit_with_reference(xin, yin, nInput, nOutput, xlb, xub, logger, ref_kwargs)
+        else:
+            yin = np.asarray(yin, dtype=np.float64).reshape(len(yin), -1)
+            xin = np.asarray(xin, dtype=np.float64)
+            if nan is not None:  # model_gpytorch.py:1668-1671
+                yin, xin = filter_samples(yin, xin, nan=nan)
+            if isinstance(top_k, int) and xin.shape[0] > top_k:  # MOEA.top_k_MO
+                from .MOEA import sortMO
+
+                xs, ys, *_ = sortMO(xin, yin)
+                xin, yin = xs[:top_k], ys[:top_k]
+            xn = (xin - self.xlb) / self.xrng
+            yn, ymean, ystd = normalise_targets(yin)
+        self._upload(xn, yn, ymean, ystd, hyperparameters)
+
+    @staticmethod
+    def _fit_with_reference(xin, yin, nInput, nOutput, xlb, xub, logger, kwargs):
+        """Train with the reference class (unchanged) and read the fitted state out of its gpytorch model."""
+        try:
+            from dmosopt.model_gpytorch import MEGP_Matern as RefMEGP
+        except Exception as e:  # dmosopt or gpytorch missing
+            raise RuntimeError("dmosopt_b200.model_gpytorch.MEGP_Matern trains through dmosopt.model_gpytorch.MEGP_Matern, "
+                               "which requires dmosopt and the GPyTorch library; pass hyperparameters= to skip training") from e
+        ref = RefMEGP(xin, yin, nInput, nOutput, np.asarray(xlb), np.asarray(xub), logger=logger, **kwargs)
+        xn, yn, hp = megp_hyperparameters(ref.sm)
+        return xn, yn, np.asarray(ref.y_train_mean, dtype=np.float64), np.asarray(ref.y_train_std, dtype=np.float64), hp
+
+    def _upload(self, xn, yn, ymean, ystd, hp):
+        """Multitask posterior -> HBM, once per epoch."""
+        M, d = self.nOutput, self.nInput
+        F = np.asarray(hp["covar_factor"], dtype=np.float64).reshape(M, -1)
+        B = F @ F.T + np.diag(np.asarray(hp["var"], dtype=np.float64).reshape(M))  # IndexKernel covar_matrix
+        B = 0.5 * (B + B.T)
+        D = np.asarray(hp["task_noises"], dtype=np.float64).reshape(M) + float(np.ravel(hp["noise"])[0])
+        ls = np.broadcast_to(np.asarray(hp["lengthscale"], dtype=np.float64).reshape(-1), (d,))
+        self._gp = _lib.MTGPHandle(xn, np.asarray(yn, dtype=np.float64).reshape(-1, M), ls, B, D,
+                                   np.asarray(hp["weights"], dtype=np.float64).reshape(M, d), np.asarray(hp["biases"], dtype=np.float64).reshape(M),
+                                   ymean, ystd, self.xlb, self.xlb + self.xrng)
+        self.log_marginal_likelihood_value = self._gp.lml
+
+    def predict(self, xin):
+        """model_gpytorch.py:1872-1919: (mean (P, M), variance (P, M)) of likelihood(model(x)) as float32 arrays."""
+        xin = np.asarray(xin, dtype=np.float64)
+        if xin.ndim == 1:
+            xin = xin.reshape((1, self.nInput))
+        mean, var = self._gp.predict(xin, return_var=True, precision=self.precision)
+        return mean.astype(np.float32), var.astype(np.float32)
+
+    def evaluate(self, x):
+        """model_gpytorch.py:1921-1926."""
         mean, var = self.predict(x)
         return (mean, var) if self.return_mean_variance else mean

@@ -58,6 +58,7 @@ extern "C" {
 
 typedef struct dmo_ctx dmo_ctx;
 typedef struct dmo_gp dmo_gp;
+typedef struct dmo_mtgp dmo_mtgp;
 
 /* ---- context ----------------------------------------------------------- */
 int dmo_version(void);
@@ -224,6 +225,27 @@ int dmo_gp_predict(dmo_ctx* ctx, dmo_gp* gp, const double* X, int64_t P, double*
  * (= P when the whole call ran in float64).  Any output pointer may be NULL. */
 int dmo_gp_auto_info(dmo_ctx* ctx, dmo_gp* gp, int* mean_tensor, int* var_tensor, double* mean_err,
                      double* var_err, double* theta, int64_t* last_refined);
+
+/* ---- A19: multitask exact-GP posterior (MEGP_Matern predict) -------------------
+ * replaces model_gpytorch.MEGP_Matern.predict (dmosopt/model_gpytorch.py:1872-1919; model :510-571): one
+ * ExactGP over N points x M tasks, covariance K_x (x) B with K_x the ARD Matern-5/2 kernel (no output scale)
+ * and B = F F' + diag(v) (IndexKernel), noise I_N (x) D (MultitaskGaussianLikelihood, D_t = task noise t +
+ * global noise), prior mean w_t . x_n + b_t per task (MultitaskMean(LinearMean)).
+ * dmo_mtgp_create uploads the posterior state once per epoch:
+ *   X_train (N,d) normalised inputs; Y (N,M) normalised targets; length_scale (d,); B (M,M) symmetric positive
+ *   semi-definite; D (M,) > 0; weight (M,d), bias (M,); y_mean, y_std (M,); xlb / xub (d,) raw input bounds.
+ *   1 <= M <= 8, d <= 90.  The posterior splits exactly into M single-output GPs over the eigenvectors of
+ *   D^-1/2 B D^-1/2 (host Jacobi, deterministic), each factorised in float64 as dmo_gp_fit does.
+ *   lml_out (may be NULL) receives the exact log marginal likelihood log p(Y).
+ * dmo_mtgp_predict: X (P,d) raw inputs -> mean (P,M), var (P,M) (var may be NULL; it includes D):
+ *   precision DMO_GP_FP64 or DMO_GP_TENSOR (d <= 64); DMO_GP_AUTO is not offered (DMO_ERR_ARG). */
+int dmo_mtgp_create(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_train, const double* Y,
+                    const double* length_scale, const double* B, const double* D, const double* weight,
+                    const double* bias, const double* y_mean, const double* y_std, const double* xlb,
+                    const double* xub, double* lml_out, dmo_mtgp** out);
+int dmo_mtgp_predict(dmo_ctx* ctx, dmo_mtgp* mt, const double* X, int64_t P, double* mean, double* var,
+                     int precision);
+int dmo_mtgp_destroy(dmo_ctx* ctx, dmo_mtgp* mt);
 
 /* ---- A16: exact hypervolume ---------------------------------------------------
  * replaces hv.AdaptiveHyperVolume.compute_hypervolume(..., 'box') (dmosopt/hv.py:123-189)

@@ -74,6 +74,52 @@ def gp_sweep():
         print(f"gp {name} (DMO_GP_TC={os.environ.get('DMO_GP_TC', 'default')}): total {ms:.3f} ms [{parts}]{err}", flush=True)
 
 
+def mtgp_sweep():
+    """MEGP_Matern's multitask posterior (dmo_mtgp_predict, tensor and fp64) next to GPR_Matern's tensor predict at the
+    same shape (P = 65536, N = 4096, M = 3, d = 30), with the K_* bytes each writes per predict."""
+    import torch
+
+    L.context()
+    rng = np.random.default_rng(3)
+    N, d, M, P = 4096, 30, 3, 65536
+    Npad = -(-N // 256) * 256
+    Xtr = rng.random((N, d))
+    Ytr = np.column_stack([np.sin(3 * Xtr[:, :4].sum(axis=1) + k) + Xtr[:, 4 + k] ** 2 for k in range(M)])
+    yn = (Ytr - Ytr.mean(0)) / Ytr.std(0)
+    ls = np.full(d, 0.5)
+    # GPR_Matern: M independent GPs (fitted on the GPU for fixed hyper-parameters)
+    Lf, alpha, _ = L.gp_fit(Xtr, yn.T, [1.0] * M, [ls] * M, [1e-3] * M, jitter=0.0)
+    gpr = L.GPHandle(Xtr, alpha, Lf, [1.0] * M, [ls] * M, [1e-3] * M, Ytr.mean(0), Ytr.std(0), np.zeros(d), np.ones(d))
+    # MEGP_Matern: one multitask GP, rank-1 task covariance plus diagonal
+    F = np.array([[0.8], [0.5], [-0.4]])
+    B = F @ F.T + np.diag([0.3, 0.4, 0.5])
+    mt = L.MTGPHandle(Xtr, yn, ls, B, np.full(M, 2e-3), np.zeros((M, d)), np.zeros(M), Ytr.mean(0), Ytr.std(0), np.zeros(d), np.ones(d))
+    X = rng.random((P, d))
+    Xd = L.DeviceArray((P, d)).upload(X)
+    md, vd = L.DeviceArray((P, M)), L.DeviceArray((P, M))
+    lib, ctx = L.load_library(), L.context()
+    import subprocess
+
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
+    print(f"device: {torch.cuda.get_device_properties(0).name}; nvidia-smi: {q.stdout.strip() or q.stderr.strip()}", flush=True)
+    out = {}
+    runs = (("GPR_Matern tensor", lambda: lib.dmo_gp_predict(ctx, gpr._h, Xd.ptr, P, md.ptr, vd.ptr, L.GP_TENSOR), M * P * Npad * 4),
+            ("MEGP_Matern tensor", lambda: lib.dmo_mtgp_predict(ctx, mt._h, Xd.ptr, P, md.ptr, vd.ptr, L.GP_TENSOR), P * Npad * 4),
+            ("MEGP_Matern fp64", lambda: lib.dmo_mtgp_predict(ctx, mt._h, Xd.ptr, P, md.ptr, vd.ptr, L.GP_FP64), P * Npad * 8))
+    for name, fn, kbytes in runs:
+        L.profile_enable(True)
+        ms = timed(lambda: L._check(fn(), name), reps=3)
+        rep = L.profile_report()
+        L.profile_enable(False)
+        out[name] = (md.download(), vd.download())
+        parts = ", ".join(f"{k} {v[0] / v[1]:.3f}" for k, v in rep.items())
+        print(f"{name} P={P} N={N} M={M} d={d}: total {ms:.3f} ms [{parts}]; K_* written per predict {kbytes / 1e9:.3f} GB", flush=True)
+    (mt_t, vt_t), (mt_f, vt_f) = out["MEGP_Matern tensor"], out["MEGP_Matern fp64"]
+    prior = (np.diag(B) + 2e-3) * Ytr.std(0) ** 2
+    print(f"MEGP tensor vs fp64: mean err / max|mean| {np.max(np.abs(mt_t - mt_f) / np.abs(mt_f).max(0)):.2e}, "
+          f"var err / prior {np.max(np.abs(vt_t - vt_f) / prior):.2e}", flush=True)
+
+
 def stream_sweep():
     """The HBM-bound kernels at the BASELINE shape: crowding / euclidean distance (n = 131072, M = 3), SBX + mutation
     (pop 65536, d 30), mean kernel's neighbours, hypervolume of a 65536-point 3-D front.  Prints time and the achieved
@@ -115,5 +161,8 @@ if __name__ == "__main__":
         sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "gp":
         gp_sweep()
+        sys.exit(0)
+    if len(sys.argv) > 1 and sys.argv[1] == "mtgp":
+        mtgp_sweep()
         sys.exit(0)
     main()
