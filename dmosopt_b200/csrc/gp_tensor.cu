@@ -676,188 +676,200 @@ __global__ void __launch_bounds__(KM_T, 4)
   }
 }
 
-// K_* producer fused with the mean (predicts with variance): the layout of gp_mean_direct_kernel (a thread owns two
-// candidates) with 16-point tiles; besides accumulating k * (c alpha) the block stages the scaled hi / lo fp16 split of
-// its 256 x 16 tile per objective in shared memory (rows of 10 words: 8-byte stores of four consecutive training points
-// are conflict free) and writes it out as full 32-byte sectors.  Replaces kstar_tensor_kernel + mean_split_kernel
-// (1.46 + 0.72 ms at the BASELINE shape): K_* is written once and not read back for the mean.
-constexpr int KF_NS = 16, KF_LD = 10;
+// K_* producer fused with the mean (predicts with variance).  A warp owns 32 candidates and walks its training-set
+// slice in 64-point chunks, each lane holding two adjacent training points (coordinates in registers) while the
+// candidates arrive as 16-byte shared-memory broadcasts.  Every K_* store is then one full, contiguous 128-byte line per
+// warp (32 lanes x half2) straight from registers: no staging tile, no block barrier between arithmetic and stores.
+// The mean keeps the rounding structure of the sums it replaces: per candidate and objective an fp32 chain
+// acc = fma(k_n, c alpha_n, acc) over 16 consecutive training points (from the slice start, in order), folded into
+// float64 in ascending order over the slice; the slices are those of pick_slices(.., KF_NS, 3 x SMs, ..).  The chains
+// run after each batch of 8 candidates from the unscaled kernel values the batch left in shared memory (one lane per
+// (candidate, 16-point group)); after each chunk, lane l of a warp folds the chunk's group sums of the warp's candidate
+// l into float64.
+constexpr int KF_NS = 16;                         // training points per fp32 partial sum of the mean
+constexpr int KS_T = 128, KS_QW = 32, KS_Q = 4 * KS_QW;  // threads, candidates per warp, candidates per block
+constexpr int KS_C = 64;                          // training points per chunk: two per lane
+constexpr int KS_B = 8;                           // candidates per batch (the chains of a batch: 8 x 4 groups = 32 lanes)
+constexpr int KS_LD = KS_C + 4;                   // row stride of the batch's kernel values (conflict-free 16-byte reads)
+
+// per warp: [MT][KS_B][KS_LD] kernel values of a batch, [MT][KS_C] c * alpha of the chunk, [MT][KS_QW][4] fp32 group sums
+constexpr int ks_warp_floats(int MT) { return MT * (KS_B * KS_LD + KS_C + KS_QW * KS_C / KF_NS); }
+// dynamic shared memory of kstar_mean_kernel<*, MT>: candidate tile, the four warps' areas, then per warp [MT][32]
+// float64 sums of the mean
+constexpr size_t kstar_mean_smem(int MT) {
+  return (size_t)(KS_Q * KM_D + 4 * ks_warp_floats(MT)) * sizeof(float) + (size_t)4 * MT * KS_QW * sizeof(double);
+}
 
 template <bool ISO, int MT>
-__global__ void __launch_bounds__(KM_T, 3)
+__global__ void __launch_bounds__(KS_T, MT <= 3 ? 4 : 3)  // 4 blocks / SM up to M = 3 (registers and shared memory)
     kstar_mean_kernel(const double* __restrict__ Xn, int64_t P, int64_t p_base, const float* __restrict__ Xtf, int64_t N,
                       int64_t Npad, int64_t n_per_block, int d, int kind, const double* __restrict__ inv_ls,
                       const double* __restrict__ constant, const int* __restrict__ k_exp, const float* __restrict__ CAf,
                       int64_t plane, uint16_t* __restrict__ Kh, uint16_t* __restrict__ Kl, double* __restrict__ mpart,
                       int64_t mp_ld) {
-  extern __shared__ __align__(16) uint32_t kf_stage[];  // [MT][2][KM_Q][KF_LD] words: (objective, hi / lo, candidate row)
-  __shared__ __align__(16) float s_x[KF_NS * KM_D];
-  __shared__ float s_al[MT * KF_NS];  // c_m * alpha_m[n] of the tile (zero beyond N)
-  __shared__ float s_live[KF_NS];     // 1 for a training point, 0 for the padding columns (written as zeros)
+  extern __shared__ __align__(16) float ks_smem[];
   __shared__ __align__(16) float s_il[MT * KM_D];
-  __shared__ float s_c[MT];           // c_m * 2^kexp_m: scale of the stored K_*
-  const int t = threadIdx.x;
-  const int64_t q_base = (int64_t)blockIdx.y * KM_Q;
-  const int64_t qa = q_base + t, qb = qa + KM_T;
-  float2 ca[KM_D / 2], cb[KM_D / 2];
-  {
-    const int64_t pa = p_base + qa, pb = p_base + qb;
-#pragma unroll
-    for (int j = 0; j < KM_D / 2; ++j) {
-      const int j0 = 2 * j, j1 = 2 * j + 1;
-      ca[j] = make_float2((pa < P && j0 < d) ? (float)Xn[pa * d + j0] : 0.f, (pa < P && j1 < d) ? (float)Xn[pa * d + j1] : 0.f);
-      cb[j] = make_float2((pb < P && j0 < d) ? (float)Xn[pb * d + j0] : 0.f, (pb < P && j1 < d) ? (float)Xn[pb * d + j1] : 0.f);
-    }
+  __shared__ float s_c[MT];  // c_m * 2^kexp_m: scale of the stored K_*
+  const int t = threadIdx.x, lane = t & 31, w = t >> 5;
+  float* s_x = ks_smem;  // [KS_Q][KM_D] candidate coordinates (zero padded)
+  float* s_k = ks_smem + KS_Q * KM_D + w * ks_warp_floats(MT);  // this warp's [MT][KS_B][KS_LD] kernel values
+  float* s_al = s_k + MT * KS_B * KS_LD;                         // this warp's [MT][KS_C] c * alpha
+  float* s_part = s_al + MT * KS_C;                              // this warp's [MT][KS_QW][4] fp32 sums of the chunk's groups
+  double* s_sum = reinterpret_cast<double*>(ks_smem + KS_Q * KM_D + 4 * ks_warp_floats(MT)) + w * MT * KS_QW;
+  const int64_t q_base = (int64_t)blockIdx.y * KS_Q;
+  for (int i = t; i < KS_Q * KM_D; i += KS_T) {
+    const int64_t p = p_base + q_base + i / KM_D;
+    const int j = i % KM_D;
+    s_x[i] = (p < P && j < d) ? (float)Xn[p * d + j] : 0.f;
   }
-  for (int i = t; i < MT * KM_D; i += KM_T) {
+  for (int i = t; i < MT * KM_D; i += KS_T) {
     const int m = i / KM_D, j = i % KM_D;
     s_il[i] = j < d ? (float)inv_ls[m * d + j] : 0.f;
   }
   if (t < MT) s_c[t] = scalbnf((float)constant[t], k_exp[t]);
-  double sum_a[MT], sum_b[MT];
-#pragma unroll
-  for (int m = 0; m < MT; ++m) sum_a[m] = sum_b[m] = 0.0;
-  const int64_t n_begin = (int64_t)blockIdx.x * n_per_block;
-  const int64_t n_end = n_begin + n_per_block < Npad ? n_begin + n_per_block : Npad;
-  uint32_t* row_a = kf_stage + (size_t)t * KF_LD;             // + (m * 2 + arr) * KM_Q * KF_LD
-  uint32_t* row_b = kf_stage + (size_t)(t + KM_T) * KF_LD;
-  // the next tile's training coordinates (one float4 per thread: KF_NS * KM_D / 4 == KM_T) and c * alpha values travel
-  // through registers while the current tile is being worked on: no global-load latency between two barriers
-  static_assert(KF_NS * KM_D / 4 == KM_T && 6 * KF_NS <= KM_T, "tile prefetch mapping");
-  float4 px = reinterpret_cast<const float4*>(Xtf + n_begin * KM_D)[t];
-  float pal = t < MT * KF_NS ? CAf[(int64_t)(t / KF_NS) * Npad + n_begin + t % KF_NS] : 0.f;
-  __syncthreads();  // s_il, s_c
-  reinterpret_cast<float4*>(s_x)[t] = px;
-  if (t < MT * KF_NS) s_al[t] = pal;
-  if (t < KF_NS) s_live[t] = (n_begin + t < N) ? 1.f : 0.f;
   __syncthreads();
-  for (int64_t n0 = n_begin; n0 < n_end; n0 += KF_NS) {
-    const bool more = n0 + KF_NS < n_end;
-    if (more) {  // in flight during the tile's arithmetic
-      px = reinterpret_cast<const float4*>(Xtf + (n0 + KF_NS) * KM_D)[t];
-      if (t < MT * KF_NS) pal = CAf[(int64_t)(t / KF_NS) * Npad + n0 + KF_NS + t % KF_NS];
+  const int64_t lo = (int64_t)blockIdx.x * n_per_block;  // slice [lo, hi): multiples of KF_NS
+  const int64_t hi = lo + n_per_block < Npad ? lo + n_per_block : Npad;
+  const int64_t q_warp = q_base + w * KS_QW;
+  const int64_t hrow = Npad >> 1, hplane = plane >> 1;  // in 32-bit words (half2)
+  const int g = lane >> 3, u = lane & 7;  // chain of a lane: 16-point group g of the chunk, candidate u of the batch
+#pragma unroll
+  for (int m = 0; m < MT; ++m) s_sum[m * KS_QW + lane] = 0.0;
+  // chunks at multiples of KS_C (full 128-byte lines), clipped to the slice
+  for (int64_t c0 = lo / KS_C * KS_C; c0 < hi; c0 += KS_C) {
+    const int64_t n0 = c0 + 2 * lane;  // this lane's points n0, n0 + 1 (c0 + KS_C <= Npad)
+    const bool mine = n0 >= lo && n0 < hi;
+    // this lane's word of the warp's first candidate row in the hi / lo planes of objective 0
+    uint32_t* kh_c = reinterpret_cast<uint32_t*>(Kh) + ((q_warp * Npad + n0) >> 1);
+    uint32_t* kl_c = reinterpret_cast<uint32_t*>(Kl) + ((q_warp * Npad + n0) >> 1);
+    float2 xa[KM_D / 2], xb[KM_D / 2];
+    {
+      const float4* ra = reinterpret_cast<const float4*>(Xtf + n0 * KM_D);
+      const float4* rb = ra + KM_D / 4;
+#pragma unroll
+      for (int j = 0; j < KM_D / 4; ++j) {
+        const float4 va = ra[j], vb = rb[j];
+        xa[2 * j] = make_float2(va.x, va.y);
+        xa[2 * j + 1] = make_float2(va.z, va.w);
+        xb[2 * j] = make_float2(vb.x, vb.y);
+        xb[2 * j + 1] = make_float2(vb.z, vb.w);
+      }
     }
-    float2 acc[MT];
 #pragma unroll
-    for (int m = 0; m < MT; ++m) acc[m] = make_float2(0.f, 0.f);
+    for (int m = 0; m < MT; ++m)
+      *reinterpret_cast<float2*>(s_al + m * KS_C + 2 * lane) = *reinterpret_cast<const float2*>(CAf + (int64_t)m * Npad + n0);
+    // padding columns (n >= N) are stored as zeros
+    const float live_a = n0 < N ? 1.f : 0.f, live_b = n0 + 1 < N ? 1.f : 0.f;
+    // 16-point groups of this chunk inside the slice (the others belong to a neighbouring slice)
+    unsigned gmask = 0;
+#pragma unroll
+    for (int gg = 0; gg < KS_C / KF_NS; ++gg)
+      if (c0 + gg * KF_NS >= lo && c0 + gg * KF_NS < hi) gmask |= 1u << gg;
+    for (int b = 0; b < KS_QW / KS_B; ++b) {
+      __syncwarp();  // s_al written; the previous batch's chains have read s_k
 #pragma unroll 1
-    for (int i4 = 0; i4 < KF_NS; i4 += 4) {
-      uint32_t wh_a[MT][2], wl_a[MT][2], wh_b[MT][2], wl_b[MT][2];  // four training points -> two half2 words each
+      for (int v = 0; v < KS_B; ++v) {
+        const int qw = b * KS_B + v;  // candidate of the warp
+        const float4* xc = reinterpret_cast<const float4*>(s_x + (w * KS_QW + qw) * KM_D);
+        uint32_t* ph = kh_c + qw * hrow;
+        uint32_t* pl = kl_c + qw * hrow;
+        float ra = 0.f, rb = 0.f;  // squared distances of the isotropic kernel
+        if (ISO) {
+          float2 a0 = make_float2(0.f, 0.f), a1 = a0, b0 = a0, b1 = a0;  // independent chains
 #pragma unroll
-      for (int u2 = 0; u2 < 2; ++u2) {
-        float2 kv[2][MT];  // scaled kernel values of the pair of points (candidates a, b)
-#pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          const int i = i4 + 2 * u2 + u;
-          const float4* xr = reinterpret_cast<const float4*>(s_x + i * KM_D);
-          float2 r2 = make_float2(0.f, 0.f);
+          for (int j = 0; j < KM_D / 4; ++j) {
+            const float4 c = xc[j];
+            const float2 nc01 = make_float2(-c.x, -c.y), nc23 = make_float2(-c.z, -c.w);
+            const float2 da0 = fadd2(xa[2 * j], nc01);
+            const float2 db0 = fadd2(xb[2 * j], nc01);
+            const float2 da1 = fadd2(xa[2 * j + 1], nc23);
+            const float2 db1 = fadd2(xb[2 * j + 1], nc23);
+            a0 = ffma2(da0, da0, a0);
+            b0 = ffma2(db0, db0, b0);
+            a1 = ffma2(da1, da1, a1);
+            b1 = ffma2(db1, db1, b1);
+          }
+          ra = (a0.x + a0.y) + (a1.x + a1.y);
+          rb = (b0.x + b0.y) + (b1.x + b1.y);
+        }
+        // one objective: kernel values of the two points, K_* hi / lo stores, unscaled values for the chains
+        auto produce = [&](int m) {
+          float2 rr;
           if (ISO) {
-            float2 a0 = make_float2(0.f, 0.f), a1 = a0, b0 = a0, b1 = a0;
+            const float il = s_il[m * KM_D];
+            const float il2 = il * il;
+            rr = fmul2(make_float2(ra, rb), make_float2(il2, il2));
+          } else {
+            const float4* il4 = reinterpret_cast<const float4*>(s_il + m * KM_D);
+            float2 aa = make_float2(0.f, 0.f), bb = aa;
 #pragma unroll
             for (int j = 0; j < KM_D / 4; ++j) {
-              const float4 c = xr[j];
-              const float2 c01 = make_float2(c.x, c.y), c23 = make_float2(c.z, c.w);
-              const float2 da0 = fadd2(c01, make_float2(-ca[2 * j].x, -ca[2 * j].y));
-              const float2 db0 = fadd2(c01, make_float2(-cb[2 * j].x, -cb[2 * j].y));
-              const float2 da1 = fadd2(c23, make_float2(-ca[2 * j + 1].x, -ca[2 * j + 1].y));
-              const float2 db1 = fadd2(c23, make_float2(-cb[2 * j + 1].x, -cb[2 * j + 1].y));
-              a0 = ffma2(da0, da0, a0);
-              b0 = ffma2(db0, db0, b0);
-              a1 = ffma2(da1, da1, a1);
-              b1 = ffma2(db1, db1, b1);
+              const float4 c = xc[j], il = il4[j];
+              const float2 nc01 = make_float2(-c.x, -c.y), nc23 = make_float2(-c.z, -c.w);
+              const float2 i01 = make_float2(il.x, il.y), i23 = make_float2(il.z, il.w);
+              const float2 da0 = fmul2(fadd2(xa[2 * j], nc01), i01);
+              const float2 db0 = fmul2(fadd2(xb[2 * j], nc01), i01);
+              const float2 da1 = fmul2(fadd2(xa[2 * j + 1], nc23), i23);
+              const float2 db1 = fmul2(fadd2(xb[2 * j + 1], nc23), i23);
+              aa = ffma2(da0, da0, aa);
+              bb = ffma2(db0, db0, bb);
+              aa = ffma2(da1, da1, aa);
+              bb = ffma2(db1, db1, bb);
             }
-            r2 = make_float2((a0.x + a0.y) + (a1.x + a1.y), (b0.x + b0.y) + (b1.x + b1.y));
+            rr = make_float2(aa.x + aa.y, bb.x + bb.y);
           }
-          const float live = s_live[i];
-#pragma unroll
-          for (int m = 0; m < MT; ++m) {
-            float2 rr;
-            if (ISO) {
-              const float il = s_il[m * KM_D];
-              const float il2 = il * il;
-              rr = fmul2(r2, make_float2(il2, il2));
-            } else {
-              const float4* il4 = reinterpret_cast<const float4*>(s_il + m * KM_D);
-              float2 aa = make_float2(0.f, 0.f), bb = aa;
-#pragma unroll
-              for (int j = 0; j < KM_D / 4; ++j) {
-                const float4 c = xr[j], il = il4[j];
-                const float2 c01 = make_float2(c.x, c.y), c23 = make_float2(c.z, c.w);
-                const float2 i01 = make_float2(il.x, il.y), i23 = make_float2(il.z, il.w);
-                const float2 da0 = fmul2(fadd2(c01, make_float2(-ca[2 * j].x, -ca[2 * j].y)), i01);
-                const float2 db0 = fmul2(fadd2(c01, make_float2(-cb[2 * j].x, -cb[2 * j].y)), i01);
-                const float2 da1 = fmul2(fadd2(c23, make_float2(-ca[2 * j + 1].x, -ca[2 * j + 1].y)), i23);
-                const float2 db1 = fmul2(fadd2(c23, make_float2(-cb[2 * j + 1].x, -cb[2 * j + 1].y)), i23);
-                aa = ffma2(da0, da0, aa);
-                bb = ffma2(db0, db0, bb);
-                aa = ffma2(da1, da1, aa);
-                bb = ffma2(db1, db1, bb);
-              }
-              rr = make_float2(aa.x + aa.y, bb.x + bb.y);
-            }
-            const float2 k0 = stationary2_f(rr, kind);
-            const float al = s_al[m * KF_NS + i];
-            acc[m] = ffma2(k0, make_float2(al, al), acc[m]);
-            const float sc = s_c[m] * live;
-            kv[u][m] = fmul2(k0, make_float2(sc, sc));  // c * k(r), scaled by 2^kexp (exact); padding columns: 0
+          const float2 k0 = stationary2_f(rr, kind);  // (point a, point b)
+          *reinterpret_cast<float2*>(s_k + (m * KS_B + v) * KS_LD + 2 * lane) = k0;
+          const float2 kv = fmul2(k0, make_float2(s_c[m] * live_a, s_c[m] * live_b));  // c * k(r) * 2^kexp (exact)
+          const __half2 h = __floats2half2_rn(kv.x, kv.y);
+          const float2 hf = __half22float2(h);
+          const __half2 l = __floats2half2_rn(kv.x - hf.x, kv.y - hf.y);
+          if (mine) {
+            ph[m * hplane] = *reinterpret_cast<const uint32_t*>(&h);
+            pl[m * hplane] = *reinterpret_cast<const uint32_t*>(&l);
           }
-        }
+        };
+        if (ISO) {
 #pragma unroll
-        for (int m = 0; m < MT; ++m) {  // pack (n, n + 1) of one candidate into half2: hi, then lo = value - hi
-          const __half2 ha = __floats2half2_rn(kv[0][m].x, kv[1][m].x), hb = __floats2half2_rn(kv[0][m].y, kv[1][m].y);
-          const float2 fa = __half22float2(ha), fb = __half22float2(hb);
-          const __half2 la = __floats2half2_rn(kv[0][m].x - fa.x, kv[1][m].x - fa.y);
-          const __half2 lb = __floats2half2_rn(kv[0][m].y - fb.x, kv[1][m].y - fb.y);
-          wh_a[m][u2] = *reinterpret_cast<const uint32_t*>(&ha);
-          wl_a[m][u2] = *reinterpret_cast<const uint32_t*>(&la);
-          wh_b[m][u2] = *reinterpret_cast<const uint32_t*>(&hb);
-          wl_b[m][u2] = *reinterpret_cast<const uint32_t*>(&lb);
+          for (int m = 0; m < MT; ++m) produce(m);
+        } else {  // a distance pass per objective: kept rolled, so its 1/l values are not held in registers across candidates
+#pragma unroll 1
+          for (int m = 0; m < MT; ++m) produce(m);
         }
       }
+      __syncwarp();  // the batch's kernel values are in s_k
 #pragma unroll
       for (int m = 0; m < MT; ++m) {
-        const size_t oh = (size_t)(m * 2) * KM_Q * KF_LD + (i4 >> 1), ol = oh + (size_t)KM_Q * KF_LD;
-        *reinterpret_cast<uint2*>(row_a + oh) = make_uint2(wh_a[m][0], wh_a[m][1]);
-        *reinterpret_cast<uint2*>(row_a + ol) = make_uint2(wl_a[m][0], wl_a[m][1]);
-        *reinterpret_cast<uint2*>(row_b + oh) = make_uint2(wh_b[m][0], wh_b[m][1]);
-        *reinterpret_cast<uint2*>(row_b + ol) = make_uint2(wl_b[m][0], wl_b[m][1]);
+        const float4* kr = reinterpret_cast<const float4*>(s_k + (m * KS_B + u) * KS_LD + g * KF_NS);
+        const float4* ar = reinterpret_cast<const float4*>(s_al + m * KS_C + g * KF_NS);
+        float acc = 0.f;
+#pragma unroll
+        for (int r = 0; r < KF_NS / 4; ++r) {
+          const float4 k4 = kr[r], a4 = ar[r];
+          acc = __fmaf_rn(k4.x, a4.x, acc);
+          acc = __fmaf_rn(k4.y, a4.y, acc);
+          acc = __fmaf_rn(k4.z, a4.z, acc);
+          acc = __fmaf_rn(k4.w, a4.w, acc);
+        }
+        s_part[(m * KS_QW + b * KS_B + u) * 4 + g] = acc;
       }
     }
+    __syncwarp();  // the chunk's group sums are in s_part
+    // lane l folds the groups of the warp's candidate l into float64, in ascending order
 #pragma unroll
     for (int m = 0; m < MT; ++m) {
-      sum_a[m] += (double)acc[m].x;
-      sum_b[m] += (double)acc[m].y;
+      const float4 part = *reinterpret_cast<const float4*>(s_part + (m * KS_QW + lane) * 4);
+      double sum = s_sum[m * KS_QW + lane];
+      if (gmask & 1u) sum += (double)part.x;
+      if (gmask & 2u) sum += (double)part.y;
+      if (gmask & 4u) sum += (double)part.z;
+      if (gmask & 8u) sum += (double)part.w;
+      s_sum[m * KS_QW + lane] = sum;
     }
-    __syncthreads();  // the tile is staged, its inputs have been consumed
-    // flush: 8-byte units, four per 32-byte row segment (a warp writes eight full sectors per instruction); thread t
-    // always moves unit t & 3 of rows (t >> 2) + 32 k, so every offset below is a compile-time constant or one add
-    {
-      const uint32_t* src = kf_stage + (size_t)(t >> 2) * KF_LD + 2 * (t & 3);
-      const int64_t row0 = (q_base + (t >> 2)) * Npad + n0 + 4 * (t & 3);
-      const int64_t kstep = (int64_t)32 * Npad;
-#pragma unroll
-      for (int ma = 0; ma < 2 * MT; ++ma) {
-        uint16_t* dst = ((ma & 1) ? Kl : Kh) + (int64_t)(ma >> 1) * plane + row0;
-#pragma unroll
-        for (int k = 0; k < KM_Q / 32; ++k) {
-          const uint2 v = *reinterpret_cast<const uint2*>(src + (size_t)(ma * KM_Q + k * 32) * KF_LD);
-          *reinterpret_cast<uint2*>(dst) = v;
-          dst += kstep;
-        }
-      }
-    }
-    if (more) {  // the next tile's inputs, from the registers filled above
-      reinterpret_cast<float4*>(s_x)[t] = px;
-      if (t < MT * KF_NS) s_al[t] = pal;
-      if (t < KF_NS) s_live[t] = (n0 + KF_NS + t < N) ? 1.f : 0.f;
-    }
-    __syncthreads();  // stage drained, next inputs in place
+    __syncwarp();  // s_al, s_k and s_part are rewritten by the next chunk
   }
 #pragma unroll
-  for (int m = 0; m < MT; ++m) {
-    mpart[((int64_t)blockIdx.x * MT + m) * mp_ld + qa] = sum_a[m];
-    mpart[((int64_t)blockIdx.x * MT + m) * mp_ld + qb] = sum_b[m];
-  }
+  for (int m = 0; m < MT; ++m) mpart[((int64_t)blockIdx.x * MT + m) * mp_ld + q_warp + lane] = s_sum[m * KS_QW + lane];
 }
 
 // mean[p][m] = y_std * sum_n K_*[p][n] alpha[n] + y_mean from the split K_* (hi + lo = 22 bits): HBM-bound pass,
@@ -1141,7 +1153,7 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
   DMO_CUDA(cudaFuncSetAttribute(gp_var_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GEMM_SMEM));
   const int64_t kplane = Pc_alloc * Npad;
   // K_* producer fused with the mean (d <= 32, M <= 6; DMO_GP_FUSED=0 keeps kstar_tensor_kernel + mean_split_kernel)
-  // (per-dimension length scales with more than two objectives spill in the fused kernel: they keep the two-kernel route)
+  // (per-dimension length scales with more than two objectives keep the two-kernel route: a distance pass per objective)
   const bool fused = !overlap && !mean_from_d && !(dbg & 8) && d <= KM_D && M <= 6 && (gp->isotropic || M <= 2) &&
                      !(getenv("DMO_GP_FUSED") && atoi(getenv("DMO_GP_FUSED")) == 0);
   DevBuf<double> mpart;
@@ -1168,14 +1180,14 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
       const int64_t n_qb = Pcpad / KM_Q;
       const int64_t nsplit = pick_slices(n_qb, Npad, KF_NS, (int64_t)3 * ctx->sm_count, &n_per_block);
       DMO_TRY(mpart.alloc(ctx, (size_t)nsplit * M * Pcpad));
-      dim3 gf((unsigned)nsplit, (unsigned)n_qb);
-      const size_t smem = (size_t)M * 2 * KM_Q * KF_LD * sizeof(uint32_t);
+      dim3 gf((unsigned)nsplit, (unsigned)(Pcpad / KS_Q));
+      const size_t smem = kstar_mean_smem(M);
       {
         ProfileScope ps_(ctx, "gp_kstar");
 #define KF_LAUNCH(ISO_, MT_)                                                                                               \
   do {                                                                                                                     \
     DMO_CUDA(cudaFuncSetAttribute(kstar_mean_kernel<ISO_, MT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));  \
-    DMO_LAUNCH((kstar_mean_kernel<ISO_, MT_>), gf, KM_T, smem, dXn, P, p_base, gp->Xtf.p, N, Npad, n_per_block, d,          \
+    DMO_LAUNCH((kstar_mean_kernel<ISO_, MT_>), gf, KS_T, smem, dXn, P, p_base, gp->Xtf.p, N, Npad, n_per_block, d,          \
                gp->kernel, gp->inv_ls.p, gp->constant.p, gp->Kexp.p, gp->CAf.p, kplane, Kh.p, Kl.p, mpart.p, Pcpad);         \
   } while (0)
 #define KF_SWITCH(ISO_)                  \

@@ -72,6 +72,67 @@ def gp_sweep():
             err = f" | vs fp64: var err/prior {np.max(np.abs(var - ref[1]) / prior):.2e}, mean err {np.max(np.abs(mean - ref[0])):.2e}"
         parts = ", ".join(f"{k} {v[0] / v[1]:.3f}" for k, v in rep.items())
         print(f"gp {name} (DMO_GP_TC={os.environ.get('DMO_GP_TC', 'default')}): total {ms:.3f} ms [{parts}]{err}", flush=True)
+    kstar_sweep(lib, ctx, h, Xd, md, vd, P, N, M)
+
+
+def device_line():
+    import subprocess
+
+    import torch
+
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
+    return f"device: {torch.cuda.get_device_properties(0).name}; nvidia-smi: {q.stdout.strip() or q.stderr.strip()}"
+
+
+def write_floor_ms(nbytes, reps=5):
+    """A write-only floor for `nbytes`: one plain store kernel (torch's fill over a contiguous byte buffer), CUDA events."""
+    import torch
+
+    buf = torch.empty(nbytes, dtype=torch.uint8, device="cuda")
+    buf.fill_(1)
+    torch.cuda.synchronize()
+    best = 1e9
+    for _ in range(reps):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        buf.fill_(0)
+        e1.record()
+        e1.synchronize()
+        best = min(best, e0.elapsed_time(e1))
+    del buf
+    torch.cuda.empty_cache()
+    return best
+
+
+def kstar_sweep(lib, ctx, h, Xd, md, vd, P, N, M):
+    """K_* producer of the tensor predict, both routes (DMO_GP_FUSED=1: K_* and the mean from one kernel; 0: K_* kernel
+    then the mean read back from K_*): time, bytes of K_* written (fp16 hi + lo, M planes of Pcpad x Npad) and the
+    achieved rate, next to a write-only floor over the same bytes measured in the same process."""
+    Npad = -(-N // 256) * 256
+    Pcpad = -(-P // 256) * 256
+    kbytes = 2 * 2 * M * Pcpad * Npad
+    print(device_line(), flush=True)
+    floor = write_floor_ms(kbytes)
+    print(f"write-only floor (one store kernel over {kbytes / 1e9:.3f} GB): {floor:.3f} ms = {kbytes / floor / 1e6:.0f} GB/s", flush=True)
+    saved = os.environ.get("DMO_GP_FUSED")
+    outs = {}
+    for fused in ("1", "0"):
+        os.environ["DMO_GP_FUSED"] = fused
+        L.profile_enable(True)
+        ms = timed(lambda: L._check(lib.dmo_gp_predict(ctx, h._h, Xd.ptr, P, md.ptr, vd.ptr, L.GP_TENSOR), "gp"), reps=3)
+        rep = L.profile_report()
+        L.profile_enable(False)
+        outs[fused] = (md.download(), vd.download())
+        ks = rep["gp_kstar"][0] / rep["gp_kstar"][1]
+        mean = f", gp_mean {rep['gp_mean'][0] / rep['gp_mean'][1]:.3f} ms" if "gp_mean" in rep else ""
+        print(f"tensor predict DMO_GP_FUSED={fused}: total {ms:.3f} ms; gp_kstar {ks:.3f} ms{mean}; K_* written {kbytes / 1e9:.3f} GB "
+              f"-> {kbytes / ks / 1e6:.0f} GB/s ({floor / ks:.2f} of the write-only floor's rate)", flush=True)
+    if saved is None:
+        del os.environ["DMO_GP_FUSED"]
+    else:
+        os.environ["DMO_GP_FUSED"] = saved
+    (m1, v1), (m0, v0) = outs["1"], outs["0"]
+    print(f"routes agree: var bit-identical {np.array_equal(v1, v0)}, max |mean difference| {np.max(np.abs(m1 - m0)):.2e}", flush=True)
 
 
 def mtgp_sweep():
