@@ -75,6 +75,7 @@ _SIGNATURES = {
                                  ctypes.POINTER(_vp)]),
     "dmo_mtgp_predict": (_c_int, [_vp, _vp, _vp, _c_i64, _vp, _vp, _c_int]),
     "dmo_mtgp_destroy": (_c_int, [_vp, _vp]),
+    "dmo_mtgp_lml_grad": (_c_int, [_vp, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dmo_nsga2_step": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_i64, _c_int, _c_int, _c_dbl, _c_dbl, _c_dbl, _vp, _vp, _vp, _vp, _c_u64, _c_u64,
                                 _c_int, _c_int, _c_int, _c_int, _vp, _vp, _vp]),
     "dmo_hypervolume": (_c_int, [_vp, _vp, _c_i64, _c_int, _vp, ctypes.POINTER(_c_dbl)]),
@@ -678,6 +679,26 @@ def gp_fit(X_train, y, constant, length_scale, noise, kernel=KERNEL_MATERN52, ji
     _check(load_library().dmo_gp_fit(context(), N, d, M, int(kernel), _ptr(X_train), _ptr(y), _ptr(cst), _ptr(ls), _ptr(nz), float(jitter), _ptr(L), _ptr(alpha),
                                      _ptr(lml)), "dmo_gp_fit")
     return L, alpha, lml
+
+
+def mtgp_lml_grad(X_train, Y, length_scale, B, D, weight, bias):
+    """(lml, grads) of the multitask exact GP (covariance K_x (x) B + I (x) diag(D), linear mean per task) for the given
+    hyper-parameters (dmo_mtgp_lml_grad): lml = log p(Y), grads a dict of d lml / d {length_scale (d,), B (M,M) with
+    independent entries, D (M,), weight (M,d), bias (M,)}.  X_train (N,d) normalised inputs, Y (N,M) normalised targets."""
+    X_train, Y = _f64(X_train), _f64(Y)
+    N, d = X_train.shape
+    if Y.ndim == 1:
+        Y = Y.reshape(-1, 1)
+    M = Y.shape[1]
+    assert Y.shape == (N, M), Y.shape
+    ls = _f64(np.broadcast_to(np.asarray(length_scale, dtype=np.float64).reshape(-1), (d,)))
+    Bm, Dv, w, b = _f64(B).reshape(M, M), _f64(D).reshape(M), _f64(weight).reshape(M, d), _f64(bias).reshape(M)
+    lml = np.empty(1)
+    g = {"length_scale": np.empty(d), "B": np.empty((M, M)), "D": np.empty(M), "weight": np.empty((M, d)), "bias": np.empty(M)}
+    _check(load_library().dmo_mtgp_lml_grad(context(), N, d, M, _ptr(X_train), _ptr(Y), _ptr(ls), _ptr(Bm), _ptr(Dv), _ptr(w), _ptr(b),
+                                            _ptr(lml), _ptr(g["length_scale"]), _ptr(g["B"]), _ptr(g["D"]), _ptr(g["weight"]),
+                                            _ptr(g["bias"])), "dmo_mtgp_lml_grad")
+    return float(lml[0]), g
 
 
 # --------------------------------------------------------------------------- A18

@@ -66,3 +66,20 @@ int gp_var_contract_tensor(dmo_ctx* ctx, dmo_gp* gp, const uint16_t* Kh, const u
                            int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag);
 // mean_from_d: take the mean from the variance contraction (needs d_var and gp->z_ready), else from the K_* alpha pass
 int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var, bool mean_from_d = false);
+
+// ---- multitask model (gp_multitask.cu): the block factorisation shared by dmo_mtgp_create and dmo_mtgp_lml_grad --
+constexpr int MT_MAX = 8;        // tasks per model
+constexpr int MT_FIT_DMAX = 90;  // input dimensions dmo_gp_fit takes
+struct MtBlocks {
+  std::vector<double> hx, ls, hB, hD, hw, hb;  // the inputs, copied to the host
+  std::vector<double> sqD, lam, Q;             // sqrt(D_s); D^-1/2 B D^-1/2 = Q diag(lam) Q' (Q row-major, Q[s * M + j])
+  std::vector<double> xs;                      // (N, d) x_n / l
+  std::vector<double> blk_lml;                 // (M,) per-block log marginal likelihoods
+  double lml = 0.0;                            // log p(Y)
+  DevBuf<double> Lf;                           // (M, N, N) lower Cholesky factors of lambda_j K_x + I
+};
+// Argument checks (messages prefixed by `who`), Jacobi, rotated residuals and dmo_gp_fit on the M blocks; alpha_out
+// ((M, N), host or device) receives the block alphas a_j.  Returns after dmo_gp_fit's synchronisation.
+int mtgp_blocks_fit(dmo_ctx* ctx, const char* who, int64_t N, int d, int M, const double* X_train, const double* Y,
+                    const double* length_scale, const double* B, const double* D, const double* weight, const double* bias,
+                    MtBlocks& mb, double* alpha_out);

@@ -24,9 +24,6 @@
 
 #include "gp.cuh"
 
-constexpr int MT_MAX = 8;     // tasks per model
-constexpr int MT_FIT_DMAX = 90;  // input dimensions dmo_gp_fit takes
-
 struct dmo_mtgp {
   int64_t N = 0, Npad = 0;
   int d = 0, M = 0;
@@ -301,21 +298,26 @@ int upload(dmo_ctx* ctx, DevBuf<T>& dst, const std::vector<T>& src) {
 
 }  // namespace
 
-extern "C" {
-
-int dmo_mtgp_create(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_train, const double* Y, const double* length_scale,
-                    const double* B, const double* D, const double* weight, const double* bias, const double* y_mean,
-                    const double* y_std, const double* xlb, const double* xub, double* lml_out, dmo_mtgp** out) {
-  if (!ctx) return DMO_ERR_ARG;
-  DMO_CUDA(cudaSetDevice(ctx->device));
-  DMO_REQUIRE(out, "mtgp_create: null output");
-  *out = nullptr;
+int mtgp_blocks_fit(dmo_ctx* ctx, const char* who, int64_t N, int d, int M, const double* X_train, const double* Y,
+                    const double* length_scale, const double* B, const double* D, const double* weight, const double* bias,
+                    MtBlocks& mb, double* alpha_out) {
   DMO_REQUIRE(N >= 1 && d >= 1 && d <= MT_FIT_DMAX && M >= 1 && M <= MT_MAX,
-              "mtgp_create: unsupported shape N=%lld d=%d M=%d (1 <= M <= %d, d <= %d)", (long long)N, d, M, MT_MAX, MT_FIT_DMAX);
-  DMO_REQUIRE(X_train && Y && length_scale && B && D && weight && bias && y_mean && y_std && xlb && xub,
-              "mtgp_create: null pointer");
+              "%s: unsupported shape N=%lld d=%d M=%d (1 <= M <= %d, d <= %d)", who, (long long)N, d, M, MT_MAX, MT_FIT_DMAX);
+  DMO_REQUIRE(X_train && Y && length_scale && B && D && weight && bias, "%s: null pointer", who);
   const size_t nd = (size_t)N * d, nm = (size_t)N * M, mm = (size_t)M * M;
-  std::vector<double> hx(nd), hy(nm), ls(d), hB(mm), hD(M), hw((size_t)M * d), hb(M), ym(M), ys(M), lb(d), ub(d);
+  std::vector<double>& hx = mb.hx;
+  std::vector<double>& ls = mb.ls;
+  std::vector<double>& hB = mb.hB;
+  std::vector<double>& hD = mb.hD;
+  std::vector<double>& hw = mb.hw;
+  std::vector<double>& hb = mb.hb;
+  std::vector<double> hy(nm);
+  hx.resize(nd);
+  ls.resize(d);
+  hB.resize(mm);
+  hD.resize(M);
+  hw.resize((size_t)M * d);
+  hb.resize(M);
   DMO_CUDA(cudaMemcpy(hx.data(), X_train, nd * sizeof(double), cudaMemcpyDefault));
   DMO_CUDA(cudaMemcpy(hy.data(), Y, nm * sizeof(double), cudaMemcpyDefault));
   DMO_CUDA(cudaMemcpy(ls.data(), length_scale, d * sizeof(double), cudaMemcpyDefault));
@@ -323,21 +325,20 @@ int dmo_mtgp_create(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_train
   DMO_CUDA(cudaMemcpy(hD.data(), D, M * sizeof(double), cudaMemcpyDefault));
   DMO_CUDA(cudaMemcpy(hw.data(), weight, (size_t)M * d * sizeof(double), cudaMemcpyDefault));
   DMO_CUDA(cudaMemcpy(hb.data(), bias, M * sizeof(double), cudaMemcpyDefault));
-  DMO_CUDA(cudaMemcpy(ym.data(), y_mean, M * sizeof(double), cudaMemcpyDefault));
-  DMO_CUDA(cudaMemcpy(ys.data(), y_std, M * sizeof(double), cudaMemcpyDefault));
-  DMO_CUDA(cudaMemcpy(lb.data(), xlb, d * sizeof(double), cudaMemcpyDefault));
-  DMO_CUDA(cudaMemcpy(ub.data(), xub, d * sizeof(double), cudaMemcpyDefault));
-  for (int j = 0; j < d; ++j)
-    DMO_REQUIRE(ls[j] > 0.0 && ub[j] != lb[j], "mtgp_create: length scale %d must be > 0 and the input range non-empty", j);
+  for (int j = 0; j < d; ++j) DMO_REQUIRE(ls[j] > 0.0, "%s: length scale %d must be > 0", who, j);
   double bmax = 0.0;
   for (double v : hB) bmax = fmax(bmax, fabs(v));
   for (int s = 0; s < M; ++s) {
-    DMO_REQUIRE(hD[s] > 0.0, "mtgp_create: noise D[%d] = %g must be > 0", s, hD[s]);
+    DMO_REQUIRE(hD[s] > 0.0, "%s: noise D[%d] = %g must be > 0", who, s, hD[s]);
     for (int t = 0; t < M; ++t)
-      DMO_REQUIRE(fabs(hB[(size_t)s * M + t] - hB[(size_t)t * M + s]) <= 1e-12 * bmax, "mtgp_create: B is not symmetric");
+      DMO_REQUIRE(fabs(hB[(size_t)s * M + t] - hB[(size_t)t * M + s]) <= 1e-12 * bmax, "%s: B is not symmetric", who);
   }
   // whitened task covariance D^-1/2 B D^-1/2 = Q diag(lam) Q'
-  std::vector<double> sqD(M), Bt(mm), lam, Q;
+  std::vector<double>& sqD = mb.sqD;
+  std::vector<double>& lam = mb.lam;
+  std::vector<double>& Q = mb.Q;
+  std::vector<double> Bt(mm);
+  sqD.resize(M);
   for (int s = 0; s < M; ++s) sqD[s] = sqrt(hD[s]);
   for (int s = 0; s < M; ++s)
     for (int t = 0; t < M; ++t)
@@ -346,11 +347,13 @@ int dmo_mtgp_create(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_train
   double lmax = 0.0;
   for (int j = 0; j < M; ++j) lmax = fmax(lmax, lam[j]);
   for (int j = 0; j < M; ++j) {
-    DMO_REQUIRE(lam[j] >= -1e-12 * lmax, "mtgp_create: B is not positive semi-definite (eigenvalue %g)", lam[j]);
+    DMO_REQUIRE(lam[j] >= -1e-12 * lmax, "%s: B is not positive semi-definite (eigenvalue %g)", who, lam[j]);
     if (lam[j] < 0.0) lam[j] = 0.0;
   }
   // rotated residuals r_j = sum_s Q_sj (y_s - w_s . x - b_s) / sqrt(D_s), (M, N)
-  std::vector<double> xs(nd), rhat(nm, 0.0), res(M);
+  std::vector<double>& xs = mb.xs;
+  std::vector<double> rhat(nm, 0.0), res(M);
+  xs.resize(nd);
   for (int64_t n = 0; n < N; ++n) {
     for (int s = 0; s < M; ++s) {
       double m = hb[s];
@@ -364,22 +367,52 @@ int dmo_mtgp_create(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_train
     }
     for (int k = 0; k < d; ++k) xs[(size_t)n * d + k] = hx[(size_t)n * d + k] / ls[k];
   }
+  // the M blocks: lambda_j K_x + I over the scaled inputs (unit length scale), factorised in float64
+  std::vector<double> ones_d((size_t)M * d, 1.0), ones_m(M, 1.0);
+  mb.blk_lml.assign(M, 0.0);
+  DMO_TRY(mb.Lf.alloc(ctx, (size_t)M * N * N));
+  DMO_TRY(dmo_gp_fit(ctx, N, d, M, DMO_KERNEL_MATERN52, xs.data(), rhat.data(), lam.data(), ones_d.data(), ones_m.data(), 0.0,
+                     mb.Lf.p, alpha_out, mb.blk_lml.data()));
+  double lml = 0.0;
+  for (int j = 0; j < M; ++j) lml += mb.blk_lml[j];
+  for (int t = 0; t < M; ++t) lml -= 0.5 * (double)N * log(hD[t]);
+  mb.lml = lml;
+  return DMO_OK;
+}
+
+extern "C" {
+
+int dmo_mtgp_create(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_train, const double* Y, const double* length_scale,
+                    const double* B, const double* D, const double* weight, const double* bias, const double* y_mean,
+                    const double* y_std, const double* xlb, const double* xub, double* lml_out, dmo_mtgp** out) {
+  if (!ctx) return DMO_ERR_ARG;
+  DMO_CUDA(cudaSetDevice(ctx->device));
+  DMO_REQUIRE(out, "mtgp_create: null output");
+  *out = nullptr;
+  DMO_REQUIRE(N >= 1 && d >= 1 && d <= MT_FIT_DMAX && M >= 1 && M <= MT_MAX,
+              "mtgp_create: unsupported shape N=%lld d=%d M=%d (1 <= M <= %d, d <= %d)", (long long)N, d, M, MT_MAX, MT_FIT_DMAX);
+  DMO_REQUIRE(y_mean && y_std && xlb && xub, "mtgp_create: null pointer");
+  const size_t nm = (size_t)N * M, mm = (size_t)M * M;
+  std::vector<double> ym(M), ys(M), lb(d), ub(d);
+  DMO_CUDA(cudaMemcpy(ym.data(), y_mean, M * sizeof(double), cudaMemcpyDefault));
+  DMO_CUDA(cudaMemcpy(ys.data(), y_std, M * sizeof(double), cudaMemcpyDefault));
+  DMO_CUDA(cudaMemcpy(lb.data(), xlb, d * sizeof(double), cudaMemcpyDefault));
+  DMO_CUDA(cudaMemcpy(ub.data(), xub, d * sizeof(double), cudaMemcpyDefault));
+  for (int j = 0; j < d; ++j) DMO_REQUIRE(ub[j] != lb[j], "mtgp_create: the input range %d must be non-empty", j);
+  MtBlocks mb;
+  DevBuf<double> alpha;
+  DMO_TRY(alpha.alloc(ctx, nm));
+  DMO_TRY(mtgp_blocks_fit(ctx, "mtgp_create", N, d, M, X_train, Y, length_scale, B, D, weight, bias, mb, alpha.p));
+  const std::vector<double>&ls = mb.ls, &hB = mb.hB, &hD = mb.hD, &hw = mb.hw, &hb = mb.hb, &sqD = mb.sqD, &lam = mb.lam,
+                     &Q = mb.Q, &xs = mb.xs;
+  DevBuf<double>& Lf = mb.Lf;
   std::unique_ptr<dmo_mtgp> mt(new dmo_mtgp());
   mt->N = N;
   mt->d = d;
   mt->M = M;
   const int64_t Npad = mt->Npad = ceil_div(N, 256) * 256;  // the float64 (128) and wgmma (256) Linv tiles
-  // the M blocks: lambda_j K_x + I over the scaled inputs (unit length scale), factorised in float64
-  std::vector<double> ones_d((size_t)M * d, 1.0), ones_m(M, 1.0), blk_lml(M);
-  DevBuf<double> Lf, alpha;
-  DMO_TRY(Lf.alloc(ctx, (size_t)M * N * N));
-  DMO_TRY(alpha.alloc(ctx, nm));
-  DMO_TRY(dmo_gp_fit(ctx, N, d, M, DMO_KERNEL_MATERN52, xs.data(), rhat.data(), lam.data(), ones_d.data(), ones_m.data(), 0.0,
-                     Lf.p, alpha.p, blk_lml.data()));
-  double lml = 0.0;
-  for (int j = 0; j < M; ++j) lml += blk_lml[j];
-  for (int t = 0; t < M; ++t) lml -= 0.5 * (double)N * log(hD[t]);
-  mt->lml = lml;
+  mt->lml = mb.lml;
+  const double lml = mb.lml;
   mt->blk.reset(new dmo_gp());
   dmo_gp* gp = mt->blk.get();
   gp->N = N;

@@ -2,10 +2,11 @@
 
 Drop-ins for ``dmosopt.model_gpytorch.EGP_Matern`` (dmosopt/model_gpytorch.py:1927-2235) and
 ``dmosopt.model_gpytorch.MEGP_Matern`` (:1623-1926), selected in dmosopt by
-``surrogate_method_name="dmosopt_b200.model_gpytorch.EGP_Matern"`` (or ``.MEGP_Matern``).  As with the scikit-learn
-surrogates, *fitting* stays with the host library -- here the reference class itself, which needs gpytorch -- and only
-the posterior is taken over: after training, the hyper-parameters and the model's own normalised training tensors are
-read out, the posterior is factorised once in float64, and every ``predict`` / ``evaluate`` runs on the GPU.
+``surrogate_method_name="dmosopt_b200.model_gpytorch.EGP_Matern"`` (or ``.MEGP_Matern``).  EGP_Matern trains through
+the reference class itself, which needs gpytorch: after training, the hyper-parameters and the model's own normalised
+training tensors are read out, the posterior is factorised once in float64, and every ``predict`` / ``evaluate`` runs
+on the GPU.  MEGP_Matern also trains on the GPU (``fit="gpu"``, ``megp_fit``): the reference's Adam loop and early
+stopping around the exact log marginal likelihood and its gradient (``dmo_mtgp_lml_grad``), without gpytorch.
 
 * ``EGP_Matern``: M independent GPs (ARD length scales, output scale, noise, linear-mean weights / bias per objective);
   ``dmo_gp_create`` / ``dmo_gp_set_linear_mean`` / ``dmo_gp_predict``.
@@ -14,8 +15,8 @@ read out, the posterior is factorised once in float64, and every ``predict`` / `
   (N*M) x (N*M) system splits exactly into M single-output blocks that share one K_* (csrc/gp_multitask.cu).
 
 The predictive variance is the exact one (gpytorch's ``fast_pred_var=False``); ``fast_pred_var=True`` (LOVE) is a
-low-rank approximation of it.  gpytorch is not part of this image, so training through the reference classes is
-untested here; the read-out of a trained model is tested on a stand-in with gpytorch's attribute names, and the
+low-rank approximation of it.  gpytorch is not available here, so training through the reference classes is
+untested; the read-out of a trained model is tested on a stand-in with gpytorch's attribute names, and the
 posterior arithmetic against oracle/egp.py and oracle/megp.py through the ``hyperparameters=`` constructor path
 (tests/test_gpu_parity.py::test_egp_linear_mean_*, tests/test_gpu_megp.py).
 """
@@ -182,20 +183,226 @@ def megp_hyperparameters(gp_model):
     return xn, arr(gp_model.train_targets).reshape(N, M), hp
 
 
+class EarlyStopping:
+    """The early-stopping rule of the reference's exact-GP training: ``AdaptiveEarlyStopping`` with
+    ``EarlyStoppingConfig.for_model_type(EXACT_GP)`` (dmosopt/model_gpytorch.py:588-812), restated.
+
+    Four tests on the loss history, over a window of the last 200 losses: the mean percentage change between successive
+    losses is below ``threshold_pct`` (needs 201 losses); the largest absolute change is below 1e-3; the change from the
+    window's first to its last loss is below 1e-2 relative (not tested when the first is below 1e-3 in magnitude); the
+    means of the first and second half of the window differ by less than 2e-2 relative to the window mean (+ 1e-3)
+    (needs 400 losses).  From iteration 1000 on, when at least two tests hold at ``patience`` = 2 successive calls the
+    rule stops, with the reasons of the tests that hold; a call with fewer than two resets the count."""
+
+    def __init__(self, threshold_pct=0.1, min_iterations=1000, window_size=200, patience=2, warmup_iterations=50,
+                 relative_tolerance=1e-2, absolute_tolerance=1e-3):
+        self.threshold_pct, self.min_iterations, self.window = threshold_pct, min_iterations, window_size
+        self.patience, self.warmup_iterations = patience, warmup_iterations
+        self.rtol, self.atol = relative_tolerance, absolute_tolerance
+        self.count = 0
+
+    def _tests(self, h):
+        w, atol = self.window, self.atol
+        out = []
+        if len(h) >= w + 1:
+            win = h[-w:]
+            pct = np.mean(np.abs(np.diff(win) / np.maximum(np.abs(win[:-1]), atol)) * 100)
+            out.append(f"Mean % change ({pct:.4f}%) < threshold" if pct < self.threshold_pct else "")
+        if len(h) >= w:
+            win = h[-w:]
+            big = np.max(np.abs(np.diff(win)))
+            out.append(f"Max absolute change ({big:.2e}) converged" if big < atol else "")
+            if abs(win[0]) >= atol:
+                rel = abs((win[-1] - win[0]) / win[0])
+                out.append(f"Relative change ({rel:.2e}) converged" if rel < self.rtol else "")
+        if len(h) >= 2 * w:
+            mid = len(h) - w
+            diff = abs(np.mean(h[mid : mid + w // 2]) - np.mean(h[-w // 2 :]))
+            rel = diff / (abs(np.mean(h[-w:])) + atol)
+            out.append(f"Loss plateau detected (relative difference: {rel:.2e})" if rel < 2 * self.rtol else "")
+        return [r for r in out if r]
+
+    def should_stop(self, iteration, loss_history):
+        """(stop, reason) after the loss of ``iteration`` was appended to ``loss_history``."""
+        reasons = self._tests(np.asarray(loss_history))
+        if iteration < self.min_iterations:
+            return False, ""
+        if len(reasons) >= 2:
+            self.count += 1
+            if self.count >= self.patience:
+                return True, "; ".join(reasons)
+        else:
+            self.count = 0
+        return False, ""
+
+
+# gpytorch 1.13's parameterisation of the MEGP model (see DESIGN.md section 4.4), in NumPy float64
+_NOISE_LOWER = 1e-4  # GreaterThan(1e-4) on the task noises and the global noise
+
+
+def _softplus(x):
+    x = np.asarray(x, dtype=np.float64)
+    return np.where(x > 20.0, x, np.log1p(np.exp(np.minimum(x, 20.0))))  # torch.nn.functional.softplus, threshold 20
+
+
+def _softplus_grad(x):
+    x = np.asarray(x, dtype=np.float64)
+    z = np.exp(np.minimum(x, 20.0))
+    return np.where(x > 20.0, 1.0, z / (z + 1.0))
+
+
+def _sigmoid(x):
+    return 1.0 / (1.0 + np.exp(-np.asarray(x, dtype=np.float64)))
+
+
+def megp_initial_raw(d, M, seed=None):
+    """Initial raw parameters: raw_lengthscale 0, covar_factor and raw_var N(0, 1), raw_task_noises and raw_noise 0,
+    one N(0, 1) draw of the LinearMean weights / bias shared by every task.  Draws from np.random.default_rng(seed),
+    seed None meaning 0, in the order covar_factor, raw_var, weights, bias."""
+    rng = np.random.default_rng(0 if seed is None else seed)
+    F = rng.standard_normal((M, 1))
+    raw_var = rng.standard_normal(M)
+    w = rng.standard_normal(d)
+    b = rng.standard_normal()
+    return {"raw_lengthscale": np.zeros(d), "covar_factor": F, "raw_var": raw_var, "raw_task_noises": np.zeros(M),
+            "raw_noise": np.zeros(1), "weights": np.tile(w, (M, 1)), "biases": np.full(M, b)}
+
+
+def megp_natural(raw, lengthscale_bounds=None):
+    """raw parameters -> (length_scale (d,), B (M,M), D (M,), weight (M,d), bias (M,))."""
+    if lengthscale_bounds is None:
+        ls = _softplus(raw["raw_lengthscale"])
+    else:
+        lo, hi = float(lengthscale_bounds[0]), float(lengthscale_bounds[1])
+        ls = lo + (hi - lo) * _sigmoid(raw["raw_lengthscale"])
+    F = raw["covar_factor"]
+    B = F @ F.T + np.diag(_softplus(raw["raw_var"]))
+    D = (_NOISE_LOWER + _softplus(raw["raw_task_noises"])) + (_NOISE_LOWER + _softplus(raw["raw_noise"]))[0]
+    return ls, B, D, raw["weights"], raw["biases"]
+
+
+def megp_raw_grad(raw, g, lengthscale_bounds=None):
+    """Chain rule: gradients with respect to (length_scale, B with independent entries, D, weight, bias) -> gradients
+    with respect to the raw parameters."""
+    x = raw["raw_lengthscale"]
+    if lengthscale_bounds is None:
+        gl = g["length_scale"] * _softplus_grad(x)
+    else:
+        lo, hi = float(lengthscale_bounds[0]), float(lengthscale_bounds[1])
+        s = _sigmoid(x)
+        gl = g["length_scale"] * ((hi - lo) * (s * (1.0 - s)))
+    gB = g["B"]
+    return {"raw_lengthscale": gl, "covar_factor": (gB + gB.T) @ raw["covar_factor"],
+            "raw_var": np.diag(gB) * _softplus_grad(raw["raw_var"]), "raw_task_noises": g["D"] * _softplus_grad(raw["raw_task_noises"]),
+            "raw_noise": np.array([np.sum(g["D"])]) * _softplus_grad(raw["raw_noise"]), "weights": g["weight"], "biases": g["bias"]}
+
+
+def _fma(a, b, c):
+    """a * b + c with one rounding (as torch's CPU kernels compute lerp / addcmul): the product split exactly
+    (Dekker), the sum exactly (Knuth's two-sum), the two error terms added before the final rounding."""
+    p = a * b
+    t = 134217729.0 * a  # 2^27 + 1
+    ah = t - (t - a)
+    t = 134217729.0 * b
+    bh = t - (t - b)
+    al, bl = a - ah, b - bh
+    e = ((ah * bh - p) + ah * bl + al * bh) + al * bl
+    s = p + c
+    z = s - p
+    return s + (((p - (s - z)) + (c - z)) + e)
+
+
+class Adam:
+    """torch.optim.Adam with its defaults (betas 0.9 / 0.999, eps 1e-8, no weight decay) on a dict of float64 arrays,
+    in torch's order of operations and roundings: m <- fma(1 - b1, g - m, m) (lerp); v <- fma((1 - b2) g, g, v b2)
+    (addcmul); denom = sqrt(v) / sqrt(1 - b2^t) + eps; p <- p + (-(lr / (1 - b1^t)) m) / denom (addcdiv)."""
+
+    def __init__(self, lr=0.01, betas=(0.9, 0.999), eps=1e-8):
+        self.lr, self.b1, self.b2, self.eps = lr, betas[0], betas[1], eps
+        self.t, self.m, self.v = 0, {}, {}
+
+    def step(self, params, grads):
+        self.t += 1
+        bc1 = 1.0 - self.b1**self.t
+        bc2_sqrt = (1.0 - self.b2**self.t) ** 0.5
+        step_size = self.lr / bc1
+        for k, g in grads.items():
+            m = self.m.get(k, np.zeros_like(g))
+            v = self.v.get(k, np.zeros_like(g))
+            m = _fma(np.full_like(g, 1.0 - self.b1), g - m, m)
+            v = _fma((1.0 - self.b2) * g, g, v * self.b2)
+            self.m[k], self.v[k] = m, v
+            params[k] = params[k] + ((-step_size) * m) / (np.sqrt(v) / bc2_sqrt + self.eps)
+
+
+def megp_fit(xn, yn, *, lengthscale_bounds=None, adam_lr=0.01, n_iter=5000, min_loss_pct_change=0.1, seed=None, logger=None,
+             initial_raw=None):
+    """Train the MEGP model on the GPU: the reference's Adam loop (dmosopt/model_gpytorch.py:1722-1829) on the exact
+    log marginal likelihood and its gradient (dmo_mtgp_lml_grad).  xn (N,d) normalised inputs, yn (N,M) normalised
+    targets.  Loss = -lml / (N M) (gpytorch's ExactMarginalLogLikelihood); the loss logged at iteration it is the one
+    before that iteration's step.  Returns (hyperparameters, info): the ``hyperparameters=`` dict of MEGP_Matern at the
+    final parameters, and info with ``loss`` (array), ``iterations``, ``stop_reason`` and ``raw`` (final raw parameters).
+    ``initial_raw`` replaces the seeded initial draws (megp_initial_raw)."""
+    xn = np.ascontiguousarray(xn, dtype=np.float64)
+    yn = np.ascontiguousarray(yn, dtype=np.float64).reshape(xn.shape[0], -1)
+    N, d = xn.shape
+    M = yn.shape[1]
+    raw = megp_initial_raw(d, M, seed) if initial_raw is None else {k: np.array(v, dtype=np.float64) for k, v in initial_raw.items()}
+    adam = Adam(lr=adam_lr)
+    stopper = EarlyStopping(threshold_pct=min_loss_pct_change)
+    losses, reason = [], "n_iter"
+    for it in range(n_iter):
+        ls, B, D, w, b = megp_natural(raw, lengthscale_bounds)
+        lml, g = _lib.mtgp_lml_grad(xn, yn, ls, B, D, w, b)
+        loss = -lml / (N * M)
+        graw = megp_raw_grad(raw, g, lengthscale_bounds)
+        adam.step(raw, {k: v * (-1.0 / (N * M)) for k, v in graw.items()})
+        losses.append(loss)
+        if it % 100 == 0 and logger is not None:
+            noise = _NOISE_LOWER + float(_softplus(raw["raw_noise"])[0])
+            logger.info(f"MEGP_Matern: iter {it}/{n_iter} - Loss: {loss:.3f}  noise: {noise:.3f}")
+        if it >= stopper.warmup_iterations:
+            stop, why = stopper.should_stop(it, np.array(losses))
+            if stop:
+                if logger is not None:
+                    logger.info(f"MEGP_Matern: early stop at iteration {it + 1}: {why}")
+                reason = why
+                break
+    ls, B, D, w, b = megp_natural(raw, lengthscale_bounds)
+    hp = {"lengthscale": ls, "covar_factor": raw["covar_factor"].copy(), "var": _softplus(raw["raw_var"]),
+          "task_noises": _NOISE_LOWER + _softplus(raw["raw_task_noises"]), "noise": _NOISE_LOWER + float(_softplus(raw["raw_noise"])[0]),
+          "weights": w.copy(), "biases": b.copy()}
+    return hp, {"loss": np.asarray(losses), "iterations": len(losses), "stop_reason": reason, "raw": raw}
+
+
+def _reference_can_train():
+    """True when dmosopt.model_gpytorch imports with gpytorch available."""
+    try:
+        import dmosopt.model_gpytorch as ref
+    except Exception:
+        return False
+    return bool(getattr(ref, "_has_gpytorch", False))
+
+
 class MEGP_Matern:
     """Multitask exact-GP surrogate; the reference constructor signature (model_gpytorch.py:1624-1647) plus
-    ``precision`` ("fp64", the default, or "tensor"; there is no "auto" calibration for this model) and
+    ``precision`` ("fp64", the default, or "tensor"; there is no "auto" calibration for this model),
     ``hyperparameters`` (dict with lengthscale (d,), covar_factor (M, rank), var (M,), task_noises (M,), noise, weights
-    (M,d), biases (M,)): when given, training is skipped.  ``log_marginal_likelihood_value`` is the exact log marginal
-    likelihood of the normalised targets under the model."""
+    (M,d), biases (M,)): when given, training is skipped, and ``fit``: "gpu" trains with megp_fit (Adam on the exact
+    log marginal likelihood, on the GPU), "reference" through the reference class (needs gpytorch); None uses the
+    reference class where it can train and "gpu" otherwise.  After a fit ``hyperparameters`` and ``fit_info`` hold the
+    result.  ``log_marginal_likelihood_value`` is the exact log marginal likelihood of the normalised targets under the
+    model."""
 
     def __init__(self, xin, yin, nInput, nOutput, xlb, xub, seed=None, gp_lengthscale_bounds=None, gp_likelihood_sigma=None,
                  batch_size=None, preconditioner_size=100, adam_lr=0.01, fast_pred_var=False, n_iter=5000,
                  min_loss_pct_change=0.1, return_mean_variance=False, use_cuda=False, nan="remove", top_k=None, logger=None,
-                 precision="fp64", hyperparameters=None, **kwargs):
+                 precision="fp64", hyperparameters=None, fit=None, **kwargs):
         codes = {"fp64": _lib.GP_FP64, "tensor": _lib.GP_TENSOR, _lib.GP_FP64: _lib.GP_FP64, _lib.GP_TENSOR: _lib.GP_TENSOR}
         if precision not in codes:
             raise ValueError(f"MEGP_Matern: precision must be 'fp64' or 'tensor' (got {precision!r})")
+        if fit not in (None, "gpu", "reference"):
+            raise ValueError(f"MEGP_Matern: fit must be 'gpu', 'reference' or None (got {fit!r})")
         self.precision = codes[precision]
         self.nInput, self.nOutput = nInput, nOutput
         self.xlb = np.asarray(xlb, dtype=np.float64)
@@ -203,7 +410,12 @@ class MEGP_Matern:
         self.xrng = np.where(np.isclose(xub - self.xlb, 0.0, rtol=1e-6, atol=1e-6), 1.0, xub - self.xlb)  # model_gpytorch.py:1662-1664
         self.return_mean_variance = return_mean_variance
         self.logger = logger
-        if hyperparameters is None:
+        self.fit_info = None
+        if hyperparameters is None and fit is None:
+            fit = "reference" if _reference_can_train() else "gpu"
+        if hyperparameters is None and fit == "gpu" and gp_likelihood_sigma is not None:
+            raise ValueError("MEGP_Matern: the GPU fit has no noise prior (gp_likelihood_sigma); use fit='reference'")
+        if hyperparameters is None and fit == "reference":
             ref_kwargs = dict(seed=seed, gp_lengthscale_bounds=gp_lengthscale_bounds, gp_likelihood_sigma=gp_likelihood_sigma,
                               batch_size=batch_size, preconditioner_size=preconditioner_size, adam_lr=adam_lr,
                               fast_pred_var=fast_pred_var, n_iter=n_iter, min_loss_pct_change=min_loss_pct_change,
@@ -221,6 +433,13 @@ class MEGP_Matern:
                 xin, yin = xs[:top_k], ys[:top_k]
             xn = (xin - self.xlb) / self.xrng
             yn, ymean, ystd = normalise_targets(yin)
+            if hyperparameters is None:
+                if logger is not None:
+                    logger.info("MEGP_Matern: optimizing regressor...")
+                hyperparameters, self.fit_info = megp_fit(xn, yn, lengthscale_bounds=gp_lengthscale_bounds, adam_lr=adam_lr,
+                                                          n_iter=n_iter, min_loss_pct_change=min_loss_pct_change, seed=seed,
+                                                          logger=logger)
+        self.hyperparameters = hyperparameters
         self._upload(xn, yn, ymean, ystd, hyperparameters)
 
     @staticmethod

@@ -246,6 +246,15 @@ int dmo_mtgp_create(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_train
 int dmo_mtgp_predict(dmo_ctx* ctx, dmo_mtgp* mt, const double* X, int64_t P, double* mean, double* var,
                      int precision);
 int dmo_mtgp_destroy(dmo_ctx* ctx, dmo_mtgp* mt);
+/* dmo_mtgp_lml_grad: the exact log marginal likelihood of the same model and its gradient, for training.
+ *   Arguments and limits as dmo_mtgp_create (host or device pointers).  lml_out (scalar) is bit-identical to what
+ *   dmo_mtgp_create reports for the same inputs; the gradients are d lml / d length_scale (d,), d lml / d B (M,M,
+ *   entries treated as independent), d lml / d D (M,), d lml / d weight (M,d), d lml / d bias (M,).  Float64,
+ *   deterministic (fixed-order reductions); returns when the outputs are filled. */
+int dmo_mtgp_lml_grad(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_train, const double* Y,
+                      const double* length_scale, const double* B, const double* D, const double* weight,
+                      const double* bias, double* lml_out, double* g_length_scale, double* g_B, double* g_D,
+                      double* g_weight, double* g_bias);
 
 /* ---- A16: exact hypervolume ---------------------------------------------------
  * replaces hv.AdaptiveHyperVolume.compute_hypervolume(..., 'box') (dmosopt/hv.py:123-189)

@@ -181,6 +181,55 @@ def mtgp_sweep():
           f"var err / prior {np.max(np.abs(vt_t - vt_f) / prior):.2e}", flush=True)
 
 
+def mtgp_fit_sweep():
+    """MEGP_Matern training: one dmo_mtgp_lml_grad evaluation (median of warm calls, CUDA events per phase) for
+    N in {1024, 2048, 4096}, M in {2, 3}, d = 30, with the counted float64 work (block Cholesky, triangular inverse and
+    the sum of lambda_j A_j^-1: about M N^3 flop; gradient pass: about N^2 (2 d + M^2) flop), then one default megp_fit
+    on ZDT1 data (d = 30, M = 2, N = 2048)."""
+    from dmosopt_b200.model_gpytorch import megp_fit, megp_initial_raw, megp_natural, normalise_targets
+
+    L.context()
+    print(device_line(), flush=True)
+    rng = np.random.default_rng(4)
+    d = 30
+    for N in (1024, 2048, 4096):
+        for M in (2, 3):
+            X = rng.random((N, d))
+            Y = np.column_stack([np.sin(3 * X[:, :4].sum(axis=1) + k) + X[:, 4 + k] ** 2 for k in range(M)])
+            yn, _, _ = normalise_targets(Y)
+            ls, B, D, w, b = megp_natural(megp_initial_raw(d, M, seed=1))
+            L.mtgp_lml_grad(X, yn, ls, B, D, w, b)  # warm-up
+            L.profile_enable(True)
+            walls = []
+            for _ in range(5):
+                L.timer_begin()
+                L.mtgp_lml_grad(X, yn, ls, B, D, w, b)
+                walls.append(L.timer_end())
+            rep = L.profile_report()
+            L.profile_enable(False)
+            ph = {k: rep[k][0] / rep[k][1] for k in ("mtgp_lg_fit", "mtgp_lg_linv", "mtgp_lg_ainv", "mtgp_lg_grad") if k in rep}
+            ms = float(np.median(walls))
+            f3 = M * float(N) ** 3
+            f2 = float(N) ** 2 * (2 * d + M * M)
+            dense = ph["mtgp_lg_fit"] + ph["mtgp_lg_linv"] + ph["mtgp_lg_ainv"]
+            parts = ", ".join(f"{k[8:]} {v:.2f} ms" for k, v in ph.items())
+            print(f"mtgp_lml_grad N={N} M={M} d={d}: {ms:.2f} ms median of 5 [{parts}]; gradient pass {100 * ph['mtgp_lg_grad'] / ms:.1f} % "
+                  f"of the call; M N^3 = {f3 / 1e9:.1f} GFLOP in {dense:.2f} ms = {f3 / dense / 1e9:.2f} TFLOP/s fp64 "
+                  f"(Sigma lambda A^-1 alone: {f3 / 3 / ph['mtgp_lg_ainv'] / 1e9:.2f} TFLOP/s); N^2 (2d + M^2) = {f2 / 1e9:.2f} GFLOP "
+                  f"in {ph['mtgp_lg_grad']:.2f} ms", flush=True)
+    N, M = 2048, 2
+    X = rng.random((N, d))
+    g = 1.0 + 9.0 / (d - 1) * X[:, 1:].sum(axis=1)
+    Y = np.column_stack((X[:, 0], g * (1.0 - np.sqrt(X[:, 0] / g))))
+    yn, _, _ = normalise_targets(Y)
+    t0 = time.perf_counter()
+    hp, info = megp_fit(X, yn)
+    wall = time.perf_counter() - t0
+    print(f"megp_fit ZDT1 N={N} M={M} d={d} (defaults: lr 0.01, n_iter 5000): {info['iterations']} iterations, {wall:.1f} s "
+          f"({1e3 * wall / info['iterations']:.1f} ms per iteration), loss {info['loss'][0]:.4f} -> {info['loss'][-1]:.4f}, "
+          f"stop: {info['stop_reason']}", flush=True)
+
+
 def stream_sweep():
     """The HBM-bound kernels at the BASELINE shape: crowding / euclidean distance (n = 131072, M = 3), SBX + mutation
     (pop 65536, d 30), mean kernel's neighbours, hypervolume of a 65536-point 3-D front.  Prints time and the achieved
@@ -225,5 +274,8 @@ if __name__ == "__main__":
         sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "mtgp":
         mtgp_sweep()
+        sys.exit(0)
+    if len(sys.argv) > 1 and sys.argv[1] == "mtgp_fit":
+        mtgp_fit_sweep()
         sys.exit(0)
     main()
