@@ -148,43 +148,22 @@ __device__ __forceinline__ void wgmma_f16_m64n256(float (&d)[128], uint64_t ades
 // ------------------------------------------------------------------------------------------------ the contraction
 // Work items and their order.  An item is (objective, 128 candidates, item q of the candidate block); the q of a
 // candidate block are adjacent in the list, so the CTAs that share a K_* tile start together at k = 0 and walk k at the
-// same (MMA-bound) rate: one of them pulls the tile from DRAM and the others hit it in L2.
-//   * paired (default): item q owns the Linv row blocks {q, n_jt - 1 - q}, so every item costs the same n_jt + 1
-//     k-blocks and a static round-robin over the persistent CTAs has a tail of at most one item;
-//   * halves (DMO_GP_TC=2, the previous schedule): item 0 owns row blocks [0, j_split), item 1 [j_split, n_jt).
-// Each item writes its partial sums to its own plane q of vnorm (and mnorm); var_finish_tc_kernel adds the planes in
-// a fixed order.
+// same (MMA-bound) rate: one of them pulls the tile from DRAM and the others hit it in L2.  Item q owns the Linv row
+// blocks {q, n_jt - 1 - q} (one block when they coincide), so every item costs the same n_jt + 1 k-blocks and a static
+// round-robin over the persistent CTAs has a tail of at most one item.  Each item writes its partial sums to its own
+// plane q of vnorm; var_finish_tc_kernel adds the planes in a fixed order.
 struct GemmParams {
   int M, n_pb, n_jt, n_q;  // n_q items per candidate block
-  int paired, j_split;
   int64_t k_rows, l_rows;
   const float* inv_scale;
   double* vnorm;  // [n_q][M][vn_ld]
   int64_t vn_ld;
   int* abort_flag;
-  const float* zf;        // [M][l_rows] whitened targets (nullptr: the mean is not taken from this contraction)
-  double* mnorm;          // [n_q][M][vn_ld] partial sums of D z
-  const unsigned* ready;  // [n_pb / 2] completion counters of the K_* producer (nullptr: K_* is complete at launch)
-  unsigned ready_target;
-  int dbg;  // DMO_GP_DBG bits (diagnostics): 1 = no proxy fence, 2 = no nanosleep in the wait loop
 };
 
-__device__ __forceinline__ int item_blocks(const GemmParams& p, int q) {
-  if (p.paired) return q == p.n_jt - 1 - q ? 1 : 2;
-  return q ? p.n_jt - p.j_split : p.j_split;
-}
-// s-th row block of item q; in the paired schedule the short one comes first: its K_* tiles are read again right away
-// by the long one
-__device__ __forceinline__ int item_row_block(const GemmParams& p, int q, int s) {
-  if (p.paired) return s ? p.n_jt - 1 - q : q;
-  return (q ? p.j_split : 0) + s;
-}
-
-__device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
-  unsigned v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
+__device__ __forceinline__ int item_blocks(const GemmParams& p, int q) { return q == p.n_jt - 1 - q ? 1 : 2; }
+// s-th row block of item q; the short one comes first: its K_* tiles are read again right away by the long one
+__device__ __forceinline__ int item_row_block(const GemmParams& p, int q, int s) { return s ? p.n_jt - 1 - q : q; }
 
 __global__ void __launch_bounds__(NTHREADS, 1)
     gp_var_wgmma_kernel(const __grid_constant__ CUtensorMap map_kh, const __grid_constant__ CUtensorMap map_kl,
@@ -217,20 +196,6 @@ __global__ void __launch_bounds__(NTHREADS, 1)
       for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
         const int m = w / per_m, r = w - m * per_m;
         const int pb = r / prm.n_q, q = r - pb * prm.n_q;
-        if (prm.ready) {  // the K_* rows of this candidate block must have been written (by another kernel, generic proxy)
-          uint32_t spins = 0;
-          while (ld_acquire_u32(prm.ready + (pb >> 1)) < prm.ready_target) {
-            if (!(prm.dbg & 2)) __nanosleep(256);
-            if ((++spins & 0xFFu) == 0u) {
-              if (*abort_flag) break;
-              if (spins > (1u << 23)) {  // ~2 s: the producer is not running
-                *abort_flag = 2;
-                break;
-              }
-            }
-          }
-          if (!(prm.dbg & 1)) asm volatile("fence.proxy.async;" ::: "memory");  // order the TMA (async proxy) reads after the acquire
-        }
         const int a_row = (int)(m * prm.k_rows + (int64_t)pb * TMV);
         const int nb = item_blocks(prm, q);
         for (int s = 0; s < nb; ++s) {
@@ -267,8 +232,7 @@ __global__ void __launch_bounds__(NTHREADS, 1)
     const int m = w / per_m, r = w - m * per_m;
     const int pb = r / prm.n_q, q = r - pb * prm.n_q;
     const float* isc = prm.inv_scale + (int64_t)m * prm.l_rows;
-    const float* zf = prm.zf ? prm.zf + (int64_t)m * prm.l_rows : nullptr;
-    double total0 = 0.0, total1 = 0.0, mtot0 = 0.0, mtot1 = 0.0;
+    double total0 = 0.0, total1 = 0.0;
     const int nb = item_blocks(prm, q);
     for (int s = 0; s < nb; ++s) {
       const int jt = item_row_block(prm, q, s);
@@ -304,11 +268,9 @@ __global__ void __launch_bounds__(NTHREADS, 1)
       // per 32 columns a thread holds 8 squares of each of its rows, in four fp32 partial sums folded into float64: the
       // rounding of the sum of squares stays at the 2^-24 level instead of growing with N
       const float* sc = isc + jt * TN + col0;
-      const float* zc = zf ? zf + jt * TN + col0 : nullptr;
 #pragma unroll
       for (int g = 0; g < TN / 32; ++g) {
         float p0[4] = {0.f, 0.f, 0.f, 0.f}, p1[4] = {0.f, 0.f, 0.f, 0.f};
-        float q0[4] = {0.f, 0.f, 0.f, 0.f}, q1[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
           const int i = 4 * g + u;
@@ -317,18 +279,9 @@ __global__ void __launch_bounds__(NTHREADS, 1)
           const float t10 = acc[4 * i + 2] * sv.x, t11 = acc[4 * i + 3] * sv.y;
           p0[u] = fmaf(t01, t01, t00 * t00);
           p1[u] = fmaf(t11, t11, t10 * t10);
-          if (zc) {  // posterior mean = D z out of the same accumulator (z = L^-1 y_n)
-            const float2 zv = __ldg(reinterpret_cast<const float2*>(zc + 8 * i));
-            q0[u] = fmaf(t01, zv.y, t00 * zv.x);
-            q1[u] = fmaf(t11, zv.y, t10 * zv.x);
-          }
         }
         total0 += ((double)p0[0] + (double)p0[1]) + ((double)p0[2] + (double)p0[3]);
         total1 += ((double)p1[0] + (double)p1[1]) + ((double)p1[2] + (double)p1[3]);
-        if (zc) {
-          mtot0 += ((double)q0[0] + (double)q0[1]) + ((double)q0[2] + (double)q0[3]);
-          mtot1 += ((double)q1[0] + (double)q1[1]) + ((double)q1[2] + (double)q1[3]);
-        }
       }
     }
     // the four lanes of a quad hold disjoint columns of the same two rows
@@ -336,17 +289,11 @@ __global__ void __launch_bounds__(NTHREADS, 1)
     for (int o = 1; o < 4; o <<= 1) {
       total0 += __shfl_xor_sync(0xffffffffu, total0, o);
       total1 += __shfl_xor_sync(0xffffffffu, total1, o);
-      mtot0 += __shfl_xor_sync(0xffffffffu, mtot0, o);
-      mtot1 += __shfl_xor_sync(0xffffffffu, mtot1, o);
     }
     if ((lane & 3) == 0) {
       const int64_t o = ((int64_t)q * prm.M + m) * prm.vn_ld + (int64_t)pb * TMV + row0;
       prm.vnorm[o] = total0;
       prm.vnorm[o + 8] = total1;
-      if (zf) {
-        prm.mnorm[o] = mtot0;
-        prm.mnorm[o + 8] = mtot1;
-      }
     }
   }
 }
@@ -434,7 +381,7 @@ __global__ void __launch_bounds__(KT_TN)
                         const double* __restrict__ Xt, int64_t N, int d, int M, int kind,
                         const double* __restrict__ inv_ls, const double* __restrict__ constant,
                         const int* __restrict__ k_exp, int64_t ldk, int64_t plane, uint16_t* __restrict__ Kh,
-                        uint16_t* __restrict__ Kl, unsigned* __restrict__ ready) {
+                        uint16_t* __restrict__ Kl) {
   extern __shared__ __align__(16) float sxf[];  // [KT_TP][DMAX] candidate tile, then [M][DMAX] 1/l, [M] c * 2^kexp
   float* s_il = sxf + KT_TP * DMAX;
   float* s_c = s_il + M * DMAX;
@@ -521,15 +468,6 @@ __global__ void __launch_bounds__(KT_TN)
       const int64_t o = (m * plane + pl * ldk + n0) >> 1;
       Kh32[o] = *reinterpret_cast<const uint32_t*>(&h);
       Kl32[o] = *reinterpret_cast<const uint32_t*>(&l);
-    }
-  }
-  if (ready) {
-    // publish this block's rows to the variance kernel that is already running (v3::gp_var_tc3_kernel): every thread's
-    // stores happen-before the barrier, the fence makes them visible at GPU scope before the counter moves
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      __threadfence();
-      atomicAdd(ready + pt0 / 256, 1u);
     }
   }
 }
@@ -900,8 +838,8 @@ __global__ void mean_split_kernel(const uint16_t* __restrict__ Kh, const uint16_
   if (lane == 0) mean[(p_base + pl) * M + m] = ystd[m] * scalbn(s, -k_exp[m]) + ymean[m];
 }
 
-// mean[p][m] = y_std * sum over the work items' partial sums of D z + y_mean (fixed order)
-__global__ void mean_finish_tc_kernel(const double* __restrict__ mnorm, int nplanes, int64_t Pc, int64_t ld, int M,
+// mean[p][m] = y_std * sum over the training-set slices' partial sums of K_* alpha + y_mean (fixed order)
+__global__ void mean_finish_tc_kernel(const double* __restrict__ mpart, int nplanes, int64_t Pc, int64_t ld, int M,
                                       const double* __restrict__ ymean, const double* __restrict__ ystd, int64_t p_base,
                                       double* __restrict__ mean) {
   int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -909,7 +847,7 @@ __global__ void mean_finish_tc_kernel(const double* __restrict__ mnorm, int npla
   int64_t pl = t / M;
   int m = (int)(t - pl * M);
   double s = 0.0;
-  for (int q = 0; q < nplanes; ++q) s += mnorm[((int64_t)q * M + m) * ld + pl];
+  for (int q = 0; q < nplanes; ++q) s += mpart[((int64_t)q * M + m) * ld + pl];
   mean[(p_base + pl) * M + m] = ystd[m] * s + ymean[m];
 }
 
@@ -1082,98 +1020,52 @@ int gp_var_contract_tensor(dmo_ctx* ctx, dmo_gp* gp, const uint16_t* Kh, const u
   prm.n_pb = (int)(Pcpad / TMV);
   prm.n_jt = (int)(Npad / TN);
   prm.n_q = gp_tensor_var_planes(Npad);
-  prm.paired = 1;
-  prm.j_split = prm.n_jt;
   prm.k_rows = k_rows;
   prm.l_rows = Npad;
   prm.inv_scale = gp->Lscale.p;
   prm.vnorm = vnorm;
   prm.vn_ld = vn_ld;
   prm.abort_flag = abort_flag;
-  prm.zf = nullptr;
-  prm.mnorm = nullptr;
-  prm.ready = nullptr;
-  prm.ready_target = 0;
-  prm.dbg = 0;
   const int n_work = prm.M * prm.n_pb * prm.n_q;
   const int grid = n_work < ctx->sm_count ? n_work : ctx->sm_count;
   DMO_LAUNCH(gp_var_wgmma_kernel, grid, NTHREADS, GEMM_SMEM, map_kh, map_kl, map_lh, map_ll, prm);
   return DMO_OK;
 }
 
-int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var, bool mean_from_d) {
+int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var) {
   const int64_t N = gp->N, Npad = gp->Npad;
   const int M = gp->M, d = gp->d;
   DMO_REQUIRE(M <= 16, "gp_predict(tensor): at most 16 objectives per model (got %d)", M);
   DMO_REQUIRE(d <= 64, "gp_predict(tensor): at most 64 input dimensions (got %d); use DMO_GP_FP64", d);
   DMO_REQUIRE(Npad % TN == 0, "gp_predict(tensor): internal padding error");
-  if (!d_var && d <= KM_D && M <= 6 && !(getenv("DMO_GP_MEAN_DIRECT") && atoi(getenv("DMO_GP_MEAN_DIRECT")) == 0))
+  if (!d_var && d <= KM_D && M <= 6)
     return gp_mean_direct(ctx, gp, dXn, P, d_mean);  // nothing but the mean is wanted: K_* stays in registers
   DMO_TRY(prepare_tensor_state(ctx, gp));
-  // work schedule of the contraction: 3 (default) = equal-cost paired row blocks, optionally overlapped with the K_*
-  // producer; 2 = the previous schedule, two halves of the row blocks per candidate block (DMO_GP_TC=2, kept for comparison)
-  int version = 3;
-  if (const char* e = getenv("DMO_GP_TC")) version = atoi(e) == 2 ? 2 : 3;
-  // DMO_GP_OVERLAP=1 (experimental, off by default): launch the contraction while the K_* producer is still running on
-  // the context's second stream and let its TMA thread wait on per-candidate-block completion counters.  The
-  // co-residency of the two kernels is not guaranteed by the hardware scheduler, so the in-line order is the product path.
-  const bool overlap = version == 3 && getenv("DMO_GP_OVERLAP") && atoi(getenv("DMO_GP_OVERLAP"));
-  const int dbg = getenv("DMO_GP_DBG") ? atoi(getenv("DMO_GP_DBG")) : 0;  // 4: event instead of flags, 8: mean after var
-  const bool use_flags = overlap && !(dbg & 4);
-  // mean from the contraction (D z) instead of the K_* alpha pass: only with the variance, version 3 and a model created from L
-  mean_from_d = mean_from_d && d_var != nullptr && version == 3 && gp->z_ready;
   constexpr int64_t TMv = KM_Q;  // candidate padding: the K_* producers write 256-candidate blocks
   // candidate chunk: K_* hi/lo (2 x M x Pc x Npad fp16) within ~6 GiB
   int64_t Pc_max = ((int64_t)6 << 30) / ((int64_t)M * Npad * 4);
   Pc_max = (Pc_max / TMv) * TMv;
   if (Pc_max < TMv) Pc_max = TMv;
   const int64_t Pc_alloc = P < Pc_max ? ceil_div(P, TMv) * TMv : Pc_max;
-  const int n_jt = (int)(Npad / TN);
-  const int n_q = version == 3 ? (n_jt + 1) / 2 : 2;
-  const int64_t n_chunks = ceil_div(P, Pc_alloc);
-  const int n_pb_alloc = (int)(Pc_alloc / TMv);
+  const int n_q = gp_tensor_var_planes(Npad);
   DevBuf<uint16_t> Kh, Kl;
   DevBuf<double> vnorm;
   DevBuf<int> abort_flag;
-  DevBuf<unsigned> ready;
   DMO_TRY(Kh.alloc(ctx, (size_t)M * Pc_alloc * Npad));
   DMO_TRY(Kl.alloc(ctx, (size_t)M * Pc_alloc * Npad));
   DMO_TRY(vnorm.alloc(ctx, (size_t)n_q * M * Pc_alloc));
-  DevBuf<double> mnorm;
-  if (mean_from_d) DMO_TRY(mnorm.alloc(ctx, (size_t)n_q * M * Pc_alloc));
   DMO_TRY(abort_flag.alloc(ctx, 1));
-  DMO_TRY(ready.alloc(ctx, (size_t)n_chunks * n_pb_alloc));
   DMO_CUDA(cudaMemsetAsync(abort_flag.p, 0, sizeof(int), ctx->stream));
-  DMO_CUDA(cudaMemsetAsync(ready.p, 0, (size_t)n_chunks * n_pb_alloc * sizeof(unsigned), ctx->stream));
-  CUtensorMap map_kh, map_kl, map_lh, map_ll;
-  DMO_TRY(make_map(ctx, &map_kh, Kh.p, (uint64_t)M * Pc_alloc, (uint64_t)Npad, TMV, TK, CU_TENSOR_MAP_SWIZZLE_64B));
-  DMO_TRY(make_map(ctx, &map_kl, Kl.p, (uint64_t)M * Pc_alloc, (uint64_t)Npad, TMV, TK, CU_TENSOR_MAP_SWIZZLE_64B));
-  DMO_TRY(make_map(ctx, &map_lh, gp->Lhi.p, (uint64_t)M * Npad, (uint64_t)Npad, TN, TK, CU_TENSOR_MAP_SWIZZLE_64B));
-  DMO_TRY(make_map(ctx, &map_ll, gp->Llo.p, (uint64_t)M * Npad, (uint64_t)Npad, TN, TK, CU_TENSOR_MAP_SWIZZLE_64B));
-  DMO_CUDA(cudaFuncSetAttribute(gp_var_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GEMM_SMEM));
   const int64_t kplane = Pc_alloc * Npad;
   // K_* producer fused with the mean (d <= 32, M <= 6; DMO_GP_FUSED=0 keeps kstar_tensor_kernel + mean_split_kernel)
   // (per-dimension length scales with more than two objectives keep the two-kernel route: a distance pass per objective)
-  const bool fused = !overlap && !mean_from_d && !(dbg & 8) && d <= KM_D && M <= 6 && (gp->isotropic || M <= 2) &&
+  const bool fused = d <= KM_D && M <= 6 && (gp->isotropic || M <= 2) &&
                      !(getenv("DMO_GP_FUSED") && atoi(getenv("DMO_GP_FUSED")) == 0);
   DevBuf<double> mpart;
   if (fused) DMO_TRY(prepare_direct_state(ctx, gp));
-  // producer side (K_* and the mean) on the second stream when overlapping, else in line
-  cudaStream_t ps = overlap ? ctx->aux : ctx->stream;
-  if (overlap) {
-    DMO_CUDA(cudaEventRecord(ctx->ev_fork, ctx->stream));  // allocations, memsets and Xn are ready
-    DMO_CUDA(cudaStreamWaitEvent(ctx->aux, ctx->ev_fork, 0));
-  }
-  int64_t chunk = 0;
-  for (int64_t p_base = 0; p_base < P; p_base += Pc_alloc, ++chunk) {
+  for (int64_t p_base = 0; p_base < P; p_base += Pc_alloc) {
     const int64_t Pc = (P - p_base) < Pc_alloc ? (P - p_base) : Pc_alloc;
     const int64_t Pcpad = ceil_div(Pc, TMv) * TMv;
-    unsigned* rdy = ready.p + chunk * n_pb_alloc;
-    dim3 gk((unsigned)(Npad / (2 * KT_TN)), (unsigned)ceil_div(Pcpad, KT_TP));
-    if (overlap && chunk > 0) {  // the K_* buffers are reused: the previous chunk's contraction must have drained them
-      DMO_CUDA(cudaEventRecord(ctx->ev_fork, ctx->stream));
-      DMO_CUDA(cudaStreamWaitEvent(ctx->aux, ctx->ev_fork, 0));
-    }
     if (fused) {
       // K_* and the mean from one kernel (kstar_mean_kernel): K_* is written once and never read back for the mean
       int64_t n_per_block = Npad;
@@ -1210,14 +1102,14 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
       DMO_LAUNCH(mean_finish_tc_kernel, (unsigned)ceil_div(Pc * M, 256), 256, 0, mpart.p, (int)nsplit, Pc, Pcpad, M, gp->ymean.p,
                  gp->ystd.p, p_base, d_mean);
     } else {
-    {
-        ProfileScope ps_(ctx, "gp_kstar", ps);
+      {
+        ProfileScope ps_(ctx, "gp_kstar");
         const int dmax = d <= 32 ? 32 : 64;
         size_t smem = (size_t)(KT_TP * dmax + M * dmax + M) * sizeof(float);
-  #define KSTAR_LAUNCH(ISO_, DM_)                                                                                   \
-    DMO_LAUNCH_ON(ps, (kstar_tensor_kernel<ISO_, DM_>), gk, KT_TN, smem, dXn, P, p_base, Pcpad, gp->Xt.p, N, d, M,    \
-                  gp->kernel, gp->inv_ls.p, gp->constant.p, gp->Kexp.p, Npad, kplane, Kh.p, Kl.p,                    \
-                  (use_flags && d_var) ? rdy : nullptr)
+        dim3 gk((unsigned)(Npad / (2 * KT_TN)), (unsigned)ceil_div(Pcpad, KT_TP));
+#define KSTAR_LAUNCH(ISO_, DM_)                                                                                          \
+  DMO_LAUNCH((kstar_tensor_kernel<ISO_, DM_>), gk, KT_TN, smem, dXn, P, p_base, Pcpad, gp->Xt.p, N, d, M, gp->kernel, \
+             gp->inv_ls.p, gp->constant.p, gp->Kexp.p, Npad, kplane, Kh.p, Kl.p)
         if (gp->isotropic) {
           if (d <= 32)
             KSTAR_LAUNCH(true, 32);
@@ -1229,75 +1121,27 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
           else
             KSTAR_LAUNCH(false, 64);
         }
-  #undef KSTAR_LAUNCH
+#undef KSTAR_LAUNCH
       }
-      if (overlap && (dbg & 4)) {  // diagnostics: the contraction waits for the whole K_* kernel by event, the mean still overlaps
-        DMO_CUDA(cudaEventRecord(ctx->ev_fork, ctx->aux));
-        DMO_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_fork, 0));
+      {
+        ProfileScope ps_(ctx, "gp_mean");
+        DMO_LAUNCH(mean_split_kernel, (unsigned)ceil_div(Pc * M * 32, 256), 256, 0, Kh.p, Kl.p, Pc, N, Npad, kplane, M,
+                   gp->Kexp.p, gp->alpha.p, gp->ymean.p, gp->ystd.p, p_base, d_mean);
       }
-      if (!(dbg & 8) && !mean_from_d) {
-        ProfileScope ps_(ctx, "gp_mean", ps);
-        DMO_LAUNCH_ON(ps, mean_split_kernel, (unsigned)ceil_div(Pc * M * 32, 256), 256, 0, Kh.p, Kl.p, Pc, N, Npad, kplane,
-                      M, gp->Kexp.p, gp->alpha.p, gp->ymean.p, gp->ystd.p, p_base, d_mean);
-      }
-}
-    if (overlap) DMO_CUDA(cudaEventRecord(ctx->ev_join, ctx->aux));
+    }
     if (d_var) {
-      GemmParams prm;
-      prm.M = M;
-      prm.n_pb = (int)(Pcpad / TMV);
-      prm.n_jt = n_jt;
-      prm.n_q = n_q;
-      prm.paired = version == 3;
-      // halves: split the row blocks where the cumulative MMA count sum_{j < J} (j + 1) is closest to half of the total
-      prm.j_split = n_jt;
-      if (!prm.paired) {
-        const int64_t tot = (int64_t)n_jt * (n_jt + 1) / 2;
-        int64_t best_d = tot;
-        for (int J = 0; J <= n_jt; ++J) {
-          const int64_t dlt = llabs(2 * ((int64_t)J * (J + 1) / 2) - tot);
-          if (dlt < best_d) {
-            best_d = dlt;
-            prm.j_split = J;
-          }
-        }
-      }
-      prm.k_rows = Pc_alloc;
-      prm.l_rows = Npad;
-      prm.inv_scale = gp->Lscale.p;
-      prm.vnorm = vnorm.p;
-      prm.vn_ld = Pc_alloc;
-      prm.abort_flag = abort_flag.p;
-      prm.zf = mean_from_d ? gp->Zf.p : nullptr;
-      prm.mnorm = mean_from_d ? mnorm.p : nullptr;
-      prm.ready = use_flags ? rdy : nullptr;
-      prm.dbg = dbg;
-      prm.ready_target = 8u * gk.x;  // KT_TP = 32 candidates per producer block: 8 tile rows x gk.x column blocks per 256
-      const int n_work = prm.M * prm.n_pb * prm.n_q;
-      const int grid = n_work < ctx->sm_count ? n_work : ctx->sm_count;
       {
         ProfileScope ps_(ctx, "gp_var");
-        DMO_LAUNCH(gp_var_wgmma_kernel, grid, NTHREADS, GEMM_SMEM, map_kh, map_kl, map_lh, map_ll, prm);
+        DMO_TRY(gp_var_contract_tensor(ctx, gp, Kh.p, Kl.p, M * Pc_alloc, Pc_alloc, Pcpad, vnorm.p, Pc_alloc, abort_flag.p));
       }
       DMO_LAUNCH(var_finish_tc_kernel, (unsigned)ceil_div(Pc * M, 256), 256, 0, vnorm.p, n_q, Pc, Pc_alloc, M,
                  gp->constant.p, gp->noise.p, gp->ystd.p, p_base, d_var);
-      if (mean_from_d)
-        DMO_LAUNCH(mean_finish_tc_kernel, (unsigned)ceil_div(Pc * M, 256), 256, 0, mnorm.p, n_q, Pc, Pc_alloc, M, gp->ymean.p,
-                   gp->ystd.p, p_base, d_mean);
-    }
-    if (overlap) DMO_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));  // mean (and K_*) of this chunk done
-    if ((dbg & 8) && !mean_from_d) {
-      ProfileScope ps_(ctx, "gp_mean");
-      DMO_LAUNCH(mean_split_kernel, (unsigned)ceil_div(Pc * M * 32, 256), 256, 0, Kh.p, Kl.p, Pc, N, Npad, kplane, M,
-                 gp->Kexp.p, gp->alpha.p, gp->ymean.p, gp->ystd.p, p_base, d_mean);
     }
   }
   DMO_CHECK_LAUNCH();
   int h_abort = 0;
   DMO_CUDA(cudaMemcpyAsync(&h_abort, abort_flag.p, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   DMO_CUDA(cudaStreamSynchronize(ctx->stream));
-  if (h_abort)
-    return dmo_fail(ctx, DMO_ERR_INTERNAL, "gp_predict(tensor): pipeline watchdog tripped (%s)",
-                    h_abort == 2 ? "K_* producer did not deliver" : "mbarrier wait timed out");
+  if (h_abort) return dmo_fail(ctx, DMO_ERR_INTERNAL, "gp_predict(tensor): pipeline watchdog tripped (mbarrier wait timed out)");
   return DMO_OK;
 }
