@@ -76,6 +76,7 @@ _SIGNATURES = {
     "dmo_mtgp_predict": (_c_int, [_vp, _vp, _vp, _c_i64, _vp, _vp, _c_int]),
     "dmo_mtgp_destroy": (_c_int, [_vp, _vp]),
     "dmo_mtgp_lml_grad": (_c_int, [_vp, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "dmo_gp_lml_grad": (_c_int, [_vp, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dmo_nsga2_step": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_i64, _c_int, _c_int, _c_dbl, _c_dbl, _c_dbl, _vp, _vp, _vp, _vp, _c_u64, _c_u64,
                                 _c_int, _c_int, _c_int, _c_int, _vp, _vp, _vp]),
     "dmo_hypervolume": (_c_int, [_vp, _vp, _c_i64, _c_int, _vp, ctypes.POINTER(_c_dbl)]),
@@ -699,6 +700,27 @@ def mtgp_lml_grad(X_train, Y, length_scale, B, D, weight, bias):
                                             _ptr(lml), _ptr(g["length_scale"]), _ptr(g["B"]), _ptr(g["D"]), _ptr(g["weight"]),
                                             _ptr(g["bias"])), "dmo_mtgp_lml_grad")
     return float(lml[0]), g
+
+
+def gp_lml_grad(X_train, Y, length_scale, outputscale, noise, weight, bias):
+    """(lml (M,), grads) of M independent exact GPs, K_m = s_m Matern52(X / l_m) + noise_m I with the linear prior mean
+    X w_m + b_m (dmo_gp_lml_grad): lml_m = log p(y_m), grads a dict of d lml_m / d {length_scale (M,d), outputscale (M,),
+    noise (M,), weight (M,d), bias (M,)}.  X_train (N,d) normalised inputs, Y (N,M) normalised targets."""
+    X_train, Y = _f64(X_train), _f64(Y)
+    N, d = X_train.shape
+    if Y.ndim == 1:
+        Y = Y.reshape(-1, 1)
+    M = Y.shape[1]
+    assert Y.shape == (N, M), Y.shape
+    yt = _f64(Y.T)
+    ls, w = _f64(length_scale).reshape(M, d), _f64(weight).reshape(M, d)
+    s, nz, b = _f64(outputscale).reshape(M), _f64(noise).reshape(M), _f64(bias).reshape(M)
+    lml = np.empty(M)
+    g = {"length_scale": np.empty((M, d)), "outputscale": np.empty(M), "noise": np.empty(M), "weight": np.empty((M, d)), "bias": np.empty(M)}
+    _check(load_library().dmo_gp_lml_grad(context(), N, d, M, _ptr(X_train), _ptr(yt), _ptr(ls), _ptr(s), _ptr(nz), _ptr(w), _ptr(b),
+                                          _ptr(lml), _ptr(g["length_scale"]), _ptr(g["outputscale"]), _ptr(g["noise"]), _ptr(g["weight"]),
+                                          _ptr(g["bias"])), "dmo_gp_lml_grad")
+    return lml, g
 
 
 # --------------------------------------------------------------------------- A18

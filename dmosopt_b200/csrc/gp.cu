@@ -16,19 +16,25 @@ namespace {
 // ---- L^-1 (once per epoch, not on the per-generation path): blocked recursive inversion
 //   inv([A 0; C B]) = [A^-1 0; -B^-1 C A^-1, B^-1].  The 128 x 128 diagonal blocks are inverted by forward substitution
 //   (one thread per column), then log2(N/128) levels of batched float64 GEMMs double the inverted block size.
-//   The matrix is embedded in a power-of-two multiple of 128 with an identity tail.
+//   The matrix is embedded in a power-of-two multiple of 128 with an identity tail.  Batched over independent factors:
+//   factor b is blockIdx.y of the embed / diagonal / extract kernels and folds into blockIdx.z of the GEMMs.
 constexpr int TRI_B = 128;
 
-__global__ void tri_embed_kernel(const double* __restrict__ L, int64_t N, int64_t Np, double* __restrict__ Lp) {
+__global__ void tri_embed_kernel(const double* __restrict__ L, int64_t ldl, int64_t sL, int64_t N, int64_t Np,
+                                 double* __restrict__ Lp) {
   int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= Np * Np) return;
+  L += (size_t)blockIdx.y * sL;
+  Lp += (size_t)blockIdx.y * Np * Np;
   int64_t r = t / Np, c = t - r * Np;
-  Lp[t] = (r < N && c < N) ? (c <= r ? L[r * N + c] : 0.0) : (r == c ? 1.0 : 0.0);
+  Lp[t] = (r < N && c < N) ? (c <= r ? L[r * ldl + c] : 0.0) : (r == c ? 1.0 : 0.0);
 }
 
 // one CTA per diagonal block, one thread per column of the block (L entries are warp-uniform loads, X column-coalesced)
 __global__ void __launch_bounds__(TRI_B) tri_diag_inverse_kernel(const double* __restrict__ Lp, int64_t Np,
                                                                  double* __restrict__ X) {
+  Lp += (size_t)blockIdx.y * Np * Np;
+  X += (size_t)blockIdx.y * Np * Np;
   const int64_t base = (int64_t)blockIdx.x * TRI_B;
   const int c = threadIdx.x;
   const double* Lb = Lp + base * Np + base;
@@ -45,16 +51,27 @@ __global__ void __launch_bounds__(TRI_B) tri_diag_inverse_kernel(const double* _
   }
 }
 
-// C = alpha * A * B, all row-major, batched over blockIdx.z; 64 x 64 tile, 16-wide k step, 256 threads x (4 x 4)
+// C = alpha * A * B, all row-major, batched over blockIdx.z: operand X of batch entry z starts at X + z * sX; with
+// FACTORS, z = q * zper + z' over several factors q, and X of entry (q, z') starts at X + z' * sX + q * bX.
+// 64 x 64 tile, 16-wide k step, 256 threads x (4 x 4)
+template <bool FACTORS>
 __global__ void __launch_bounds__(256) gemm_nn_f64_kernel(const double* __restrict__ A, int64_t lda, int64_t sA,
                                                           const double* __restrict__ B, int64_t ldb, int64_t sB,
                                                           double* __restrict__ C, int64_t ldc, int64_t sC, int64_t Msz,
-                                                          int64_t Nsz, int64_t Ksz, double alpha) {
+                                                          int64_t Nsz, int64_t Ksz, double alpha, int zper, int64_t bA,
+                                                          int64_t bB, int64_t bC) {
   __shared__ double As[16][64 + 1];
   __shared__ double Bs[16][64 + 1];
-  A += (int64_t)blockIdx.z * sA;
-  B += (int64_t)blockIdx.z * sB;
-  C += (int64_t)blockIdx.z * sC;
+  if constexpr (FACTORS) {
+    const int64_t zq = (int64_t)(blockIdx.z / zper), zz = (int64_t)(blockIdx.z - zq * zper);
+    A += zz * sA + zq * bA;
+    B += zz * sB + zq * bB;
+    C += zz * sC + zq * bC;
+  } else {
+    A += (int64_t)blockIdx.z * sA;
+    B += (int64_t)blockIdx.z * sB;
+    C += (int64_t)blockIdx.z * sC;
+  }
   const int64_t m0 = (int64_t)blockIdx.y * 64, n0 = (int64_t)blockIdx.x * 64;
   const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
   double acc[4][4] = {};
@@ -89,10 +106,12 @@ __global__ void __launch_bounds__(256) gemm_nn_f64_kernel(const double* __restri
   (void)Nsz;
 }
 
-__global__ void tri_extract_kernel(const double* __restrict__ X, int64_t Np, int64_t N, int64_t ldo,
+__global__ void tri_extract_kernel(const double* __restrict__ X, int64_t Np, int64_t N, int64_t ldo, int64_t sout,
                                    double* __restrict__ out) {
   int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= N * N) return;
+  X += (size_t)blockIdx.y * Np * Np;
+  out += (size_t)blockIdx.y * sout;
   int64_t r = t / N, c = t - r * N;
   out[r * ldo + c] = (c <= r) ? X[r * Np + c] : 0.0;
 }
@@ -329,29 +348,37 @@ __global__ void var_finish_kernel(const double* __restrict__ vnorm, int nplanes,
 
 }  // namespace
 
-int gp_linv_from_factor(dmo_ctx* ctx, const double* L, int64_t N, int64_t ldo, double* dst) {
+int gp_linv_from_factor_batched(dmo_ctx* ctx, const double* L, int64_t ldl, int64_t sL, int64_t N, int nbat, int64_t ldo,
+                                int64_t sdst, double* dst) {
   int64_t Np = TRI_B;
   while (Np < N) Np *= 2;
+  const int64_t np2 = Np * Np;
   DevBuf<double> Lp, X, T;
-  DMO_TRY(Lp.alloc(ctx, (size_t)Np * Np));
-  DMO_TRY(X.alloc(ctx, (size_t)Np * Np));
-  DMO_TRY(T.alloc(ctx, (size_t)Np * Np / 2));
-  DMO_CUDA(cudaMemsetAsync(X.p, 0, (size_t)Np * Np * sizeof(double), ctx->stream));
-  DMO_LAUNCH(tri_embed_kernel, (unsigned)ceil_div(Np * Np, 256), 256, 0, L, N, Np, Lp.p);
-  DMO_LAUNCH(tri_diag_inverse_kernel, (unsigned)(Np / TRI_B), TRI_B, 0, Lp.p, Np, X.p);
+  DMO_TRY(Lp.alloc(ctx, (size_t)nbat * np2));
+  DMO_TRY(X.alloc(ctx, (size_t)nbat * np2));
+  DMO_TRY(T.alloc(ctx, (size_t)nbat * np2 / 2));
+  DMO_CUDA(cudaMemsetAsync(X.p, 0, (size_t)nbat * np2 * sizeof(double), ctx->stream));
+  DMO_LAUNCH(tri_embed_kernel, dim3((unsigned)ceil_div(np2, 256), (unsigned)nbat), 256, 0, L, ldl, sL, N, Np, Lp.p);
+  DMO_LAUNCH(tri_diag_inverse_kernel, dim3((unsigned)(Np / TRI_B), (unsigned)nbat), TRI_B, 0, Lp.p, Np, X.p);
   for (int64_t sz = TRI_B; sz < Np; sz *= 2) {
     const int64_t pairs = Np / (2 * sz);
     const int64_t stride = 2 * sz * Np + 2 * sz;  // next diagonal 2s x 2s block
-    dim3 grid((unsigned)(sz / 64), (unsigned)(sz / 64), (unsigned)pairs);
+    dim3 grid((unsigned)(sz / 64), (unsigned)(sz / 64), (unsigned)(pairs * nbat));
     // T = C * A^-1        (C = Lp[s:2s, 0:s], A^-1 = X[0:s, 0:s])
-    DMO_LAUNCH(gemm_nn_f64_kernel, grid, 256, 0, Lp.p + sz * Np, Np, stride, X.p, Np, stride, T.p, sz, sz * sz, sz, sz,
-               sz, 1.0);
+    auto gemm = nbat == 1 ? gemm_nn_f64_kernel<false> : gemm_nn_f64_kernel<true>;  // one factor: no factor offsets
+    DMO_LAUNCH(gemm, grid, 256, 0, Lp.p + sz * Np, Np, stride, X.p, Np, stride, T.p, sz, sz * sz, sz, sz, sz, 1.0, (int)pairs, np2,
+               np2, np2 / 2);
     // X[s:2s, 0:s] = -B^-1 * T   (B^-1 = X[s:2s, s:2s])
-    DMO_LAUNCH(gemm_nn_f64_kernel, grid, 256, 0, X.p + sz * Np + sz, Np, stride, T.p, sz, sz * sz, X.p + sz * Np, Np,
-               stride, sz, sz, sz, -1.0);
+    DMO_LAUNCH(gemm, grid, 256, 0, X.p + sz * Np + sz, Np, stride, T.p, sz, sz * sz, X.p + sz * Np, Np, stride, sz, sz, sz, -1.0,
+               (int)pairs, np2, np2 / 2, np2);
   }
-  DMO_LAUNCH(tri_extract_kernel, (unsigned)ceil_div(N * N, 256), 256, 0, X.p, Np, N, ldo, dst);
+  DMO_LAUNCH(tri_extract_kernel, dim3((unsigned)ceil_div(N * N, 256), (unsigned)nbat), 256, 0, X.p, Np, N, ldo, sdst, dst);
   DMO_CUDA(cudaGetLastError());
+  return DMO_OK;
+}
+
+int gp_linv_from_factor(dmo_ctx* ctx, const double* L, int64_t N, int64_t ldo, double* dst) {
+  DMO_TRY(gp_linv_from_factor_batched(ctx, L, N, 0, N, 1, ldo, 0, dst));
   DMO_CUDA(cudaStreamSynchronize(ctx->stream));
   return DMO_OK;
 }

@@ -42,6 +42,13 @@ int gp_predict_fp64(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, doub
 // Building blocks shared with the multitask posterior (gp_multitask.cu).  All pointers are device pointers.
 // L^-1 of the lower Cholesky factor L (N, N) into dst (rows of ldo doubles, lower triangle; the rest is left untouched)
 int gp_linv_from_factor(dmo_ctx* ctx, const double* L, int64_t N, int64_t ldo, double* dst);
+// the same for nbat factors L + b * sL (rows of ldl doubles) into dst + b * sdst, in one pass; not synchronised.  Scratch:
+// 2.5 nbat Np^2 doubles, Np the power of two >= max(N, 128)
+int gp_linv_from_factor_batched(dmo_ctx* ctx, const double* L, int64_t ldl, int64_t sL, int64_t N, int nbat, int64_t ldo,
+                                int64_t sdst, double* dst);
+// nbat independent exact-GP factorisations in one pass of the blocked Cholesky (gp_fit.cu; see its definition)
+int gp_fit_batched(dmo_ctx* ctx, int64_t N, int d, int nbat, int kernel, const double* X, const double* inv_ls, const double* constant,
+                   const double* diag_add, const double* y, double* A, int64_t ld, int* info, double* work, double* alpha, double* lml);
 // float64 variance contraction (var_kernel): vnorm[z][m][p] = partial sums over the row blocks z (mod nsplit) of
 // ||Linv_m Ks_m[p]||^2, Ks_m = Ks + m * kplane with rows of gp->Npad doubles (kplane = 0: one K_* plane for every m);
 // Pcpad is a multiple of GP_F64_TILE

@@ -13,7 +13,7 @@
 // likelihood need no separate forward solve; alpha = L^-T z is one backward sweep (one CTA, only when alpha is wanted).
 #include <math_constants.h>
 
-#include "common.cuh"
+#include "gp.cuh"
 
 namespace {
 
@@ -29,11 +29,18 @@ __device__ __forceinline__ double stationary_fit(double s2, int kind) {
 
 // lower triangle (and diagonal) of K, row-major with leading dimension ld; the strict upper triangle is zeroed.
 // One CTA per 32 x 32 tile of K: the 64 rows of X it needs are staged in shared memory once (scaled by 1 / l), tiles
-// strictly above the diagonal only write zeros.
+// strictly above the diagonal only write zeros.  Batched over blockIdx.z: problem b has its own inv_ls (d), constant,
+// diag_add, targets y (N) and matrix K + b * sK; X is shared.
 __global__ void __launch_bounds__(256) kernel_matrix_kernel(const double* __restrict__ X, int64_t N, int d, int kind,
-                                                            const double* __restrict__ inv_ls, double constant, double diag_add,
-                                                            const double* __restrict__ y, int64_t ld, double* __restrict__ K) {
+                                                            const double* __restrict__ inv_ls, const double* __restrict__ constant_b,
+                                                            const double* __restrict__ diag_add_b, const double* __restrict__ y,
+                                                            int64_t ld, double* __restrict__ K, int64_t sK) {
   extern __shared__ double xs[];  // [64][d + 1]: rows i0 .. i0+31 then j0 .. j0+31 of X, scaled
+  const int bz = blockIdx.z;
+  inv_ls += (size_t)bz * d;
+  y += (size_t)bz * N;
+  K += (size_t)bz * sK;
+  const double constant = constant_b[bz], diag_add = diag_add_b[bz];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;  // 32 x 8
   const int64_t i0 = (int64_t)blockIdx.y * 32, j0 = (int64_t)blockIdx.x * 32;
   const int dp = d + 1;
@@ -74,7 +81,12 @@ __global__ void __launch_bounds__(256) kernel_matrix_kernel(const double* __rest
 }
 
 // ---- Cholesky steps (A: lower triangle, in place, leading dimension ld, ld % CB == 0) ----------------------------------
-__global__ void __launch_bounds__(256) potrf_diag_kernel(double* __restrict__ A, int64_t ld, int64_t k0, int* __restrict__ info) {
+// Every step is batched over independent matrices A + b * sA (b: blockIdx.x of potrf_diag_kernel, blockIdx.y of the panel
+// and trailing-update kernels); a CTA never mixes matrices, so each one's arithmetic is the same however many run.
+__global__ void __launch_bounds__(256) potrf_diag_kernel(double* __restrict__ A, int64_t ld, int64_t sA, int64_t k0,
+                                                         int* __restrict__ info) {
+  A += (size_t)blockIdx.x * sA;
+  info += blockIdx.x;
   // Thread (w, c) = (tid >> 6, tid & 63) keeps the 16 elements (r = w + 4 u, c) of the block in registers for the whole
   // factorisation.  Column j: its four owner threads publish the (unscaled) column to shared memory, one barrier, then every
   // thread scales what it needs itself (L_rj = a_rj / sqrt(a_jj)) and updates its own elements -- 16 independent FMAs per
@@ -125,8 +137,9 @@ __global__ void __launch_bounds__(256) potrf_diag_kernel(double* __restrict__ A,
 // A_ik <- A_ik L_kk^-T for the block rows below the diagonal block: thread r owns row r of the 64 x 64 block
 constexpr size_t PAIR_SMEM = (size_t)2 * CB * (CB + 1) * sizeof(double);  // two padded 64 x 64 blocks: above the 48 KB static limit
 
-__global__ void __launch_bounds__(CB) trsm_panel_kernel(double* __restrict__ A, int64_t ld, int64_t k0) {
+__global__ void __launch_bounds__(CB) trsm_panel_kernel(double* __restrict__ A, int64_t ld, int64_t sA, int64_t k0) {
   extern __shared__ double dyn_sm[];
+  A += (size_t)blockIdx.y * sA;
   double (*l)[CB + 1] = reinterpret_cast<double (*)[CB + 1]>(dyn_sm);
   double (*x)[CB + 1] = reinterpret_cast<double (*)[CB + 1]>(dyn_sm + CB * (CB + 1));
   __shared__ double linv[CB];
@@ -162,8 +175,9 @@ __global__ void __launch_bounds__(CB) trsm_panel_kernel(double* __restrict__ A, 
 }
 
 // A_ij -= A_ik A_jk' for the tiles i >= j > k of the lower triangle; 256 threads, 4 x 4 outputs each
-__global__ void __launch_bounds__(256) syrk_tile_kernel(double* __restrict__ A, int64_t ld, int64_t k0, int nrem) {
+__global__ void __launch_bounds__(256) syrk_tile_kernel(double* __restrict__ A, int64_t ld, int64_t sA, int64_t k0, int nrem) {
   extern __shared__ double dyn_sm[];
+  A += (size_t)blockIdx.y * sA;
   double (*sa)[CB + 1] = reinterpret_cast<double (*)[CB + 1]>(dyn_sm);                  // A_ik  [row][kk]
   double (*sb)[CB + 1] = reinterpret_cast<double (*)[CB + 1]>(dyn_sm + CB * (CB + 1));  // A_jk  [row][kk]
   // tile index -> (ti, tj) with ti >= tj, both in [0, nrem)
@@ -204,10 +218,16 @@ __global__ void __launch_bounds__(256) syrk_tile_kernel(double* __restrict__ A, 
     }
 }
 
-// ---- log marginal likelihood from the augmented row, alpha = L^-T z by one backward sweep: one CTA ----------------------------
+// ---- log marginal likelihood from the augmented row, alpha = L^-T z by one backward sweep: one CTA per factor ---------------
+// (factor b: L + b * sL, work + b * ld, alpha + b * N, lml + b)
 constexpr int SV_T = 1024;
-__global__ void __launch_bounds__(SV_T) finish_fit_kernel(const double* __restrict__ L, int64_t ld, int64_t N, double* __restrict__ work,
-                                                          double* __restrict__ alpha, double* __restrict__ lml, int want_alpha) {
+__global__ void __launch_bounds__(SV_T) finish_fit_kernel(const double* __restrict__ L, int64_t ld, int64_t sL, int64_t N,
+                                                          double* __restrict__ work, double* __restrict__ alpha, double* __restrict__ lml,
+                                                          int want_alpha) {
+  L += (size_t)blockIdx.x * sL;
+  work += (size_t)blockIdx.x * ld;
+  alpha += (size_t)blockIdx.x * N;
+  lml += blockIdx.x;
   __shared__ double xs[CB];
   __shared__ double red[SV_T / 32];
   __shared__ double dl[CB][CB + 1];  // the current diagonal block of L
@@ -286,6 +306,31 @@ __global__ void extract_lower_kernel(const double* __restrict__ A, int64_t ld, i
 
 }  // namespace
 
+// nbat independent problems in one pass: problem b factors [K_b y_b; y_b' big] in A + b * ld^2 (ld = ceil((N + 1) / 64) * 64)
+// with K_b = constant[b] k(X / l_b, X / l_b) + diag_add[b] I (inv_ls: (nbat, d)); info[b] (zeroed by the caller) receives a non-positive pivot + 1.
+// lml (may be NULL: no finish) receives log p(y_b), alpha (may be NULL) K_b^-1 y_b, rows of N; work holds nbat * ld doubles.
+// All pointers are device pointers; nothing is synchronised.
+int gp_fit_batched(dmo_ctx* ctx, int64_t N, int d, int nbat, int kernel, const double* X, const double* inv_ls, const double* constant,
+                   const double* diag_add, const double* y, double* A, int64_t ld, int* info, double* work, double* alpha, double* lml) {
+  const int64_t nb = ld / CB, sA = ld * ld;
+  DMO_CUDA(cudaFuncSetAttribute(trsm_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PAIR_SMEM));
+  DMO_CUDA(cudaFuncSetAttribute(syrk_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PAIR_SMEM));
+  dim3 kg((unsigned)ceil_div(ld, 32), (unsigned)ceil_div(ld, 32), (unsigned)nbat);
+  DMO_LAUNCH(kernel_matrix_kernel, kg, 256, (size_t)64 * (d + 1) * sizeof(double), X, N, d, kernel, inv_ls, constant, diag_add, y, ld,
+             A, sA);
+  for (int64_t k = 0; k < nb; ++k) {
+    const int64_t k0 = k * CB;
+    DMO_LAUNCH(potrf_diag_kernel, (unsigned)nbat, 256, 0, A, ld, sA, k0, info);
+    const int nrem = (int)(nb - k - 1);
+    if (nrem > 0) {
+      DMO_LAUNCH(trsm_panel_kernel, dim3((unsigned)nrem, (unsigned)nbat), CB, PAIR_SMEM, A, ld, sA, k0);
+      DMO_LAUNCH(syrk_tile_kernel, dim3((unsigned)((int64_t)nrem * (nrem + 1) / 2), (unsigned)nbat), 256, PAIR_SMEM, A, ld, sA, k0, nrem);
+    }
+  }
+  if (lml) DMO_LAUNCH(finish_fit_kernel, (unsigned)nbat, SV_T, 0, A, ld, sA, N, work, alpha, lml, alpha ? 1 : 0);
+  return DMO_OK;
+}
+
 extern "C" {
 
 int dmo_gp_fit(dmo_ctx* ctx, int64_t N, int d, int M, int kernel, const double* X_train, const double* y, const double* constant,
@@ -295,11 +340,12 @@ int dmo_gp_fit(dmo_ctx* ctx, int64_t N, int d, int M, int kernel, const double* 
   DMO_REQUIRE(N >= 1 && d >= 1 && d <= 90 && M >= 1 && X_train && y && constant && length_scale && noise, "gp_fit: bad arguments");
   DMO_REQUIRE(kernel == DMO_KERNEL_MATERN52 || kernel == DMO_KERNEL_RBF, "gp_fit: unknown kernel %d", kernel);
   DMO_REQUIRE(alpha_out || lml_out || L_out, "gp_fit: nothing to compute");
-  std::vector<double> h_c(M), h_n(M), h_ls((size_t)M * d), h_inv((size_t)M * d);
+  std::vector<double> h_c(M), h_n(M), h_ls((size_t)M * d), h_inv((size_t)M * d), h_dadd(M);
   DMO_CUDA(cudaMemcpy(h_c.data(), constant, M * sizeof(double), cudaMemcpyDefault));
   DMO_CUDA(cudaMemcpy(h_n.data(), noise, M * sizeof(double), cudaMemcpyDefault));
   DMO_CUDA(cudaMemcpy(h_ls.data(), length_scale, (size_t)M * d * sizeof(double), cudaMemcpyDefault));
   for (size_t t = 0; t < h_ls.size(); ++t) h_inv[t] = 1.0 / h_ls[t];
+  for (int m = 0; m < M; ++m) h_dadd[m] = h_n[m] + jitter;
   const int64_t nb = ceil_div(N + 1, CB), ld = nb * CB;  // N rows of K + the row that carries the targets
   In<double> ix, iy;
   DMO_TRY(ix.init(ctx, X_train, (size_t)N * d));
@@ -308,34 +354,25 @@ int dmo_gp_fit(dmo_ctx* ctx, int64_t N, int d, int M, int kernel, const double* 
   DMO_TRY(oL.init(ctx, L_out, L_out ? (size_t)M * N * N : 0));
   DMO_TRY(oa.init(ctx, alpha_out, alpha_out ? (size_t)M * N : 0));
   DMO_TRY(ol.init(ctx, lml_out, lml_out ? (size_t)M : 0));
-  DevBuf<double> A, inv_ls, work, alpha_d, lml_d;
+  DevBuf<double> A, inv_ls, cd, work, alpha_d, lml_d;
   DevBuf<int> info;
   DMO_TRY(A.alloc(ctx, (size_t)ld * ld));
   DMO_TRY(inv_ls.alloc(ctx, (size_t)M * d));
+  DMO_TRY(cd.alloc(ctx, (size_t)2 * M));
   DMO_TRY(work.alloc(ctx, (size_t)ld));
   DMO_TRY(alpha_d.alloc(ctx, (size_t)N));
   DMO_TRY(lml_d.alloc(ctx, 1));
   DMO_TRY(info.alloc(ctx, 1));
   DMO_CUDA(cudaMemcpyAsync(inv_ls.p, h_inv.data(), h_inv.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  DMO_CUDA(cudaMemcpyAsync(cd.p, h_c.data(), M * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  DMO_CUDA(cudaMemcpyAsync(cd.p + M, h_dadd.data(), M * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
   DMO_CUDA(cudaMemsetAsync(info.p, 0, sizeof(int), ctx->stream));
-  DMO_CUDA(cudaFuncSetAttribute(trsm_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PAIR_SMEM));
-  DMO_CUDA(cudaFuncSetAttribute(syrk_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PAIR_SMEM));
   ProfileScope ps(ctx, "gp_fit");
   for (int m = 0; m < M; ++m) {
-    dim3 kg((unsigned)ceil_div(ld, 32), (unsigned)ceil_div(ld, 32));
-    DMO_LAUNCH(kernel_matrix_kernel, kg, 256, (size_t)64 * (d + 1) * sizeof(double), ix.d, N, d, kernel, inv_ls.p + (size_t)m * d, h_c[m],
-               h_n[m] + jitter, iy.d + (size_t)m * N, ld, A.p);
-    for (int64_t k = 0; k < nb; ++k) {
-      const int64_t k0 = k * CB;
-      DMO_LAUNCH(potrf_diag_kernel, 1, 256, 0, A.p, ld, k0, info.p);
-      const int nrem = (int)(nb - k - 1);
-      if (nrem > 0) {
-        DMO_LAUNCH(trsm_panel_kernel, (unsigned)nrem, CB, PAIR_SMEM, A.p, ld, k0);
-        DMO_LAUNCH(syrk_tile_kernel, (unsigned)((int64_t)nrem * (nrem + 1) / 2), 256, PAIR_SMEM, A.p, ld, k0, nrem);
-      }
-    }
+    // one objective at a time (a batch of one), sharing the scratch matrix
+    DMO_TRY(gp_fit_batched(ctx, N, d, 1, kernel, ix.d, inv_ls.p + (size_t)m * d, cd.p + m, cd.p + M + m, iy.d + (size_t)m * N, A.p, ld,
+                           info.p, work.p, oa.d ? alpha_d.p : nullptr, (oa.d || ol.d) ? lml_d.p : nullptr));
     if (oa.d || ol.d) {
-      DMO_LAUNCH(finish_fit_kernel, 1, SV_T, 0, A.p, ld, N, work.p, alpha_d.p, lml_d.p, oa.d ? 1 : 0);
       if (oa.d) DMO_CUDA(cudaMemcpyAsync(oa.d + (size_t)m * N, alpha_d.p, (size_t)N * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
       if (ol.d) DMO_CUDA(cudaMemcpyAsync(ol.d + m, lml_d.p, sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
     }

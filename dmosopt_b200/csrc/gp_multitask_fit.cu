@@ -19,6 +19,14 @@
 //     terms alpha_.s' K_x alpha_.t.
 //   Both write one partial per tile and target; mt_fold_kernel adds them in tile order.  No atomics: deterministic.
 // The rest (alpha from a_j, X' alpha, 1' alpha, the final combinations) is O(N M (M + d)) host arithmetic.
+//
+// Both kernels and the fold (their MODELS = true instances) also take a model index (blockIdx.y) over independent
+// models with their own scaled inputs, L^-1 blocks, S, alpha, B alpha and partials; the MODELS = false instances, which
+// dmo_mtgp_lml_grad launches, are the one-model kernels without those offsets.  dmo_gp_lml_grad uses the index for EGP_Matern's M independent GPs
+// K_m = s_m K_x(X / l_m) + sigma2_m I, each a model with one block: lambda = s_m and "B" = s_m, with L^-1 the inverse
+// factor of K_m itself, so S = s_m K_m^-1, W = s_m (alpha alpha' - K_m^-1), and the traces tr(K_x K_m^-1), tr(K_m^-1)
+// come from the unscaled accumulators.  Every CTA works on one model and every sum runs in a fixed order, so a model's
+// outputs do not depend on which other models share the launch.
 #include <math.h>
 
 #include <vector>
@@ -54,11 +62,20 @@ __device__ __forceinline__ double block_sum256(double v, double* red) {
 // part[tile][j] = sum_{i,i'} K_x(i,i') A_j^-1(i,i') over the tile's lower triangle (twice off the diagonal) and
 // part[tile][M + j] = its diagonal part of tr(A_j^-1).  Linv: (M, ld, ld), zero above the diagonal and in the padding;
 // A_j^-1(i,i') = sum_{k >= max(i,i')} Linv_j(k,i) Linv_j(k,i'), so the k loop starts at the tile's first row.
+template <bool MODELS>  // false: one model (MEGP), the kernel without the model offsets
 __global__ void __launch_bounds__(256) mt_ainv_syrk_kernel(const double* __restrict__ Linv, int64_t ld, int64_t N, int M,
                                                            const double* __restrict__ lam, const double* __restrict__ xs, int d,
                                                            double* __restrict__ S, double* __restrict__ part) {
   __shared__ double sa[GT * XP], sb[GT * XP];  // [KC][GT] rows of L^-1, or [GT][XP] coordinate slices
   __shared__ double red[8];
+  if constexpr (MODELS) {
+    const size_t mdl = blockIdx.y;  // model index
+    Linv += mdl * M * ld * ld;
+    lam += mdl * M;
+    xs += mdl * N * d;
+    S += mdl * ld * ld;
+    part += mdl * gridDim.x * 2 * M;
+  }
   int ti, tj;
   tile_of(blockIdx.x, ti, tj);
   const int64_t i0 = (int64_t)ti * GT, j0 = (int64_t)tj * GT;
@@ -169,6 +186,7 @@ __global__ void __launch_bounds__(256) mt_ainv_syrk_kernel(const double* __restr
 // target, lanes over i'): part[tile][k] = sum f (x_ik / l_k - x_i'k / l_k)^2 for k < d, and for the pairs s <= t
 // part[tile][d + p(s,t)] = sum kw (alpha_is alpha_i't + alpha_it alpha_i's).  Summed over the tiles:
 // d lml / d l_k = part_k / l_k, alpha_.s' K_x alpha_.t = part_{d + p(s,t)}.
+template <bool MODELS>
 __global__ void __launch_bounds__(256) mt_grad_pass_kernel(const double* __restrict__ xs, int64_t N, int d, int M,
                                                            const double* __restrict__ S, int64_t ld, const double* __restrict__ al,
                                                            const double* __restrict__ bal, double* __restrict__ part, int nq) {
@@ -181,6 +199,14 @@ __global__ void __launch_bounds__(256) mt_grad_pass_kernel(const double* __restr
   double* ai = kw + GT * (GT + 1);  // [GT][M] alpha rows of tile ti
   double* aj = ai + GT * M;         // [GT][M] alpha rows of tile tj
   double* bj = aj + GT * M;         // [GT][M] (B alpha) rows of tile tj
+  if constexpr (MODELS) {
+    const size_t mdl = blockIdx.y;  // model index
+    xs += mdl * N * d;
+    S += mdl * ld * ld;
+    al += mdl * N * M;
+    bal += mdl * N * M;
+    part += mdl * gridDim.x * nq;
+  }
   int ti, tj;
   tile_of(blockIdx.x, ti, tj);
   const int64_t i0 = (int64_t)ti * GT, j0 = (int64_t)tj * GT;
@@ -255,10 +281,16 @@ __global__ void __launch_bounds__(256) mt_grad_pass_kernel(const double* __restr
   }
 }
 
-// out[q] = sum over tiles, in tile order, of part[tile][q]
+// out[q] = sum over tiles, in tile order, of part[tile][q]; with MODELS, model blockIdx.y: part + y * n_tiles * nq,
+// out + y * nq
+template <bool MODELS>
 __global__ void mt_fold_kernel(const double* __restrict__ part, int n_tiles, int nq, double* __restrict__ out) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= nq) return;
+  if constexpr (MODELS) {
+    part += (size_t)blockIdx.y * n_tiles * nq;
+    out += (size_t)blockIdx.y * nq;
+  }
   double s = 0.0;
   for (int t = 0; t < n_tiles; ++t) s += part[(size_t)t * nq + q];
   out[q] = s;
@@ -322,16 +354,16 @@ int dmo_mtgp_lml_grad(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_tra
   DMO_CUDA(cudaMemcpyAsync(bal_d.p, bal.data(), (size_t)N * M * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
   {
     ProfileScope ps(ctx, "mtgp_lg_ainv");
-    DMO_LAUNCH(mt_ainv_syrk_kernel, (unsigned)n_tiles, 256, 0, Linv.p, Npad, N, M, lam_d.p, xs_d.p, d, S.p, part_a.p);
-    DMO_LAUNCH(mt_fold_kernel, 1, 64, 0, part_a.p, n_tiles, 2 * M, red.p);
+    DMO_LAUNCH(mt_ainv_syrk_kernel<false>, (unsigned)n_tiles, 256, 0, Linv.p, Npad, N, M, lam_d.p, xs_d.p, d, S.p, part_a.p);
+    DMO_LAUNCH(mt_fold_kernel<false>, 1, 64, 0, part_a.p, n_tiles, 2 * M, red.p);
   }
   Linv.release();
   {
     ProfileScope ps(ctx, "mtgp_lg_grad");
     const size_t smem = ((size_t)2 * GT * (d + 1) + (size_t)2 * GT * (GT + 1) + (size_t)3 * GT * M) * sizeof(double);
-    DMO_CUDA(cudaFuncSetAttribute(mt_grad_pass_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    DMO_LAUNCH(mt_grad_pass_kernel, (unsigned)n_tiles, 256, smem, xs_d.p, N, d, M, S.p, Npad, al_d.p, bal_d.p, part_g.p, nq);
-    DMO_LAUNCH(mt_fold_kernel, (unsigned)ceil_div(nq, 128), 128, 0, part_g.p, n_tiles, nq, red.p + 2 * M);
+    DMO_CUDA(cudaFuncSetAttribute(mt_grad_pass_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    DMO_LAUNCH(mt_grad_pass_kernel<false>, (unsigned)n_tiles, 256, smem, xs_d.p, N, d, M, S.p, Npad, al_d.p, bal_d.p, part_g.p, nq);
+    DMO_LAUNCH(mt_fold_kernel<false>, (unsigned)ceil_div(nq, 128), 128, 0, part_g.p, n_tiles, nq, red.p + 2 * M);
   }
   DMO_CHECK_LAUNCH();
   std::vector<double> hr((size_t)2 * M + nq);
@@ -369,6 +401,148 @@ int dmo_mtgp_lml_grad(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_tra
   DMO_CUDA(cudaMemcpy(g_B, gB.data(), (size_t)M * M * sizeof(double), cudaMemcpyDefault));
   DMO_CUDA(cudaMemcpy(g_D, gD.data(), M * sizeof(double), cudaMemcpyDefault));
   DMO_CUDA(cudaMemcpy(g_weight, gw.data(), (size_t)M * d * sizeof(double), cudaMemcpyDefault));
+  DMO_CUDA(cudaMemcpy(g_bias, gb.data(), M * sizeof(double), cudaMemcpyDefault));
+  return DMO_OK;
+}
+
+
+int dmo_gp_lml_grad(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_train, const double* y, const double* length_scale,
+                    const double* outputscale, const double* noise, const double* weight, const double* bias, double* lml_out,
+                    double* g_length_scale, double* g_outputscale, double* g_noise, double* g_weight, double* g_bias) {
+  if (!ctx) return DMO_ERR_ARG;
+  DMO_CUDA(cudaSetDevice(ctx->device));
+  DMO_REQUIRE(N >= 1 && d >= 1 && d <= MT_FIT_DMAX && M >= 1 && M <= MT_MAX,
+              "gp_lml_grad: unsupported shape N=%lld d=%d M=%d (1 <= M <= %d, d <= %d)", (long long)N, d, M, MT_MAX, MT_FIT_DMAX);
+  DMO_REQUIRE(X_train && y && length_scale && outputscale && noise && weight && bias, "gp_lml_grad: null pointer");
+  DMO_REQUIRE(lml_out && g_length_scale && g_outputscale && g_noise && g_weight && g_bias, "gp_lml_grad: null output");
+  const size_t nd = (size_t)N * d, mn = (size_t)M * N, md = (size_t)M * d;
+  std::vector<double> hx(nd), hy(mn), ls(md), hs(M), hn(M), hw(md), hb(M);
+  DMO_CUDA(cudaMemcpy(hx.data(), X_train, nd * sizeof(double), cudaMemcpyDefault));
+  DMO_CUDA(cudaMemcpy(hy.data(), y, mn * sizeof(double), cudaMemcpyDefault));
+  DMO_CUDA(cudaMemcpy(ls.data(), length_scale, md * sizeof(double), cudaMemcpyDefault));
+  DMO_CUDA(cudaMemcpy(hs.data(), outputscale, M * sizeof(double), cudaMemcpyDefault));
+  DMO_CUDA(cudaMemcpy(hn.data(), noise, M * sizeof(double), cudaMemcpyDefault));
+  DMO_CUDA(cudaMemcpy(hw.data(), weight, md * sizeof(double), cudaMemcpyDefault));
+  DMO_CUDA(cudaMemcpy(hb.data(), bias, M * sizeof(double), cudaMemcpyDefault));
+  for (int m = 0; m < M; ++m) {
+    for (int k = 0; k < d; ++k) DMO_REQUIRE(ls[(size_t)m * d + k] > 0.0, "gp_lml_grad: objective %d: length scale %d must be > 0", m, k);
+    DMO_REQUIRE(hs[m] > 0.0, "gp_lml_grad: objective %d: output scale %g must be > 0", m, hs[m]);
+    DMO_REQUIRE(hn[m] > 0.0, "gp_lml_grad: objective %d: noise %g must be > 0", m, hn[m]);
+  }
+  // per objective: 1 / l_m, the scaled inputs x_n / l_m (the products kernel_matrix_kernel forms), the residuals y_m - m_m(X)
+  std::vector<double> inv(md), xs((size_t)M * nd), res(mn), sd((size_t)2 * M);
+  for (size_t t = 0; t < md; ++t) inv[t] = 1.0 / ls[t];
+  for (int m = 0; m < M; ++m) {
+    sd[m] = hs[m];
+    sd[M + m] = hn[m];
+    for (int64_t n = 0; n < N; ++n) {
+      double mu = hb[m];
+      for (int k = 0; k < d; ++k) {
+        mu += hw[(size_t)m * d + k] * hx[(size_t)n * d + k];
+        xs[((size_t)m * N + n) * d + k] = hx[(size_t)n * d + k] * inv[(size_t)m * d + k];
+      }
+      res[(size_t)m * N + n] = hy[(size_t)m * N + n] - mu;
+    }
+  }
+  const int64_t ld = ceil_div(N + 1, GT) * GT;  // the fit's padded edge: N rows of K_m + the row that carries r_m
+  const int64_t Npad = ceil_div(N, GT) * GT;
+  const int T = (int)(Npad / GT), n_tiles = T * (T + 1) / 2;
+  DevBuf<double> x_d, inv_d, sd_d, r_d, A, work, alpha_d, lml_d;
+  DevBuf<int> info;
+  DMO_TRY(x_d.alloc(ctx, nd));
+  DMO_TRY(inv_d.alloc(ctx, md));
+  DMO_TRY(sd_d.alloc(ctx, (size_t)2 * M));
+  DMO_TRY(r_d.alloc(ctx, mn));
+  DMO_TRY(A.alloc(ctx, (size_t)M * ld * ld));
+  DMO_TRY(work.alloc(ctx, (size_t)M * ld));
+  DMO_TRY(alpha_d.alloc(ctx, mn));
+  DMO_TRY(lml_d.alloc(ctx, M));
+  DMO_TRY(info.alloc(ctx, M));
+  DMO_CUDA(cudaMemcpyAsync(x_d.p, hx.data(), nd * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  DMO_CUDA(cudaMemcpyAsync(inv_d.p, inv.data(), md * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  DMO_CUDA(cudaMemcpyAsync(sd_d.p, sd.data(), (size_t)2 * M * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  DMO_CUDA(cudaMemcpyAsync(r_d.p, res.data(), mn * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  DMO_CUDA(cudaMemsetAsync(info.p, 0, M * sizeof(int), ctx->stream));
+  {
+    // K_m = s_m K_x + sigma2_m I (no jitter): all M factorisations in one pass of the blocked Cholesky
+    ProfileScope ps(ctx, "gp_lg_fit");
+    DMO_TRY(gp_fit_batched(ctx, N, d, M, DMO_KERNEL_MATERN52, x_d.p, inv_d.p, sd_d.p, sd_d.p + M, r_d.p, A.p, ld, info.p, work.p, alpha_d.p,
+                           lml_d.p));
+  }
+  DMO_CHECK_LAUNCH();
+  std::vector<int> h_info(M);
+  std::vector<double> h_lml(M), al(mn);
+  DMO_CUDA(cudaMemcpyAsync(h_info.data(), info.p, M * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  DMO_CUDA(cudaMemcpyAsync(h_lml.data(), lml_d.p, M * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  DMO_CUDA(cudaMemcpyAsync(al.data(), alpha_d.p, mn * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  for (int m = 0; m < M; ++m)
+    if (h_info[m])
+      return dmo_fail(ctx, DMO_ERR_ARG, "gp_lml_grad: the kernel matrix of objective %d is not positive definite (pivot %d)", m,
+                      h_info[m] - 1);
+  work.release();
+  r_d.release();
+  DevBuf<double> Linv;
+  {
+    ProfileScope ps(ctx, "gp_lg_linv");
+    DMO_TRY(Linv.alloc(ctx, (size_t)M * Npad * Npad));
+    DMO_CUDA(cudaMemsetAsync(Linv.p, 0, (size_t)M * Npad * Npad * sizeof(double), ctx->stream));
+    DMO_TRY(gp_linv_from_factor_batched(ctx, A.p, ld, ld * ld, N, M, Npad, Npad * Npad, Linv.p));
+  }
+  A.release();
+  // "B alpha" of the one-block model: s_m alpha_m
+  std::vector<double> bal(mn);
+  for (int m = 0; m < M; ++m)
+    for (int64_t n = 0; n < N; ++n) bal[(size_t)m * N + n] = hs[m] * al[(size_t)m * N + n];
+  const int nq = d + 1;
+  DevBuf<double> xs_d, bal_d, S, part_a, part_g, red;
+  DMO_TRY(xs_d.alloc(ctx, (size_t)M * nd));
+  DMO_TRY(bal_d.alloc(ctx, mn));
+  DMO_TRY(S.alloc(ctx, (size_t)M * Npad * Npad));
+  DMO_TRY(part_a.alloc(ctx, (size_t)M * n_tiles * 2));
+  DMO_TRY(part_g.alloc(ctx, (size_t)M * n_tiles * nq));
+  DMO_TRY(red.alloc(ctx, (size_t)M * (2 + nq)));
+  DMO_CUDA(cudaMemcpyAsync(xs_d.p, xs.data(), (size_t)M * nd * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  DMO_CUDA(cudaMemcpyAsync(bal_d.p, bal.data(), mn * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  {
+    ProfileScope ps(ctx, "gp_lg_ainv");
+    DMO_LAUNCH(mt_ainv_syrk_kernel<true>, dim3((unsigned)n_tiles, (unsigned)M), 256, 0, Linv.p, Npad, N, 1, sd_d.p, xs_d.p, d, S.p, part_a.p);
+    DMO_LAUNCH(mt_fold_kernel<true>, dim3(1, (unsigned)M), 64, 0, part_a.p, n_tiles, 2, red.p);
+  }
+  Linv.release();
+  {
+    ProfileScope ps(ctx, "gp_lg_grad");
+    const size_t smem = ((size_t)2 * GT * (d + 1) + (size_t)2 * GT * (GT + 1) + (size_t)3 * GT) * sizeof(double);
+    DMO_CUDA(cudaFuncSetAttribute(mt_grad_pass_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    DMO_LAUNCH(mt_grad_pass_kernel<true>, dim3((unsigned)n_tiles, (unsigned)M), 256, smem, xs_d.p, N, d, 1, S.p, Npad, alpha_d.p, bal_d.p,
+               part_g.p, nq);
+    DMO_LAUNCH(mt_fold_kernel<true>, dim3((unsigned)ceil_div(nq, 128), (unsigned)M), 128, 0, part_g.p, n_tiles, nq, red.p + 2 * M);
+  }
+  DMO_CHECK_LAUNCH();
+  std::vector<double> hr((size_t)M * (2 + nq));
+  DMO_CUDA(cudaMemcpyAsync(hr.data(), red.p, hr.size() * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  // per objective: tr(K_x K_m^-1), tr(K_m^-1), then sum W dK_x / dl_k * l_k (k < d) and alpha' K_x alpha
+  std::vector<double> gl(md), gs(M), gn(M), gw(md, 0.0), gb(M, 0.0);
+  for (int m = 0; m < M; ++m) {
+    const double trKA = hr[(size_t)2 * m], trA = hr[(size_t)2 * m + 1];
+    const double* G = hr.data() + 2 * M + (size_t)m * nq;
+    const double* a = al.data() + (size_t)m * N;
+    for (int k = 0; k < d; ++k) gl[(size_t)m * d + k] = G[k] / ls[(size_t)m * d + k];
+    gs[m] = 0.5 * (G[d] - trKA);
+    double q = 0.0;
+    for (int64_t n = 0; n < N; ++n) {
+      q += a[n] * a[n];
+      for (int k = 0; k < d; ++k) gw[(size_t)m * d + k] += a[n] * hx[(size_t)n * d + k];
+      gb[m] += a[n];
+    }
+    gn[m] = 0.5 * (q - trA);
+  }
+  DMO_CUDA(cudaMemcpy(lml_out, h_lml.data(), M * sizeof(double), cudaMemcpyDefault));
+  DMO_CUDA(cudaMemcpy(g_length_scale, gl.data(), md * sizeof(double), cudaMemcpyDefault));
+  DMO_CUDA(cudaMemcpy(g_outputscale, gs.data(), M * sizeof(double), cudaMemcpyDefault));
+  DMO_CUDA(cudaMemcpy(g_noise, gn.data(), M * sizeof(double), cudaMemcpyDefault));
+  DMO_CUDA(cudaMemcpy(g_weight, gw.data(), md * sizeof(double), cudaMemcpyDefault));
   DMO_CUDA(cudaMemcpy(g_bias, gb.data(), M * sizeof(double), cudaMemcpyDefault));
   return DMO_OK;
 }

@@ -2,11 +2,12 @@
 
 Drop-ins for ``dmosopt.model_gpytorch.EGP_Matern`` (dmosopt/model_gpytorch.py:1927-2235) and
 ``dmosopt.model_gpytorch.MEGP_Matern`` (:1623-1926), selected in dmosopt by
-``surrogate_method_name="dmosopt_b200.model_gpytorch.EGP_Matern"`` (or ``.MEGP_Matern``).  EGP_Matern trains through
-the reference class itself, which needs gpytorch: after training, the hyper-parameters and the model's own normalised
-training tensors are read out, the posterior is factorised once in float64, and every ``predict`` / ``evaluate`` runs
-on the GPU.  MEGP_Matern also trains on the GPU (``fit="gpu"``, ``megp_fit``): the reference's Adam loop and early
-stopping around the exact log marginal likelihood and its gradient (``dmo_mtgp_lml_grad``), without gpytorch.
+``surrogate_method_name="dmosopt_b200.model_gpytorch.EGP_Matern"`` (or ``.MEGP_Matern``).  Both train either through
+the reference class itself, which needs gpytorch (``fit="reference"``: after training, the hyper-parameters and the
+model's own normalised training tensors are read out), or on the GPU without gpytorch (``fit="gpu"``: the reference's
+Adam loop and early stopping around the exact log marginal likelihood and its gradient, ``egp_fit`` with
+``dmo_gp_lml_grad`` and ``megp_fit`` with ``dmo_mtgp_lml_grad``).  The posterior is then factorised once in float64,
+and every ``predict`` / ``evaluate`` runs on the GPU.
 
 * ``EGP_Matern``: M independent GPs (ARD length scales, output scale, noise, linear-mean weights / bias per objective);
   ``dmo_gp_create`` / ``dmo_gp_set_linear_mean`` / ``dmo_gp_predict``.
@@ -36,8 +37,21 @@ def _matern52_ard(xn, ls):
 
 
 class EGP_Matern:
-    def __init__(self, xin, yin, nInput, nOutput, xlb, xub, return_mean_variance=False, logger=None, precision="fp64",
-                 hyperparameters=None, **kwargs):
+    """M independent exact GPs; the reference constructor signature (model_gpytorch.py:1928-1950) plus ``precision``
+    ("fp64", the default, or "tensor"), ``hyperparameters`` (dict with lengthscale (M,d), outputscale (M,), noise
+    (M,), weight (M,d), bias (M,)): when given, training is skipped, and ``fit``: "gpu" trains with egp_fit (Adam on the
+    exact log marginal likelihood of every objective, on the GPU), "reference" through the reference class (needs
+    gpytorch; every keyword is forwarded); None uses the reference class where it can train and "gpu" otherwise.  The
+    GPU fit has no noise prior (``gp_likelihood_sigma``) and no batched-model mode (``batch_size``); it ignores
+    ``preconditioner_size``, ``fast_pred_var`` and ``use_cuda`` (the likelihood is exact, the variance always the exact
+    one).  After a fit ``hyperparameters`` and ``fit_info`` (one dict per objective) hold the result."""
+
+    def __init__(self, xin, yin, nInput, nOutput, xlb, xub, seed=None, gp_lengthscale_bounds=None, gp_likelihood_sigma=None,
+                 preconditioner_size=100, adam_lr=0.01, fast_pred_var=True, n_iter=5000, min_loss_pct_change=0.1,
+                 return_mean_variance=False, batch_size=None, use_cuda=False, nan="remove", top_k=None, logger=None,
+                 precision="fp64", hyperparameters=None, fit=None, **kwargs):
+        if fit not in (None, "gpu", "reference"):
+            raise ValueError(f"EGP_Matern: fit must be 'gpu', 'reference' or None (got {fit!r})")
         self.nInput, self.nOutput = nInput, nOutput
         self.xlb = np.asarray(xlb, dtype=np.float64)
         xub = np.asarray(xub, dtype=np.float64)
@@ -46,18 +60,36 @@ class EGP_Matern:
         self.logger = logger
         self.precision = _lib.GP_TENSOR if precision in ("tensor", _lib.GP_TENSOR) else _lib.GP_FP64
         self.stats = {}
-        if hyperparameters is None:
-            xn, yn, ymean, ystd, hyperparameters = self._fit_with_reference(xin, yin, nInput, nOutput, xlb, xub, logger, kwargs)
+        self.fit_info = None
+        if hyperparameters is None and fit is None:
+            fit = "reference" if _reference_can_train() else "gpu"
+        if hyperparameters is None and fit == "gpu":
+            if gp_likelihood_sigma is not None:
+                raise ValueError("EGP_Matern: the GPU fit has no noise prior (gp_likelihood_sigma); use fit='reference'")
+            if batch_size is not None:
+                raise ValueError("EGP_Matern: the GPU fit trains one exact GP per objective (batch_size=None); use fit='reference'")
+        if hyperparameters is None and fit == "reference":
+            ref_kwargs = dict(seed=seed, gp_lengthscale_bounds=gp_lengthscale_bounds, gp_likelihood_sigma=gp_likelihood_sigma,
+                              preconditioner_size=preconditioner_size, adam_lr=adam_lr, fast_pred_var=fast_pred_var, n_iter=n_iter,
+                              min_loss_pct_change=min_loss_pct_change, batch_size=batch_size, use_cuda=use_cuda, nan=nan,
+                              top_k=top_k, **kwargs)
+            xn, yn, ymean, ystd, hyperparameters = self._fit_with_reference(xin, yin, nInput, nOutput, xlb, xub, logger, ref_kwargs)
         else:
             xin = np.asarray(xin, dtype=np.float64)
             yin = np.asarray(yin, dtype=np.float64)
             if yin.ndim == 1:
                 yin = yin.reshape(-1, 1)
+            if hyperparameters is None:
+                xin, yin = filter_and_top_k(xin, yin, nan, top_k)  # model_gpytorch.py:1974-1977
             xn = (xin - self.xlb) / self.xrng
             ymean = yin.mean(axis=0)
             ystd = yin.std(axis=0)
             ystd = np.where(ystd == 0.0, 1.0, ystd)  # handle_zeros_in_scale, model_gpytorch.py:1995-2001
             yn = (yin - ymean) / ystd
+            if hyperparameters is None:
+                hyperparameters, self.fit_info = egp_fit(xn, yn, lengthscale_bounds=gp_lengthscale_bounds, adam_lr=adam_lr, n_iter=n_iter,
+                                                         min_loss_pct_change=min_loss_pct_change, seed=seed, logger=logger)
+        self.hyperparameters = hyperparameters
         self._upload(xn, yn, ymean, ystd, hyperparameters)
 
     @staticmethod
@@ -135,6 +167,19 @@ def filter_samples(y, x, nan="remove"):
         keep = ~np.any(np.isnan(y), axis=1)
         return y[keep], x[keep]
     return np.nan_to_num(y, nan=nan), x
+
+
+def filter_and_top_k(xin, yin, nan, top_k):
+    """The reference surrogates' sample selection before normalisation: filter_samples for a non-None ``nan``, then for
+    an integer ``top_k`` below the sample count the first ``top_k`` samples of a non-dominated sort (MOEA.top_k_MO)."""
+    if nan is not None:
+        yin, xin = filter_samples(yin, xin, nan=nan)
+    if isinstance(top_k, int) and xin.shape[0] > top_k:
+        from .MOEA import sortMO
+
+        xs, ys, *_ = sortMO(xin, yin)
+        xin, yin = xs[:top_k], ys[:top_k]
+    return xin, yin
 
 
 def normalise_targets(yin):
@@ -375,6 +420,99 @@ def megp_fit(xn, yn, *, lengthscale_bounds=None, adam_lr=0.01, n_iter=5000, min_
     return hp, {"loss": np.asarray(losses), "iterations": len(losses), "stop_reason": reason, "raw": raw}
 
 
+# gpytorch 1.13's parameterisation of GPyTorchExactGPModelMatern (dmosopt/model_gpytorch.py:455-508; DESIGN.md section 4.4),
+# one row per objective: raw_lengthscale (M,d), raw_outputscale (M,), raw_noise (M,), weights (M,d), bias (M,)
+EGP_MAX_BATCH = 8  # objectives per dmo_gp_lml_grad call
+
+
+def egp_initial_raw(d, M, seed=None):
+    """Initial raw parameters: raw_lengthscale, raw_outputscale and raw_noise 0; the LinearMean weights and bias N(0, 1),
+    drawn from np.random.default_rng(seed), seed None meaning 0, objective by objective: weights (d), then bias."""
+    rng = np.random.default_rng(0 if seed is None else seed)
+    w, b = np.empty((M, d)), np.empty(M)
+    for m in range(M):
+        w[m] = rng.standard_normal(d)
+        b[m] = rng.standard_normal()
+    return {"raw_lengthscale": np.zeros((M, d)), "raw_outputscale": np.zeros(M), "raw_noise": np.zeros(M), "weights": w, "bias": b}
+
+
+def egp_natural(raw, lengthscale_bounds=None):
+    """raw parameters -> (length_scale (M,d), outputscale (M,), noise (M,), weight (M,d), bias (M,))."""
+    if lengthscale_bounds is None:
+        ls = _softplus(raw["raw_lengthscale"])
+    else:
+        lo, hi = float(lengthscale_bounds[0]), float(lengthscale_bounds[1])
+        ls = lo + (hi - lo) * _sigmoid(raw["raw_lengthscale"])
+    return ls, _softplus(raw["raw_outputscale"]), _NOISE_LOWER + _softplus(raw["raw_noise"]), raw["weights"], raw["bias"]
+
+
+def egp_raw_grad(raw, g, lengthscale_bounds=None):
+    """Chain rule: gradients with respect to (length_scale, outputscale, noise, weight, bias), the keys of
+    _lib.gp_lml_grad -> gradients with respect to the raw parameters."""
+    x = raw["raw_lengthscale"]
+    if lengthscale_bounds is None:
+        gl = g["length_scale"] * _softplus_grad(x)
+    else:
+        lo, hi = float(lengthscale_bounds[0]), float(lengthscale_bounds[1])
+        s = _sigmoid(x)
+        gl = g["length_scale"] * ((hi - lo) * (s * (1.0 - s)))
+    return {"raw_lengthscale": gl, "raw_outputscale": g["outputscale"] * _softplus_grad(raw["raw_outputscale"]),
+            "raw_noise": g["noise"] * _softplus_grad(raw["raw_noise"]), "weights": g["weight"], "bias": g["bias"]}
+
+
+def egp_fit(xn, yn, *, lengthscale_bounds=None, adam_lr=0.01, n_iter=5000, min_loss_pct_change=0.1, seed=None, logger=None,
+            initial_raw=None):
+    """Train the EGP model on the GPU: per objective the reference's Adam loop (dmosopt/model_gpytorch.py:2023-2126) on
+    the exact log marginal likelihood and its gradient (dmo_gp_lml_grad).  xn (N,d) normalised inputs, yn (N,M)
+    normalised targets.  Per objective: loss = -lml_m / N, the loss logged at iteration it is the one before that
+    iteration's step, its own Adam and early-stopping rule.  The objectives advance in lockstep, one dmo_gp_lml_grad call
+    per iteration and group of at most EGP_MAX_BATCH objectives still training; an objective that stops leaves the batch.
+    Every objective's arithmetic is its own (the call is deterministic per objective, the host steps work on per-objective
+    arrays), so its trajectory is bit-identical to training it alone.  Returns (hyperparameters, info): the
+    ``hyperparameters=`` dict of EGP_Matern at the final parameters, and one dict per objective with ``loss`` (array),
+    ``iterations``, ``stop_reason`` and ``raw`` (its final raw parameters, rows of one).  ``initial_raw`` (the layout of
+    egp_initial_raw) replaces the seeded initial draws."""
+    xn = np.ascontiguousarray(xn, dtype=np.float64)
+    yn = np.ascontiguousarray(yn, dtype=np.float64).reshape(xn.shape[0], -1)
+    N, d = xn.shape
+    M = yn.shape[1]
+    raw0 = egp_initial_raw(d, M, seed) if initial_raw is None else initial_raw
+    raws = [{k: np.array(np.asarray(v, dtype=np.float64)[m : m + 1]) for k, v in raw0.items()} for m in range(M)]
+    adams = [Adam(lr=adam_lr) for _ in range(M)]
+    stoppers = [EarlyStopping(threshold_pct=min_loss_pct_change) for _ in range(M)]
+    losses = [[] for _ in range(M)]
+    reasons = ["n_iter"] * M
+    active = list(range(M))
+    for it in range(n_iter):
+        if not active:
+            break
+        stopped = []
+        for g0 in range(0, len(active), EGP_MAX_BATCH):
+            group = active[g0 : g0 + EGP_MAX_BATCH]
+            nat = [egp_natural(raws[m], lengthscale_bounds) for m in group]
+            lml, g = _lib.gp_lml_grad(xn, yn[:, group], *(np.concatenate([p[i] for p in nat]) for i in range(5)))
+            for j, m in enumerate(group):
+                loss = -lml[j] / N
+                graw = egp_raw_grad(raws[m], {k: v[j : j + 1] for k, v in g.items()}, lengthscale_bounds)
+                adams[m].step(raws[m], {k: v * (-1.0 / N) for k, v in graw.items()})
+                losses[m].append(loss)
+                if it % 100 == 0 and logger is not None:
+                    noise = _NOISE_LOWER + float(_softplus(raws[m]["raw_noise"])[0])
+                    logger.info(f"EGP_Matern: iter {it}/{n_iter} - Loss: {loss:.3f}  noise: {noise:.3f}")
+                if it >= stoppers[m].warmup_iterations:
+                    stop, why = stoppers[m].should_stop(it, np.array(losses[m]))
+                    if stop:
+                        if logger is not None:
+                            logger.info(f"EGP_Matern: early stop at iteration {it + 1}: {why}")
+                        reasons[m] = why
+                        stopped.append(m)
+        active = [m for m in active if m not in stopped]
+    nat = [egp_natural(r, lengthscale_bounds) for r in raws]
+    hp = {k: np.concatenate([p[i] for p in nat]) for i, k in enumerate(("lengthscale", "outputscale", "noise", "weight", "bias"))}
+    info = [{"loss": np.asarray(losses[m]), "iterations": len(losses[m]), "stop_reason": reasons[m], "raw": raws[m]} for m in range(M)]
+    return hp, info
+
+
 def _reference_can_train():
     """True when dmosopt.model_gpytorch imports with gpytorch available."""
     try:
@@ -424,13 +562,7 @@ class MEGP_Matern:
         else:
             yin = np.asarray(yin, dtype=np.float64).reshape(len(yin), -1)
             xin = np.asarray(xin, dtype=np.float64)
-            if nan is not None:  # model_gpytorch.py:1668-1671
-                yin, xin = filter_samples(yin, xin, nan=nan)
-            if isinstance(top_k, int) and xin.shape[0] > top_k:  # MOEA.top_k_MO
-                from .MOEA import sortMO
-
-                xs, ys, *_ = sortMO(xin, yin)
-                xin, yin = xs[:top_k], ys[:top_k]
+            xin, yin = filter_and_top_k(xin, yin, nan, top_k)  # model_gpytorch.py:1668-1671
             xn = (xin - self.xlb) / self.xrng
             yn, ymean, ystd = normalise_targets(yin)
             if hyperparameters is None:

@@ -254,6 +254,18 @@ int dmo_mtgp_lml_grad(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_tra
                       const double* length_scale, const double* B, const double* D, const double* weight,
                       const double* bias, double* lml_out, double* g_length_scale, double* g_B, double* g_D,
                       double* g_weight, double* g_bias);
+/* dmo_gp_lml_grad: training of M independent exact GPs (EGP_Matern): per objective m the exact log marginal
+ *   likelihood of y_m under K_m = s_m Matern52(X / l_m) + sigma2_m I (no jitter) with the linear prior mean
+ *   X w_m + b_m, and its gradient.  X_train (N,d) normalised inputs, y (M,N) normalised targets (as dmo_gp_fit),
+ *   length_scale and weight (M,d), outputscale, noise and bias (M,); host or device pointers; 1 <= M <= 8, d <= 90.
+ *   Outputs, same shapes: lml_out (M,), d lml_m / d length_scale_m (M,d), / d outputscale_m, / d noise_m (M,),
+ *   / d weight_m (M,d), / d bias_m (M,).  A K_m that is not positive definite gives DMO_ERR_ARG naming the objective.
+ *   Float64, deterministic: objective m's outputs are bit-identical whichever other objectives are evaluated with it,
+ *   in any order, and on repeated calls.  Returns when the outputs are filled. */
+int dmo_gp_lml_grad(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_train, const double* y,
+                    const double* length_scale, const double* outputscale, const double* noise, const double* weight,
+                    const double* bias, double* lml_out, double* g_length_scale, double* g_outputscale,
+                    double* g_noise, double* g_weight, double* g_bias);
 
 /* ---- A16: exact hypervolume ---------------------------------------------------
  * replaces hv.AdaptiveHyperVolume.compute_hypervolume(..., 'box') (dmosopt/hv.py:123-189)

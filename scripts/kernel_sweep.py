@@ -230,6 +230,66 @@ def mtgp_fit_sweep():
           f"stop: {info['stop_reason']}", flush=True)
 
 
+def egp_fit_sweep():
+    """EGP_Matern training: one dmo_gp_lml_grad evaluation over M objectives (median of 5 warm calls, CUDA events per
+    phase) for N in {1024, 2048, 4096}, M in {1, 2, 3}, d = 30, with the counted float64 work (Cholesky, triangular
+    inverse and K^-1: about M N^3 flop), beside the same objectives as M one-task dmo_mtgp_lml_grad calls (the
+    one-objective-at-a-time route), then one default egp_fit on ZDT1 data (d = 30, M = 2, N = 2048)."""
+    from dmosopt_b200.model_gpytorch import egp_fit, egp_initial_raw, egp_natural
+
+    L.context()
+    print(device_line(), flush=True)
+    rng = np.random.default_rng(5)
+    d = 30
+    phases = ("gp_lg_fit", "gp_lg_linv", "gp_lg_ainv", "gp_lg_grad")
+    for N in (1024, 2048, 4096):
+        X = rng.random((N, d))
+        Y = np.column_stack([np.sin(3 * X[:, :4].sum(axis=1) + k) + X[:, 4 + k] ** 2 for k in range(3)])
+        yn = (Y - Y.mean(0)) / Y.std(0)
+        for M in (1, 2, 3):
+            ls, s, nz, w, b = egp_natural(egp_initial_raw(d, M, seed=1))
+            L.gp_lml_grad(X, yn[:, :M], ls, s, nz, w, b)  # warm-up
+            L.profile_enable(True)
+            walls = []
+            for _ in range(5):
+                L.timer_begin()
+                L.gp_lml_grad(X, yn[:, :M], ls, s, nz, w, b)
+                walls.append(L.timer_end())
+            rep = L.profile_report()
+            L.profile_enable(False)
+            ph = {k: rep[k][0] / rep[k][1] for k in phases if k in rep}
+            ms = float(np.median(walls))
+
+            def one_task_calls():
+                for m in range(M):
+                    L.mtgp_lml_grad(X, yn[:, m], ls[m], np.array([[s[m]]]), nz[m : m + 1], w[m : m + 1], b[m : m + 1])
+
+            one_task_calls()  # warm-up
+            walls1 = []
+            for _ in range(5):
+                L.timer_begin()
+                one_task_calls()
+                walls1.append(L.timer_end())
+            ms1 = float(np.median(walls1))
+            f3 = M * float(N) ** 3
+            dense = ph["gp_lg_fit"] + ph["gp_lg_linv"] + ph["gp_lg_ainv"]
+            parts = ", ".join(f"{k[6:]} {v:.2f} ms" for k, v in ph.items())
+            print(f"gp_lml_grad N={N} M={M} d={d}: {ms:.2f} ms median of 5 [{parts}]; M N^3 = {f3 / 1e9:.1f} GFLOP in {dense:.2f} ms = "
+                  f"{f3 / dense / 1e9:.2f} TFLOP/s fp64 | {M} one-task mtgp_lml_grad calls: {ms1:.2f} ms median of 5 "
+                  f"({ms1 / ms:.2f}x the batched call)", flush=True)
+    N, M = 2048, 2
+    X = rng.random((N, d))
+    g = 1.0 + 9.0 / (d - 1) * X[:, 1:].sum(axis=1)
+    Y = np.column_stack((X[:, 0], g * (1.0 - np.sqrt(X[:, 0] / g))))
+    yn = (Y - Y.mean(0)) / Y.std(0)
+    t0 = time.perf_counter()
+    hp, info = egp_fit(X, yn)
+    wall = time.perf_counter() - t0
+    its = [i["iterations"] for i in info]
+    print(f"egp_fit ZDT1 N={N} M={M} d={d} (defaults: lr 0.01, n_iter 5000): iterations per output {its}, {wall:.1f} s "
+          f"({1e3 * wall / max(its):.1f} ms per lockstep iteration); stop: {[i['stop_reason'] for i in info]}", flush=True)
+
+
 def stream_sweep():
     """The HBM-bound kernels at the BASELINE shape: crowding / euclidean distance (n = 131072, M = 3), SBX + mutation
     (pop 65536, d 30), mean kernel's neighbours, hypervolume of a 65536-point 3-D front.  Prints time and the achieved
@@ -277,5 +337,8 @@ if __name__ == "__main__":
         sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "mtgp_fit":
         mtgp_fit_sweep()
+        sys.exit(0)
+    if len(sys.argv) > 1 and sys.argv[1] == "egp_fit":
+        egp_fit_sweep()
         sys.exit(0)
     main()
