@@ -71,6 +71,7 @@ _SIGNATURES = {
     "dmo_gp_predict": (_c_int, [_vp, _vp, _vp, _c_i64, _vp, _vp, _c_int]),
     "dmo_gp_auto_info": (_c_int, [_vp, _vp, ctypes.POINTER(_c_int), ctypes.POINTER(_c_int), ctypes.POINTER(_c_dbl), ctypes.POINTER(_c_dbl),
                                   ctypes.POINTER(_c_dbl), ctypes.POINTER(_c_i64)]),
+    "dmo_gp_covariance_groups": (_c_int, [_vp, _vp, ctypes.POINTER(_c_int), _vp]),
     "dmo_mtgp_create": (_c_int, [_vp, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.POINTER(_c_dbl),
                                  ctypes.POINTER(_vp)]),
     "dmo_mtgp_predict": (_c_int, [_vp, _vp, _vp, _c_i64, _vp, _vp, _c_int]),
@@ -779,6 +780,15 @@ class GPHandle:
         return {"mean_tensor": bool(mt.value & 1), "mean_only_tensor": bool(mt.value & 4),
                 "var_tensor": bool(vt.value), "mean_err": em.value,
                 "var_err": ev.value, "theta": th.value, "last_refined": int(rows.value)}
+
+    def covariance_groups(self):
+        """``(G, group_of)``: the number of distinct posterior covariances and, per objective, the group whose L^-1, K_*
+        and variance contraction it shares (groups numbered in order of first appearance)."""
+        n = _c_int(0)
+        grp = np.zeros(self.M, dtype=np.int32)
+        _check(load_library().dmo_gp_covariance_groups(context(), self._h, ctypes.byref(n), grp.ctypes.data_as(_vp)),
+               "dmo_gp_covariance_groups")
+        return int(n.value), [int(g) for g in grp]
 
     def close(self):
         if getattr(self, "_h", None) is not None and _lib is not None and _ctx is not None:

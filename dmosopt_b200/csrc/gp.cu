@@ -9,6 +9,10 @@
 //
 // This file holds the float64 CUDA-core path (DMO_GP_FP64, the parity anchor, ~1e-10 of sklearn) and the object
 // management; the wgmma split-precision path lives in gp_tensor.cu.
+#include <string.h>
+
+#include <algorithm>
+
 #include "gp.cuh"
 
 namespace {
@@ -132,7 +136,7 @@ __global__ void normalise_x_kernel(const double* __restrict__ X, int64_t P, int 
   Xn[t] = (X[t] - xlb[j]) / xrg[j];  // model.py:1262-1263
 }
 
-// ---- K_* tiles: Ks[m][p][n] = c_m * k(||x_p - x_n|| / l_m), float64 ---------------------------------------
+// ---- K_* tiles: Ks[g][p][n] = c_g * k(||x_p - x_n|| / l_g), float64, one plane per covariance g ------------------
 constexpr int KS_TN = 128;  // train points per block (one per thread)
 constexpr int KS_TP = 32;   // candidates per block
 constexpr int KS_DMAX = 64; // input dimensions held in registers
@@ -197,16 +201,16 @@ __global__ void __launch_bounds__(KS_TN) kstar_kernel(const double* __restrict__
   }
 }
 
-// ---- mean[p][m] = y_std * (Ks[m][p][:] . alpha[m]) + y_mean: one warp per row ---------------------------------
+// ---- mean[p][m] = y_std * (Ks[cov[m]][p][:] . alpha[m]) + y_mean: one warp per row ---------------------------
 __global__ void mean_kernel(const double* __restrict__ Ks, int64_t Pc, int64_t N, int64_t ldk, int64_t plane, int M,
-                            const double* __restrict__ alpha, const double* __restrict__ ymean,
+                            const int* __restrict__ cov, const double* __restrict__ alpha, const double* __restrict__ ymean,
                             const double* __restrict__ ystd, int64_t p_base, double* __restrict__ mean) {
   const int64_t w = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (w >= Pc * M) return;
   const int m = (int)(w / Pc);
   const int64_t pl = w - (int64_t)m * Pc;
-  const double* row = Ks + m * plane + pl * ldk;
+  const double* row = Ks + cov[m] * plane + pl * ldk;
   const double* a = alpha + (int64_t)m * N;
   double s = 0.0;
   for (int64_t n = lane; n < N; n += 32) s += row[n] * a[n];
@@ -229,10 +233,10 @@ __global__ void __launch_bounds__(256, 1)
   extern __shared__ __align__(16) double vsm[];
   double* As = vsm;                      // [2][VK][VLD]
   double* Bs = vsm + 2 * VK * VLD;       // [2][VK][VLD]
-  const int m = blockIdx.y;
+  const int g = blockIdx.y;  // covariance
   const int64_t p0 = (int64_t)blockIdx.x * VB;
-  const double* A = Linv + (int64_t)m * lplane;
-  const double* B = Ks + (int64_t)m * kplane + p0 * ldk;
+  const double* A = Linv + (int64_t)g * lplane;
+  const double* B = Ks + (int64_t)g * kplane + p0 * ldk;
   const int tid = threadIdx.x;
   const int ti = tid >> 4, tj = tid & 15;  // 16 x 16 thread grid, 8 x 8 elements each
   const int lrow = tid >> 1;               // global->shared: each thread moves 8 doubles of A and of B per k step
@@ -327,23 +331,48 @@ __global__ void __launch_bounds__(256, 1)
     double s = 0.0;
 #pragma unroll
     for (int r = 0; r < 16; ++r) s += red[r * VB + tid];
-    vnorm[((int64_t)blockIdx.z * gridDim.y + m) * Pcpad + p0 + tid] = s;
+    vnorm[((int64_t)blockIdx.z * gridDim.y + g) * Pcpad + p0 + tid] = s;
   }
 }
 
-__global__ void var_finish_kernel(const double* __restrict__ vnorm, int nplanes, int64_t Pc, int64_t Pcpad, int M,
-                                  const double* __restrict__ constant, const double* __restrict__ noise,
+// objective m reads the sums of its covariance cov[m] < G and keeps its own constant, noise and y_std
+__global__ void var_finish_kernel(const double* __restrict__ vnorm, int nplanes, int64_t Pc, int64_t Pcpad, int M, int G,
+                                  const int* __restrict__ cov, const double* __restrict__ constant, const double* __restrict__ noise,
                                   const double* __restrict__ ystd, int64_t p_base, double* __restrict__ var) {
   int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= Pc * M) return;
   int64_t pl = t / M;
   int m = (int)(t - pl * M);
   double vn = 0.0;
-  for (int z = 0; z < nplanes; ++z) vn += vnorm[((int64_t)z * M + m) * Pcpad + pl];  // row-block groups, fixed order
+  const int g = cov[m];
+  for (int z = 0; z < nplanes; ++z) vn += vnorm[((int64_t)z * G + g) * Pcpad + pl];  // row-block groups, fixed order
   double v = (constant[m] + noise[m]) - vn;  // kernel_.diag(X) - einsum(V^2)
   if (v < 0.0) v = 0.0;                                                  // sklearn clamps negative variances
   double sd = sqrt(v * (ystd[m] * ystd[m]));                             // sklearn returns the std ...
   var[(p_base + pl) * M + m] = sd * sd;                                  // ... dmosopt squares it (model.py:1267)
+}
+
+// diff[m] bit l (l < m < M <= 16): factor planes l and m (n doubles each) differ bitwise somewhere.  Every plane is read
+// once; the caller zeroes diff.
+constexpr int GP_MAX_M = 16;
+__global__ void factor_diff_kernel(const unsigned long long* __restrict__ F, int64_t n, int M, unsigned* __restrict__ diff) {
+  unsigned dm[GP_MAX_M];
+#pragma unroll
+  for (int m = 0; m < GP_MAX_M; ++m) dm[m] = 0u;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += (int64_t)gridDim.x * blockDim.x) {
+    unsigned long long v[GP_MAX_M];
+#pragma unroll
+    for (int m = 0; m < GP_MAX_M; ++m) v[m] = m < M ? F[m * n + t] : 0ull;
+#pragma unroll
+    for (int m = 1; m < GP_MAX_M; ++m)
+#pragma unroll
+      for (int l = 0; l < m; ++l) dm[m] |= v[m] != v[l] ? 1u << l : 0u;
+  }
+#pragma unroll
+  for (int m = 1; m < GP_MAX_M; ++m) {
+    const unsigned r = __reduce_or_sync(0xffffffffu, dm[m]);
+    if ((threadIdx.x & 31) == 0 && r && m < M) atomicOr(diff + m, r);
+  }
 }
 
 }  // namespace
@@ -387,7 +416,7 @@ static_assert(VB == GP_F64_TILE, "gp.cuh exports the float64 variance tile edge"
 
 int gp_var_contract_fp64(dmo_ctx* ctx, const dmo_gp* gp, const double* Ks, int64_t kplane, int64_t Pcpad, int nsplit,
                          double* vnorm, int64_t vn_ld) {
-  dim3 gv((unsigned)(Pcpad / VB), (unsigned)gp->M, (unsigned)nsplit);
+  dim3 gv((unsigned)(Pcpad / VB), (unsigned)gp->G, (unsigned)nsplit);
   DMO_CUDA(cudaFuncSetAttribute(var_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)VAR_SMEM));
   DMO_LAUNCH(var_kernel, gv, 256, VAR_SMEM, gp->Linv.p, gp->Npad, gp->Npad * gp->Npad, Ks, gp->Npad, kplane, gp->Npad, vnorm,
              vn_ld);
@@ -396,10 +425,10 @@ int gp_var_contract_fp64(dmo_ctx* ctx, const dmo_gp* gp, const double* Ks, int64
 
 int gp_predict_fp64(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var) {
   const int64_t N = gp->N, Npad = gp->Npad;
-  const int M = gp->M, d = gp->d;
-  // candidate chunk so that Ks (M x Pc x Npad float64) stays within ~8 GiB
+  const int M = gp->M, G = gp->G, d = gp->d;
+  // candidate chunk so that Ks (G x Pc x Npad float64) stays within ~8 GiB
   int64_t budget = (int64_t)8 << 30;
-  int64_t Pc_max = budget / ((int64_t)M * Npad * 8);
+  int64_t Pc_max = budget / ((int64_t)G * Npad * 8);
   Pc_max = (Pc_max / VB) * VB;
   if (Pc_max < VB) Pc_max = VB;
   const int64_t Pc_alloc = P < Pc_max ? ceil_div(P, VB) * VB : Pc_max;
@@ -409,8 +438,8 @@ int gp_predict_fp64(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, doub
   if (nsplit > ntile) nsplit = ntile;
   if (nsplit < 1) nsplit = 1;
   DevBuf<double> Ks, vnorm;
-  DMO_TRY(Ks.alloc(ctx, (size_t)M * Pc_alloc * Npad));
-  DMO_TRY(vnorm.alloc(ctx, (size_t)nsplit * M * Pc_alloc));
+  DMO_TRY(Ks.alloc(ctx, (size_t)G * Pc_alloc * Npad));
+  DMO_TRY(vnorm.alloc(ctx, (size_t)nsplit * G * Pc_alloc));
   const int64_t kplane = Pc_alloc * Npad;
   for (int64_t p_base = 0; p_base < P; p_base += Pc_alloc) {
     const int64_t Pc = (P - p_base) < Pc_alloc ? (P - p_base) : Pc_alloc;
@@ -420,24 +449,22 @@ int gp_predict_fp64(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, doub
     {
       ProfileScope ps(ctx, "gp_kstar");
       if (gp->isotropic)
-      DMO_LAUNCH(kstar_kernel<true>, gk, KS_TN, smem, dXn, P, p_base, Pcpad, gp->Xt.p, N, d, M, gp->kernel,
-                 gp->inv_ls.p, gp->constant.p, Npad, kplane, Ks.p);
+      DMO_LAUNCH(kstar_kernel<true>, gk, KS_TN, smem, dXn, P, p_base, Pcpad, gp->Xt.p, N, d, G, gp->kernel,
+                 gp->g_inv_ls.p, gp->g_constant.p, Npad, kplane, Ks.p);
     else
-      DMO_LAUNCH(kstar_kernel<false>, gk, KS_TN, smem, dXn, P, p_base, Pcpad, gp->Xt.p, N, d, M, gp->kernel,
-                 gp->inv_ls.p, gp->constant.p, Npad, kplane, Ks.p);
+      DMO_LAUNCH(kstar_kernel<false>, gk, KS_TN, smem, dXn, P, p_base, Pcpad, gp->Xt.p, N, d, G, gp->kernel,
+                 gp->g_inv_ls.p, gp->g_constant.p, Npad, kplane, Ks.p);
     }
     {
       ProfileScope ps(ctx, "gp_mean");
-    DMO_LAUNCH(mean_kernel, (unsigned)ceil_div(Pc * M * 32, 256), 256, 0, Ks.p, Pc, N, Npad, kplane, M, gp->alpha.p,
+    DMO_LAUNCH(mean_kernel, (unsigned)ceil_div(Pc * M * 32, 256), 256, 0, Ks.p, Pc, N, Npad, kplane, M, gp->cov.p, gp->alpha.p,
                gp->ymean.p, gp->ystd.p, p_base, d_mean);
     }
     if (d_var) {
       ProfileScope ps(ctx, "gp_var");
-      dim3 gv((unsigned)(Pcpad / VB), (unsigned)M, (unsigned)nsplit);
-      DMO_CUDA(cudaFuncSetAttribute(var_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)VAR_SMEM));
-      DMO_LAUNCH(var_kernel, gv, 256, VAR_SMEM, gp->Linv.p, Npad, Npad * Npad, Ks.p, Npad, kplane, Npad, vnorm.p, Pc_alloc);
-      DMO_LAUNCH(var_finish_kernel, (unsigned)ceil_div(Pc * M, 256), 256, 0, vnorm.p, (int)nsplit, Pc, Pc_alloc, M,
-                 gp->constant.p, gp->noise.p, gp->ystd.p, p_base, d_var);
+      DMO_TRY(gp_var_contract_fp64(ctx, gp, Ks.p, kplane, Pcpad, (int)nsplit, vnorm.p, Pc_alloc));
+      DMO_LAUNCH(var_finish_kernel, (unsigned)ceil_div(Pc * M, 256), 256, 0, vnorm.p, (int)nsplit, Pc, Pc_alloc, M, G,
+                 gp->cov.p, gp->constant.p, gp->noise.p, gp->ystd.p, p_base, d_var);
     }
   }
   DMO_CHECK_LAUNCH();
@@ -623,14 +650,15 @@ int dmo_gp_create(dmo_ctx* ctx, int64_t N, int d, int M, int kernel, const doubl
   DMO_CUDA(cudaSetDevice(ctx->device));
   DMO_REQUIRE(out, "gp_create: null output");
   *out = nullptr;
-  DMO_REQUIRE(N >= 1 && d >= 1 && d <= KS_DMAX && M >= 1 && M <= 16, "gp_create: unsupported shape N=%lld d=%d M=%d",
+  DMO_REQUIRE(N >= 1 && d >= 1 && d <= KS_DMAX && M >= 1 && M <= GP_MAX_M, "gp_create: unsupported shape N=%lld d=%d M=%d",
               (long long)N, d, M);
   DMO_REQUIRE(kernel == DMO_KERNEL_MATERN52 || kernel == DMO_KERNEL_RBF, "gp_create: unknown kernel %d", kernel);
   DMO_REQUIRE(X_train && alpha && factor && constant && length_scale && noise && y_mean && y_std && xlb && xub,
               "gp_create: null pointer");
   // host copies of the small parameter vectors (needed to derive 1/l, ranges, isotropy)
-  std::vector<double> h_ls((size_t)M * d), h_lb(d), h_ub(d);
+  std::vector<double> h_ls((size_t)M * d), h_lb(d), h_ub(d), h_c(M);
   DMO_CUDA(cudaMemcpy(h_ls.data(), length_scale, h_ls.size() * sizeof(double), cudaMemcpyDefault));
+  DMO_CUDA(cudaMemcpy(h_c.data(), constant, M * sizeof(double), cudaMemcpyDefault));
   DMO_CUDA(cudaMemcpy(h_lb.data(), xlb, d * sizeof(double), cudaMemcpyDefault));
   DMO_CUDA(cudaMemcpy(h_ub.data(), xub, d * sizeof(double), cudaMemcpyDefault));
   dmo_gp* gp = new dmo_gp();
@@ -666,7 +694,6 @@ int dmo_gp_create(dmo_ctx* ctx, int64_t N, int d, int M, int kernel, const doubl
   const int64_t Npad = gp->Npad;
   GP_TRY(gp->Xt.alloc(ctx, (size_t)N * d));
   GP_TRY(gp->alpha.alloc(ctx, (size_t)M * N));
-  GP_TRY(gp->Linv.alloc(ctx, (size_t)M * Npad * Npad));
   GP_TRY(gp->inv_ls.alloc(ctx, (size_t)M * d));
   GP_TRY(gp->constant.alloc(ctx, M));
   GP_TRY(gp->noise.alloc(ctx, M));
@@ -683,13 +710,52 @@ int dmo_gp_create(dmo_ctx* ctx, int64_t N, int d, int M, int kernel, const doubl
   GP_CUDA(cudaMemcpyAsync(gp->ystd.p, y_std, M * sizeof(double), cudaMemcpyDefault, ctx->stream));
   GP_CUDA(cudaMemcpyAsync(gp->xlb.p, h_lb.data(), d * sizeof(double), cudaMemcpyDefault, ctx->stream));
   GP_CUDA(cudaMemcpyAsync(gp->xrg.p, h_rg.data(), d * sizeof(double), cudaMemcpyDefault, ctx->stream));
-  GP_CUDA(cudaMemsetAsync(gp->Linv.p, 0, (size_t)M * Npad * Npad * sizeof(double), ctx->stream));
+  std::vector<double> h_ginv, h_gc;
   {
     In<double> f;
     GP_TRY(f.init(ctx, factor, (size_t)M * N * N));
+    // covariance groups: objective m shares the covariance of the first earlier group whose leader has bitwise the same
+    // constant, length scales and factor plane
+    std::vector<unsigned> h_diff(M, 0u);
+    if (M > 1) {
+      DevBuf<unsigned> diff;
+      GP_TRY(diff.alloc(ctx, M));
+      GP_CUDA(cudaMemsetAsync(diff.p, 0, M * sizeof(unsigned), ctx->stream));
+      const int64_t n = N * N;
+      const int64_t nb = std::min<int64_t>(ceil_div(n, 256), (int64_t)8 * ctx->sm_count);
+      DMO_LAUNCH(factor_diff_kernel, (unsigned)nb, 256, 0, reinterpret_cast<const unsigned long long*>(f.d), n, M, diff.p);
+      GP_CUDA(cudaMemcpyAsync(h_diff.data(), diff.p, M * sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));
+      GP_CUDA(cudaStreamSynchronize(ctx->stream));
+    }
+    gp->h_cov.assign(M, -1);
     for (int m = 0; m < M; ++m) {
-      const double* src = f.d + (size_t)m * N * N;
-      double* dst = gp->Linv.p + (size_t)m * Npad * Npad;
+      for (int l : gp->h_lead)
+        if (memcmp(&h_c[l], &h_c[m], sizeof(double)) == 0 &&
+            memcmp(&h_ls[(size_t)l * d], &h_ls[(size_t)m * d], d * sizeof(double)) == 0 && !((h_diff[m] >> l) & 1u)) {
+          gp->h_cov[m] = gp->h_cov[l];
+          break;
+        }
+      if (gp->h_cov[m] < 0) {
+        gp->h_cov[m] = (int)gp->h_lead.size();
+        gp->h_lead.push_back(m);
+      }
+    }
+    const int G = gp->G = (int)gp->h_lead.size();
+    for (int l : gp->h_lead) {
+      h_ginv.insert(h_ginv.end(), h_inv.begin() + (size_t)l * d, h_inv.begin() + (size_t)(l + 1) * d);
+      h_gc.push_back(h_c[l]);
+    }
+    GP_TRY(gp->cov.alloc(ctx, M));
+    GP_TRY(gp->g_inv_ls.alloc(ctx, (size_t)G * d));
+    GP_TRY(gp->g_constant.alloc(ctx, G));
+    GP_CUDA(cudaMemcpyAsync(gp->cov.p, gp->h_cov.data(), M * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+    GP_CUDA(cudaMemcpyAsync(gp->g_inv_ls.p, h_ginv.data(), h_ginv.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    GP_CUDA(cudaMemcpyAsync(gp->g_constant.p, h_gc.data(), G * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    GP_TRY(gp->Linv.alloc(ctx, (size_t)G * Npad * Npad));
+    GP_CUDA(cudaMemsetAsync(gp->Linv.p, 0, (size_t)G * Npad * Npad * sizeof(double), ctx->stream));
+    for (int g = 0; g < G; ++g) {
+      const double* src = f.d + (size_t)gp->h_lead[g] * N * N;
+      double* dst = gp->Linv.p + (size_t)g * Npad * Npad;
       if (factor_is_inverse) {
         DMO_LAUNCH(copy_pad_kernel, (unsigned)ceil_div(N * N, 256), 256, 0, src, N, N, Npad, dst);
       } else {
@@ -700,10 +766,9 @@ int dmo_gp_create(dmo_ctx* ctx, int64_t N, int d, int M, int kernel, const doubl
     GP_CUDA(cudaStreamSynchronize(ctx->stream));
   }
   // host copies used by the tensor path's scaling
-  gp->h_constant.resize(M);
+  gp->h_constant = h_c;
   gp->h_noise.resize(M);
   gp->h_ystd.resize(M);
-  GP_CUDA(cudaMemcpy(gp->h_constant.data(), constant, M * sizeof(double), cudaMemcpyDefault));
   GP_CUDA(cudaMemcpy(gp->h_noise.data(), noise, M * sizeof(double), cudaMemcpyDefault));
   GP_CUDA(cudaMemcpy(gp->h_ystd.data(), y_std, M * sizeof(double), cudaMemcpyDefault));
 #undef GP_TRY
@@ -767,6 +832,14 @@ int dmo_gp_auto_info(dmo_ctx* ctx, dmo_gp* gp, int* mean_tensor, int* var_tensor
   if (var_err) *var_err = gp->cal_var_err;
   if (theta) *theta = gp->refine_theta;
   if (last_refined) *last_refined = gp->last_refined;
+  return DMO_OK;
+}
+
+int dmo_gp_covariance_groups(dmo_ctx* ctx, dmo_gp* gp, int* n_groups, int* group_of) {
+  if (!ctx) return DMO_ERR_ARG;
+  DMO_REQUIRE(gp, "gp_covariance_groups: null model");
+  if (n_groups) *n_groups = gp->G;
+  if (group_of) memcpy(group_of, gp->h_cov.data(), (size_t)gp->M * sizeof(int));
   return DMO_OK;
 }
 

@@ -8,10 +8,18 @@ struct dmo_gp {
   int64_t N = 0, Npad = 0;  // training points; padded to the variance tile edge
   int d = 0, M = 0, kernel = 0;
   bool isotropic = true;
+  // Objectives that share a posterior covariance (bitwise equal constant, length scales and factor plane; noise may
+  // differ, it only enters the final subtraction) share one L^-1, one K_* and one variance contraction.  Decided once
+  // by dmo_gp_create: G groups numbered in order of first appearance, cov[m] the group of objective m, lead[g] the first
+  // objective of group g.  Every per-covariance array below has G planes.
+  int G = 0;
+  std::vector<int> h_cov, h_lead;  // (M,), (G,)
+  DevBuf<int> cov;                 // (M,) device copy of h_cov
   DevBuf<double> Xt;        // (N, d) normalised training inputs
   DevBuf<double> alpha;     // (M, N)
-  DevBuf<double> Linv;      // (M, Npad, Npad) lower-triangular inverse Cholesky factors, zero padded
+  DevBuf<double> Linv;      // (G, Npad, Npad) lower-triangular inverse Cholesky factors, zero padded
   DevBuf<double> inv_ls;    // (M, d) 1 / length_scale
+  DevBuf<double> g_inv_ls, g_constant;  // (G, d), (G,) 1 / length_scale and constant of each group (its first objective)
   DevBuf<double> constant, noise, ymean, ystd;  // (M,)
   DevBuf<double> xlb, xrg;  // (d,)
   std::vector<double> h_constant, h_noise, h_ystd;
@@ -20,9 +28,9 @@ struct dmo_gp {
   DevBuf<double> lin_w, lin_b;  // (M, d), (M,)
   // tensor path (built lazily on first DMO_GP_TENSOR predict)
   bool tensor_ready = false;
-  DevBuf<uint16_t> Lhi, Llo;  // (M, Npad, Npad) fp16 split of the row-scaled L^-1
-  DevBuf<float> Lscale;       // (M, Npad) 1 / (row scale * K_* scale), powers of two
-  DevBuf<int> Kexp;           // (M,) K_* scaling exponents
+  DevBuf<uint16_t> Lhi, Llo;  // (G, Npad, Npad) fp16 split of the row-scaled L^-1
+  DevBuf<float> Lscale;       // (G, Npad) 1 / (row scale * K_* scale), powers of two
+  DevBuf<int> Kexp;           // (G,) K_* scaling exponents
   DevBuf<float> Xtf;          // (Npad, 32) float copy of Xt, zero padded (mean-only direct kernel, d <= 32); built lazily
   DevBuf<float> CAf;          // (M, Npad) c_m * alpha_m as float, zero padded (fused K_* + mean kernel); built with Xtf
   // DMO_GP_AUTO: per-model calibration of the tensor path against the float64 path on probe candidates (gp.cu)
@@ -49,17 +57,17 @@ int gp_linv_from_factor_batched(dmo_ctx* ctx, const double* L, int64_t ldl, int6
 // nbat independent exact-GP factorisations in one pass of the blocked Cholesky (gp_fit.cu; see its definition)
 int gp_fit_batched(dmo_ctx* ctx, int64_t N, int d, int nbat, int kernel, const double* X, const double* inv_ls, const double* constant,
                    const double* diag_add, const double* y, double* A, int64_t ld, int* info, double* work, double* alpha, double* lml);
-// float64 variance contraction (var_kernel): vnorm[z][m][p] = partial sums over the row blocks z (mod nsplit) of
-// ||Linv_m Ks_m[p]||^2, Ks_m = Ks + m * kplane with rows of gp->Npad doubles (kplane = 0: one K_* plane for every m);
-// Pcpad is a multiple of GP_F64_TILE
+// float64 variance contraction (var_kernel) over the gp->G covariances: vnorm[z][g][p] = partial sums over the row
+// blocks z (mod nsplit) of ||Linv_g Ks_g[p]||^2, Ks_g = Ks + g * kplane with rows of gp->Npad doubles (kplane = 0: one
+// K_* plane for every g); Pcpad is a multiple of GP_F64_TILE
 constexpr int GP_F64_TILE = 128;
 int gp_var_contract_fp64(dmo_ctx* ctx, const dmo_gp* gp, const double* Ks, int64_t kplane, int64_t Pcpad, int nsplit,
                          double* vnorm, int64_t vn_ld);
 // the fp16 hi / lo split of L^-1 and its row scales (built once per model; gp->Kexp holds the K_* scaling exponents)
 int gp_prepare_tensor(dmo_ctx* ctx, dmo_gp* gp);
 // wgmma variance contraction (gp_var_wgmma_kernel, paired schedule) over K_* hi / lo rows of gp->Npad fp16 values:
-// k_alloc rows are allocated, objective m reads rows m * k_rows + [0, Pcpad) (k_rows = 0: one plane for every m);
-// Pcpad is a multiple of GP_TC_TILE.  vnorm[q][m][p], q < gp_tensor_var_planes(gp->Npad), holds the partial sums.
+// k_alloc rows are allocated, covariance g < gp->G reads rows g * k_rows + [0, Pcpad) (k_rows = 0: one plane for every
+// g); Pcpad is a multiple of GP_TC_TILE.  vnorm[q][g][p], q < gp_tensor_var_planes(gp->Npad), holds the partial sums.
 // abort_flag (device int, zeroed by the caller) is set when the pipeline watchdog trips.
 constexpr int GP_TC_TILE = 128;
 int gp_tensor_var_planes(int64_t Npad);

@@ -419,6 +419,11 @@ int dmo_mtgp_create(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_train
   gp->Npad = Npad;
   gp->d = d;
   gp->M = M;
+  gp->G = M;  // the blocks share K_* but not L_j^-1: one covariance each
+  for (int j = 0; j < M; ++j) {
+    gp->h_cov.push_back(j);
+    gp->h_lead.push_back(j);
+  }
   gp->kernel = DMO_KERNEL_MATERN52;
   gp->h_constant.assign(M, 1.0);  // K_* carries no output scale: one K_* scaling exponent for every block
   gp->h_noise.assign(M, 1.0);

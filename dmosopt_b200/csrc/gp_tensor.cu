@@ -146,14 +146,14 @@ __device__ __forceinline__ void wgmma_f16_m64n256(float (&d)[128], uint64_t ades
 }
 
 // ------------------------------------------------------------------------------------------------ the contraction
-// Work items and their order.  An item is (objective, 128 candidates, item q of the candidate block); the q of a
+// Work items and their order.  An item is (covariance, 128 candidates, item q of the candidate block); the q of a
 // candidate block are adjacent in the list, so the CTAs that share a K_* tile start together at k = 0 and walk k at the
 // same (MMA-bound) rate: one of them pulls the tile from DRAM and the others hit it in L2.  Item q owns the Linv row
 // blocks {q, n_jt - 1 - q} (one block when they coincide), so every item costs the same n_jt + 1 k-blocks and a static
 // round-robin over the persistent CTAs has a tail of at most one item.  Each item writes its partial sums to its own
 // plane q of vnorm; var_finish_tc_kernel adds the planes in a fixed order.
 struct GemmParams {
-  int M, n_pb, n_jt, n_q;  // n_q items per candidate block
+  int M, n_pb, n_jt, n_q;  // M covariance planes (K_* and Linv), n_q items per candidate block
   int64_t k_rows, l_rows;
   const float* inv_scale;
   double* vnorm;  // [n_q][M][vn_ld]
@@ -299,11 +299,11 @@ __global__ void __launch_bounds__(NTHREADS, 1)
 }
 
 // ------------------------------------------------------------------------------------------------ operand preparation
-// Linv row -> scaled fp16 hi / lo.  One block per (objective, row).
-__global__ void split_linv_kernel(const double* __restrict__ Linv, int64_t Npad, int M, const int* __restrict__ k_exp,
+// Linv row -> scaled fp16 hi / lo.  One block per (covariance, row).
+__global__ void split_linv_kernel(const double* __restrict__ Linv, int64_t Npad, const int* __restrict__ k_exp,
                                   uint16_t* __restrict__ Lh, uint16_t* __restrict__ Ll, float* __restrict__ inv_scale) {
-  const int64_t row = blockIdx.x;  // m * Npad + i
-  const int m = (int)(row / Npad);
+  const int64_t row = blockIdx.x;  // g * Npad + i
+  const int g = (int)(row / Npad);
   const double* src = Linv + row * Npad;
   __shared__ double red[256];
   double mx = 0.0;
@@ -325,7 +325,7 @@ __global__ void split_linv_kernel(const double* __restrict__ Linv, int64_t Npad,
     Lh[row * Npad + k] = __half_as_ushort(h);
     Ll[row * Npad + k] = __half_as_ushort(l);
   }
-  if (threadIdx.x == 0) inv_scale[row] = (mx > 0.0) ? (float)scalbn(1.0, -e - k_exp[m]) : 0.f;
+  if (threadIdx.x == 0) inv_scale[row] = (mx > 0.0) ? (float)scalbn(1.0, -e - k_exp[g]) : 0.f;
 }
 
 constexpr int KT_TN = 128, KT_TP = 32;
@@ -371,7 +371,8 @@ __device__ __forceinline__ float2 stationary2_f(float2 s2, int kind) {
   return e;
 }
 
-// K_* in fp32 -> scaled fp16 hi / lo.  Each thread owns two adjacent training points (their coordinates live in
+// K_* in fp32 -> scaled fp16 hi / lo, one plane per covariance (M = the number of planes, inv_ls / constant / k_exp
+// per plane).  Each thread owns two adjacent training points (their coordinates live in
 // registers, results leave as packed half2), a block covers 256 training points x KT_TP candidates; the candidate
 // tile is read from shared memory as 16-byte broadcasts (rows padded with zeros to DMAX coordinates, so the
 // distance loops need no bounds tests and the LSU pipe carries a quarter of the instructions of scalar loads).
@@ -618,6 +619,9 @@ __global__ void __launch_bounds__(KM_T, 4)
 // slice in 64-point chunks, each lane holding two adjacent training points (coordinates in registers) while the
 // candidates arrive as 16-byte shared-memory broadcasts.  Every K_* store is then one full, contiguous 128-byte line per
 // warp (32 lanes x half2) straight from registers: no staging tile, no block barrier between arithmetic and stores.
+// Kernel values and K_* planes are produced once per covariance g < G (inv_ls, constant, k_exp per covariance); the mean
+// chains of objective m read those of its covariance cov[m].  GROUPED = false is the model without shared covariances
+// (G = MT, cov[m] = m): its indices stay compile-time constants, so the objectives' evaluations interleave freely.
 // The mean keeps the rounding structure of the sums it replaces: per candidate and objective an fp32 chain
 // acc = fma(k_n, c alpha_n, acc) over 16 consecutive training points (from the slice start, in order), folded into
 // float64 in ascending order over the slice; the slices are those of pick_slices(.., KF_NS, 3 x SMs, ..).  The chains
@@ -638,19 +642,22 @@ constexpr size_t kstar_mean_smem(int MT) {
   return (size_t)(KS_Q * KM_D + 4 * ks_warp_floats(MT)) * sizeof(float) + (size_t)4 * MT * KS_QW * sizeof(double);
 }
 
-template <bool ISO, int MT>
+template <bool ISO, int MT, bool GROUPED>
 __global__ void __launch_bounds__(KS_T, MT <= 3 ? 4 : 3)  // 4 blocks / SM up to M = 3 (registers and shared memory)
     kstar_mean_kernel(const double* __restrict__ Xn, int64_t P, int64_t p_base, const float* __restrict__ Xtf, int64_t N,
-                      int64_t Npad, int64_t n_per_block, int d, int kind, const double* __restrict__ inv_ls,
-                      const double* __restrict__ constant, const int* __restrict__ k_exp, const float* __restrict__ CAf,
+                      int64_t Npad, int64_t n_per_block, int d, int kind, int G, const int* __restrict__ cov,
+                      const double* __restrict__ inv_ls, const double* __restrict__ constant, const int* __restrict__ k_exp,
+                      const float* __restrict__ CAf,
                       int64_t plane, uint16_t* __restrict__ Kh, uint16_t* __restrict__ Kl, double* __restrict__ mpart,
                       int64_t mp_ld) {
   extern __shared__ __align__(16) float ks_smem[];
   __shared__ __align__(16) float s_il[MT * KM_D];
-  __shared__ float s_c[MT];  // c_m * 2^kexp_m: scale of the stored K_*
+  __shared__ float s_c[MT];  // c_g * 2^kexp_g: scale of the stored K_*
+  __shared__ int s_cov[MT];
   const int t = threadIdx.x, lane = t & 31, w = t >> 5;
+  const int NG = GROUPED ? G : MT;  // covariances
   float* s_x = ks_smem;  // [KS_Q][KM_D] candidate coordinates (zero padded)
-  float* s_k = ks_smem + KS_Q * KM_D + w * ks_warp_floats(MT);  // this warp's [MT][KS_B][KS_LD] kernel values
+  float* s_k = ks_smem + KS_Q * KM_D + w * ks_warp_floats(MT);  // this warp's [MT][KS_B][KS_LD] kernel values (g < G in use)
   float* s_al = s_k + MT * KS_B * KS_LD;                         // this warp's [MT][KS_C] c * alpha
   float* s_part = s_al + MT * KS_C;                              // this warp's [MT][KS_QW][4] fp32 sums of the chunk's groups
   double* s_sum = reinterpret_cast<double*>(ks_smem + KS_Q * KM_D + 4 * ks_warp_floats(MT)) + w * MT * KS_QW;
@@ -660,11 +667,12 @@ __global__ void __launch_bounds__(KS_T, MT <= 3 ? 4 : 3)  // 4 blocks / SM up to
     const int j = i % KM_D;
     s_x[i] = (p < P && j < d) ? (float)Xn[p * d + j] : 0.f;
   }
-  for (int i = t; i < MT * KM_D; i += KS_T) {
-    const int m = i / KM_D, j = i % KM_D;
-    s_il[i] = j < d ? (float)inv_ls[m * d + j] : 0.f;
+  for (int i = t; i < NG * KM_D; i += KS_T) {
+    const int g = i / KM_D, j = i % KM_D;
+    s_il[i] = j < d ? (float)inv_ls[g * d + j] : 0.f;
   }
-  if (t < MT) s_c[t] = scalbnf((float)constant[t], k_exp[t]);
+  if (t < NG) s_c[t] = scalbnf((float)constant[t], k_exp[t]);
+  if (GROUPED && t < MT) s_cov[t] = cov[t];
   __syncthreads();
   const int64_t lo = (int64_t)blockIdx.x * n_per_block;  // slice [lo, hi): multiples of KF_NS
   const int64_t hi = lo + n_per_block < Npad ? lo + n_per_block : Npad;
@@ -677,7 +685,7 @@ __global__ void __launch_bounds__(KS_T, MT <= 3 ? 4 : 3)  // 4 blocks / SM up to
   for (int64_t c0 = lo / KS_C * KS_C; c0 < hi; c0 += KS_C) {
     const int64_t n0 = c0 + 2 * lane;  // this lane's points n0, n0 + 1 (c0 + KS_C <= Npad)
     const bool mine = n0 >= lo && n0 < hi;
-    // this lane's word of the warp's first candidate row in the hi / lo planes of objective 0
+    // this lane's word of the warp's first candidate row in the hi / lo planes of covariance 0
     uint32_t* kh_c = reinterpret_cast<uint32_t*>(Kh) + ((q_warp * Npad + n0) >> 1);
     uint32_t* kl_c = reinterpret_cast<uint32_t*>(Kl) + ((q_warp * Npad + n0) >> 1);
     float2 xa[KM_D / 2], xb[KM_D / 2];
@@ -730,7 +738,7 @@ __global__ void __launch_bounds__(KS_T, MT <= 3 ? 4 : 3)  // 4 blocks / SM up to
           ra = (a0.x + a0.y) + (a1.x + a1.y);
           rb = (b0.x + b0.y) + (b1.x + b1.y);
         }
-        // one objective: kernel values of the two points, K_* hi / lo stores, unscaled values for the chains
+        // one covariance: kernel values of the two points, K_* hi / lo stores, unscaled values for the chains
         auto produce = [&](int m) {
           float2 rr;
           if (ISO) {
@@ -769,16 +777,18 @@ __global__ void __launch_bounds__(KS_T, MT <= 3 ? 4 : 3)  // 4 blocks / SM up to
         };
         if (ISO) {
 #pragma unroll
-          for (int m = 0; m < MT; ++m) produce(m);
-        } else {  // a distance pass per objective: kept rolled, so its 1/l values are not held in registers across candidates
+          for (int m = 0; m < MT; ++m)
+            if (m < NG) produce(m);
+        } else {  // a distance pass per covariance: kept rolled, so its 1/l values are not held in registers across candidates
 #pragma unroll 1
-          for (int m = 0; m < MT; ++m) produce(m);
+          for (int m = 0; m < NG; ++m) produce(m);
         }
       }
       __syncwarp();  // the batch's kernel values are in s_k
 #pragma unroll
       for (int m = 0; m < MT; ++m) {
-        const float4* kr = reinterpret_cast<const float4*>(s_k + (m * KS_B + u) * KS_LD + g * KF_NS);
+        const int cm = GROUPED ? s_cov[m] : m;
+        const float4* kr = reinterpret_cast<const float4*>(s_k + (cm * KS_B + u) * KS_LD + g * KF_NS);
         const float4* ar = reinterpret_cast<const float4*>(s_al + m * KS_C + g * KF_NS);
         float acc = 0.f;
 #pragma unroll
@@ -810,10 +820,10 @@ __global__ void __launch_bounds__(KS_T, MT <= 3 ? 4 : 3)  // 4 blocks / SM up to
   for (int m = 0; m < MT; ++m) mpart[((int64_t)blockIdx.x * MT + m) * mp_ld + q_warp + lane] = s_sum[m * KS_QW + lane];
 }
 
-// mean[p][m] = y_std * sum_n K_*[p][n] alpha[n] + y_mean from the split K_* (hi + lo = 22 bits): HBM-bound pass,
-// one warp per (objective, candidate) row, float64 accumulation in a fixed order
+// mean[p][m] = y_std * sum_n K_*[p][n] alpha[n] + y_mean from the split K_* (hi + lo = 22 bits) of covariance cov[m]:
+// HBM-bound pass, one warp per (objective, candidate) row, float64 accumulation in a fixed order
 __global__ void mean_split_kernel(const uint16_t* __restrict__ Kh, const uint16_t* __restrict__ Kl, int64_t Pc, int64_t N,
-                                  int64_t ldk, int64_t plane, int M, const int* __restrict__ k_exp,
+                                  int64_t ldk, int64_t plane, int M, const int* __restrict__ cov, const int* __restrict__ k_exp,
                                   const double* __restrict__ alpha, const double* __restrict__ ymean,
                                   const double* __restrict__ ystd, int64_t p_base, double* __restrict__ mean) {
   const int64_t w = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -821,8 +831,9 @@ __global__ void mean_split_kernel(const uint16_t* __restrict__ Kh, const uint16_
   if (w >= Pc * M) return;
   const int m = (int)(w / Pc);
   const int64_t pl = w - (int64_t)m * Pc;
-  const uint32_t* rh = reinterpret_cast<const uint32_t*>(Kh + m * plane + pl * ldk);
-  const uint32_t* rl = reinterpret_cast<const uint32_t*>(Kl + m * plane + pl * ldk);
+  const int g = cov[m];
+  const uint32_t* rh = reinterpret_cast<const uint32_t*>(Kh + g * plane + pl * ldk);
+  const uint32_t* rl = reinterpret_cast<const uint32_t*>(Kl + g * plane + pl * ldk);
   const double* a = alpha + (int64_t)m * N;
   double s = 0.0;
 #pragma unroll 8
@@ -835,7 +846,7 @@ __global__ void mean_split_kernel(const uint16_t* __restrict__ Kh, const uint16_
     if (n + 1 < N) s += (double)k1 * a[n + 1];
   }
   s = warp_sum(s);
-  if (lane == 0) mean[(p_base + pl) * M + m] = ystd[m] * scalbn(s, -k_exp[m]) + ymean[m];
+  if (lane == 0) mean[(p_base + pl) * M + m] = ystd[m] * scalbn(s, -k_exp[g]) + ymean[m];
 }
 
 // mean[p][m] = y_std * sum over the training-set slices' partial sums of K_* alpha + y_mean (fixed order)
@@ -851,15 +862,17 @@ __global__ void mean_finish_tc_kernel(const double* __restrict__ mpart, int npla
   mean[(p_base + pl) * M + m] = ystd[m] * s + ymean[m];
 }
 
-__global__ void var_finish_tc_kernel(const double* __restrict__ vnorm, int nplanes, int64_t Pc, int64_t ld, int M,
-                                     const double* __restrict__ constant, const double* __restrict__ noise,
+// objective m reads the sums of its covariance cov[m] < G and keeps its own constant, noise and y_std
+__global__ void var_finish_tc_kernel(const double* __restrict__ vnorm, int nplanes, int64_t Pc, int64_t ld, int M, int G,
+                                     const int* __restrict__ cov, const double* __restrict__ constant, const double* __restrict__ noise,
                                      const double* __restrict__ ystd, int64_t p_base, double* __restrict__ var) {
   int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= Pc * M) return;
   int64_t pl = t / M;
   int m = (int)(t - pl * M);
   double vn = 0.0;
-  for (int q = 0; q < nplanes; ++q) vn += vnorm[((int64_t)q * M + m) * ld + pl];  // partial sums of the work items, fixed order
+  const int g = cov[m];
+  for (int q = 0; q < nplanes; ++q) vn += vnorm[((int64_t)q * G + g) * ld + pl];  // partial sums of the work items, fixed order
   double v = (constant[m] + noise[m]) - vn;
   if (v < 0.0) v = 0.0;
   double sd = sqrt(v * (ystd[m] * ystd[m]));
@@ -897,20 +910,20 @@ int make_map(dmo_ctx* ctx, CUtensorMap* map, const void* base, uint64_t rows, ui
 
 int prepare_tensor_state(dmo_ctx* ctx, dmo_gp* gp) {
   if (gp->tensor_ready) return DMO_OK;
-  const int M = gp->M;
+  const int G = gp->G;
   const int64_t Npad = gp->Npad;
-  std::vector<int> kexp(M);
-  for (int m = 0; m < M; ++m) {
-    double c = gp->h_constant[m];
-    kexp[m] = (c > 0.0) ? 13 - ilogb(c) : 13;  // scaled K_* <= 2^14
+  std::vector<int> kexp(G);
+  for (int g = 0; g < G; ++g) {
+    double c = gp->h_constant[gp->h_lead[g]];
+    kexp[g] = (c > 0.0) ? 13 - ilogb(c) : 13;  // scaled K_* <= 2^14
   }
-  DMO_TRY(gp->Kexp.alloc(ctx, M));
-  DMO_CUDA(cudaMemcpyAsync(gp->Kexp.p, kexp.data(), M * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+  DMO_TRY(gp->Kexp.alloc(ctx, G));
+  DMO_CUDA(cudaMemcpyAsync(gp->Kexp.p, kexp.data(), G * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
   DMO_CUDA(cudaStreamSynchronize(ctx->stream));  // kexp is a stack vector
-  DMO_TRY(gp->Lhi.alloc(ctx, (size_t)M * Npad * Npad));
-  DMO_TRY(gp->Llo.alloc(ctx, (size_t)M * Npad * Npad));
-  DMO_TRY(gp->Lscale.alloc(ctx, (size_t)M * Npad));
-  DMO_LAUNCH(split_linv_kernel, (unsigned)(M * Npad), 256, 0, gp->Linv.p, Npad, M, gp->Kexp.p, gp->Lhi.p, gp->Llo.p,
+  DMO_TRY(gp->Lhi.alloc(ctx, (size_t)G * Npad * Npad));
+  DMO_TRY(gp->Llo.alloc(ctx, (size_t)G * Npad * Npad));
+  DMO_TRY(gp->Lscale.alloc(ctx, (size_t)G * Npad));
+  DMO_LAUNCH(split_linv_kernel, (unsigned)(G * Npad), 256, 0, gp->Linv.p, Npad, gp->Kexp.p, gp->Lhi.p, gp->Llo.p,
              gp->Lscale.p);
   DMO_CHECK_LAUNCH();
   gp->tensor_ready = true;
@@ -1012,11 +1025,11 @@ int gp_var_contract_tensor(dmo_ctx* ctx, dmo_gp* gp, const uint16_t* Kh, const u
   CUtensorMap map_kh, map_kl, map_lh, map_ll;
   DMO_TRY(make_map(ctx, &map_kh, Kh, (uint64_t)k_alloc, (uint64_t)Npad, TMV, TK, CU_TENSOR_MAP_SWIZZLE_64B));
   DMO_TRY(make_map(ctx, &map_kl, Kl, (uint64_t)k_alloc, (uint64_t)Npad, TMV, TK, CU_TENSOR_MAP_SWIZZLE_64B));
-  DMO_TRY(make_map(ctx, &map_lh, gp->Lhi.p, (uint64_t)gp->M * Npad, (uint64_t)Npad, TN, TK, CU_TENSOR_MAP_SWIZZLE_64B));
-  DMO_TRY(make_map(ctx, &map_ll, gp->Llo.p, (uint64_t)gp->M * Npad, (uint64_t)Npad, TN, TK, CU_TENSOR_MAP_SWIZZLE_64B));
+  DMO_TRY(make_map(ctx, &map_lh, gp->Lhi.p, (uint64_t)gp->G * Npad, (uint64_t)Npad, TN, TK, CU_TENSOR_MAP_SWIZZLE_64B));
+  DMO_TRY(make_map(ctx, &map_ll, gp->Llo.p, (uint64_t)gp->G * Npad, (uint64_t)Npad, TN, TK, CU_TENSOR_MAP_SWIZZLE_64B));
   DMO_CUDA(cudaFuncSetAttribute(gp_var_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GEMM_SMEM));
   GemmParams prm;
-  prm.M = gp->M;
+  prm.M = gp->G;
   prm.n_pb = (int)(Pcpad / TMV);
   prm.n_jt = (int)(Npad / TN);
   prm.n_q = gp_tensor_var_planes(Npad);
@@ -1034,7 +1047,7 @@ int gp_var_contract_tensor(dmo_ctx* ctx, dmo_gp* gp, const uint16_t* Kh, const u
 
 int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var) {
   const int64_t N = gp->N, Npad = gp->Npad;
-  const int M = gp->M, d = gp->d;
+  const int M = gp->M, G = gp->G, d = gp->d;
   DMO_REQUIRE(M <= 16, "gp_predict(tensor): at most 16 objectives per model (got %d)", M);
   DMO_REQUIRE(d <= 64, "gp_predict(tensor): at most 64 input dimensions (got %d); use DMO_GP_FP64", d);
   DMO_REQUIRE(Npad % TN == 0, "gp_predict(tensor): internal padding error");
@@ -1042,8 +1055,8 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
     return gp_mean_direct(ctx, gp, dXn, P, d_mean);  // nothing but the mean is wanted: K_* stays in registers
   DMO_TRY(prepare_tensor_state(ctx, gp));
   constexpr int64_t TMv = KM_Q;  // candidate padding: the K_* producers write 256-candidate blocks
-  // candidate chunk: K_* hi/lo (2 x M x Pc x Npad fp16) within ~6 GiB
-  int64_t Pc_max = ((int64_t)6 << 30) / ((int64_t)M * Npad * 4);
+  // candidate chunk: K_* hi/lo (2 x G x Pc x Npad fp16) within ~6 GiB
+  int64_t Pc_max = ((int64_t)6 << 30) / ((int64_t)G * Npad * 4);
   Pc_max = (Pc_max / TMv) * TMv;
   if (Pc_max < TMv) Pc_max = TMv;
   const int64_t Pc_alloc = P < Pc_max ? ceil_div(P, TMv) * TMv : Pc_max;
@@ -1051,15 +1064,15 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
   DevBuf<uint16_t> Kh, Kl;
   DevBuf<double> vnorm;
   DevBuf<int> abort_flag;
-  DMO_TRY(Kh.alloc(ctx, (size_t)M * Pc_alloc * Npad));
-  DMO_TRY(Kl.alloc(ctx, (size_t)M * Pc_alloc * Npad));
-  DMO_TRY(vnorm.alloc(ctx, (size_t)n_q * M * Pc_alloc));
+  DMO_TRY(Kh.alloc(ctx, (size_t)G * Pc_alloc * Npad));
+  DMO_TRY(Kl.alloc(ctx, (size_t)G * Pc_alloc * Npad));
+  DMO_TRY(vnorm.alloc(ctx, (size_t)n_q * G * Pc_alloc));
   DMO_TRY(abort_flag.alloc(ctx, 1));
   DMO_CUDA(cudaMemsetAsync(abort_flag.p, 0, sizeof(int), ctx->stream));
   const int64_t kplane = Pc_alloc * Npad;
   // K_* producer fused with the mean (d <= 32, M <= 6; DMO_GP_FUSED=0 keeps kstar_tensor_kernel + mean_split_kernel)
-  // (per-dimension length scales with more than two objectives keep the two-kernel route: a distance pass per objective)
-  const bool fused = d <= KM_D && M <= 6 && (gp->isotropic || M <= 2) &&
+  // (per-dimension length scales with more than two covariances keep the two-kernel route: a distance pass per covariance)
+  const bool fused = d <= KM_D && M <= 6 && (gp->isotropic || G <= 2) &&
                      !(getenv("DMO_GP_FUSED") && atoi(getenv("DMO_GP_FUSED")) == 0);
   DevBuf<double> mpart;
   if (fused) DMO_TRY(prepare_direct_state(ctx, gp));
@@ -1076,20 +1089,31 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
       const size_t smem = kstar_mean_smem(M);
       {
         ProfileScope ps_(ctx, "gp_kstar");
-#define KF_LAUNCH(ISO_, MT_)                                                                                               \
+#define KF_LAUNCH(ISO_, MT_, GR_)                                                                                          \
   do {                                                                                                                     \
-    DMO_CUDA(cudaFuncSetAttribute(kstar_mean_kernel<ISO_, MT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));  \
-    DMO_LAUNCH((kstar_mean_kernel<ISO_, MT_>), gf, KS_T, smem, dXn, P, p_base, gp->Xtf.p, N, Npad, n_per_block, d,          \
-               gp->kernel, gp->inv_ls.p, gp->constant.p, gp->Kexp.p, gp->CAf.p, kplane, Kh.p, Kl.p, mpart.p, Pcpad);         \
+    DMO_CUDA(cudaFuncSetAttribute(kstar_mean_kernel<ISO_, MT_, GR_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+    DMO_LAUNCH((kstar_mean_kernel<ISO_, MT_, GR_>), gf, KS_T, smem, dXn, P, p_base, gp->Xtf.p, N, Npad, n_per_block, d,          \
+               gp->kernel, G, gp->cov.p, gp->g_inv_ls.p, gp->g_constant.p, gp->Kexp.p, gp->CAf.p, kplane, Kh.p, Kl.p,       \
+               mpart.p, Pcpad);                                                                                            \
   } while (0)
-#define KF_SWITCH(ISO_)                  \
-  switch (M) {                           \
-    case 1: KF_LAUNCH(ISO_, 1); break;   \
-    case 2: KF_LAUNCH(ISO_, 2); break;   \
-    case 3: KF_LAUNCH(ISO_, 3); break;   \
-    case 4: KF_LAUNCH(ISO_, 4); break;   \
-    case 5: KF_LAUNCH(ISO_, 5); break;   \
-    default: KF_LAUNCH(ISO_, 6); break;  \
+#define KF_SWITCH(ISO_)                                         \
+  if (G < M) {                                                  \
+    switch (M) { /* M >= 2 */                                   \
+      case 2: KF_LAUNCH(ISO_, 2, true); break;                  \
+      case 3: KF_LAUNCH(ISO_, 3, true); break;                  \
+      case 4: KF_LAUNCH(ISO_, 4, true); break;                  \
+      case 5: KF_LAUNCH(ISO_, 5, true); break;                  \
+      default: KF_LAUNCH(ISO_, 6, true); break;                 \
+    }                                                           \
+  } else {                                                      \
+    switch (M) {                                                \
+      case 1: KF_LAUNCH(ISO_, 1, false); break;                 \
+      case 2: KF_LAUNCH(ISO_, 2, false); break;                 \
+      case 3: KF_LAUNCH(ISO_, 3, false); break;                 \
+      case 4: KF_LAUNCH(ISO_, 4, false); break;                 \
+      case 5: KF_LAUNCH(ISO_, 5, false); break;                 \
+      default: KF_LAUNCH(ISO_, 6, false); break;                \
+    }                                                           \
   }
         if (gp->isotropic) {
           KF_SWITCH(true)
@@ -1105,11 +1129,11 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
       {
         ProfileScope ps_(ctx, "gp_kstar");
         const int dmax = d <= 32 ? 32 : 64;
-        size_t smem = (size_t)(KT_TP * dmax + M * dmax + M) * sizeof(float);
+        size_t smem = (size_t)(KT_TP * dmax + G * dmax + G) * sizeof(float);
         dim3 gk((unsigned)(Npad / (2 * KT_TN)), (unsigned)ceil_div(Pcpad, KT_TP));
 #define KSTAR_LAUNCH(ISO_, DM_)                                                                                          \
-  DMO_LAUNCH((kstar_tensor_kernel<ISO_, DM_>), gk, KT_TN, smem, dXn, P, p_base, Pcpad, gp->Xt.p, N, d, M, gp->kernel, \
-             gp->inv_ls.p, gp->constant.p, gp->Kexp.p, Npad, kplane, Kh.p, Kl.p)
+  DMO_LAUNCH((kstar_tensor_kernel<ISO_, DM_>), gk, KT_TN, smem, dXn, P, p_base, Pcpad, gp->Xt.p, N, d, G, gp->kernel, \
+             gp->g_inv_ls.p, gp->g_constant.p, gp->Kexp.p, Npad, kplane, Kh.p, Kl.p)
         if (gp->isotropic) {
           if (d <= 32)
             KSTAR_LAUNCH(true, 32);
@@ -1126,16 +1150,16 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
       {
         ProfileScope ps_(ctx, "gp_mean");
         DMO_LAUNCH(mean_split_kernel, (unsigned)ceil_div(Pc * M * 32, 256), 256, 0, Kh.p, Kl.p, Pc, N, Npad, kplane, M,
-                   gp->Kexp.p, gp->alpha.p, gp->ymean.p, gp->ystd.p, p_base, d_mean);
+                   gp->cov.p, gp->Kexp.p, gp->alpha.p, gp->ymean.p, gp->ystd.p, p_base, d_mean);
       }
     }
     if (d_var) {
       {
         ProfileScope ps_(ctx, "gp_var");
-        DMO_TRY(gp_var_contract_tensor(ctx, gp, Kh.p, Kl.p, M * Pc_alloc, Pc_alloc, Pcpad, vnorm.p, Pc_alloc, abort_flag.p));
+        DMO_TRY(gp_var_contract_tensor(ctx, gp, Kh.p, Kl.p, G * Pc_alloc, Pc_alloc, Pcpad, vnorm.p, Pc_alloc, abort_flag.p));
       }
-      DMO_LAUNCH(var_finish_tc_kernel, (unsigned)ceil_div(Pc * M, 256), 256, 0, vnorm.p, n_q, Pc, Pc_alloc, M,
-                 gp->constant.p, gp->noise.p, gp->ystd.p, p_base, d_var);
+      DMO_LAUNCH(var_finish_tc_kernel, (unsigned)ceil_div(Pc * M, 256), 256, 0, vnorm.p, n_q, Pc, Pc_alloc, M, G,
+                 gp->cov.p, gp->constant.p, gp->noise.p, gp->ystd.p, p_base, d_var);
     }
   }
   DMO_CHECK_LAUNCH();

@@ -224,6 +224,12 @@ int dmo_gp_predict(dmo_ctx* ctx, dmo_gp* gp, const double* X, int64_t P, double*
  * (= P when the whole call ran in float64).  Any output pointer may be NULL. */
 int dmo_gp_auto_info(dmo_ctx* ctx, dmo_gp* gp, int* mean_tensor, int* var_tensor, double* mean_err,
                      double* var_err, double* theta, int64_t* last_refined);
+/* Objectives that share a posterior covariance: dmo_gp_create puts objective m in the group of an earlier
+ * objective l when their constant, length scales and uploaded factor planes are bitwise equal (noise may differ).
+ * Each group's L^-1, K_* and variance contraction are computed once and the variance is scaled per objective.
+ * n_groups receives the number of groups G; group_of (M,) host array, may be NULL, receives each objective's
+ * group, numbered 0 .. G-1 in order of first appearance. */
+int dmo_gp_covariance_groups(dmo_ctx* ctx, dmo_gp* gp, int* n_groups, int* group_of);
 
 /* ---- A19: multitask exact-GP posterior (MEGP_Matern predict) -------------------
  * replaces model_gpytorch.MEGP_Matern.predict (dmosopt/model_gpytorch.py:1872-1919; model :510-571): one

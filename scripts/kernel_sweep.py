@@ -41,7 +41,11 @@ def main():
 
 
 def gp_sweep():
-    """GP posterior at the BASELINE shape: fp64 vs tensor path, accuracy and time."""
+    """GP posterior at the BASELINE shape: fp64 vs tensor path, accuracy and time, for two models: the reference's
+    fixed initial theta for every objective (one shared covariance, as bench.py's model) and three distinct constants
+    (1.0, 1.5, 2.0: three covariances).  The executed rate of the variance contraction counts the MMAs issued:
+    2 N^2 G flop per candidate for G covariances, times 1.59 for the split-fp16 products over the lower triangle plus the
+    diagonal blocks (DESIGN 4.1)."""
     L.context()
     rng = np.random.default_rng(1)
     N, d, M, P = 4096, 30, 3, 65536
@@ -49,30 +53,38 @@ def gp_sweep():
 
     Xtr = rng.random((N, d))
     Ytr = np.column_stack([np.sin(3 * Xtr[:, :4].sum(axis=1) + k) + Xtr[:, 4 + k] ** 2 for k in range(M)])
-    st = ogp.fit_fixed(Xtr, Ytr, np.zeros(d), np.ones(d), 1.0, 0.5, 1e-6)
-    h = L.GPHandle(st.X_train, np.stack([o.alpha for o in st.objectives]), np.stack([o.L for o in st.objectives]), [o.constant for o in st.objectives],
-                   [np.full(d, 0.5)] * M, [o.noise for o in st.objectives], [o.y_mean for o in st.objectives], [o.y_std for o in st.objectives],
-                   np.zeros(d), np.ones(d))
     X = rng.random((P, d))
     Xd = L.DeviceArray((P, d)).upload(X)
     md, vd = L.DeviceArray((P, M)), L.DeviceArray((P, M))
     lib, ctx = L.load_library(), L.context()
-    prior = np.array([(o.constant + o.noise) * o.y_std**2 for o in st.objectives])
-    ref = None
-    for name, prec in (("fp64", L.GP_FP64), ("tensor", L.GP_TENSOR)):
-        L.profile_enable(True)
-        ms = timed(lambda: L._check(lib.dmo_gp_predict(ctx, h._h, Xd.ptr, P, md.ptr, vd.ptr, prec), "gp"), reps=2)
-        rep = L.profile_report()
-        L.profile_enable(False)
-        mean, var = md.download(), vd.download()
-        if ref is None:
-            ref = (mean, var)
-            err = ""
-        else:
-            err = f" | vs fp64: var err/prior {np.max(np.abs(var - ref[1]) / prior):.2e}, mean err {np.max(np.abs(mean - ref[0])):.2e}"
-        parts = ", ".join(f"{k} {v[0] / v[1]:.3f}" for k, v in rep.items())
-        print(f"gp {name}: total {ms:.3f} ms [{parts}]{err}", flush=True)
-    kstar_sweep(lib, ctx, h, Xd, md, vd, P, N, M)
+    print(device_line(), flush=True)
+    for label, consts in (("shared theta", [1.0] * M), ("distinct constants", [1.0, 1.5, 2.0])):
+        st = ogp.fit_fixed(Xtr, Ytr, np.zeros(d), np.ones(d), consts, 0.5, 1e-6)
+        h = L.GPHandle(st.X_train, np.stack([o.alpha for o in st.objectives]), np.stack([o.L for o in st.objectives]), [o.constant for o in st.objectives],
+                       [np.full(d, 0.5)] * M, [o.noise for o in st.objectives], [o.y_mean for o in st.objectives], [o.y_std for o in st.objectives],
+                       np.zeros(d), np.ones(d))
+        G, group_of = h.covariance_groups()
+        print(f"== model: {label}, constants {consts}: covariance_groups() = ({G}, {group_of})", flush=True)
+        prior = np.array([(o.constant + o.noise) * o.y_std**2 for o in st.objectives])
+        ref = None
+        for name, prec in (("fp64", L.GP_FP64), ("tensor", L.GP_TENSOR)):
+            L.profile_enable(True)
+            ms = timed(lambda: L._check(lib.dmo_gp_predict(ctx, h._h, Xd.ptr, P, md.ptr, vd.ptr, prec), "gp"), reps=2)
+            rep = L.profile_report()
+            L.profile_enable(False)
+            mean, var = md.download(), vd.download()
+            if ref is None:
+                ref = (mean, var)
+                err = ""
+            else:
+                tv = rep["gp_var"][0] / rep["gp_var"][1]
+                flop = 2.0 * N * N * G * P * 1.59
+                err = (f" | vs fp64: var err/prior {np.max(np.abs(var - ref[1]) / prior):.2e}, mean err {np.max(np.abs(mean - ref[0])):.2e}"
+                       f" | contraction executes {flop:.3e} flop: {flop / tv / 1e9:.0f} TFLOP/s")
+            parts = ", ".join(f"{k} {v[0] / v[1]:.3f}" for k, v in rep.items())
+            print(f"gp {name}: total {ms:.3f} ms [{parts}]{err}", flush=True)
+        kstar_sweep(lib, ctx, h, Xd, md, vd, P, N, G)
+        h.close()
 
 
 def device_line():
@@ -104,14 +116,14 @@ def write_floor_ms(nbytes, reps=5):
     return best
 
 
-def kstar_sweep(lib, ctx, h, Xd, md, vd, P, N, M):
+def kstar_sweep(lib, ctx, h, Xd, md, vd, P, N, G):
     """K_* producer of the tensor predict, both routes (DMO_GP_FUSED=1: K_* and the mean from one kernel; 0: K_* kernel
-    then the mean read back from K_*): time, bytes of K_* written (fp16 hi + lo, M planes of Pcpad x Npad) and the
-    achieved rate, next to a write-only floor over the same bytes measured in the same process."""
+    then the mean read back from K_*): time, bytes of K_* written (fp16 hi + lo, one plane of Pcpad x Npad per covariance:
+    4 G Pcpad Npad bytes) and the achieved rate, next to a write-only floor over the same bytes measured in the same
+    process."""
     Npad = -(-N // 256) * 256
     Pcpad = -(-P // 256) * 256
-    kbytes = 2 * 2 * M * Pcpad * Npad
-    print(device_line(), flush=True)
+    kbytes = 4 * G * Pcpad * Npad
     floor = write_floor_ms(kbytes)
     print(f"write-only floor (one store kernel over {kbytes / 1e9:.3f} GB): {floor:.3f} ms = {kbytes / floor / 1e6:.0f} GB/s", flush=True)
     saved = os.environ.get("DMO_GP_FUSED")
@@ -164,7 +176,8 @@ def mtgp_sweep():
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
     print(f"device: {torch.cuda.get_device_properties(0).name}; nvidia-smi: {q.stdout.strip() or q.stderr.strip()}", flush=True)
     out = {}
-    runs = (("GPR_Matern tensor", lambda: lib.dmo_gp_predict(ctx, gpr._h, Xd.ptr, P, md.ptr, vd.ptr, L.GP_TENSOR), M * P * Npad * 4),
+    G = gpr.covariance_groups()[0]  # one K_* plane per distinct covariance
+    runs = (("GPR_Matern tensor", lambda: lib.dmo_gp_predict(ctx, gpr._h, Xd.ptr, P, md.ptr, vd.ptr, L.GP_TENSOR), G * P * Npad * 4),
             ("MEGP_Matern tensor", lambda: lib.dmo_mtgp_predict(ctx, mt._h, Xd.ptr, P, md.ptr, vd.ptr, L.GP_TENSOR), P * Npad * 4),
             ("MEGP_Matern fp64", lambda: lib.dmo_mtgp_predict(ctx, mt._h, Xd.ptr, P, md.ptr, vd.ptr, L.GP_FP64), P * Npad * 8))
     for name, fn, kbytes in runs:
