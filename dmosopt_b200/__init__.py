@@ -4,6 +4,8 @@ Plugin import paths (dmosopt resolves them with ``config.import_object_by_path``
 
     optimizer_name         = "dmosopt_b200.NSGA2" | "dmosopt_b200.AGEMOEA" | "dmosopt_b200.SMPSO" | "dmosopt_b200.CMAES" | "dmosopt_b200.TRS"
     surrogate_method_name  = "dmosopt_b200.GPR_Matern" | "dmosopt_b200.GPR_RBF"
+                             | "dmosopt_b200.SVGP_Matern" | "dmosopt_b200.VGP_Matern" | "dmosopt_b200.SIV_Matern"
+                             | "dmosopt_b200.SPV_Matern" | "dmosopt_b200.CRV_Matern"
 
 ``dmosopt_b200.install()`` additionally routes the controller-side helpers that dmosopt calls on its own modules
 (resample / get_best duplicates + sort, per-generation termination hypervolume) to the same kernels.
@@ -17,6 +19,7 @@ from .MOEA import MOEA as MOEABase  # noqa: F401
 from .MOEA import Struct  # noqa: F401
 from .NSGA2 import NSGA2  # noqa: F401
 from .model import GPR_Matern, GPR_RBF, Model  # noqa: F401
+from .model_gpflow import CRV_Matern, SIV_Matern, SPV_Matern, SVGP_Matern, VGP_Matern  # noqa: F401
 
 from .AGEMOEA import AGEMOEA  # noqa: F401
 from .CMAES import CMAES  # noqa: F401

@@ -76,6 +76,12 @@ _SIGNATURES = {
                                  ctypes.POINTER(_vp)]),
     "dmo_mtgp_predict": (_c_int, [_vp, _vp, _vp, _c_i64, _vp, _vp, _c_int]),
     "dmo_mtgp_destroy": (_c_int, [_vp, _vp]),
+    "dmo_svgp_create": (_c_int, [_vp, _c_int, _c_int, _c_i64, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _c_dbl, _vp, _vp, _vp, _vp, _vp,
+                                 ctypes.POINTER(_vp)]),
+    "dmo_svgp_predict": (_c_int, [_vp, _vp, _vp, _c_i64, _vp, _vp, _c_int]),
+    "dmo_svgp_groups": (_c_int, [_vp, _vp, ctypes.POINTER(_c_int), ctypes.POINTER(_c_int)]),
+    "dmo_svgp_destroy": (_c_int, [_vp, _vp]),
+    "dmo_svgp_optimal_q": (_c_int, [_vp, _c_i64, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _c_dbl, _c_int, _vp, _vp]),
     "dmo_mtgp_lml_grad": (_c_int, [_vp, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dmo_gp_lml_grad": (_c_int, [_vp, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dmo_nsga2_step": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_i64, _c_int, _c_int, _c_dbl, _c_dbl, _c_dbl, _vp, _vp, _vp, _vp, _c_u64, _c_u64,
@@ -848,6 +854,84 @@ class MTGPHandle:
             self.close()
         except Exception:
             pass
+
+
+class SVGPHandle:
+    """Owns a dmo_svgp object: the whitened variational GP posterior of L latent GPs (inducing points Zpts (L,Z,d),
+    Matern-5/2 ARD kernels, q_mu (L,Z), lower-triangular q_sqrt (L,Z,Z)) mixed into M outputs by W (M,L) (None: the
+    identity), resident in HBM.  ``y_var_scale`` (M,) multiplies the variance (None: y_std**2)."""
+
+    def __init__(self, Zpts, variance, length_scale, q_mu, q_sqrt, y_mean, y_std, xlb, xrng, W=None, jitter=1e-2, y_var_scale=None):
+        lib = load_library()
+        Zp = _f64(Zpts)
+        if Zp.ndim != 3:
+            raise DmoError(f"dmo_svgp_create: Zpts must be (L, Z, d), got shape {Zp.shape}")
+        L, Z, d = Zp.shape
+        Wm = None if W is None else _f64(W)
+        if Wm is not None and (Wm.ndim != 2 or Wm.shape[1] != L):
+            raise DmoError(f"dmo_svgp_create: W must be (M, {L}), got shape {Wm.shape}")
+        M = L if Wm is None else Wm.shape[0]
+        s, ls, qm, qs = _f64(variance), _f64(length_scale), _f64(q_mu), _f64(q_sqrt)
+        ym, ys, lb, rg = _f64(y_mean), _f64(y_std), _f64(xlb), _f64(xrng)
+        vs = None if y_var_scale is None else _f64(y_var_scale)
+        for name, a, shape in (("variance", s, (L,)), ("length_scale", ls, (L, d)), ("q_mu", qm, (L, Z)), ("q_sqrt", qs, (L, Z, Z)),
+                               ("y_mean", ym, (M,)), ("y_std", ys, (M,)), ("xlb", lb, (d,)), ("xrng", rg, (d,)),
+                               ("y_var_scale", vs, (M,))):
+            if a is not None and a.shape != shape:
+                raise DmoError(f"dmo_svgp_create: {name} must have shape {shape}, got {a.shape}")
+        self.L, self.M, self.Z, self.d = L, M, Z, d
+        h = _vp()
+        _check(
+            lib.dmo_svgp_create(context(), L, M, Z, d, _ptr(Zp), _ptr(s), _ptr(ls), _ptr(qm), _ptr(qs), _ptr(Wm), float(jitter), _ptr(ym),
+                                _ptr(ys), _ptr(vs), _ptr(lb), _ptr(rg), ctypes.byref(h)),
+            "dmo_svgp_create",
+        )
+        self._h = h
+
+    def predict(self, X, return_var=True, precision=GP_FP64):
+        X = _f64(X)
+        if X.ndim == 1:
+            X = X.reshape(1, -1)
+        P = X.shape[0]
+        mean = pinned_empty((P, self.M), np.float64)
+        var = pinned_empty((P, self.M), np.float64) if return_var else None
+        _check(load_library().dmo_svgp_predict(context(), self._h, _in(X), P, _ptr(mean), _ptr(var), int(precision)), "dmo_svgp_predict")
+        return mean, var
+
+    def groups(self):
+        """(distinct K_* planes, operator planes) that one predict produces and contracts."""
+        g, p = _c_int(0), _c_int(0)
+        _check(load_library().dmo_svgp_groups(context(), self._h, ctypes.byref(g), ctypes.byref(p)), "dmo_svgp_groups")
+        return int(g.value), int(p.value)
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and _lib is not None and _ctx is not None:
+            _lib.dmo_svgp_destroy(_ctx, self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def svgp_optimal_q(X, y, Zpts, variance, length_scale, noise, jitter=1e-2, inducing_is_data=False):
+    """The optimal whitened q for a Gaussian likelihood (dmo_svgp_optimal_q): X (N,d), y (L,N), Zpts (L,Z,d), variance
+    (L,), length_scale (L,d), noise (L,) -> q_mu (L,Z), lower-triangular q_sqrt (L,Z,Z).  inducing_is_data: GPflow's VGP
+    (Z = X, f(X) = Lz v; Zpts is ignored and may be None)."""
+    X = _f64(X)
+    N, d = X.shape
+    L = len(np.atleast_1d(variance))
+    Zp = None if inducing_is_data else _f64(Zpts)
+    Z = N if inducing_is_data else Zp.shape[1]
+    y = _f64(y).reshape(L, N)
+    s, ls, nz = _f64(variance).reshape(L), _f64(length_scale).reshape(L, d), _f64(noise).reshape(L)
+    q_mu = np.empty((L, Z), np.float64)
+    q_sqrt = np.empty((L, Z, Z), np.float64)
+    _check(load_library().dmo_svgp_optimal_q(context(), N, Z, d, L, _ptr(X), _ptr(y), _ptr(Zp), _ptr(s), _ptr(ls), _ptr(nz), float(jitter),
+                                             int(bool(inducing_is_data)), _ptr(q_mu), _ptr(q_sqrt)), "dmo_svgp_optimal_q")
+    return q_mu, q_sqrt
 
 
 # --------------------------------------------------------------------------- A16/A17

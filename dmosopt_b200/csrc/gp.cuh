@@ -57,6 +57,10 @@ int gp_linv_from_factor_batched(dmo_ctx* ctx, const double* L, int64_t ldl, int6
 // nbat independent exact-GP factorisations in one pass of the blocked Cholesky (gp_fit.cu; see its definition)
 int gp_fit_batched(dmo_ctx* ctx, int64_t N, int d, int nbat, int kernel, const double* X, const double* inv_ls, const double* constant,
                    const double* diag_add, const double* y, double* A, int64_t ld, int* info, double* work, double* alpha, double* lml);
+// in-place lower Cholesky factorisation of nbat symmetric matrices A + b * ld^2 (lower triangles read, row-major, ld a
+// multiple of 64; pad with an identity tail); info[b] (zeroed by the caller) receives a non-positive pivot + 1.  Not
+// synchronised.
+int gp_potrf_batched(dmo_ctx* ctx, double* A, int64_t ld, int nbat, int* info);
 // float64 variance contraction (var_kernel) over the gp->G covariances: vnorm[z][g][p] = partial sums over the row
 // blocks z (mod nsplit) of ||Linv_g Ks_g[p]||^2, Ks_g = Ks + g * kplane with rows of gp->Npad doubles (kplane = 0: one
 // K_* plane for every g); Pcpad is a multiple of GP_F64_TILE
@@ -91,3 +95,16 @@ struct MtBlocks {
 int mtgp_blocks_fit(dmo_ctx* ctx, const char* who, int64_t N, int d, int M, const double* X_train, const double* Y,
                     const double* length_scale, const double* B, const double* D, const double* weight, const double* bias,
                     MtBlocks& mb, double* alpha_out);
+
+// The multitask producers (gp_multitask.cu), also used by the variational posterior (gp_variational.cu).
+// xs = ((X - xlb) / xrg) * inv_ls, (P, d)
+int mt_scale_inputs(dmo_ctx* ctx, const double* X, int64_t P, int d, const double* xlb, const double* xrg, const double* inv_ls,
+                    double* xs);
+// training points per producer block: mpart has Npad / mt_kstar_span(tensor) row-block planes
+int64_t mt_kstar_span(bool tensor);
+// One unit-scale Matern-5/2 K_* plane k(xs_p, XtT[:, n]) for the candidates p_base + [0, Pcpad) (float64 Ks, or fp16 hi / lo
+// Kh / Kl scaled by 2^k_exp[0]; NULL: not written) and the partial sums mpart[z][j][p] of k' A_j, j < M <= MT_MAX.
+// tensor: d <= 64.
+int mt_kstar_produce(dmo_ctx* ctx, bool tensor, const double* xs, int64_t P, int64_t p_base, int64_t Pcpad, const double* XtT, int64_t N,
+                     int64_t Npad, int d, int M, const double* A, const int* k_exp, double* Ks, uint16_t* Kh, uint16_t* Kl,
+                     double* mpart, int64_t mp_ld);

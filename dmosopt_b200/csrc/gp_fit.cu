@@ -312,12 +312,20 @@ __global__ void extract_lower_kernel(const double* __restrict__ A, int64_t ld, i
 // All pointers are device pointers; nothing is synchronised.
 int gp_fit_batched(dmo_ctx* ctx, int64_t N, int d, int nbat, int kernel, const double* X, const double* inv_ls, const double* constant,
                    const double* diag_add, const double* y, double* A, int64_t ld, int* info, double* work, double* alpha, double* lml) {
-  const int64_t nb = ld / CB, sA = ld * ld;
-  DMO_CUDA(cudaFuncSetAttribute(trsm_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PAIR_SMEM));
-  DMO_CUDA(cudaFuncSetAttribute(syrk_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PAIR_SMEM));
+  const int64_t sA = ld * ld;
   dim3 kg((unsigned)ceil_div(ld, 32), (unsigned)ceil_div(ld, 32), (unsigned)nbat);
   DMO_LAUNCH(kernel_matrix_kernel, kg, 256, (size_t)64 * (d + 1) * sizeof(double), X, N, d, kernel, inv_ls, constant, diag_add, y, ld,
              A, sA);
+  DMO_TRY(gp_potrf_batched(ctx, A, ld, nbat, info));
+  if (lml) DMO_LAUNCH(finish_fit_kernel, (unsigned)nbat, SV_T, 0, A, ld, sA, N, work, alpha, lml, alpha ? 1 : 0);
+  return DMO_OK;
+}
+
+int gp_potrf_batched(dmo_ctx* ctx, double* A, int64_t ld, int nbat, int* info) {
+  const int64_t nb = ld / CB, sA = ld * ld;
+  DMO_REQUIRE(ld % CB == 0, "gp_potrf_batched: ld %lld is not a multiple of %d", (long long)ld, CB);
+  DMO_CUDA(cudaFuncSetAttribute(trsm_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PAIR_SMEM));
+  DMO_CUDA(cudaFuncSetAttribute(syrk_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PAIR_SMEM));
   for (int64_t k = 0; k < nb; ++k) {
     const int64_t k0 = k * CB;
     DMO_LAUNCH(potrf_diag_kernel, (unsigned)nbat, 256, 0, A, ld, sA, k0, info);
@@ -327,7 +335,6 @@ int gp_fit_batched(dmo_ctx* ctx, int64_t N, int d, int nbat, int kernel, const d
       DMO_LAUNCH(syrk_tile_kernel, dim3((unsigned)((int64_t)nrem * (nrem + 1) / 2), (unsigned)nbat), 256, PAIR_SMEM, A, ld, sA, k0, nrem);
     }
   }
-  if (lml) DMO_LAUNCH(finish_fit_kernel, (unsigned)nbat, SV_T, 0, A, ld, sA, N, work, alpha, lml, alpha ? 1 : 0);
   return DMO_OK;
 }
 

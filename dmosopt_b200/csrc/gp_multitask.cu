@@ -298,6 +298,32 @@ int upload(dmo_ctx* ctx, DevBuf<T>& dst, const std::vector<T>& src) {
 
 }  // namespace
 
+int mt_scale_inputs(dmo_ctx* ctx, const double* X, int64_t P, int d, const double* xlb, const double* xrg, const double* inv_ls,
+                    double* xs) {
+  DMO_LAUNCH(mt_scale_inputs_kernel, (unsigned)ceil_div(P * d, 256), 256, 0, X, P, d, xlb, xrg, inv_ls, xs);
+  return DMO_OK;
+}
+
+int64_t mt_kstar_span(bool tensor) { return tensor ? 2 * PT_TN : PF_TN; }
+
+int mt_kstar_produce(dmo_ctx* ctx, bool tensor, const double* xs, int64_t P, int64_t p_base, int64_t Pcpad, const double* XtT, int64_t N,
+                     int64_t Npad, int d, int M, const double* A, const int* k_exp, double* Ks, uint16_t* Kh, uint16_t* Kl,
+                     double* mpart, int64_t mp_ld) {
+  const unsigned n_mp = (unsigned)(Npad / mt_kstar_span(tensor));
+  if (tensor) {
+    dim3 g(n_mp, (unsigned)(Pcpad / PT_TP));
+    if (d <= 32)
+      DMO_LAUNCH(mt_kstar_tensor_kernel<32>, g, PT_TN, 0, xs, P, p_base, XtT, N, Npad, d, M, A, k_exp, Kh, Kl, mpart, mp_ld);
+    else
+      DMO_LAUNCH(mt_kstar_tensor_kernel<64>, g, PT_TN, 0, xs, P, p_base, XtT, N, Npad, d, M, A, k_exp, Kh, Kl, mpart, mp_ld);
+  } else {
+    dim3 g(n_mp, (unsigned)(Pcpad / PF_TP));
+    DMO_LAUNCH(mt_kstar_f64_kernel, g, PF_TN, (size_t)PF_TP * d * sizeof(double), xs, P, p_base, XtT, N, Npad, d, M, A, Ks, mpart,
+               mp_ld);
+  }
+  return DMO_OK;
+}
+
 int mtgp_blocks_fit(dmo_ctx* ctx, const char* who, int64_t N, int d, int M, const double* X_train, const double* Y,
                     const double* length_scale, const double* B, const double* D, const double* weight, const double* bias,
                     MtBlocks& mb, double* alpha_out) {
@@ -496,7 +522,7 @@ int dmo_mtgp_predict(dmo_ctx* ctx, dmo_mtgp* mt, const double* X, int64_t P, dou
   const bool want_var = ov.d != nullptr;
   DevBuf<double> xs;
   DMO_TRY(xs.alloc(ctx, (size_t)P * d));
-  DMO_LAUNCH(mt_scale_inputs_kernel, (unsigned)ceil_div(P * d, 256), 256, 0, x.d, P, d, mt->xlb.p, mt->xrg.p, mt->inv_ls.p, xs.p);
+  DMO_TRY(mt_scale_inputs(ctx, x.d, P, d, mt->xlb.p, mt->xrg.p, mt->inv_ls.p, xs.p));
   if (tensor && want_var) DMO_TRY(gp_prepare_tensor(ctx, gp));
   // candidate chunk: the one K_* plane (fp16 hi + lo, or float64) within ~6 GiB; the producer grid's y extent stays < 2^16
   const int64_t tile = tensor ? GP_TC_TILE : GP_F64_TILE;
@@ -505,8 +531,7 @@ int dmo_mtgp_predict(dmo_ctx* ctx, dmo_mtgp* mt, const double* X, int64_t P, dou
   Pc_max = (Pc_max / tile) * tile;
   if (Pc_max < tile) Pc_max = tile;
   const int64_t Pc_alloc = P < Pc_max ? ceil_div(P, tile) * tile : Pc_max;
-  const int64_t n_tn = tensor ? 2 * PT_TN : PF_TN;  // training points per producer block
-  const int n_mp = (int)(Npad / n_tn);
+  const int n_mp = (int)(Npad / mt_kstar_span(tensor));
   int n_vp = 0;
   if (want_var) {
     if (tensor) {
@@ -537,19 +562,8 @@ int dmo_mtgp_predict(dmo_ctx* ctx, dmo_mtgp* mt, const double* X, int64_t P, dou
     const int64_t Pcpad = ceil_div(Pc, tile) * tile;
     {
       ProfileScope ps(ctx, "mtgp_kstar");
-      if (tensor) {
-        dim3 g((unsigned)n_mp, (unsigned)(Pcpad / PT_TP));
-        if (d <= 32)
-          DMO_LAUNCH(mt_kstar_tensor_kernel<32>, g, PT_TN, 0, xs.p, P, p_base, mt->XtT.p, N, Npad, d, M, mt->A.p,
-                     want_var ? gp->Kexp.p : nullptr, Kh.p, Kl.p, mpart.p, Pc_alloc);
-        else
-          DMO_LAUNCH(mt_kstar_tensor_kernel<64>, g, PT_TN, 0, xs.p, P, p_base, mt->XtT.p, N, Npad, d, M, mt->A.p,
-                     want_var ? gp->Kexp.p : nullptr, Kh.p, Kl.p, mpart.p, Pc_alloc);
-      } else {
-        dim3 g((unsigned)n_mp, (unsigned)(Pcpad / PF_TP));
-        DMO_LAUNCH(mt_kstar_f64_kernel, g, PF_TN, (size_t)PF_TP * d * sizeof(double), xs.p, P, p_base, mt->XtT.p, N, Npad, d, M,
-                   mt->A.p, Ks.p, mpart.p, Pc_alloc);
-      }
+      DMO_TRY(mt_kstar_produce(ctx, tensor, xs.p, P, p_base, Pcpad, mt->XtT.p, N, Npad, d, M, mt->A.p,
+                               tensor && want_var ? gp->Kexp.p : nullptr, Ks.p, Kh.p, Kl.p, mpart.p, Pc_alloc));
     }
     if (want_var) {
       ProfileScope ps(ctx, "mtgp_var");

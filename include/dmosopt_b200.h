@@ -59,6 +59,7 @@ extern "C" {
 typedef struct dmo_ctx dmo_ctx;
 typedef struct dmo_gp dmo_gp;
 typedef struct dmo_mtgp dmo_mtgp;
+typedef struct dmo_svgp dmo_svgp;
 
 /* ---- context ----------------------------------------------------------- */
 int dmo_version(void);
@@ -272,6 +273,39 @@ int dmo_gp_lml_grad(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_train
                     const double* length_scale, const double* outputscale, const double* noise, const double* weight,
                     const double* bias, double* lml_out, double* g_length_scale, double* g_outputscale,
                     double* g_noise, double* g_weight, double* g_bias);
+
+/* ---- variational GP posterior (SVGP_Matern / VGP_Matern / SIV_Matern / SPV_Matern / CRV_Matern predict) --------
+ * replaces predict_f of the GPflow posteriors behind dmosopt/model.py's variational surrogates (:290-318, 509-537,
+ * 730-757, 953-981, 1143-1172): per latent GP l a whitened variational posterior q(v) = N(q_mu_l, q_sqrt_l q_sqrt_l')
+ * over inducing points Z_l with kernel variance_l Matern52(. / length_scale_l) (ARD), zero mean, and jitter added to
+ * K(Z, Z); the variance is that of the latent f (no likelihood noise) and is not clamped.
+ * dmo_svgp_create: 1 <= L, M <= 8 latents and outputs, 1 <= Z <= 8192 inducing points per latent, 1 <= d <= 90;
+ *   Zpts (L,Z,d) normalised inputs; variance (L,) > 0; length_scale (L,d) > 0; q_mu (L,Z); q_sqrt (L,Z,Z) lower
+ *   triangular (a non-zero above the diagonal is DMO_ERR_ARG), any rank; W (M,L) output mixing (NULL: identity, M == L);
+ *   y_mean, y_std (M,); y_var_scale (M,) multiplies the variance (NULL: y_std^2); xlb, xrng (d,) with xrng > 0:
+ *   x_n = (x - xlb) / xrng.  Latents with bitwise equal Z planes and length scales share one K_* plane per predict.
+ * dmo_svgp_predict: X (P,d) raw inputs -> mean (P,M) = y_std (W g_mean) + y_mean, var (P,M) = ((W o W) g_var) y_var_scale
+ *   (var may be NULL); precision DMO_GP_FP64 or DMO_GP_TENSOR (d <= 64); DMO_GP_AUTO is not offered (DMO_ERR_ARG).
+ * dmo_svgp_groups: the number of distinct K_* planes and of operator planes the variance contracts per candidate.
+ * dmo_svgp_optimal_q: the closed-form optimum of q for a Gaussian likelihood (Titsias 2009) in whitened coordinates, per
+ *   latent: A = Lz^-1 K(Z, X), B = I + A A' / noise, q_mu = B^-1 A y / noise, q_sqrt q_sqrt' = B^-1 (q_sqrt lower
+ *   triangular).  X (N,d) normalised inputs, y (L,N) normalised targets, Zpts / variance / length_scale as above, noise
+ *   (L,) > 0; outputs q_mu (L,Z), q_sqrt (L,Z,Z).  Not defined for coupled latents (CRV).
+ *   inducing_is_data != 0 (GPflow's VGP): the inducing points are X itself (Zpts ignored, may be NULL; Z == N) and
+ *   f(X) = Lz v, so A = Lz' -- the data term sees K(X, X) + jitter I, and the posterior is the exact GP with noise
+ *   noise + jitter.  With inducing_is_data = 0 and Z = X (SVGP with every point) the data term sees K(X, X) without the
+ *   jitter; that posterior equals the exact GP only as the jitter goes to 0.
+ *   Cost: dmo_svgp_create runs a Householder QR per latent (2 (Z - 1) launches, ~4/3 Z^3 flop) whatever q is. */
+int dmo_svgp_create(dmo_ctx* ctx, int L, int M, int64_t Z, int d, const double* Zpts, const double* variance,
+                    const double* length_scale, const double* q_mu, const double* q_sqrt, const double* W, double jitter,
+                    const double* y_mean, const double* y_std, const double* y_var_scale, const double* xlb,
+                    const double* xrng, dmo_svgp** out);
+int dmo_svgp_predict(dmo_ctx* ctx, dmo_svgp* sv, const double* X, int64_t P, double* mean, double* var, int precision);
+int dmo_svgp_groups(dmo_ctx* ctx, dmo_svgp* sv, int* n_groups, int* n_planes);
+int dmo_svgp_destroy(dmo_ctx* ctx, dmo_svgp* sv);
+int dmo_svgp_optimal_q(dmo_ctx* ctx, int64_t N, int64_t Z, int d, int L, const double* X, const double* y,
+                       const double* Zpts, const double* variance, const double* length_scale, const double* noise,
+                       double jitter, int inducing_is_data, double* q_mu_out, double* q_sqrt_out);
 
 /* ---- A16: exact hypervolume ---------------------------------------------------
  * replaces hv.AdaptiveHyperVolume.compute_hypervolume(..., 'box') (dmosopt/hv.py:123-189)

@@ -338,6 +338,62 @@ def stream_sweep():
     print(f"hypervolume n={pop} M=3 (whole set non-dominated): {ms:.3f} ms, value {out.value:.6f}", flush=True)
 
 
+def svgp_sweep():
+    """The variational posterior (dmo_svgp_predict, fp64 and tensor) at P = 65536, d = 30, M = 3: SVGP with Z = 819 (its
+    round(0.2 N) at N = 4096, its own Z per output: 3 K_* planes, 6 operator planes) and VGP with Z = N = 4096 (one K_*
+    plane; one Lz^-1 shared by the outputs plus 3 q operators: 4 planes), both with q at its optimum; next to
+    dmo_gp_predict with three distinct covariances (3 planes of N = 4096) in the same run.  Per plane: the variance
+    contraction's time over the operator planes it walks.  Also the create time (Householder QR per latent) and
+    dmo_svgp_optimal_q at N = 4096."""
+    L.context()
+    rng = np.random.default_rng(5)
+    N, d, M, P = 4096, 30, 3, 65536
+    Xtr = rng.random((N, d))
+    Ytr = np.column_stack([np.sin(3 * Xtr[:, :4].sum(axis=1) + k) + Xtr[:, 4 + k] ** 2 for k in range(M)])
+    yn = (Ytr - Ytr.mean(0)) / Ytr.std(0)
+    ls, s = np.full((M, d), 0.5 * np.sqrt(d / 4)), np.ones(M)
+    X = rng.random((P, d))
+    Xd = L.DeviceArray((P, d)).upload(X)
+    md, vd = L.DeviceArray((P, M)), L.DeviceArray((P, M))
+    lib, ctx = L.load_library(), L.context()
+    print(device_line(), flush=True)
+    # GPR_Matern reference: three covariances (constants 1.0, 1.5, 2.0)
+    cs = [1.0, 1.5, 2.0]
+    Lf, alpha, _ = L.gp_fit(Xtr, yn.T, cs, [ls[0]] * M, [1e-3] * M, jitter=0.0)
+    gpr = L.GPHandle(Xtr, alpha, Lf, cs, [ls[0]] * M, [1e-3] * M, Ytr.mean(0), Ytr.std(0), np.zeros(d), np.ones(d))
+    models = [("GPR_Matern", None, gpr.covariance_groups()[0],
+               lambda prec: lib.dmo_gp_predict(ctx, gpr._h, Xd.ptr, P, md.ptr, vd.ptr, prec), "gp_var")]
+    for name, Zn in (("SVGP_Matern", 819), ("VGP_Matern", N)):
+        vgp = Zn == N
+        Z = np.stack([Xtr] * M) if vgp else np.stack([Xtr[rng.choice(N, Zn, replace=False)] for _ in range(M)])
+        t0 = time.perf_counter()
+        qm, qs = L.svgp_optimal_q(Xtr, yn.T, None if vgp else Z, s, ls, np.full(M, 1e-3), inducing_is_data=vgp)
+        t_q = time.perf_counter() - t0
+        t0 = time.perf_counter()
+        h = L.SVGPHandle(Z, s, ls, qm, qs, Ytr.mean(0), Ytr.std(0), np.zeros(d), np.ones(d))
+        t_c = time.perf_counter() - t0
+        groups, planes = h.groups()
+        print(f"{name} N={N} Z={Zn}: dmo_svgp_optimal_q {t_q * 1e3:.1f} ms, dmo_svgp_create {t_c * 1e3:.1f} ms; "
+              f"{groups} K_* planes, {planes} operator planes", flush=True)
+        models.append((name, h, planes, lambda prec, h=h: lib.dmo_svgp_predict(ctx, h._h, Xd.ptr, P, md.ptr, vd.ptr, prec), "svgp_var"))
+    out = {}
+    for name, _, planes, fn, var_key in models:
+        for prec, pname in ((L.GP_FP64, "fp64"), (L.GP_TENSOR, "tensor")):
+            L.profile_enable(True)
+            ms = timed(lambda: L._check(fn(prec), name), reps=3)
+            rep = L.profile_report()
+            L.profile_enable(False)
+            out[(name, pname)] = (md.download(), vd.download())
+            vms = rep[var_key][0] / rep[var_key][1] if var_key in rep else float("nan")
+            parts = ", ".join(f"{k} {v[0] / v[1]:.3f}" for k, v in rep.items())
+            print(f"{name} {pname} P={P} d={d} M={M}: total {ms:.3f} ms [{parts}]; variance contraction per operator plane "
+                  f"{vms / planes:.3f} ms ({planes} planes)", flush=True)
+    for name in ("SVGP_Matern", "VGP_Matern"):
+        (mf, vf), (mt, vt) = out[(name, "fp64")], out[(name, "tensor")]
+        print(f"{name} tensor vs fp64: mean err / max|mean| {np.max(np.abs(mt - mf) / np.abs(mf).max(0)):.2e}, "
+              f"var err / prior {np.max(np.abs(vt - vf) / Ytr.std(0) ** 2):.2e}", flush=True)
+
+
 if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] == "stream":
         stream_sweep()
@@ -350,6 +406,9 @@ if __name__ == "__main__":
         sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "mtgp_fit":
         mtgp_fit_sweep()
+        sys.exit(0)
+    if len(sys.argv) > 1 and sys.argv[1] == "svgp":
+        svgp_sweep()
         sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "egp_fit":
         egp_fit_sweep()
