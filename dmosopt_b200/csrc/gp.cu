@@ -412,20 +412,29 @@ int gp_linv_from_factor(dmo_ctx* ctx, const double* L, int64_t N, int64_t ldo, d
   return DMO_OK;
 }
 
+int GpVarOps::alloc(dmo_ctx* ctx, int64_t N, int G_) {
+  Npad = ceil_div(N, 256) * 256;
+  G = G_;
+  h_kscale.assign(G, 1.0);
+  DMO_TRY(Linv.alloc(ctx, (size_t)G * Npad * Npad));
+  DMO_CUDA(cudaMemsetAsync(Linv.p, 0, (size_t)G * Npad * Npad * sizeof(double), ctx->stream));
+  return DMO_OK;
+}
+
 static_assert(VB == GP_F64_TILE, "gp.cuh exports the float64 variance tile edge");
 
-int gp_var_contract_fp64(dmo_ctx* ctx, const dmo_gp* gp, const double* Ks, int64_t kplane, int64_t Pcpad, int nsplit,
+int gp_var_contract_fp64(dmo_ctx* ctx, const GpVarOps& ops, const double* Ks, int64_t kplane, int64_t Pcpad, int nsplit,
                          double* vnorm, int64_t vn_ld) {
-  dim3 gv((unsigned)(Pcpad / VB), (unsigned)gp->G, (unsigned)nsplit);
+  dim3 gv((unsigned)(Pcpad / VB), (unsigned)ops.G, (unsigned)nsplit);
   DMO_CUDA(cudaFuncSetAttribute(var_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)VAR_SMEM));
-  DMO_LAUNCH(var_kernel, gv, 256, VAR_SMEM, gp->Linv.p, gp->Npad, gp->Npad * gp->Npad, Ks, gp->Npad, kplane, gp->Npad, vnorm,
+  DMO_LAUNCH(var_kernel, gv, 256, VAR_SMEM, ops.Linv.p, ops.Npad, ops.Npad * ops.Npad, Ks, ops.Npad, kplane, ops.Npad, vnorm,
              vn_ld);
   return DMO_OK;
 }
 
 int gp_predict_fp64(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var) {
-  const int64_t N = gp->N, Npad = gp->Npad;
-  const int M = gp->M, G = gp->G, d = gp->d;
+  const int64_t N = gp->N, Npad = gp->ops.Npad;
+  const int M = gp->M, G = gp->ops.G, d = gp->d;
   // candidate chunk so that Ks (G x Pc x Npad float64) stays within ~8 GiB
   int64_t budget = (int64_t)8 << 30;
   int64_t Pc_max = budget / ((int64_t)G * Npad * 8);
@@ -462,7 +471,7 @@ int gp_predict_fp64(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, doub
     }
     if (d_var) {
       ProfileScope ps(ctx, "gp_var");
-      DMO_TRY(gp_var_contract_fp64(ctx, gp, Ks.p, kplane, Pcpad, (int)nsplit, vnorm.p, Pc_alloc));
+      DMO_TRY(gp_var_contract_fp64(ctx, gp->ops, Ks.p, kplane, Pcpad, (int)nsplit, vnorm.p, Pc_alloc));
       DMO_LAUNCH(var_finish_kernel, (unsigned)ceil_div(Pc * M, 256), 256, 0, vnorm.p, (int)nsplit, Pc, Pc_alloc, M, G,
                  gp->cov.p, gp->constant.p, gp->noise.p, gp->ystd.p, p_base, d_var);
     }
@@ -666,7 +675,6 @@ int dmo_gp_create(dmo_ctx* ctx, int64_t N, int d, int M, int kernel, const doubl
   gp->d = d;
   gp->M = M;
   gp->kernel = kernel;
-  gp->Npad = ceil_div(N, 256) * 256;  // multiple of the fp64 tile (128) and of the tensor path's Linv tile (256)
   gp->isotropic = true;
   std::vector<double> h_inv((size_t)M * d), h_rg(d);
   for (int m = 0; m < M; ++m)
@@ -691,7 +699,6 @@ int dmo_gp_create(dmo_ctx* ctx, int64_t N, int d, int M, int kernel, const doubl
     if (e__ != cudaSuccess)                                                                           \
       return fail(dmo_fail(ctx, DMO_ERR_CUDA, "%s failed: %s", #call, cudaGetErrorString(e__)));      \
   } while (0)
-  const int64_t Npad = gp->Npad;
   GP_TRY(gp->Xt.alloc(ctx, (size_t)N * d));
   GP_TRY(gp->alpha.alloc(ctx, (size_t)M * N));
   GP_TRY(gp->inv_ls.alloc(ctx, (size_t)M * d));
@@ -740,7 +747,7 @@ int dmo_gp_create(dmo_ctx* ctx, int64_t N, int d, int M, int kernel, const doubl
         gp->h_lead.push_back(m);
       }
     }
-    const int G = gp->G = (int)gp->h_lead.size();
+    const int G = (int)gp->h_lead.size();
     for (int l : gp->h_lead) {
       h_ginv.insert(h_ginv.end(), h_inv.begin() + (size_t)l * d, h_inv.begin() + (size_t)(l + 1) * d);
       h_gc.push_back(h_c[l]);
@@ -751,11 +758,12 @@ int dmo_gp_create(dmo_ctx* ctx, int64_t N, int d, int M, int kernel, const doubl
     GP_CUDA(cudaMemcpyAsync(gp->cov.p, gp->h_cov.data(), M * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
     GP_CUDA(cudaMemcpyAsync(gp->g_inv_ls.p, h_ginv.data(), h_ginv.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     GP_CUDA(cudaMemcpyAsync(gp->g_constant.p, h_gc.data(), G * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    GP_TRY(gp->Linv.alloc(ctx, (size_t)G * Npad * Npad));
-    GP_CUDA(cudaMemsetAsync(gp->Linv.p, 0, (size_t)G * Npad * Npad * sizeof(double), ctx->stream));
+    GP_TRY(gp->ops.alloc(ctx, N, G));
+    gp->ops.h_kscale = h_gc;
+    const int64_t Npad = gp->ops.Npad;
     for (int g = 0; g < G; ++g) {
       const double* src = f.d + (size_t)gp->h_lead[g] * N * N;
-      double* dst = gp->Linv.p + (size_t)g * Npad * Npad;
+      double* dst = gp->ops.Linv.p + (size_t)g * Npad * Npad;
       if (factor_is_inverse) {
         DMO_LAUNCH(copy_pad_kernel, (unsigned)ceil_div(N * N, 256), 256, 0, src, N, N, Npad, dst);
       } else {
@@ -838,7 +846,7 @@ int dmo_gp_auto_info(dmo_ctx* ctx, dmo_gp* gp, int* mean_tensor, int* var_tensor
 int dmo_gp_covariance_groups(dmo_ctx* ctx, dmo_gp* gp, int* n_groups, int* group_of) {
   if (!ctx) return DMO_ERR_ARG;
   DMO_REQUIRE(gp, "gp_covariance_groups: null model");
-  if (n_groups) *n_groups = gp->G;
+  if (n_groups) *n_groups = gp->ops.G;
   if (group_of) memcpy(group_of, gp->h_cov.data(), (size_t)gp->M * sizeof(int));
   return DMO_OK;
 }

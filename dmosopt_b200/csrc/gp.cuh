@@ -1,23 +1,41 @@
-// GP posterior state shared by gp.cu (float64 path) and gp_tensor.cu (wgmma path).
+// GP posterior state shared by gp.cu (float64 path) and gp_tensor.cu (wgmma path), and the variance operators that the
+// exact, multitask (gp_multitask.cu) and variational (gp_variational.cu) posteriors contract against.
 #pragma once
 #include <vector>
 
 #include "common.cuh"
 
+// G lower-triangular float64 planes Linv_g: a posterior's variance terms are the column sums of squares ||Linv_g k_*||^2
+// against a K_* plane.  The exact GP's planes are the L^-1 of its covariances; MEGP's the L_j^-1 of its blocks; the
+// variational posterior's the operators s Lz^-1 and s T.  h_kscale[g] is the output scale of the K_* plane that plane g
+// is contracted against; it fixes that plane's K_* scaling exponent on the tensor path.
+struct GpVarOps {
+  int64_t Npad = 0;  // rows and columns of a plane: N rounded up to the float64 (128) and wgmma (256) tiles
+  int G = 0;
+  std::vector<double> h_kscale;  // (G,)
+  DevBuf<double> Linv;           // (G, Npad, Npad), zero above the diagonal and in the padding
+  // tensor path (built lazily by gp_prepare_tensor)
+  bool tensor_ready = false;
+  DevBuf<uint16_t> Lhi, Llo;  // (G, Npad, Npad) fp16 split of the row-scaled Linv
+  DevBuf<float> Lscale;       // (G, Npad) 1 / (row scale * K_* scale), powers of two
+  DevBuf<int> Kexp;           // (G,) K_* scaling exponents
+  // G zeroed planes for N points, K_* scales 1
+  int alloc(dmo_ctx* ctx, int64_t N, int G);
+};
+
 struct dmo_gp {
-  int64_t N = 0, Npad = 0;  // training points; padded to the variance tile edge
+  int64_t N = 0;  // training points
   int d = 0, M = 0, kernel = 0;
   bool isotropic = true;
   // Objectives that share a posterior covariance (bitwise equal constant, length scales and factor plane; noise may
   // differ, it only enters the final subtraction) share one L^-1, one K_* and one variance contraction.  Decided once
-  // by dmo_gp_create: G groups numbered in order of first appearance, cov[m] the group of objective m, lead[g] the first
-  // objective of group g.  Every per-covariance array below has G planes.
-  int G = 0;
+  // by dmo_gp_create: ops.G groups numbered in order of first appearance, cov[m] the group of objective m, lead[g] the
+  // first objective of group g.  Every per-covariance array below has ops.G planes.
+  GpVarOps ops;                    // the L^-1 of each group, K_* scales the group constants
   std::vector<int> h_cov, h_lead;  // (M,), (G,)
   DevBuf<int> cov;                 // (M,) device copy of h_cov
   DevBuf<double> Xt;        // (N, d) normalised training inputs
   DevBuf<double> alpha;     // (M, N)
-  DevBuf<double> Linv;      // (G, Npad, Npad) lower-triangular inverse Cholesky factors, zero padded
   DevBuf<double> inv_ls;    // (M, d) 1 / length_scale
   DevBuf<double> g_inv_ls, g_constant;  // (G, d), (G,) 1 / length_scale and constant of each group (its first objective)
   DevBuf<double> constant, noise, ymean, ystd;  // (M,)
@@ -26,11 +44,6 @@ struct dmo_gp {
   // optional linear prior mean m(x) = w . x_n + b in the normalised-output space (gpytorch LinearMean, A19)
   bool has_linear_mean = false;
   DevBuf<double> lin_w, lin_b;  // (M, d), (M,)
-  // tensor path (built lazily on first DMO_GP_TENSOR predict)
-  bool tensor_ready = false;
-  DevBuf<uint16_t> Lhi, Llo;  // (G, Npad, Npad) fp16 split of the row-scaled L^-1
-  DevBuf<float> Lscale;       // (G, Npad) 1 / (row scale * K_* scale), powers of two
-  DevBuf<int> Kexp;           // (G,) K_* scaling exponents
   DevBuf<float> Xtf;          // (Npad, 32) float copy of Xt, zero padded (mean-only direct kernel, d <= 32); built lazily
   DevBuf<float> CAf;          // (M, Npad) c_m * alpha_m as float, zero padded (fused K_* + mean kernel); built with Xtf
   // DMO_GP_AUTO: per-model calibration of the tensor path against the float64 path on probe candidates (gp.cu)
@@ -61,23 +74,52 @@ int gp_fit_batched(dmo_ctx* ctx, int64_t N, int d, int nbat, int kernel, const d
 // multiple of 64; pad with an identity tail); info[b] (zeroed by the caller) receives a non-positive pivot + 1.  Not
 // synchronised.
 int gp_potrf_batched(dmo_ctx* ctx, double* A, int64_t ld, int nbat, int* info);
-// float64 variance contraction (var_kernel) over the gp->G covariances: vnorm[z][g][p] = partial sums over the row
-// blocks z (mod nsplit) of ||Linv_g Ks_g[p]||^2, Ks_g = Ks + g * kplane with rows of gp->Npad doubles (kplane = 0: one
-// K_* plane for every g); Pcpad is a multiple of GP_F64_TILE
+// float64 variance contraction (var_kernel) over the ops.G planes: vnorm[z][g][p] = partial sums over the row blocks z
+// (mod nsplit) of ||Linv_g Ks_g[p]||^2, Ks_g = Ks + g * kplane with rows of ops.Npad doubles (kplane = 0: one K_* plane
+// for every g); Pcpad is a multiple of GP_F64_TILE
 constexpr int GP_F64_TILE = 128;
-int gp_var_contract_fp64(dmo_ctx* ctx, const dmo_gp* gp, const double* Ks, int64_t kplane, int64_t Pcpad, int nsplit,
+int gp_var_contract_fp64(dmo_ctx* ctx, const GpVarOps& ops, const double* Ks, int64_t kplane, int64_t Pcpad, int nsplit,
                          double* vnorm, int64_t vn_ld);
-// the fp16 hi / lo split of L^-1 and its row scales (built once per model; gp->Kexp holds the K_* scaling exponents)
-int gp_prepare_tensor(dmo_ctx* ctx, dmo_gp* gp);
-// wgmma variance contraction (gp_var_wgmma_kernel, paired schedule) over K_* hi / lo rows of gp->Npad fp16 values:
-// k_alloc rows are allocated, covariance g < gp->G reads rows g * k_rows + [0, Pcpad) (k_rows = 0: one plane for every
-// g); Pcpad is a multiple of GP_TC_TILE.  vnorm[q][g][p], q < gp_tensor_var_planes(gp->Npad), holds the partial sums.
+// the fp16 hi / lo split of the planes and its row scales, and the K_* scaling exponents ops.Kexp (built once)
+int gp_prepare_tensor(dmo_ctx* ctx, GpVarOps& ops);
+// wgmma variance contraction (gp_var_wgmma_kernel, paired schedule) over K_* hi / lo rows of ops.Npad fp16 values:
+// k_alloc rows are allocated, plane g < ops.G reads rows g * k_rows + [0, Pcpad) (k_rows = 0: one K_* plane for every
+// g); Pcpad is a multiple of GP_TC_TILE.  vnorm[q][g][p], q < gp_tensor_var_planes(ops.Npad), holds the partial sums.
 // abort_flag (device int, zeroed by the caller) is set when the pipeline watchdog trips.
 constexpr int GP_TC_TILE = 128;
 int gp_tensor_var_planes(int64_t Npad);
-int gp_var_contract_tensor(dmo_ctx* ctx, dmo_gp* gp, const uint16_t* Kh, const uint16_t* Kl, int64_t k_alloc, int64_t k_rows,
-                           int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag);
+int gp_var_contract_tensor(dmo_ctx* ctx, const GpVarOps& ops, const uint16_t* Kh, const uint16_t* Kl, int64_t k_alloc,
+                           int64_t k_rows, int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag);
 int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var);
+
+// Candidate chunks and variance scratch of the unit-scale posteriors (MEGP, variational; gp_multitask.cu): one K_* plane
+// per chunk (float64 Ks, or fp16 Kh / Kl) contracted against up to `planes` operator planes, partial sums in vnorm (rows
+// of Pc_alloc).  Messages are prefixed by `who`.
+struct GpUnitPredict {
+  const char* who = "";
+  bool tensor = false;
+  int64_t tile = 0;      // candidate padding of a chunk
+  int64_t Pc_alloc = 0;  // candidates per chunk
+  int n_vp = 0;          // vnorm partial-sum planes per operator plane
+  DevBuf<double> vnorm, Ks;
+  DevBuf<uint16_t> Kh, Kl;
+  DevBuf<int> abort_flag;
+  // precision is DMO_GP_FP64 or DMO_GP_TENSOR, and d fits the tensor path
+  int check(dmo_ctx* ctx, const char* who, int precision, int d);
+  // chunk size and scratch for P candidates against Npad-row planes
+  int alloc(dmo_ctx* ctx, int64_t P, int64_t Npad, int planes, bool want_var);
+  // the variance partial sums of one chunk of Pcpad candidates, its K_* plane already produced
+  int contract(dmo_ctx* ctx, const GpVarOps& ops, int64_t Pcpad);
+  // fails when the tensor pipeline's watchdog tripped (synchronises)
+  int watchdog(dmo_ctx* ctx);
+};
+
+template <typename T>
+int upload(dmo_ctx* ctx, DevBuf<T>& dst, const std::vector<T>& src) {
+  DMO_TRY(dst.alloc(ctx, src.size()));
+  DMO_CUDA(cudaMemcpyAsync(dst.p, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
+  return DMO_OK;
+}
 
 // ---- multitask model (gp_multitask.cu): the block factorisation shared by dmo_mtgp_create and dmo_mtgp_lml_grad --
 constexpr int MT_MAX = 8;        // tasks per model
@@ -102,6 +144,14 @@ int mt_scale_inputs(dmo_ctx* ctx, const double* X, int64_t P, int d, const doubl
                     double* xs);
 // training points per producer block: mpart has Npad / mt_kstar_span(tensor) row-block planes
 int64_t mt_kstar_span(bool tensor);
+// the producer's (d, Npad) training inputs: XtT[k][n] = x(n, k), the scaled coordinate k of point n < N; zero padded
+template <typename F>
+std::vector<double> mt_xt_transposed(int64_t N, int d, int64_t Npad, F x) {
+  std::vector<double> xtT((size_t)d * Npad, 0.0);
+  for (int64_t n = 0; n < N; ++n)
+    for (int k = 0; k < d; ++k) xtT[(size_t)k * Npad + n] = x(n, k);
+  return xtT;
+}
 // One unit-scale Matern-5/2 K_* plane k(xs_p, XtT[:, n]) for the candidates p_base + [0, Pcpad) (float64 Ks, or fp16 hi / lo
 // Kh / Kl scaled by 2^k_exp[0]; NULL: not written) and the partial sums mpart[z][j][p] of k' A_j, j < M <= MT_MAX.
 // tensor: d <= 64.

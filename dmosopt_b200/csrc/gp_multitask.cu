@@ -13,8 +13,10 @@
 // Every block sees the same k_*: the inputs are pre-scaled by 1 / l, so the kernel is isotropic with unit length, and
 // one K_* plane serves all M blocks.  Per predict this file's producer writes that plane once (fp16 hi / lo for the
 // tensor path, float64 for the float64 path) and accumulates the M block means k_*' a_j from the same kernel values;
-// the variance contractions of the single-output GP (var_kernel, gp_var_wgmma_kernel) run unchanged with K_* plane
-// stride 0; mt_mix_kernel adds their partial sums in a fixed order and mixes the blocks back into tasks.
+// the L_j^-1 are the M planes of one GpVarOps, contracted against that plane (K_* plane stride 0) by the exact GP's
+// variance contractions (var_kernel, gp_var_wgmma_kernel); mt_mix_kernel adds their partial sums in a fixed order and
+// mixes the blocks back into tasks.  GpUnitPredict, the chunking and scratch of that predict, is shared with the
+// variational posterior (gp_variational.cu).
 #include <math.h>
 
 #include <memory>
@@ -25,11 +27,10 @@
 #include "gp.cuh"
 
 struct dmo_mtgp {
-  int64_t N = 0, Npad = 0;
+  int64_t N = 0;
   int d = 0, M = 0;
   double lml = 0.0;
-  // the M blocks as the objectives of one single-output state: only Linv (and its tensor split) are used
-  std::unique_ptr<dmo_gp> blk;
+  GpVarOps blk;                    // (M, Npad, Npad) L_j^-1 of the blocks, zero padded
   DevBuf<double> XtT;              // (d, Npad) scaled training inputs x_n / l, transposed, zero padded
   DevBuf<double> A;                // (M, Npad) a_j, zero padded
   DevBuf<double> inv_ls, xlb, xrg; // (d,)
@@ -289,13 +290,6 @@ void jacobi_eigh(int M, std::vector<double> A, std::vector<double>& lam, std::ve
   for (int i = 0; i < M; ++i) lam[i] = A[(size_t)i * M + i];
 }
 
-template <typename T>
-int upload(dmo_ctx* ctx, DevBuf<T>& dst, const std::vector<T>& src) {
-  DMO_TRY(dst.alloc(ctx, src.size()));
-  DMO_CUDA(cudaMemcpyAsync(dst.p, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
-  return DMO_OK;
-}
-
 }  // namespace
 
 int mt_scale_inputs(dmo_ctx* ctx, const double* X, int64_t P, int d, const double* xlb, const double* xrg, const double* inv_ls,
@@ -321,6 +315,57 @@ int mt_kstar_produce(dmo_ctx* ctx, bool tensor, const double* xs, int64_t P, int
     DMO_LAUNCH(mt_kstar_f64_kernel, g, PF_TN, (size_t)PF_TP * d * sizeof(double), xs, P, p_base, XtT, N, Npad, d, M, A, Ks, mpart,
                mp_ld);
   }
+  return DMO_OK;
+}
+
+int GpUnitPredict::check(dmo_ctx* ctx, const char* who_, int precision, int d) {
+  who = who_;
+  DMO_REQUIRE(precision == DMO_GP_FP64 || precision == DMO_GP_TENSOR, "%s: precision must be DMO_GP_FP64 or DMO_GP_TENSOR (got %d)",
+              who, precision);
+  tensor = precision == DMO_GP_TENSOR;
+  DMO_REQUIRE(!tensor || d <= 64, "%s(tensor): at most 64 input dimensions (got %d); use DMO_GP_FP64", who, d);
+  return DMO_OK;
+}
+
+int GpUnitPredict::alloc(dmo_ctx* ctx, int64_t P, int64_t Npad, int planes, bool want_var) {
+  // candidate chunk: the one K_* plane (fp16 hi + lo, or float64) within ~6 GiB; the producer grid's y extent stays < 2^16
+  tile = tensor ? GP_TC_TILE : GP_F64_TILE;
+  int64_t Pc_max = ((int64_t)6 << 30) / (Npad * (tensor ? 4 : 8));
+  if (Pc_max > ((int64_t)1 << 20)) Pc_max = (int64_t)1 << 20;
+  Pc_max = (Pc_max / tile) * tile;
+  if (Pc_max < tile) Pc_max = tile;
+  Pc_alloc = P < Pc_max ? ceil_div(P, tile) * tile : Pc_max;
+  if (!want_var) return DMO_OK;
+  if (tensor) {
+    n_vp = gp_tensor_var_planes(Npad);
+  } else {  // the row blocks of the planes are split so that at least ~2 CTAs per SM exist for small candidate sets
+    int64_t nsplit = ceil_div((int64_t)2 * ctx->sm_count, (Pc_alloc / GP_F64_TILE) * planes);
+    const int64_t ntile = Npad / GP_F64_TILE;
+    n_vp = (int)(nsplit > ntile ? ntile : (nsplit < 1 ? 1 : nsplit));
+  }
+  DMO_TRY(vnorm.alloc(ctx, (size_t)n_vp * planes * Pc_alloc));
+  if (tensor) {
+    DMO_TRY(Kh.alloc(ctx, (size_t)Pc_alloc * Npad));
+    DMO_TRY(Kl.alloc(ctx, (size_t)Pc_alloc * Npad));
+    DMO_TRY(abort_flag.alloc(ctx, 1));
+    DMO_CUDA(cudaMemsetAsync(abort_flag.p, 0, sizeof(int), ctx->stream));
+  } else {
+    DMO_TRY(Ks.alloc(ctx, (size_t)Pc_alloc * Npad));
+  }
+  return DMO_OK;
+}
+
+int GpUnitPredict::contract(dmo_ctx* ctx, const GpVarOps& ops, int64_t Pcpad) {
+  if (tensor) return gp_var_contract_tensor(ctx, ops, Kh.p, Kl.p, Pc_alloc, 0, Pcpad, vnorm.p, Pc_alloc, abort_flag.p);
+  return gp_var_contract_fp64(ctx, ops, Ks.p, 0, Pcpad, n_vp, vnorm.p, Pc_alloc);
+}
+
+int GpUnitPredict::watchdog(dmo_ctx* ctx) {
+  if (!abort_flag.p) return DMO_OK;  // no tensor-core contraction ran
+  int h_abort = 0;
+  DMO_CUDA(cudaMemcpyAsync(&h_abort, abort_flag.p, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (h_abort) return dmo_fail(ctx, DMO_ERR_INTERNAL, "%s(tensor): pipeline watchdog tripped", who);
   return DMO_OK;
 }
 
@@ -436,36 +481,19 @@ int dmo_mtgp_create(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_train
   mt->N = N;
   mt->d = d;
   mt->M = M;
-  const int64_t Npad = mt->Npad = ceil_div(N, 256) * 256;  // the float64 (128) and wgmma (256) Linv tiles
   mt->lml = mb.lml;
   const double lml = mb.lml;
-  mt->blk.reset(new dmo_gp());
-  dmo_gp* gp = mt->blk.get();
-  gp->N = N;
-  gp->Npad = Npad;
-  gp->d = d;
-  gp->M = M;
-  gp->G = M;  // the blocks share K_* but not L_j^-1: one covariance each
-  for (int j = 0; j < M; ++j) {
-    gp->h_cov.push_back(j);
-    gp->h_lead.push_back(j);
-  }
-  gp->kernel = DMO_KERNEL_MATERN52;
-  gp->h_constant.assign(M, 1.0);  // K_* carries no output scale: one K_* scaling exponent for every block
-  gp->h_noise.assign(M, 1.0);
-  gp->h_ystd.assign(M, 1.0);
-  DMO_TRY(gp->Linv.alloc(ctx, (size_t)M * Npad * Npad));
-  DMO_CUDA(cudaMemsetAsync(gp->Linv.p, 0, (size_t)M * Npad * Npad * sizeof(double), ctx->stream));
+  DMO_TRY(mt->blk.alloc(ctx, N, M));  // the blocks share K_* (unit scale) but not L_j^-1: one plane each
+  const int64_t Npad = mt->blk.Npad;
   for (int j = 0; j < M; ++j)
-    DMO_TRY(gp_linv_from_factor(ctx, Lf.p + (size_t)j * N * N, N, Npad, gp->Linv.p + (size_t)j * Npad * Npad));
+    DMO_TRY(gp_linv_from_factor(ctx, Lf.p + (size_t)j * N * N, N, Npad, mt->blk.Linv.p + (size_t)j * Npad * Npad));
   DMO_TRY(mt->A.alloc(ctx, (size_t)M * Npad));
   DMO_CUDA(cudaMemsetAsync(mt->A.p, 0, (size_t)M * Npad * sizeof(double), ctx->stream));
   DMO_CUDA(cudaMemcpy2DAsync(mt->A.p, Npad * sizeof(double), alpha.p, N * sizeof(double), N * sizeof(double), M,
                              cudaMemcpyDeviceToDevice, ctx->stream));
   // small state
-  std::vector<double> xtT((size_t)d * Npad, 0.0), inv(d), rg(d), mix(mm), prior(M), ws((size_t)M * d);
-  for (int64_t n = 0; n < N; ++n)
-    for (int k = 0; k < d; ++k) xtT[(size_t)k * Npad + n] = xs[(size_t)n * d + k];
+  const std::vector<double> xtT = mt_xt_transposed(N, d, Npad, [&](int64_t n, int k) { return xs[(size_t)n * d + k]; });
+  std::vector<double> inv(d), rg(d), mix(mm), prior(M), ws((size_t)M * d);
   for (int k = 0; k < d; ++k) {
     inv[k] = 1.0 / ls[k];
     rg[k] = ub[k] - lb[k];
@@ -505,15 +533,13 @@ int dmo_mtgp_predict(dmo_ctx* ctx, dmo_mtgp* mt, const double* X, int64_t P, dou
   if (!ctx) return DMO_ERR_ARG;
   DMO_CUDA(cudaSetDevice(ctx->device));
   DMO_REQUIRE(mt, "mtgp_predict: null model");
-  DMO_REQUIRE(precision == DMO_GP_FP64 || precision == DMO_GP_TENSOR,
-              "mtgp_predict: precision must be DMO_GP_FP64 or DMO_GP_TENSOR (got %d)", precision);
-  const bool tensor = precision == DMO_GP_TENSOR;
   const int M = mt->M, d = mt->d;
-  const int64_t N = mt->N, Npad = mt->Npad;
-  DMO_REQUIRE(!tensor || d <= 64, "mtgp_predict(tensor): at most 64 input dimensions (got %d); use DMO_GP_FP64", d);
+  const int64_t N = mt->N, Npad = mt->blk.Npad;
+  GpUnitPredict up;
+  DMO_TRY(up.check(ctx, "mtgp_predict", precision, d));
+  const bool tensor = up.tensor;
   if (P == 0) return DMO_OK;
   DMO_REQUIRE(P > 0 && X && mean, "mtgp_predict: bad arguments");
-  dmo_gp* gp = mt->blk.get();
   In<double> x;
   Out<double> om, ov;
   DMO_TRY(x.init(ctx, X, (size_t)P * d));
@@ -523,68 +549,32 @@ int dmo_mtgp_predict(dmo_ctx* ctx, dmo_mtgp* mt, const double* X, int64_t P, dou
   DevBuf<double> xs;
   DMO_TRY(xs.alloc(ctx, (size_t)P * d));
   DMO_TRY(mt_scale_inputs(ctx, x.d, P, d, mt->xlb.p, mt->xrg.p, mt->inv_ls.p, xs.p));
-  if (tensor && want_var) DMO_TRY(gp_prepare_tensor(ctx, gp));
-  // candidate chunk: the one K_* plane (fp16 hi + lo, or float64) within ~6 GiB; the producer grid's y extent stays < 2^16
-  const int64_t tile = tensor ? GP_TC_TILE : GP_F64_TILE;
-  int64_t Pc_max = ((int64_t)6 << 30) / (Npad * (tensor ? 4 : 8));
-  if (Pc_max > ((int64_t)1 << 20)) Pc_max = (int64_t)1 << 20;
-  Pc_max = (Pc_max / tile) * tile;
-  if (Pc_max < tile) Pc_max = tile;
-  const int64_t Pc_alloc = P < Pc_max ? ceil_div(P, tile) * tile : Pc_max;
+  if (tensor && want_var) DMO_TRY(gp_prepare_tensor(ctx, mt->blk));
+  DMO_TRY(up.alloc(ctx, P, Npad, M, want_var));
+  const int64_t Pc_alloc = up.Pc_alloc;
   const int n_mp = (int)(Npad / mt_kstar_span(tensor));
-  int n_vp = 0;
-  if (want_var) {
-    if (tensor) {
-      n_vp = gp_tensor_var_planes(Npad);
-    } else {  // the row blocks of L^-1 are split so that at least ~2 CTAs per SM exist for small candidate sets
-      int64_t nsplit = ceil_div((int64_t)2 * ctx->sm_count, (Pc_alloc / GP_F64_TILE) * M);
-      const int64_t ntile = Npad / GP_F64_TILE;
-      n_vp = (int)(nsplit > ntile ? ntile : (nsplit < 1 ? 1 : nsplit));
-    }
-  }
-  DevBuf<double> mpart, vnorm, Ks;
-  DevBuf<uint16_t> Kh, Kl;
-  DevBuf<int> abort_flag;
+  DevBuf<double> mpart;
   DMO_TRY(mpart.alloc(ctx, (size_t)n_mp * M * Pc_alloc));
-  if (want_var) {
-    DMO_TRY(vnorm.alloc(ctx, (size_t)n_vp * M * Pc_alloc));
-    if (tensor) {
-      DMO_TRY(Kh.alloc(ctx, (size_t)Pc_alloc * Npad));
-      DMO_TRY(Kl.alloc(ctx, (size_t)Pc_alloc * Npad));
-      DMO_TRY(abort_flag.alloc(ctx, 1));
-      DMO_CUDA(cudaMemsetAsync(abort_flag.p, 0, sizeof(int), ctx->stream));
-    } else {
-      DMO_TRY(Ks.alloc(ctx, (size_t)Pc_alloc * Npad));
-    }
-  }
   for (int64_t p_base = 0; p_base < P; p_base += Pc_alloc) {
     const int64_t Pc = (P - p_base) < Pc_alloc ? (P - p_base) : Pc_alloc;
-    const int64_t Pcpad = ceil_div(Pc, tile) * tile;
+    const int64_t Pcpad = ceil_div(Pc, up.tile) * up.tile;
     {
       ProfileScope ps(ctx, "mtgp_kstar");
       DMO_TRY(mt_kstar_produce(ctx, tensor, xs.p, P, p_base, Pcpad, mt->XtT.p, N, Npad, d, M, mt->A.p,
-                               tensor && want_var ? gp->Kexp.p : nullptr, Ks.p, Kh.p, Kl.p, mpart.p, Pc_alloc));
+                               tensor && want_var ? mt->blk.Kexp.p : nullptr, up.Ks.p, up.Kh.p, up.Kl.p, mpart.p, Pc_alloc));
     }
     if (want_var) {
       ProfileScope ps(ctx, "mtgp_var");
-      if (tensor)
-        DMO_TRY(gp_var_contract_tensor(ctx, gp, Kh.p, Kl.p, Pc_alloc, 0, Pcpad, vnorm.p, Pc_alloc, abort_flag.p));
-      else
-        DMO_TRY(gp_var_contract_fp64(ctx, gp, Ks.p, 0, Pcpad, n_vp, vnorm.p, Pc_alloc));
+      DMO_TRY(up.contract(ctx, mt->blk, Pcpad));
     }
     {
       ProfileScope ps(ctx, "mtgp_mix");
-      DMO_LAUNCH(mt_mix_kernel, (unsigned)ceil_div(Pc, 256), 256, 0, xs.p, Pc, d, M, mpart.p, n_mp, Pc_alloc, vnorm.p, n_vp,
+      DMO_LAUNCH(mt_mix_kernel, (unsigned)ceil_div(Pc, 256), 256, 0, xs.p, Pc, d, M, mpart.p, n_mp, Pc_alloc, up.vnorm.p, up.n_vp,
                  Pc_alloc, mt->mix.p, mt->prior.p, mt->w.p, mt->b.p, mt->ymean.p, mt->ystd.p, p_base, om.d, ov.d);
     }
   }
   DMO_CHECK_LAUNCH();
-  if (tensor && want_var) {
-    int h_abort = 0;
-    DMO_CUDA(cudaMemcpyAsync(&h_abort, abort_flag.p, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (h_abort) return dmo_fail(ctx, DMO_ERR_INTERNAL, "mtgp_predict(tensor): pipeline watchdog tripped");
-  }
+  DMO_TRY(up.watchdog(ctx));
   DMO_TRY(om.finish(ctx));
   DMO_TRY(ov.finish(ctx));
   DMO_CUDA(cudaStreamSynchronize(ctx->stream));

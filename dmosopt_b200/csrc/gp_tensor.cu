@@ -908,32 +908,10 @@ int make_map(dmo_ctx* ctx, CUtensorMap* map, const void* base, uint64_t rows, ui
   return DMO_OK;
 }
 
-int prepare_tensor_state(dmo_ctx* ctx, dmo_gp* gp) {
-  if (gp->tensor_ready) return DMO_OK;
-  const int G = gp->G;
-  const int64_t Npad = gp->Npad;
-  std::vector<int> kexp(G);
-  for (int g = 0; g < G; ++g) {
-    double c = gp->h_constant[gp->h_lead[g]];
-    kexp[g] = (c > 0.0) ? 13 - ilogb(c) : 13;  // scaled K_* <= 2^14
-  }
-  DMO_TRY(gp->Kexp.alloc(ctx, G));
-  DMO_CUDA(cudaMemcpyAsync(gp->Kexp.p, kexp.data(), G * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));  // kexp is a stack vector
-  DMO_TRY(gp->Lhi.alloc(ctx, (size_t)G * Npad * Npad));
-  DMO_TRY(gp->Llo.alloc(ctx, (size_t)G * Npad * Npad));
-  DMO_TRY(gp->Lscale.alloc(ctx, (size_t)G * Npad));
-  DMO_LAUNCH(split_linv_kernel, (unsigned)(G * Npad), 256, 0, gp->Linv.p, Npad, gp->Kexp.p, gp->Lhi.p, gp->Llo.p,
-             gp->Lscale.p);
-  DMO_CHECK_LAUNCH();
-  gp->tensor_ready = true;
-  return DMO_OK;
-}
-
 // float copies of the training inputs and of c * alpha, zero padded to Npad (once per model)
 int prepare_direct_state(dmo_ctx* ctx, dmo_gp* gp) {
   if (gp->Xtf.p && gp->CAf.p) return DMO_OK;
-  const int64_t N = gp->N, Npad = gp->Npad;
+  const int64_t N = gp->N, Npad = gp->ops.Npad;
   DMO_TRY(gp->Xtf.alloc(ctx, (size_t)Npad * KM_D));
   DMO_TRY(gp->CAf.alloc(ctx, (size_t)gp->M * Npad));
   DMO_LAUNCH(pad_xt_f32_kernel, (unsigned)ceil_div(Npad * KM_D, 256), 256, 0, gp->Xt.p, N, gp->d, Npad, gp->Xtf.p);
@@ -966,7 +944,7 @@ int64_t pick_slices(int64_t n_qb, int64_t Npad, int tile, int64_t slots, int64_t
 
 // mean-only predict without K_* in memory (d <= 32, M <= 6): see gp_mean_direct_kernel
 int gp_mean_direct(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean) {
-  const int64_t N = gp->N, Npad = gp->Npad;
+  const int64_t N = gp->N, Npad = gp->ops.Npad;
   const int M = gp->M, d = gp->d;
   DMO_TRY(prepare_direct_state(ctx, gp));
   const int64_t n_qb = ceil_div(P, KM_Q);
@@ -1012,30 +990,50 @@ int gp_mean_direct(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, doubl
 
 }  // namespace
 
-int gp_prepare_tensor(dmo_ctx* ctx, dmo_gp* gp) { return prepare_tensor_state(ctx, gp); }
+int gp_prepare_tensor(dmo_ctx* ctx, GpVarOps& ops) {
+  if (ops.tensor_ready) return DMO_OK;
+  const int G = ops.G;
+  const int64_t Npad = ops.Npad;
+  std::vector<int> kexp(G);
+  for (int g = 0; g < G; ++g) {
+    double c = ops.h_kscale[g];
+    kexp[g] = (c > 0.0) ? 13 - ilogb(c) : 13;  // scaled K_* <= 2^14
+  }
+  DMO_TRY(ops.Kexp.alloc(ctx, G));
+  DMO_CUDA(cudaMemcpyAsync(ops.Kexp.p, kexp.data(), G * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+  DMO_CUDA(cudaStreamSynchronize(ctx->stream));  // kexp is a stack vector
+  DMO_TRY(ops.Lhi.alloc(ctx, (size_t)G * Npad * Npad));
+  DMO_TRY(ops.Llo.alloc(ctx, (size_t)G * Npad * Npad));
+  DMO_TRY(ops.Lscale.alloc(ctx, (size_t)G * Npad));
+  DMO_LAUNCH(split_linv_kernel, (unsigned)(G * Npad), 256, 0, ops.Linv.p, Npad, ops.Kexp.p, ops.Lhi.p, ops.Llo.p,
+             ops.Lscale.p);
+  DMO_CHECK_LAUNCH();
+  ops.tensor_ready = true;
+  return DMO_OK;
+}
 
 static_assert(TMV == GP_TC_TILE, "gp.cuh exports the wgmma candidate tile");
 
 int gp_tensor_var_planes(int64_t Npad) { return (int)((Npad / TN + 1) / 2); }
 
-int gp_var_contract_tensor(dmo_ctx* ctx, dmo_gp* gp, const uint16_t* Kh, const uint16_t* Kl, int64_t k_alloc, int64_t k_rows,
-                           int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag) {
-  const int64_t Npad = gp->Npad;
+int gp_var_contract_tensor(dmo_ctx* ctx, const GpVarOps& ops, const uint16_t* Kh, const uint16_t* Kl, int64_t k_alloc,
+                           int64_t k_rows, int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag) {
+  const int64_t Npad = ops.Npad;
   DMO_REQUIRE(Npad % TN == 0 && Pcpad % TMV == 0, "gp_var_contract_tensor: internal padding error");
   CUtensorMap map_kh, map_kl, map_lh, map_ll;
   DMO_TRY(make_map(ctx, &map_kh, Kh, (uint64_t)k_alloc, (uint64_t)Npad, TMV, TK, CU_TENSOR_MAP_SWIZZLE_64B));
   DMO_TRY(make_map(ctx, &map_kl, Kl, (uint64_t)k_alloc, (uint64_t)Npad, TMV, TK, CU_TENSOR_MAP_SWIZZLE_64B));
-  DMO_TRY(make_map(ctx, &map_lh, gp->Lhi.p, (uint64_t)gp->G * Npad, (uint64_t)Npad, TN, TK, CU_TENSOR_MAP_SWIZZLE_64B));
-  DMO_TRY(make_map(ctx, &map_ll, gp->Llo.p, (uint64_t)gp->G * Npad, (uint64_t)Npad, TN, TK, CU_TENSOR_MAP_SWIZZLE_64B));
+  DMO_TRY(make_map(ctx, &map_lh, ops.Lhi.p, (uint64_t)ops.G * Npad, (uint64_t)Npad, TN, TK, CU_TENSOR_MAP_SWIZZLE_64B));
+  DMO_TRY(make_map(ctx, &map_ll, ops.Llo.p, (uint64_t)ops.G * Npad, (uint64_t)Npad, TN, TK, CU_TENSOR_MAP_SWIZZLE_64B));
   DMO_CUDA(cudaFuncSetAttribute(gp_var_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GEMM_SMEM));
   GemmParams prm;
-  prm.M = gp->G;
+  prm.M = ops.G;
   prm.n_pb = (int)(Pcpad / TMV);
   prm.n_jt = (int)(Npad / TN);
   prm.n_q = gp_tensor_var_planes(Npad);
   prm.k_rows = k_rows;
   prm.l_rows = Npad;
-  prm.inv_scale = gp->Lscale.p;
+  prm.inv_scale = ops.Lscale.p;
   prm.vnorm = vnorm;
   prm.vn_ld = vn_ld;
   prm.abort_flag = abort_flag;
@@ -1046,14 +1044,14 @@ int gp_var_contract_tensor(dmo_ctx* ctx, dmo_gp* gp, const uint16_t* Kh, const u
 }
 
 int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var) {
-  const int64_t N = gp->N, Npad = gp->Npad;
-  const int M = gp->M, G = gp->G, d = gp->d;
+  const int64_t N = gp->N, Npad = gp->ops.Npad;
+  const int M = gp->M, G = gp->ops.G, d = gp->d;
   DMO_REQUIRE(M <= 16, "gp_predict(tensor): at most 16 objectives per model (got %d)", M);
   DMO_REQUIRE(d <= 64, "gp_predict(tensor): at most 64 input dimensions (got %d); use DMO_GP_FP64", d);
   DMO_REQUIRE(Npad % TN == 0, "gp_predict(tensor): internal padding error");
   if (!d_var && d <= KM_D && M <= 6)
     return gp_mean_direct(ctx, gp, dXn, P, d_mean);  // nothing but the mean is wanted: K_* stays in registers
-  DMO_TRY(prepare_tensor_state(ctx, gp));
+  DMO_TRY(gp_prepare_tensor(ctx, gp->ops));
   constexpr int64_t TMv = KM_Q;  // candidate padding: the K_* producers write 256-candidate blocks
   // candidate chunk: K_* hi/lo (2 x G x Pc x Npad fp16) within ~6 GiB
   int64_t Pc_max = ((int64_t)6 << 30) / ((int64_t)G * Npad * 4);
@@ -1093,7 +1091,7 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
   do {                                                                                                                     \
     DMO_CUDA(cudaFuncSetAttribute(kstar_mean_kernel<ISO_, MT_, GR_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
     DMO_LAUNCH((kstar_mean_kernel<ISO_, MT_, GR_>), gf, KS_T, smem, dXn, P, p_base, gp->Xtf.p, N, Npad, n_per_block, d,          \
-               gp->kernel, G, gp->cov.p, gp->g_inv_ls.p, gp->g_constant.p, gp->Kexp.p, gp->CAf.p, kplane, Kh.p, Kl.p,       \
+               gp->kernel, G, gp->cov.p, gp->g_inv_ls.p, gp->g_constant.p, gp->ops.Kexp.p, gp->CAf.p, kplane, Kh.p, Kl.p,   \
                mpart.p, Pcpad);                                                                                            \
   } while (0)
 #define KF_SWITCH(ISO_)                                         \
@@ -1133,7 +1131,7 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
         dim3 gk((unsigned)(Npad / (2 * KT_TN)), (unsigned)ceil_div(Pcpad, KT_TP));
 #define KSTAR_LAUNCH(ISO_, DM_)                                                                                          \
   DMO_LAUNCH((kstar_tensor_kernel<ISO_, DM_>), gk, KT_TN, smem, dXn, P, p_base, Pcpad, gp->Xt.p, N, d, G, gp->kernel, \
-             gp->g_inv_ls.p, gp->g_constant.p, gp->Kexp.p, Npad, kplane, Kh.p, Kl.p)
+             gp->g_inv_ls.p, gp->g_constant.p, gp->ops.Kexp.p, Npad, kplane, Kh.p, Kl.p)
         if (gp->isotropic) {
           if (d <= 32)
             KSTAR_LAUNCH(true, 32);
@@ -1150,13 +1148,13 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
       {
         ProfileScope ps_(ctx, "gp_mean");
         DMO_LAUNCH(mean_split_kernel, (unsigned)ceil_div(Pc * M * 32, 256), 256, 0, Kh.p, Kl.p, Pc, N, Npad, kplane, M,
-                   gp->cov.p, gp->Kexp.p, gp->alpha.p, gp->ymean.p, gp->ystd.p, p_base, d_mean);
+                   gp->cov.p, gp->ops.Kexp.p, gp->alpha.p, gp->ymean.p, gp->ystd.p, p_base, d_mean);
       }
     }
     if (d_var) {
       {
         ProfileScope ps_(ctx, "gp_var");
-        DMO_TRY(gp_var_contract_tensor(ctx, gp, Kh.p, Kl.p, G * Pc_alloc, Pc_alloc, Pcpad, vnorm.p, Pc_alloc, abort_flag.p));
+        DMO_TRY(gp_var_contract_tensor(ctx, gp->ops, Kh.p, Kl.p, G * Pc_alloc, Pc_alloc, Pcpad, vnorm.p, Pc_alloc, abort_flag.p));
       }
       DMO_LAUNCH(var_finish_tc_kernel, (unsigned)ceil_div(Pc * M, 256), 256, 0, vnorm.p, n_q, Pc, Pc_alloc, M, G,
                  gp->cov.p, gp->constant.p, gp->noise.p, gp->ystd.p, p_base, d_var);

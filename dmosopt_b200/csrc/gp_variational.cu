@@ -194,13 +194,6 @@ __global__ void sv_mix_kernel(int64_t P, int L, int M, const double* __restrict_
   if (var) var[t] = v * vscale[m];
 }
 
-template <typename T>
-int upload(dmo_ctx* ctx, DevBuf<T>& dst, const T* src, size_t n) {
-  DMO_TRY(dst.alloc(ctx, n));
-  DMO_CUDA(cudaMemcpyAsync(dst.p, src, n * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
-  return DMO_OK;
-}
-
 int gemm(dmo_ctx* ctx, int64_t m, int64_t n, int64_t K, double alpha, const double* A, int64_t sai, int64_t sak, const double* B,
          int64_t sbk, int64_t sbj, double diag, double* C, int64_t ldc) {
   dim3 g((unsigned)ceil_div(n, GT), (unsigned)ceil_div(m, GT));
@@ -238,7 +231,7 @@ bool bits_equal(const double* a, const double* b, size_t n) { return memcmp(a, b
 struct SvGroup {
   std::vector<int> lat, o0;       // latents of the group; the O0 plane of each (its O1 plane is n_o0 + its index)
   int n_o0 = 0;
-  std::unique_ptr<dmo_gp> ops;    // the operator planes as the covariances of one single-output state (Linv = planes)
+  GpVarOps ops;                   // (n_o0 + nlat, Npad, Npad) the O0 planes, then the O1 plane of each latent
   DevBuf<double> XtT;             // (d, Npad) Z / ell, transposed, zero padded
   DevBuf<double> A;               // (nlat, Npad) mean vectors a_l, zero padded
   DevBuf<double> inv_ls;          // (d,)
@@ -246,7 +239,7 @@ struct SvGroup {
 };
 
 struct dmo_svgp {
-  int64_t Z = 0, Npad = 0;
+  int64_t Z = 0;
   int d = 0, L = 0, M = 0;
   std::vector<std::unique_ptr<SvGroup>> groups;
   DevBuf<double> xlb, xrg, W, ymean, ystd, vscale;
@@ -304,8 +297,6 @@ int dmo_svgp_create(dmo_ctx* ctx, int L, int M, int64_t Z, int d, const double* 
   sv->d = d;
   sv->L = L;
   sv->M = M;
-  const int64_t Npad = sv->Npad = ceil_div(Z, 256) * 256;  // the float64 (128) and wgmma (256) operator tiles
-  const size_t plane = (size_t)Npad * Npad;
   // K_* groups: bitwise equal Z planes and length scales
   std::vector<int> grp_of(L, -1);
   std::vector<int> lead;
@@ -323,8 +314,8 @@ int dmo_svgp_create(dmo_ctx* ctx, int L, int M, int64_t Z, int d, const double* 
     }
   }
   DevBuf<double> qm_d, qs_d, Ct, tau;
-  DMO_TRY(upload(ctx, qm_d, hqm.data(), hqm.size()));
-  DMO_TRY(upload(ctx, qs_d, hqs.data(), hqs.size()));
+  DMO_TRY(upload(ctx, qm_d, hqm));
+  DMO_TRY(upload(ctx, qs_d, hqs));
   DMO_TRY(Ct.alloc(ctx, zz));
   DMO_TRY(tau.alloc(ctx, 1));
   for (size_t g = 0; g < lead.size(); ++g) {
@@ -343,48 +334,36 @@ int dmo_svgp_create(dmo_ctx* ctx, int L, int M, int64_t Z, int d, const double* 
       gr->o0.push_back(o);
     }
     const int nlat = (int)gr->lat.size(), n_o0 = gr->n_o0 = (int)o0_src.size(), G = n_o0 + nlat;
-    gr->ops.reset(new dmo_gp());
-    dmo_gp* ops = gr->ops.get();
-    ops->N = Z;
-    ops->Npad = Npad;
-    ops->d = d;
-    ops->M = ops->G = G;
-    ops->kernel = DMO_KERNEL_MATERN52;
-    for (int k = 0; k < G; ++k) {
-      ops->h_cov.push_back(k);
-      ops->h_lead.push_back(k);
-    }
-    ops->h_constant.assign(G, 1.0);  // K_* carries no output scale: one K_* scaling exponent for every plane
-    ops->h_noise.assign(G, 0.0);
-    ops->h_ystd.assign(G, 1.0);
-    DMO_TRY(ops->Linv.alloc(ctx, (size_t)G * plane));
-    DMO_CUDA(cudaMemsetAsync(ops->Linv.p, 0, (size_t)G * plane * sizeof(double), ctx->stream));
+    GpVarOps& ops = gr->ops;
+    DMO_TRY(ops.alloc(ctx, Z, G));  // K_* carries no output scale: unit K_* scales
+    const int64_t Npad = ops.Npad;
+    const size_t plane = (size_t)Npad * Npad;
     const int f = lead[g];
     for (int k = 0; k < n_o0; ++k) {
       const int l = o0_src[k];
       DMO_TRY(inducing_inverse_factor(ctx, "svgp_create", l, Z, d, &hZ[f * zd], hs[l], &hls[(size_t)f * d], jitter, Npad,
-                                      ops->Linv.p + k * plane));
+                                      ops.Linv.p + k * plane));
     }
     DMO_TRY(gr->A.alloc(ctx, (size_t)nlat * Npad));
     DMO_CUDA(cudaMemsetAsync(gr->A.p, 0, (size_t)nlat * Npad * sizeof(double), ctx->stream));
     for (int j = 0; j < nlat; ++j) {
       const int l = gr->lat[j];
-      const double* Li = ops->Linv.p + gr->o0[j] * plane;  // unscaled Lz^-1 (the O0 planes are scaled below)
+      const double* Li = ops.Linv.p + gr->o0[j] * plane;  // unscaled Lz^-1 (the O0 planes are scaled below)
       // a_l = s_l Lz^-T q_mu:  a[i] = s sum_k Li[k][i] q_mu[k]
       DMO_TRY(gemm(ctx, Z, 1, Z, hs[l], Li, 1, Npad, qm_d.p + (size_t)l * Z, 1, 0, 0.0, gr->A.p + (size_t)j * Npad, 1));
       // V J by columns: column c = row c of Ct, Ct[c][r] = V[r][Z-1-c] = sum_k Li[k][Z-1-c] q_sqrt[k][r]
       DMO_TRY(gemm(ctx, Z, Z, Z, 1.0, Li + (Z - 1), -1, Npad, qs_d.p + (size_t)l * zz, Z, 1, 0.0, Ct.p, Z));
       DMO_TRY(householder_qr(ctx, Ct.p, Z, tau.p));
-      DMO_LAUNCH(sv_flip_kernel, (unsigned)ceil_div((int64_t)zz, 256), 256, 0, Ct.p, Z, hs[l], ops->Linv.p + (n_o0 + j) * plane, Npad);
+      DMO_LAUNCH(sv_flip_kernel, (unsigned)ceil_div((int64_t)zz, 256), 256, 0, Ct.p, Z, hs[l], ops.Linv.p + (n_o0 + j) * plane, Npad);
     }
     for (int k = 0; k < n_o0; ++k)
-      DMO_LAUNCH(sv_scale_kernel, (unsigned)ceil_div((int64_t)plane, 256), 256, 0, ops->Linv.p + k * plane, (int64_t)plane, hs[o0_src[k]]);
-    std::vector<double> xtT((size_t)d * Npad, 0.0), inv(d);
+      DMO_LAUNCH(sv_scale_kernel, (unsigned)ceil_div((int64_t)plane, 256), 256, 0, ops.Linv.p + k * plane, (int64_t)plane, hs[o0_src[k]]);
+    std::vector<double> inv(d);
     for (int k = 0; k < d; ++k) inv[k] = 1.0 / hls[(size_t)f * d + k];
-    for (int64_t n = 0; n < Z; ++n)
-      for (int k = 0; k < d; ++k) xtT[(size_t)k * Npad + n] = hZ[f * zd + (size_t)n * d + k] * inv[k];
-    DMO_TRY(upload(ctx, gr->XtT, xtT.data(), xtT.size()));
-    DMO_TRY(upload(ctx, gr->inv_ls, inv.data(), inv.size()));
+    const std::vector<double> xtT =
+        mt_xt_transposed(Z, d, Npad, [&](int64_t n, int k) { return hZ[f * zd + (size_t)n * d + k] * inv[k]; });
+    DMO_TRY(upload(ctx, gr->XtT, xtT));
+    DMO_TRY(upload(ctx, gr->inv_ls, inv));
     SvGather& ga = gr->gather;
     ga.nlat = nlat;
     ga.n_o0 = n_o0;
@@ -398,12 +377,12 @@ int dmo_svgp_create(dmo_ctx* ctx, int L, int M, int64_t Z, int d, const double* 
     DMO_CUDA(cudaStreamSynchronize(ctx->stream));  // host vectors above are staged from the stack
     sv->groups.push_back(std::move(gr));
   }
-  DMO_TRY(upload(ctx, sv->xlb, lb.data(), d));
-  DMO_TRY(upload(ctx, sv->xrg, rg.data(), d));
-  DMO_TRY(upload(ctx, sv->W, hW.data(), hW.size()));
-  DMO_TRY(upload(ctx, sv->ymean, ym.data(), M));
-  DMO_TRY(upload(ctx, sv->ystd, ys.data(), M));
-  DMO_TRY(upload(ctx, sv->vscale, vs.data(), M));
+  DMO_TRY(upload(ctx, sv->xlb, lb));
+  DMO_TRY(upload(ctx, sv->xrg, rg));
+  DMO_TRY(upload(ctx, sv->W, hW));
+  DMO_TRY(upload(ctx, sv->ymean, ym));
+  DMO_TRY(upload(ctx, sv->ystd, ys));
+  DMO_TRY(upload(ctx, sv->vscale, vs));
   DMO_CHECK_LAUNCH();
   DMO_CUDA(cudaStreamSynchronize(ctx->stream));
   *out = sv.release();
@@ -435,12 +414,11 @@ int dmo_svgp_predict(dmo_ctx* ctx, dmo_svgp* sv, const double* X, int64_t P, dou
   if (!ctx) return DMO_ERR_ARG;
   DMO_CUDA(cudaSetDevice(ctx->device));
   DMO_REQUIRE(sv, "svgp_predict: null model");
-  DMO_REQUIRE(precision == DMO_GP_FP64 || precision == DMO_GP_TENSOR,
-              "svgp_predict: precision must be DMO_GP_FP64 or DMO_GP_TENSOR (got %d)", precision);
-  const bool tensor = precision == DMO_GP_TENSOR;
   const int M = sv->M, L = sv->L, d = sv->d;
-  const int64_t Z = sv->Z, Npad = sv->Npad;
-  DMO_REQUIRE(!tensor || d <= 64, "svgp_predict(tensor): at most 64 input dimensions (got %d); use DMO_GP_FP64", d);
+  const int64_t Z = sv->Z, Npad = sv->groups[0]->ops.Npad;  // every group's planes have Z rows
+  GpUnitPredict up;
+  DMO_TRY(up.check(ctx, "svgp_predict", precision, d));
+  const bool tensor = up.tensor;
   if (P == 0) return DMO_OK;
   DMO_REQUIRE(P > 0 && X && mean, "svgp_predict: bad arguments");
   In<double> x;
@@ -451,70 +429,38 @@ int dmo_svgp_predict(dmo_ctx* ctx, dmo_svgp* sv, const double* X, int64_t P, dou
   const bool want_var = ov.d != nullptr;
   int Gmax = 0;
   for (auto& g : sv->groups) Gmax = g->gather.G > Gmax ? g->gather.G : Gmax;
-  // candidate chunk: one K_* plane (fp16 hi + lo, or float64) within ~6 GiB; the producer grid's y extent stays < 2^16
-  const int64_t tile = tensor ? GP_TC_TILE : GP_F64_TILE;
-  int64_t Pc_max = ((int64_t)6 << 30) / (Npad * (tensor ? 4 : 8));
-  if (Pc_max > ((int64_t)1 << 20)) Pc_max = (int64_t)1 << 20;
-  Pc_max = (Pc_max / tile) * tile;
-  if (Pc_max < tile) Pc_max = tile;
-  const int64_t Pc_alloc = P < Pc_max ? ceil_div(P, tile) * tile : Pc_max;
+  DMO_TRY(up.alloc(ctx, P, Npad, Gmax, want_var));
+  const int64_t Pc_alloc = up.Pc_alloc;
   const int n_mp = (int)(Npad / mt_kstar_span(false));  // the means always come from float64 kernel values
-  int n_vp = 0;
-  if (want_var) {
-    if (tensor) {
-      n_vp = gp_tensor_var_planes(Npad);
-    } else {  // the row blocks of the operators are split so that at least ~2 CTAs per SM exist for small candidate sets
-      int64_t nsplit = ceil_div((int64_t)2 * ctx->sm_count, (Pc_alloc / GP_F64_TILE) * Gmax);
-      const int64_t ntile = Npad / GP_F64_TILE;
-      n_vp = (int)(nsplit > ntile ? ntile : (nsplit < 1 ? 1 : nsplit));
-    }
-  }
-  DevBuf<double> xs, fm, fv, mpart, vnorm, Ks;
-  DevBuf<uint16_t> Kh, Kl;
-  DevBuf<int> abort_flag;
+  DevBuf<double> xs, fm, fv, mpart;
   DMO_TRY(xs.alloc(ctx, (size_t)P * d));
   DMO_TRY(fm.alloc(ctx, (size_t)L * P));
   DMO_TRY(mpart.alloc(ctx, (size_t)n_mp * SV_MAX * Pc_alloc));
-  if (want_var) {
-    DMO_TRY(fv.alloc(ctx, (size_t)L * P));
-    DMO_TRY(vnorm.alloc(ctx, (size_t)n_vp * Gmax * Pc_alloc));
-    if (tensor) {
-      DMO_TRY(Kh.alloc(ctx, (size_t)Pc_alloc * Npad));
-      DMO_TRY(Kl.alloc(ctx, (size_t)Pc_alloc * Npad));
-      DMO_TRY(abort_flag.alloc(ctx, 1));
-      DMO_CUDA(cudaMemsetAsync(abort_flag.p, 0, sizeof(int), ctx->stream));
-    } else {
-      DMO_TRY(Ks.alloc(ctx, (size_t)Pc_alloc * Npad));
-    }
-  }
+  if (want_var) DMO_TRY(fv.alloc(ctx, (size_t)L * P));
   for (auto& gp_ : sv->groups) {
     SvGroup& gr = *gp_;
-    dmo_gp* ops = gr.ops.get();
-    if (tensor && want_var) DMO_TRY(gp_prepare_tensor(ctx, ops));
+    if (tensor && want_var) DMO_TRY(gp_prepare_tensor(ctx, gr.ops));
     DMO_TRY(mt_scale_inputs(ctx, x.d, P, d, sv->xlb.p, sv->xrg.p, gr.inv_ls.p, xs.p));
     for (int64_t p_base = 0; p_base < P; p_base += Pc_alloc) {
       const int64_t Pc = (P - p_base) < Pc_alloc ? (P - p_base) : Pc_alloc;
-      const int64_t Pcpad = ceil_div(Pc, tile) * tile;
+      const int64_t Pcpad = ceil_div(Pc, up.tile) * up.tile;
       {
         ProfileScope ps(ctx, "svgp_kstar");
         // The mean sums k_u' a_l in float64 kernel values on both paths: a_l = s Lz^-T q_mu alternates in sign near
         // interpolation, so sum |k_u a_l| can be ~100 times the mean and fp32 kernel values (~2^-22) would cost ~1e-5.
         // The tensor path adds a K_*-only pass for its fp16 hi / lo plane.
         if (tensor && want_var)
-          DMO_TRY(mt_kstar_produce(ctx, true, xs.p, P, p_base, Pcpad, gr.XtT.p, Z, Npad, d, 0, nullptr, ops->Kexp.p, nullptr, Kh.p,
-                                   Kl.p, mpart.p, Pc_alloc));
+          DMO_TRY(mt_kstar_produce(ctx, true, xs.p, P, p_base, Pcpad, gr.XtT.p, Z, Npad, d, 0, nullptr, gr.ops.Kexp.p, nullptr,
+                                   up.Kh.p, up.Kl.p, mpart.p, Pc_alloc));
         DMO_TRY(mt_kstar_produce(ctx, false, xs.p, P, p_base, Pcpad, gr.XtT.p, Z, Npad, d, gr.gather.nlat, gr.A.p, nullptr,
-                                 tensor ? nullptr : Ks.p, nullptr, nullptr, mpart.p, Pc_alloc));
+                                 tensor ? nullptr : up.Ks.p, nullptr, nullptr, mpart.p, Pc_alloc));
       }
       if (want_var) {
         ProfileScope ps(ctx, "svgp_var");
-        if (tensor)
-          DMO_TRY(gp_var_contract_tensor(ctx, ops, Kh.p, Kl.p, Pc_alloc, 0, Pcpad, vnorm.p, Pc_alloc, abort_flag.p));
-        else
-          DMO_TRY(gp_var_contract_fp64(ctx, ops, Ks.p, 0, Pcpad, n_vp, vnorm.p, Pc_alloc));
+        DMO_TRY(up.contract(ctx, gr.ops, Pcpad));
       }
-      DMO_LAUNCH(sv_gather_kernel, (unsigned)ceil_div(Pc, 256), 256, 0, gr.gather, Pc, p_base, P, mpart.p, n_mp, Pc_alloc, vnorm.p, n_vp,
-                 Pc_alloc, fm.p, want_var ? fv.p : nullptr);
+      DMO_LAUNCH(sv_gather_kernel, (unsigned)ceil_div(Pc, 256), 256, 0, gr.gather, Pc, p_base, P, mpart.p, n_mp, Pc_alloc, up.vnorm.p,
+                 up.n_vp, Pc_alloc, fm.p, want_var ? fv.p : nullptr);
     }
   }
   {
@@ -523,12 +469,7 @@ int dmo_svgp_predict(dmo_ctx* ctx, dmo_svgp* sv, const double* X, int64_t P, dou
                sv->vscale.p, om.d, ov.d);
   }
   DMO_CHECK_LAUNCH();
-  if (tensor && want_var) {
-    int h_abort = 0;
-    DMO_CUDA(cudaMemcpyAsync(&h_abort, abort_flag.p, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (h_abort) return dmo_fail(ctx, DMO_ERR_INTERNAL, "svgp_predict(tensor): pipeline watchdog tripped");
-  }
+  DMO_TRY(up.watchdog(ctx));
   DMO_TRY(om.finish(ctx));
   DMO_TRY(ov.finish(ctx));
   DMO_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -599,13 +540,13 @@ int dmo_svgp_optimal_q(dmo_ctx* ctx, int64_t N, int64_t Z, int d, int L, const d
     DMO_CUDA(cudaMemsetAsync(Li.p, 0, zz * sizeof(double), ctx->stream));
     DMO_TRY(inducing_inverse_factor(ctx, "svgp_optimal_q", l, Z, d, &hZ[l * zd], s, ls, jitter, Z, Li.p));
     // unit K(X, Z) rows of Npad, from the multitask producer with the training inputs as candidates
-    std::vector<double> xsh((size_t)N * d), xtT((size_t)d * Npad, 0.0);
+    std::vector<double> xsh((size_t)N * d);
     for (int64_t n = 0; n < N; ++n)
       for (int k = 0; k < d; ++k) xsh[(size_t)n * d + k] = hx[(size_t)n * d + k] / ls[k];
-    for (int64_t n = 0; n < Z; ++n)
-      for (int k = 0; k < d; ++k) xtT[(size_t)k * Npad + n] = hZ[l * zd + (size_t)n * d + k] / ls[k];
-    DMO_TRY(upload(ctx, xs, xsh.data(), xsh.size()));
-    DMO_TRY(upload(ctx, XtT, xtT.data(), xtT.size()));
+    const std::vector<double> xtT =
+        mt_xt_transposed(Z, d, Npad, [&](int64_t n, int k) { return hZ[l * zd + (size_t)n * d + k] / ls[k]; });
+    DMO_TRY(upload(ctx, xs, xsh));
+    DMO_TRY(upload(ctx, XtT, xtT));
     DevBuf<double> mpart;
     DMO_TRY(mpart.alloc(ctx, (size_t)n_mp));
     DMO_TRY(mt_kstar_produce(ctx, false, xs.p, N, 0, Pcpad, XtT.p, Z, Npad, d, 0, nullptr, nullptr, Kxz.p, nullptr, nullptr, mpart.p,
