@@ -435,9 +435,10 @@ int gp_var_contract_fp64(dmo_ctx* ctx, const GpVarOps& ops, const double* Ks, in
 int gp_predict_fp64(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var) {
   const int64_t N = gp->N, Npad = gp->ops.Npad;
   const int M = gp->M, G = gp->ops.G, d = gp->d;
-  // candidate chunk so that Ks (G x Pc x Npad float64) stays within ~8 GiB
+  // candidate chunk so that Ks (G x Pc x Npad float64) stays within ~8 GiB and kstar_kernel's grid within its limit
   int64_t budget = (int64_t)8 << 30;
   int64_t Pc_max = budget / ((int64_t)G * Npad * 8);
+  if (Pc_max > GP_MAX_CHUNK) Pc_max = GP_MAX_CHUNK;
   Pc_max = (Pc_max / VB) * VB;
   if (Pc_max < VB) Pc_max = VB;
   const int64_t Pc_alloc = P < Pc_max ? ceil_div(P, VB) * VB : Pc_max;

@@ -58,6 +58,10 @@ struct dmo_gp {
   int64_t last_refined = 0;       // rows recomputed by the last DMO_GP_AUTO predict
 };
 
+// Candidates per chunk of any predict, whatever its memory budget allows: the K_* producers put chunk / 32 blocks on
+// the grid's y extent (at most 65535), so 2^20 keeps it at 32768.
+constexpr int64_t GP_MAX_CHUNK = (int64_t)1 << 20;
+
 int gp_predict_fp64(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var);
 
 // Building blocks shared with the multitask posterior (gp_multitask.cu).  All pointers are device pointers.

@@ -331,7 +331,7 @@ int GpUnitPredict::alloc(dmo_ctx* ctx, int64_t P, int64_t Npad, int planes, bool
   // candidate chunk: the one K_* plane (fp16 hi + lo, or float64) within ~6 GiB; the producer grid's y extent stays < 2^16
   tile = tensor ? GP_TC_TILE : GP_F64_TILE;
   int64_t Pc_max = ((int64_t)6 << 30) / (Npad * (tensor ? 4 : 8));
-  if (Pc_max > ((int64_t)1 << 20)) Pc_max = (int64_t)1 << 20;
+  if (Pc_max > GP_MAX_CHUNK) Pc_max = GP_MAX_CHUNK;
   Pc_max = (Pc_max / tile) * tile;
   if (Pc_max < tile) Pc_max = tile;
   Pc_alloc = P < Pc_max ? ceil_div(P, tile) * tile : Pc_max;

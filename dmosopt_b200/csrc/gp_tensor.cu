@@ -942,27 +942,30 @@ int64_t pick_slices(int64_t n_qb, int64_t Npad, int tile, int64_t slots, int64_t
   return best;
 }
 
-// mean-only predict without K_* in memory (d <= 32, M <= 6): see gp_mean_direct_kernel
+// mean-only predict without K_* in memory (d <= 32, M <= 6): see gp_mean_direct_kernel.  Candidate chunks of
+// GP_MAX_CHUNK keep the grid's y extent (candidate blocks of KM_Q) within its limit.
 int gp_mean_direct(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean) {
   const int64_t N = gp->N, Npad = gp->ops.Npad;
   const int M = gp->M, d = gp->d;
   DMO_TRY(prepare_direct_state(ctx, gp));
-  const int64_t n_qb = ceil_div(P, KM_Q);
-  int64_t n_per_block = Npad;
-  const int64_t nsplit = pick_slices(n_qb, Npad, KM_NS, (int64_t)4 * ctx->sm_count, &n_per_block);
-  const int64_t ld = n_qb * KM_Q;
   DevBuf<double> mpart;
-  DMO_TRY(mpart.alloc(ctx, (size_t)nsplit * M * ld));
-  dim3 grid((unsigned)nsplit, (unsigned)n_qb);
-  {
-    ProfileScope ps_(ctx, "gp_mean_direct");
+  for (int64_t p_base = 0; p_base < P; p_base += GP_MAX_CHUNK) {
+    const int64_t Pc = (P - p_base) < GP_MAX_CHUNK ? (P - p_base) : GP_MAX_CHUNK;
+    const int64_t n_qb = ceil_div(Pc, KM_Q);
+    int64_t n_per_block = Npad;
+    const int64_t nsplit = pick_slices(n_qb, Npad, KM_NS, (int64_t)4 * ctx->sm_count, &n_per_block);
+    const int64_t ld = n_qb * KM_Q;
+    DMO_TRY(mpart.alloc(ctx, (size_t)nsplit * M * ld));
+    dim3 grid((unsigned)nsplit, (unsigned)n_qb);
+    {
+      ProfileScope ps_(ctx, "gp_mean_direct");
 #define KM_LAUNCH(ISO_, MT_)                                                                                                  \
   do {                                                                                                                      \
     if (d <= 16)                                                                                                            \
-      DMO_LAUNCH((gp_mean_direct_kernel<ISO_, MT_, 4>), grid, KM_T, 0, dXn, P, (int64_t)0, gp->Xtf.p, N, Npad, n_per_block, \
+      DMO_LAUNCH((gp_mean_direct_kernel<ISO_, MT_, 4>), grid, KM_T, 0, dXn, P, p_base, gp->Xtf.p, N, Npad, n_per_block,     \
                  d, gp->kernel, gp->inv_ls.p, gp->constant.p, gp->alpha.p, mpart.p, ld);                                    \
     else                                                                                                                    \
-      DMO_LAUNCH((gp_mean_direct_kernel<ISO_, MT_, 8>), grid, KM_T, 0, dXn, P, (int64_t)0, gp->Xtf.p, N, Npad, n_per_block, \
+      DMO_LAUNCH((gp_mean_direct_kernel<ISO_, MT_, 8>), grid, KM_T, 0, dXn, P, p_base, gp->Xtf.p, N, Npad, n_per_block,     \
                  d, gp->kernel, gp->inv_ls.p, gp->constant.p, gp->alpha.p, mpart.p, ld);                                    \
   } while (0)
 #define KM_SWITCH(ISO_)        \
@@ -974,16 +977,17 @@ int gp_mean_direct(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, doubl
     case 5: KM_LAUNCH(ISO_, 5); break; \
     default: KM_LAUNCH(ISO_, 6); break; \
   }
-    if (gp->isotropic) {
-      KM_SWITCH(true)
-    } else {
-      KM_SWITCH(false)
-    }
+      if (gp->isotropic) {
+        KM_SWITCH(true)
+      } else {
+        KM_SWITCH(false)
+      }
 #undef KM_SWITCH
 #undef KM_LAUNCH
+    }
+    DMO_LAUNCH(mean_finish_tc_kernel, (unsigned)ceil_div(Pc * M, 256), 256, 0, mpart.p, (int)nsplit, Pc, ld, M, gp->ymean.p,
+               gp->ystd.p, p_base, d_mean);
   }
-  DMO_LAUNCH(mean_finish_tc_kernel, (unsigned)ceil_div(P * M, 256), 256, 0, mpart.p, (int)nsplit, P, ld, M, gp->ymean.p,
-             gp->ystd.p, (int64_t)0, d_mean);
   DMO_CHECK_LAUNCH();
   return DMO_OK;  // mpart is released in stream order
 }
@@ -1053,8 +1057,9 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
     return gp_mean_direct(ctx, gp, dXn, P, d_mean);  // nothing but the mean is wanted: K_* stays in registers
   DMO_TRY(gp_prepare_tensor(ctx, gp->ops));
   constexpr int64_t TMv = KM_Q;  // candidate padding: the K_* producers write 256-candidate blocks
-  // candidate chunk: K_* hi/lo (2 x G x Pc x Npad fp16) within ~6 GiB
+  // candidate chunk: K_* hi/lo (2 x G x Pc x Npad fp16) within ~6 GiB, and the producers' grids within their limit
   int64_t Pc_max = ((int64_t)6 << 30) / ((int64_t)G * Npad * 4);
+  if (Pc_max > GP_MAX_CHUNK) Pc_max = GP_MAX_CHUNK;
   Pc_max = (Pc_max / TMv) * TMv;
   if (Pc_max < TMv) Pc_max = TMv;
   const int64_t Pc_alloc = P < Pc_max ? ceil_div(P, TMv) * TMv : Pc_max;
