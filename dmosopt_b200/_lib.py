@@ -82,6 +82,11 @@ _SIGNATURES = {
     "dmo_svgp_groups": (_c_int, [_vp, _vp, ctypes.POINTER(_c_int), ctypes.POINTER(_c_int)]),
     "dmo_svgp_destroy": (_c_int, [_vp, _vp]),
     "dmo_svgp_optimal_q": (_c_int, [_vp, _c_i64, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _c_dbl, _c_int, _vp, _vp]),
+    "dmo_svgp_fit_create": (_c_int, [_vp, _c_i64, _c_int, _c_int, _c_int, _c_i64, _vp, _vp, _vp, _c_int, _c_dbl, ctypes.POINTER(_vp)]),
+    "dmo_svgp_fit_destroy": (_c_int, [_vp, _vp]),
+    "dmo_svgp_fit_natgrad": (_c_int, [_vp, _vp, _vp, _c_i64, _vp, _vp, _vp, _vp, _c_dbl]),
+    "dmo_svgp_fit_elbo_grad": (_c_int, [_vp, _vp, _vp, _c_i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "dmo_svgp_fit_q": (_c_int, [_vp, _vp, _vp, _vp]),
     "dmo_mtgp_lml_grad": (_c_int, [_vp, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dmo_gp_lml_grad": (_c_int, [_vp, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dmo_nsga2_step": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_i64, _c_int, _c_int, _c_dbl, _c_dbl, _c_dbl, _vp, _vp, _vp, _vp, _c_u64, _c_u64,
@@ -932,6 +937,73 @@ def svgp_optimal_q(X, y, Zpts, variance, length_scale, noise, jitter=1e-2, induc
     _check(load_library().dmo_svgp_optimal_q(context(), N, Z, d, L, _ptr(X), _ptr(y), _ptr(Zp), _ptr(s), _ptr(ls), _ptr(nz), float(jitter),
                                              int(bool(inducing_is_data)), _ptr(q_mu), _ptr(q_sqrt)), "dmo_svgp_optimal_q")
     return q_mu, q_sqrt
+
+
+class SVGPFitState:
+    """Owns a dmo_svgp_fit: the training state of one GPflow variational model (L latents over the inducing points Zpts
+    (Z,d), M outputs; inducing_is_data: VGP, Z = X) on X (N,d), Y (N,M), with q starting at N(0, I)."""
+
+    def __init__(self, X, Y, Zpts, L, jitter=1e-2, inducing_is_data=False):
+        X = _f64(X)
+        N, d = X.shape
+        Yt = _f64(np.asarray(Y, dtype=np.float64).reshape(N, -1).T)
+        M = Yt.shape[0]
+        Zp = None if inducing_is_data else _f64(Zpts)
+        Z = N if inducing_is_data else Zp.shape[0]
+        if Zp is not None and Zp.shape != (Z, d):
+            raise DmoError(f"dmo_svgp_fit_create: Zpts must be (Z, {d}), got shape {Zp.shape}")
+        self.N, self.d, self.M, self.L, self.Z = N, d, M, int(L), Z
+        h = _vp()
+        _check(load_library().dmo_svgp_fit_create(context(), N, d, M, self.L, Z, _ptr(X), _ptr(Yt), _ptr(Zp), int(bool(inducing_is_data)),
+                                                  float(jitter), ctypes.byref(h)), "dmo_svgp_fit_create")
+        self._h = h
+
+    def _args(self, batch, variance, length_scale, noise, W):
+        b = np.ascontiguousarray(batch, dtype=np.int64).reshape(-1)
+        s = _f64(variance).reshape(self.L)
+        ls = _f64(length_scale).reshape(self.L, self.d)
+        nz = _f64(noise).reshape(self.M)
+        Wm = None if W is None else _f64(W).reshape(self.M, self.L)
+        return b, s, ls, nz, Wm
+
+    def natgrad(self, batch, variance, length_scale, noise, W=None, gamma=1.0):
+        """One natural-gradient step on q (in place)."""
+        b, s, ls, nz, Wm = self._args(batch, variance, length_scale, noise, W)
+        _check(load_library().dmo_svgp_fit_natgrad(context(), self._h, _ptr(b), b.shape[0], _ptr(s), _ptr(ls), _ptr(nz), _ptr(Wm), float(gamma)),
+               "dmo_svgp_fit_natgrad")
+
+    def elbo_grad(self, batch, variance, length_scale, noise, W=None, grad=True):
+        """(ell (M,), kl (L,), grads or None): grads a dict of d ELBO / d variance (L,), length_scale (L,d), noise (M,) and
+        W (M,L) (when W is given) at the current q."""
+        b, s, ls, nz, Wm = self._args(batch, variance, length_scale, noise, W)
+        ell, kl = np.empty(self.M), np.empty(self.L)
+        g = None
+        if grad:
+            g = {"variance": np.empty(self.L), "length_scale": np.empty((self.L, self.d)), "noise": np.empty(self.M),
+                 "W": None if Wm is None else np.empty((self.M, self.L))}
+        gp = (lambda k: None) if g is None else (lambda k: _ptr(g[k]))
+        _check(load_library().dmo_svgp_fit_elbo_grad(context(), self._h, _ptr(b), b.shape[0], _ptr(s), _ptr(ls), _ptr(nz), _ptr(Wm), _ptr(ell),
+                                                     _ptr(kl), gp("variance"), gp("length_scale"), gp("noise"), gp("W")),
+               "dmo_svgp_fit_elbo_grad")
+        return ell, kl, g
+
+    def q(self):
+        """(q_mu (L,Z), lower-triangular q_sqrt (L,Z,Z))."""
+        q_mu = np.empty((self.L, self.Z))
+        q_sqrt = np.empty((self.L, self.Z, self.Z))
+        _check(load_library().dmo_svgp_fit_q(context(), self._h, _ptr(q_mu), _ptr(q_sqrt)), "dmo_svgp_fit_q")
+        return q_mu, q_sqrt
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and _lib is not None and _ctx is not None:
+            _lib.dmo_svgp_fit_destroy(_ctx, self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 # --------------------------------------------------------------------------- A16/A17

@@ -125,6 +125,14 @@ int upload(dmo_ctx* ctx, DevBuf<T>& dst, const std::vector<T>& src) {
   return DMO_OK;
 }
 
+// ---- dense float64 helpers of the variational posterior (gp_variational.cu), shared with its training (gp_variational_fit.cu)
+// C[i][j] = alpha sum_k A(i, k) B(k, j) + (i == j ? diag : 0), i < m, j < n (rows of ldc), A(i, k) = A[i sai + k sak],
+// B(k, j) = B[k sbk + j sbj]; every output one fixed-order chain.  Not synchronised.
+int sv_gemm(dmo_ctx* ctx, int64_t m, int64_t n, int64_t K, double alpha, const double* A, int64_t sai, int64_t sak, const double* B,
+            int64_t sbk, int64_t sbj, double diag, double* C, int64_t ldc);
+// O = s J C' J (rows of ldo) for a row-major n x n lower-triangular C (J reverses the order): lower triangular
+int sv_flip(dmo_ctx* ctx, const double* C, int64_t n, double s, double* O, int64_t ldo);
+
 // ---- multitask model (gp_multitask.cu): the block factorisation shared by dmo_mtgp_create and dmo_mtgp_lml_grad --
 constexpr int MT_MAX = 8;        // tasks per model
 constexpr int MT_FIT_DMAX = 90;  // input dimensions dmo_gp_fit takes

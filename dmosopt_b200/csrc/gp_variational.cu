@@ -194,13 +194,6 @@ __global__ void sv_mix_kernel(int64_t P, int L, int M, const double* __restrict_
   if (var) var[t] = v * vscale[m];
 }
 
-int gemm(dmo_ctx* ctx, int64_t m, int64_t n, int64_t K, double alpha, const double* A, int64_t sai, int64_t sak, const double* B,
-         int64_t sbk, int64_t sbj, double diag, double* C, int64_t ldc) {
-  dim3 g((unsigned)ceil_div(n, GT), (unsigned)ceil_div(m, GT));
-  DMO_LAUNCH(sv_gemm_kernel, g, 256, 0, m, n, K, alpha, A, sai, sak, B, sbk, sbj, diag, C, ldc);
-  return DMO_OK;
-}
-
 // Lz^-1 (rows of ldo, lower triangle; the rest untouched) of K(Z, Z) = s k(Z / ell) + jitter I, Z (n, d) on the host
 int inducing_inverse_factor(dmo_ctx* ctx, const char* who, int l, int64_t n, int d, const double* Zl, double s, const double* ls,
                             double jitter, int64_t ldo, double* dst) {
@@ -227,6 +220,18 @@ int householder_qr(dmo_ctx* ctx, double* C, int64_t n, double* tau) {
 bool bits_equal(const double* a, const double* b, size_t n) { return memcmp(a, b, n * sizeof(double)) == 0; }
 
 }  // namespace
+
+int sv_gemm(dmo_ctx* ctx, int64_t m, int64_t n, int64_t K, double alpha, const double* A, int64_t sai, int64_t sak, const double* B,
+            int64_t sbk, int64_t sbj, double diag, double* C, int64_t ldc) {
+  dim3 g((unsigned)ceil_div(n, GT), (unsigned)ceil_div(m, GT));
+  DMO_LAUNCH(sv_gemm_kernel, g, 256, 0, m, n, K, alpha, A, sai, sak, B, sbk, sbj, diag, C, ldc);
+  return DMO_OK;
+}
+
+int sv_flip(dmo_ctx* ctx, const double* C, int64_t n, double s, double* O, int64_t ldo) {
+  DMO_LAUNCH(sv_flip_kernel, (unsigned)ceil_div(n * n, 256), 256, 0, C, n, s, O, ldo);
+  return DMO_OK;
+}
 
 struct SvGroup {
   std::vector<int> lat, o0;       // latents of the group; the O0 plane of each (its O1 plane is n_o0 + its index)
@@ -350,9 +355,9 @@ int dmo_svgp_create(dmo_ctx* ctx, int L, int M, int64_t Z, int d, const double* 
       const int l = gr->lat[j];
       const double* Li = ops.Linv.p + gr->o0[j] * plane;  // unscaled Lz^-1 (the O0 planes are scaled below)
       // a_l = s_l Lz^-T q_mu:  a[i] = s sum_k Li[k][i] q_mu[k]
-      DMO_TRY(gemm(ctx, Z, 1, Z, hs[l], Li, 1, Npad, qm_d.p + (size_t)l * Z, 1, 0, 0.0, gr->A.p + (size_t)j * Npad, 1));
+      DMO_TRY(sv_gemm(ctx,Z, 1, Z, hs[l], Li, 1, Npad, qm_d.p + (size_t)l * Z, 1, 0, 0.0, gr->A.p + (size_t)j * Npad, 1));
       // V J by columns: column c = row c of Ct, Ct[c][r] = V[r][Z-1-c] = sum_k Li[k][Z-1-c] q_sqrt[k][r]
-      DMO_TRY(gemm(ctx, Z, Z, Z, 1.0, Li + (Z - 1), -1, Npad, qs_d.p + (size_t)l * zz, Z, 1, 0.0, Ct.p, Z));
+      DMO_TRY(sv_gemm(ctx,Z, Z, Z, 1.0, Li + (Z - 1), -1, Npad, qs_d.p + (size_t)l * zz, Z, 1, 0.0, Ct.p, Z));
       DMO_TRY(householder_qr(ctx, Ct.p, Z, tau.p));
       DMO_LAUNCH(sv_flip_kernel, (unsigned)ceil_div((int64_t)zz, 256), 256, 0, Ct.p, Z, hs[l], ops.Linv.p + (n_o0 + j) * plane, Npad);
     }
@@ -552,14 +557,14 @@ int dmo_svgp_optimal_q(dmo_ctx* ctx, int64_t N, int64_t Z, int d, int L, const d
     DMO_TRY(mt_kstar_produce(ctx, false, xs.p, N, 0, Pcpad, XtT.p, Z, Npad, d, 0, nullptr, nullptr, Kxz.p, nullptr, nullptr, mpart.p,
                              Pcpad));
     // A' = s K(X, Z) Lz^-T  (N x Z):  At[p][i] = s sum_k Kxz[p][k] Li[i][k]
-    DMO_TRY(gemm(ctx, N, Z, Z, s, Kxz.p, Npad, 1, Li.p, 1, Z, 0.0, At.p, Z));
+    DMO_TRY(sv_gemm(ctx,N, Z, Z, s, Kxz.p, Npad, 1, Li.p, 1, Z, 0.0, At.p, Z));
     DMO_CHECK_LAUNCH();
     DMO_CUDA(cudaStreamSynchronize(ctx->stream));  // xsh / xtT are staged from the stack
     }
     // B = I + A A' / sigma^2 (Z x Z)
-    DMO_TRY(gemm(ctx, Z, Z, N, 1.0 / s2, At.p, 1, Z, At.p, Z, 1, 1.0, Bm.p, Z));
+    DMO_TRY(sv_gemm(ctx,Z, Z, N, 1.0 / s2, At.p, 1, Z, At.p, Z, 1, 1.0, Bm.p, Z));
     // b = A y / sigma^2
-    DMO_TRY(gemm(ctx, Z, 1, N, 1.0 / s2, At.p, 1, Z, iy.d + (size_t)l * N, 1, 0, 0.0, bvec.p, 1));
+    DMO_TRY(sv_gemm(ctx,Z, 1, N, 1.0 / s2, At.p, 1, Z, iy.d + (size_t)l * N, 1, 0, 0.0, bvec.p, 1));
     // S = B^-1 = U U' with U = J Lc^-T J lower triangular, Lc = chol(J B J):  B^-1 = J (Lc Lc')^-1 J = (J Lc^-T J)(J Lc^-1 J)
     DMO_LAUNCH(sv_reverse_pad_kernel, (unsigned)ceil_div(ld * ld, 256), 256, 0, Bm.p, Z, ld, Lci.p);
     DMO_CUDA(cudaMemsetAsync(info.p, 0, sizeof(int), ctx->stream));
@@ -573,8 +578,8 @@ int dmo_svgp_optimal_q(dmo_ctx* ctx, int64_t N, int64_t Z, int d, int L, const d
     double* U = oqs.d + (size_t)l * zz;
     DMO_LAUNCH(sv_flip_kernel, (unsigned)ceil_div((int64_t)zz, 256), 256, 0, Bm.p, Z, 1.0, U, Z);
     // q_mu = U (U' b)
-    DMO_TRY(gemm(ctx, Z, 1, Z, 1.0, U, 1, Z, bvec.p, 1, 0, 0.0, tvec.p, 1));
-    DMO_TRY(gemm(ctx, Z, 1, Z, 1.0, U, Z, 1, tvec.p, 1, 0, 0.0, oqm.d + (size_t)l * Z, 1));
+    DMO_TRY(sv_gemm(ctx,Z, 1, Z, 1.0, U, 1, Z, bvec.p, 1, 0, 0.0, tvec.p, 1));
+    DMO_TRY(sv_gemm(ctx,Z, 1, Z, 1.0, U, Z, 1, tvec.p, 1, 0, 0.0, oqm.d + (size_t)l * Z, 1));
     DMO_CHECK_LAUNCH();
     DMO_CUDA(cudaStreamSynchronize(ctx->stream));  // xsh / xtT are staged from the stack
   }

@@ -10,8 +10,10 @@ Every class keeps the reference's constructor keywords and adds:
   reference's rule with ``np.random.default_rng(seed)`` instead of the global generator (a documented deviation); without
   ``q_mu`` / ``q_sqrt`` q is set to its optimum for the Gaussian likelihood (dmo_svgp_optimal_q).  CRV requires q and W.
   This trains nothing: the kernel hyper-parameters are taken as given.
-- ``fit``: "reference" trains through the reference class (needs gpflow and tensorflow) and reads its ``posterior()``
-  objects out by gpflow 2.9.2's attribute names; None means "reference" when gpflow imports.
+- ``fit``: "gpu" trains on the GPU (svgp_fit: natural-gradient steps on q, keras' Adam on the hyper-parameters, the
+  reference's stopping rule; the reference's training keywords apply) and keeps ``hyperparameters`` and ``fit_info``;
+  "reference" trains through the reference class (needs gpflow and tensorflow) and reads its ``posterior()`` objects out
+  by gpflow 2.9.2's attribute names; None means "reference" when gpflow imports.
 
 The variance is that of the latent f (GPflow's predict_f: no likelihood noise).  ``predict``'s ``batch_size`` split of
 the reference is row-independent and is not repeated.
@@ -100,6 +102,186 @@ def choose_inducing(xn, inducing_fraction, min_inducing, rng):
     return xn[rng.choice(N, size=m, replace=False), :].copy()
 
 
+# ---- training on the GPU (fit="gpu") ---------------------------------------------------------------------------------
+# The reference's parameterisation (DESIGN.md section 4.4, restated from gpflow 2.9.2, not checked against it): length
+# scales lo + (hi - lo) sigmoid(raw) (bounded_parameter), kernel variance softplus(raw), likelihood variance
+# 1e-6 + softplus(raw); W (CRV) untransformed.  Z, q_mu and q_sqrt are not trained by Adam.
+LIKELIHOOD_LOWER = 1e-6
+TRAIN_DEFAULTS = {"svgp": dict(batch_size=50, natgrad_gamma=0.1, n_iter=30000), "vgp": dict(batch_size=None, natgrad_gamma=1.0, n_iter=3000)}
+
+
+def _softplus(x):
+    return np.logaddexp(0.0, x)
+
+
+def _sigmoid(x):
+    return 1.0 / (1.0 + np.exp(-x))
+
+
+def _inv_softplus(y):
+    y = np.asarray(y, dtype=np.float64)
+    return y + np.log(-np.expm1(-y))
+
+
+class KerasAdam:
+    """keras 2.14's Adam (beta 0.9 / 0.999, epsilon 1e-7) on a dict of float64 arrays: m <- m + (g - m)(1 - b1),
+    v <- v + (g^2 - v)(1 - b2), p <- p - lr sqrt(1 - b2^t) / (1 - b1^t) m / (sqrt(v) + eps)."""
+
+    def __init__(self, lr=0.01, beta_1=0.9, beta_2=0.999, epsilon=1e-7):
+        self.lr, self.b1, self.b2, self.eps = lr, beta_1, beta_2, epsilon
+        self.t, self.m, self.v = 0, {}, {}
+
+    def step(self, params, grads):
+        self.t += 1
+        alpha = self.lr * np.sqrt(1.0 - self.b2**self.t) / (1.0 - self.b1**self.t)
+        for k, g in grads.items():
+            m = self.m.get(k, np.zeros_like(g))
+            v = self.v.get(k, np.zeros_like(g))
+            m = m + (g - m) * (1.0 - self.b1)
+            v = v + (g * g - v) * (1.0 - self.b2)
+            self.m[k], self.v[k] = m, v
+            params[k] = params[k] - alpha * m / (np.sqrt(v) + self.eps)
+
+
+def mean_elbo_pct_change(elbo_log):
+    """The reference's stopping statistic: mean percent change of the ELBO log over its last 100 differences."""
+    elbo_change = np.convolve(elbo_log, np.array([1, -1]), "same")[1:]
+    return float(np.mean((elbo_change / np.abs(elbo_log[1:]) * 100)[-100:]))
+
+
+class MinibatchStream:
+    """Consecutive B-slices of a stream of independent permutations of range(N) drawn from np.random.default_rng(seed)
+    (the reference shuffles a repeated tf.data set; a documented deviation)."""
+
+    def __init__(self, N, B, seed):
+        self.N, self.B = int(N), int(B)
+        self.rng = np.random.default_rng(seed)
+        self.buf = np.empty(0, dtype=np.int64)
+
+    def next(self):
+        while self.buf.shape[0] < self.B:
+            self.buf = np.concatenate([self.buf, self.rng.permutation(self.N).astype(np.int64)])
+        b, self.buf = self.buf[: self.B], self.buf[self.B :]
+        return b
+
+
+class _FitModel:
+    """One GPflow model in training: its state on the GPU, raw parameters, Adam, batch stream and ELBO log.  outs: the
+    columns of Y it models; K: distinct kernels (1: SIV's shared kernel, else one per latent)."""
+
+    def __init__(self, xn, yn, Z, outs, L, K, vgp, opts, seed, W0):
+        self.outs, self.L, self.K, self.vgp = outs, L, K, vgp
+        self.N, d = xn.shape
+        self.state = _lib.SVGPFitState(xn, yn[:, outs], Z, L, jitter=JITTER, inducing_is_data=vgp)
+        lo, hi = opts["lengthscale_bounds"]
+        self.lo, self.hi = float(lo), float(hi)
+        self.raw = {"lengthscale": np.full((K, d), np.log((1.0 - self.lo) / (self.hi - 1.0))),
+                    "variance": np.full(K, _inv_softplus(1.0)),
+                    "noise": np.array([_inv_softplus(opts["likelihood_sigma"] - LIKELIHOOD_LOWER)])}
+        if W0 is not None:
+            self.raw["W"] = np.array(W0, dtype=np.float64)
+        self.adam = KerasAdam(lr=opts["adam_lr"])
+        B = self.N if vgp or opts["batch_size"] is None else min(int(opts["batch_size"]), self.N)
+        self.stream = None if vgp else MinibatchStream(self.N, B, seed)
+        self.elbo_log, self.iterations, self.stop_reason = [], 0, "n_iter"
+
+    def natural(self):
+        M = len(self.outs)
+        ls = np.broadcast_to(self.lo + (self.hi - self.lo) * _sigmoid(self.raw["lengthscale"]), (self.L, self.raw["lengthscale"].shape[1]))
+        s = np.broadcast_to(_softplus(self.raw["variance"]), (self.L,))
+        noise = np.full(M, LIKELIHOOD_LOWER + _softplus(self.raw["noise"][0]))
+        return np.ascontiguousarray(s), np.ascontiguousarray(ls), noise, self.raw.get("W")
+
+    def batch(self):
+        return np.arange(self.N, dtype=np.int64) if self.stream is None else self.stream.next()
+
+    def elbo(self, batch):
+        ell, kl, _ = self.state.elbo_grad(batch, *self.natural(), grad=False)
+        return float(np.sum(ell) - np.sum(kl))
+
+    def step(self, gamma):
+        """Natural-gradient step on one batch, then an Adam step on the next at the new q."""
+        self.state.natgrad(self.batch(), *self.natural(), gamma=gamma)
+        s, ls, noise, W = self.natural()
+        _, _, g = self.state.elbo_grad(self.batch(), s, ls, noise, W)
+        raw = self.raw
+        gl = g["length_scale"] if self.K == self.L else g["length_scale"].sum(axis=0, keepdims=True)
+        gs = g["variance"] if self.K == self.L else g["variance"].sum(keepdims=True)
+        sg = _sigmoid(raw["lengthscale"])
+        # loss = -ELBO: gradients with respect to the raw parameters, negated
+        grads = {"lengthscale": -gl * ((self.hi - self.lo) * (sg * (1.0 - sg))),
+                 "variance": -gs * _sigmoid(raw["variance"]),
+                 "noise": -np.array([np.sum(g["noise"])]) * _sigmoid(raw["noise"])}
+        if "W" in raw:
+            grads["W"] = -g["W"]
+        self.adam.step(raw, grads)
+
+
+def svgp_fit(kind, xn, yn, Z=None, *, lengthscale_bounds=(1e-6, 100.0), likelihood_sigma=1e-4, natgrad_gamma=None, adam_lr=0.01,
+             n_iter=None, min_elbo_pct_change=0.1, batch_size=-1, seed=None, logger=None, W0=None, name=None):
+    """Train a variational surrogate on the GPU with the reference's loop (dmosopt/model.py:98-1179): per iteration a
+    natural-gradient step on q (batch b1), an Adam step on the hyper-parameters at the new q (batch b2) and, every 10th
+    iteration, the ELBO on batch b3 appended to the log (VGP: full data, the ELBO after every iteration); the stopping
+    rule from iteration 2000 (VGP: 200).  kind: "svgp" / "vgp" (one model per output, trained in lockstep; a model
+    that stops leaves the loop), "siv" (one model, one shared kernel), "spv" (one model, a kernel per output) or "crv"
+    (like spv, plus W (M,M) trained by Adam, initial W0).  xn (N,d), yn (N,M) normalised; Z (Z,d) shared, or
+    (M,Z,d) one set per output for svgp; None for vgp.  natgrad_gamma / n_iter / batch_size default to the reference's
+    per class.  Returns (hyperparameters, info): the ``hyperparameters=`` dict of the class (with Z, q_mu, q_sqrt and W),
+    and info with ``elbo`` (one log per model), ``iterations`` and ``stop_reason`` (one per model)."""
+    xn = np.ascontiguousarray(xn, dtype=np.float64)
+    yn = np.ascontiguousarray(yn, dtype=np.float64).reshape(xn.shape[0], -1)
+    N, d = xn.shape
+    M = yn.shape[1]
+    vgp = kind == "vgp"
+    dflt = TRAIN_DEFAULTS["vgp" if vgp else "svgp"]
+    gamma = dflt["natgrad_gamma"] if natgrad_gamma is None else float(natgrad_gamma)
+    n_iter = dflt["n_iter"] if n_iter is None else int(n_iter)
+    batch_size = dflt["batch_size"] if batch_size == -1 else batch_size
+    name = name or {"svgp": "SVGP_Matern", "vgp": "VGP_Matern", "siv": "SIV_Matern", "spv": "SPV_Matern", "crv": "CRV_Matern"}[kind]
+    opts = dict(lengthscale_bounds=lengthscale_bounds, likelihood_sigma=float(likelihood_sigma), adam_lr=adam_lr, batch_size=batch_size)
+    base = 0 if seed is None else int(seed)
+    if kind in ("svgp", "vgp"):
+        Zs = [None] * M if vgp else list(np.broadcast_to(np.asarray(Z, dtype=np.float64), (M,) + np.shape(Z)[-2:]))
+        models = [_FitModel(xn, yn, Zs[i], [i], 1, 1, vgp, opts, [base, i], None) for i in range(M)]
+    else:
+        Zs = np.asarray(Z, dtype=np.float64).reshape(-1, d)
+        models = [_FitModel(xn, yn, Zs, list(range(M)), M, 1 if kind == "siv" else M, False, opts, [base, 0],
+                            W0 if kind == "crv" else None)]
+    log_every, warmup, report = (1, 200, 100) if vgp else (10, 2000, 1000)
+    active = list(models)
+    for it in range(n_iter):
+        if not active:
+            break
+        for mdl in list(active):
+            mdl.step(gamma)
+            mdl.iterations = it + 1
+            if it % log_every == 0:
+                mdl.elbo_log.append(mdl.elbo(mdl.batch()))
+            if it % report == 0 and logger is not None:
+                logger.info(f"{name}: iteration {it} likelihood: {mdl.elbo_log[-1]:.04f}")
+            if it >= warmup:
+                pct = mean_elbo_pct_change(np.asarray(mdl.elbo_log))
+                if it % 1000 == 0 and logger is not None:
+                    logger.info(f"{name}: iteration {it} mean elbo pct change: {pct:.04f}")
+                if pct < min_elbo_pct_change:
+                    if logger is not None:
+                        logger.info(f"{name}: likelihood change at iteration {it + 1} is less than {min_elbo_pct_change} percent")
+                    mdl.stop_reason = "elbo_pct_change"
+                    active.remove(mdl)
+    nat = [m.natural() for m in models]
+    qs = [m.state.q() for m in models]
+    hp = {"lengthscales": np.concatenate([n[1] for n in nat]), "variance": np.concatenate([n[0] for n in nat]),
+          "likelihood_variance": np.concatenate([n[2] for n in nat]), "q_mu": np.concatenate([q[0] for q in qs]),
+          "q_sqrt": np.concatenate([q[1] for q in qs])}
+    if not vgp:
+        hp["Z"] = np.stack(Zs) if kind == "svgp" else np.broadcast_to(Zs, (M,) + Zs.shape).copy()
+    if kind == "crv":
+        hp["W"] = models[0].raw["W"].copy()
+    info = {"elbo": [np.asarray(m.elbo_log) for m in models], "iterations": [m.iterations for m in models],
+            "stop_reason": [m.stop_reason for m in models]}
+    return hp, info
+
+
 class _VariationalGP:
     """Shared body of the five classes: data selection and normalisation as the reference's, then the posterior state
     (from the reference fit or from ``hyperparameters``) uploaded to one dmo_svgp."""
@@ -123,16 +305,21 @@ class _VariationalGP:
         self.return_mean_variance = return_mean_variance
         self.precision = _lib.GP_TENSOR if precision in ("tensor", _lib.GP_TENSOR) else _lib.GP_FP64
         self.stats = {}
+        self.fit_info = None
         if hyperparameters is not None and fit is not None:
             raise ValueError(f"{self.name}: fit={fit!r} and hyperparameters= conflict; pass one of them")
-        if hyperparameters is None:
+        if fit not in (None, "reference", "gpu"):
+            raise ValueError(f"{self.name}: fit must be 'gpu', 'reference' or None (got {fit!r})")
+        if self.name == "CRV_Matern" and fit == "gpu" and num_latent_gps not in (None, nOutput):
+            raise ValueError(f"CRV_Matern: the GPU fit builds one kernel per output and an (M, M) W; num_latent_gps must be "
+                             f"None or nOutput={nOutput} (got {num_latent_gps})")
+        if hyperparameters is None and fit != "gpu":
             if fit is None:
                 if not _gpflow_available():
                     raise RuntimeError(f"{self.name}: training needs gpflow and tensorflow, which are not importable; pass "
-                                       "hyperparameters= (lengthscales, variance, likelihood_variance) to predict without them")
+                                       "hyperparameters= (lengthscales, variance, likelihood_variance) to predict without them, "
+                                       "or fit='gpu' to train on the GPU")
                 fit = "reference"
-            if fit != "reference":
-                raise ValueError(f"{self.name}: fit must be 'reference' or None (got {fit!r})")
             if batch_size is not None:  # else the reference class's own default (50 for the SVGP forms, None for VGP)
                 kwargs["batch_size"] = batch_size
             ref = self._fit_with_reference(xin, yin, nInput, nOutput, xlb, xub, seed=seed, inducing_fraction=inducing_fraction,
@@ -159,6 +346,8 @@ class _VariationalGP:
         std = [np.std(yin[:, i], axis=0) for i in range(nOutput)]
         self.y_train_std = np.asarray([s if s != 0.0 else 1.0 for s in std], dtype=self.std_dtype)  # handle_zeros_in_scale
         yn = np.column_stack([(yin[:, i] - self.y_train_mean[i]) / self.y_train_std[i] for i in range(nOutput)])
+        if fit == "gpu":
+            hyperparameters = self._fit_on_gpu(xn, yn, nOutput, seed, inducing_fraction, min_inducing, batch_size, logger, kwargs)
         hp = hyperparameters
         L = nOutput if self.name != "CRV_Matern" else int(num_latent_gps or nOutput)
         ls = np.asarray(hp["lengthscales"], dtype=np.float64).reshape(-1, nInput)
@@ -191,7 +380,30 @@ class _VariationalGP:
         if self.name == "CRV_Matern" and W is None:
             raise ValueError("CRV_Matern: hyperparameters need W (M, L)")
         self.hyperparameters = dict(hp, Z=Z, q_mu=q_mu, q_sqrt=q_sqrt)
+        if fit == "gpu" and self.all_points:
+            del self.hyperparameters["Z"]  # the training inputs: hyperparameters= takes no Z for VGP
         self._upload(dict(Z=Z, variance=var, lengthscales=ls, q_mu=q_mu, q_sqrt=q_sqrt, W=W), JITTER)
+
+    def _fit_on_gpu(self, xn, yn, nOutput, seed, inducing_fraction, min_inducing, batch_size, logger, kw):
+        """svgp_fit on the normalised data, with the inducing points of the hyperparameters= path (the same seeded
+        draws) and, for CRV, W ~ N(0, 1) drawn next from the same generator; fit_info keeps the training record."""
+        kind = {"SVGP_Matern": "svgp", "VGP_Matern": "vgp", "SIV_Matern": "siv", "SPV_Matern": "spv", "CRV_Matern": "crv"}[self.name]
+        rng = np.random.default_rng(seed)
+        Z = None
+        if self.per_output_inducing:
+            Z = np.stack([choose_inducing(xn, inducing_fraction, min_inducing, rng) for _ in range(nOutput)])
+        elif not self.all_points:
+            Z = choose_inducing(xn, inducing_fraction, min_inducing, rng)
+        W0 = rng.standard_normal((nOutput, nOutput)) if kind == "crv" else None
+        opts = {k: kw[k] for k in ("natgrad_gamma", "adam_lr", "n_iter", "min_elbo_pct_change") if kw.get(k) is not None}
+        if kw.get("gp_lengthscale_bounds") is not None:
+            opts["lengthscale_bounds"] = kw["gp_lengthscale_bounds"]
+        if kw.get("gp_likelihood_sigma") is not None:
+            opts["likelihood_sigma"] = kw["gp_likelihood_sigma"]
+        if batch_size is not None:
+            opts["batch_size"] = batch_size
+        hp, self.fit_info = svgp_fit(kind, xn, yn, Z, seed=seed, logger=logger, W0=W0, name=self.name, **opts)
+        return hp
 
     def _fit_with_reference(self, xin, yin, nInput, nOutput, xlb, xub, **kw):
         """Train with the reference class (unchanged)."""

@@ -307,6 +307,39 @@ int dmo_svgp_optimal_q(dmo_ctx* ctx, int64_t N, int64_t Z, int d, int L, const d
                        const double* Zpts, const double* variance, const double* length_scale, const double* noise,
                        double jitter, int inducing_is_data, double* q_mu_out, double* q_sqrt_out);
 
+/* ---- training of the variational surrogates (gp_variational_fit.cu) ------------------------------------------------
+ * A dmo_svgp_fit is the device-resident training state of one GPflow model: L <= 8 whitened latents over one set of
+ * inducing points, mixed into M <= 8 outputs by W (M,L) (NULL: the identity, M == L).  SVGP_Matern and VGP_Matern are
+ * one state per output (L = M = 1), SIV / SPV / CRV one state for the whole model.  q_l is held in natural
+ * parameters (Lambda_l = S_l^-1, theta1_l = Lambda_l m_l) with its factor kept current; it starts at N(0, I).
+ * dmo_svgp_fit_create: X (N,d) normalised inputs, Y (M,N) normalised targets, Zpts (Z,d) the inducing points shared by
+ *   the latents (1 <= Z <= 8192, d <= 90); inducing_is_data != 0 is GPflow's VGP: Z = X (Zpts ignored, Z == N),
+ *   f(X) = Lz v, and every call takes the full data.  jitter is added to K(Z, Z).
+ * Every call takes the model's hyper-parameters -- variance (L,) > 0, length_scale (L,d) > 0, noise (M,) > 0 (one
+ * likelihood variance per output; a model with one variance passes copies), W (M,L) or NULL -- and one minibatch:
+ * batch (B,) int64 indices into [0, N), 1 <= B <= N (VGP: a permutation of [0, N)); the data term is scaled by N / B.
+ * A K(Z, Z) + jitter I that is not positive definite gives DMO_ERR_ARG naming the latent.
+ * dmo_svgp_fit_natgrad: one natural-gradient step on q with step gamma in (0, 1] (GPflow's NaturalGradient, XiNat
+ *   parameters, Gaussian likelihood), in place: Lambda_l <- (1 - g) Lambda_l + g (I + (N / B) c_l A_l A_l'),
+ *   theta1_l <- (1 - g) theta1_l + g (N / B) A_l r~_l, c_l = sum_m W_ml^2 / noise_m, r~_l = sum_m W_ml (y_m - sum_{l' != l}
+ *   W_ml' mu_l') / noise_m.  At gamma = 1 on the full batch with one latent this is dmo_svgp_optimal_q's optimum.
+ * dmo_svgp_fit_elbo_grad: the ELBO pieces at the current q -- ell_out (M,) the expected log likelihood of each output
+ *   over the batch times N / B, kl_out (L,) KL(q_l || N(0, I)) -- and, when g_variance, g_length_scale and g_noise are
+ *   not NULL, d ELBO / d variance (L,), d length_scale (L,d), d noise (M,) and (g_W, needs W) d W (M,L) at fixed q.
+ * dmo_svgp_fit_q: q_mu (L,Z) and lower-triangular q_sqrt (L,Z,Z), the input of dmo_svgp_create.
+ * Host or device pointers; float64; deterministic (fixed-order reductions, no atomics): repeated calls are
+ * bit-identical.  Each call returns when its outputs are filled. */
+typedef struct dmo_svgp_fit dmo_svgp_fit;
+int dmo_svgp_fit_create(dmo_ctx* ctx, int64_t N, int d, int M, int L, int64_t Z, const double* X, const double* Y,
+                        const double* Zpts, int inducing_is_data, double jitter, dmo_svgp_fit** out);
+int dmo_svgp_fit_destroy(dmo_ctx* ctx, dmo_svgp_fit* st);
+int dmo_svgp_fit_natgrad(dmo_ctx* ctx, dmo_svgp_fit* st, const int64_t* batch, int64_t B, const double* variance,
+                         const double* length_scale, const double* noise, const double* W, double gamma);
+int dmo_svgp_fit_elbo_grad(dmo_ctx* ctx, dmo_svgp_fit* st, const int64_t* batch, int64_t B, const double* variance,
+                           const double* length_scale, const double* noise, const double* W, double* ell_out,
+                           double* kl_out, double* g_variance, double* g_length_scale, double* g_noise, double* g_W);
+int dmo_svgp_fit_q(dmo_ctx* ctx, dmo_svgp_fit* st, double* q_mu_out, double* q_sqrt_out);
+
 /* ---- A16: exact hypervolume ---------------------------------------------------
  * replaces hv.AdaptiveHyperVolume.compute_hypervolume(..., 'box') (dmosopt/hv.py:123-189)
  * -> HyperVolumeBoxDecomposition.compute_hypervolume (dmosopt/hv_box_decomposition.py:86-304)

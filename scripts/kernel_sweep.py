@@ -303,6 +303,60 @@ def egp_fit_sweep():
           f"({1e3 * wall / max(its):.1f} ms per lockstep iteration); stop: {[i['stop_reason'] for i in info]}", flush=True)
 
 
+def svgp_fit_sweep(n_iter=None):
+    """Variational training: per-call times (median of 5 warm calls, host clock around calls that end in a device
+    synchronise) of dmo_svgp_fit_natgrad and dmo_svgp_fit_elbo_grad at d = 30, B = 50 for Z in {256, 512, 819, 1024, 2048}
+    and L in {1, 3}, and of the VGP form at N in {1024, 2048, 4096}; then one fit of each class on ZDT1 data (N 2048, d 30,
+    M 2) with the reference's defaults (n_iter: the reference's per class unless given)."""
+    from dmosopt_b200 import model_gpflow as mg
+
+    L.context()
+    print(device_line(), flush=True)
+    rng = np.random.default_rng(6)
+    d, B = 30, 50
+
+    def med(f):
+        f()
+        ts = []
+        for _ in range(5):
+            t0 = time.perf_counter()
+            f()
+            ts.append(time.perf_counter() - t0)
+        return 1e3 * float(np.median(ts))
+
+    for Zn in (256, 512, 819, 1024, 2048):
+        N = max(4096, Zn)
+        X = rng.random((N, d))
+        for Lat in (1, 3):
+            Y = np.column_stack([np.sin(3 * X[:, :4].sum(1) + k) for k in range(Lat)])
+            st = L.SVGPFitState(X, Y, X[:Zn], Lat)
+            s, ls, nz = np.ones(Lat), np.full((Lat, d), 1.0 + 0.1 * np.arange(Lat)[:, None]), np.full(Lat, 1e-2)
+            b = rng.permutation(N)[:B]
+            t_ng = med(lambda: st.natgrad(b, s, ls, nz, gamma=0.1))
+            t_eg = med(lambda: st.elbo_grad(b, s, ls, nz))
+            print(f"svgp_fit Z={Zn} L={Lat} d={d} B={B}: natgrad {t_ng:.2f} ms, elbo_grad {t_eg:.2f} ms", flush=True)
+    for N in (1024, 2048, 4096):
+        X = rng.random((N, d))
+        Y = np.sin(3 * X[:, :4].sum(1))[:, None]
+        st = L.SVGPFitState(X, Y, None, 1, inducing_is_data=True)
+        s, ls, nz, b = np.ones(1), np.ones((1, d)), np.full(1, 1e-2), np.arange(N)
+        t_ng = med(lambda: st.natgrad(b, s, ls, nz, gamma=1.0))
+        t_eg = med(lambda: st.elbo_grad(b, s, ls, nz))
+        print(f"vgp_fit N={N} d={d}: natgrad {t_ng:.2f} ms, elbo_grad {t_eg:.2f} ms", flush=True)
+    N, M = 2048, 2
+    X = rng.random((N, d))
+    g = 1.0 + 9.0 / (d - 1) * X[:, 1:].sum(axis=1)
+    Y = np.column_stack((X[:, 0], g * (1.0 - np.sqrt(X[:, 0] / g))))
+    for cls in ("SVGP_Matern", "VGP_Matern", "SIV_Matern", "SPV_Matern", "CRV_Matern"):
+        kw = {} if n_iter is None else {"n_iter": n_iter}
+        t0 = time.perf_counter()
+        m = getattr(mg, cls)(X, Y, d, M, np.zeros(d), np.ones(d), seed=1, fit="gpu", **kw)
+        wall = time.perf_counter() - t0
+        fi = m.fit_info
+        print(f"{cls} fit ZDT1 N={N} d={d} M={M}{'' if n_iter is None else f' n_iter={n_iter}'}: iterations {fi['iterations']}, "
+              f"stop {fi['stop_reason']}, {wall:.1f} s, ELBO {[round(float(e[-1]), 1) for e in fi['elbo']]}", flush=True)
+
+
 def stream_sweep():
     """The HBM-bound kernels at the BASELINE shape: crowding / euclidean distance (n = 131072, M = 3), SBX + mutation
     (pop 65536, d 30), mean kernel's neighbours, hypervolume of a 65536-point 3-D front.  Prints time and the achieved
@@ -412,5 +466,8 @@ if __name__ == "__main__":
         sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "egp_fit":
         egp_fit_sweep()
+        sys.exit(0)
+    if len(sys.argv) > 1 and sys.argv[1] == "svgp_fit":
+        svgp_fit_sweep(int(sys.argv[2]) if len(sys.argv) > 2 else None)
         sys.exit(0)
     main()
