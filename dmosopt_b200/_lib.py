@@ -20,6 +20,8 @@ LIB_PATH = os.path.join(_HERE, "libdmosopt_b200.so")
 METRIC_NONE, METRIC_CROWDING, METRIC_EUCLIDEAN = 0, 1, 2
 KERNEL_MATERN52, KERNEL_RBF = 0, 1
 GP_FP64, GP_TENSOR, GP_AUTO = 0, 1, 2
+GP_PREDICT_MAX_D = 64  # input dimensions of dmo_gp_create (csrc/gp.cu KS_DMAX) and of every tensor-core predict
+GP_PREDICT_MAX_M = 16  # objectives of dmo_gp_create (csrc/gp.cu GP_MAX_M)
 HV_MAX_OBJECTIVES = 8  # dmo_hypervolume: exact, chain sums for M <= 5 (csrc/hv.cu), limit-set recursion for 6 .. 8 (csrc/hv_many.cu)
 
 _c_i64 = ctypes.c_int64

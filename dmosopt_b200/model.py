@@ -86,6 +86,11 @@ class _GPRBase:
         if precision not in codes:
             raise ValueError(f"{self._name}: precision must be 'auto', 'tensor' or 'fp64' (got {precision!r})")
         self.precision = codes[precision]
+        # the exact-GP predict (dmo_gp_create) is narrower than dmo_gp_fit: refuse before any training starts
+        if nInput > _lib.GP_PREDICT_MAX_D:
+            raise ValueError(f"{self._name}: the GPU predict takes at most {_lib.GP_PREDICT_MAX_D} input dimensions (got nInput={nInput})")
+        if nOutput > _lib.GP_PREDICT_MAX_M:
+            raise ValueError(f"{self._name}: the GPU predict takes at most {_lib.GP_PREDICT_MAX_M} objectives (got nOutput={nOutput})")
         self.stats = {}
 
         xin = np.asarray(xin, dtype=np.float64)

@@ -306,6 +306,9 @@ class _VariationalGP:
         self.precision = _lib.GP_TENSOR if precision in ("tensor", _lib.GP_TENSOR) else _lib.GP_FP64
         self.stats = {}
         self.fit_info = None
+        if self.precision == _lib.GP_TENSOR and nInput > _lib.GP_PREDICT_MAX_D:  # refused before any training starts
+            raise ValueError(f"{self.name}: the tensor-core predict takes at most {_lib.GP_PREDICT_MAX_D} input dimensions "
+                             f"(got nInput={nInput}); use precision='fp64'")
         if hyperparameters is not None and fit is not None:
             raise ValueError(f"{self.name}: fit={fit!r} and hyperparameters= conflict; pass one of them")
         if fit not in (None, "reference", "gpu"):

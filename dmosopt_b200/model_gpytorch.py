@@ -52,6 +52,11 @@ class EGP_Matern:
                  precision="fp64", hyperparameters=None, fit=None, **kwargs):
         if fit not in (None, "gpu", "reference"):
             raise ValueError(f"EGP_Matern: fit must be 'gpu', 'reference' or None (got {fit!r})")
+        # the exact-GP predict (dmo_gp_create) is narrower than the training: refuse before any training starts
+        if nInput > _lib.GP_PREDICT_MAX_D:
+            raise ValueError(f"EGP_Matern: the GPU predict takes at most {_lib.GP_PREDICT_MAX_D} input dimensions (got nInput={nInput})")
+        if nOutput > _lib.GP_PREDICT_MAX_M:
+            raise ValueError(f"EGP_Matern: the GPU predict takes at most {_lib.GP_PREDICT_MAX_M} objectives (got nOutput={nOutput})")
         self.nInput, self.nOutput = nInput, nOutput
         self.xlb = np.asarray(xlb, dtype=np.float64)
         xub = np.asarray(xub, dtype=np.float64)
@@ -542,6 +547,9 @@ class MEGP_Matern:
         if fit not in (None, "gpu", "reference"):
             raise ValueError(f"MEGP_Matern: fit must be 'gpu', 'reference' or None (got {fit!r})")
         self.precision = codes[precision]
+        if self.precision == _lib.GP_TENSOR and nInput > _lib.GP_PREDICT_MAX_D:  # refused before any training starts
+            raise ValueError(f"MEGP_Matern: the tensor-core predict takes at most {_lib.GP_PREDICT_MAX_D} input dimensions "
+                             f"(got nInput={nInput}); use precision='fp64'")
         self.nInput, self.nOutput = nInput, nOutput
         self.xlb = np.asarray(xlb, dtype=np.float64)
         xub = np.asarray(xub, dtype=np.float64)
