@@ -89,6 +89,10 @@ _SIGNATURES = {
     "dmo_svgp_fit_natgrad": (_c_int, [_vp, _vp, _vp, _c_i64, _vp, _vp, _vp, _vp, _c_dbl]),
     "dmo_svgp_fit_elbo_grad": (_c_int, [_vp, _vp, _vp, _c_i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dmo_svgp_fit_q": (_c_int, [_vp, _vp, _vp, _vp]),
+    "dmo_dgp_create": (_c_int, [_vp, _c_int, _c_int, _c_int, _c_i64, _c_i64, _vp, _vp, _vp, _vp, _vp, _vp, _c_dbl, _vp, _vp, _vp, _vp, _vp,
+                                _c_dbl, _vp, _c_dbl, _c_dbl, _c_int, _vp, _vp, _vp, _vp, _vp, ctypes.POINTER(_vp)]),
+    "dmo_dgp_predict": (_c_int, [_vp, _vp, _vp, _c_i64, _c_u64, _c_u64, _vp, _vp, _vp, _c_int]),
+    "dmo_dgp_destroy": (_c_int, [_vp, _vp]),
     "dmo_mtgp_lml_grad": (_c_int, [_vp, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dmo_gp_lml_grad": (_c_int, [_vp, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dmo_nsga2_step": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_i64, _c_int, _c_int, _c_dbl, _c_dbl, _c_dbl, _vp, _vp, _vp, _vp, _c_u64, _c_u64,
@@ -939,6 +943,68 @@ def svgp_optimal_q(X, y, Zpts, variance, length_scale, noise, jitter=1e-2, induc
     _check(load_library().dmo_svgp_optimal_q(context(), N, Z, d, L, _ptr(X), _ptr(y), _ptr(Zp), _ptr(s), _ptr(ls), _ptr(nz), float(jitter),
                                              int(bool(inducing_is_data)), _ptr(q_mu), _ptr(q_sqrt)), "dmo_svgp_optimal_q")
     return q_mu, q_sqrt
+
+
+class DGPHandle:
+    """Owns a dmo_dgp: the two-layer deep GP posterior of gpytorch's DSPP / DeepGP (dmo_dgp_create), resident in HBM.
+    Hidden layer: Z1pts (H,Z1,d), s1 (H,), ls1 (H,d), q_mu1 (H,Z1), q_sqrt1 (H,Z1,Z1), w1 (d,), b1; last layer: Z2pts
+    (T,Z2,H), s2 (T,), ls2 (T,H), q_mu2 (T,Z2), q_sqrt2 (T,Z2,Z2), c2; noise (T,) task + global noise.  quad_sites (J,H)
+    selects quadrature (DSPP); None means ``n_sites`` Monte Carlo draws per predict (DeepGP)."""
+
+    def __init__(self, Z1pts, s1, ls1, q_mu1, q_sqrt1, w1, b1, Z2pts, s2, ls2, q_mu2, q_sqrt2, c2, noise, y_mean, y_std, xlb, xrng,
+                 quad_sites=None, n_sites=None, jitter=1e-4, min_variance=1e-6):
+        Z1p, Z2p = _f64(Z1pts), _f64(Z2pts)
+        if Z1p.ndim != 3 or Z2p.ndim != 3:
+            raise DmoError(f"dmo_dgp_create: Z1pts must be (H, Z1, d) and Z2pts (T, Z2, H), got {Z1p.shape} and {Z2p.shape}")
+        H, Z1, d = Z1p.shape
+        T, Z2 = Z2p.shape[:2]
+        qs = None if quad_sites is None else _f64(quad_sites)
+        if qs is not None:
+            if qs.ndim != 2 or qs.shape[1] != H:
+                raise DmoError(f"dmo_dgp_create: quad_sites must be (J, {H}), got shape {qs.shape}")
+            n_sites = qs.shape[0]
+        if n_sites is None:
+            raise DmoError("dmo_dgp_create: n_sites is required without quad_sites")
+        arrs = {"s1": (_f64(s1), (H,)), "ls1": (_f64(ls1), (H, d)), "q_mu1": (_f64(q_mu1), (H, Z1)), "q_sqrt1": (_f64(q_sqrt1), (H, Z1, Z1)),
+                "w1": (_f64(w1), (d,)), "Z2pts": (Z2p, (T, Z2, H)), "s2": (_f64(s2), (T,)), "ls2": (_f64(ls2), (T, H)),
+                "q_mu2": (_f64(q_mu2), (T, Z2)), "q_sqrt2": (_f64(q_sqrt2), (T, Z2, Z2)), "noise": (_f64(noise), (T,)),
+                "y_mean": (_f64(y_mean), (T,)), "y_std": (_f64(y_std), (T,)), "xlb": (_f64(xlb), (d,)), "xrng": (_f64(xrng), (d,))}
+        for name, (a, shape) in arrs.items():
+            if a.shape != shape:
+                raise DmoError(f"dmo_dgp_create: {name} must have shape {shape}, got {a.shape}")
+        a = {k: v[0] for k, v in arrs.items()}
+        self.d, self.H, self.T, self.J = d, H, T, int(n_sites)
+        h = _vp()
+        _check(load_library().dmo_dgp_create(
+            context(), d, H, T, Z1, Z2, _ptr(Z1p), _ptr(a["s1"]), _ptr(a["ls1"]), _ptr(a["q_mu1"]), _ptr(a["q_sqrt1"]), _ptr(a["w1"]), float(b1),
+            _ptr(Z2p), _ptr(a["s2"]), _ptr(a["ls2"]), _ptr(a["q_mu2"]), _ptr(a["q_sqrt2"]), float(c2), _ptr(a["noise"]), float(jitter),
+            float(min_variance), self.J, _ptr(qs), _ptr(a["y_mean"]), _ptr(a["y_std"]), _ptr(a["xlb"]), _ptr(a["xrng"]), ctypes.byref(h)),
+            "dmo_dgp_create")
+        self._h = h
+
+    def predict(self, X, seed=0, stream_id=0, return_var=True, return_eps=False, precision=GP_FP64):
+        """(mean (P,T), var (P,T) or None[, eps (J,P,H)]) at the raw inputs X (P,d)."""
+        X = _f64(X)
+        if X.ndim == 1:
+            X = X.reshape(1, -1)
+        P = X.shape[0]
+        mean = pinned_empty((P, self.T), np.float64)
+        var = pinned_empty((P, self.T), np.float64) if return_var else None
+        eps = np.empty((self.J, P, self.H), np.float64) if return_eps else None
+        _check(load_library().dmo_dgp_predict(context(), self._h, _in(X), P, int(seed), int(stream_id), _ptr(eps), _ptr(mean), _ptr(var),
+                                              int(precision)), "dmo_dgp_predict")
+        return (mean, var, eps) if return_eps else (mean, var)
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and _lib is not None and _ctx is not None:
+            _lib.dmo_dgp_destroy(_ctx, self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 class SVGPFitState:

@@ -132,6 +132,16 @@ int sv_gemm(dmo_ctx* ctx, int64_t m, int64_t n, int64_t K, double alpha, const d
             int64_t sbk, int64_t sbj, double diag, double* C, int64_t ldc);
 // O = s J C' J (rows of ldo) for a row-major n x n lower-triangular C (J reverses the order): lower triangular
 int sv_flip(dmo_ctx* ctx, const double* C, int64_t n, double s, double* O, int64_t ldo);
+// dmo_svgp_predict before its output mix: the latent moments fm (L,P) and fv (L,P) (fv NULL: means only) of the DEVICE
+// inputs X (P,d), with up checked by the caller (GpUnitPredict::check).  Not synchronised; the caller runs up.watchdog.
+int svgp_latent_moments(dmo_ctx* ctx, dmo_svgp* sv, GpUnitPredict& up, const double* X, int64_t P, double* fm, double* fv);
+// Latent l's device operands, for a caller that forms its own K_*: the operator planes O0 = s Lz^-1 and O1 = s T (rows
+// of Npad, zero padded), the mean vector a_l (Npad,), the scaled inducing points XtT (d, Npad) and 1 / ell (d,).
+struct SvLatentView {
+  const double *O0, *O1, *A, *XtT, *inv_ls;
+  int64_t Npad;
+};
+int svgp_latent_view(const dmo_svgp* sv, int l, SvLatentView* v);
 
 // ---- multitask model (gp_multitask.cu): the block factorisation shared by dmo_mtgp_create and dmo_mtgp_lml_grad --
 constexpr int MT_MAX = 8;        // tasks per model

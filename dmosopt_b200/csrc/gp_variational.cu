@@ -250,6 +250,66 @@ struct dmo_svgp {
   DevBuf<double> xlb, xrg, W, ymean, ystd, vscale;
 };
 
+int svgp_latent_moments(dmo_ctx* ctx, dmo_svgp* sv, GpUnitPredict& up, const double* X, int64_t P, double* fm, double* fv) {
+  const int d = sv->d;
+  const int64_t Z = sv->Z, Npad = sv->groups[0]->ops.Npad;  // every group's planes have Z rows
+  const bool tensor = up.tensor, want_var = fv != nullptr;
+  int Gmax = 0;
+  for (auto& g : sv->groups) Gmax = g->gather.G > Gmax ? g->gather.G : Gmax;
+  DMO_TRY(up.alloc(ctx, P, Npad, Gmax, want_var));
+  const int64_t Pc_alloc = up.Pc_alloc;
+  const int n_mp = (int)(Npad / mt_kstar_span(false));  // the means always come from float64 kernel values
+  DevBuf<double> xs, mpart;
+  DMO_TRY(xs.alloc(ctx, (size_t)P * d));
+  DMO_TRY(mpart.alloc(ctx, (size_t)n_mp * SV_MAX * Pc_alloc));
+  for (auto& gp_ : sv->groups) {
+    SvGroup& gr = *gp_;
+    if (tensor && want_var) DMO_TRY(gp_prepare_tensor(ctx, gr.ops));
+    DMO_TRY(mt_scale_inputs(ctx, X, P, d, sv->xlb.p, sv->xrg.p, gr.inv_ls.p, xs.p));
+    for (int64_t p_base = 0; p_base < P; p_base += Pc_alloc) {
+      const int64_t Pc = (P - p_base) < Pc_alloc ? (P - p_base) : Pc_alloc;
+      const int64_t Pcpad = ceil_div(Pc, up.tile) * up.tile;
+      {
+        ProfileScope ps(ctx, "svgp_kstar");
+        // The mean sums k_u' a_l in float64 kernel values on both paths: a_l = s Lz^-T q_mu alternates in sign near
+        // interpolation, so sum |k_u a_l| can be ~100 times the mean and fp32 kernel values (~2^-22) would cost ~1e-5.
+        // The tensor path adds a K_*-only pass for its fp16 hi / lo plane.
+        if (tensor && want_var)
+          DMO_TRY(mt_kstar_produce(ctx, true, xs.p, P, p_base, Pcpad, gr.XtT.p, Z, Npad, d, 0, nullptr, gr.ops.Kexp.p, nullptr,
+                                   up.Kh.p, up.Kl.p, mpart.p, Pc_alloc));
+        DMO_TRY(mt_kstar_produce(ctx, false, xs.p, P, p_base, Pcpad, gr.XtT.p, Z, Npad, d, gr.gather.nlat, gr.A.p, nullptr,
+                                 tensor ? nullptr : up.Ks.p, nullptr, nullptr, mpart.p, Pc_alloc));
+      }
+      if (want_var) {
+        ProfileScope ps(ctx, "svgp_var");
+        DMO_TRY(up.contract(ctx, gr.ops, Pcpad));
+      }
+      DMO_LAUNCH(sv_gather_kernel, (unsigned)ceil_div(Pc, 256), 256, 0, gr.gather, Pc, p_base, P, mpart.p, n_mp, Pc_alloc, up.vnorm.p,
+                 up.n_vp, Pc_alloc, fm, fv);
+    }
+  }
+  return DMO_OK;
+}
+
+int svgp_latent_view(const dmo_svgp* sv, int l, SvLatentView* v) {
+  for (auto& gp_ : sv->groups) {
+    const SvGroup& gr = *gp_;
+    for (size_t j = 0; j < gr.lat.size(); ++j) {
+      if (gr.lat[j] != l) continue;
+      const int64_t Npad = gr.ops.Npad;
+      const size_t plane = (size_t)Npad * Npad;
+      v->O0 = gr.ops.Linv.p + gr.o0[j] * plane;
+      v->O1 = gr.ops.Linv.p + (gr.n_o0 + j) * plane;
+      v->A = gr.A.p + j * Npad;
+      v->XtT = gr.XtT.p;
+      v->inv_ls = gr.inv_ls.p;
+      v->Npad = Npad;
+      return DMO_OK;
+    }
+  }
+  return DMO_ERR_ARG;
+}
+
 extern "C" {
 
 int dmo_svgp_create(dmo_ctx* ctx, int L, int M, int64_t Z, int d, const double* Zpts, const double* variance,
@@ -420,10 +480,8 @@ int dmo_svgp_predict(dmo_ctx* ctx, dmo_svgp* sv, const double* X, int64_t P, dou
   DMO_CUDA(cudaSetDevice(ctx->device));
   DMO_REQUIRE(sv, "svgp_predict: null model");
   const int M = sv->M, L = sv->L, d = sv->d;
-  const int64_t Z = sv->Z, Npad = sv->groups[0]->ops.Npad;  // every group's planes have Z rows
   GpUnitPredict up;
   DMO_TRY(up.check(ctx, "svgp_predict", precision, d));
-  const bool tensor = up.tensor;
   if (P == 0) return DMO_OK;
   DMO_REQUIRE(P > 0 && X && mean, "svgp_predict: bad arguments");
   In<double> x;
@@ -432,42 +490,10 @@ int dmo_svgp_predict(dmo_ctx* ctx, dmo_svgp* sv, const double* X, int64_t P, dou
   DMO_TRY(om.init(ctx, mean, (size_t)P * M));
   DMO_TRY(ov.init(ctx, var, (size_t)P * M));
   const bool want_var = ov.d != nullptr;
-  int Gmax = 0;
-  for (auto& g : sv->groups) Gmax = g->gather.G > Gmax ? g->gather.G : Gmax;
-  DMO_TRY(up.alloc(ctx, P, Npad, Gmax, want_var));
-  const int64_t Pc_alloc = up.Pc_alloc;
-  const int n_mp = (int)(Npad / mt_kstar_span(false));  // the means always come from float64 kernel values
-  DevBuf<double> xs, fm, fv, mpart;
-  DMO_TRY(xs.alloc(ctx, (size_t)P * d));
+  DevBuf<double> fm, fv;
   DMO_TRY(fm.alloc(ctx, (size_t)L * P));
-  DMO_TRY(mpart.alloc(ctx, (size_t)n_mp * SV_MAX * Pc_alloc));
   if (want_var) DMO_TRY(fv.alloc(ctx, (size_t)L * P));
-  for (auto& gp_ : sv->groups) {
-    SvGroup& gr = *gp_;
-    if (tensor && want_var) DMO_TRY(gp_prepare_tensor(ctx, gr.ops));
-    DMO_TRY(mt_scale_inputs(ctx, x.d, P, d, sv->xlb.p, sv->xrg.p, gr.inv_ls.p, xs.p));
-    for (int64_t p_base = 0; p_base < P; p_base += Pc_alloc) {
-      const int64_t Pc = (P - p_base) < Pc_alloc ? (P - p_base) : Pc_alloc;
-      const int64_t Pcpad = ceil_div(Pc, up.tile) * up.tile;
-      {
-        ProfileScope ps(ctx, "svgp_kstar");
-        // The mean sums k_u' a_l in float64 kernel values on both paths: a_l = s Lz^-T q_mu alternates in sign near
-        // interpolation, so sum |k_u a_l| can be ~100 times the mean and fp32 kernel values (~2^-22) would cost ~1e-5.
-        // The tensor path adds a K_*-only pass for its fp16 hi / lo plane.
-        if (tensor && want_var)
-          DMO_TRY(mt_kstar_produce(ctx, true, xs.p, P, p_base, Pcpad, gr.XtT.p, Z, Npad, d, 0, nullptr, gr.ops.Kexp.p, nullptr,
-                                   up.Kh.p, up.Kl.p, mpart.p, Pc_alloc));
-        DMO_TRY(mt_kstar_produce(ctx, false, xs.p, P, p_base, Pcpad, gr.XtT.p, Z, Npad, d, gr.gather.nlat, gr.A.p, nullptr,
-                                 tensor ? nullptr : up.Ks.p, nullptr, nullptr, mpart.p, Pc_alloc));
-      }
-      if (want_var) {
-        ProfileScope ps(ctx, "svgp_var");
-        DMO_TRY(up.contract(ctx, gr.ops, Pcpad));
-      }
-      DMO_LAUNCH(sv_gather_kernel, (unsigned)ceil_div(Pc, 256), 256, 0, gr.gather, Pc, p_base, P, mpart.p, n_mp, Pc_alloc, up.vnorm.p,
-                 up.n_vp, Pc_alloc, fm.p, want_var ? fv.p : nullptr);
-    }
-  }
+  DMO_TRY(svgp_latent_moments(ctx, sv, up, x.d, P, fm.p, want_var ? fv.p : nullptr));
   {
     ProfileScope ps(ctx, "svgp_mix");
     DMO_LAUNCH(sv_mix_kernel, (unsigned)ceil_div(P * M, 256), 256, 0, P, L, M, fm.p, fv.p, sv->W.p, sv->ymean.p, sv->ystd.p,

@@ -1,4 +1,5 @@
-"""gpytorch exact-GP surrogates on the GPU path: ``EGP_Matern`` and ``MEGP_Matern`` (row A19).
+"""gpytorch surrogates on the GPU path: the exact GPs ``EGP_Matern`` and ``MEGP_Matern`` (row A19), and the deep GPs
+``MDSPP_Matern`` and ``MDGP_Matern`` (their posterior; see the end of this module).
 
 Drop-ins for ``dmosopt.model_gpytorch.EGP_Matern`` (dmosopt/model_gpytorch.py:1927-2235) and
 ``dmosopt.model_gpytorch.MEGP_Matern`` (:1623-1926), selected in dmosopt by
@@ -619,3 +620,227 @@ class MEGP_Matern:
         """model_gpytorch.py:1921-1926."""
         mean, var = self.predict(x)
         return (mean, var) if self.return_mean_variance else mean
+
+
+# ------------------------------------------------------------------------------------------------------ deep GPs
+DEEPGP_JITTER = 1e-4  # gpytorch's settings.variational_cholesky_jitter for the float32 models the reference trains
+DEEPGP_MIN_VARIANCE = 1e-6  # gpytorch's settings.min_variance for float32
+MDGP_DEFAULT_SEED = 0x5EED_D6B  # the Philox key of MDGP_Matern's draws when seed is None
+
+_DEEPGP_KEYS = {
+    # key: (shape in terms of H, T, Z1, Z2, J, d; None for a scalar)
+    "hidden_inducing_points": ("H", "Z1", "d"), "hidden_outputscale": ("H",), "hidden_lengthscale": ("H", "d"),
+    "hidden_variational_mean": ("H", "Z1"), "hidden_chol_variational_covar": ("H", "Z1", "Z1"), "mean_weights": ("d",),
+    "mean_bias": None, "last_inducing_points": ("T", "Z2", "H"), "last_outputscale": ("T",), "last_lengthscale": ("T", "H"),
+    "last_variational_mean": ("T", "Z2"), "last_chol_variational_covar": ("T", "Z2", "Z2"), "mean_constant": None,
+    "task_noises": ("T",), "noise": None,
+}
+
+
+def deepgp_hyperparameters(model, nInput, nOutput, quadrature):
+    """Read a trained ``GPyTorchMultitaskDSPPMatern`` / ``GPyTorchMultitaskDeepGPMatern`` (dmosopt/model_gpytorch.py
+    :185-277, 359-453) out into the ``hyperparameters=`` dict of MDSPP_Matern / MDGP_Matern, by gpytorch's attribute
+    names.  Inducing points shared by the hidden units are expanded to one plane per unit, a single length scale per unit
+    to all input dimensions, and chol_variational_covar is masked to its lower triangle (as
+    CholeskyVariationalDistribution does).  Refuses any strategy but a whitened VariationalStrategy and any distribution
+    but a CholeskyVariationalDistribution."""
+
+    def arr(t):
+        return np.asarray(t.detach().cpu().numpy(), dtype=np.float64)
+
+    def unit(layer, name, n_units, in_dims):
+        vs = layer.variational_strategy
+        if type(vs).__name__ != "VariationalStrategy":
+            raise ValueError(f"{name}: a whitened VariationalStrategy is required (got {type(vs).__name__})")
+        dist = vs._variational_distribution
+        if type(dist).__name__ != "CholeskyVariationalDistribution":
+            raise ValueError(f"{name}: a CholeskyVariationalDistribution is required (got {type(dist).__name__})")
+        Z = arr(vs.inducing_points)
+        Z = np.broadcast_to(Z.reshape((-1,) + Z.shape[-2:]), (n_units,) + Z.shape[-2:]).copy()
+        cm = getattr(layer.covar_module, "module", layer.covar_module)  # MultiDeviceKernel wraps the ScaleKernel
+        ls = arr(cm.base_kernel.lengthscale).reshape(n_units, -1)
+        return {"inducing_points": Z, "outputscale": arr(cm.outputscale).reshape(n_units),
+                "lengthscale": np.broadcast_to(ls, (n_units, in_dims)).copy(),
+                "variational_mean": arr(dist.variational_mean).reshape(n_units, Z.shape[1]),
+                "chol_variational_covar": np.tril(arr(dist.chol_variational_covar).reshape(n_units, Z.shape[1], Z.shape[1]))}
+
+    H = int(model.hidden_layer.output_dims)
+    hid = unit(model.hidden_layer, "hidden_layer", H, nInput)
+    last = unit(model.last_layer, "last_layer", nOutput, H)
+    hp = {f"hidden_{k}": v for k, v in hid.items()}
+    hp.update({f"last_{k}": v for k, v in last.items()})
+    mm = model.hidden_layer.mean_module
+    hp["mean_weights"] = arr(mm.weights).reshape(nInput)
+    hp["mean_bias"] = float(arr(mm.bias).reshape(-1)[0])
+    hp["mean_constant"] = float(arr(model.last_layer.mean_module.constant).reshape(-1)[0])
+    lik = model.likelihood
+    hp["task_noises"] = arr(lik.task_noises).reshape(nOutput) if getattr(lik, "has_task_noise", True) else np.zeros(nOutput)
+    hp["noise"] = float(arr(lik.noise).reshape(-1)[0]) if getattr(lik, "has_global_noise", True) else 0.0
+    if quadrature:
+        hp["quad_sites"] = arr(model.last_layer.quad_sites).reshape(-1, H)  # J from the parameter's shape
+    return hp
+
+
+def deepgp_check_hyperparameters(hp, nInput, nOutput, quadrature, who):
+    """float64 copies of the ``hyperparameters=`` arrays, their shapes checked; a ValueError names the first problem."""
+    if not isinstance(hp, dict):
+        raise ValueError(f"{who}: hyperparameters must be a dict (got {type(hp).__name__})")
+    keys = dict(_DEEPGP_KEYS, **({"quad_sites": ("J", "H")} if quadrature else {}))
+    missing = [k for k in keys if k not in hp]
+    if missing:
+        raise ValueError(f"{who}: hyperparameters is missing {', '.join(missing)}")
+    out = {k: np.asarray(hp[k], dtype=np.float64) for k in keys}
+    def lead(k, axis):  # axis 0 or -1 of array k; -1 for a scalar
+        return out[k].shape[axis] if out[k].ndim >= 1 else -1
+
+    dims = {"d": nInput, "T": nOutput, "H": lead("hidden_outputscale", 0), "Z1": lead("hidden_variational_mean", -1),
+            "Z2": lead("last_variational_mean", -1), "J": lead("quad_sites", 0) if quadrature else -1}
+    for k, shape in keys.items():
+        want = () if shape is None else tuple(dims[s] for s in shape)
+        if out[k].shape != want:
+            raise ValueError(f"{who}: hyperparameters[{k!r}] must have shape {want}, got {out[k].shape}")
+        if not np.all(np.isfinite(out[k])):
+            raise ValueError(f"{who}: hyperparameters[{k!r}] must be finite")
+    return out
+
+
+class _DeepGP:
+    """Shared construction and predict of MDSPP_Matern and MDGP_Matern (see their docstrings)."""
+
+    NAME = ""
+    QUADRATURE = False
+
+    def _setup(self, xin, yin, nInput, nOutput, xlb, xub, fit, precision, hyperparameters, jitter, return_mean_variance, nan, top_k,
+               logger, ref_kwargs):
+        codes = {"fp64": _lib.GP_FP64, "tensor": _lib.GP_TENSOR, _lib.GP_FP64: _lib.GP_FP64, _lib.GP_TENSOR: _lib.GP_TENSOR}
+        who = self.NAME
+        if precision not in codes:
+            raise ValueError(f"{who}: precision must be 'fp64' or 'tensor' (got {precision!r})")
+        if fit not in (None, "gpu", "reference"):
+            raise ValueError(f"{who}: fit must be 'reference', 'gpu' or None (got {fit!r})")
+        if fit == "gpu":
+            raise ValueError(f"{who}: training on the GPU is not built yet; use fit='reference' or pass hyperparameters=")
+        self.precision = codes[precision]
+        if self.precision == _lib.GP_TENSOR and nInput > _lib.GP_PREDICT_MAX_D:
+            raise ValueError(f"{who}: the tensor-core predict takes at most {_lib.GP_PREDICT_MAX_D} input dimensions "
+                             f"(got nInput={nInput}); use precision='fp64'")
+        self.nInput, self.nOutput = nInput, nOutput
+        self.xlb = np.asarray(xlb, dtype=np.float64)
+        xub = np.asarray(xub, dtype=np.float64)
+        self.xrng = np.where(np.isclose(xub - self.xlb, 0.0, rtol=1e-6, atol=1e-6), 1.0, xub - self.xlb)  # model_gpytorch.py:1034-1036
+        self.return_mean_variance = return_mean_variance
+        self.logger = logger
+        if hyperparameters is not None:
+            hp = deepgp_check_hyperparameters(hyperparameters, nInput, nOutput, self.QUADRATURE, who)
+            yin = np.asarray(yin, dtype=np.float64).reshape(len(yin), -1)
+            xin, yin = filter_and_top_k(np.asarray(xin, dtype=np.float64), yin, nan, top_k)
+            # float64 statistics (the reference's are float32); handle_zeros_in_scale
+            ymean = yin.mean(axis=0)
+            ystd = yin.std(axis=0)
+            ystd = np.where(ystd < 10 * np.finfo(np.float64).eps, 1.0, ystd)
+        else:
+            try:
+                import dmosopt.model_gpytorch as ref
+            except Exception as e:
+                raise RuntimeError(f"dmosopt_b200.model_gpytorch.{who} trains through dmosopt.model_gpytorch.{who}, which requires "
+                                   "dmosopt and the GPyTorch library; pass hyperparameters= to skip training") from e
+            if not getattr(ref, "_has_gpytorch", False):
+                raise RuntimeError(f"dmosopt_b200.model_gpytorch.{who} trains through dmosopt.model_gpytorch.{who}, which requires "
+                                   "the GPyTorch library; pass hyperparameters= to skip training")
+            model = getattr(ref, who)(xin, yin, nInput, nOutput, np.asarray(xlb), np.asarray(xub), logger=logger, nan=nan, top_k=top_k,
+                                      **ref_kwargs)
+            hp = deepgp_hyperparameters(model.sm, nInput, nOutput, self.QUADRATURE)
+            ymean = np.asarray(model.y_train_mean, dtype=np.float64)
+            ystd = np.asarray(model.y_train_std, dtype=np.float64)
+        self.hyperparameters = hp
+        self.y_train_mean, self.y_train_std = ymean, ystd
+        self._gp = _lib.DGPHandle(
+            hp["hidden_inducing_points"], hp["hidden_outputscale"], hp["hidden_lengthscale"], hp["hidden_variational_mean"],
+            np.tril(hp["hidden_chol_variational_covar"]), hp["mean_weights"], float(hp["mean_bias"]), hp["last_inducing_points"],
+            hp["last_outputscale"], hp["last_lengthscale"], hp["last_variational_mean"], np.tril(hp["last_chol_variational_covar"]),
+            float(hp["mean_constant"]), hp["task_noises"] + float(hp["noise"]), ymean, ystd, self.xlb, self.xrng,
+            quad_sites=hp.get("quad_sites"), n_sites=self._n_sites(), jitter=jitter, min_variance=DEEPGP_MIN_VARIANCE)
+
+    def _n_sites(self):
+        return None
+
+    def _draw_key(self):
+        return 0, 0
+
+    def predict(self, xin):
+        """(mean (P, T), variance (P, T)) as float64 arrays (the reference returns float32)."""
+        xin = np.asarray(xin, dtype=np.float64)
+        if xin.ndim == 1:
+            xin = xin.reshape((1, self.nInput))
+        seed, stream_id = self._draw_key()
+        return self._gp.predict(xin, seed=seed, stream_id=stream_id, return_var=True, precision=self.precision)
+
+    def evaluate(self, x):
+        mean, var = self.predict(x)
+        return (mean, var) if self.return_mean_variance else mean
+
+
+class MDSPP_Matern(_DeepGP):
+    """Deep sigma-point process surrogate: the reference constructor signature (model_gpytorch.py:991-1019) plus
+    ``precision`` ("fp64", the default, or "tensor": the hidden layer's variance through the split-fp16 contraction, d <=
+    64), ``hyperparameters`` (dict, see oracle/deepgp.py and ``deepgp_check_hyperparameters``; training is skipped and the
+    y statistics are computed in float64), ``jitter`` (gpytorch's variational_cholesky_jitter, 1e-4 for float32 models)
+    and ``fit`` ("reference" or None: train through the reference class, which needs gpytorch; "gpu" is not built yet).
+
+    predict is deterministic: the hidden layer's mean and standard deviation are combined with the learned quadrature
+    sites ``last_layer.quad_sites`` (J of them, J from the parameter's shape, not ``Q``), the last layer is evaluated at
+    each site, and the result is the reference's ``batch_preds.mean.mean(0)`` / ``.variance.mean(0)``: an unweighted
+    average over the sites (the learned quadrature weights are not used, and there is no between-site spread term).
+    ``fast_pred_var``, ``preconditioner_size`` and ``use_cuda`` are ignored; the reference's ``batch_size`` only affects
+    its training."""
+
+    NAME = "MDSPP_Matern"
+    QUADRATURE = True
+
+    def __init__(self, xin, yin, nInput, nOutput, xlb, xub, num_hidden_dims=3, Q=8, num_inducing_points=128, seed=None,
+                 gp_lengthscale_bounds=None, gp_likelihood_sigma=None, linear_mean=True, preconditioner_size=100, adam_lr=0.1,
+                 fast_pred_var=False, n_iter=2000, min_loss_pct_change=1.0, batch_size=10, return_mean_variance=False, use_cuda=False,
+                 nan="remove", top_k=None, logger=None, precision="fp64", hyperparameters=None, jitter=DEEPGP_JITTER, fit=None,
+                 **kwargs):
+        ref_kwargs = dict(num_hidden_dims=num_hidden_dims, Q=Q, num_inducing_points=num_inducing_points, seed=seed,
+                          gp_lengthscale_bounds=gp_lengthscale_bounds, gp_likelihood_sigma=gp_likelihood_sigma, linear_mean=linear_mean,
+                          preconditioner_size=preconditioner_size, adam_lr=adam_lr, fast_pred_var=fast_pred_var, n_iter=n_iter,
+                          min_loss_pct_change=min_loss_pct_change, batch_size=batch_size, use_cuda=use_cuda, **kwargs)
+        self._setup(xin, yin, nInput, nOutput, xlb, xub, fit, precision, hyperparameters, jitter, return_mean_variance, nan, top_k,
+                    logger, ref_kwargs)
+
+
+class MDGP_Matern(_DeepGP):
+    """Doubly stochastic deep GP surrogate: the reference constructor signature (model_gpytorch.py:1308-1335) plus
+    ``precision``, ``hyperparameters``, ``jitter`` and ``fit`` as MDSPP_Matern, and ``num_samples`` (10: gpytorch's
+    default num_likelihood_samples, which the reference sets only during training).
+
+    predict is a Monte Carlo average over ``num_samples`` draws of the hidden layer's output per candidate, as the
+    reference's: mean and variance are the unweighted averages over the draws.  The draws come from Philox4x32-10 keyed
+    by ``seed`` (None: MDGP_DEFAULT_SEED) with the call index as stream, so every predict draws afresh and the sequence of
+    predicts is reproducible from (seed, call index).  torch's random stream is not reproduced."""
+
+    NAME = "MDGP_Matern"
+    QUADRATURE = False
+
+    def __init__(self, xin, yin, nInput, nOutput, xlb, xub, num_hidden_dims=3, num_inducing_points=128, seed=None,
+                 gp_lengthscale_bounds=None, gp_likelihood_sigma=None, linear_mean=True, preconditioner_size=100, adam_lr=0.1,
+                 fast_pred_var=False, n_iter=2000, min_loss_pct_change=1.0, batch_size=50, return_mean_variance=False, use_cuda=False,
+                 nan="remove", top_k=None, logger=None, precision="fp64", hyperparameters=None, jitter=DEEPGP_JITTER, fit=None,
+                 num_samples=10, **kwargs):
+        self.num_samples = int(num_samples)
+        self.seed = MDGP_DEFAULT_SEED if seed is None else int(seed)
+        self.calls = 0
+        ref_kwargs = dict(num_hidden_dims=num_hidden_dims, num_inducing_points=num_inducing_points, seed=seed,
+                          gp_lengthscale_bounds=gp_lengthscale_bounds, gp_likelihood_sigma=gp_likelihood_sigma, linear_mean=linear_mean,
+                          preconditioner_size=preconditioner_size, adam_lr=adam_lr, fast_pred_var=fast_pred_var, n_iter=n_iter,
+                          min_loss_pct_change=min_loss_pct_change, batch_size=batch_size, use_cuda=use_cuda, **kwargs)
+        self._setup(xin, yin, nInput, nOutput, xlb, xub, fit, precision, hyperparameters, jitter, return_mean_variance, nan, top_k,
+                    logger, ref_kwargs)
+
+    def _n_sites(self):
+        return self.num_samples
+
+    def _draw_key(self):
+        self.calls += 1
+        return self.seed, self.calls - 1

@@ -340,6 +340,36 @@ int dmo_svgp_fit_elbo_grad(dmo_ctx* ctx, dmo_svgp_fit* st, const int64_t* batch,
                            double* kl_out, double* g_variance, double* g_length_scale, double* g_noise, double* g_W);
 int dmo_svgp_fit_q(dmo_ctx* ctx, dmo_svgp_fit* st, double* q_mu_out, double* q_sqrt_out);
 
+/* ---- two-layer deep GP posterior (MDSPP_Matern / MDGP_Matern predict) ------------------------------------------------
+ * replaces the predict of gpytorch's DSPP / DeepGP behind dmosopt/model_gpytorch.py's MDSPP_Matern (:991-1306) and
+ * MDGP_Matern (:1308-1620): two whitened variational GP layers with Matern-5/2 kernels (csrc/gp_deep.cu).
+ * dmo_dgp_create: hidden layer of H units over d inputs -- Z1pts (H,Z1,d) normalised inducing points, s1 (H,) output
+ *   scales, ls1 (H,d) length scales, q_mu1 (H,Z1), q_sqrt1 (H,Z1,Z1) lower triangular, prior mean w1 . x_n + b1 (w1 (d,))
+ *   shared by every unit; last layer of T tasks over the H hidden outputs -- Z2pts (T,Z2,H), s2 (T,), ls2 (T,H), q_mu2
+ *   (T,Z2), q_sqrt2 (T,Z2,Z2), constant prior mean c2; noise (T,) the task noise plus the global noise; jitter is added to
+ *   K(Z, Z) and k(x, x) in both layers; min_variance floors the hidden variance and every site's predictive variance.
+ *   quad_sites (n_sites,H) non-NULL: quadrature sites (DSPP); NULL: n_sites Monte Carlo draws per predict (DeepGP).
+ *   y_mean, y_std (T,); xlb, xrng (d,), x_n = (x - xlb) / xrng.  1 <= H, T <= 8, 1 <= n_sites <= 64, Z1, Z2 <= 8192,
+ *   d <= 90.  DMO_ERR_ARG names the problem: a q_sqrt that is not lower triangular, xrng <= 0, a non-finite or
+ *   non-positive scale, length scale or noise, or a K(Z, Z) + jitter I that is not positive definite (with its layer and
+ *   unit).
+ * dmo_dgp_predict: X (P,d) raw inputs -> mean (P,T), var (P,T) (may be NULL) averaged over the n_sites sites:
+ *   u_j = mean1 + e_j o sqrt(var1), e_j the quadrature sites or N(0, I) draws from Philox4x32-10 keyed by seed with the
+ *   counter (candidate, site * H + h, stream_id < 2^54) -- independent of chunking and of T.  eps_out (n_sites,P,H), may
+ *   be NULL, receives the e_j used.  precision DMO_GP_FP64, or DMO_GP_TENSOR (d <= 64: the hidden variance through the
+ *   split-fp16 contraction); the last layer is always float64.  DMO_GP_AUTO is refused.
+ * Host or device pointers; deterministic (fixed-order sums): repeated calls are bit-identical. */
+typedef struct dmo_dgp dmo_dgp;
+int dmo_dgp_create(dmo_ctx* ctx, int d, int H, int T, int64_t Z1, int64_t Z2, const double* Z1pts, const double* s1,
+                   const double* ls1, const double* q_mu1, const double* q_sqrt1, const double* w1, double b1,
+                   const double* Z2pts, const double* s2, const double* ls2, const double* q_mu2, const double* q_sqrt2,
+                   double c2, const double* noise, double jitter, double min_variance, int n_sites,
+                   const double* quad_sites, const double* y_mean, const double* y_std, const double* xlb,
+                   const double* xrng, dmo_dgp** out);
+int dmo_dgp_predict(dmo_ctx* ctx, dmo_dgp* g, const double* X, int64_t P, uint64_t seed, uint64_t stream_id,
+                    double* eps_out, double* mean, double* var, int precision);
+int dmo_dgp_destroy(dmo_ctx* ctx, dmo_dgp* g);
+
 /* ---- A16: exact hypervolume ---------------------------------------------------
  * replaces hv.AdaptiveHyperVolume.compute_hypervolume(..., 'box') (dmosopt/hv.py:123-189)
  * -> HyperVolumeBoxDecomposition.compute_hypervolume (dmosopt/hv_box_decomposition.py:86-304)

@@ -448,7 +448,46 @@ def svgp_sweep():
               f"var err / prior {np.max(np.abs(vt - vf) / Ytr.std(0) ** 2):.2e}", flush=True)
 
 
+def deepgp_sweep():
+    """The deep GP predict (dmo_dgp_predict) at P = 65536, d = 30, H = 3, T = 3, Z1 = Z2 = 128: MDSPP at J 3 and 8, MDGP at
+    J 10, fp64 and tensor.  Per predict: the hidden layer (ProfileScope dgp_hidden: the dmo_svgp latent moments and the
+    epilogue) and the layer-2 kernel (dgp_layer2) timed apart.  The layer-2 rate counts the useful work, 2 Z2^2 flop per
+    (site, candidate, task): the two triangular mat-vecs; K_* and the mean are not counted."""
+    L.context()
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    from test_deepgp_cpu import problem
+
+    rng = np.random.default_rng(7)
+    P, d, H, T, Z = 65536, 30, 3, 3, 128
+    lib, ctx = L.load_library(), L.context()
+    print(device_line(), flush=True)
+    X = rng.random((P, d))
+    Xd = L.DeviceArray((P, d)).upload(X)
+    md, vd = L.DeviceArray((P, T)), L.DeviceArray((P, T))
+    for label, J, quad in (("MDSPP", 3, True), ("MDSPP", 8, True), ("MDGP", 10, False)):
+        hp, ym, ys, _, _ = problem(rng, d, H, T, Z, Z, J=J, quadrature=quad)
+        g = L.DGPHandle(hp["hidden_inducing_points"], hp["hidden_outputscale"], hp["hidden_lengthscale"], hp["hidden_variational_mean"],
+                        np.tril(hp["hidden_chol_variational_covar"]), hp["mean_weights"], hp["mean_bias"], hp["last_inducing_points"],
+                        hp["last_outputscale"], hp["last_lengthscale"], hp["last_variational_mean"],
+                        np.tril(hp["last_chol_variational_covar"]), hp["mean_constant"], hp["task_noises"] + hp["noise"], ym, ys, np.zeros(d),
+                        np.ones(d), quad_sites=hp["quad_sites"] if quad else None, n_sites=J)
+        flop = 2.0 * Z * Z * J * P * T
+        for pname, prec in (("fp64", L.GP_FP64), ("tensor", L.GP_TENSOR)):
+            L.profile_enable(True)
+            ms = timed(lambda: L._check(lib.dmo_dgp_predict(ctx, g._h, Xd.ptr, P, 1, 0, None, md.ptr, vd.ptr, prec), "dgp"), reps=5)
+            rep = L.profile_report()
+            L.profile_enable(False)
+            hid = rep["dgp_hidden"][0] / rep["dgp_hidden"][1]
+            l2 = rep["dgp_layer2"][0] / rep["dgp_layer2"][1]
+            print(f"{label} J={J} {pname} P={P} d={d} H={H} T={T} Z1=Z2={Z}: predict {ms:.3f} ms; hidden layer {hid:.3f} ms, "
+                  f"layer-2 kernel {l2:.3f} ms = {flop / l2 / 1e9:.2f} TFLOP/s useful ({flop:.3e} flop)", flush=True)
+        g.close()
+
+
 if __name__ == "__main__":
+    if len(sys.argv) > 1 and sys.argv[1] == "deepgp":
+        deepgp_sweep()
+        sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "stream":
         stream_sweep()
         sys.exit(0)
