@@ -93,6 +93,14 @@ _SIGNATURES = {
                                 _c_dbl, _vp, _c_dbl, _c_dbl, _c_int, _vp, _vp, _vp, _vp, _vp, ctypes.POINTER(_vp)]),
     "dmo_dgp_predict": (_c_int, [_vp, _vp, _vp, _c_i64, _c_u64, _c_u64, _vp, _vp, _vp, _c_int]),
     "dmo_dgp_destroy": (_c_int, [_vp, _vp]),
+    "dmo_dgp_fit_create": (_c_int, [_vp, _c_i64, _c_int, _c_int, _c_int, _c_i64, _c_i64, _c_int, _c_int, _c_i64, _vp, _vp, _vp, _c_dbl, _c_dbl,
+                                    ctypes.POINTER(_vp)]),
+    "dmo_dgp_fit_destroy": (_c_int, [_vp, _vp]),
+    "dmo_dgp_fit_set_params": (_c_int, [_vp, _vp, _vp, _c_i64]),
+    "dmo_dgp_fit_get_params": (_c_int, [_vp, _vp, _vp, _c_i64]),
+    "dmo_dgp_fit_loss_grad": (_c_int, [_vp, _vp, _vp, _c_i64, _c_u64, _c_u64, _vp, _vp, _vp, _vp]),
+    "dmo_dgp_fit_adam_step": (_c_int, [_vp, _vp, _c_dbl]),
+    "dmo_dgp_fit_epoch": (_c_int, [_vp, _vp, _vp, _c_i64, _c_dbl, _c_u64, _c_u64, _vp]),
     "dmo_mtgp_lml_grad": (_c_int, [_vp, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dmo_gp_lml_grad": (_c_int, [_vp, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dmo_nsga2_step": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_i64, _c_int, _c_int, _c_dbl, _c_dbl, _c_dbl, _vp, _vp, _vp, _vp, _c_u64, _c_u64,
@@ -1065,6 +1073,74 @@ class SVGPFitState:
     def close(self):
         if getattr(self, "_h", None) is not None and _lib is not None and _ctx is not None:
             _lib.dmo_svgp_fit_destroy(_ctx, self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class DGPFitState:
+    """Owns a dmo_dgp_fit: the training state of the two-layer deep GP behind MDSPP_Matern (quadrature, n_sites sites)
+    and MDGP_Matern (n_sites draws per row) on X (N,d) normalised inputs and Y (N,T) normalised targets, with H hidden
+    units, Z1 / Z2 inducing points per layer and batches of at most batch_max rows.  The raw vector's layout is
+    dmosopt_b200.h's (model_gpytorch.deepgp_flatten builds it); it starts at zero."""
+
+    def __init__(self, X, Y, H, Z1, Z2, n_sites, quadrature, batch_max, lengthscale_bounds=None, jitter=1e-4, min_variance=1e-6):
+        X = _f64(X)
+        N, d = X.shape
+        Y = _f64(np.asarray(Y, dtype=np.float64).reshape(N, -1))
+        T = Y.shape[1]
+        lb = None if lengthscale_bounds is None else _f64(np.asarray(lengthscale_bounds, dtype=np.float64).reshape(2))
+        self.N, self.d, self.H, self.T, self.Z1, self.Z2 = N, d, int(H), T, int(Z1), int(Z2)
+        self.J, self.quadrature, self.batch_max = int(n_sites), bool(quadrature), int(batch_max)
+        self.n_params = (self.Z1 * d + 2 * self.H + self.H * self.Z1 + self.H * self.Z1 * self.Z1 + d + 1 + T * self.Z2 * self.H + 2 * T
+                         + T * self.Z2 + T * self.Z2 * self.Z2 + 1 + T + 1 + (self.J * self.H if self.quadrature else 0))
+        h = _vp()
+        _check(load_library().dmo_dgp_fit_create(context(), N, d, self.H, T, self.Z1, self.Z2, self.J, int(self.quadrature), self.batch_max,
+                                                 _ptr(X), _ptr(Y), _ptr(lb), float(jitter), float(min_variance), ctypes.byref(h)),
+               "dmo_dgp_fit_create")
+        self._h = h
+
+    def set_params(self, raw):
+        r = _f64(raw).reshape(-1)
+        _check(load_library().dmo_dgp_fit_set_params(context(), self._h, _ptr(r), r.shape[0]), "dmo_dgp_fit_set_params")
+
+    def get_params(self):
+        r = np.empty(self.n_params, np.float64)
+        _check(load_library().dmo_dgp_fit_get_params(context(), self._h, _ptr(r), r.shape[0]), "dmo_dgp_fit_get_params")
+        return r
+
+    def loss_grad(self, batch, seed=0, step=0, eps=None, grad=True, return_eps=False):
+        """(loss, grad (n_params,) or None[, eps (J,B,H)]) of the minibatch rows ``batch`` at the current parameters;
+        ``eps`` (J,B,H) replaces MDGP's Philox draws keyed by (seed, step)."""
+        b = np.ascontiguousarray(batch, dtype=np.int64).reshape(-1)
+        e = None if eps is None else _f64(eps)
+        loss = np.empty(1, np.float64)
+        g = np.empty(self.n_params, np.float64) if grad else None
+        eo = np.empty((self.J, b.shape[0], self.H), np.float64) if return_eps else None
+        _check(load_library().dmo_dgp_fit_loss_grad(context(), self._h, _ptr(b), b.shape[0], int(seed), int(step), _ptr(e), _ptr(eo), _ptr(loss),
+                                                    _ptr(g)), "dmo_dgp_fit_loss_grad")
+        return (float(loss[0]), g, eo) if return_eps else (float(loss[0]), g)
+
+    def adam_step(self, lr):
+        _check(load_library().dmo_dgp_fit_adam_step(context(), self._h, float(lr)), "dmo_dgp_fit_adam_step")
+
+    def epoch(self, perm, batch_size, lr, seed=0, step0=0):
+        """The batch losses of one epoch over the permutation ``perm`` of range(N), one Adam step per batch."""
+        p = np.ascontiguousarray(perm, dtype=np.int64).reshape(-1)
+        if p.shape[0] != self.N:
+            raise DmoError(f"dmo_dgp_fit_epoch: perm must have {self.N} entries, got {p.shape[0]}")
+        out = np.empty(-(-self.N // int(batch_size)), np.float64)
+        _check(load_library().dmo_dgp_fit_epoch(context(), self._h, _ptr(p), int(batch_size), float(lr), int(seed), int(step0), _ptr(out)),
+               "dmo_dgp_fit_epoch")
+        return out
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and _lib is not None and _ctx is not None:
+            _lib.dmo_dgp_fit_destroy(_ctx, self._h)
             self._h = None
 
     def __del__(self):

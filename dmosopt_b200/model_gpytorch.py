@@ -1,5 +1,5 @@
 """gpytorch surrogates on the GPU path: the exact GPs ``EGP_Matern`` and ``MEGP_Matern`` (row A19), and the deep GPs
-``MDSPP_Matern`` and ``MDGP_Matern`` (their posterior; see the end of this module).
+``MDSPP_Matern`` and ``MDGP_Matern`` (their posterior and training; see the end of this module).
 
 Drop-ins for ``dmosopt.model_gpytorch.EGP_Matern`` (dmosopt/model_gpytorch.py:1927-2235) and
 ``dmosopt.model_gpytorch.MEGP_Matern`` (:1623-1926), selected in dmosopt by
@@ -704,6 +704,201 @@ def deepgp_check_hyperparameters(hp, nInput, nOutput, quadrature, who):
     return out
 
 
+# ---- deep GP training on the GPU (fit="gpu-seeded")
+DEEPGP_FIT_MAX_Z = 128  # inducing points per layer of dmo_dgp_fit (one CTA holds K(Z, Z) in shared memory)
+DEEPGP_FIT_MAX_HT = 8  # hidden units and tasks
+DEEPGP_FIT_MAX_D = 90  # input dimensions
+DSPP_NUM_QUAD_SITES = 3  # gpytorch DSPPLayer's default num_quad_sites
+
+# raw parameters of the deep GP, in the order of the flat vector of dmo_dgp_fit (include/dmosopt_b200.h): key -> shape
+DEEPGP_RAW_KEYS = ("hidden_inducing_points", "hidden_raw_lengthscale", "hidden_raw_outputscale", "hidden_variational_mean",
+                   "hidden_chol_variational_covar", "mean_weights", "mean_bias", "last_inducing_points", "last_raw_lengthscale",
+                   "last_raw_outputscale", "last_variational_mean", "last_chol_variational_covar", "mean_constant", "raw_task_noises",
+                   "raw_noise", "quad_sites")
+
+
+def deepgp_raw_shapes(d, T, H, Z1, Z2, quadrature):
+    """{key: shape} of the raw parameters, in flat-vector order."""
+    shapes = {"hidden_inducing_points": (Z1, d), "hidden_raw_lengthscale": (H,), "hidden_raw_outputscale": (H,),
+              "hidden_variational_mean": (H, Z1), "hidden_chol_variational_covar": (H, Z1, Z1), "mean_weights": (d,), "mean_bias": (1,),
+              "last_inducing_points": (T, Z2, H), "last_raw_lengthscale": (T,), "last_raw_outputscale": (T,),
+              "last_variational_mean": (T, Z2), "last_chol_variational_covar": (T, Z2, Z2), "mean_constant": (1,),
+              "raw_task_noises": (T,), "raw_noise": (1,)}
+    if quadrature:
+        shapes["quad_sites"] = (DSPP_NUM_QUAD_SITES, H)
+    return shapes
+
+
+def deepgp_flatten(raw):
+    """raw dict -> the flat float64 vector of dmo_dgp_fit."""
+    return np.concatenate([np.asarray(raw[k], dtype=np.float64).reshape(-1) for k in DEEPGP_RAW_KEYS if k in raw])
+
+
+def deepgp_unflatten(flat, shapes):
+    """The flat vector -> raw dict with the given {key: shape}."""
+    out, o = {}, 0
+    for k, shp in shapes.items():
+        n = int(np.prod(shp))
+        out[k] = np.asarray(flat[o : o + n], dtype=np.float64).reshape(shp).copy()
+        o += n
+    return out
+
+
+def deepgp_initial_raw(xn, T, *, quadrature, num_hidden_dims=3, num_inducing_points=128, rng=None):
+    """Initial raw parameters of the reference's DSPP / DeepGP model (dmosopt/model_gpytorch.py:185-247, 359-416) at the
+    normalised inputs xn (N,d).  Z = min(num_inducing_points, N) in both layers.  Raw length scales, output scales and
+    noises 0; chol_variational_covar I; mean constant 0.  Draws from ``rng`` (np.random.Generator) in this order: the
+    hidden inducing points, kmeans2(xn, xn[permutation(N)[:Z]], minit="matrix"); the LinearMean weights (d) and bias;
+    the hidden variational means (H,Z) then the last-layer ones (T,Z), both 1e-3 N(0,1); the last-layer inducing points
+    (T,Z,H) N(0,1); the quadrature sites (3,H) N(0,1) (quadrature only)."""
+    from scipy.cluster.vq import kmeans2
+
+    xn = np.asarray(xn, dtype=np.float64)
+    N, d = xn.shape
+    H = int(num_hidden_dims)
+    Z = min(int(num_inducing_points), N)
+    perm = rng.permutation(N)
+    Z1 = kmeans2(xn, xn[perm[:Z]].copy(), minit="matrix")[0]
+    w = rng.standard_normal(d)
+    b = rng.standard_normal(1)
+    mu1 = 1e-3 * rng.standard_normal((H, Z))
+    mu2 = 1e-3 * rng.standard_normal((T, Z))
+    Z2 = rng.standard_normal((T, Z, H))
+    raw = {"hidden_inducing_points": Z1, "hidden_raw_lengthscale": np.zeros(H), "hidden_raw_outputscale": np.zeros(H),
+           "hidden_variational_mean": mu1, "hidden_chol_variational_covar": np.tile(np.eye(Z), (H, 1, 1)), "mean_weights": w,
+           "mean_bias": b, "last_inducing_points": Z2, "last_raw_lengthscale": np.zeros(T), "last_raw_outputscale": np.zeros(T),
+           "last_variational_mean": mu2, "last_chol_variational_covar": np.tile(np.eye(Z), (T, 1, 1)), "mean_constant": np.zeros(1),
+           "raw_task_noises": np.zeros(T), "raw_noise": np.zeros(1)}
+    if quadrature:
+        raw["quad_sites"] = rng.standard_normal((DSPP_NUM_QUAD_SITES, H))
+    return raw
+
+
+def deepgp_natural(raw, lengthscale_bounds=None):
+    """raw parameters -> the ``hyperparameters=`` dict of MDSPP_Matern / MDGP_Matern: the shared hidden inducing points
+    expanded to one plane per unit, each isotropic length scale broadcast over its unit's input dimensions, chol masked to
+    its lower triangle, the transforms applied."""
+
+    def ls(x):
+        if lengthscale_bounds is None:
+            return _softplus(x)
+        lo, hi = float(lengthscale_bounds[0]), float(lengthscale_bounds[1])
+        return lo + (hi - lo) * _sigmoid(x)
+
+    Z1 = np.asarray(raw["hidden_inducing_points"], dtype=np.float64)
+    H = raw["hidden_raw_outputscale"].shape[0]
+    d = Z1.shape[1]
+    hp = {"hidden_inducing_points": np.broadcast_to(Z1, (H,) + Z1.shape).copy(), "hidden_outputscale": _softplus(raw["hidden_raw_outputscale"]),
+          "hidden_lengthscale": np.repeat(ls(raw["hidden_raw_lengthscale"])[:, None], d, axis=1),
+          "hidden_variational_mean": raw["hidden_variational_mean"].copy(),
+          "hidden_chol_variational_covar": np.tril(raw["hidden_chol_variational_covar"]), "mean_weights": raw["mean_weights"].copy(),
+          "mean_bias": float(raw["mean_bias"][0]), "last_inducing_points": raw["last_inducing_points"].copy(),
+          "last_outputscale": _softplus(raw["last_raw_outputscale"]), "last_lengthscale": np.repeat(ls(raw["last_raw_lengthscale"])[:, None], H, axis=1),
+          "last_variational_mean": raw["last_variational_mean"].copy(), "last_chol_variational_covar": np.tril(raw["last_chol_variational_covar"]),
+          "mean_constant": float(raw["mean_constant"][0]), "task_noises": _NOISE_LOWER + _softplus(raw["raw_task_noises"]),
+          "noise": _NOISE_LOWER + float(_softplus(raw["raw_noise"])[0])}
+    if "quad_sites" in raw:
+        hp["quad_sites"] = raw["quad_sites"].copy()
+    return hp
+
+
+class ReduceLROnPlateau:
+    """torch.optim.lr_scheduler.ReduceLROnPlateau(mode="min", patience=3, threshold=0.01) with torch's other defaults
+    (factor 0.1, threshold_mode "rel", cooldown 0, min_lr 0, eps 1e-8), restated: a loss below best (1 - threshold) is an
+    improvement and resets the count of bad epochs; when the count exceeds patience the lr becomes max(lr factor,
+    min_lr) if that lowers it by more than eps, and the count restarts."""
+
+    def __init__(self, lr, factor=0.1, patience=3, threshold=0.01, min_lr=0.0, eps=1e-8):
+        self.lr, self.factor, self.patience, self.threshold, self.min_lr, self.eps = float(lr), factor, patience, threshold, min_lr, eps
+        self.best = float("inf")
+        self.num_bad_epochs = 0
+
+    def step(self, metric):
+        """The lr after the epoch loss ``metric``."""
+        current = float(metric)
+        if current < self.best * (1.0 - self.threshold):
+            self.best = current
+            self.num_bad_epochs = 0
+        else:
+            self.num_bad_epochs += 1
+        if self.num_bad_epochs > self.patience:
+            new_lr = max(self.lr * self.factor, self.min_lr)
+            if self.lr - new_lr > self.eps:
+                self.lr = new_lr
+            self.num_bad_epochs = 0
+        return self.lr
+
+
+def deepgp_stopper(quadrature, min_loss_pct_change):
+    """The reference's AdaptiveEarlyStopping for the deep GPs: DEEP_STOCHASTIC (MDSPP, from epoch 2000) or DEEP_GP (MDGP,
+    from 1500); window 500, patience 3, warmup 200, threshold_pct = min_loss_pct_change."""
+    return EarlyStopping(threshold_pct=min_loss_pct_change, min_iterations=2000 if quadrature else 1500, window_size=500, patience=3,
+                         warmup_iterations=200)
+
+
+def deepgp_fit(xn, yn, *, quadrature, num_hidden_dims=3, num_inducing_points=128, lengthscale_bounds=None, adam_lr=0.1, n_iter=2000,
+               min_loss_pct_change=1.0, batch_size=None, seed=None, logger=None, initial_raw=None):
+    """Train MDSPP_Matern (quadrature) or MDGP_Matern on the GPU: the reference's loop (dmosopt/model_gpytorch.py:1179-1216,
+    1495-1532) on the minibatch loss and gradient of dmo_dgp_fit.  xn (N,d) normalised inputs, yn (N,T) normalised targets.
+
+    Per epoch: a fresh permutation of the rows, batches of batch_size (default 10 for MDSPP, 50 for MDGP; the last may be
+    partial), one Adam step each, all on the device; the epoch loss is the unweighted mean of the batch losses and steps
+    ReduceLROnPlateau; every 100 epochs the reference's log line; from epoch 200 the early-stopping rule, which -- as in
+    the reference, whose ``break`` sits inside ``if logger is not None`` -- stops the loop only when a logger is given.
+    MDGP draws J = batch_size samples per row (num_likelihood_samples during the reference's training) from Philox4x32-10
+    keyed by the seed and the step counter.  Randomness: np.random.default_rng(seed) (seed None meaning 0) makes the
+    initial draws (deepgp_initial_raw, made even when ``initial_raw`` replaces them) and then one permutation per epoch.
+
+    Returns (hyperparameters, info): the ``hyperparameters=`` dict at the final parameters, and info with ``loss`` (epoch
+    losses), ``lr`` (the lr of each epoch), ``iterations``, ``stop_reason`` and ``raw`` (final raw parameters)."""
+    xn = np.ascontiguousarray(xn, dtype=np.float64)
+    yn = np.ascontiguousarray(yn, dtype=np.float64).reshape(xn.shape[0], -1)
+    N, d = xn.shape
+    T = yn.shape[1]
+    H = int(num_hidden_dims)
+    B = int(batch_size if batch_size is not None else (10 if quadrature else 50))
+    B = min(B, N)
+    name = "MDSPP_Matern" if quadrature else "MDGP_Matern"
+    seed_v = 0 if seed is None else int(seed)
+    rng = np.random.default_rng(seed_v)
+    raw = deepgp_initial_raw(xn, T, quadrature=quadrature, num_hidden_dims=H, num_inducing_points=num_inducing_points, rng=rng)
+    if initial_raw is not None:
+        raw = {k: np.array(v, dtype=np.float64) for k, v in initial_raw.items()}
+    Z1 = raw["hidden_variational_mean"].shape[1]
+    Z2 = raw["last_variational_mean"].shape[1]
+    shapes = deepgp_raw_shapes(d, T, H, Z1, Z2, quadrature)
+    J = DSPP_NUM_QUAD_SITES if quadrature else B
+    state = _lib.DGPFitState(xn, yn, H, Z1, Z2, J, quadrature, B, lengthscale_bounds=lengthscale_bounds, jitter=DEEPGP_JITTER,
+                             min_variance=DEEPGP_MIN_VARIANCE)
+    state.set_params(deepgp_flatten(raw))
+    sched = ReduceLROnPlateau(adam_lr)
+    stopper = deepgp_stopper(quadrature, min_loss_pct_change)
+    losses, lrs, reason, step = [], [], "n_iter", 0
+    nb = -(-N // B)
+    for it in range(n_iter):
+        lr = sched.lr
+        batch_losses = state.epoch(rng.permutation(N), B, lr, seed=seed_v, step0=step)
+        step += nb
+        mean_loss = float(np.mean(batch_losses))
+        losses.append(mean_loss)
+        lrs.append(lr)
+        sched.step(mean_loss)
+        if it % 100 == 0 and logger is not None:
+            noise = _NOISE_LOWER + float(_softplus(state.get_params()[-(1 + (J * H if quadrature else 0))]))
+            sep = "  " if quadrature else "  noise:  "
+            logger.info(f"{name}: iter {it}/{n_iter} - Loss: {mean_loss:.3f}{sep}{noise:.3f}")
+        if it >= stopper.warmup_iterations:
+            stop, why = stopper.should_stop(it, np.array(losses))
+            if stop and logger is not None:
+                logger.info(f"{name}: early stop at iteration {it + 1}: {why}")
+                reason = why
+                break
+    raw = deepgp_unflatten(state.get_params(), shapes)
+    state.close()
+    hp = deepgp_natural(raw, lengthscale_bounds)
+    return hp, {"loss": np.asarray(losses), "lr": np.asarray(lrs), "iterations": len(losses), "stop_reason": reason, "raw": raw}
+
+
 class _DeepGP:
     """Shared construction and predict of MDSPP_Matern and MDGP_Matern (see their docstrings)."""
 
@@ -716,10 +911,11 @@ class _DeepGP:
         who = self.NAME
         if precision not in codes:
             raise ValueError(f"{who}: precision must be 'fp64' or 'tensor' (got {precision!r})")
-        if fit not in (None, "gpu", "reference"):
-            raise ValueError(f"{who}: fit must be 'reference', 'gpu' or None (got {fit!r})")
+        if fit not in (None, "gpu", "gpu-seeded", "reference"):
+            raise ValueError(f"{who}: fit must be 'reference', 'gpu-seeded', 'gpu' or None (got {fit!r})")
         if fit == "gpu":
-            raise ValueError(f"{who}: training on the GPU is not built yet; use fit='reference' or pass hyperparameters=")
+            raise ValueError(f"{who}: training on the GPU with torch's own random streams is not built yet; fit='gpu-seeded' "
+                             "trains on the GPU with seeded streams (or use fit='reference', or pass hyperparameters=)")
         self.precision = codes[precision]
         if self.precision == _lib.GP_TENSOR and nInput > _lib.GP_PREDICT_MAX_D:
             raise ValueError(f"{who}: the tensor-core predict takes at most {_lib.GP_PREDICT_MAX_D} input dimensions "
@@ -730,14 +926,26 @@ class _DeepGP:
         self.xrng = np.where(np.isclose(xub - self.xlb, 0.0, rtol=1e-6, atol=1e-6), 1.0, xub - self.xlb)  # model_gpytorch.py:1034-1036
         self.return_mean_variance = return_mean_variance
         self.logger = logger
-        if hyperparameters is not None:
-            hp = deepgp_check_hyperparameters(hyperparameters, nInput, nOutput, self.QUADRATURE, who)
+        self.fit_info = None
+        if hyperparameters is None and fit == "gpu-seeded":
+            self._check_gpu_fit(nInput, nOutput, len(xin), ref_kwargs)
+        if hyperparameters is not None or fit == "gpu-seeded":
             yin = np.asarray(yin, dtype=np.float64).reshape(len(yin), -1)
             xin, yin = filter_and_top_k(np.asarray(xin, dtype=np.float64), yin, nan, top_k)
             # float64 statistics (the reference's are float32); handle_zeros_in_scale
             ymean = yin.mean(axis=0)
             ystd = yin.std(axis=0)
             ystd = np.where(ystd < 10 * np.finfo(np.float64).eps, 1.0, ystd)
+            if hyperparameters is None:
+                if logger is not None:
+                    logger.info(f"{who}: optimizing regressor...")
+                xn = (xin - self.xlb) / self.xrng
+                hyperparameters, self.fit_info = deepgp_fit(
+                    xn, (yin - ymean) / ystd, quadrature=self.QUADRATURE, num_hidden_dims=ref_kwargs["num_hidden_dims"],
+                    num_inducing_points=ref_kwargs["num_inducing_points"], lengthscale_bounds=ref_kwargs["gp_lengthscale_bounds"],
+                    adam_lr=ref_kwargs["adam_lr"], n_iter=ref_kwargs["n_iter"], min_loss_pct_change=ref_kwargs["min_loss_pct_change"],
+                    batch_size=ref_kwargs["batch_size"], seed=ref_kwargs["seed"], logger=logger)
+            hp = deepgp_check_hyperparameters(hyperparameters, nInput, nOutput, self.QUADRATURE, who)
         else:
             try:
                 import dmosopt.model_gpytorch as ref
@@ -760,6 +968,22 @@ class _DeepGP:
             hp["last_outputscale"], hp["last_lengthscale"], hp["last_variational_mean"], np.tril(hp["last_chol_variational_covar"]),
             float(hp["mean_constant"]), hp["task_noises"] + float(hp["noise"]), ymean, ystd, self.xlb, self.xrng,
             quad_sites=hp.get("quad_sites"), n_sites=self._n_sites(), jitter=jitter, min_variance=DEEPGP_MIN_VARIANCE)
+
+    def _check_gpu_fit(self, nInput, nOutput, N, kw):
+        """Refuse, before any training starts, what dmo_dgp_fit does not train."""
+        who = self.NAME
+        if kw.get("gp_likelihood_sigma") is not None:
+            raise ValueError(f"{who}: the GPU fit has no noise prior (gp_likelihood_sigma); use fit='reference'")
+        H = int(kw["num_hidden_dims"])
+        if not 1 <= H <= DEEPGP_FIT_MAX_HT or not 1 <= nOutput <= DEEPGP_FIT_MAX_HT:
+            raise ValueError(f"{who}: the GPU fit takes 1 to {DEEPGP_FIT_MAX_HT} hidden units and objectives (got num_hidden_dims={H}, "
+                             f"nOutput={nOutput}); use fit='reference'")
+        if nInput > DEEPGP_FIT_MAX_D:
+            raise ValueError(f"{who}: the GPU fit takes at most {DEEPGP_FIT_MAX_D} input dimensions (got nInput={nInput}); "
+                             "use fit='reference'")
+        if min(int(kw["num_inducing_points"]), N) > DEEPGP_FIT_MAX_Z:  # the reference clips Z at N
+            raise ValueError(f"{who}: the GPU fit takes at most {DEEPGP_FIT_MAX_Z} inducing points per layer (got "
+                             f"num_inducing_points={kw['num_inducing_points']}); use fit='reference'")
 
     def _n_sites(self):
         return None
@@ -785,7 +1009,9 @@ class MDSPP_Matern(_DeepGP):
     ``precision`` ("fp64", the default, or "tensor": the hidden layer's variance through the split-fp16 contraction, d <=
     64), ``hyperparameters`` (dict, see oracle/deepgp.py and ``deepgp_check_hyperparameters``; training is skipped and the
     y statistics are computed in float64), ``jitter`` (gpytorch's variational_cholesky_jitter, 1e-4 for float32 models)
-    and ``fit`` ("reference" or None: train through the reference class, which needs gpytorch; "gpu" is not built yet).
+    and ``fit`` ("reference" or None: train through the reference class, which needs gpytorch; "gpu-seeded": train on the
+    GPU with deepgp_fit, seeded streams in place of torch's; "gpu", replaying torch's streams, is refused).  After a
+    GPU fit ``fit_info`` holds the epoch losses, the lr history, the epoch count, the stop reason and the raw parameters.
 
     predict is deterministic: the hidden layer's mean and standard deviation are combined with the learned quadrature
     sites ``last_layer.quad_sites`` (J of them, J from the parameter's shape, not ``Q``), the last layer is evaluated at

@@ -370,6 +370,42 @@ int dmo_dgp_predict(dmo_ctx* ctx, dmo_dgp* g, const double* X, int64_t P, uint64
                     double* eps_out, double* mean, double* var, int precision);
 int dmo_dgp_destroy(dmo_ctx* ctx, dmo_dgp* g);
 
+/* ---- two-layer deep GP training (MDSPP_Matern / MDGP_Matern fit) ---------------------------------------------------
+ * A dmo_dgp_fit is the device-resident training state of gpytorch's DSPP / DeepGP model behind MDSPP_Matern and
+ * MDGP_Matern (csrc/gp_deep_fit.cu): X (N,d) normalised inputs, Y (N,T) normalised targets, a flat float64 vector of raw
+ * parameters, its gradient and the Adam moments.  The raw vector, in order: hidden inducing points Z1 (Z1,d) shared by
+ * the H units, raw length scales (H,), raw output scales (H,), variational means (H,Z1), chol_variational_covar
+ * (H,Z1,Z1), linear-mean weights (d,) and bias (1); last-layer inducing points (T,Z2,H), raw length scales (T,), raw
+ * output scales (T,), variational means (T,Z2), chol_variational_covar (T,Z2,Z2), constant mean (1); raw task noises
+ * (T,), raw global noise (1); with quadrature the sites (n_sites,H).  Transforms: output scale softplus; length scale
+ * softplus, or lo + (hi - lo) sigmoid with lengthscale_bounds (2,) non-NULL; noises 1e-4 + softplus; the rest
+ * untransformed (chol masked to its lower triangle).
+ * dmo_dgp_fit_create: 1 <= H, T <= 8, 1 <= Z1, Z2 <= 128, d <= 90, 1 <= batch_max <= N, n_sites * batch_max <= 65536
+ *   (n_sites: the quadrature sites, or MDGP's draws per row).  The raw vector starts at zero.
+ * dmo_dgp_fit_set_params / get_params: the raw vector (n its length).
+ * dmo_dgp_fit_loss_grad: the minibatch loss -ELBO / B of the rows batch (B,) at the current parameters into *loss_out and
+ *   its gradient by the raw vector into grad_out (may be NULL; kept for adam_step).  Without quadrature the draws are
+ *   eps_in (n_sites,B,H) when given, else N(0,1) from Philox4x32-10 keyed by seed with the counter (step, row, site *
+ *   H + h); eps_out (n_sites,B,H), may be NULL, receives the draws used.
+ * dmo_dgp_fit_adam_step: one torch.optim.Adam step (betas 0.9 / 0.999, eps 1e-8) with the last gradient.
+ * dmo_dgp_fit_epoch: every step of one epoch -- batches perm[b B : (b + 1) B] of the permutation perm (N,) of
+ *   range(N), the last one partial, draws keyed by step step0 + b -- each a loss_grad and an Adam step with lr, with no
+ *   host synchronisation in between; losses_out (ceil(N / B),) the batch losses.
+ * A K(Z, Z) + jitter I that is not positive definite is DMO_ERR_ARG naming its layer and unit.  Host or device
+ * pointers; deterministic (fixed-order sums, no atomics): repeated calls are bit-identical. */
+typedef struct dmo_dgp_fit dmo_dgp_fit;
+int dmo_dgp_fit_create(dmo_ctx* ctx, int64_t N, int d, int H, int T, int64_t Z1, int64_t Z2, int n_sites, int quadrature,
+                       int64_t batch_max, const double* X, const double* Y, const double* lengthscale_bounds, double jitter,
+                       double min_variance, dmo_dgp_fit** out);
+int dmo_dgp_fit_destroy(dmo_ctx* ctx, dmo_dgp_fit* st);
+int dmo_dgp_fit_set_params(dmo_ctx* ctx, dmo_dgp_fit* st, const double* raw, int64_t n);
+int dmo_dgp_fit_get_params(dmo_ctx* ctx, dmo_dgp_fit* st, double* raw, int64_t n);
+int dmo_dgp_fit_loss_grad(dmo_ctx* ctx, dmo_dgp_fit* st, const int64_t* batch, int64_t B, uint64_t seed, uint64_t step,
+                          const double* eps_in, double* eps_out, double* loss_out, double* grad_out);
+int dmo_dgp_fit_adam_step(dmo_ctx* ctx, dmo_dgp_fit* st, double lr);
+int dmo_dgp_fit_epoch(dmo_ctx* ctx, dmo_dgp_fit* st, const int64_t* perm, int64_t B, double lr, uint64_t seed, uint64_t step0,
+                      double* losses_out);
+
 /* ---- A16: exact hypervolume ---------------------------------------------------
  * replaces hv.AdaptiveHyperVolume.compute_hypervolume(..., 'box') (dmosopt/hv.py:123-189)
  * -> HyperVolumeBoxDecomposition.compute_hypervolume (dmosopt/hv_box_decomposition.py:86-304)

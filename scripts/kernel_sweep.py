@@ -484,7 +484,66 @@ def deepgp_sweep():
         g.close()
 
 
+def deepgp_fit_sweep(n_epochs=200):
+    """Deep GP training (dmo_dgp_fit) at N = 1000, d = 30, H = 3, T = 3, Z1 = Z2 = 128: MDSPP at B 10 (J 3 sites) and MDGP
+    at B 50 (J = B = 50 draws per row).  Per configuration: the time of one epoch (dmo_dgp_fit_epoch: every loss_grad and
+    Adam step, no host synchronisation inside) and of one step, the launches per step, the last layer's kernels timed
+    apart (ProfileScope dgp_fit_last_fwd / dgp_fit_last_bwd / dgp_fit_gram) with their FP64 rate, and one capped
+    deepgp_fit of n_epochs epochs.  The last-layer flop count from shapes, R = J B rows per task: the forward solve and
+    Lq' a (2 R T Z^2), the backward Lq g and back solve (2 R T Z^2) and the lower halves of the two Gram products
+    (2 R T Z^2)."""
+    from dmosopt_b200 import model_gpytorch as mg
+
+    L.context()
+    print(device_line(), flush=True)
+    rng = np.random.default_rng(3)
+    N, d, H, T, Z = 1000, 30, 3, 3, 128
+    X = rng.random((N, d))
+    g = 1.0 + 9.0 / (d - 1) * X[:, 1:].sum(axis=1)
+    Y = np.column_stack((X[:, 0], g * (1.0 - np.sqrt(X[:, 0] / g)), X[:, 0] * X[:, 1] + X[:, 2]))
+    Y = (Y - Y.mean(0)) / Y.std(0)
+    for label, quad, B in (("MDSPP", True, 10), ("MDGP", False, 50)):
+        J = 3 if quad else B
+        raw = mg.deepgp_initial_raw(X, T, quadrature=quad, num_hidden_dims=H, num_inducing_points=Z, rng=np.random.default_rng(1))
+        st = L.DGPFitState(X, Y, H, Z, Z, J, quad, B)
+        st.set_params(mg.deepgp_flatten(raw))
+        perm = rng.permutation(N)
+        nb = -(-N // B)
+        st.epoch(perm, B, 0.01)  # warm-up
+        n0 = L.launch_count()
+        st.epoch(perm, B, 0.01)
+        per_step = (L.launch_count() - n0) / nb
+        L.synchronize()
+        times = []
+        for _ in range(3):
+            t0 = time.perf_counter()
+            st.epoch(perm, B, 0.01)  # ends in a device synchronise
+            times.append((time.perf_counter() - t0) * 1e3)
+        ms = min(times)
+        L.profile_enable(True)
+        st.epoch(perm, B, 0.01)
+        rep = L.profile_report()
+        L.profile_enable(False)
+        R = J * B
+        flop = 6.0 * R * T * Z * Z
+        kms = {k: rep[k][0] / rep[k][1] for k in ("dgp_fit_last_fwd", "dgp_fit_last_bwd", "dgp_fit_gram")}
+        last = sum(kms.values())
+        parts = ", ".join(f"{k[8:]} {v:.3f} ms" for k, v in kms.items())
+        print(f"{label} N={N} d={d} H={H} T={T} Z={Z} B={B} J={J}: epoch {ms:.2f} ms ({nb} steps), step {ms / nb:.3f} ms, "
+              f"{per_step:.1f} launches per step; last layer per step {last:.3f} ms [{parts}] = "
+              f"{flop / last / 1e9:.2f} TFLOP/s FP64 ({flop:.3e} flop)", flush=True)
+        st.close()
+        t0 = time.perf_counter()
+        _, info = mg.deepgp_fit(X, Y, quadrature=quad, num_hidden_dims=H, num_inducing_points=Z, n_iter=n_epochs, batch_size=B, seed=0)
+        s = time.perf_counter() - t0
+        print(f"{label} deepgp_fit capped at {n_epochs} epochs: {s:.1f} s ({info['iterations']} epochs, {info['iterations'] * nb} steps), "
+              f"loss {info['loss'][0]:.4f} -> {info['loss'][-1]:.4f}, final lr {info['lr'][-1]:g}", flush=True)
+
+
 if __name__ == "__main__":
+    if len(sys.argv) > 1 and sys.argv[1] == "deepgp_fit":
+        deepgp_fit_sweep(int(sys.argv[2]) if len(sys.argv) > 2 else 200)
+        sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "deepgp":
         deepgp_sweep()
         sys.exit(0)
