@@ -32,7 +32,7 @@ def euclidean_distance_metric(Y):
     return _lib.euclidean_distance(Y)
 
 
-MAX_OBJECTIVES = 8  # dmo_rank_nd / dmo_crowding_distance (exact hypervolume: the same limit, _lib.HV_MAX_OBJECTIVES)
+MAX_OBJECTIVES = 16  # dmo_rank_nd / dmo_crowding_distance / dmo_age_survival / dmo_ehvi_select (exact hypervolume: 8, _lib.HV_MAX_OBJECTIVES)
 
 _METRIC_CODES = {None: _lib.METRIC_NONE, "crowding": _lib.METRIC_CROWDING, "euclidean": _lib.METRIC_EUCLIDEAN}
 
@@ -107,7 +107,7 @@ class MOEA(object):
         self.local_random = None
         self.state = None
         # limits of the kernels, checked before an epoch starts rather than at the first sortMO (csrc/rank.cu, sortmo.cu:
-        # records and per-objective tables are sized for at most 8 objectives; optimize_mean_variance doubles the count)
+        # records and per-objective tables are sized for at most 16 objectives; optimize_mean_variance doubles the count)
         n_sorted = nOutput * (2 if doubled else 1)
         if n_sorted > MAX_OBJECTIVES:
             raise ValueError(f"dmosopt_b200.{name}: {n_sorted} objectives to sort (nOutput={nOutput}"

@@ -107,6 +107,8 @@ _SIGNATURES = {
                                 _c_int, _c_int, _c_int, _c_int, _vp, _vp, _vp]),
     "dmo_hypervolume": (_c_int, [_vp, _vp, _c_i64, _c_int, _vp, ctypes.POINTER(_c_dbl)]),
     "dmo_hypervolume_ranked": (_c_int, [_vp, _vp, _c_i64, _c_int, _vp, _vp, ctypes.POINTER(_c_dbl)]),
+    "dmo_hypervolume_mc": (_c_int, [_vp, _vp, _c_i64, _c_int, _vp, _c_int, _c_dbl, _c_dbl, _c_i64, _c_u64, _c_u64, ctypes.POINTER(_c_dbl),
+                                    ctypes.POINTER(_c_i64), ctypes.POINTER(_c_i64), ctypes.POINTER(_c_int)]),
     "dmo_ehvi_select": (_c_int, [_vp, _vp, _c_i64, _vp, _vp, _c_i64, _c_int, _vp, _c_int, _c_i64, _vp, _vp]),
     "dmo_get_duplicates": (_c_int, [_vp, _vp, _c_i64, _c_int, _c_dbl, _vp]),
     "dmo_get_duplicates_pair": (_c_int, [_vp, _vp, _c_i64, _vp, _c_i64, _c_int, _c_dbl, _vp]),
@@ -1167,6 +1169,39 @@ def hypervolume(F, ref, rank=None):
         assert rk.shape == (n,)
         _check(load_library().dmo_hypervolume_ranked(context(), _ptr(F), n, M, _ptr(ref), _ptr(rk), ctypes.byref(out)), "dmo_hypervolume_ranked")
     return float(out.value)
+
+
+HVMC_ALGORITHMS = {"hybrid": 0, "fpras": 1, "mcm2rv": 2, "monte_carlo": 3}
+HVMC_MAX_OBJECTIVES = 16  # dmo_hypervolume_mc (csrc/hv_mc.cu)
+_HVMC_RAN = {1: "FPRAS", 2: "MCM2RV", 3: "MonteCarlo", 4: "Hybrid-FPRAS", 5: "Hybrid-MCM2RV"}
+
+
+def hypervolume_mc(F, ref, algorithm="hybrid", epsilon=0.01, delta=0.25, n_samples=100000, seed=0, stream=0):
+    """Monte-Carlo hypervolume estimate of the rows of F strictly inside ref (2 <= M <= 16), on the GPU.
+
+    ``algorithm``: "hybrid", "fpras", "mcm2rv" (the (epsilon, delta) estimators of dmosopt/hv_adaptive.py) or
+    "monte_carlo" (``n_samples`` uniform points, dmosopt/hv.py:191-241).  The result is a pure function of the filtered
+    front, ``seed`` and ``stream`` (< 2^24).  Returns (value, info) with info = {"samples", "tests", "algorithm"}; "tests" counts
+    the point-against-row tests performed (dmo_hypervolume_mc in include/dmosopt_b200.h says how that differs from the
+    reference's num_comparisons for mcm2rv and monte_carlo)."""
+    if algorithm not in HVMC_ALGORITHMS:
+        raise ValueError(f"hypervolume_mc: unknown algorithm {algorithm!r} (one of {sorted(HVMC_ALGORITHMS)})")
+    F = _f64(F)
+    if F.ndim == 1:
+        F = F.reshape(1, -1)
+    n, M = F.shape
+    ref = _f64(ref).reshape(-1)
+    if ref.shape[0] != M:
+        raise ValueError(f"hypervolume_mc: ref has {ref.shape[0]} coordinates, the points have {M}")
+    out = _c_dbl(0.0)
+    ns, nt, ran = _c_i64(0), _c_i64(0), _c_int(0)
+    _check(
+        load_library().dmo_hypervolume_mc(context(), _ptr(F), n, M, _ptr(ref), HVMC_ALGORITHMS[algorithm], float(epsilon), float(delta),
+                                          int(n_samples), int(seed) & (2**64 - 1), int(stream), ctypes.byref(out), ctypes.byref(ns),
+                                          ctypes.byref(nt), ctypes.byref(ran)),
+        "dmo_hypervolume_mc",
+    )
+    return float(out.value), {"samples": int(ns.value), "tests": int(nt.value), "algorithm": _HVMC_RAN.get(ran.value)}
 
 
 def ehvi_select(F, means, variances, ref, k, nds=True, return_scores=False):

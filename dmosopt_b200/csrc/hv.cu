@@ -87,7 +87,8 @@ __global__ void min_col_kernel(const double* __restrict__ F, int64_t n, double* 
 // objective 0 is <= its own and stops at the first dominator (warp-wide early exit).  For a scattered cloud almost
 // every point finds a dominator within the first tile; for a true front it is the full n^2/2 scan.
 constexpr int ND_T = 128;
-constexpr int ND_MAXM = 8;
+// ND_MAXM: size of the target's register copy, 8 or 16 (two instances, so that the one for M <= 8 is unchanged)
+template <int ND_MAXM>
 __global__ void __launch_bounds__(ND_T) nondominated_flag_kernel(const double* __restrict__ F, const uint32_t* __restrict__ sidx,
                                                                  int64_t n, int M, int32_t* __restrict__ flag) {
   extern __shared__ double tile_nd[];  // [ND_T][M]
@@ -358,7 +359,7 @@ __global__ void hv_volume_terms_kernel(HvArrays A, int64_t n, double* __restrict
 }
 
 // ---- EHVI -----------------------------------------------------------------------------------------------
-constexpr int EH_MAXM = 8;
+constexpr int EH_MAX_OBJ = 16;
 
 // boxes between consecutive f0-sorted front points (hv_box_decomposition.py:418-437)
 __global__ void box_flag_kernel(const double* __restrict__ front, const uint32_t* __restrict__ sidx, int64_t nf, int M,
@@ -389,6 +390,8 @@ __global__ void box_write_kernel(const double* __restrict__ front, const uint32_
 }
 
 // score_c = sum_b prod_j [ sd (phi(zl) - phi(zu)) + mu (Phi(zu) - Phi(zl)) ]   (hv_box_decomposition.py:353-416)
+// EH_MAXM: size of the candidate's register copy, 8 or 16 (two instances, so that the one for M <= 8 is unchanged)
+template <int EH_MAXM>
 __global__ void ehvi_kernel(const double* __restrict__ lower, const double* __restrict__ upper, int64_t nb, int M,
                             const double* __restrict__ means, const double* __restrict__ variances, int64_t nc,
                             double* __restrict__ score) {
@@ -477,8 +480,12 @@ int nondominated_subset(dmo_ctx* ctx, const double* dF, int64_t n, int M, DevBuf
   DMO_TRY(sort_by_column(ctx, dF, n, M, 0, sidx));
   {
     ProfileScope ps(ctx, "nd_filter");
-    DMO_LAUNCH(nondominated_flag_kernel, (unsigned)ceil_div(n, ND_T), ND_T, (size_t)ND_T * M * sizeof(double), dF, sidx.p, n, M,
-               flag.p);
+    if (M <= 8)
+      DMO_LAUNCH(nondominated_flag_kernel<8>, (unsigned)ceil_div(n, ND_T), ND_T, (size_t)ND_T * M * sizeof(double), dF, sidx.p, n, M,
+                 flag.p);
+    else
+      DMO_LAUNCH(nondominated_flag_kernel<16>, (unsigned)ceil_div(n, ND_T), ND_T, (size_t)ND_T * M * sizeof(double), dF, sidx.p, n, M,
+                 flag.p);
   }
   DMO_TRY(compact_rows(ctx, dF, n, M, flag, out, count));
   return DMO_OK;
@@ -507,6 +514,20 @@ int sum_partials(dmo_ctx* ctx, DevBuf<double>& partial, int64_t nb, double* h_ou
 }
 
 }  // namespace
+
+// Rows strictly inside ref, then their non-dominated subset, in row order (the Monte-Carlo estimators' front, hv_mc.cu).
+int hv_inside_nondominated(dmo_ctx* ctx, const double* dF, int64_t n, int M, const double* dref, DevBuf<double>& out,
+                           int64_t* count) {
+  *count = 0;
+  DevBuf<int32_t> flag;
+  DevBuf<double> Fin;
+  int64_t n1 = 0;
+  DMO_TRY(flag.alloc(ctx, n + 1));
+  DMO_LAUNCH(inside_flag_kernel, (unsigned)ceil_div(n + 1, 256), 256, 0, dF, n, M, dref, (const int32_t*)nullptr, flag.p);
+  DMO_TRY(compact_rows(ctx, dF, n, M, flag, Fin, &n1));
+  if (n1 == 0) return DMO_OK;
+  return nondominated_subset(ctx, Fin.p, n1, M, out, count);
+}
 
 // d_rank (optional, device, (n,)): non-dominated ranks of the rows within a SUPERSET they were selected from by rank
 // (dmo_remove_worst).  Rows with rank > 0 are dominated by a rank-0 row of the same set, so they add no volume and are
@@ -703,7 +724,7 @@ int dmo_ehvi_select(dmo_ctx* ctx, const double* F, int64_t nf, const double* mea
                     int M, const double* ref, int nds, int64_t k, int64_t* sel, double* score) {
   if (!ctx) return DMO_ERR_ARG;
   DMO_CUDA(cudaSetDevice(ctx->device));
-  DMO_REQUIRE(F && means && variances && ref && sel && nf > 0 && nc > 0 && k > 0 && M >= 1 && M <= EH_MAXM,
+  DMO_REQUIRE(F && means && variances && ref && sel && nf > 0 && nc > 0 && k > 0 && M >= 1 && M <= EH_MAX_OBJ,
               "ehvi_select: bad arguments");
   if (k > nc) k = nc;
   In<double> f, mu, var, r;
@@ -739,8 +760,12 @@ int dmo_ehvi_select(dmo_ctx* ctx, const double* F, int64_t nf, const double* mea
   if (nb > 0)
     DMO_LAUNCH(box_write_kernel, (unsigned)ceil_div(nfr + 1, 256), 256, 0, front, sidx.p, nfr, M, r.d, flag.p, pos.p,
                lower.p, upper.p);
-  DMO_LAUNCH(ehvi_kernel, (unsigned)ceil_div(nc, 128), 128, 2 * 64 * M * sizeof(double), lower.p, upper.p, (int64_t)nb,
-             M, mu.d, var.d, nc, sc.p);
+  if (M <= 8)
+    DMO_LAUNCH(ehvi_kernel<8>, (unsigned)ceil_div(nc, 128), 128, 2 * 64 * M * sizeof(double), lower.p, upper.p, (int64_t)nb,
+               M, mu.d, var.d, nc, sc.p);
+  else
+    DMO_LAUNCH(ehvi_kernel<16>, (unsigned)ceil_div(nc, 128), 128, 2 * 64 * M * sizeof(double), lower.p, upper.p, (int64_t)nb,
+               M, mu.d, var.d, nc, sc.p);
   // k largest scores, ties by candidate index
   DevBuf<uint64_t> k0, k1;
   DevBuf<uint32_t> i0, i1;

@@ -18,7 +18,7 @@ namespace {
 // and receives that sum as its crowding value (:410-428).  One CTA; every thread owns a strided slice of the points and
 // keeps their two smallest distances in shared memory; per step one block-wide arg-max and one distance update.
 constexpr int AGE_T = 1024;
-constexpr int AGE_MAXM = 8;
+constexpr int AGE_MAXM = 16;
 
 __device__ __forceinline__ double minkowski(const double* a, const double* b, int M, double p) {
   double s = 0.0;

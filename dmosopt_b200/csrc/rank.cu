@@ -321,8 +321,9 @@ __device__ __forceinline__ int maxplus_packed(const int8_t* row, const int16_t* 
   return max((int)(int16_t)(m & 0xFFFFu), (int)(int16_t)(m >> 16));
 }
 
+// Above eight objectives the shared memory alone limits a CTA to four per SM, so the register cap follows that.
 template <int M, int T, bool SEG>
-__global__ void __launch_bounds__(T, SEG ? 4 : 5) rank_chain_kernel(uint32_t* rec, int nblocks, int* __restrict__ rankS, int* ticket,
+__global__ void __launch_bounds__(T, (SEG || M > 8) ? 4 : 5) rank_chain_kernel(uint32_t* rec, int nblocks, int* __restrict__ rankS, int* ticket,
                                                                  int* errflag, long long* trace, RankSeg sg) {
   // optional per-block time stamps (DMO_RANK_TRACE=<file>): 16 x globaltimer ns, then 16 x clock64, see scripts/rank_trace.py
 #define RANK_TRACE(slot)                                                         \
@@ -342,7 +343,12 @@ __global__ void __launch_bounds__(T, SEG ? 4 : 5) rank_chain_kernel(uint32_t* re
   constexpr int DLD = T + 16;
   constexpr int SENT = -128;  // "no in-block path"; real path lengths are 0 .. T-1 <= 127
   constexpr int PACK_LIMIT = 32000;  // ranks up to here take the packed 16-bit max-plus path
-  __shared__ uint4 tile[T * NV];   // own block's records during table construction, then stream buffer 0
+  // own block's records during table construction, then stream buffer 0.  With five uint4 per record (M == 16) it
+  // would take the static shared memory past 48 KB, so there it is the kernel's dynamic shared memory instead.
+  constexpr bool DYN_TILE = NV > 4;
+  __shared__ uint4 tile_s[DYN_TILE ? 1 : T * NV];
+  extern __shared__ uint4 tile_dyn[];
+  uint4* const tile = DYN_TILE ? tile_dyn : tile_s;
   constexpr bool DBUF = NV <= 2;  // M == 8 (three uint4 per record) would exceed 48 KB of static shared memory
   __shared__ uint4 tile2[DBUF ? T * NV : 1];  // stream buffer 1
   __shared__ __align__(16) int sh_r1[T];
@@ -981,8 +987,12 @@ int launch_chain(dmo_ctx* ctx, uint32_t* rec, int nblocks, int* rankS, int* tick
     DMO_TRY(trace.alloc(ctx, (size_t)nblocks * 32));
     DMO_CUDA(cudaMemsetAsync(trace.p, 0, (size_t)nblocks * 32 * sizeof(long long), ctx->stream));
   }
+  constexpr int NV = (M + 1 + 3) / 4;
+  const size_t dyn = NV > 4 ? (size_t)RANK_T * NV * sizeof(uint4) : 0;  // the kernel's DYN_TILE
+  if (dyn > 0)
+    DMO_CUDA(cudaFuncSetAttribute(rank_chain_kernel<M, RANK_T, SEG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
   int occ = 0;
-  DMO_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, rank_chain_kernel<M, RANK_T, SEG>, RANK_T, 0));
+  DMO_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, rank_chain_kernel<M, RANK_T, SEG>, RANK_T, dyn));
   if (occ < 1) occ = 1;
   // fewer co-resident CTAs per SM shorten the serial chain (the block on the critical path shares its SM's issue
   // slots with the others); DMO_RANK_OCC overrides for tuning
@@ -992,7 +1002,7 @@ int launch_chain(dmo_ctx* ctx, uint32_t* rec, int nblocks, int* rankS, int* tick
   int nctas = nblocks < occ * ctx->sm_count ? nblocks : occ * ctx->sm_count;
   {
     ProfileScope ps(ctx, "rank_chain");
-    DMO_LAUNCH((rank_chain_kernel<M, RANK_T, SEG>), nctas, RANK_T, 0, rec, nblocks, rankS, ticket, errflag, trace.p, sg);
+    DMO_LAUNCH((rank_chain_kernel<M, RANK_T, SEG>), nctas, RANK_T, dyn, rec, nblocks, rankS, ticket, errflag, trace.p, sg);
     DMO_CHECK_LAUNCH();
   }
   if (trace.p) {
@@ -1297,7 +1307,7 @@ int rank_by_peeling(dmo_ctx* ctx, const uint32_t* R, const uint32_t* maxid, int6
 
 int rank_nd_device_ex(dmo_ctx* ctx, const double* dY, int64_t n, int M, int32_t* d_rank, bool flags_only, int64_t keep = 0) {
   if (n <= 0) return DMO_OK;
-  DMO_REQUIRE(M >= 1 && M <= 8, "rank_nd: M=%d out of range [1,8]", M);
+  DMO_REQUIRE(M >= 1 && M <= 16, "rank_nd: M=%d out of range [1,16]", M);
   DMO_REQUIRE(n < ((int64_t)1 << 31) - 4096, "rank_nd: n too large");
   const unsigned g = (unsigned)ceil_div(n, 256);
 
@@ -1408,7 +1418,15 @@ int rank_nd_device_ex(dmo_ctx* ctx, const double* dY, int64_t n, int M, int32_t*
       case 5: DMO_TRY(launch_nd_flags<5>(ctx, rec.p, (int)nblocks, rankS.p)); break;
       case 6: DMO_TRY(launch_nd_flags<6>(ctx, rec.p, (int)nblocks, rankS.p)); break;
       case 7: DMO_TRY(launch_nd_flags<7>(ctx, rec.p, (int)nblocks, rankS.p)); break;
-      default: DMO_TRY(launch_nd_flags<8>(ctx, rec.p, (int)nblocks, rankS.p)); break;
+      case 8: DMO_TRY(launch_nd_flags<8>(ctx, rec.p, (int)nblocks, rankS.p)); break;
+      case 9: DMO_TRY(launch_nd_flags<9>(ctx, rec.p, (int)nblocks, rankS.p)); break;
+      case 10: DMO_TRY(launch_nd_flags<10>(ctx, rec.p, (int)nblocks, rankS.p)); break;
+      case 11: DMO_TRY(launch_nd_flags<11>(ctx, rec.p, (int)nblocks, rankS.p)); break;
+      case 12: DMO_TRY(launch_nd_flags<12>(ctx, rec.p, (int)nblocks, rankS.p)); break;
+      case 13: DMO_TRY(launch_nd_flags<13>(ctx, rec.p, (int)nblocks, rankS.p)); break;
+      case 14: DMO_TRY(launch_nd_flags<14>(ctx, rec.p, (int)nblocks, rankS.p)); break;
+      case 15: DMO_TRY(launch_nd_flags<15>(ctx, rec.p, (int)nblocks, rankS.p)); break;
+      default: DMO_TRY(launch_nd_flags<16>(ctx, rec.p, (int)nblocks, rankS.p)); break;
     }
     DMO_LAUNCH(scatter_rank_kernel, g, 256, 0, rankS.p, perm, n, d_rank);
     DMO_CHECK_LAUNCH();
@@ -1450,7 +1468,15 @@ int rank_nd_device_ex(dmo_ctx* ctx, const double* dY, int64_t n, int M, int32_t*
       case 5: DMO_TRY((launch_chain<5, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
       case 6: DMO_TRY((launch_chain<6, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
       case 7: DMO_TRY((launch_chain<7, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
-      default: DMO_TRY((launch_chain<8, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
+      case 8: DMO_TRY((launch_chain<8, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
+      case 9: DMO_TRY((launch_chain<9, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
+      case 10: DMO_TRY((launch_chain<10, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
+      case 11: DMO_TRY((launch_chain<11, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
+      case 12: DMO_TRY((launch_chain<12, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
+      case 13: DMO_TRY((launch_chain<13, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
+      case 14: DMO_TRY((launch_chain<14, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
+      case 15: DMO_TRY((launch_chain<15, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
+      default: DMO_TRY((launch_chain<16, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
     }
   }
   DMO_LAUNCH(scatter_rank_kernel, g, 256, 0, rankS.p, perm, n, d_rank);

@@ -9,7 +9,7 @@
 
 namespace {
 
-constexpr int MAXM = 8;
+constexpr int MAX_OBJ = 16;  // objectives; the kernels below size their register arrays MAXM = 8 or 16
 
 __global__ void minmax_init_kernel(uint64_t* mn, uint64_t* mx, int M) {
   int j = threadIdx.x;
@@ -20,6 +20,7 @@ __global__ void minmax_init_kernel(uint64_t* mn, uint64_t* mx, int M) {
 }
 
 // column-wise min / max of a row-major (n, M) matrix through order-preserving 64-bit keys
+template <int MAXM>
 __global__ void minmax_kernel(const double* __restrict__ Y, int64_t n, int M, uint64_t* mn, uint64_t* mx) {
   __shared__ uint64_t smn[MAXM], smx[MAXM];
   if (threadIdx.x < M) {
@@ -96,6 +97,7 @@ __global__ void crowd_contrib_kernel(const uint64_t* __restrict__ skeys, const u
 }
 
 // D[i] = sum of the M contributions in (sorted position, objective) order (indicators.py:46-49)
+template <int MAXM>
 __global__ void crowd_sum_kernel(const double* __restrict__ contrib, const uint32_t* __restrict__ pos, int64_t n, int M,
                                  double* __restrict__ D) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -108,7 +110,7 @@ __global__ void crowd_sum_kernel(const double* __restrict__ contrib, const uint3
       key[j] = (uint64_t)pos[i * M + j] * (uint64_t)M + (uint64_t)j;
       c[j] = contrib[i * M + j];
     }
-  // insertion sort of <= 8 items by key
+  // insertion sort of <= MAXM items by key
 #pragma unroll
   for (int a = 1; a < MAXM; ++a)
     if (a < M) {
@@ -137,6 +139,7 @@ __global__ void fill_f64_kernel(double* out, int64_t n, double v) {
   if (i < n) out[i] = v;
 }
 
+template <int MAXM>
 __global__ void euclid_kernel(const double* __restrict__ Y, int64_t n, int M, const uint64_t* mn, const uint64_t* mx,
                               double* __restrict__ D) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -149,7 +152,16 @@ __global__ void euclid_kernel(const double* __restrict__ Y, int64_t n, int M, co
       sq[j] = __dmul_rn(u, u);
     }
   double s;
-  if (M == 8) {  // numpy's pairwise sum switches to 8 accumulators at 8 elements
+  if (MAXM > 8 && M > 8) {
+    // numpy's pairwise sum from 8 elements on: 8 accumulators over the blocks of 8, combined as a tree, then the rest in order
+    double r[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) r[j] = (M == 16) ? __dadd_rn(sq[j], sq[8 + j]) : sq[j];
+    s = __dadd_rn(__dadd_rn(__dadd_rn(r[0], r[1]), __dadd_rn(r[2], r[3])), __dadd_rn(__dadd_rn(r[4], r[5]), __dadd_rn(r[6], r[7])));
+#pragma unroll
+    for (int j = 8; j < MAXM; ++j)
+      if (j < M && M < 16) s = __dadd_rn(s, sq[j]);
+  } else if (M == 8) {  // numpy's pairwise sum switches to 8 accumulators at 8 elements
     s = __dadd_rn(__dadd_rn(__dadd_rn(sq[0], sq[1]), __dadd_rn(sq[2], sq[3])),
                   __dadd_rn(__dadd_rn(sq[4], sq[5]), __dadd_rn(sq[6], sq[7])));
   } else {
@@ -295,7 +307,10 @@ __global__ void duplicates_kernel(const double* __restrict__ X, const uint64_t* 
 int column_minmax(dmo_ctx* ctx, const double* dY, int64_t n, int M, uint64_t* mn, uint64_t* mx) {
   DMO_LAUNCH(minmax_init_kernel, 1, 32, 0, mn, mx, M);
   int grid = (int)(ceil_div(n, 256) < ctx->sm_count * 4 ? ceil_div(n, 256) : ctx->sm_count * 4);
-  DMO_LAUNCH(minmax_kernel, grid, 256, 0, dY, n, M, mn, mx);
+  if (M <= 8)
+    DMO_LAUNCH(minmax_kernel<8>, grid, 256, 0, dY, n, M, mn, mx);
+  else
+    DMO_LAUNCH(minmax_kernel<16>, grid, 256, 0, dY, n, M, mn, mx);
   DMO_CHECK_LAUNCH();
   return DMO_OK;
 }
@@ -304,7 +319,7 @@ int column_minmax(dmo_ctx* ctx, const double* dY, int64_t n, int M, uint64_t* mn
 
 int crowding_device(dmo_ctx* ctx, const double* dY, int64_t n, int M, double* dD) {
   if (n <= 0) return DMO_OK;
-  DMO_REQUIRE(M >= 1 && M <= MAXM, "crowding: M=%d out of range [1,%d]", M, MAXM);
+  DMO_REQUIRE(M >= 1 && M <= MAX_OBJ, "crowding: M=%d out of range [1,%d]", M, MAX_OBJ);
   const unsigned g = (unsigned)ceil_div(n, 256);
   if (n == 1) {  // indicators.py:23-24
     DMO_LAUNCH(fill_f64_kernel, 1, 32, 0, dD, 1, 1.0);
@@ -314,31 +329,37 @@ int crowding_device(dmo_ctx* ctx, const double* dY, int64_t n, int M, double* dD
   DevBuf<uint64_t> mm, k0, k1;
   DevBuf<uint32_t> i0, i1, pos;
   DevBuf<double> contrib;
-  DMO_TRY(mm.alloc(ctx, 2 * MAXM));
+  DMO_TRY(mm.alloc(ctx, 2 * MAX_OBJ));
   DMO_TRY(k0.alloc(ctx, n));
   DMO_TRY(k1.alloc(ctx, n));
   DMO_TRY(i0.alloc(ctx, n));
   DMO_TRY(i1.alloc(ctx, n));
   DMO_TRY(pos.alloc(ctx, (size_t)n * M));
   DMO_TRY(contrib.alloc(ctx, (size_t)n * M));
-  DMO_TRY(column_minmax(ctx, dY, n, M, mm.p, mm.p + MAXM));
+  DMO_TRY(column_minmax(ctx, dY, n, M, mm.p, mm.p + MAX_OBJ));
   for (int j = 0; j < M; ++j) {
-    DMO_LAUNCH(crowd_keys_kernel, g, 256, 0, dY, n, M, j, mm.p, mm.p + MAXM, k0.p, i0.p);
+    DMO_LAUNCH(crowd_keys_kernel, g, 256, 0, dY, n, M, j, mm.p, mm.p + MAX_OBJ, k0.p, i0.p);
     DMO_TRY(prim_sort_pairs_u64(ctx, k0.p, k1.p, i0.p, i1.p, n, 0, 64));
     DMO_LAUNCH(crowd_contrib_kernel, g, 256, 0, k1.p, i1.p, n, M, j, contrib.p, pos.p);
   }
-  DMO_LAUNCH(crowd_sum_kernel, g, 256, 0, contrib.p, pos.p, n, M, dD);
+  if (M <= 8)
+    DMO_LAUNCH(crowd_sum_kernel<8>, g, 256, 0, contrib.p, pos.p, n, M, dD);
+  else
+    DMO_LAUNCH(crowd_sum_kernel<16>, g, 256, 0, contrib.p, pos.p, n, M, dD);
   DMO_CHECK_LAUNCH();
   return DMO_OK;
 }
 
 int euclidean_device(dmo_ctx* ctx, const double* dY, int64_t n, int M, double* dD) {
   if (n <= 0) return DMO_OK;
-  DMO_REQUIRE(M >= 1 && M <= MAXM, "euclidean: M=%d out of range [1,%d]", M, MAXM);
+  DMO_REQUIRE(M >= 1 && M <= MAX_OBJ, "euclidean: M=%d out of range [1,%d]", M, MAX_OBJ);
   DevBuf<uint64_t> mm;
-  DMO_TRY(mm.alloc(ctx, 2 * MAXM));
-  DMO_TRY(column_minmax(ctx, dY, n, M, mm.p, mm.p + MAXM));
-  DMO_LAUNCH(euclid_kernel, (unsigned)ceil_div(n, 256), 256, 0, dY, n, M, mm.p, mm.p + MAXM, dD);
+  DMO_TRY(mm.alloc(ctx, 2 * MAX_OBJ));
+  DMO_TRY(column_minmax(ctx, dY, n, M, mm.p, mm.p + MAX_OBJ));
+  if (M <= 8)
+    DMO_LAUNCH(euclid_kernel<8>, (unsigned)ceil_div(n, 256), 256, 0, dY, n, M, mm.p, mm.p + MAX_OBJ, dD);
+  else
+    DMO_LAUNCH(euclid_kernel<16>, (unsigned)ceil_div(n, 256), 256, 0, dY, n, M, mm.p, mm.p + MAX_OBJ, dD);
   DMO_CHECK_LAUNCH();
   return DMO_OK;
 }

@@ -8,7 +8,9 @@ called by the reference's controller code directly on its own modules, so swappi
   * ``MOASMO.get_best``                   ``MOEA.get_duplicates(y)`` + ``MOEA.sortMO`` (dmosopt/MOASMO.py:581-639)
   * per-generation termination            ``dmosopt.hv.AdaptiveHyperVolume.compute_hypervolume`` of the whole
                                           population (dmosopt/hv_termination.py:1093-1134 via the multi-fidelity
-                                          tracker; dmosopt/hv.py:123-189)
+                                          tracker; dmosopt/hv.py:123-241): 'box' exactly for 1 .. 8 objectives, the
+                                          Monte-Carlo branches for 2 .. 16 objectives (hv.HV_MC_DEFAULT_SEED,
+                                          consecutive calls on consecutive streams); the rest stays with the reference
   * the rank function of every ``sortMO`` ``dmosopt.dda.dda_ens`` (dmosopt/dda.py:97-152)
 
 ``install()`` rebinds exactly those module attributes of an already importable ``dmosopt`` package to the functions of
@@ -22,6 +24,7 @@ import numpy as np
 
 from . import MOEA as _MOEA
 from . import _lib
+from . import hv as _hv
 from . import indicators as _ind
 
 _saved = []
@@ -57,14 +60,29 @@ def install(package="dmosopt"):
         _set(moea, "dda_ens", _dda_ens)
 
     original = hv.AdaptiveHyperVolume.compute_hypervolume
+    mc_seed = _hv.HV_MC_DEFAULT_SEED
+    mc_calls = [0]
 
     def compute_hypervolume(self, pareto_front, algorithm=None, verbose=False):
-        exact = algorithm == "box" or (algorithm in (None, "auto") and self.n_objectives < self.dimension_threshold_exact)
+        auto = algorithm in (None, "auto")
+        exact = algorithm == "box" or (auto and self.n_objectives < self.dimension_threshold_exact)
         if exact and 1 <= self.n_objectives <= _lib.HV_MAX_OBJECTIVES:
             pf = np.asarray(pareto_front, dtype=np.float64)
             if len(pf) == 0:
                 return 0.0
             return _lib.hypervolume(pf, self.ref_point)  # points not strictly inside ref are ignored, as hv.py:159 does
+        if not exact and 2 <= self.n_objectives <= _lib.HVMC_MAX_OBJECTIVES:
+            # the Monte-Carlo branches; the reference's defaults for attributes a subclass or stand-in may lack
+            if auto:
+                algorithm = "hybrid" if getattr(self, "use_adaptive_mc", True) else "monte_carlo"
+            if algorithm in _lib.HVMC_ALGORITHMS:
+                pf = np.asarray(pareto_front, dtype=np.float64)
+                if len(pf) == 0:
+                    return 0.0
+                value, _ = _lib.hypervolume_mc(pf, self.ref_point, algorithm, getattr(self, "mc_epsilon", 0.01), getattr(self, "mc_delta", 0.25),
+                                               getattr(self, "monte_carlo_samples", 100000), seed=mc_seed, stream=mc_calls[0] % (1 << 24))
+                mc_calls[0] += 1
+                return value
         return original(self, pareto_front, algorithm, verbose)
 
     _set(hv.AdaptiveHyperVolume, "compute_hypervolume", compute_hypervolume)

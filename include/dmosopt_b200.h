@@ -421,6 +421,28 @@ int dmo_hypervolume(dmo_ctx* ctx, const double* F, int64_t n, int M, const doubl
 int dmo_hypervolume_ranked(dmo_ctx* ctx, const double* F, int64_t n, int M, const double* ref,
                            const int32_t* rank, double* out);
 
+/* ---- A16: Monte-Carlo hypervolume (2 <= M <= 16) -----------------------------
+ * replaces the non-'box' branches of hv.AdaptiveHyperVolume.compute_hypervolume (dmosopt/hv.py:123-241) and
+ * compute_hypervolume_fpras / _mcm2rv / _hybrid (dmosopt/hv_adaptive.py:188-855).  F (n,M) host or device, ref (M,).
+ * Estimates the volume of the rows strictly inside ref, after their non-dominated filter (the reference passes the
+ * unfiltered front; see DESIGN.md section 4.3).  algorithm: DMO_HVMC_HYBRID / _FPRAS / _MCM2RV (epsilon, delta in (0, 1))
+ * or _MONTE_CARLO (n_samples uniform points).  Random numbers: Philox keyed by seed and stream_id (< 2^24); the result
+ * is bit-identical for the same (front, seed, stream_id).  samples_out: N (successful samples; monte_carlo: points
+ * drawn), tests_out: dominance tests (point against one front row) performed: for fpras the budget M1, as the
+ * reference counts; for mcm2rv and monte_carlo the rows scanned up to the first dominator of each point, plus one per
+ * eta (the reference counts n rows per point, or one per point with its k-d tree); algorithm_out: the estimator that ran
+ * (a DMO_HVMC_* code, _HYBRID_FPRAS / _HYBRID_MCM2RV when the hybrid decided after its FPRAS rounds); each may be NULL.
+ * FPRAS budgets M1 = 8 (1 + epsilon) n ln(2 / delta) / epsilon^2 must stay below 2^34 tests (DMO_ERR_ARG otherwise). */
+#define DMO_HVMC_HYBRID 0
+#define DMO_HVMC_FPRAS 1
+#define DMO_HVMC_MCM2RV 2
+#define DMO_HVMC_MONTE_CARLO 3
+#define DMO_HVMC_HYBRID_FPRAS 4
+#define DMO_HVMC_HYBRID_MCM2RV 5
+int dmo_hypervolume_mc(dmo_ctx* ctx, const double* F, int64_t n, int M, const double* ref, int algorithm, double epsilon,
+                       double delta, int64_t n_samples, uint64_t seed, uint64_t stream_id, double* out,
+                       int64_t* samples_out, int64_t* tests_out, int* algorithm_out);
+
 /* ---- A17: HV-improvement (EHVI) candidate selection -----------------------------
  * replaces indicators.HypervolumeImprovement._do (dmosopt/indicators.py:295-313) ->
  * HyperVolumeBoxDecomposition.select_candidates / _compute_batch_ehvi /

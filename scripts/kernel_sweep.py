@@ -540,7 +540,76 @@ def deepgp_fit_sweep(n_epochs=200):
               f"loss {info['loss'][0]:.4f} -> {info['loss'][-1]:.4f}, final lr {info['lr'][-1]:g}", flush=True)
 
 
+def many_sweep():
+    """Many-objective runs.  (1) Rank (dmo_rank_nd) and truncation to half (dmo_remove_worst, no metric) at n = 131072,
+    M 10 and 16, on bench.objective_sets' uniform and sphere sets, device-resident, CUDA events.  (2) dmo_hypervolume_mc
+    per algorithm (epsilon 0.01, delta 0.25, 100000 monte_carlo points) on sphere fronts of 1000, 4000 and 16000 points,
+    M 10 and 16, ref 1.1: host time of the whole call (it ends in a device synchronise), samples, dominance tests and
+    tests/s, and the rate of the front-row bytes those tests read (M float64 each).  (3) The reference's
+    compute_hypervolume_hybrid (oracle/_ref, on the host) at epsilon 0.05 on a 200-point front, with the GPU's hybrid on the
+    same front and settings."""
+    import bench
+
+    L.context()
+    print(device_line(), flush=True)
+    lib, ctx = L.load_library(), L.context()
+    n = 131072
+    for M in (10, 16):
+        for kind, Y in bench.objective_sets(n, M).items():
+            d = L.DeviceArray((n, M)).upload(Y)
+            x = L.DeviceArray((n, 1)).upload(np.zeros((n, 1)))
+            r = L.DeviceArray((n,), np.int32)
+            keep = n // 2
+            perm = L.DeviceArray((keep,), np.int64)
+            ms_rank = timed(lambda: L._check(lib.dmo_rank_nd(ctx, d.ptr, n, M, r.ptr), "rank"))
+            ms_trunc = timed(lambda: L._check(lib.dmo_remove_worst(ctx, x.ptr, d.ptr, n, 1, M, L.METRIC_NONE, None, 0, keep, None, None, None,
+                                                                   perm.ptr), "remove_worst"))
+            rk = r.download()
+            print(f"rank n={n} M={M} {kind}: {ms_rank:.3f} ms ({rk.max() + 1} fronts, {int((rk == 0).sum())} in front 0); "
+                  f"truncation to {keep}: {ms_trunc:.3f} ms", flush=True)
+    for M in (10, 16):
+        for nf in (1000, 4000, 16000):
+            F = bench.objective_sets(nf, M)["sphere"]
+            ref = np.full(M, 1.1)
+            for algo in ("hybrid", "fpras", "mcm2rv", "monte_carlo"):
+                L.hypervolume_mc(F, ref, algo, 0.01, 0.25, seed=1, stream=0)  # warm-up
+                t0 = time.perf_counter()
+                v, info = L.hypervolume_mc(F, ref, algo, 0.01, 0.25, seed=1, stream=1)
+                s = time.perf_counter() - t0
+                rate = info["tests"] / s
+                print(f"hv_mc n={nf} M={M} {algo}: {s * 1e3:.1f} ms, value {v:.6g}, ran {info['algorithm']}, samples {info['samples']}, "
+                      f"tests {info['tests']:.3e}, {rate:.3e} tests/s, front-row reads {rate * M * 8 / 1e9:.1f} GB/s", flush=True)
+    from oracle import reference_build
+
+    path = reference_build.reference_path()
+    if path is None:
+        print("reference hybrid: not measured (oracle/_ref not built)", flush=True)
+        return
+    sys.path.insert(0, path)
+    import contextlib
+    import io
+
+    from dmosopt import hv_adaptive
+
+    for M in (10, 16):
+        F = bench.objective_sets(200, M)["sphere"]
+        ref = np.full(M, 1.1)
+        t0 = time.perf_counter()
+        v, info = L.hypervolume_mc(F, ref, "hybrid", 0.05, 0.25, seed=1, stream=2)
+        s_gpu = time.perf_counter() - t0
+        np.random.seed(0)
+        t0 = time.perf_counter()
+        with contextlib.redirect_stdout(io.StringIO()):  # the reference prints once per MCM2RV iteration
+            res = hv_adaptive.compute_hypervolume_hybrid(F, ref, 0.05, 0.25)
+        s_ref = time.perf_counter() - t0
+        print(f"hybrid n=200 M={M} eps 0.05: GPU {s_gpu * 1e3:.1f} ms ({info['algorithm']}, {v:.6g}); reference on the host "
+              f"{s_ref * 1e3:.1f} ms ({res.algorithm_used}, {res.hypervolume:.6g}, {res.num_comparisons} comparisons)", flush=True)
+
+
 if __name__ == "__main__":
+    if len(sys.argv) > 1 and sys.argv[1] == "many":
+        many_sweep()
+        sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "deepgp_fit":
         deepgp_fit_sweep(int(sys.argv[2]) if len(sys.argv) > 2 else 200)
         sys.exit(0)
