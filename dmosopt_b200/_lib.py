@@ -122,6 +122,9 @@ _SIGNATURES = {
     "dmo_cmaes_step_z": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_i64, _c_int, _vp]),
     "dmo_scale_rows": (_c_int, [_vp, _vp, _c_i64, _c_i64, _vp, _vp, _vp, _c_i64]),
     "dmo_benchmark_eval": (_c_int, [_vp, _c_int, _vp, _c_i64, _c_int, _c_int, _c_dbl, _vp]),
+    "dmo_sa_dgsm_design": (_c_int, [_vp, _vp, _c_i64, _c_int, _vp, _vp, _c_dbl, _vp]),
+    "dmo_sa_fast_design": (_c_int, [_vp, _c_i64, _c_int, _vp, _vp, _vp, _vp, _vp]),
+    "dmo_sa_dgsm_stats": (_c_int, [_vp, _vp, _vp, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _c_int, _c_dbl, _vp, _vp, _vp, _vp]),
     "dmo_smpso_generate": (_c_int, [_vp, _vp, _vp, _c_int, _c_i64, _c_int, _vp, _vp, _vp, _c_dbl, _c_u64, _c_u64, _vp, _vp]),
     "dmo_smpso_update": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_int, _vp, _c_int, _c_i64, _c_int, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
 }
@@ -1539,3 +1542,83 @@ def cmaes_update_cholesky(A, Ainv, pc, z, psucc, cc, ccov, pthresh):
     _check(load_library().dmo_cmaes_update_cholesky(context(), _ptr(A), _ptr(Ainv), _ptr(pc), _ptr(z), _ptr(ps), n, d, float(cc), float(ccov), float(pthresh)),
            "dmo_cmaes_update_cholesky")
     return A, Ainv, pc
+
+
+# --------------------------------------------------------------------------- sensitivity analysis (SA_DGSM / SA_FAST)
+def _design_out(shape, write, mirror):
+    """(rows, d) design written by ``write(pointer)``: with ``mirror`` a read-only page-locked array whose device copy the
+    library keeps (a surrogate predict of it uploads nothing), else an ordinary NumPy array."""
+    if not mirror:
+        out = np.empty(shape, dtype=np.float64)
+        write(out.ctypes.data)
+        return out
+    dev = DeviceArray(shape, np.float64)
+    write(dev.ptr)
+    if _pin_live_bytes < _PIN_LIVE_LIMIT:
+        out = pinned_empty(shape, np.float64)
+    else:  # page-locked budget spent: pageable memory (mirror dropped with the array)
+        import weakref
+
+        out = np.empty(shape, dtype=np.float64)
+        weakref.finalize(out, _mirrors.pop, out.ctypes.data, None)
+    memcpy(out, dev.ptr, out.nbytes)
+    mirror_register(out, dev)
+    out.flags.writeable = False
+    return out
+
+
+def _bounds(xlb, xub, d):
+    lb, ub = _f64(xlb).reshape(-1), _f64(xub).reshape(-1)
+    if lb.shape != (d,) or ub.shape != (d,):
+        raise ValueError(f"bounds must have {d} entries (got {lb.shape[0]} and {ub.shape[0]})")
+    return lb, ub
+
+
+def sa_dgsm_design(base, xlb, xub, delta=0.01, mirror=True):
+    """(N (d+1), d) DGSM design from the base points ``base`` (N, d) in the unit cube (dmo_sa_dgsm_design): row i (d+1)
+    is base_i, row i (d+1) + 1 + j is base_i + delta e_j, every row scaled to u (xub - xlb) + xlb."""
+    B = _f64(base)
+    if B.ndim != 2 or B.shape[0] < 1 or B.shape[1] < 1:
+        raise ValueError(f"base must be a non-empty (N, d) array (got shape {B.shape})")
+    N, d = B.shape
+    lb, ub = _bounds(xlb, xub, d)
+    write = lambda p: _check(load_library().dmo_sa_dgsm_design(context(), _ptr(B), N, d, _ptr(lb), _ptr(ub), float(delta), p), "dmo_sa_dgsm_design")
+    return _design_out((N * (d + 1), d), write, mirror)
+
+
+def sa_fast_design(N, omega, phi, xlb, xub, mirror=True):
+    """(N d, d) eFAST design (dmo_sa_fast_design) for the frequencies ``omega`` (d,) and per-block phases ``phi`` (d,)."""
+    w, ph = _f64(omega).reshape(-1), _f64(phi).reshape(-1)
+    d, N = w.shape[0], int(N)
+    if ph.shape != (d,):
+        raise ValueError(f"phi must have {d} entries (got {ph.shape[0]})")
+    lb, ub = _bounds(xlb, xub, d)
+    write = lambda p: _check(load_library().dmo_sa_fast_design(context(), N, d, _ptr(w), _ptr(ph), _ptr(lb), _ptr(ub), p), "dmo_sa_fast_design")
+    return _design_out((N * d, d), write, mirror)
+
+
+def sa_dgsm_stats(X, Y, xlb, xub, boot_idx, conf_level=0.95):
+    """{vi, vi_std, dgsm, conf}, each (M, d), of a DGSM design X (N (d+1), d) and its outputs Y (N (d+1), M)
+    (dmo_sa_dgsm_stats).  X and Y may be host arrays (a mirrored design is read from its device copy) or device arrays
+    (``data_ptr()``); boot_idx (R, N) are the base indices of the R bootstrap replicates."""
+    from statistics import NormalDist
+
+    xs, ys = tuple(X.shape), tuple(Y.shape)
+    X = _f64(X) if isinstance(X, np.ndarray) else X
+    Y = _f64(Y) if isinstance(Y, np.ndarray) else Y
+    if len(xs) != 2 or xs[1] < 1 or xs[0] % (xs[1] + 1) != 0:
+        raise ValueError(f"X must be a DGSM design of N (d+1) rows and d columns (got shape {xs})")
+    d = xs[1]
+    N = xs[0] // (d + 1)
+    M = 1 if len(ys) == 1 else ys[1]
+    if ys[0] != xs[0] or len(ys) > 2:
+        raise ValueError(f"Y must have the design's {xs[0]} rows (got shape {ys})")
+    idx = np.ascontiguousarray(boot_idx, dtype=np.int32)
+    if idx.ndim != 2 or idx.shape[1] != N:
+        raise ValueError(f"boot_idx must be (R, N={N}) (got shape {idx.shape})")
+    lb, ub = _bounds(xlb, xub, d)
+    z = NormalDist().inv_cdf(0.5 + conf_level / 2)
+    out = {k: np.empty((M, d), dtype=np.float64) for k in ("vi", "vi_std", "dgsm", "conf")}
+    _check(load_library().dmo_sa_dgsm_stats(context(), _in(X), _in(Y), N, d, M, _ptr(lb), _ptr(ub), _ptr(idx), idx.shape[0], float(z),
+                                            _ptr(out["vi"]), _ptr(out["vi_std"]), _ptr(out["dgsm"]), _ptr(out["conf"])), "dmo_sa_dgsm_stats")
+    return out

@@ -559,6 +559,29 @@ int dmo_gather_rows(dmo_ctx* ctx, const double* src, const double* alt, const ui
 int dmo_benchmark_eval(dmo_ctx* ctx, int problem, const double* X, int64_t n, int n_var, int n_obj, double alpha,
                        double* Y);
 
+/* ---- Sensitivity analysis: SA_DGSM / SA_FAST -------------------------------------------------
+ * replaces SALib's finite_diff / fast_sampler samplers and dgsm.analyze behind dmosopt/sa.py:11-80 (SALib 1.5's
+ * definitions, restated in oracle/sa.py).
+ * dmo_sa_dgsm_design: base (N, d) points in the unit cube -> X (N (d+1), d): row i (d+1) is base_i, row i (d+1) + 1 + j
+ *   is base_i + delta e_j, every row scaled to u (xub - xlb) + xlb with one rounding per operation in that order (no
+ *   fused multiply-add), so X is bit-identical to the NumPy expression.
+ * dmo_sa_fast_design: X (N d, d) of eFAST (interference factor 4): block i gives parameter i the frequency omega[0] and
+ *   the others omega[1..d-1] in order; X[i N + k, j] = (0.5 + arcsin(sin(w_j s_k + phi[i])) / pi) (xub - xlb) + xlb with
+ *   s_k = (2 pi / N) k.  arcsin(sin(.)) is evaluated as the triangle wave after an exact reduction modulo pi/2, which
+ *   keeps it accurate next to the peaks.  64 < N <= 2^20; reads no input rows.
+ * dmo_sa_dgsm_stats: X (N (d+1), d) the DGSM design, Y (N (d+1), M) its outputs, boot_idx (R, N) int32 base indices in
+ *   [0, N) of R bootstrap replicates (R <= 4096), z the normal quantile of the confidence level -> vi, vi_std, dgsm,
+ *   conf, each (M, d): with q_i = (Y[pert_ij, m] - Y[base_i, m]) / (X[pert_ij, j] - X[base_i, j]), vi = mean(q^2),
+ *   vi_std = std(q^2), dgsm = vi (xub_j - xlb_j)^2 / (pi^2 var(Y[base, m])), conf = z std_ddof1(dgsm over the
+ *   replicates).  One CTA per (m, j); sums in a fixed order, so the results do not depend on the launch. */
+int dmo_sa_dgsm_design(dmo_ctx* ctx, const double* base, int64_t N, int d, const double* xlb, const double* xub,
+                       double delta, double* X);
+int dmo_sa_fast_design(dmo_ctx* ctx, int64_t N, int d, const double* omega, const double* phi, const double* xlb,
+                       const double* xub, double* X);
+int dmo_sa_dgsm_stats(dmo_ctx* ctx, const double* X, const double* Y, int64_t N, int d, int M, const double* xlb,
+                      const double* xub, const int32_t* boot_idx, int R, double z, double* vi, double* vi_std,
+                      double* dgsm, double* conf);
+
 #ifdef __cplusplus
 }
 #endif
