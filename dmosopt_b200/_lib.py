@@ -125,6 +125,9 @@ _SIGNATURES = {
     "dmo_sa_dgsm_design": (_c_int, [_vp, _vp, _c_i64, _c_int, _vp, _vp, _c_dbl, _vp]),
     "dmo_sa_fast_design": (_c_int, [_vp, _c_i64, _c_int, _vp, _vp, _vp, _vp, _vp]),
     "dmo_sa_dgsm_stats": (_c_int, [_vp, _vp, _vp, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _c_int, _c_dbl, _vp, _vp, _vp, _vp]),
+    "dmo_l2_discrepancy_terms": (_c_int, [_vp, _c_int, _vp, _c_i64, _c_int, _vp, _vp]),
+    "dmo_glp_cd2_terms": (_c_int, [_vp, _vp, _c_i64, _c_int, _c_i64, _c_i64, _vp, _vp]),
+    "dmo_glp_cd2_pairs": (_c_int, [_vp, _vp, _c_i64, _c_int, _c_i64, _c_i64, _vp]),
     "dmo_smpso_generate": (_c_int, [_vp, _vp, _vp, _c_int, _c_i64, _c_int, _vp, _vp, _vp, _c_dbl, _c_u64, _c_u64, _vp, _vp]),
     "dmo_smpso_update": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_int, _vp, _c_int, _c_i64, _c_int, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
 }
@@ -1622,3 +1625,52 @@ def sa_dgsm_stats(X, Y, xlb, xub, boot_idx, conf_level=0.95):
     _check(load_library().dmo_sa_dgsm_stats(context(), _in(X), _in(Y), N, d, M, _ptr(lb), _ptr(ub), _ptr(idx), idx.shape[0], float(z),
                                             _ptr(out["vi"]), _ptr(out["vi_std"]), _ptr(out["dgsm"]), _ptr(out["conf"])), "dmo_sa_dgsm_stats")
     return out
+
+
+# --------------------------------------------------------------------------- uniform designs (discrepancy / GLP search)
+L2_METRICS = {"MD2": 0, "CD2": 1, "SD2": 2, "WD2": 3}  # DMO_L2_*
+GLP_MAX_CANDIDATES = 65535  # lattices per dmo_glp_cd2_terms / _pairs call (csrc/design.cu, one grid row each)
+GLP_MAX_LATTICE = 2**31 - 1  # (k + 1) h stays below 2^62 in int64
+
+
+def l2_discrepancy_terms(X, metric):
+    """(D2, D3) of the design X (n, s) for ``metric`` in MD2 / CD2 / SD2 / WD2 (dmo_l2_discrepancy_terms)."""
+    A = _f64(X)
+    if A.ndim != 2 or A.shape[0] < 1 or A.shape[1] < 1:
+        raise ValueError(f"X must be a non-empty (n, s) array (got shape {A.shape})")
+    d2, d3 = np.empty(1), np.empty(1)
+    _check(load_library().dmo_l2_discrepancy_terms(context(), L2_METRICS[metric], _ptr(A), A.shape[0], A.shape[1], _ptr(d2), _ptr(d3)),
+           "dmo_l2_discrepancy_terms")
+    return float(d2[0]), float(d3[0])
+
+
+def _multipliers(H, lattice, rows):
+    H = np.ascontiguousarray(H, dtype=np.int64)
+    if H.ndim != 2 or H.shape[1] < 1:
+        raise ValueError(f"H must be a (C, s) array of multipliers (got shape {H.shape})")
+    if not 2 <= lattice <= GLP_MAX_LATTICE or not 1 <= rows <= lattice:
+        raise ValueError(f"lattice {lattice} outside [2, 2^31 - 1] or rows {rows} outside [1, lattice]")
+    return H
+
+
+def glp_cd2_terms(H, lattice, rows):
+    """CD2's (D2, D3), each (C,), of the rank-1 lattices with multipliers H (C, s) (dmo_glp_cd2_terms), in chunks of
+    GLP_MAX_CANDIDATES."""
+    H = _multipliers(H, lattice, rows)
+    C, s = H.shape
+    d2, d3 = np.empty(C), np.empty(C)
+    for c0 in range(0, C, GLP_MAX_CANDIDATES):
+        h = np.ascontiguousarray(H[c0 : c0 + GLP_MAX_CANDIDATES])
+        _check(load_library().dmo_glp_cd2_terms(context(), _ptr(h), h.shape[0], s, int(lattice), int(rows), _ptr(d2[c0:]), _ptr(d3[c0:])),
+               "dmo_glp_cd2_terms")
+    return d2, d3
+
+
+def glp_cd2_pairs(H, lattice, rows):
+    """(L, rows^2) CD2 pair products of the lattices H (L, s) in the reference's operation order (dmo_glp_cd2_pairs)."""
+    H = _multipliers(H, lattice, rows)
+    if H.shape[0] > GLP_MAX_CANDIDATES:
+        raise ValueError(f"at most {GLP_MAX_CANDIDATES} lattices per call (got {H.shape[0]})")
+    P = np.empty((H.shape[0], rows * rows))
+    _check(load_library().dmo_glp_cd2_pairs(context(), _ptr(H), H.shape[0], H.shape[1], int(lattice), int(rows), _ptr(P)), "dmo_glp_cd2_pairs")
+    return P

@@ -582,6 +582,30 @@ int dmo_sa_dgsm_stats(dmo_ctx* ctx, const double* X, const double* Y, int64_t N,
                       const double* xub, const int32_t* boot_idx, int R, double z, double* vi, double* vi_std,
                       double* dgsm, double* conf);
 
+/* ---- Uniform designs: L2 discrepancies and the good-lattice-point search ----------------------
+ * replaces the sums of dmosopt/discrepancy.py:38-129 and the candidate scoring of dmosopt/GLP.py:31-70.  A discrepancy
+ * is D^2 = D1 + c2 D2 + c3 D3 with D2 = sum_k prod_i row(x_ki) and D3 = sum_{k,j} prod_i pair(x_ki, x_ji); these entry
+ * points return D2 and D3 in float64, summed in a fixed order that differs from the reference's (results repeat bit
+ * for bit from call to call).
+ * dmo_l2_discrepancy_terms: X (n, s), metric DMO_L2_MD2 / CD2 / SD2 / WD2 -> d2[1], d3[1] (WD2 has no D2 sum: d2 = n).
+ *   n <= 46340 * 64.
+ * dmo_glp_cd2_terms: H (C, s) int64 multipliers in [0, lattice) -> CD2's d2[C], d3[C] of the C rank-1 lattices
+ *   x_ki = (u - 0.5) / rows, u = ((k + 1) H[c, i] mod lattice) with 0 replaced by lattice, k < rows.  The designs are
+ *   generated inside the kernel.  1 <= C <= 65535 (one grid row each), 2 <= lattice <= 2^31 - 1 (int64 products
+ *   (k + 1) h), 1 <= rows <= lattice.
+ * dmo_glp_cd2_pairs: the same lattices (L of them, same limits) -> P (L, rows^2): P[l, k rows + j] is the reference's
+ *   CD2 pair product for rows (k, j), ((1 + 0.5 |x_ki - 0.5|) + 0.5 |x_ji - 0.5|) - 0.5 |x_ki - x_ji| multiplied over
+ *   i = 0 .. s-1 from 1.0, each operation rounded on its own; summed sequentially in row-major order it is the
+ *   reference's D3 bit for bit. */
+#define DMO_L2_MD2 0
+#define DMO_L2_CD2 1
+#define DMO_L2_SD2 2
+#define DMO_L2_WD2 3
+int dmo_l2_discrepancy_terms(dmo_ctx* ctx, int metric, const double* X, int64_t n, int s, double* d2, double* d3);
+int dmo_glp_cd2_terms(dmo_ctx* ctx, const int64_t* H, int64_t C, int s, int64_t lattice, int64_t rows, double* d2,
+                      double* d3);
+int dmo_glp_cd2_pairs(dmo_ctx* ctx, const int64_t* H, int64_t L, int s, int64_t lattice, int64_t rows, double* P);
+
 #ifdef __cplusplus
 }
 #endif
