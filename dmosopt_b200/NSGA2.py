@@ -6,7 +6,8 @@ fields and ``generate / update`` contract, selected in dmosopt by
 
 Per generation (MOASMO.optimize, dmosopt/MOASMO.py:105-116):
   generate_strategy : dmo_tournament -> dmo_nsga2_generate   (NSGA2.py:116-185)
-  update_strategy   : dmo_remove_worst on vstack(children, parents)  (NSGA2.py:187-236)
+  update_strategy   : dmo_remove_worst on vstack(children, parents)  (NSGA2.py:187-236); with this package's
+                      feasibility model as the x-metric, dmo_remove_worst_pair_keys evaluates its rank on the device
 The state lives in NumPy arrays exactly as in the reference (so dmosopt's HDF5 save / restart keeps
 working); survivors are written back in place, which rounds the objectives to the state dtype
 (float32 inside MOASMO.optimize) just as NSGA2.py:228-230 does.
@@ -32,6 +33,19 @@ def population_diversity(rank, Y):
     else:
         cd_spread = 0
     return diversity, cd_spread
+
+
+def _device_feasibility_key(x_distance_metrics):
+    """The device model behind x_distance_metrics == [m.rank] for a GPU LogisticFeasibilityModel m, else None."""
+    from .feasibility import LogisticFeasibilityModel
+
+    if x_distance_metrics is None or len(x_distance_metrics) != 1:
+        return None
+    m = x_distance_metrics[0]
+    owner = getattr(m, "__self__", None)
+    if not isinstance(owner, LogisticFeasibilityModel) or getattr(m, "__func__", None) is not LogisticFeasibilityModel.rank:
+        return None
+    return owner.device_model
 
 
 class NSGA2(MOEA):
@@ -125,8 +139,10 @@ class NSGA2(MOEA):
         """NSGA2.py:187-236."""
         st = self.state
         popsize = self.opt_params.popsize
-        builtin = self.x_distance_metrics is None and (self.y_distance_metrics is None or self.y_distance_metrics[0] in ("crowding", "euclidean"))
-        if builtin and not self.opt_params.adaptive_population_size:
+        builtin_y = self.y_distance_metrics is None or self.y_distance_metrics[0] in ("crowding", "euclidean")
+        builtin = self.x_distance_metrics is None and builtin_y
+        key = _device_feasibility_key(self.x_distance_metrics) if builtin_y else None
+        if (builtin or key is not None) and not self.opt_params.adaptive_population_size:
             # children stacked over parents (NSGA2.py:205-206) on the device; survivors land directly in the state array
             code = {None: _lib.METRIC_NONE, "crowding": _lib.METRIC_CROWDING, "euclidean": _lib.METRIC_EUCLIDEAN}[
                 None if self.y_distance_metrics is None else self.y_distance_metrics[0]]
@@ -136,8 +152,12 @@ class NSGA2(MOEA):
             out_x = base
             if out_x is None and st.population_parm.flags.writeable and st.population_parm.dtype == np.float64 and st.population_parm.shape[0] == popsize:
                 out_x = st.population_parm
-            population_parm, population_obj, rank, perm = _lib.remove_worst_pair(
-                x_gen, y_gen, st.population_parm, st.population_obj, popsize, code, out_X=out_x)
+            if key is not None:  # the feasibility rank of [x_gen; parents] is evaluated where the rows already are
+                population_parm, population_obj, rank, perm = _lib.remove_worst_pair_keys(
+                    x_gen, y_gen, st.population_parm, st.population_obj, popsize, key, code, out_X=out_x)
+            else:
+                population_parm, population_obj, rank, perm = _lib.remove_worst_pair(
+                    x_gen, y_gen, st.population_parm, st.population_obj, popsize, code, out_X=out_x)
             if population_parm is base:
                 population_parm = st.population_parm  # survivors are already in the (mirrored) state array
         else:

@@ -6,6 +6,7 @@ Plugin import paths (dmosopt resolves them with ``config.import_object_by_path``
     surrogate_method_name  = "dmosopt_b200.GPR_Matern" | "dmosopt_b200.GPR_RBF"
                              | "dmosopt_b200.SVGP_Matern" | "dmosopt_b200.VGP_Matern" | "dmosopt_b200.SIV_Matern"
                              | "dmosopt_b200.SPV_Matern" | "dmosopt_b200.CRV_Matern"
+    surrogate_custom_training = "dmosopt_b200.feasibility.train_with_feasibility"   (a GPU logistic feasibility model)
 
 ``dmosopt_b200.install()`` additionally routes the controller-side helpers that dmosopt calls on its own modules
 (resample / get_best duplicates + sort, per-generation termination hypervolume) to the same kernels.
@@ -25,6 +26,7 @@ from .AGEMOEA import AGEMOEA  # noqa: F401
 from .CMAES import CMAES  # noqa: F401
 from .SMPSO import SMPSO  # noqa: F401
 from .TRS import TRS  # noqa: F401
+from .feasibility import LogisticFeasibilityModel, train_with_feasibility  # noqa: F401
 
 
 def install(package="dmosopt"):

@@ -58,6 +58,7 @@ _SIGNATURES = {
     "dmo_order_mo": (_c_int, [_vp, _vp, _c_i64, _c_int, _c_int, _vp, _c_int, _vp, _vp, _vp]),
     "dmo_remove_worst": (_c_int, [_vp, _vp, _vp, _c_i64, _c_int, _c_int, _c_int, _vp, _c_int, _c_i64, _vp, _vp, _vp, _vp]),
     "dmo_remove_worst_pair": (_c_int, [_vp, _vp, _vp, _c_i64, _vp, _vp, _c_i64, _c_int, _c_int, _c_int, _c_i64, _vp, _vp, _vp, _vp]),
+    "dmo_remove_worst_pair_keys": (_c_int, [_vp, _vp, _vp, _c_i64, _vp, _vp, _c_i64, _c_int, _c_int, _c_int, _vp, _c_i64, _vp, _vp, _vp, _vp]),
     "dmo_tournament": (_c_int, [_vp, _vp, _vp, _c_i64, _c_i64, _c_u64, _c_u64, _vp, _vp]),
     "dmo_mutation_u": (_c_int, [_vp, _vp, _vp, _c_i64, _c_int, _vp, _vp, _vp, _c_dbl, _vp]),
     "dmo_sbx_u": (_c_int, [_vp, _vp, _vp, _vp, _c_i64, _c_int, _vp, _vp, _vp, _vp, _vp]),
@@ -128,6 +129,11 @@ _SIGNATURES = {
     "dmo_l2_discrepancy_terms": (_c_int, [_vp, _c_int, _vp, _c_i64, _c_int, _vp, _vp]),
     "dmo_glp_cd2_terms": (_c_int, [_vp, _vp, _c_i64, _c_int, _c_i64, _c_i64, _vp, _vp]),
     "dmo_glp_cd2_pairs": (_c_int, [_vp, _vp, _c_i64, _c_int, _c_i64, _c_i64, _vp]),
+    "dmo_feas_fit": (_c_int, [_vp, _vp, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _vp, _c_int, _vp, _c_int, _c_dbl, _vp, _vp, _vp, _vp, _vp, _vp,
+                              _vp, _vp]),
+    "dmo_feas_create": (_c_int, [_vp, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.POINTER(_vp)]),
+    "dmo_feas_destroy": (_c_int, [_vp, _vp]),
+    "dmo_feas_eval": (_c_int, [_vp, _vp, _vp, _c_i64, _c_int, _vp, _vp, _vp]),
     "dmo_smpso_generate": (_c_int, [_vp, _vp, _vp, _c_int, _c_i64, _c_int, _vp, _vp, _vp, _c_dbl, _c_u64, _c_u64, _vp, _vp]),
     "dmo_smpso_update": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_int, _vp, _c_int, _c_i64, _c_int, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
 }
@@ -593,6 +599,31 @@ def remove_worst_pair(Xa, Ya, Xb, Yb, keep, metric=METRIC_NONE, out_X=None):
         load_library().dmo_remove_worst_pair(context(), _in(Xa), _in(Ya), na, _in(Xb), _in(Yb), nb, d, M, metric, keep,
                                              xo_dev if xo_dev is not None else _ptr(Xo), _ptr(Yo), _ptr(rank), _ptr(perm)),
         "dmo_remove_worst_pair",
+    )
+    if xo_dev is not None:
+        memcpy(Xo, xo_dev, Xo.nbytes)
+    return Xo, Yo, rank.astype(np.intp), perm
+
+
+def remove_worst_pair_keys(Xa, Ya, Xb, Yb, keep, key, metric=METRIC_NONE, out_X=None):
+    """remove_worst_pair with the rank of the feasibility model ``key`` (FeasModel) over [Xa; Xb] evaluated on the device
+    as the least significant descending key (MOEA.remove_worst with x_distance_metrics=[key.rank])."""
+    Xa, Ya, Xb, Yb = _f64(Xa), _f64(Ya), _f64(Xb), _f64(Yb)
+    na, d = Xa.shape
+    nb = Xb.shape[0]
+    M = Ya.shape[1]
+    keep = int(min(keep, na + nb))
+    if out_X is not None and (out_X.dtype != np.float64 or not out_X.flags.c_contiguous or out_X.shape != (keep, d)):
+        out_X = None
+    Xo = out_X if out_X is not None else pinned_empty((keep, d), np.float64)
+    Yo = np.empty((keep, M), dtype=np.float64)
+    rank = np.empty(keep, dtype=np.int32)
+    perm = np.empty(keep, dtype=np.int64)
+    xo_dev = mirror_ptr(Xo, require_readonly=False) if out_X is not None else None
+    _check(
+        load_library().dmo_remove_worst_pair_keys(context(), _in(Xa), _in(Ya), na, _in(Xb), _in(Yb), nb, d, M, metric, key.handle, keep,
+                                                  xo_dev if xo_dev is not None else _ptr(Xo), _ptr(Yo), _ptr(rank), _ptr(perm)),
+        "dmo_remove_worst_pair_keys",
     )
     if xo_dev is not None:
         memcpy(Xo, xo_dev, Xo.nbytes)
@@ -1674,3 +1705,81 @@ def glp_cd2_pairs(H, lattice, rows):
     P = np.empty((H.shape[0], rows * rows))
     _check(load_library().dmo_glp_cd2_pairs(context(), _ptr(H), H.shape[0], H.shape[1], int(lattice), int(rows), _ptr(P)), "dmo_glp_cd2_pairs")
     return P
+
+
+# --------------------------------------------------------------------------- logistic feasibility model
+FEAS_MAX_D = 90  # input dimensions of dmo_feas_fit / dmo_feas_create (csrc/feasibility.cu FEAS_MAX_D)
+FEAS_MAX_J = 32  # constraints
+FEAS_MAX_N = 65536  # training rows of dmo_feas_fit
+
+
+def feas_fit(X, labels, folds, pca_mean, pca_comps, Cs, max_iter=100, tol=1e-11):
+    """dmo_feas_fit: every (dataset, C, k) L1-logistic problem of J two-class constraints in one batch.
+
+    X (N, d); labels (J, N) 0/1; folds (J, N) test-fold ids; pca_mean (6 J, d), pca_comps (6 J, d-1, d).  Returns a dict
+    with scaler_mean / scaler_scale (6 J, d-1) and, per problem p = (s nC + c)(d-1) + k-1, coef (P, d), iters,
+    objective, kkt, converged, correct."""
+    X = _f64(X)
+    N, d = X.shape
+    labels = np.ascontiguousarray(labels, dtype=np.uint8)
+    folds = np.ascontiguousarray(folds, dtype=np.int8)
+    J = labels.shape[0]
+    pca_mean, pca_comps, Cs = _f64(pca_mean), _f64(pca_comps), _f64(Cs)
+    assert labels.shape == (J, N) and folds.shape == (J, N), "feas_fit: labels / folds must be (J, N)"
+    assert pca_mean.shape == (6 * J, d) and pca_comps.shape == (6 * J, d - 1, d), "feas_fit: bad PCA shapes"
+    nC = Cs.size
+    P = 6 * J * nC * (d - 1)
+    out = {
+        "scaler_mean": np.empty((6 * J, d - 1)), "scaler_scale": np.empty((6 * J, d - 1)), "coef": np.empty((P, d)),
+        "iters": np.empty(P, dtype=np.int32), "objective": np.empty(P), "kkt": np.empty(P),
+        "converged": np.empty(P, dtype=np.int8), "correct": np.empty(P, dtype=np.int64),
+    }
+    _check(
+        load_library().dmo_feas_fit(context(), _ptr(X), N, d, J, _ptr(labels), _ptr(folds), _ptr(pca_mean), _ptr(pca_comps), nC, _ptr(Cs),
+                                    int(max_iter), float(tol), *[_ptr(out[k]) for k in ("scaler_mean", "scaler_scale", "coef", "iters",
+                                                                                          "objective", "kkt", "converged", "correct")]),
+        "dmo_feas_fit",
+    )
+    return out
+
+
+class FeasModel:
+    """A fitted feasibility model held on the device (dmo_feas): J constraints over d inputs."""
+
+    def __init__(self, k, mean, comps, smean, sscale, coef, intercept):
+        k = np.ascontiguousarray(k, dtype=np.int32)
+        mean = _f64(mean)
+        J, d = mean.shape
+        arrs = [_f64(a) for a in (comps, smean, sscale, coef, intercept)]
+        assert k.shape == (J,) and arrs[0].shape == (J, d - 1, d) and arrs[4].shape == (J,)
+        assert all(a.shape == (J, d - 1) for a in arrs[1:4])
+        self.d, self.J = d, J
+        h = _vp()
+        self.handle = None
+        _check(load_library().dmo_feas_create(context(), d, J, _ptr(k), _ptr(mean), *[_ptr(a) for a in arrs], ctypes.byref(h)),
+               "dmo_feas_create")
+        self.handle = h.value
+
+    def eval(self, X, rank=True, proba=False, decision=False):
+        """(rank (n,), proba (J, n), decision (J, n)); the ones not asked for are None.  X may be a host array (its device
+        mirror is read when it has one) or a device tensor."""
+        if isinstance(X, np.ndarray) or not hasattr(X, "data_ptr"):
+            X = np.ascontiguousarray(X, dtype=np.float64)
+            n = X.shape[0]
+            if X.ndim != 2 or X.shape[1] != self.d:
+                raise ValueError(f"feasibility model: x must be (n, {self.d}), got {X.shape}")
+        else:
+            n = int(X.shape[0])
+        r = np.empty(n) if rank else None
+        p = np.empty((self.J, n)) if proba else None
+        t = np.empty((self.J, n)) if decision else None
+        _check(load_library().dmo_feas_eval(context(), self.handle, _in(X), n, self.d, _ptr(r), _ptr(p), _ptr(t)), "dmo_feas_eval")
+        return r, p, t
+
+    def __del__(self):
+        try:
+            if self.handle and _lib is not None and _ctx is not None:
+                _lib.dmo_feas_destroy(_ctx, self.handle)
+        except Exception:
+            pass
+        self.handle = None

@@ -253,3 +253,6 @@ int hypervolume_device(dmo_ctx* ctx, const double* dF, int64_t n, int M, const d
 // the same when the rows carry their non-dominated ranks within a superset (rank > 0 rows are skipped, no filter pass)
 int hypervolume_device_ranked(dmo_ctx* ctx, const double* dF, int64_t n, int M, const double* h_ref, const int32_t* d_rank,
                               double* h_out);
+// the feasibility model's rank (csrc/feasibility.cu) of n device rows into d_rank, enqueued on the context's stream
+int feas_rank_device(dmo_ctx* ctx, const dmo_feas* m, const double* dX, int64_t n, double* d_rank);
+int feas_model_dim(const dmo_feas* m);

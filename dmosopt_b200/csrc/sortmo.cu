@@ -541,9 +541,10 @@ int dmo_remove_worst(dmo_ctx* ctx, const double* X, const double* Y, int64_t n, 
 
 // dmo_remove_worst on the row-wise concatenation [A; B] without materialising it on the host: the two blocks are
 // staged into adjacent regions of one device buffer (NSGA2.update_strategy stacks children over parents, NSGA2.py:205-206)
-int dmo_remove_worst_pair(dmo_ctx* ctx, const double* Xa, const double* Ya, int64_t na, const double* Xb, const double* Yb,
-                          int64_t nb, int d, int M, int metric, int64_t keep, double* X_out, double* Y_out,
-                          int32_t* rank_out, int64_t* perm_out) {
+// key (optional): a feasibility model evaluated on the staged rows, the least significant descending key
+static int remove_worst_pair_impl(dmo_ctx* ctx, const double* Xa, const double* Ya, int64_t na, const double* Xb,
+                                  const double* Yb, int64_t nb, int d, int M, int metric, const dmo_feas* key, int64_t keep,
+                                  double* X_out, double* Y_out, int32_t* rank_out, int64_t* perm_out) {
   if (!ctx) return DMO_ERR_ARG;
   DMO_CUDA(cudaSetDevice(ctx->device));
   const int64_t n = na + nb;
@@ -564,10 +565,17 @@ int dmo_remove_worst_pair(dmo_ctx* ctx, const double* Xa, const double* Ya, int6
   DMO_TRY(stage(x.p + (size_t)na * d, Xb, (size_t)nb * d));
   DMO_TRY(stage(y.p, Ya, (size_t)na * M));
   DMO_TRY(stage(y.p + (size_t)na * M, Yb, (size_t)nb * M));
+  DevBuf<double> kx;
+  const double* kp[1] = {nullptr};
+  if (key) {
+    DMO_TRY(kx.alloc(ctx, (size_t)n));
+    DMO_TRY(feas_rank_device(ctx, key, x.p, n, kx.p));
+    kp[0] = kx.p;
+  }
   DevBuf<int32_t> rank;
   DevBuf<double> dist;
   DevBuf<uint32_t> p;
-  DMO_TRY(order_mo_device(ctx, y.p, n, M, metric, nullptr, 0, rank, dist, p, keep));
+  DMO_TRY(order_mo_device(ctx, y.p, n, M, metric, key ? kp : nullptr, key ? 1 : 0, rank, dist, p, keep));
   Out<double> ox, oy;
   Out<int32_t> orank;
   Out<int64_t> op;
@@ -586,6 +594,21 @@ int dmo_remove_worst_pair(dmo_ctx* ctx, const double* Xa, const double* Ya, int6
   DMO_TRY(op.finish(ctx));
   DMO_CUDA(cudaStreamSynchronize(ctx->stream));
   return DMO_OK;
+}
+
+int dmo_remove_worst_pair(dmo_ctx* ctx, const double* Xa, const double* Ya, int64_t na, const double* Xb, const double* Yb,
+                          int64_t nb, int d, int M, int metric, int64_t keep, double* X_out, double* Y_out,
+                          int32_t* rank_out, int64_t* perm_out) {
+  return remove_worst_pair_impl(ctx, Xa, Ya, na, Xb, Yb, nb, d, M, metric, nullptr, keep, X_out, Y_out, rank_out, perm_out);
+}
+
+int dmo_remove_worst_pair_keys(dmo_ctx* ctx, const double* Xa, const double* Ya, int64_t na, const double* Xb,
+                               const double* Yb, int64_t nb, int d, int M, int metric, const dmo_feas* key, int64_t keep,
+                               double* X_out, double* Y_out, int32_t* rank_out, int64_t* perm_out) {
+  if (!ctx) return DMO_ERR_ARG;
+  DMO_REQUIRE(key, "remove_worst_pair_keys: no key model");
+  DMO_REQUIRE(feas_model_dim(key) == d, "remove_worst_pair_keys: the key model takes %d columns, X has %d", feas_model_dim(key), d);
+  return remove_worst_pair_impl(ctx, Xa, Ya, na, Xb, Yb, nb, d, M, metric, key, keep, X_out, Y_out, rank_out, perm_out);
 }
 
 int dmo_get_duplicates(dmo_ctx* ctx, const double* X, int64_t n, int d, double eps, uint8_t* is_dup) {

@@ -60,6 +60,7 @@ typedef struct dmo_ctx dmo_ctx;
 typedef struct dmo_gp dmo_gp;
 typedef struct dmo_mtgp dmo_mtgp;
 typedef struct dmo_svgp dmo_svgp;
+typedef struct dmo_feas dmo_feas;
 
 /* ---- context ----------------------------------------------------------- */
 int dmo_version(void);
@@ -123,6 +124,12 @@ int dmo_remove_worst(dmo_ctx* ctx, const double* X, const double* Y, int64_t n, 
 int dmo_remove_worst_pair(dmo_ctx* ctx, const double* Xa, const double* Ya, int64_t na, const double* Xb,
                           const double* Yb, int64_t nb, int d, int M, int metric, int64_t keep,
                           double* X_out, double* Y_out, int32_t* rank_out, int64_t* perm_out);
+/* dmo_remove_worst_pair with the feasibility rank of `key` (dmo_feas_create) evaluated on the device over [Xa; Xb] as
+ * the least significant descending key: np.lexsort((-key, -ydist, rank)), MOEA.remove_worst with
+ * x_distance_metrics = [feasibility.rank] (dmosopt/NSGA2.py:54-55).  key's d must equal d. */
+int dmo_remove_worst_pair_keys(dmo_ctx* ctx, const double* Xa, const double* Ya, int64_t na, const double* Xb,
+                               const double* Yb, int64_t nb, int d, int M, int metric, const dmo_feas* key,
+                               int64_t keep, double* X_out, double* Y_out, int32_t* rank_out, int64_t* perm_out);
 
 /* ---- A6: tournament selection ---------------------------------------------
  * replaces MOEA.tournament_selection (dmosopt/MOEA.py:375-395): candidates ordered by
@@ -605,6 +612,34 @@ int dmo_l2_discrepancy_terms(dmo_ctx* ctx, int metric, const double* X, int64_t 
 int dmo_glp_cd2_terms(dmo_ctx* ctx, const int64_t* H, int64_t C, int s, int64_t lattice, int64_t rows, double* d2,
                       double* d3);
 int dmo_glp_cd2_pairs(dmo_ctx* ctx, const int64_t* H, int64_t L, int s, int64_t lattice, int64_t rows, double* P);
+
+/* ---- Logistic feasibility model ------------------------------------------------------------------------
+ * replaces dmosopt/feasibility.py: per constraint, GridSearchCV over PCA(k) -> StandardScaler -> L1 logistic
+ * regression, k in 1 .. d-1, C in Cs, 5 stratified folds, accuracy, refit on all rows.  2 <= d <= 90, 1 <= J <= 32.
+ * dmo_feas_fit: X (N, d), 5 <= N <= 65536; labels (J, N) 0/1 and folds (J, N) test-fold ids 0..4 of the J two-class
+ *   constraints; datasets s = 6 j + f (f < 5: the rows outside fold f, f = 5: all rows) with pca_mean (6 J, d) and
+ *   pca_comps (6 J, d-1, d) the components of each dataset's training rows in descending eigenvalue order.  The
+ *   scores are standardised with each dataset's training-row mean and population std -> scaler_mean, scaler_scale
+ *   (6 J, d-1).  Problem p = (s nC + c)(d-1) + k-1 minimises C_c sum log(1 + exp(-s_i (z_i[:k] w + b))) + |w|_1 by
+ *   proximal Newton (at most max_iter updates) until the minimum-norm subgradient is <= tol max(1, C n_train):
+ *   coef (P, d) holds w in [0, k) and b in column d-1; iters (P) Newton updates (-1: the training rows hold one class,
+ *   no fit), objective, kkt (P) at the returned w, converged (P) 0/1, correct (P) int64 held-out rows with
+ *   (t > 0) == label (-1 without a fit, 0 for f = 5).  1 <= nC <= 16.
+ * dmo_feas_create: a fitted model of J constraints from host arrays: k (J) components (0: single-class constraint,
+ *   probability 1), mean (J, d), comps (J, d-1, d), smean, sscale, coef (J, d-1), intercept (J); rows past k unused.
+ * dmo_feas_eval: X (n, d) -> rank (n) = sum_j p_j / J, proba (J, n) = p_j, decision (J, n) = t_j (+inf for a
+ *   single-class constraint), each optional; per row and constraint in this order: centre, project, standardise,
+ *   dot, + b, p = 1 / (1 + exp(-t)), all float64. */
+int dmo_feas_fit(dmo_ctx* ctx, const double* X, int64_t N, int d, int J, const uint8_t* labels, const int8_t* folds,
+                 const double* pca_mean, const double* pca_comps, int nC, const double* Cs, int max_iter, double tol,
+                 double* scaler_mean, double* scaler_scale, double* coef, int32_t* iters, double* objective, double* kkt,
+                 int8_t* converged, int64_t* correct);
+int dmo_feas_create(dmo_ctx* ctx, int d, int J, const int32_t* k, const double* mean, const double* comps,
+                    const double* smean, const double* sscale, const double* coef, const double* intercept,
+                    dmo_feas** out);
+int dmo_feas_destroy(dmo_ctx* ctx, dmo_feas* m);
+int dmo_feas_eval(dmo_ctx* ctx, const dmo_feas* m, const double* X, int64_t n, int d, double* rank, double* proba,
+                  double* decision);
 
 #ifdef __cplusplus
 }
