@@ -108,6 +108,7 @@ _SIGNATURES = {
                                 _c_int, _c_int, _c_int, _c_int, _vp, _vp, _vp]),
     "dmo_hypervolume": (_c_int, [_vp, _vp, _c_i64, _c_int, _vp, ctypes.POINTER(_c_dbl)]),
     "dmo_hypervolume_ranked": (_c_int, [_vp, _vp, _c_i64, _c_int, _vp, _vp, ctypes.POINTER(_c_dbl)]),
+    "dmo_nondominated_flags": (_c_int, [_vp, _vp, _c_i64, _c_int, _vp]),
     "dmo_hypervolume_mc": (_c_int, [_vp, _vp, _c_i64, _c_int, _vp, _c_int, _c_dbl, _c_dbl, _c_i64, _c_u64, _c_u64, ctypes.POINTER(_c_dbl),
                                     ctypes.POINTER(_c_i64), ctypes.POINTER(_c_i64), ctypes.POINTER(_c_int)]),
     "dmo_ehvi_select": (_c_int, [_vp, _vp, _c_i64, _vp, _vp, _c_i64, _c_int, _vp, _c_int, _c_i64, _vp, _vp]),
@@ -518,6 +519,15 @@ def rank_nd(Y):
     rank = np.empty(n, dtype=np.int32)
     _check(load_library().dmo_rank_nd(context(), _ptr(Y), n, M, _ptr(rank)), "dmo_rank_nd")
     return rank.astype(np.intp)
+
+
+def nondominated_flags(Y):
+    """int32 (n,) array: 0 for the rank-0 rows, 1 for the dominated ones -- the hypervolume / EHVI filter's own route."""
+    Y = _f64(Y)
+    n, M = Y.shape
+    flags = np.empty(n, dtype=np.int32)
+    _check(load_library().dmo_nondominated_flags(context(), _ptr(Y), n, M, _ptr(flags)), "dmo_nondominated_flags")
+    return flags
 
 
 # --------------------------------------------------------------------------- A3/A4

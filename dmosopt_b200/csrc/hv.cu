@@ -462,9 +462,8 @@ int compact_rows(dmo_ctx* ctx, const double* dF, int64_t n, int M, DevBuf<int32_
 
 int sort_by_column(dmo_ctx* ctx, const double* dF, int64_t n, int M, int j, DevBuf<uint32_t>& sidx);
 
-// rank-0 subset of a device point set (identical vectors are mutually non-dominating and are all kept)
-int nondominated_subset(dmo_ctx* ctx, const double* dF, int64_t n, int M, DevBuf<double>& out, int64_t* count) {
-  DevBuf<int32_t> flag;
+// flag[i] = 1 iff row i is rank 0 (identical vectors are mutually non-dominating), flag[n] = 0; flag holds n + 1 entries
+int nondominated_keep_flags(dmo_ctx* ctx, const double* dF, int64_t n, int M, DevBuf<int32_t>& flag) {
   DevBuf<uint32_t> sidx;
   DMO_TRY(flag.alloc(ctx, n + 1));
   if (n >= 1024) {
@@ -474,7 +473,6 @@ int nondominated_subset(dmo_ctx* ctx, const double* dF, int64_t n, int M, DevBuf
     DMO_TRY(rank.alloc(ctx, n));
     DMO_TRY(nondominated_flags_device(ctx, dF, n, M, rank.p));
     DMO_LAUNCH(rank0_flag_kernel, (unsigned)ceil_div(n + 1, 256), 256, 0, rank.p, n, flag.p);
-    DMO_TRY(compact_rows(ctx, dF, n, M, flag, out, count));
     return DMO_OK;
   }
   DMO_TRY(sort_by_column(ctx, dF, n, M, 0, sidx));
@@ -487,8 +485,20 @@ int nondominated_subset(dmo_ctx* ctx, const double* dF, int64_t n, int M, DevBuf
       DMO_LAUNCH(nondominated_flag_kernel<16>, (unsigned)ceil_div(n, ND_T), ND_T, (size_t)ND_T * M * sizeof(double), dF, sidx.p, n, M,
                  flag.p);
   }
+  return DMO_OK;
+}
+
+// rank-0 subset of a device point set (identical vectors are mutually non-dominating and are all kept)
+int nondominated_subset(dmo_ctx* ctx, const double* dF, int64_t n, int M, DevBuf<double>& out, int64_t* count) {
+  DevBuf<int32_t> flag;
+  DMO_TRY(nondominated_keep_flags(ctx, dF, n, M, flag));
   DMO_TRY(compact_rows(ctx, dF, n, M, flag, out, count));
   return DMO_OK;
+}
+
+__global__ void dominated_flag_kernel(const int32_t* __restrict__ keep, int64_t n, int32_t* __restrict__ out) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = keep[i] ? 0 : 1;
 }
 
 int sort_by_column(dmo_ctx* ctx, const double* dF, int64_t n, int M, int j, DevBuf<uint32_t>& sidx) {
@@ -699,6 +709,25 @@ int dmo_hypervolume(dmo_ctx* ctx, const double* F, int64_t n, int M, const doubl
   In<double> f;
   DMO_TRY(f.init(ctx, F, (size_t)n * M));
   DMO_TRY(hypervolume_device(ctx, f.d, n, M, h_ref, out));
+  return DMO_OK;
+}
+
+int dmo_nondominated_flags(dmo_ctx* ctx, const double* Y, int64_t n, int M, int32_t* flags) {
+  if (!ctx) return DMO_ERR_ARG;
+  DMO_CUDA(cudaSetDevice(ctx->device));
+  DMO_REQUIRE(n >= 0 && M >= 1 && M <= 16, "nondominated_flags: bad shape n=%lld M=%d", (long long)n, M);
+  if (n == 0) return DMO_OK;
+  DMO_REQUIRE(Y && flags, "nondominated_flags: null pointer");
+  In<double> y;
+  Out<int32_t> f;
+  DMO_TRY(y.init(ctx, Y, (size_t)n * M));
+  DMO_TRY(f.init(ctx, flags, (size_t)n));
+  DevBuf<int32_t> keep;
+  DMO_TRY(nondominated_keep_flags(ctx, y.d, n, M, keep));
+  DMO_LAUNCH(dominated_flag_kernel, (unsigned)ceil_div(n, 256), 256, 0, keep.p, n, f.d);
+  DMO_CHECK_LAUNCH();
+  DMO_TRY(f.finish(ctx));
+  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
   return DMO_OK;
 }
 

@@ -96,7 +96,7 @@ int dmo_flush_l2(dmo_ctx* ctx);
  * replaces dda.dda_ens (dmosopt/dda.py:97-152), the rank used by every sortMO.
  * Y (n, M) -> rank (n,), the canonical Pareto front index; identical vectors are
  * mutually non-dominating (dda.py:108-115).  Equal to dda_ens whenever
- * objective 0 is tie-free.  1 <= M <= 8. */
+ * objective 0 is tie-free.  1 <= M <= 16. */
 int dmo_rank_nd(dmo_ctx* ctx, const double* Y, int64_t n, int M, int32_t* rank);
 
 /* ---- A3/A4: distance metrics ---------------------------------------------
@@ -427,6 +427,10 @@ int dmo_hypervolume(dmo_ctx* ctx, const double* F, int64_t n, int M, const doubl
  * by a rank-0 row of the same set and add no volume, so the non-dominated filter pass is skipped.  rank (n,) int32. */
 int dmo_hypervolume_ranked(dmo_ctx* ctx, const double* F, int64_t n, int M, const double* ref,
                            const int32_t* rank, double* out);
+/* The non-dominated filter in front of the hypervolume and EHVI, on its own: flags (n,) int32, 0 for a rank-0 row,
+ * 1 for a dominated one (identical vectors are mutually non-dominating).  The same route as the filter: a float64 scan
+ * below 1024 rows, the integer-id scan from 1024 rows, the cell grid for M <= 3 from 8192 rows.  1 <= M <= 16. */
+int dmo_nondominated_flags(dmo_ctx* ctx, const double* Y, int64_t n, int M, int32_t* flags);
 
 /* ---- A16: Monte-Carlo hypervolume (2 <= M <= 16) -----------------------------
  * replaces the non-'box' branches of hv.AdaptiveHyperVolume.compute_hypervolume (dmosopt/hv.py:123-241) and
