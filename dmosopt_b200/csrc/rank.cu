@@ -19,14 +19,16 @@
 //      Blocks are handed out by an atomic ticket, so a block only ever waits for blocks whose CTAs are already running
 //      (no co-residency assumption, no deadlock); every wait is bounded by a watchdog that raises an error flag.
 //
-// Rank-0-only queries (the hypervolume's filter) take the cell-grid kernels `ndg_*` (M <= 3) or a plain block scan.
-// Truncations (remove_worst: only the ranks of the kept rows matter) of three-objective sets peel the fronts they need off
-// the same kind of grid instead of running the chain, when those fronts are few (`rank_by_peeling`, below).
+// Rank-0-only queries (the hypervolume's filter) take a plain block scan of the lexicographic records or, for two and three
+// objectives, one test on the cell grid `grid_*`, which needs the dense ids alone.  Truncations (remove_worst: only the
+// ranks of the kept rows matter) of three-objective sets peel the fronts they need off the same grid instead of running
+// the chain, when those fronts are few (`rank_by_peeling`, below).
 //
 // Algorithmic bytes: 8 n M read + 4 n written; pair tests <= n^2 / 2 (compare / latency bound, see DESIGN.md section 4.2).
 #include <stdlib.h>
 
 #include <cstdio>
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -812,153 +814,6 @@ __global__ void __launch_bounds__(T) nd_flag_kernel(const uint32_t* __restrict__
   flagS[i] = dominated ? 1 : 0;
 }
 
-// ------------------------------------------------------------------------------------------------ rank-0 test on a cell grid
-// For two and three objectives the records carry one or two compare words (the first objective is implied by the
-// lexicographic order).  A G x G grid over those words answers most rank-0 queries with one table lookup: a point in a
-// cell strictly below the target's cell in both words, and earlier in lexicographic order, dominates it, so the target
-// is dominated iff the minimum position over those cells (an exclusive 2-D prefix minimum of the per-cell minima) is
-// smaller than its own.  Only the points in the target's own cell row and cell column need the exact test; two
-// cell-ordered copies of the records (row-major and column-major) make both of them contiguous streams.
-// (M == 2 duplicates its single compare word, i.e. only the diagonal cells are populated.)
-// cell of a dense id: the ids of an objective run from 0 to maxid (its number of distinct values - 1), which can be far below
-// n (quantised or heavily tied objectives); the shift follows maxid, so the grid stays populated evenly either way
-__device__ __forceinline__ int cell_shift(uint32_t maxid, int gbits) {
-  const int b = 32 - __clz(maxid | 1u);
-  return b > gbits ? b - gbits : 0;
-}
-
-__global__ void ndg_key_kernel(const uint32_t* __restrict__ rec, int64_t npad, int M, const uint32_t* __restrict__ maxid, int gbits,
-                               uint32_t* __restrict__ keyA, uint32_t* __restrict__ keyB, uint32_t* __restrict__ pos) {
-  int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= npad) return;
-  const uint32_t G1 = (1u << gbits) - 1u;
-  const uint32_t* w = rec + p * 4;  // W == 4 for M <= 3
-  const uint32_t a = min(w[0] >> cell_shift(maxid[1], gbits), G1);
-  const uint32_t b = (M == 3) ? min(w[1] >> cell_shift(maxid[2], gbits), G1) : a;
-  keyA[p] = (a << gbits) | b;
-  keyB[p] = (b << gbits) | a;
-  pos[p] = (uint32_t)p;
-}
-
-// cell-ordered copy: (word 0, word 1 (word 0 again for M == 2), group id, lexicographic position)
-__global__ void ndg_gather_kernel(const uint32_t* __restrict__ rec, const uint32_t* __restrict__ order, int64_t npad,
-                                  int M, uint4* __restrict__ crec) {
-  int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= npad) return;
-  const uint32_t p = order[t];
-  const uint4 r = *reinterpret_cast<const uint4*>(rec + (int64_t)p * 4);
-  crec[t] = (M == 3) ? make_uint4(r.x, r.y, r.z, p) : make_uint4(r.x, r.x, r.y, p);
-}
-
-// cstart[c] = first slot whose key is >= c, c = 0 .. ncell (lower bounds over the sorted keys)
-__global__ void ndg_start_kernel(const uint32_t* __restrict__ skey, int64_t npad, int ncell, uint32_t* __restrict__ cstart) {
-  int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c > ncell) return;
-  int64_t lo = 0, hi = npad;
-  while (lo < hi) {
-    const int64_t mid = (lo + hi) >> 1;
-    if (skey[mid] < (uint32_t)c) lo = mid + 1; else hi = mid;
-  }
-  cstart[c] = (uint32_t)lo;
-}
-
-// inclusive prefix minimum of the per-cell minimum positions: pass 0 along each row, pass 1 along each column
-__global__ void ndg_prefix_min_kernel(const uint32_t* __restrict__ cstartA, const uint4* __restrict__ crecA, int gbits,
-                                      int pass, uint32_t* __restrict__ pm) {
-  extern __shared__ uint32_t sh_scan[];
-  const int G = 1 << gbits;
-  const int line = blockIdx.x, t = threadIdx.x;  // pass 0: line = row a, t = column b; pass 1: line = column b, t = row a
-  const int cell = pass == 0 ? line * G + t : t * G + line;
-  uint32_t v;
-  if (pass == 0) {
-    const uint32_t s0 = cstartA[cell], s1 = cstartA[cell + 1];
-    v = s0 < s1 ? crecA[s0].w : 0xFFFFFFFFu;  // stable sort: the first record of a cell has its smallest position
-  } else {
-    v = pm[cell];
-  }
-  sh_scan[t] = v;
-  __syncthreads();
-  for (int off = 1; off < G; off <<= 1) {
-    const uint32_t o = t >= off ? sh_scan[t - off] : 0xFFFFFFFFu;
-    __syncthreads();
-    v = min(v, o);
-    sh_scan[t] = v;
-    __syncthreads();
-  }
-  pm[cell] = v;
-}
-
-__global__ void ndg_flag_kernel(const uint32_t* __restrict__ rec, int64_t n, int M, const uint32_t* __restrict__ maxid, int gbits,
-                                const uint32_t* __restrict__ pm, const uint32_t* __restrict__ cstartA,
-                                const uint32_t* __restrict__ cstartB, const uint4* __restrict__ crecA,
-                                const uint4* __restrict__ crecB, int* __restrict__ flagS) {
-  const int64_t p64 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p64 >= n) return;
-  const uint32_t p = (uint32_t)p64;
-  const int G = 1 << gbits;
-  const uint4 r = *reinterpret_cast<const uint4*>(rec + p64 * 4);
-  const uint32_t c0 = r.x, c1 = (M == 3) ? r.y : r.x, gid = (M == 3) ? r.z : r.y;
-  const int sh0 = cell_shift(maxid[1], gbits), sh1 = (M == 3) ? cell_shift(maxid[2], gbits) : sh0;
-  const int a = (int)min(c0 >> sh0, (uint32_t)(G - 1)), b = (int)min(c1 >> sh1, (uint32_t)(G - 1));
-  bool dom = a > 0 && b > 0 && __ldg(pm + (a - 1) * G + (b - 1)) < p;
-#pragma unroll
-  for (int pass = 0; pass < 2; ++pass) {
-    if (dom) break;
-    const uint4* cr = pass == 0 ? crecA : crecB;
-    uint32_t t = pass == 0 ? __ldg(cstartA + a * G) : __ldg(cstartB + b * G);
-    const uint32_t t1 = pass == 0 ? __ldg(cstartA + a * G + b + 1) : __ldg(cstartB + b * G + a);
-#define DMO_NDG_TEST(q) ((q).w < p && (q).x <= c0 && (q).y <= c1 && (q).z != gid)
-    for (; t + 4 <= t1 && !dom; t += 4) {
-      const uint4 q0 = __ldg(cr + t), q1 = __ldg(cr + t + 1), q2 = __ldg(cr + t + 2), q3 = __ldg(cr + t + 3);
-      dom = DMO_NDG_TEST(q0) || DMO_NDG_TEST(q1) || DMO_NDG_TEST(q2) || DMO_NDG_TEST(q3);
-    }
-    for (; t < t1 && !dom; ++t) {
-      const uint4 q0 = __ldg(cr + t);
-      dom = DMO_NDG_TEST(q0);
-    }
-#undef DMO_NDG_TEST
-  }
-  flagS[p64] = dom ? 1 : 0;
-}
-
-int bits_for(int64_t n);
-
-// flagS[p] = 1 iff the record at lexicographic position p is dominated (M <= 3, W == 4)
-int nd_flags_grid(dmo_ctx* ctx, const uint32_t* rec, int64_t n, int64_t npad, int M, const uint32_t* maxid, int* flagS) {
-  const int bits = bits_for(n);
-  int gbits = bits / 2;
-  if (gbits < 4) gbits = 4;
-  if (gbits > 9) gbits = 9;
-  const int G = 1 << gbits, GG = G * G;
-  DevBuf<uint32_t> keyA, keyB, keyS, pos, ord, cstartA, cstartB, pm;
-  DevBuf<uint4> crecA, crecB;
-  DMO_TRY(keyA.alloc(ctx, npad));
-  DMO_TRY(keyB.alloc(ctx, npad));
-  DMO_TRY(keyS.alloc(ctx, npad));
-  DMO_TRY(pos.alloc(ctx, npad));
-  DMO_TRY(ord.alloc(ctx, npad));
-  DMO_TRY(cstartA.alloc(ctx, GG + 1));
-  DMO_TRY(cstartB.alloc(ctx, GG + 1));
-  DMO_TRY(pm.alloc(ctx, GG));
-  DMO_TRY(crecA.alloc(ctx, npad));
-  DMO_TRY(crecB.alloc(ctx, npad));
-  const unsigned gp = (unsigned)ceil_div(npad, 256);
-  ProfileScope ps(ctx, "nd_flags");
-  DMO_LAUNCH(ndg_key_kernel, gp, 256, 0, rec, npad, M, maxid, gbits, keyA.p, keyB.p, pos.p);
-  for (int pass = 0; pass < 2; ++pass) {  // stable sorts: positions stay ascending inside a cell
-    DMO_TRY(prim_sort_pairs_u32(ctx, pass == 0 ? keyA.p : keyB.p, keyS.p, pos.p, ord.p, npad, 0, 2 * gbits));
-    DMO_LAUNCH(ndg_gather_kernel, gp, 256, 0, rec, ord.p, npad, M, pass == 0 ? crecA.p : crecB.p);
-    DMO_LAUNCH(ndg_start_kernel, (unsigned)ceil_div(GG + 1, 256), 256, 0, keyS.p, npad, GG,
-               pass == 0 ? cstartA.p : cstartB.p);
-  }
-  DMO_LAUNCH(ndg_prefix_min_kernel, G, G, G * sizeof(uint32_t), cstartA.p, crecA.p, gbits, 0, pm.p);
-  DMO_LAUNCH(ndg_prefix_min_kernel, G, G, G * sizeof(uint32_t), cstartA.p, crecA.p, gbits, 1, pm.p);
-  DMO_LAUNCH(ndg_flag_kernel, (unsigned)ceil_div(n, 128), 128, 0, rec, n, M, maxid, gbits, pm.p, cstartA.p, cstartB.p,
-             crecA.p, crecB.p, flagS);
-  DMO_CHECK_LAUNCH();
-  return DMO_OK;
-}
-
 template <int M>
 int launch_nd_flags(dmo_ctx* ctx, const uint32_t* rec, int nblocks, int* flagS) {
   ProfileScope ps(ctx, "nd_flags");
@@ -1017,61 +872,106 @@ int launch_chain(dmo_ctx* ctx, uint32_t* rec, int nblocks, int* rankS, int* tick
   return DMO_OK;
 }
 
+// f(std::integral_constant<int, M>()) for a runtime objective count M in 2 .. 16: one instantiation per count
+template <int MC = 2, class F>
+int dispatch_m(int M, F&& f) {
+  if constexpr (MC < 16) {
+    if (M != MC) return dispatch_m<MC + 1>(M, f);
+  }
+  return f(std::integral_constant<int, MC>());
+}
+
 int bits_for(int64_t n) {
   int b = 1;
   while (((int64_t)1 << b) < n) ++b;
   return b;
 }
 
-// ------------------------------------------------------------------------------------------------ front peeling (M == 3)
-// A truncation (remove_worst: keep the best `keep` of n rows) needs the ranks of the kept rows only.  When those rows span
-// few fronts -- a converging population: the bench's merged sets put the best 65 536 of 131 072 points into 7 fronts, a
-// sphere-shaped set into 2 -- peeling them one by one is cheaper than the chain, whose 1024 links are serial whatever the
-// data looks like.  Front k = the points of the remaining set that no remaining point dominates, found with the cell grid
-// of the rank-0 filter above, built once on the dense ids (cells over objectives 2 and 3; inside a cell the records are
-// ordered by their objective-1 id, so the smallest living id of a cell is its first living record):
-//   * per peel: per-cell minimum of the living objective-1 ids, its 2-D prefix minimum, one pass over the living points
-//     (table lookup for the cells strictly below, exact tests along the own cell row and column), then the new front is
-//     marked: rank written, its records in both cell-ordered copies overwritten with an id that dominates nothing;
-//   * the loop stops once `keep` rows are ranked (the others get the next rank: they are truncated away), or gives up
-//     when the fronts turn out to be small (many peels ahead): the chain then runs as if nothing had happened.
-constexpr uint32_t PEEL_DEAD = 0xFFFFFFFFu;
+// ------------------------------------------------------------------------------------------------ cell grid (M <= 3)
+// A G x G grid over the dense ids of objectives 2 and 3 answers most "does a living point dominate me" queries with one
+// table lookup.  Inside a cell the records are ordered by their objective-1 id, so the first living record of a cell
+// carries its smallest living id.  A point in a cell strictly below the target's cell in both objectives dominates it iff
+// its objective-1 id is <= the target's, so those cells hold a dominator iff the exclusive 2-D prefix minimum of the
+// per-cell minima is <= the target's id.  Only the points in the target's own cell row and cell column need the exact
+// test; two cell-ordered copies of the records (row-major and column-major) make both of them contiguous streams.
+// Two objectives lay the grid over objective 2 twice: only the diagonal cells fill.
+// The rank-0 filter runs one such test with every point alive; front peeling (below) runs one per front.
+constexpr uint32_t PEEL_DEAD = 0xFFFFFFFFu;  // objective-1 id of a dead record, minimum of an empty cell
 
-__global__ void peel_key_kernel(const uint32_t* __restrict__ R, int64_t n, const uint32_t* __restrict__ maxid, int gbits,
-                                uint32_t* __restrict__ key0, uint32_t* __restrict__ keyA, uint32_t* __restrict__ keyB) {
+// cell of a dense id: the ids of an objective run from 0 to maxid (its number of distinct values - 1), which can be far below
+// n (quantised or heavily tied objectives); the shift follows maxid, so the grid stays populated evenly either way
+__device__ __forceinline__ int cell_shift(uint32_t maxid, int gbits) {
+  const int b = 32 - __clz(maxid | 1u);
+  return b > gbits ? b - gbits : 0;
+}
+
+// the three id columns a grid compares, and the largest ids of the two it is laid over (device pointers)
+struct GridIds {
+  const uint32_t *c0, *c1, *c2;
+  const uint32_t *max1, *max2;
+};
+
+GridIds grid_ids(const uint32_t* R, const uint32_t* maxid, int64_t n, int M) {
+  const int j2 = M == 3 ? 2 : 1;
+  return GridIds{R, R + n, R + (size_t)j2 * n, maxid + 1, maxid + j2};
+}
+
+struct CellGrid {
+  int gbits = 0;
+  DevBuf<uint32_t> cstartA, cstartB;     // [G*G + 1] first slot of every cell in the row-major / column-major copy
+  DevBuf<uint4> crecA, crecB;            // [n] (objective-1, -2, -3 id, row) in cell order
+  DevBuf<uint32_t> pm;                   // [G*G] per-cell minimum of the living objective-1 ids, then its prefix minimum
+  DevBuf<uint32_t> first, slotA, slotB;  // peeling only: first living slot of every cell, slot of every row per copy
+};
+
+__global__ void grid_key_kernel(GridIds ids, int64_t n, int gbits, uint32_t* __restrict__ key0, uint32_t* __restrict__ keyA,
+                                uint32_t* __restrict__ keyB) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const uint32_t G1 = (1u << gbits) - 1u;
-  const uint32_t a = min(R[n + i] >> cell_shift(maxid[1], gbits), G1), b = min(R[2 * n + i] >> cell_shift(maxid[2], gbits), G1);
-  key0[i] = R[i];
+  const uint32_t a = min(ids.c1[i] >> cell_shift(*ids.max1, gbits), G1), b = min(ids.c2[i] >> cell_shift(*ids.max2, gbits), G1);
+  key0[i] = ids.c0[i];
   keyA[i] = (a << gbits) | b;
   keyB[i] = (b << gbits) | a;
 }
 
-// cell-ordered copy (ids of the three objectives, point index) and the slot of every point in it
-__global__ void peel_gather_kernel(const uint32_t* __restrict__ R, const uint32_t* __restrict__ order, int64_t n,
-                                   uint4* __restrict__ crec, uint32_t* __restrict__ slot) {
+// cell-ordered copy (ids of the three objectives, row) and, when peeling, the slot of every row in it
+__global__ void grid_gather_kernel(GridIds ids, const uint32_t* __restrict__ order, int64_t n, uint4* __restrict__ crec,
+                                   uint32_t* __restrict__ slot) {
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= n) return;
   const uint32_t i = order[t];
-  crec[t] = make_uint4(R[i], R[n + i], R[2 * n + i], i);
-  slot[i] = (uint32_t)t;
+  crec[t] = make_uint4(ids.c0[i], ids.c1[i], ids.c2[i], i);
+  if (slot != nullptr) slot[i] = (uint32_t)t;
 }
 
-// smallest living objective-1 id of every cell (the pointer to a cell's first living record only ever moves forward)
-__global__ void peel_cellmin_kernel(const uint32_t* __restrict__ cstart, const uint4* __restrict__ crec, int ncell,
+// cstart[c] = first slot whose key is >= c, c = 0 .. ncell (lower bounds over the sorted keys)
+__global__ void grid_start_kernel(const uint32_t* __restrict__ skey, int64_t n, int ncell, uint32_t* __restrict__ cstart) {
+  int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c > ncell) return;
+  int64_t lo = 0, hi = n;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (skey[mid] < (uint32_t)c) lo = mid + 1; else hi = mid;
+  }
+  cstart[c] = (uint32_t)lo;
+}
+
+// smallest living objective-1 id of every cell.  Peeling keeps a pointer to each cell's first living record, which only
+// ever moves forward; without one (first == nullptr: every record lives) a cell's first record is its smallest.
+__global__ void grid_cellmin_kernel(const uint32_t* __restrict__ cstart, const uint4* __restrict__ crec, int ncell,
                                     uint32_t* __restrict__ first, uint32_t* __restrict__ pm) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= ncell) return;
-  uint32_t f = first[c];
+  uint32_t f = first != nullptr ? first[c] : cstart[c];
   const uint32_t e = cstart[c + 1];
   while (f < e && crec[f].x == PEEL_DEAD) ++f;
-  first[c] = f;
+  if (first != nullptr) first[c] = f;
   pm[c] = f < e ? crec[f].x : PEEL_DEAD;
 }
 
 // in-place inclusive prefix minimum: pass 0 along each row of the G x G table, pass 1 along each column
-__global__ void peel_prefix_min_kernel(uint32_t* __restrict__ pm, int gbits, int pass) {
+__global__ void grid_prefix_min_kernel(uint32_t* __restrict__ pm, int gbits, int pass) {
   extern __shared__ uint32_t sh_scan[];
   const int G = 1 << gbits;
   const int line = blockIdx.x, t = threadIdx.x;
@@ -1089,18 +989,18 @@ __global__ void peel_prefix_min_kernel(uint32_t* __restrict__ pm, int gbits, int
   pm[cell] = v;
 }
 
-// dom[i] = 1 iff a living point dominates the living point i
-__global__ void peel_flag_kernel(const uint32_t* __restrict__ R, int64_t n, const uint32_t* __restrict__ maxid, int gbits,
-                                 const uint32_t* __restrict__ pm,
+// dom[i] = 1 iff a living point dominates the living point i (alive == nullptr: every point lives)
+template <typename OutT>
+__global__ void grid_flag_kernel(GridIds ids, int64_t n, int gbits, const uint32_t* __restrict__ pm,
                                  const uint32_t* __restrict__ cstartA, const uint32_t* __restrict__ cstartB,
                                  const uint4* __restrict__ crecA, const uint4* __restrict__ crecB,
-                                 const uint8_t* __restrict__ alive, uint8_t* __restrict__ dom_out) {
+                                 const uint8_t* __restrict__ alive, OutT* __restrict__ dom_out) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n || !alive[i]) return;
+  if (i >= n || (alive != nullptr && !alive[i])) return;
   const int G = 1 << gbits;
-  const uint32_t c0 = R[i], c1 = R[n + i], c2 = R[2 * n + i];
-  const int a = (int)min(c1 >> cell_shift(maxid[1], gbits), (uint32_t)(G - 1));
-  const int b = (int)min(c2 >> cell_shift(maxid[2], gbits), (uint32_t)(G - 1));
+  const uint32_t c0 = ids.c0[i], c1 = ids.c1[i], c2 = ids.c2[i];
+  const int a = (int)min(c1 >> cell_shift(*ids.max1, gbits), (uint32_t)(G - 1));
+  const int b = (int)min(c2 >> cell_shift(*ids.max2, gbits), (uint32_t)(G - 1));
   // cells strictly below in both words hold different vectors: "<=" on the first objective is enough there
   bool dom = a > 0 && b > 0 && __ldg(pm + (a - 1) * G + (b - 1)) <= c0;
 #pragma unroll
@@ -1130,8 +1030,82 @@ __global__ void peel_flag_kernel(const uint32_t* __restrict__ R, int64_t n, cons
     }
 #undef DMO_PEEL_TEST
   }
-  dom_out[i] = dom ? 1 : 0;
+  dom_out[i] = (OutT)(dom ? 1 : 0);
 }
+
+// Sorted by objective-1 id, then stably by cell for each copy, so that inside a cell the records ascend in that id.
+int build_cell_grid(dmo_ctx* ctx, const GridIds& ids, int64_t n, int gbits, bool peel, CellGrid& cg) {
+  cg.gbits = gbits;
+  const int GG = 1 << (2 * gbits);
+  const unsigned g = (unsigned)ceil_div(n, 256);
+  DevBuf<uint32_t> key0, keyA, keyB, keyS, keyT, ord0, ordS, iota;
+  DMO_TRY(key0.alloc(ctx, n));
+  DMO_TRY(keyA.alloc(ctx, n));
+  DMO_TRY(keyB.alloc(ctx, n));
+  DMO_TRY(keyS.alloc(ctx, n));
+  DMO_TRY(keyT.alloc(ctx, n));
+  DMO_TRY(ord0.alloc(ctx, n));
+  DMO_TRY(ordS.alloc(ctx, n));
+  DMO_TRY(iota.alloc(ctx, n));
+  DMO_TRY(cg.cstartA.alloc(ctx, GG + 1));
+  DMO_TRY(cg.cstartB.alloc(ctx, GG + 1));
+  DMO_TRY(cg.crecA.alloc(ctx, n));
+  DMO_TRY(cg.crecB.alloc(ctx, n));
+  DMO_TRY(cg.pm.alloc(ctx, GG));
+  if (peel) {
+    DMO_TRY(cg.first.alloc(ctx, GG));
+    DMO_TRY(cg.slotA.alloc(ctx, n));
+    DMO_TRY(cg.slotB.alloc(ctx, n));
+  }
+  DMO_LAUNCH(grid_key_kernel, g, 256, 0, ids, n, gbits, key0.p, keyA.p, keyB.p);
+  DMO_TRY(prim_iota_u32(ctx, iota.p, n));
+  DMO_TRY(prim_sort_pairs_u32(ctx, key0.p, keyS.p, iota.p, ord0.p, n, 0, bits_for(n)));  // by objective-1 id ...
+  for (int pass = 0; pass < 2; ++pass) {                                                // ... then stably by cell
+    DMO_LAUNCH(gather_u32_kernel, g, 256, 0, pass == 0 ? keyA.p : keyB.p, ord0.p, n, keyT.p);
+    DMO_TRY(prim_sort_pairs_u32(ctx, keyT.p, keyS.p, ord0.p, ordS.p, n, 0, 2 * gbits));
+    DMO_LAUNCH(grid_gather_kernel, g, 256, 0, ids, ordS.p, n, pass == 0 ? cg.crecA.p : cg.crecB.p, pass == 0 ? cg.slotA.p : cg.slotB.p);
+    DMO_LAUNCH(grid_start_kernel, (unsigned)ceil_div(GG + 1, 256), 256, 0, keyS.p, n, GG, pass == 0 ? cg.cstartA.p : cg.cstartB.p);
+  }
+  if (peel) DMO_CUDA(cudaMemcpyAsync(cg.first.p, cg.cstartA.p, (size_t)GG * sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->stream));
+  DMO_CHECK_LAUNCH();
+  return DMO_OK;
+}
+
+// dom[i] = 1 iff a living point dominates the living point i: per-cell minima, their 2-D prefix minimum, one flag pass
+template <typename OutT>
+int grid_dominated(dmo_ctx* ctx, CellGrid& cg, const GridIds& ids, int64_t n, const uint8_t* alive, OutT* dom) {
+  const int G = 1 << cg.gbits, GG = G * G;
+  DMO_LAUNCH(grid_cellmin_kernel, (unsigned)ceil_div(GG, 256), 256, 0, cg.cstartA.p, cg.crecA.p, GG, cg.first.p, cg.pm.p);
+  DMO_LAUNCH(grid_prefix_min_kernel, G, G, G * sizeof(uint32_t), cg.pm.p, cg.gbits, 0);
+  DMO_LAUNCH(grid_prefix_min_kernel, G, G, G * sizeof(uint32_t), cg.pm.p, cg.gbits, 1);
+  DMO_LAUNCH((grid_flag_kernel<OutT>), (unsigned)ceil_div(n, 128), 128, 0, ids, n, cg.gbits, cg.pm.p, cg.cstartA.p, cg.cstartB.p,
+             cg.crecA.p, cg.crecB.p, alive, dom);
+  DMO_CHECK_LAUNCH();
+  return DMO_OK;
+}
+
+// flag[i] = 1 iff some row dominates row i (M <= 3), written in row order
+int nd_flags_cell_grid(dmo_ctx* ctx, const uint32_t* R, const uint32_t* maxid, int64_t n, int M, int32_t* d_flag01) {
+  int gbits = bits_for(n) / 2;
+  if (gbits < 4) gbits = 4;
+  if (gbits > 9) gbits = 9;
+  const GridIds ids = grid_ids(R, maxid, n, M);
+  CellGrid cg;
+  ProfileScope ps(ctx, "nd_flags");
+  DMO_TRY(build_cell_grid(ctx, ids, n, gbits, false, cg));
+  return grid_dominated(ctx, cg, ids, n, nullptr, d_flag01);
+}
+
+// ------------------------------------------------------------------------------------------------ front peeling (M == 3)
+// A truncation (remove_worst: keep the best `keep` of n rows) needs the ranks of the kept rows only.  When those rows span
+// few fronts -- a converging population: the bench's merged sets put the best 65 536 of 131 072 points into 7 fronts, a
+// sphere-shaped set into 2 -- peeling them one by one is cheaper than the chain, whose 1024 links are serial whatever the
+// data looks like.  Front k = the points of the remaining set that no remaining point dominates, found on the cell grid
+// above, built once:
+//   * per peel: the grid's test over the living points, then the new front is marked: rank written, its records in both
+//     cell-ordered copies overwritten with an id that dominates nothing;
+//   * the loop stops once `keep` rows are ranked (the others get the next rank: they are truncated away), or gives up
+//     when the fronts turn out to be small (many peels ahead): the chain then runs as if nothing had happened.
 
 // the living points nobody dominates form front k: rank, death, count
 __global__ void peel_mark_kernel(int64_t n, uint8_t* __restrict__ alive, const uint8_t* __restrict__ dom, int k,
@@ -1228,53 +1202,23 @@ int rank_by_peeling(dmo_ctx* ctx, const uint32_t* R, const uint32_t* maxid, int6
   if (gbits < 4) gbits = 4;
   if (const char* e = getenv("DMO_PEEL_GBITS")) gbits = atoi(e);
   if (gbits > 9) gbits = 9;
-  const int G = 1 << gbits, GG = G * G;
   const unsigned g = (unsigned)ceil_div(n, 256);
-  DevBuf<uint32_t> key0, keyA, keyB, keyS, keyT, ord0, ordS, iota, cstartA, cstartB, firstA, pm, slotA, slotB;
-  DevBuf<uint4> crecA, crecB;
+  const GridIds ids = grid_ids(R, maxid, n, 3);
+  CellGrid cg;
+  DMO_TRY(build_cell_grid(ctx, ids, n, gbits, true, cg));
   DevBuf<uint8_t> alive, dom;
   DevBuf<unsigned long long> count;
-  DMO_TRY(key0.alloc(ctx, n));
-  DMO_TRY(keyA.alloc(ctx, n));
-  DMO_TRY(keyB.alloc(ctx, n));
-  DMO_TRY(keyS.alloc(ctx, n));
-  DMO_TRY(keyT.alloc(ctx, n));
-  DMO_TRY(ord0.alloc(ctx, n));
-  DMO_TRY(ordS.alloc(ctx, n));
-  DMO_TRY(iota.alloc(ctx, n));
-  DMO_TRY(cstartA.alloc(ctx, GG + 1));
-  DMO_TRY(cstartB.alloc(ctx, GG + 1));
-  DMO_TRY(firstA.alloc(ctx, GG));
-  DMO_TRY(pm.alloc(ctx, GG));
-  DMO_TRY(slotA.alloc(ctx, n));
-  DMO_TRY(slotB.alloc(ctx, n));
-  DMO_TRY(crecA.alloc(ctx, n));
-  DMO_TRY(crecB.alloc(ctx, n));
   DMO_TRY(alive.alloc(ctx, n));
   DMO_TRY(dom.alloc(ctx, n));
   DMO_TRY(count.alloc(ctx, 1));
-  DMO_LAUNCH(peel_key_kernel, g, 256, 0, R, n, maxid, gbits, key0.p, keyA.p, keyB.p);
-  DMO_TRY(prim_iota_u32(ctx, iota.p, n));
-  DMO_TRY(prim_sort_pairs_u32(ctx, key0.p, keyS.p, iota.p, ord0.p, n, 0, bits));  // by objective-1 id ...
-  for (int pass = 0; pass < 2; ++pass) {                                        // ... then stably by cell
-    DMO_LAUNCH(gather_u32_kernel, g, 256, 0, pass == 0 ? keyA.p : keyB.p, ord0.p, n, keyT.p);
-    DMO_TRY(prim_sort_pairs_u32(ctx, keyT.p, keyS.p, ord0.p, ordS.p, n, 0, 2 * gbits));
-    DMO_LAUNCH(peel_gather_kernel, g, 256, 0, R, ordS.p, n, pass == 0 ? crecA.p : crecB.p, pass == 0 ? slotA.p : slotB.p);
-    DMO_LAUNCH(ndg_start_kernel, (unsigned)ceil_div(GG + 1, 256), 256, 0, keyS.p, n, GG, pass == 0 ? cstartA.p : cstartB.p);
-  }
-  DMO_CUDA(cudaMemcpyAsync(firstA.p, cstartA.p, (size_t)GG * sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->stream));
   DMO_LAUNCH(fill_u8_kernel, g, 256, 0, alive.p, n, (uint8_t)1);
   DMO_CUDA(cudaMemsetAsync(count.p, 0, sizeof(unsigned long long), ctx->stream));
   unsigned long long ranked = 0, before = 0;
   double prev_front = 0.0;
   int k = 0;
   for (;; ++k) {
-    DMO_LAUNCH(peel_cellmin_kernel, (unsigned)ceil_div(GG, 256), 256, 0, cstartA.p, crecA.p, GG, firstA.p, pm.p);
-    DMO_LAUNCH(peel_prefix_min_kernel, G, G, G * sizeof(uint32_t), pm.p, gbits, 0);
-    DMO_LAUNCH(peel_prefix_min_kernel, G, G, G * sizeof(uint32_t), pm.p, gbits, 1);
-    DMO_LAUNCH(peel_flag_kernel, (unsigned)ceil_div(n, 128), 128, 0, R, n, maxid, gbits, pm.p, cstartA.p, cstartB.p, crecA.p, crecB.p,
-               alive.p, dom.p);
-    DMO_LAUNCH(peel_mark_kernel, g, 256, 0, n, alive.p, dom.p, k, d_rank, slotA.p, slotB.p, crecA.p, crecB.p, count.p);
+    DMO_TRY(grid_dominated(ctx, cg, ids, n, alive.p, dom.p));
+    DMO_LAUNCH(peel_mark_kernel, g, 256, 0, n, alive.p, dom.p, k, d_rank, cg.slotA.p, cg.slotB.p, cg.crecA.p, cg.crecB.p, count.p);
     DMO_CHECK_LAUNCH();
     before = ranked;
     DMO_CUDA(cudaMemcpyAsync(&ranked, count.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1303,68 +1247,55 @@ int rank_by_peeling(dmo_ctx* ctx, const uint32_t* R, const uint32_t* maxid, int6
   return DMO_OK;
 }
 
-}  // namespace
-
-int rank_nd_device_ex(dmo_ctx* ctx, const double* dY, int64_t n, int M, int32_t* d_rank, bool flags_only, int64_t keep = 0) {
-  if (n <= 0) return DMO_OK;
+// ------------------------------------------------------------------------------------------------ stages of the rank
+// 1. R[j * n + i] = dense id of Y[i, j] (order- and equality-preserving), maxid[j] = largest id of objective j
+int dense_ids(dmo_ctx* ctx, const double* dY, int64_t n, int M, DevBuf<uint32_t>& R, DevBuf<uint32_t>& maxid) {
   DMO_REQUIRE(M >= 1 && M <= 16, "rank_nd: M=%d out of range [1,16]", M);
   DMO_REQUIRE(n < ((int64_t)1 << 31) - 4096, "rank_nd: n too large");
   const unsigned g = (unsigned)ceil_div(n, 256);
-
-  DevBuf<uint32_t> R;  // M x n dense integer ids (SoA)
-  DevBuf<uint32_t> maxid;  // largest id per objective (= number of distinct values - 1)
   DMO_TRY(R.alloc(ctx, (size_t)M * n));
   DMO_TRY(maxid.alloc(ctx, M));
-  {
-    DevBuf<uint64_t> k0, k1;
-    DevBuf<uint32_t> i0, i1, flag, dense;
-    DMO_TRY(k0.alloc(ctx, n));
-    DMO_TRY(k1.alloc(ctx, n));
-    DMO_TRY(i0.alloc(ctx, n));
-    DMO_TRY(i1.alloc(ctx, n));
-    DMO_TRY(flag.alloc(ctx, n));
-    DMO_TRY(dense.alloc(ctx, n));
-    for (int j = 0; j < M; ++j) {
-      DMO_LAUNCH(col_keys_kernel, g, 256, 0, dY, n, M, j, k0.p, i0.p);
-      DMO_TRY(prim_sort_pairs_u64(ctx, k0.p, k1.p, i0.p, i1.p, n, 0, 64));
-      DMO_LAUNCH(flag_new_u64_kernel, g, 256, 0, k1.p, n, flag.p);
-      DMO_TRY(prim_inclusive_sum_u32(ctx, flag.p, dense.p, n));
-      DMO_LAUNCH(scatter_dense_kernel, g, 256, 0, dense.p, i1.p, n, R.p + (size_t)j * n);
-      DMO_CUDA(cudaMemcpyAsync(maxid.p + j, dense.p + (n - 1), sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->stream));
-    }
-    DMO_CHECK_LAUNCH();
+  DevBuf<uint64_t> k0, k1;
+  DevBuf<uint32_t> i0, i1, flag, dense;
+  DMO_TRY(k0.alloc(ctx, n));
+  DMO_TRY(k1.alloc(ctx, n));
+  DMO_TRY(i0.alloc(ctx, n));
+  DMO_TRY(i1.alloc(ctx, n));
+  DMO_TRY(flag.alloc(ctx, n));
+  DMO_TRY(dense.alloc(ctx, n));
+  for (int j = 0; j < M; ++j) {
+    DMO_LAUNCH(col_keys_kernel, g, 256, 0, dY, n, M, j, k0.p, i0.p);
+    DMO_TRY(prim_sort_pairs_u64(ctx, k0.p, k1.p, i0.p, i1.p, n, 0, 64));
+    DMO_LAUNCH(flag_new_u64_kernel, g, 256, 0, k1.p, n, flag.p);
+    DMO_TRY(prim_inclusive_sum_u32(ctx, flag.p, dense.p, n));
+    DMO_LAUNCH(scatter_dense_kernel, g, 256, 0, dense.p, i1.p, n, R.p + (size_t)j * n);
+    DMO_CUDA(cudaMemcpyAsync(maxid.p + j, dense.p + (n - 1), sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->stream));
   }
-  if (M == 1) {
-    DMO_LAUNCH(copy_u32_to_i32_kernel, g, 256, 0, R.p, n, d_rank);
-    DMO_CHECK_LAUNCH();
-    return DMO_OK;
-  }
-  if (!flags_only && M == 3 && keep > 0 && n >= 8192 && 4 * keep <= 3 * n) {  // truncation: the best `keep` rows are enough
-    bool done = false;
-    DMO_TRY(rank_by_peeling(ctx, R.p, maxid.p, n, keep, d_rank, &done));
-    if (done) return DMO_OK;
-  }
+  DMO_CHECK_LAUNCH();
+  return DMO_OK;
+}
 
-  // lexicographic order of the id vectors: LSD passes, least significant objective first
+// 2. An order of the points in which a point can only be dominated by points before it, the group ids of identical
+//    vectors, and the chain's padded records in that order.  sshift == 0: lexicographic order (LSD passes, least
+//    significant objective first); sshift > 0: the segmented order of RankSeg, key = (objective-1 id >> sshift,
+//    objective 2, ..., objective M, objective 1).
+struct RankOrder {
+  DevBuf<uint32_t> permA, permB, rec;
+  const uint32_t* perm = nullptr;  // position -> row
+  int64_t nblocks = 0, npad = 0;
+};
+
+int rank_order(dmo_ctx* ctx, const uint32_t* R, int64_t n, int M, int sshift, RankOrder& o) {
   const int bits = bits_for(n);
-  DevBuf<uint32_t> permA, permB, keyA, keyB;
-  DMO_TRY(permA.alloc(ctx, n));
-  DMO_TRY(permB.alloc(ctx, n));
+  const unsigned g = (unsigned)ceil_div(n, 256);
+  DevBuf<uint32_t> keyA, keyB, gid;
+  DMO_TRY(o.permA.alloc(ctx, n));
+  DMO_TRY(o.permB.alloc(ctx, n));
   DMO_TRY(keyA.alloc(ctx, n));
   DMO_TRY(keyB.alloc(ctx, n));
-  DMO_TRY(prim_iota_u32(ctx, permA.p, n));
-  uint32_t* pin = permA.p;
-  uint32_t* pout = permB.p;
-  // The chain kernel for two and three objectives takes the segmented order (RankSeg): key = (segment of objective 1,
-  // objective 2, ..., objective M, objective 1).  Everything else keeps the plain lexicographic order.
-  const int64_t nblocks_est = ceil_div(n, RANK_T);
-  int segbits = bits - 10;  // segments of 1024 dense ids of objective 1 (8 blocks), at most 128 segments
-  if (segbits > 7) segbits = 7;
-  if (const char* e = getenv("DMO_RANK_SEGBITS")) segbits = atoi(e);
-  if (segbits < 1) segbits = 1;
-  const bool use_seg = !flags_only && M <= 3 && nblocks_est >= 16 && nblocks_est <= RANK_SEG_MAXT && bits > segbits + 7 &&
-                       getenv("DMO_RANK_NOSEG") == nullptr;
-  const int sshift = bits - segbits;
+  DMO_TRY(prim_iota_u32(ctx, o.permA.p, n));
+  uint32_t* pin = o.permA.p;
+  uint32_t* pout = o.permB.p;
   auto sort_pass = [&](const uint32_t* col, int shift, int nbits) -> int {
     if (shift == 0) {
       DMO_LAUNCH(gather_u32_kernel, g, 256, 0, col, pin, n, keyA.p);
@@ -1377,77 +1308,68 @@ int rank_nd_device_ex(dmo_ctx* ctx, const double* dY, int64_t n, int M, int32_t*
     pout = t;
     return DMO_OK;
   };
-  if (use_seg) {
-    DMO_TRY(sort_pass(R.p, 0, bits));  // least significant: objective 1 itself
-    for (int j = M - 1; j >= 1; --j) DMO_TRY(sort_pass(R.p + (size_t)j * n, 0, bits));
-    DMO_TRY(sort_pass(R.p, sshift, bits - sshift));  // most significant: the segment
+  if (sshift > 0) {
+    DMO_TRY(sort_pass(R, 0, bits));  // least significant: objective 1 itself
+    for (int j = M - 1; j >= 1; --j) DMO_TRY(sort_pass(R + (size_t)j * n, 0, bits));
+    DMO_TRY(sort_pass(R, sshift, bits - sshift));  // most significant: the segment
   } else {
-    for (int j = M - 1; j >= 0; --j) DMO_TRY(sort_pass(R.p + (size_t)j * n, 0, bits));
+    for (int j = M - 1; j >= 0; --j) DMO_TRY(sort_pass(R + (size_t)j * n, 0, bits));
   }
-  const uint32_t* perm = pin;
+  o.perm = pin;
 
   // group ids (identical vectors share one)
-  DevBuf<uint32_t> gid;
   DMO_TRY(gid.alloc(ctx, n));
-  DMO_LAUNCH(flag_new_vec_kernel, g, 256, 0, R.p, perm, n, M, keyA.p);
+  DMO_LAUNCH(flag_new_vec_kernel, g, 256, 0, R, o.perm, n, M, keyA.p);
   DMO_TRY(prim_inclusive_sum_u32(ctx, keyA.p, gid.p, n));
 
   const int W = 4 * ((M + 1 + 3) / 4);
+  o.nblocks = ceil_div(n, RANK_T);
+  o.npad = o.nblocks * RANK_T;
+  DMO_TRY(o.rec.alloc(ctx, (size_t)o.npad * W));
+  DMO_LAUNCH(build_records_kernel, (unsigned)ceil_div(o.npad, 256), 256, 0, R, o.perm, gid.p, n, o.npad, M, W, o.rec.p);
+  DMO_CHECK_LAUNCH();
+  return DMO_OK;
+}
+
+// segment shift of the chain's order: two and three objectives take the segmented order (RankSeg) from 16 to
+// RANK_SEG_MAXT blocks, everything else the plain lexicographic order (0)
+int seg_shift(int64_t n, int M) {
+  const int bits = bits_for(n);
+  int segbits = bits - 10;  // segments of 1024 dense ids of objective 1 (8 blocks), at most 128 segments
+  if (segbits > 7) segbits = 7;
+  if (const char* e = getenv("DMO_RANK_SEGBITS")) segbits = atoi(e);
+  if (segbits < 1) segbits = 1;
   const int64_t nblocks = ceil_div(n, RANK_T);
-  const int64_t npad = nblocks * RANK_T;
-  DevBuf<uint32_t> rec;
+  const bool seg = M <= 3 && nblocks >= 16 && nblocks <= RANK_SEG_MAXT && bits > segbits + 7 && getenv("DMO_RANK_NOSEG") == nullptr;
+  return seg ? bits - segbits : 0;
+}
+
+// 3. the chain kernel over the records of `o`, ranks scattered back to row order
+int rank_chain(dmo_ctx* ctx, const uint32_t* R, int64_t n, int M, int sshift, RankOrder& o, int32_t* d_rank) {
+  const int nblocks = (int)o.nblocks;
   DevBuf<int> rankS, sync;
-  DMO_TRY(rec.alloc(ctx, (size_t)npad * W));
-  DMO_TRY(rankS.alloc(ctx, npad));
+  DMO_TRY(rankS.alloc(ctx, o.npad));
   DMO_TRY(sync.alloc(ctx, nblocks + 2));
   DMO_CUDA(cudaMemsetAsync(sync.p, 0, (nblocks + 2) * sizeof(int), ctx->stream));
-  DMO_LAUNCH(build_records_kernel, (unsigned)ceil_div(npad, 256), 256, 0, R.p, perm, gid.p, n, npad, M, W, rec.p);
   int* ticket = sync.p + nblocks;
   int* errflag = sync.p + nblocks + 1;
-  if (flags_only && M <= 3 && n >= 8192 && getenv("DMO_ND_BRUTE") == nullptr) {
-    DMO_TRY(nd_flags_grid(ctx, rec.p, n, npad, M, maxid.p, rankS.p));
-    DMO_LAUNCH(scatter_rank_kernel, g, 256, 0, rankS.p, perm, n, d_rank);
-    DMO_CHECK_LAUNCH();
-    return DMO_OK;
-  }
-  if (flags_only) {  // d_rank receives 0 for non-dominated points and 1 otherwise
-    switch (M) {
-      case 2: DMO_TRY(launch_nd_flags<2>(ctx, rec.p, (int)nblocks, rankS.p)); break;
-      case 3: DMO_TRY(launch_nd_flags<3>(ctx, rec.p, (int)nblocks, rankS.p)); break;
-      case 4: DMO_TRY(launch_nd_flags<4>(ctx, rec.p, (int)nblocks, rankS.p)); break;
-      case 5: DMO_TRY(launch_nd_flags<5>(ctx, rec.p, (int)nblocks, rankS.p)); break;
-      case 6: DMO_TRY(launch_nd_flags<6>(ctx, rec.p, (int)nblocks, rankS.p)); break;
-      case 7: DMO_TRY(launch_nd_flags<7>(ctx, rec.p, (int)nblocks, rankS.p)); break;
-      case 8: DMO_TRY(launch_nd_flags<8>(ctx, rec.p, (int)nblocks, rankS.p)); break;
-      case 9: DMO_TRY(launch_nd_flags<9>(ctx, rec.p, (int)nblocks, rankS.p)); break;
-      case 10: DMO_TRY(launch_nd_flags<10>(ctx, rec.p, (int)nblocks, rankS.p)); break;
-      case 11: DMO_TRY(launch_nd_flags<11>(ctx, rec.p, (int)nblocks, rankS.p)); break;
-      case 12: DMO_TRY(launch_nd_flags<12>(ctx, rec.p, (int)nblocks, rankS.p)); break;
-      case 13: DMO_TRY(launch_nd_flags<13>(ctx, rec.p, (int)nblocks, rankS.p)); break;
-      case 14: DMO_TRY(launch_nd_flags<14>(ctx, rec.p, (int)nblocks, rankS.p)); break;
-      case 15: DMO_TRY(launch_nd_flags<15>(ctx, rec.p, (int)nblocks, rankS.p)); break;
-      default: DMO_TRY(launch_nd_flags<16>(ctx, rec.p, (int)nblocks, rankS.p)); break;
-    }
-    DMO_LAUNCH(scatter_rank_kernel, g, 256, 0, rankS.p, perm, n, d_rank);
-    DMO_CHECK_LAUNCH();
-    return DMO_OK;
-  }
   RankSeg sg;
   DevBuf<uint32_t> c1rec, seg_start;
   DevBuf<uint16_t> tile_q;
   DevBuf<unsigned long long> stair;
-  if (use_seg) {
-    DMO_TRY(stair.alloc(ctx, npad));
-    DMO_CUDA(cudaMemsetAsync(stair.p, 0, (size_t)npad * sizeof(unsigned long long), ctx->stream));
+  if (sshift > 0) {
+    const int bits = bits_for(n);
+    DMO_TRY(stair.alloc(ctx, o.npad));
+    DMO_CUDA(cudaMemsetAsync(stair.p, 0, (size_t)o.npad * sizeof(unsigned long long), ctx->stream));
     const int nseg = (int)(((uint32_t)(n - 1)) >> sshift) + 1;
     int qshift = bits - 8;
     if (qshift < 0) qshift = 0;
-    DMO_TRY(c1rec.alloc(ctx, npad));
+    DMO_TRY(c1rec.alloc(ctx, o.npad));
     DMO_TRY(seg_start.alloc(ctx, nseg + 1));
     DMO_TRY(tile_q.alloc(ctx, nblocks));
-    DMO_LAUNCH(seg_c1_kernel, (unsigned)ceil_div(npad, 256), 256, 0, R.p, perm, n, npad, c1rec.p);
+    DMO_LAUNCH(seg_c1_kernel, (unsigned)ceil_div(o.npad, 256), 256, 0, R, o.perm, n, o.npad, c1rec.p);
     DMO_LAUNCH(seg_start_kernel, (unsigned)ceil_div(nseg + 1, 128), 128, 0, c1rec.p, n, sshift, nseg, seg_start.p);
-    DMO_LAUNCH(seg_tile_band_kernel, (unsigned)ceil_div(nblocks * 32, 256), 256, 0, rec.p, (int)nblocks, RANK_T, qshift, tile_q.p);
+    DMO_LAUNCH(seg_tile_band_kernel, (unsigned)ceil_div(o.nblocks * 32, 256), 256, 0, o.rec.p, nblocks, RANK_T, qshift, tile_q.p);
     DMO_CHECK_LAUNCH();
     sg.c1rec = c1rec.p;
     sg.seg_start = seg_start.p;
@@ -1456,30 +1378,16 @@ int rank_nd_device_ex(dmo_ctx* ctx, const double* dY, int64_t n, int M, int32_t*
     sg.sshift = sshift;
     sg.qshift = qshift;
     if (M == 2) {
-      DMO_TRY((launch_chain<2, true>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg)));
+      DMO_TRY((launch_chain<2, true>(ctx, o.rec.p, nblocks, rankS.p, ticket, errflag, sg)));
     } else {
-      DMO_TRY((launch_chain<3, true>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg)));
+      DMO_TRY((launch_chain<3, true>(ctx, o.rec.p, nblocks, rankS.p, ticket, errflag, sg)));
     }
   } else {
-    switch (M) {
-      case 2: DMO_TRY((launch_chain<2, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
-      case 3: DMO_TRY((launch_chain<3, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
-      case 4: DMO_TRY((launch_chain<4, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
-      case 5: DMO_TRY((launch_chain<5, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
-      case 6: DMO_TRY((launch_chain<6, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
-      case 7: DMO_TRY((launch_chain<7, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
-      case 8: DMO_TRY((launch_chain<8, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
-      case 9: DMO_TRY((launch_chain<9, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
-      case 10: DMO_TRY((launch_chain<10, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
-      case 11: DMO_TRY((launch_chain<11, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
-      case 12: DMO_TRY((launch_chain<12, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
-      case 13: DMO_TRY((launch_chain<13, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
-      case 14: DMO_TRY((launch_chain<14, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
-      case 15: DMO_TRY((launch_chain<15, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
-      default: DMO_TRY((launch_chain<16, false>(ctx, rec.p, (int)nblocks, rankS.p, ticket, errflag, sg))); break;
-    }
+    DMO_TRY(dispatch_m(M, [&](auto m) {
+      return launch_chain<decltype(m)::value, false>(ctx, o.rec.p, nblocks, rankS.p, ticket, errflag, sg);
+    }));
   }
-  DMO_LAUNCH(scatter_rank_kernel, g, 256, 0, rankS.p, perm, n, d_rank);
+  DMO_LAUNCH(scatter_rank_kernel, (unsigned)ceil_div(n, 256), 256, 0, rankS.p, o.perm, n, d_rank);
   DMO_CHECK_LAUNCH();
   int herr = 0;
   DMO_CUDA(cudaMemcpyAsync(&herr, errflag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1488,15 +1396,47 @@ int rank_nd_device_ex(dmo_ctx* ctx, const double* dY, int64_t n, int M, int32_t*
   return DMO_OK;
 }
 
-int rank_nd_device(dmo_ctx* ctx, const double* dY, int64_t n, int M, int32_t* d_rank) {
-  return rank_nd_device_ex(ctx, dY, n, M, d_rank, false);
-}
+}  // namespace
+
 // ranks that are exact for (at least) the `keep` best rows; the other rows share one larger value (see rank_by_peeling)
 int rank_nd_device_keep(dmo_ctx* ctx, const double* dY, int64_t n, int M, int64_t keep, int32_t* d_rank) {
-  return rank_nd_device_ex(ctx, dY, n, M, d_rank, false, keep);
+  if (n <= 0) return DMO_OK;
+  DevBuf<uint32_t> R, maxid;
+  DMO_TRY(dense_ids(ctx, dY, n, M, R, maxid));
+  if (M == 1) {  // the dense id is the rank
+    DMO_LAUNCH(copy_u32_to_i32_kernel, (unsigned)ceil_div(n, 256), 256, 0, R.p, n, d_rank);
+    DMO_CHECK_LAUNCH();
+    return DMO_OK;
+  }
+  if (M == 3 && keep > 0 && n >= 8192 && 4 * keep <= 3 * n) {  // truncation: the best `keep` rows are enough
+    bool done = false;
+    DMO_TRY(rank_by_peeling(ctx, R.p, maxid.p, n, keep, d_rank, &done));
+    if (done) return DMO_OK;
+  }
+  const int sshift = seg_shift(n, M);
+  RankOrder o;
+  DMO_TRY(rank_order(ctx, R.p, n, M, sshift, o));
+  return rank_chain(ctx, R.p, n, M, sshift, o, d_rank);
 }
+
+int rank_nd_device(dmo_ctx* ctx, const double* dY, int64_t n, int M, int32_t* d_rank) {
+  return rank_nd_device_keep(ctx, dY, n, M, 0, d_rank);
+}
+
 int nondominated_flags_device(dmo_ctx* ctx, const double* dY, int64_t n, int M, int32_t* d_flag01) {
-  return rank_nd_device_ex(ctx, dY, n, M, d_flag01, true);
+  if (n <= 0) return DMO_OK;
+  if (M == 1) return rank_nd_device(ctx, dY, n, M, d_flag01);  // the rank itself: 0 exactly for the rank-0 rows
+  DevBuf<uint32_t> R, maxid;
+  DMO_TRY(dense_ids(ctx, dY, n, M, R, maxid));
+  if (M <= 3 && n >= 8192 && getenv("DMO_ND_BRUTE") == nullptr) return nd_flags_cell_grid(ctx, R.p, maxid.p, n, M, d_flag01);
+  RankOrder o;  // the block scan over the lexicographic records
+  DMO_TRY(rank_order(ctx, R.p, n, M, 0, o));
+  DevBuf<int> flagS;
+  DMO_TRY(flagS.alloc(ctx, o.npad));
+  DMO_TRY(dispatch_m(M, [&](auto m) { return launch_nd_flags<decltype(m)::value>(ctx, o.rec.p, (int)o.nblocks, flagS.p); }));
+  DMO_LAUNCH(scatter_rank_kernel, (unsigned)ceil_div(n, 256), 256, 0, flagS.p, o.perm, n, d_flag01);
+  DMO_CHECK_LAUNCH();
+  return DMO_OK;
 }
 
 extern "C" int dmo_rank_nd(dmo_ctx* ctx, const double* Y, int64_t n, int M, int32_t* rank) {
