@@ -1328,7 +1328,8 @@ def mutate_groups(pop_x, group_size, n_groups, per_group, di_mutation, xlb, xub,
     return (out, par) if return_parents else out
 
 
-BENCHMARKS = {"zdt1": 0, "zdt3": 1, "dtlz1": 10, "dtlz2": 11, "dtlz3": 12, "dtlz4": 13, "dtlz5": 14, "dtlz7": 16, "wfg4": 24}
+BENCHMARKS = {"zdt1": 0, "zdt3": 1, "dtlz1": 10, "dtlz2": 11, "dtlz3": 12, "dtlz4": 13, "dtlz5": 14, "dtlz7": 16, "wfg1": 21, "wfg4": 24,
+              "maf1": 31, "maf2": 32, "maf4": 34}
 
 
 def benchmark_eval(name, X, n_obj, alpha=100.0):

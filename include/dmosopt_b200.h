@@ -555,9 +555,14 @@ int dmo_gather_rows(dmo_ctx* ctx, const double* src, const double* alt, const ui
 
 /* ---- N4: vectorised benchmark objective functions --------------------------------------------
  * replaces the row-at-a-time Python functions of dmosopt/benchmarks/moo_benchmarks.py (dtlz1 :21, dtlz2 :59,
- * dtlz3 :97, dtlz4 :136, dtlz5 :174, dtlz7 :218, wfg4 :335) and the example objectives ZDT1 / ZDT3
- * (examples/example_dmosopt_zdt1.py:9-20, examples/example_dmosopt_zdt3.py:9-21): X (n, n_var) -> Y (n, n_obj).
- * alpha is DTLZ4's bias exponent (the reference's default is 100), ignored elsewhere. */
+ * dtlz3 :97, dtlz4 :136, dtlz5 :174, dtlz7 :218, wfg1 :286, wfg4 :335, maf1 :384, maf2 :422, maf4 :460) and the example
+ * objectives ZDT1 / ZDT3 (examples/example_dmosopt_zdt1.py:9-20, examples/example_dmosopt_zdt3.py:9-21):
+ * X (n, n_var) -> Y (n, n_obj), 2 <= n_obj <= 16, n_var >= n_obj except for ZDT (n_obj = 2).  X may be a device address.
+ * alpha is DTLZ4's bias exponent (the reference's default is 100), ignored elsewhere.  WFG1 and WFG4 take the reference's
+ * default position parameter k = n_obj - 1.  WFG1 refuses shapes whose last maximum window is empty,
+ * (n_obj - 2) (n_var - n_obj + 1) >= n_var (np.max of an empty slice raises in the reference): at n_obj >= 4 only a few
+ * variables are allowed.  WFG4 returns NaN for such a window (np.mean of an empty slice).  MaF4 multiplies objective i
+ * by the correctly rounded double of 10^(2i). */
 #define DMO_BM_ZDT1 0
 #define DMO_BM_ZDT3 1
 #define DMO_BM_DTLZ1 10
@@ -566,7 +571,11 @@ int dmo_gather_rows(dmo_ctx* ctx, const double* src, const double* alt, const ui
 #define DMO_BM_DTLZ4 13
 #define DMO_BM_DTLZ5 14
 #define DMO_BM_DTLZ7 16
+#define DMO_BM_WFG1 21
 #define DMO_BM_WFG4 24
+#define DMO_BM_MAF1 31
+#define DMO_BM_MAF2 32
+#define DMO_BM_MAF4 34
 int dmo_benchmark_eval(dmo_ctx* ctx, int problem, const double* X, int64_t n, int n_var, int n_obj, double alpha,
                        double* Y);
 
