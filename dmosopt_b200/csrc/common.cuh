@@ -192,6 +192,13 @@ __device__ __forceinline__ uint32_t f32_to_ordered(float x) {
   return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
 
+// np.clip(x, lo, hi) == np.minimum(np.maximum(x, lo), hi): a NaN in any operand propagates (fmin / fmax would drop it),
+// and between equal operands (+0.0 / -0.0) the first one is kept, as NumPy's maximum / minimum do
+__device__ __forceinline__ double np_clip(double x, double lo, double hi) {
+  const double m = (x >= lo || isnan(x)) ? x : lo;
+  return (m <= hi || isnan(m)) ? m : hi;
+}
+
 // Philox4x32-10 (Salmon, Moraes, Dror, Shaw 2011): counter-based, no state in memory.
 struct Philox {
   uint32_t k0, k1;
@@ -246,9 +253,11 @@ int rank_nd_device_keep(dmo_ctx* ctx, const double* dY, int64_t n, int M, int64_
 int nondominated_flags_device(dmo_ctx* ctx, const double* dY, int64_t n, int M, int32_t* d_flag01);
 int crowding_device(dmo_ctx* ctx, const double* dY, int64_t n, int M, double* dD);
 int euclidean_device(dmo_ctx* ctx, const double* dY, int64_t n, int M, double* dD);
-// perm (uint32, n) sorted by (rank asc, then each desc key descending, stable on index)
+// perm (uint32, n) sorted by (rank asc, then each desc key descending, stable on index).  rank_below_n: the ranks are
+// known to lie in [0, n) (ranks from rank_nd), so the radix sort needs only the bits of n; otherwise any int32 value
+// (caller-supplied ranks, negative or >= n) sorts over all 32 bits
 int lexsort_device(dmo_ctx* ctx, const int32_t* d_rank, const double* const* d_desc_keys, int nkeys,
-                   int64_t n, uint32_t* d_perm);
+                   int64_t n, uint32_t* d_perm, bool rank_below_n);
 int hypervolume_device(dmo_ctx* ctx, const double* dF, int64_t n, int M, const double* h_ref, double* h_out);
 // the same when the rows carry their non-dominated ranks within a superset (rank > 0 rows are skipped, no filter pass)
 int hypervolume_device_ranked(dmo_ctx* ctx, const double* dF, int64_t n, int M, const double* h_ref, const int32_t* d_rank,

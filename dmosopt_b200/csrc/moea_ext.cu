@@ -146,7 +146,7 @@ __global__ void smpso_velocity_kernel(const float* __restrict__ pos, const doubl
   }
   const double delta = (xub[j] - xlb[j]) / 2;
   double v = __dmul_rn(__dadd_rn(__dadd_rn(__dmul_rn(w, vel[t]), __dmul_rn(c1r1, d1)), __dmul_rn(c2r2, d2)), chi);
-  out[t] = fmin(fmax(v, -delta), delta);
+  out[t] = np_clip(v, -delta, delta);
 }
 
 // ---------------------------------------------------------------------------------------------- batched mutation
@@ -159,7 +159,7 @@ __device__ __forceinline__ double mutate_gene2(double parent, double u, double d
     delta = __dsub_rn(pow(__dmul_rn(2.0, u), e), 1.0);
   else
     delta = __dsub_rn(1.0, pow(__dmul_rn(2.0, __dsub_rn(1.0, u)), e));
-  return fmin(fmax(__dadd_rn(parent, __dmul_rn(__dsub_rn(ub, lb), delta)), lb), ub);
+  return np_clip(__dadd_rn(parent, __dmul_rn(__dsub_rn(ub, lb), delta)), lb, ub);
 }
 
 // child c of group g mutates parent (g * group_size + randint(group_size)) of pop_x: SMPSO's per-swarm mutants
@@ -299,7 +299,7 @@ __global__ void cmaes_rescale_kernel(double* __restrict__ x, int64_t n, int d, c
   const double mx = __longlong_as_double((long long)*mx_bits);
   const double lb = xlb[j], ub = xub[j];
   const double v = __dadd_rn(__dmul_rn(__ddiv_rn(x[t], mx), __dsub_rn(ub, lb)), lb);
-  x[t] = fmin(fmax(v, lb), ub);
+  x[t] = np_clip(v, lb, ub);
 }
 
 // z[i] = ((x_gen[ci[i]] - parents_x[pi[i]]) / (xub - xlb)) / step[i]: the offspring's move in its parent's coordinates

@@ -19,7 +19,7 @@ __device__ __forceinline__ double mutate_gene_sm(double parent, double u, double
     delta = __dsub_rn(pow(__dmul_rn(2.0, u), e), 1.0);
   else
     delta = __dsub_rn(1.0, pow(__dmul_rn(2.0, __dsub_rn(1.0, u)), e));
-  return fmin(fmax(__dadd_rn(parent, __dmul_rn(__dsub_rn(ub, lb), delta)), lb), ub);
+  return np_clip(__dadd_rn(parent, __dmul_rn(__dsub_rn(ub, lb), delta)), lb, ub);
 }
 
 // x_gen rows, swarm-major: [swarm p][0 .. pop) = clip(x + v) of the swarm's particles, [pop .. 2 pop) = its mutants
@@ -36,7 +36,7 @@ __global__ void smpso_generate_kernel(const double* __restrict__ parm, const dou
   double v;
   if (k < pop) {
     const int64_t row = p * pop + k;
-    v = fmin(fmax(parm[row * d + j] + vel[row * d + j], xlb[j]), xub[j]);  // update_position, SMPSO.py:311-313
+    v = np_clip(parm[row * d + j] + vel[row * d + j], xlb[j], xub[j]);  // update_position, SMPSO.py:311-313
   } else {
     const int64_t c = p * pop + (k - pop);  // child index of mutate_groups: group p, child k - pop
     Philox ph(seed);
@@ -77,7 +77,7 @@ __global__ void smpso_velocity_resident_kernel(const double* __restrict__ parm, 
   }
   const double delta = (xub[j] - xlb[j]) / 2;
   const double v = __dmul_rn(__dadd_rn(__dadd_rn(__dmul_rn(w, vel[t]), __dmul_rn(c1r1, d1)), __dmul_rn(c2r2, d2)), chi);
-  vel[t] = fmin(fmax(v, -delta), delta);
+  vel[t] = np_clip(v, -delta, delta);
 }
 
 __global__ void f32_to_f64_kernel(const float* __restrict__ a, int64_t n, double* __restrict__ out) {

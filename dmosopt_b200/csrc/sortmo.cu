@@ -182,7 +182,7 @@ __global__ void desc_key_kernel(const double* __restrict__ key, const uint32_t* 
 __global__ void rank_key_kernel(const int32_t* __restrict__ rank, const uint32_t* __restrict__ perm, int64_t n,
                                 uint32_t* __restrict__ out) {
   int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p < n) out[p] = (uint32_t)rank[perm[p]];
+  if (p < n) out[p] = (uint32_t)rank[perm[p]] ^ 0x80000000u;  // int32 order as unsigned order
 }
 
 __global__ void gather_rows_kernel(const double* __restrict__ src, const uint32_t* __restrict__ perm, int64_t keep, int w,
@@ -365,7 +365,7 @@ int euclidean_device(dmo_ctx* ctx, const double* dY, int64_t n, int M, double* d
 }
 
 int lexsort_device(dmo_ctx* ctx, const int32_t* d_rank, const double* const* d_desc_keys, int nkeys, int64_t n,
-                   uint32_t* d_perm) {
+                   uint32_t* d_perm, bool rank_below_n) {
   if (n <= 0) return DMO_OK;
   const unsigned g = (unsigned)ceil_div(n, 256);
   DevBuf<uint32_t> pa, pb, r0, r1;
@@ -389,8 +389,12 @@ int lexsort_device(dmo_ctx* ctx, const int32_t* d_rank, const double* const* d_d
   if (d_rank) {
     DMO_TRY(r0.alloc(ctx, n));
     DMO_TRY(r1.alloc(ctx, n));
-    int bits = 1;
-    while (((int64_t)1 << bits) < n + 1) ++bits;
+    // keys in [0, n) share the flipped sign bit, so their low bits alone order them; other ranks need all 32
+    int bits = 32;
+    if (rank_below_n) {
+      bits = 1;
+      while (((int64_t)1 << bits) < n + 1) ++bits;
+    }
     DMO_LAUNCH(rank_key_kernel, g, 256, 0, d_rank, pin, n, r0.p);
     DMO_TRY(prim_sort_pairs_u32(ctx, r0.p, r1.p, pin, pout, n, 0, bits));
     uint32_t* t = pin;
@@ -427,7 +431,7 @@ static int order_mo_device(dmo_ctx* ctx, const double* dY, int64_t n, int M, int
   } else if (metric != DMO_METRIC_NONE) {
     return dmo_fail(ctx, DMO_ERR_ARG, "order_mo: unknown metric %d", metric);
   }
-  DMO_TRY(lexsort_device(ctx, rank.p, keys, nk, n, perm.p));
+  DMO_TRY(lexsort_device(ctx, rank.p, keys, nk, n, perm.p, true));
   return DMO_OK;
 }
 

@@ -14,13 +14,14 @@ enum Purpose : uint64_t { P_TOURNAMENT = 1, P_DECIDE = 2, P_PAIR = 3, P_SINGLE =
 
 __device__ __forceinline__ uint64_t ctr_hi(uint64_t stream_id, uint64_t purpose) { return (stream_id << 8) | purpose; }
 
-// open-interval uniform (0,1): never 0 so that log(-log(u)) is finite
+// uniform in (0, 1]: never 0, so that -log(u) stays finite.  The top of the grid, (2^53 - 1) + 0.5, rounds to 2^53:
+// once in 2^53 draws u == 1.0, and that candidate's key is +inf (it is drawn first)
 __device__ __forceinline__ double u01_open(uint32_t hi, uint32_t lo) {
   return ((double)((((uint64_t)(hi >> 5)) << 26) | (uint64_t)(lo >> 6)) + 0.5) * (1.0 / 9007199254740992.0);
 }
 
 // ---- operators (float64, NumPy operation order, no FMA contraction) -----------------------------
-__device__ __forceinline__ double clip(double x, double lo, double hi) { return fmin(fmax(x, lo), hi); }
+__device__ __forceinline__ double clip(double x, double lo, double hi) { return np_clip(x, lo, hi); }
 
 // MOEA.py:204-211
 __device__ __forceinline__ double mutate_gene(double parent, double u, double di, double lb, double ub, double rate) {
@@ -247,7 +248,7 @@ int dmo_tournament(dmo_ctx* ctx, const int32_t* rank, const double* crowd, int64
   DMO_TRY(k0.alloc(ctx, pop));
   DMO_TRY(k1.alloc(ctx, pop));
   const double* keys[1] = {icr.d};
-  DMO_TRY(lexsort_device(ctx, ir.d, keys, crowd ? 1 : 0, pop, order.p));
+  DMO_TRY(lexsort_device(ctx, ir.d, keys, crowd ? 1 : 0, pop, order.p, false));  // caller ranks: any int32
   DMO_LAUNCH(gumbel_keys_kernel, (unsigned)ceil_div(pop, 256), 256, 0, pop, seed, stream_id, log(0.5), k0.p, i0.p,
              ou.d);
   DMO_TRY(prim_sort_pairs_u64(ctx, k0.p, k1.p, i0.p, i1.p, pop, 0, 64));
@@ -312,7 +313,8 @@ int dmo_nsga2_generate(dmo_ctx* ctx, const double* pop_x, int64_t npop, int d, c
   DMO_TRY(flags.alloc(ctx, T));
   DMO_TRY(parents.alloc(ctx, 3 * T));
   DMO_TRY(nch.alloc(ctx, 1));
-  DMO_CUDA(cudaMemsetAsync(nch.p, 0xFF, sizeof(int64_t), ctx->stream));  // -1 = loop never finished
+  // -1 = loop never finished; popsize 1: `while count < popsize - 1` never runs, no children
+  DMO_CUDA(cudaMemsetAsync(nch.p, popsize > 1 ? 0xFF : 0, sizeof(int64_t), ctx->stream));
   DMO_CUDA(cudaMemsetAsync(okind.d, 0xFF, cap * sizeof(int32_t), ctx->stream));
   DMO_LAUNCH(plan_kernel, (unsigned)ceil_div(T + 1, 256), 256, 0, T, poolsize, crossover_prob, mutation_prob, seed,
              stream_id, count.p, flags.p, parents.p, odraws.d);

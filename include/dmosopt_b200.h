@@ -136,6 +136,7 @@ int dmo_remove_worst_pair_keys(dmo_ctx* ctx, const double* Xa, const double* Ya,
  * lexsort(metrics) (rank primary; AGE-MOEA adds -crowd_dist as secondary,
  * AGEMOEA.py:140-142), P(i-th best) ~ p (1-p)^i, poolsize draws WITHOUT replacement.
  * Implemented in log space (Gumbel-top-k), so it does not underflow for pop > 2150.
+ * rank may hold any int32 values (negative, or >= pop), ordered ascending as np.lexsort does.
  * crowd may be NULL.  u_out (pop,) optionally receives the uniforms used, in candidate
  * order position (for distribution / replay tests). */
 int dmo_tournament(dmo_ctx* ctx, const int32_t* rank, const double* crowd, int64_t pop,
@@ -159,7 +160,7 @@ int dmo_sbx_u(dmo_ctx* ctx, const double* parent1, const double* parent2, const 
  * planned in parallel from counter-based Philox4x32-10 draws (seed, stream_id).
  * pop_x (npop, d); pool_idx (poolsize,) rows of pop_x forming the mating pool.
  * x_gen has room for popsize+1 rows; child_kind (popsize+1,) gets 0/1 = SBX child 1/2,
- * 2 = mutant; n_children the number of rows produced.
+ * 2 = mutant; n_children the number of rows produced (0 for popsize 1, where the loop does not run).
  * draws (optional, may be NULL): receives the random draws actually used so the CPU
  * oracle can replay them: T * (5 + 2 d) doubles, T = dmo_nsga2_plan_length(...) planned
  * iterations, layout documented in dmosopt_b200/_lib.py (nsga2_generate).
