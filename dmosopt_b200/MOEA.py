@@ -9,11 +9,13 @@ Mirrors ``dmosopt/MOEA.py`` (reference @ 5cd63e4c):
   * ``tournament_selection``         MOEA.py:375-395  -> dmo_tournament (log-space, scales past pop 2150)
   * ``mutation / crossover_sbx``     MOEA.py:191-239  -> dmo_mutation_u / dmo_sbx_u
   * ``get_duplicates / remove_duplicates``  MOEA.py:426-442 -> dmo_get_duplicates
+  * ``EpsilonSort``                  MOEA.py:470-595  -> dmo_epsilon_sort (rows buffered, resolved in one call)
 
 All numerical work happens on the GPU through ``_lib``; this module only adapts shapes, dtypes and
 the reference's calling conventions.
 """
 
+import math
 from typing import Any, Dict, Optional, Tuple
 
 import numpy as np
@@ -305,3 +307,73 @@ def remove_duplicates(population_parm, population_obj, eps=1e-16):
     """MOEA.remove_duplicates (MOEA.py:440-442)."""
     dup = get_duplicates(population_parm, eps=eps)
     return population_parm[~dup, :], population_obj[~dup, :]
+
+
+class EpsilonSort:
+    """MOEA.EpsilonSort (MOEA.py:470-595): an archive of epsilon-nondominated solutions with tag-along data.
+
+    Same interface (``epsilons``, ``itobj``, ``archive``, ``tagalongs``, ``boxes``, ``add``, ``remove``, ``sortinto``), at
+    most ``_lib.EPSILON_MAX_OBJECTIVES`` objectives.  ``sortinto`` only buffers its row (it still raises OverflowError
+    at once where the reference's would); reading ``archive`` / ``tagalongs`` / ``boxes``, or calling ``add`` /
+    ``remove``, sorts the buffered rows together with the current archive in one ``dmo_epsilon_sort`` call.  That gives
+    the archive of one-by-one insertion: a row that left the archive loses again to whatever displaced it.
+    """
+
+    def __init__(self, epsilons):
+        if len(epsilons) > _lib.EPSILON_MAX_OBJECTIVES:
+            raise ValueError(f"dmosopt_b200.EpsilonSort: {len(epsilons)} objectives; dmo_epsilon_sort takes at most {_lib.EPSILON_MAX_OBJECTIVES}")
+        self.epsilons = [e if e != 0 and not np.isnan(e) else 1e-8 for e in epsilons]
+        self.itobj = range(len(epsilons))
+        self._eps = np.array(self.epsilons, dtype=np.float64)
+        self._archive, self._tagalongs, self._boxes = [], [], []
+        self._pending = []  # (objectives, tagalong) not yet sorted in
+
+    @property
+    def archive(self):
+        self._resolve()
+        return self._archive
+
+    @property
+    def tagalongs(self):
+        self._resolve()
+        return self._tagalongs
+
+    @property
+    def boxes(self):
+        self._resolve()
+        return self._boxes
+
+    def add(self, objectives, tagalong, ebox):
+        """add a solution to the archive, plus auxiliary information"""
+        self._resolve()
+        self._archive.append(objectives)
+        self._tagalongs.append(tagalong)
+        self._boxes.append(ebox)
+
+    def remove(self, index):
+        """remove a solution from the archive"""
+        self._resolve()
+        self._archive.pop(index)
+        self._tagalongs.pop(index)
+        self._boxes.pop(index)
+
+    def sortinto(self, objectives, tagalong=None):
+        """Sort a solution into the archive (minimisation); ``tagalong`` is kept with it while it stays."""
+        objectives = np.nan_to_num(objectives)
+        with np.errstate(over="ignore"):
+            if np.isinf(np.asarray(objectives[: len(self._eps)], dtype=np.float64) / self._eps).any():
+                raise OverflowError("cannot convert float infinity to integer")
+        self._pending.append((objectives, tagalong))
+
+    def _resolve(self):
+        if not self._pending:
+            return
+        rows = self._archive + [o for o, _ in self._pending]
+        tags = self._tagalongs + [t for _, t in self._pending]
+        self._pending = []
+        M = len(self._eps)
+        Y = np.array([np.asarray(r, dtype=np.float64)[:M] for r in rows])
+        keep = _lib.epsilon_sort(Y, self._eps)
+        self._archive = [rows[i] for i in keep]
+        self._tagalongs = [tags[i] for i in keep]
+        self._boxes = [[math.floor(v) for v in b] for b in np.floor(Y[keep] / self._eps)]

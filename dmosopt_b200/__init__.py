@@ -9,7 +9,9 @@ Plugin import paths (dmosopt resolves them with ``config.import_object_by_path``
     surrogate_custom_training = "dmosopt_b200.feasibility.train_with_feasibility"   (a GPU logistic feasibility model)
 
 ``dmosopt_b200.install()`` additionally routes the controller-side helpers that dmosopt calls on its own modules
-(resample / get_best duplicates + sort, per-generation termination hypervolume) to the same kernels.
+(resample / get_best duplicates + sort, per-generation termination hypervolume, the epsilon-nondominated archive of
+epsilon_get_best) to the same kernels.  ``dmosopt_b200.MOEA.EpsilonSort`` and ``dmosopt_b200.MOASMO.epsilon_get_best``
+are the GPU archive's own mirrors of the reference's.
 
 Importing the package does not touch CUDA; the first numerical call loads
 ``libdmosopt_b200.so`` and creates the context, and fails loudly when either
@@ -31,7 +33,8 @@ from .feasibility import LogisticFeasibilityModel, train_with_feasibility  # noq
 
 def install(package="dmosopt"):
     """Route the reference controller's own hot helpers (resample duplicates / crowding, get_best, termination
-    hypervolume, dda_ens) to the GPU library: see dmosopt_b200/patch.py.  Opt-in; nothing is patched on import."""
+    hypervolume, dda_ens, EpsilonSort) to the GPU library: see dmosopt_b200/patch.py.  Opt-in; nothing is patched on
+    import."""
     from . import patch
 
     return patch.install(package)

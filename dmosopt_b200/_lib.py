@@ -114,6 +114,7 @@ _SIGNATURES = {
     "dmo_ehvi_select": (_c_int, [_vp, _vp, _c_i64, _vp, _vp, _c_i64, _c_int, _vp, _c_int, _c_i64, _vp, _vp]),
     "dmo_get_duplicates": (_c_int, [_vp, _vp, _c_i64, _c_int, _c_dbl, _vp]),
     "dmo_get_duplicates_pair": (_c_int, [_vp, _vp, _c_i64, _vp, _c_i64, _c_int, _c_dbl, _vp]),
+    "dmo_epsilon_sort": (_c_int, [_vp, _vp, _c_i64, _c_int, _vp, _vp, ctypes.POINTER(_c_i64)]),
     "dmo_age_survival": (_c_int, [_vp, _vp, _vp, _c_i64, _c_int, _c_dbl, _vp, _c_int, _vp]),
     "dmo_smpso_velocity": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_int, _c_i64, _c_int, _c_dbl, _c_dbl, _c_dbl, _c_dbl, _c_dbl, _c_dbl, _vp, _vp, _vp]),
     "dmo_mutate_groups": (_c_int, [_vp, _vp, _c_i64, _c_i64, _c_i64, _c_int, _vp, _vp, _vp, _c_dbl, _c_u64, _c_u64, _vp, _vp]),
@@ -1280,6 +1281,31 @@ def get_duplicates(X, eps=1e-16, Y=None):
         assert Y.ndim == 2 and Y.shape[1] == d, (X.shape, Y.shape)
         _check(load_library().dmo_get_duplicates_pair(context(), _in(X), n, _in(Y), Y.shape[0], d, float(eps), _ptr(out)), "dmo_get_duplicates_pair")
     return out.astype(bool)
+
+
+ERR_OVERFLOW = 6  # DMO_ERR_OVERFLOW
+EPSILON_MAX_OBJECTIVES = 16  # dmo_epsilon_sort (csrc/epsilon.cu)
+
+
+def epsilon_sort(Y, eps):
+    """Ascending int64 row indices of the epsilon-nondominated archive of Y's rows (MOEA.EpsilonSort fed every row in
+    order, dmosopt/MOEA.py:470-595).  Rows sort on their first len(eps) columns; an eps of 0 or NaN counts as 1e-8.
+    Raises OverflowError when some y / eps overflows, where the reference's math.floor does."""
+    eps = _f64(eps).reshape(-1)
+    M = eps.shape[0]
+    Y = _f64(Y)
+    if Y.ndim != 2 or Y.shape[1] < M:
+        raise ValueError(f"epsilon_sort: Y must be (n, >= {M}) for {M} epsilons, got shape {Y.shape}")
+    if Y.shape[1] != M:
+        Y = np.ascontiguousarray(Y[:, :M])
+    n = Y.shape[0]
+    idx = np.empty(n, dtype=np.int64)
+    count = _c_i64(0)
+    st = load_library().dmo_epsilon_sort(context(), _ptr(Y), n, M, _ptr(eps), _ptr(idx), ctypes.byref(count))
+    if st == ERR_OVERFLOW:
+        raise OverflowError(_lib.dmo_last_error(_ctx).decode())
+    _check(st, "dmo_epsilon_sort")
+    return idx[: count.value]
 
 
 # --------------------------------------------------------------------------- A11 AGE-MOEA

@@ -251,6 +251,14 @@ int rank_nd_device(dmo_ctx* ctx, const double* dY, int64_t n, int M, int32_t* d_
 int rank_nd_device_keep(dmo_ctx* ctx, const double* dY, int64_t n, int M, int64_t keep, int32_t* d_rank);
 // 0 for non-dominated rows, non-zero otherwise (no ranks: no dependency chain)
 int nondominated_flags_device(dmo_ctx* ctx, const double* dY, int64_t n, int M, int32_t* d_flag01);
+// flag[i] = 1 iff row i is non-dominated (identical rows do not dominate each other); flag holds n + 1 entries, flag[n] = 0
+int nondominated_keep_flags(dmo_ctx* ctx, const double* dF, int64_t n, int M, DevBuf<int32_t>& flag);
+// steps 1 and 2 of the rank (csrc/rank.cu): R[j * n + i] = dense id of Y[i, j] (order- and equality-preserving, -0.0 ==
+// +0.0; 1 <= M <= 16), maxid[j] = its largest id; and the stable lexicographic order of the id vectors (sshift = 0), ties in
+// ascending row order, *perm (position -> row) pointing into permA or permB
+int dense_ids(dmo_ctx* ctx, const double* dY, int64_t n, int M, DevBuf<uint32_t>& R, DevBuf<uint32_t>& maxid);
+int lex_order(dmo_ctx* ctx, const uint32_t* R, int64_t n, int M, int sshift, DevBuf<uint32_t>& permA, DevBuf<uint32_t>& permB,
+              const uint32_t** perm);
 int crowding_device(dmo_ctx* ctx, const double* dY, int64_t n, int M, double* dD);
 int euclidean_device(dmo_ctx* ctx, const double* dY, int64_t n, int M, double* dD);
 // perm (uint32, n) sorted by (rank asc, then each desc key descending, stable on index).  rank_below_n: the ranks are

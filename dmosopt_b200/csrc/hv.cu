@@ -462,6 +462,8 @@ int compact_rows(dmo_ctx* ctx, const double* dF, int64_t n, int M, DevBuf<int32_
 
 int sort_by_column(dmo_ctx* ctx, const double* dF, int64_t n, int M, int j, DevBuf<uint32_t>& sidx);
 
+}  // namespace
+
 // flag[i] = 1 iff row i is rank 0 (identical vectors are mutually non-dominating), flag[n] = 0; flag holds n + 1 entries
 int nondominated_keep_flags(dmo_ctx* ctx, const double* dF, int64_t n, int M, DevBuf<int32_t>& flag) {
   DevBuf<uint32_t> sidx;
@@ -487,6 +489,8 @@ int nondominated_keep_flags(dmo_ctx* ctx, const double* dF, int64_t n, int M, De
   }
   return DMO_OK;
 }
+
+namespace {
 
 // rank-0 subset of a device point set (identical vectors are mutually non-dominating and are all kept)
 int nondominated_subset(dmo_ctx* ctx, const double* dF, int64_t n, int M, DevBuf<double>& out, int64_t* count) {

@@ -1247,6 +1247,8 @@ int rank_by_peeling(dmo_ctx* ctx, const uint32_t* R, const uint32_t* maxid, int6
   return DMO_OK;
 }
 
+}  // namespace
+
 // ------------------------------------------------------------------------------------------------ stages of the rank
 // 1. R[j * n + i] = dense id of Y[i, j] (order- and equality-preserving), maxid[j] = largest id of objective j
 int dense_ids(dmo_ctx* ctx, const double* dY, int64_t n, int M, DevBuf<uint32_t>& R, DevBuf<uint32_t>& maxid) {
@@ -1275,27 +1277,22 @@ int dense_ids(dmo_ctx* ctx, const double* dY, int64_t n, int M, DevBuf<uint32_t>
   return DMO_OK;
 }
 
-// 2. An order of the points in which a point can only be dominated by points before it, the group ids of identical
-//    vectors, and the chain's padded records in that order.  sshift == 0: lexicographic order (LSD passes, least
-//    significant objective first); sshift > 0: the segmented order of RankSeg, key = (objective-1 id >> sshift,
-//    objective 2, ..., objective M, objective 1).
-struct RankOrder {
-  DevBuf<uint32_t> permA, permB, rec;
-  const uint32_t* perm = nullptr;  // position -> row
-  int64_t nblocks = 0, npad = 0;
-};
-
-int rank_order(dmo_ctx* ctx, const uint32_t* R, int64_t n, int M, int sshift, RankOrder& o) {
+// 2. An order of the points in which a point can only be dominated by points before it.  sshift == 0: lexicographic
+//    order (LSD passes, least significant objective first); sshift > 0: the segmented order of RankSeg, key =
+//    (objective-1 id >> sshift, objective 2, ..., objective M, objective 1).  The passes are stable and start from row
+//    order, so identical vectors stay in ascending row order.  *perm (position -> row) points into permA or permB.
+int lex_order(dmo_ctx* ctx, const uint32_t* R, int64_t n, int M, int sshift, DevBuf<uint32_t>& permA, DevBuf<uint32_t>& permB,
+              const uint32_t** perm) {
   const int bits = bits_for(n);
   const unsigned g = (unsigned)ceil_div(n, 256);
-  DevBuf<uint32_t> keyA, keyB, gid;
-  DMO_TRY(o.permA.alloc(ctx, n));
-  DMO_TRY(o.permB.alloc(ctx, n));
+  DevBuf<uint32_t> keyA, keyB;
+  DMO_TRY(permA.alloc(ctx, n));
+  DMO_TRY(permB.alloc(ctx, n));
   DMO_TRY(keyA.alloc(ctx, n));
   DMO_TRY(keyB.alloc(ctx, n));
-  DMO_TRY(prim_iota_u32(ctx, o.permA.p, n));
-  uint32_t* pin = o.permA.p;
-  uint32_t* pout = o.permB.p;
+  DMO_TRY(prim_iota_u32(ctx, permA.p, n));
+  uint32_t* pin = permA.p;
+  uint32_t* pout = permB.p;
   auto sort_pass = [&](const uint32_t* col, int shift, int nbits) -> int {
     if (shift == 0) {
       DMO_LAUNCH(gather_u32_kernel, g, 256, 0, col, pin, n, keyA.p);
@@ -1315,12 +1312,29 @@ int rank_order(dmo_ctx* ctx, const uint32_t* R, int64_t n, int M, int sshift, Ra
   } else {
     for (int j = M - 1; j >= 0; --j) DMO_TRY(sort_pass(R + (size_t)j * n, 0, bits));
   }
-  o.perm = pin;
+  *perm = pin;
+  return DMO_OK;
+}
+
+namespace {
+
+// The order of lex_order, the group ids of identical vectors, and the chain's padded records in that order.
+struct RankOrder {
+  DevBuf<uint32_t> permA, permB, rec;
+  const uint32_t* perm = nullptr;  // position -> row
+  int64_t nblocks = 0, npad = 0;
+};
+
+int rank_order(dmo_ctx* ctx, const uint32_t* R, int64_t n, int M, int sshift, RankOrder& o) {
+  const unsigned g = (unsigned)ceil_div(n, 256);
+  DMO_TRY(lex_order(ctx, R, n, M, sshift, o.permA, o.permB, &o.perm));
 
   // group ids (identical vectors share one)
+  DevBuf<uint32_t> flag, gid;
+  DMO_TRY(flag.alloc(ctx, n));
   DMO_TRY(gid.alloc(ctx, n));
-  DMO_LAUNCH(flag_new_vec_kernel, g, 256, 0, R, o.perm, n, M, keyA.p);
-  DMO_TRY(prim_inclusive_sum_u32(ctx, keyA.p, gid.p, n));
+  DMO_LAUNCH(flag_new_vec_kernel, g, 256, 0, R, o.perm, n, M, flag.p);
+  DMO_TRY(prim_inclusive_sum_u32(ctx, flag.p, gid.p, n));
 
   const int W = 4 * ((M + 1 + 3) / 4);
   o.nblocks = ceil_div(n, RANK_T);

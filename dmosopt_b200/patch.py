@@ -12,6 +12,10 @@ called by the reference's controller code directly on its own modules, so swappi
                                           Monte-Carlo branches for 2 .. 16 objectives (hv.HV_MC_DEFAULT_SEED,
                                           consecutive calls on consecutive streams); the rest stays with the reference
   * the rank function of every ``sortMO`` ``dmosopt.dda.dda_ens`` (dmosopt/dda.py:97-152)
+  * ``MOASMO.epsilon_get_best``           ``MOEA.get_duplicates(y)`` + ``MOEA.EpsilonSort`` (dmosopt/MOASMO.py:703-758,
+                                          dmosopt/MOEA.py:470-595): ``MOEA.EpsilonSort`` becomes a factory that builds
+                                          this package's lazy archive for up to 16 objectives and the reference's own
+                                          class for wider archives
 
 ``install()`` rebinds exactly those module attributes of an already importable ``dmosopt`` package to the functions of
 this package (same signatures, same results: see tests/test_gpu_reference_loop.py) and ``uninstall()`` restores them.
@@ -56,6 +60,15 @@ def install(package="dmosopt"):
             if hasattr(mod, name):
                 _set(mod, name, getattr(_ind, name))
     _set(dda, "dda_ens", _dda_ens)
+    if hasattr(moea, "EpsilonSort"):
+        reference_epsilon_sort = moea.EpsilonSort
+
+        def EpsilonSort(epsilons):
+            if len(epsilons) > _lib.EPSILON_MAX_OBJECTIVES:
+                return reference_epsilon_sort(epsilons)
+            return _MOEA.EpsilonSort(epsilons)
+
+        _set(moea, "EpsilonSort", EpsilonSort)
     if hasattr(moea, "dda_ens"):
         _set(moea, "dda_ens", _dda_ens)
 

@@ -39,6 +39,7 @@ extern "C" {
 #define DMO_ERR_STATE 3       /* object used before it was initialised          */
 #define DMO_ERR_UNSUPPORTED 4 /* valid request that this build does not cover   */
 #define DMO_ERR_INTERNAL 5    /* watchdog / consistency check tripped           */
+#define DMO_ERR_OVERFLOW 6    /* dmo_epsilon_sort: some y / eps is infinite     */
 
 /* distance metrics of MOEA.sortMO (dmosopt/MOEA.py:256-266) */
 #define DMO_METRIC_NONE 0
@@ -474,6 +475,17 @@ int dmo_get_duplicates(dmo_ctx* ctx, const double* X, int64_t n, int d, double e
  * the upper triangle of cdist(X, Y) including the diagonal (MOEA.py:430). */
 int dmo_get_duplicates_pair(dmo_ctx* ctx, const double* X, int64_t n, const double* Y, int64_t ny, int d,
                             double eps, uint8_t* is_dup);
+
+/* ---- epsilon-nondominated archive ---------------------------------------------------
+ * replaces MOEA.EpsilonSort (dmosopt/MOEA.py:470-595) fed every row in order, as MOASMO.epsilon_get_best does
+ * (dmosopt/MOASMO.py:743-748).  Y (n,M) and eps (M,) host or device; 1 <= M <= 16 (DMO_ERR_ARG otherwise), n < 2^31 - 4096.
+ * An eps of 0 or NaN counts as 1e-8 (MOEA.py:509).  Per row: y = nan_to_num(row), box_j = floor(y_j / eps_j),
+ * dist = sum_j (y_j - box_j eps_j)^2 in objective order (correctly rounded squares).  The archive keeps, in every box,
+ * the row of least dist, the last one on a tie (every row's dist is NaN when some eps is infinite: the last row), of
+ * the boxes no other occupied box dominates.  idx (n,) host or device receives their row indices in ascending order,
+ * *count (host) their number.  A y_j / eps_j that overflows to +-inf (where the reference's math.floor raises
+ * OverflowError) fails with DMO_ERR_OVERFLOW and the first such row in the message. */
+int dmo_epsilon_sort(dmo_ctx* ctx, const double* Y, int64_t n, int M, const double* eps, int64_t* idx, int64_t* count);
 
 /* ---- A11: AGE-MOEA survival score (greedy part) -------------------------------------
  * replaces the O(m^2) greedy loop of AGEMOEA.survival_score (dmosopt/AGEMOEA.py:398-428):
