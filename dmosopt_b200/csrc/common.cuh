@@ -243,6 +243,7 @@ int prim_sort_pairs_u32(dmo_ctx* ctx, const uint32_t* kin, uint32_t* kout, const
                         uint32_t* vout, int64_t n, int begin_bit, int end_bit);
 int prim_inclusive_sum_u32(dmo_ctx* ctx, const uint32_t* in, uint32_t* out, int64_t n);
 int prim_exclusive_sum_i32(dmo_ctx* ctx, const int32_t* in, int32_t* out, int64_t n);
+int prim_inclusive_min_f64(dmo_ctx* ctx, const double* in, double* out, int64_t n);
 int prim_iota_u32(dmo_ctx* ctx, uint32_t* out, int64_t n);
 
 // internal device-pointer entry points shared between translation units

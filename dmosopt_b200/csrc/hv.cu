@@ -7,7 +7,7 @@
 // Hypervolume algorithm (not a transliteration of the reference's sequential local-upper-bound lists):
 //   points outside ref are dropped (hv.py:159), then only the rank-0 subset is kept (the HV of a set is the HV of
 //   its non-dominated subset).
-//   M = 2: sort by f0; the staircase strips are independent -> one parallel reduction.
+//   M = 2: sort by f0, min-scan of f1 along that order; the staircase strips are independent -> one parallel reduction.
 //   M = 3: HV = sum_k (r_z - z_k) * A_k, where A_k is the area of the xy-quadrant of k that is NOT covered by points
 //          with smaller z.  Every A_k is an independent sweep over the x-sorted points (running min of y among the
 //          points with smaller z), so the whole computation is n independent O(n) scans: thread-per-point, sources
@@ -158,15 +158,17 @@ __global__ void final_sum_kernel(const double* __restrict__ partial, int64_t nb,
   if (threadIdx.x == 0) out[0] = s[0];
 }
 
-// M = 2: points are mutually non-dominated, sidx sorts them by f0 ascending => f1 is non-increasing along the order
-__global__ void hv2_kernel(const double* __restrict__ F, const uint32_t* __restrict__ sidx, int64_t n, double r0,
-                           double r1, double* __restrict__ partial) {
+// M = 2: sidx sorts the points by f0 ascending, ymin[p] = min of f1 over sorted positions 0 .. p.  The strip over
+// [x_p, x_{p+1}) lies under the running minimum, so the sum holds for any set: f0 ties, duplicates and weakly or
+// strictly dominated rows (the ranked entry keeps such rows after a float32 rounding) add no volume.
+__global__ void hv2_kernel(const double* __restrict__ F, const uint32_t* __restrict__ sidx, const double* __restrict__ ymin,
+                           int64_t n, double r0, double r1, double* __restrict__ partial) {
   int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   double v = 0.0;
   if (p < n) {
-    const double x = F[(int64_t)sidx[p] * 2], y = F[(int64_t)sidx[p] * 2 + 1];
+    const double x = F[(int64_t)sidx[p] * 2];
     const double xn = (p + 1 < n) ? F[(int64_t)sidx[p + 1] * 2] : r0;
-    v = (xn - x) * (r1 - y);
+    v = (xn - x) * (r1 - ymin[p]);
   }
   block_sum_store(v, partial);
 }
@@ -546,7 +548,15 @@ int hv_inside_nondominated(dmo_ctx* ctx, const double* dF, int64_t n, int M, con
 // d_rank (optional, device, (n,)): non-dominated ranks of the rows within a SUPERSET they were selected from by rank
 // (dmo_remove_worst).  Rows with rank > 0 are dominated by a rank-0 row of the same set, so they add no volume and are
 // dropped without running the non-dominated filter again; this stays true after a monotone rounding of the
-// coordinates (float64 -> float32 state), which can only turn strict dominance into weak dominance.
+// coordinates (float64 -> float32 state).  The rank-0 rows kept are then not mutually non-dominated in general: the
+// rounding can make two of them tie in a coordinate, or one Pareto-dominate the other (equal f0, smaller f1).  So every
+// route behind this entry must be valid for any point set, and each is:
+//   M = 1: the minimum.  M = 2: strips under the running minimum of f1 along the f0 order (hv2_kernel).
+//   M = 3 (sweep and tree), M = 4, 5 (chain sums), M = 6 .. 8 (limit sets): the slicing identity
+//   HV(S_<=k) - HV(S_<k) = (r - z_k) * [vol(k) - HV(S_<k clipped to k)] holds for any order that is non-decreasing
+//   along the slicing axis, whatever the dominance among the points, and every lower level is evaluated by the same
+//   identity or by a staircase under a running minimum.
+// tests/test_gpu_hv_exact.py checks every route, ranked and unranked, for exact equality on dyadic inputs.
 int hypervolume_device_ranked(dmo_ctx* ctx, const double* dF, int64_t n, int M, const double* h_ref, const int32_t* d_rank,
                               double* h_out);
 
@@ -601,9 +611,13 @@ int hypervolume_device_ranked(dmo_ctx* ctx, const double* dF, int64_t n, int M, 
   DMO_TRY(sort_by_column(ctx, Fnd.p, n2, M, 0, sx));
   if (M == 2) {
     const int64_t nb = ceil_div(n2, 256);
-    DevBuf<double> partial;
+    DevBuf<double> partial, ys, ymin;
     DMO_TRY(partial.alloc(ctx, nb));
-    DMO_LAUNCH(hv2_kernel, (unsigned)nb, 256, 0, Fnd.p, sx.p, n2, h_ref[0], h_ref[1], partial.p);
+    DMO_TRY(ys.alloc(ctx, n2));
+    DMO_TRY(ymin.alloc(ctx, n2));
+    DMO_LAUNCH(gather_col_kernel, (unsigned)nb, 256, 0, Fnd.p, sx.p, n2, M, 1, ys.p);
+    DMO_TRY(prim_inclusive_min_f64(ctx, ys.p, ymin.p, n2));
+    DMO_LAUNCH(hv2_kernel, (unsigned)nb, 256, 0, Fnd.p, sx.p, ymin.p, n2, h_ref[0], h_ref[1], partial.p);
     DMO_TRY(sum_partials(ctx, partial, nb, h_out));
     return DMO_OK;
   }

@@ -54,6 +54,21 @@ int prim_exclusive_sum_i32(dmo_ctx* ctx, const int32_t* in, int32_t* out, int64_
   return DMO_OK;
 }
 
+struct MinF64 {
+  __device__ __forceinline__ double operator()(double a, double b) const { return b < a ? b : a; }
+};
+
+int prim_inclusive_min_f64(dmo_ctx* ctx, const double* in, double* out, int64_t n) {
+  if (n <= 0) return DMO_OK;
+  size_t tmp = 0;
+  DMO_CUDA(cub::DeviceScan::InclusiveScan(nullptr, tmp, in, out, MinF64{}, (int)n, ctx->stream));
+  DevBuf<uint8_t> t;
+  DMO_TRY(t.alloc(ctx, tmp));
+  DMO_CUDA(cub::DeviceScan::InclusiveScan(t.p, tmp, in, out, MinF64{}, (int)n, ctx->stream));
+  ctx->launches += 2;
+  return DMO_OK;
+}
+
 __global__ void iota_kernel(uint32_t* out, int64_t n) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) out[i] = (uint32_t)i;
