@@ -11,6 +11,7 @@ context raises.
 import ctypes
 import os
 import threading
+import weakref
 
 import numpy as np
 
@@ -249,6 +250,16 @@ def _f64(a):
     return np.ascontiguousarray(a, dtype=np.float64)
 
 
+def _per_dim(v, d):
+    """A scalar or (d,) distribution index as a (d,) float64 array."""
+    return _f64(np.broadcast_to(np.asarray(v, dtype=np.float64), (d,)))
+
+
+def _seed(seed):
+    """A seed as the library's uint64."""
+    return int(seed) & (2**64 - 1)
+
+
 # --------------------------------------------------------------------------- context utilities
 def synchronize():
     _check(load_library().dmo_synchronize(context()), "dmo_synchronize")
@@ -388,8 +399,6 @@ def _pin_release(ptr, nbytes):
 def pinned_empty(shape, dtype=np.float64):
     """NumPy array backed by page-locked host memory (pooled; recycled when the last view is collected)."""
     global _pin_pool_bytes, _pin_live_bytes
-    import weakref
-
     lib = load_library()
     context()
     dt = np.dtype(dtype)
@@ -415,6 +424,32 @@ def mirror_register(host, dev):
     _mirrors[host.ctypes.data] = (host.nbytes, dev)
 
 
+def _mirror_of(addr):
+    """(base, nbytes, DeviceArray) of the registered host block that starts at or contains ``addr``, else None."""
+    ent = _mirrors.get(addr)
+    if ent is not None:
+        return (addr,) + ent
+    for base, (nbytes, dev) in list(_mirrors.items()):  # a finaliser may drop an entry while we look
+        if base <= addr < base + nbytes:
+            return base, nbytes, dev
+    return None
+
+
+def _mirrored_out(dev, nbytes=None):
+    """Read-only host copy of ``dev`` (a DeviceArray the library has written; only its first ``nbytes`` are copied back
+    when given) that keeps ``dev`` as its device mirror.  It is page-locked while the page-locked budget lasts; past it
+    the caller is hoarding outputs, so it is pageable and its mirror is dropped with it."""
+    if _pin_live_bytes < _PIN_LIVE_LIMIT:
+        out = pinned_empty(dev.shape, dev.dtype)
+    else:
+        out = np.empty(dev.shape, dtype=dev.dtype)
+        weakref.finalize(out, _mirrors.pop, out.ctypes.data, None)
+    memcpy(out, dev.ptr, dev.nbytes if nbytes is None else nbytes)
+    mirror_register(out, dev)
+    out.flags.writeable = False
+    return out
+
+
 def mirror_drop(a):
     """Forget (and free) the device copy of ``a``: the host array stays valid, later uses simply upload it again.
 
@@ -422,16 +457,10 @@ def mirror_drop(a):
     epoch (MOASMO.optimize's history) holds host memory only, not one HBM buffer per generation."""
     if not isinstance(a, np.ndarray):
         return
-    addr = a.ctypes.data
-    ent = _mirrors.get(addr)
-    if ent is None:
-        for base, (nbytes, dev) in list(_mirrors.items()):
-            if base <= addr < base + nbytes:
-                addr, ent = base, (nbytes, dev)
-                break
-    if ent is not None:
-        _mirrors.pop(addr, None)
-        ent[1].free()
+    m = _mirror_of(a.ctypes.data)
+    if m is not None:
+        _mirrors.pop(m[0], None)
+        m[2].free()
 
 
 def mirror_upload(host):
@@ -447,14 +476,12 @@ def mirror_ptr(a, require_readonly=True):
         return None
     if require_readonly and a.flags.writeable:
         return None
-    addr = a.ctypes.data
-    ent = _mirrors.get(addr)
-    if ent is not None:
-        return ent[1].ptr if a.nbytes <= ent[0] and ent[1].ptr else None
-    for base, (nbytes, dev) in list(_mirrors.items()):  # a finaliser may drop an entry while we look
-        if base <= addr and addr + a.nbytes <= base + nbytes and dev.ptr:
-            return dev.ptr + (addr - base)
-    return None
+    m = _mirror_of(a.ctypes.data)
+    if m is None:
+        return None
+    base, nbytes, dev = m
+    off = a.ctypes.data - base
+    return dev.ptr + off if dev.ptr and off + a.nbytes <= nbytes else None
 
 
 def _in(a):
@@ -588,11 +615,13 @@ def remove_worst(X, Y, keep, metric=METRIC_NONE, extra_desc_keys=None):
     return Xo, Yo, rank.astype(np.intp), perm
 
 
-def remove_worst_pair(Xa, Ya, Xb, Yb, keep, metric=METRIC_NONE, out_X=None):
+def remove_worst_pair(Xa, Ya, Xb, Yb, keep, metric=METRIC_NONE, out_X=None, key=None):
     """remove_worst(vstack(Xa, Xb), vstack(Ya, Yb), keep) without the host-side concatenation.
 
     ``out_X`` (optional, float64 C-contiguous (keep, d)) receives the surviving rows directly; it may be the writable
     base of ``Xb``.  When ``out_X`` has a device mirror the survivors are written to the mirror and copied out once.
+    ``key`` (optional FeasModel): its rank over [Xa; Xb], evaluated on the device, is the least significant descending
+    key (MOEA.remove_worst with x_distance_metrics=[key.rank]).
     """
     Xa, Ya, Xb, Yb = _f64(Xa), _f64(Ya), _f64(Xb), _f64(Yb)
     na, d = Xa.shape
@@ -606,35 +635,11 @@ def remove_worst_pair(Xa, Ya, Xb, Yb, keep, metric=METRIC_NONE, out_X=None):
     rank = np.empty(keep, dtype=np.int32)
     perm = np.empty(keep, dtype=np.int64)
     xo_dev = mirror_ptr(Xo, require_readonly=False) if out_X is not None else None
+    fn, keys = ("dmo_remove_worst_pair", ()) if key is None else ("dmo_remove_worst_pair_keys", (key._h,))
     _check(
-        load_library().dmo_remove_worst_pair(context(), _in(Xa), _in(Ya), na, _in(Xb), _in(Yb), nb, d, M, metric, keep,
-                                             xo_dev if xo_dev is not None else _ptr(Xo), _ptr(Yo), _ptr(rank), _ptr(perm)),
-        "dmo_remove_worst_pair",
-    )
-    if xo_dev is not None:
-        memcpy(Xo, xo_dev, Xo.nbytes)
-    return Xo, Yo, rank.astype(np.intp), perm
-
-
-def remove_worst_pair_keys(Xa, Ya, Xb, Yb, keep, key, metric=METRIC_NONE, out_X=None):
-    """remove_worst_pair with the rank of the feasibility model ``key`` (FeasModel) over [Xa; Xb] evaluated on the device
-    as the least significant descending key (MOEA.remove_worst with x_distance_metrics=[key.rank])."""
-    Xa, Ya, Xb, Yb = _f64(Xa), _f64(Ya), _f64(Xb), _f64(Yb)
-    na, d = Xa.shape
-    nb = Xb.shape[0]
-    M = Ya.shape[1]
-    keep = int(min(keep, na + nb))
-    if out_X is not None and (out_X.dtype != np.float64 or not out_X.flags.c_contiguous or out_X.shape != (keep, d)):
-        out_X = None
-    Xo = out_X if out_X is not None else pinned_empty((keep, d), np.float64)
-    Yo = np.empty((keep, M), dtype=np.float64)
-    rank = np.empty(keep, dtype=np.int32)
-    perm = np.empty(keep, dtype=np.int64)
-    xo_dev = mirror_ptr(Xo, require_readonly=False) if out_X is not None else None
-    _check(
-        load_library().dmo_remove_worst_pair_keys(context(), _in(Xa), _in(Ya), na, _in(Xb), _in(Yb), nb, d, M, metric, key.handle, keep,
-                                                  xo_dev if xo_dev is not None else _ptr(Xo), _ptr(Yo), _ptr(rank), _ptr(perm)),
-        "dmo_remove_worst_pair_keys",
+        getattr(load_library(), fn)(context(), _in(Xa), _in(Ya), na, _in(Xb), _in(Yb), nb, d, M, metric, *keys, keep,
+                                    xo_dev if xo_dev is not None else _ptr(Xo), _ptr(Yo), _ptr(rank), _ptr(perm)),
+        fn,
     )
     if xo_dev is not None:
         memcpy(Xo, xo_dev, Xo.nbytes)
@@ -649,7 +654,7 @@ def tournament(rank, poolsize, seed, stream_id, crowd=None, return_uniforms=Fals
     pool = np.empty(int(poolsize), dtype=np.int64)
     u = np.empty(pop, dtype=np.float64) if return_uniforms else None
     _check(
-        load_library().dmo_tournament(context(), _ptr(rank), _ptr(cr), pop, int(poolsize), int(seed) & (2**64 - 1), int(stream_id), _ptr(pool), _ptr(u)),
+        load_library().dmo_tournament(context(), _ptr(rank), _ptr(cr), pop, int(poolsize), _seed(seed), int(stream_id), _ptr(pool), _ptr(u)),
         "dmo_tournament",
     )
     return (pool, u) if return_uniforms else pool
@@ -660,7 +665,7 @@ def mutation_u(parents, u, di_mutation, xlb, xub, mutation_rate):
     parents = np.atleast_2d(_f64(parents))
     u = np.atleast_2d(_f64(u))
     n, d = parents.shape
-    di = _f64(np.broadcast_to(np.asarray(di_mutation, dtype=np.float64), (d,)))
+    di = _per_dim(di_mutation, d)
     out = np.empty((n, d), dtype=np.float64)
     lb, ub = _f64(xlb), _f64(xub)  # named: the arrays must outlive the call
     _check(load_library().dmo_mutation_u(context(), _ptr(parents), _ptr(u), n, d, _ptr(di), _ptr(lb), _ptr(ub), float(mutation_rate), _ptr(out)), "dmo_mutation_u")
@@ -672,7 +677,7 @@ def sbx_u(parent1, parent2, u, di_crossover, xlb, xub):
     p2 = np.atleast_2d(_f64(parent2))
     u = np.atleast_2d(_f64(u))
     n, d = p1.shape
-    di = _f64(np.broadcast_to(np.asarray(di_crossover, dtype=np.float64), (d,)))
+    di = _per_dim(di_crossover, d)
     c1 = np.empty((n, d), dtype=np.float64)
     c2 = np.empty((n, d), dtype=np.float64)
     lb, ub = _f64(xlb), _f64(xub)
@@ -701,29 +706,18 @@ def nsga2_generate(pop_x, pool_idx, popsize, crossover_prob, mutation_prob, muta
     kind = np.empty(popsize + 1, dtype=np.int32)
     nch = np.zeros(1, dtype=np.int64)
     draws = np.empty(T * (5 + 2 * d), dtype=np.float64) if return_draws else None
-    dic = _f64(np.broadcast_to(np.asarray(di_crossover, dtype=np.float64), (d,)))
-    dim = _f64(np.broadcast_to(np.asarray(di_mutation, dtype=np.float64), (d,)))
+    dic, dim = _per_dim(di_crossover, d), _per_dim(di_mutation, d)
     lb, ub = _f64(xlb), _f64(xub)
     _check(
         load_library().dmo_nsga2_generate(
             context(), _in(pop_x), npop, d, _ptr(pool_idx), pool_idx.shape[0], popsize, float(crossover_prob), float(mutation_prob),
-            float(mutation_rate), _ptr(dic), _ptr(dim), _ptr(lb), _ptr(ub), int(seed) & (2**64 - 1), int(stream_id),
+            float(mutation_rate), _ptr(dic), _ptr(dim), _ptr(lb), _ptr(ub), _seed(seed), int(stream_id),
             x_dev.ptr, _ptr(kind), _ptr(nch), _ptr(draws),
         ),
         "dmo_nsga2_generate",
     )
     P = int(nch[0])
-    if _pin_live_bytes < _PIN_LIVE_LIMIT:
-        x_gen = pinned_empty((popsize + 1, d), np.float64)
-    else:  # the caller is hoarding offspring matrices: pageable memory from here on (mirror dropped with the array)
-        import weakref
-
-        x_gen = np.empty((popsize + 1, d), dtype=np.float64)
-        weakref.finalize(x_gen, _mirrors.pop, x_gen.ctypes.data, None)
-    if P:
-        memcpy(x_gen, x_dev.ptr, P * d * 8)
-    mirror_register(x_gen, x_dev)
-    x_gen.flags.writeable = False
+    x_gen = _mirrored_out(x_dev, P * d * 8)
     if not return_draws:
         return x_gen[:P], kind[:P]
     dd = {
@@ -768,7 +762,7 @@ def mtgp_lml_grad(X_train, Y, length_scale, B, D, weight, bias):
         Y = Y.reshape(-1, 1)
     M = Y.shape[1]
     assert Y.shape == (N, M), Y.shape
-    ls = _f64(np.broadcast_to(np.asarray(length_scale, dtype=np.float64).reshape(-1), (d,)))
+    ls = _per_dim(np.reshape(length_scale, -1), d)
     Bm, Dv, w, b = _f64(B).reshape(M, M), _f64(D).reshape(M), _f64(weight).reshape(M, d), _f64(bias).reshape(M)
     lml = np.empty(1)
     g = {"length_scale": np.empty(d), "B": np.empty((M, M)), "D": np.empty(M), "weight": np.empty((M, d)), "bias": np.empty(M)}
@@ -799,9 +793,53 @@ def gp_lml_grad(X_train, Y, length_scale, outputscale, noise, weight, bias):
     return lml, g
 
 
+# --------------------------------------------------------------------------- objects the library owns
+class _LibObject:
+    """Owns one library object: the handle ``_h`` (ctypes.c_void_p), released through the symbol ``_destroy`` by
+    close() or on collection.  Nothing is destroyed once the library or the main context is gone (interpreter exit)."""
+
+    _destroy = None
+    _h = None
+
+    def close(self):
+        if self._h is not None and _lib is not None and _ctx is not None:
+            getattr(_lib, self._destroy)(_ctx, self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def _predict_io(X, width, return_var):
+    """(X as (P, d) float64, page-locked mean (P, width), page-locked var (P, width) or None) of a posterior predict."""
+    X = _f64(X)
+    if X.ndim == 1:
+        X = X.reshape(1, -1)
+    mean = pinned_empty((X.shape[0], width), np.float64)
+    var = pinned_empty((X.shape[0], width), np.float64) if return_var else None
+    return X, mean, var
+
+
+class _Posterior(_LibObject):
+    """A resident posterior of ``M`` outputs whose predict symbol ``_predict`` takes (ctx, h, X, P, mean, var, precision)."""
+
+    _predict = None
+
+    def predict(self, X, return_var=True, precision=GP_FP64):
+        X, mean, var = _predict_io(X, self.M, return_var)
+        _check(getattr(load_library(), self._predict)(context(), self._h, _in(X), X.shape[0], _ptr(mean), _ptr(var), int(precision)),
+               self._predict)
+        return mean, var
+
+
 # --------------------------------------------------------------------------- A18
-class GPHandle:
+class GPHandle(_Posterior):
     """Owns a dmo_gp object (posterior state resident in HBM)."""
+
+    _destroy, _predict = "dmo_gp_destroy", "dmo_gp_predict"
 
     def __init__(self, X_train, alpha, factor, constant, length_scale, noise, y_mean, y_std, xlb, xub, kernel=KERNEL_MATERN52, factor_is_inverse=False):
         lib = load_library()
@@ -836,16 +874,6 @@ class GPHandle:
         b = _f64(np.asarray(bias, dtype=np.float64).reshape(self.M))
         _check(load_library().dmo_gp_set_linear_mean(context(), self._h, _ptr(w), _ptr(b)), "dmo_gp_set_linear_mean")
 
-    def predict(self, X, return_var=True, precision=GP_FP64):
-        X = _f64(X)
-        if X.ndim == 1:
-            X = X.reshape(1, -1)
-        P = X.shape[0]
-        mean = pinned_empty((P, self.M), np.float64)
-        var = pinned_empty((P, self.M), np.float64) if return_var else None
-        _check(load_library().dmo_gp_predict(context(), self._h, _in(X), P, _ptr(mean), _ptr(var), int(precision)), "dmo_gp_predict")
-        return mean, var
-
     def auto_info(self):
         """What precision=GP_AUTO does for this model (runs the one-off calibration if needed)."""
         mt, vt, rows = _c_int(0), _c_int(0), _c_i64(0)
@@ -865,22 +893,13 @@ class GPHandle:
                "dmo_gp_covariance_groups")
         return int(n.value), [int(g) for g in grp]
 
-    def close(self):
-        if getattr(self, "_h", None) is not None and _lib is not None and _ctx is not None:
-            _lib.dmo_gp_destroy(_ctx, self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
 
 # --------------------------------------------------------------------------- A19: multitask exact GP (MEGP_Matern)
-class MTGPHandle:
+class MTGPHandle(_Posterior):
     """Owns a dmo_mtgp object: the multitask posterior (covariance K_x (x) B + I (x) diag(D), linear mean per task)
     resident in HBM.  ``lml`` is the exact log marginal likelihood of the normalised targets."""
+
+    _destroy, _predict = "dmo_mtgp_destroy", "dmo_mtgp_predict"
 
     def __init__(self, X_train, Y, length_scale, B, D, weight, bias, y_mean, y_std, xlb, xub):
         lib = load_library()
@@ -890,7 +909,7 @@ class MTGPHandle:
             Y = Y.reshape(-1, 1)
         M = Y.shape[1]
         assert Y.shape == (N, M), Y.shape
-        ls, Bm, Dv = _f64(np.broadcast_to(np.asarray(length_scale, dtype=np.float64).reshape(-1), (d,))), _f64(B).reshape(M, M), _f64(D).reshape(M)
+        ls, Bm, Dv = _per_dim(np.reshape(length_scale, -1), d), _f64(B).reshape(M, M), _f64(D).reshape(M)
         w, b = _f64(weight).reshape(M, d), _f64(bias).reshape(M)
         ym, ys, lb, ub = _f64(y_mean).reshape(M), _f64(y_std).reshape(M), _f64(xlb).reshape(d), _f64(xub).reshape(d)
         self.N, self.d, self.M = N, d, M
@@ -903,32 +922,13 @@ class MTGPHandle:
         self._h = h
         self.lml = float(lml.value)
 
-    def predict(self, X, return_var=True, precision=GP_FP64):
-        X = _f64(X)
-        if X.ndim == 1:
-            X = X.reshape(1, -1)
-        P = X.shape[0]
-        mean = pinned_empty((P, self.M), np.float64)
-        var = pinned_empty((P, self.M), np.float64) if return_var else None
-        _check(load_library().dmo_mtgp_predict(context(), self._h, _in(X), P, _ptr(mean), _ptr(var), int(precision)), "dmo_mtgp_predict")
-        return mean, var
 
-    def close(self):
-        if getattr(self, "_h", None) is not None and _lib is not None and _ctx is not None:
-            _lib.dmo_mtgp_destroy(_ctx, self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class SVGPHandle:
+class SVGPHandle(_Posterior):
     """Owns a dmo_svgp object: the whitened variational GP posterior of L latent GPs (inducing points Zpts (L,Z,d),
     Matern-5/2 ARD kernels, q_mu (L,Z), lower-triangular q_sqrt (L,Z,Z)) mixed into M outputs by W (M,L) (None: the
     identity), resident in HBM.  ``y_var_scale`` (M,) multiplies the variance (None: y_std**2)."""
+
+    _destroy, _predict = "dmo_svgp_destroy", "dmo_svgp_predict"
 
     def __init__(self, Zpts, variance, length_scale, q_mu, q_sqrt, y_mean, y_std, xlb, xrng, W=None, jitter=1e-2, y_var_scale=None):
         lib = load_library()
@@ -957,32 +957,11 @@ class SVGPHandle:
         )
         self._h = h
 
-    def predict(self, X, return_var=True, precision=GP_FP64):
-        X = _f64(X)
-        if X.ndim == 1:
-            X = X.reshape(1, -1)
-        P = X.shape[0]
-        mean = pinned_empty((P, self.M), np.float64)
-        var = pinned_empty((P, self.M), np.float64) if return_var else None
-        _check(load_library().dmo_svgp_predict(context(), self._h, _in(X), P, _ptr(mean), _ptr(var), int(precision)), "dmo_svgp_predict")
-        return mean, var
-
     def groups(self):
         """(distinct K_* planes, operator planes) that one predict produces and contracts."""
         g, p = _c_int(0), _c_int(0)
         _check(load_library().dmo_svgp_groups(context(), self._h, ctypes.byref(g), ctypes.byref(p)), "dmo_svgp_groups")
         return int(g.value), int(p.value)
-
-    def close(self):
-        if getattr(self, "_h", None) is not None and _lib is not None and _ctx is not None:
-            _lib.dmo_svgp_destroy(_ctx, self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def svgp_optimal_q(X, y, Zpts, variance, length_scale, noise, jitter=1e-2, inducing_is_data=False):
@@ -1003,11 +982,13 @@ def svgp_optimal_q(X, y, Zpts, variance, length_scale, noise, jitter=1e-2, induc
     return q_mu, q_sqrt
 
 
-class DGPHandle:
+class DGPHandle(_LibObject):
     """Owns a dmo_dgp: the two-layer deep GP posterior of gpytorch's DSPP / DeepGP (dmo_dgp_create), resident in HBM.
     Hidden layer: Z1pts (H,Z1,d), s1 (H,), ls1 (H,d), q_mu1 (H,Z1), q_sqrt1 (H,Z1,Z1), w1 (d,), b1; last layer: Z2pts
     (T,Z2,H), s2 (T,), ls2 (T,H), q_mu2 (T,Z2), q_sqrt2 (T,Z2,Z2), c2; noise (T,) task + global noise.  quad_sites (J,H)
     selects quadrature (DSPP); None means ``n_sites`` Monte Carlo draws per predict (DeepGP)."""
+
+    _destroy = "dmo_dgp_destroy"
 
     def __init__(self, Z1pts, s1, ls1, q_mu1, q_sqrt1, w1, b1, Z2pts, s2, ls2, q_mu2, q_sqrt2, c2, noise, y_mean, y_std, xlb, xrng,
                  quad_sites=None, n_sites=None, jitter=1e-4, min_variance=1e-6):
@@ -1042,32 +1023,19 @@ class DGPHandle:
 
     def predict(self, X, seed=0, stream_id=0, return_var=True, return_eps=False, precision=GP_FP64):
         """(mean (P,T), var (P,T) or None[, eps (J,P,H)]) at the raw inputs X (P,d)."""
-        X = _f64(X)
-        if X.ndim == 1:
-            X = X.reshape(1, -1)
+        X, mean, var = _predict_io(X, self.T, return_var)
         P = X.shape[0]
-        mean = pinned_empty((P, self.T), np.float64)
-        var = pinned_empty((P, self.T), np.float64) if return_var else None
         eps = np.empty((self.J, P, self.H), np.float64) if return_eps else None
         _check(load_library().dmo_dgp_predict(context(), self._h, _in(X), P, int(seed), int(stream_id), _ptr(eps), _ptr(mean), _ptr(var),
                                               int(precision)), "dmo_dgp_predict")
         return (mean, var, eps) if return_eps else (mean, var)
 
-    def close(self):
-        if getattr(self, "_h", None) is not None and _lib is not None and _ctx is not None:
-            _lib.dmo_dgp_destroy(_ctx, self._h)
-            self._h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class SVGPFitState:
+class SVGPFitState(_LibObject):
     """Owns a dmo_svgp_fit: the training state of one GPflow variational model (L latents over the inducing points Zpts
     (Z,d), M outputs; inducing_is_data: VGP, Z = X) on X (N,d), Y (N,M), with q starting at N(0, I)."""
+
+    _destroy = "dmo_svgp_fit_destroy"
 
     def __init__(self, X, Y, Zpts, L, jitter=1e-2, inducing_is_data=False):
         X = _f64(X)
@@ -1120,23 +1088,14 @@ class SVGPFitState:
         _check(load_library().dmo_svgp_fit_q(context(), self._h, _ptr(q_mu), _ptr(q_sqrt)), "dmo_svgp_fit_q")
         return q_mu, q_sqrt
 
-    def close(self):
-        if getattr(self, "_h", None) is not None and _lib is not None and _ctx is not None:
-            _lib.dmo_svgp_fit_destroy(_ctx, self._h)
-            self._h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class DGPFitState:
+class DGPFitState(_LibObject):
     """Owns a dmo_dgp_fit: the training state of the two-layer deep GP behind MDSPP_Matern (quadrature, n_sites sites)
     and MDGP_Matern (n_sites draws per row) on X (N,d) normalised inputs and Y (N,T) normalised targets, with H hidden
     units, Z1 / Z2 inducing points per layer and batches of at most batch_max rows.  The raw vector's layout is
     dmosopt_b200.h's (model_gpytorch.deepgp_flatten builds it); it starts at zero."""
+
+    _destroy = "dmo_dgp_fit_destroy"
 
     def __init__(self, X, Y, H, Z1, Z2, n_sites, quadrature, batch_max, lengthscale_bounds=None, jitter=1e-4, min_variance=1e-6):
         X = _f64(X)
@@ -1188,17 +1147,6 @@ class DGPFitState:
                "dmo_dgp_fit_epoch")
         return out
 
-    def close(self):
-        if getattr(self, "_h", None) is not None and _lib is not None and _ctx is not None:
-            _lib.dmo_dgp_fit_destroy(_ctx, self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
 
 # --------------------------------------------------------------------------- A16/A17
 def hypervolume(F, ref, rank=None):
@@ -1245,7 +1193,7 @@ def hypervolume_mc(F, ref, algorithm="hybrid", epsilon=0.01, delta=0.25, n_sampl
     ns, nt, ran = _c_i64(0), _c_i64(0), _c_int(0)
     _check(
         load_library().dmo_hypervolume_mc(context(), _ptr(F), n, M, _ptr(ref), HVMC_ALGORITHMS[algorithm], float(epsilon), float(delta),
-                                          int(n_samples), int(seed) & (2**64 - 1), int(stream), ctypes.byref(out), ctypes.byref(ns),
+                                          int(n_samples), _seed(seed), int(stream), ctypes.byref(out), ctypes.byref(ns),
                                           ctypes.byref(nt), ctypes.byref(ran)),
         "dmo_hypervolume_mc",
     )
@@ -1342,13 +1290,13 @@ def mutate_groups(pop_x, group_size, n_groups, per_group, di_mutation, xlb, xub,
     pop_x = _f64(pop_x)
     d = pop_x.shape[1]
     total = int(n_groups) * int(per_group)
-    di = _f64(np.broadcast_to(np.asarray(di_mutation, dtype=np.float64), (d,)))
+    di = _per_dim(di_mutation, d)
     lb, ub = _f64(xlb), _f64(xub)
     out = np.empty((total, d), dtype=np.float64)
     par = np.empty(total, dtype=np.int64) if return_parents else None
     _check(
         load_library().dmo_mutate_groups(context(), _ptr(pop_x), int(group_size), int(n_groups), int(per_group), d, _ptr(di), _ptr(lb), _ptr(ub),
-                                         float(mutation_rate), int(seed) & (2**64 - 1), int(stream_id), _ptr(out), _ptr(par)),
+                                         float(mutation_rate), _seed(seed), int(stream_id), _ptr(out), _ptr(par)),
         "dmo_mutate_groups",
     )
     return (out, par) if return_parents else out
@@ -1384,17 +1332,12 @@ class SmpsoSwarms:
         """x_gen (2 * swarms * pop, d), laid out as SMPSO.py:163-184 does: the reference's float32 values, handed out as the
         float64 array MOEA.generate turns them into (np.clip against float64 bounds, MOEA.py:155) -- read-only, page-locked,
         with its device copy kept as a mirror so that evaluate(x_gen) / update(x_gen, ...) do not ship it back over PCIe."""
-        di = _f64(np.broadcast_to(np.asarray(di_mutation, dtype=np.float64), (self.d,)))
+        di = _per_dim(di_mutation, self.d)
         lb, ub = _f64(xlb), _f64(xub)
-        rows = 2 * self.swarms * self.pop
-        x_dev = DeviceArray((rows, self.d), np.float64)
+        x_dev = DeviceArray((2 * self.swarms * self.pop, self.d), np.float64)
         _check(load_library().dmo_smpso_generate(context(), self.parm.ptr, self.vel.ptr, self.swarms, self.pop, self.d, _ptr(di), _ptr(lb), _ptr(ub),
-                                                 float(mutation_rate), int(seed) & (2**64 - 1), int(stream_id), None, x_dev.ptr), "dmo_smpso_generate")
-        out = pinned_empty((rows, self.d), np.float64)
-        memcpy(out, x_dev.ptr, out.nbytes)
-        mirror_register(out, x_dev)
-        out.flags.writeable = False
-        return out
+                                                 float(mutation_rate), _seed(seed), int(stream_id), None, x_dev.ptr), "dmo_smpso_generate")
+        return _mirrored_out(x_dev)
 
     def update(self, x_gen, y_gen, scalars, xlb, xub, metric, parm_out, obj_out):
         """One update_strategy (SMPSO.py:187-238) on the resident state; writes the new float32 state into parm_out /
@@ -1575,11 +1518,7 @@ def cmaes_generate(parents_x, sigmas, A, p_idx, z, xlb, xub):
     x_dev = DeviceArray((n, d), np.float64)
     _check(load_library().dmo_cmaes_generate(context(), px.ptr, sg.ptr, cols, A.ptr, px.shape[0], _ptr(pi), _ptr(z), n, d, _ptr(lb), _ptr(ub), x_dev.ptr),
            "dmo_cmaes_generate")
-    out = pinned_empty((n, d), np.float64)
-    memcpy(out, x_dev.ptr, out.nbytes)
-    mirror_register(out, x_dev)
-    out.flags.writeable = False
-    return out
+    return _mirrored_out(x_dev)
 
 
 def cmaes_step_z(x_gen, cand_idx, parents_x, par_idx, xlb, xub, steps):
@@ -1625,17 +1564,7 @@ def _design_out(shape, write, mirror):
         return out
     dev = DeviceArray(shape, np.float64)
     write(dev.ptr)
-    if _pin_live_bytes < _PIN_LIVE_LIMIT:
-        out = pinned_empty(shape, np.float64)
-    else:  # page-locked budget spent: pageable memory (mirror dropped with the array)
-        import weakref
-
-        out = np.empty(shape, dtype=np.float64)
-        weakref.finalize(out, _mirrors.pop, out.ctypes.data, None)
-    memcpy(out, dev.ptr, out.nbytes)
-    mirror_register(out, dev)
-    out.flags.writeable = False
-    return out
+    return _mirrored_out(dev)
 
 
 def _bounds(xlb, xub, d):
@@ -1780,8 +1709,10 @@ def feas_fit(X, labels, folds, pca_mean, pca_comps, Cs, max_iter=100, tol=1e-11)
     return out
 
 
-class FeasModel:
+class FeasModel(_LibObject):
     """A fitted feasibility model held on the device (dmo_feas): J constraints over d inputs."""
+
+    _destroy = "dmo_feas_destroy"
 
     def __init__(self, k, mean, comps, smean, sscale, coef, intercept):
         k = np.ascontiguousarray(k, dtype=np.int32)
@@ -1792,10 +1723,9 @@ class FeasModel:
         assert all(a.shape == (J, d - 1) for a in arrs[1:4])
         self.d, self.J = d, J
         h = _vp()
-        self.handle = None
         _check(load_library().dmo_feas_create(context(), d, J, _ptr(k), _ptr(mean), *[_ptr(a) for a in arrs], ctypes.byref(h)),
                "dmo_feas_create")
-        self.handle = h.value
+        self._h = h
 
     def eval(self, X, rank=True, proba=False, decision=False):
         """(rank (n,), proba (J, n), decision (J, n)); the ones not asked for are None.  X may be a host array (its device
@@ -1810,13 +1740,5 @@ class FeasModel:
         r = np.empty(n) if rank else None
         p = np.empty((self.J, n)) if proba else None
         t = np.empty((self.J, n)) if decision else None
-        _check(load_library().dmo_feas_eval(context(), self.handle, _in(X), n, self.d, _ptr(r), _ptr(p), _ptr(t)), "dmo_feas_eval")
+        _check(load_library().dmo_feas_eval(context(), self._h, _in(X), n, self.d, _ptr(r), _ptr(p), _ptr(t)), "dmo_feas_eval")
         return r, p, t
-
-    def __del__(self):
-        try:
-            if self.handle and _lib is not None and _ctx is not None:
-                _lib.dmo_feas_destroy(_ctx, self.handle)
-        except Exception:
-            pass
-        self.handle = None

@@ -52,7 +52,7 @@ def remove_worst(X, Y, keep, metric=METRIC_NONE, extra_desc_keys=None):
     return X[perm], Y[perm], rank[perm], perm.astype(np.int64)
 
 
-def remove_worst_pair(Xa, Ya, Xb, Yb, keep, metric=METRIC_NONE, out_X=None):
+def remove_worst_pair(Xa, Ya, Xb, Yb, keep, metric=METRIC_NONE, out_X=None, key=None):
     Xo, Yo, rank, perm = remove_worst(np.vstack((Xa, Xb)), np.vstack((Ya, Yb)), keep, metric)
     if out_X is not None and out_X.dtype == np.float64 and out_X.shape == Xo.shape:
         out_X[:] = Xo

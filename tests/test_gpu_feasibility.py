@@ -230,7 +230,7 @@ def test_nsga2_update_with_the_device_key_equals_the_host_path(L):
     parm, obj = np.array(opt.state.population_parm), opt.state.population_obj.copy()
     xs, ys, rank, perm = remove_worst(np.vstack((x_gen, parm)), np.vstack((y_gen, obj)), pop, x_distance_metrics=[fm.rank],
                                       y_distance_metrics=None, return_perm=True)
-    xd, yd, rd, pd = L.remove_worst_pair_keys(x_gen, y_gen, parm, obj, pop, fm.device_model)
+    xd, yd, rd, pd = L.remove_worst_pair(x_gen, y_gen, parm, obj, pop, key=fm.device_model)
     assert np.array_equal(pd, perm) and np.array_equal(rd, rank) and np.array_equal(xd, xs) and np.array_equal(yd, ys)
     h0, _ = L.transfer_bytes()
     opt.update(x_gen, y_gen, state)
