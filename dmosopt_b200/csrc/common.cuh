@@ -182,6 +182,11 @@ __device__ __forceinline__ uint64_t f64_to_ordered(double x) {
   uint64_t b = (uint64_t)__double_as_longlong(x);
   return (b & 0x8000000000000000ull) ? ~b : (b | 0x8000000000000000ull);
 }
+// the same, with every NaN (either sign bit, any payload) mapped to one key above +inf: the order of NumPy's sorts, which
+// put NaN last and keep NaNs in input order.  The sort keys that mirror a NumPy sort use it; the key decodes to a NaN.
+__device__ __forceinline__ uint64_t f64_to_ordered_nan_last(double x) {
+  return isnan(x) ? 0xFFF8000000000000ull : f64_to_ordered(x);
+}
 __device__ __forceinline__ double ordered_to_f64(uint64_t k) {
   uint64_t b = (k & 0x8000000000000000ull) ? (k & 0x7fffffffffffffffull) : ~k;
   return __longlong_as_double((long long)b);

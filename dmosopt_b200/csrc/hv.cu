@@ -437,7 +437,7 @@ __global__ void neg_key_kernel(const double* __restrict__ score, int64_t n, uint
                                uint32_t* __restrict__ idx) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) {
-    keys[i] = f64_to_ordered(-score[i]);
+    keys[i] = f64_to_ordered_nan_last(-score[i]);
     idx[i] = (uint32_t)i;
   }
 }

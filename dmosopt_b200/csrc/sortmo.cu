@@ -76,7 +76,7 @@ __global__ void crowd_keys_kernel(const double* __restrict__ Y, int64_t n, int M
                                   const uint64_t* mx, uint64_t* __restrict__ keys, uint32_t* __restrict__ idx) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) {
-    keys[i] = f64_to_ordered(normalise(Y[i * M + j], mn[j], mx[j]));
+    keys[i] = f64_to_ordered_nan_last(normalise(Y[i * M + j], mn[j], mx[j]));
     idx[i] = (uint32_t)i;
   }
 }
@@ -177,7 +177,7 @@ __global__ void euclid_kernel(const double* __restrict__ Y, int64_t n, int M, co
 __global__ void desc_key_kernel(const double* __restrict__ key, const uint32_t* __restrict__ perm, int64_t n,
                                 uint64_t* __restrict__ out) {
   int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p < n) out[p] = f64_to_ordered(-key[perm[p]]);
+  if (p < n) out[p] = f64_to_ordered_nan_last(-key[perm[p]]);
 }
 __global__ void rank_key_kernel(const int32_t* __restrict__ rank, const uint32_t* __restrict__ perm, int64_t n,
                                 uint32_t* __restrict__ out) {
