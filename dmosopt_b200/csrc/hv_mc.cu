@@ -274,24 +274,21 @@ int run_fpras(dmo_ctx* ctx, const McFront& f, int64_t target, FprasState& st) {
       st.next += (uint64_t)S;
       continue;
     }
-    // the budget runs out inside this wave: find the stopping index in sample order
+    // the budget runs out inside this wave (a wave that fits whole took the branch above): find the stopping index in
+    // sample order.  Either sample s - 1 meets the target exactly, and the next round starts at sample s, or sample s
+    // straddles the target: it is discarded, its tests are spent, and the next round starts at the sample after it.
     hxi.resize((size_t)S);
     DMO_CUDA(cudaMemcpyAsync(hxi.data(), xi.p, (size_t)S * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
     DMO_CUDA(cudaStreamSynchronize(ctx->stream));
     int64_t used = 0, s = 0;
-    for (; s < S; ++s) {
+    for (; s < S && used < R; ++s) {
       if (hxi[s] == 0 || used + hxi[s] > R) break;
       used += hxi[s];
       ++st.N;
     }
     st.sum_xi += used;
-    if (s < S) {  // sample s straddles the target: discarded, its tests spent
-      st.tests = target;
-      st.next += (uint64_t)(s + 1);
-    } else {
-      st.tests += used;
-      st.next += (uint64_t)S;
-    }
+    st.tests = target;
+    st.next += (uint64_t)(used < R ? s + 1 : s);
   }
   return DMO_OK;
 }
@@ -384,6 +381,9 @@ extern "C" int dmo_hypervolume_mc(dmo_ctx* ctx, const double* F, int64_t n, int 
     return DMO_OK;
   }
   DMO_REQUIRE(nf < ((int64_t)1 << 32), "hypervolume_mc: front too large (%lld rows)", (long long)nf);
+  // dominated_wave_kernel's per-sample record holds up to nf + 1 tests in 30 bits
+  DMO_REQUIRE(algorithm == DMO_HVMC_FPRAS || algorithm == DMO_HVMC_MONTE_CARLO || nf < ((int64_t)1 << 30) - 1,
+              "hypervolume_mc: front too large for mcm2rv and hybrid (%lld rows, below 2^30 - 1 needed)", (long long)nf);
   // box volumes, W, the sampling CDF, the ideal point and U: O(n M) once, in row order on the host
   std::vector<double> hF((size_t)nf * M), cdf((size_t)nf), ideal(M);
   DMO_CUDA(cudaMemcpyAsync(hF.data(), front.p, hF.size() * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));

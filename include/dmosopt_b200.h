@@ -445,7 +445,9 @@ int dmo_nondominated_flags(dmo_ctx* ctx, const double* Y, int64_t n, int M, int3
  * reference counts; for mcm2rv and monte_carlo the rows scanned up to the first dominator of each point, plus one per
  * eta (the reference counts n rows per point, or one per point with its k-d tree); algorithm_out: the estimator that ran
  * (a DMO_HVMC_* code, _HYBRID_FPRAS / _HYBRID_MCM2RV when the hybrid decided after its FPRAS rounds); each may be NULL.
- * FPRAS budgets M1 = 8 (1 + epsilon) n ln(2 / delta) / epsilon^2 must stay below 2^34 tests (DMO_ERR_ARG otherwise). */
+ * FPRAS budgets M1 = 8 (1 + epsilon) n ln(2 / delta) / epsilon^2 must stay below 2^34 tests, and the filtered front
+ * of the mcm2rv and hybrid routes below 2^30 - 1 rows (a sample's record holds its row count in 30 bits); DMO_ERR_ARG
+ * otherwise. */
 #define DMO_HVMC_HYBRID 0
 #define DMO_HVMC_FPRAS 1
 #define DMO_HVMC_MCM2RV 2
