@@ -80,26 +80,34 @@ def l1_logistic(Z, y, C, gtol=1e-12):
 
 
 def _polish(Z, y, C, w, b, steps=8):
-    """Newton steps on the smooth problem of L-BFGS-B's support and signs (F is smooth there), kept while F does not
-    grow and no sign flips: at large C the bound-constrained search stops on its f-tolerance short of the optimum."""
+    """Newton steps on the smooth problem of L-BFGS-B's support and signs (F is smooth there), kept while no sign flips
+    and F does not grow, or grows by no more than its rounding (n eps |F|) while the gradient shrinks: at large C the
+    bound-constrained search stops on its f-tolerance short of the optimum, and near the optimum a Newton step's
+    decrease of F is below F's rounding."""
     s = np.where(y > 0, 1.0, -1.0)
     S = np.flatnonzero(w != 0.0)
     sg = np.sign(w[S])
     A = np.column_stack((Z[:, S], np.ones(len(Z))))
     F = objective(Z, y, C, w, b)
-    for _ in range(steps):
+    slack = len(Z) * np.finfo(np.float64).eps
+
+    def grad(w, b):
         t = Z @ w + b
         p = 1.0 / (1.0 + np.exp(-t))
-        g = A.T @ (C * (p - (s > 0))) + np.append(sg, 0.0)
+        return p, A.T @ (C * (p - (s > 0))) + np.append(sg, 0.0)
+
+    p, g = grad(w, b)
+    for _ in range(steps):
         H = (A * (C * p * (1 - p))[:, None]).T @ A
         step = np.linalg.solve(H, -g)
         w2 = w.copy()
         w2[S] += step[:-1]
         b2 = b + step[-1]
         F2 = objective(Z, y, C, w2, b2)
-        if F2 > F or np.any(np.sign(w2[S]) != sg):
+        p2, g2 = grad(w2, b2)
+        if np.any(np.sign(w2[S]) != sg) or F2 > F + slack * abs(F) or (F2 > F and np.max(np.abs(g2)) >= np.max(np.abs(g))):
             break
-        w, b, F = w2, b2, F2
+        w, b, F, p, g = w2, b2, F2, p2, g2
     return w, b
 
 
