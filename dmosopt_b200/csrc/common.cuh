@@ -238,6 +238,25 @@ __device__ __forceinline__ double warp_sum(double v) {
   return v;
 }
 
+// Sum of one value per thread over a CTA of NW warps in a fixed order: warp_sum in each warp, then s = 0.0 + red[0] + ...
+// + red[NW - 1] (red: NW doubles of shared memory), so repeated calls are bit-identical.  Every thread of the CTA must call
+// it, and every thread gets the result.  The barriers before the slots are written and after they are read let a caller
+// call it back to back or reuse red at once; the trailing one also completes the caller's earlier shared-memory writes.
+// Reductions that combine the warps in another order (pairwise, or a shared-memory tree) keep their own code: folding them
+// in here would change their bits.
+template <int NW>
+__device__ __forceinline__ double block_sum(double v, double* red) {
+  v = warp_sum(v);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double s = 0.0;
+#pragma unroll 8  // whole for CTAs of up to 256 threads; a whole 32-warp unroll spills in finish_fit_kernel (gp_fit.cu)
+  for (int w = 0; w < NW; ++w) s += red[w];
+  __syncthreads();
+  return s;
+}
+
 #endif  // __CUDACC__
 
 // ---------------------------------------------------------------------------
@@ -250,6 +269,15 @@ int prim_inclusive_sum_u32(dmo_ctx* ctx, const uint32_t* in, uint32_t* out, int6
 int prim_exclusive_sum_i32(dmo_ctx* ctx, const int32_t* in, int32_t* out, int64_t n);
 int prim_inclusive_min_f64(dmo_ctx* ctx, const double* in, double* out, int64_t n);
 int prim_iota_u32(dmo_ctx* ctx, uint32_t* out, int64_t n);
+// out[p] = src[idx[p]], p < n
+int prim_gather_u32(dmo_ctx* ctx, const uint32_t* src, const uint32_t* idx, int64_t n, uint32_t* out);
+// in place a[i] = (double)(float)a[i], i < n
+int prim_round_f32(dmo_ctx* ctx, double* a, int64_t n);
+// keys[i] = f64_to_ordered(F[i][j]) (-0.0 == +0.0) and idx[i] = i, i < n, of the row-major (n, M) F
+int prim_col_keys(dmo_ctx* ctx, const double* dF, int64_t n, int M, int j, uint64_t* keys, uint32_t* idx);
+// sidx (allocated here, n): the rows of F in ascending order of column j (prim_col_keys, then the radix sort), ties in row
+// order.  dense_ids (rank.cu) runs the same two steps on scratch it keeps across the objectives, and also reads the keys.
+int prim_sort_by_column(dmo_ctx* ctx, const double* dF, int64_t n, int M, int j, DevBuf<uint32_t>& sidx);
 
 // internal device-pointer entry points shared between translation units
 // (all pointers are device pointers; outputs in caller-provided device buffers)

@@ -184,20 +184,13 @@ int dmo_profile_report(dmo_ctx* ctx, char* buf, uint64_t cap) {
   return DMO_OK;
 }
 
-__global__ void round_f32_kernel(double* a, int64_t n) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) a[i] = (double)(float)a[i];
-}
-
 // in-place float64 -> float32 -> float64 rounding of a DEVICE array: what storing survivors into the
 // reference's float32 state arrays does (dmosopt/NSGA2.py:228-230 with MOASMO.py:64)
 int dmo_round_f32(dmo_ctx* ctx, double* a, int64_t n) {
   DMO_CUDA(cudaSetDevice(ctx->device));
   if (n <= 0) return DMO_OK;
   DMO_REQUIRE(a && dmo_is_device_ptr(a), "round_f32: expects a device pointer");
-  DMO_LAUNCH(round_f32_kernel, (unsigned)ceil_div(n, 256), 256, 0, a, n);
-  DMO_CHECK_LAUNCH();
-  return DMO_OK;
+  return prim_round_f32(ctx, a, n);
 }
 
 int dmo_flush_l2(dmo_ctx* ctx) {

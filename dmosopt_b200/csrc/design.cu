@@ -81,18 +81,6 @@ struct WD2 {
   }
 };
 
-// sum over the CTA in a fixed order: lanes (butterfly), then warps 0..L2_WARPS-1
-__device__ __forceinline__ double l2_block_sum(double v, double* part) {
-  v = warp_sum(v);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = 0.0;
-#pragma unroll
-  for (int w = 0; w < L2_WARPS; ++w) s += part[w];
-  return s;
-}
-
 // CTA (tile pair blockIdx.x = tk T + tj, design blockIdx.y): partial[design T^2 + tk T + tj] = weight * sum of the
 // 64 x 64 pair products; CTAs with tk > tj return at once (their slot is never read).
 template <class Src, class Metric>
@@ -144,7 +132,7 @@ __global__ void __launch_bounds__(L2_THREADS) l2_pairs_kernel(Src src, int64_t n
 #pragma unroll
     for (int b = 0; b < 4; ++b)
       if (k0 + ty + 16 * a < n && j0 + tx + 16 * b < n) acc += p[a][b];
-  const double sum = l2_block_sum(acc, part);
+  const double sum = block_sum<L2_WARPS>(acc, part);
   if (threadIdx.x == 0) partial[c * T * T + blockIdx.x] = tk == tj ? sum : 2.0 * sum;
 }
 
@@ -157,14 +145,14 @@ __global__ void __launch_bounds__(L2_THREADS) l2_finish_kernel(Src src, int64_t 
   double a = 0.0;
   for (int64_t t = threadIdx.x; t < T * T; t += L2_THREADS)
     if (t / T <= t % T) a += partial[c * T * T + t];
-  const double s3 = l2_block_sum(a, part);
+  const double s3 = block_sum<L2_WARPS>(a, part);
   double b = 0.0;
   for (int64_t k = threadIdx.x; k < n; k += L2_THREADS) {
     double q = 1.0;
     for (int i = 0; i < s; ++i) q *= Metric::row(src(c, k, i));
     b += q;
   }
-  const double s2 = l2_block_sum(b, part);
+  const double s2 = block_sum<L2_WARPS>(b, part);
   if (threadIdx.x == 0) {
     d2[c] = s2;
     d3[c] = s3;

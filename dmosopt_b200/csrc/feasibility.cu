@@ -39,17 +39,6 @@ constexpr size_t FEAS_SCORE_BYTES = size_t(1) << 31;  // score matrices of one b
 
 int64_t feas_stride(int d) { return (int64_t)d + (int64_t)(d - 1) * d + 3 * (int64_t)(d - 1) + 1; }
 
-__device__ __forceinline__ double block_sum(double v, double* part) {
-  v = warp_sum(v);
-  const int w = threadIdx.x >> 5;
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) part[w] = v;
-  __syncthreads();
-  double s = 0.0;
-  for (int k = 0; k < (int)(blockDim.x >> 5); ++k) s += part[k];
-  return s;
-}
-
 // log(1 + exp(-m)) without overflow
 __device__ __forceinline__ double log1pexp_neg(double m) { return m > 0.0 ? log1p(exp(-m)) : -m + log1p(exp(m)); }
 
@@ -93,15 +82,15 @@ __global__ void __launch_bounds__(FS_THREADS) feas_scaler_kernel(const double* _
       a += z[i * km];
       n += 1.0;
     }
-  const double cnt = block_sum(n, part);
-  const double mean = block_sum(a, part) / cnt;
+  const double cnt = block_sum<FS_WARPS>(n, part);
+  const double mean = block_sum<FS_WARPS>(a, part) / cnt;
   a = 0.0;
   for (int64_t i = threadIdx.x; i < N; i += FS_THREADS)
     if (f == FEAS_SETS - 1 || fo[i] != f) {
       const double e = z[i * km] - mean;
       a += e * e;
     }
-  const double var = block_sum(a, part) / cnt;
+  const double var = block_sum<FS_WARPS>(a, part) / cnt;
   if (threadIdx.x == 0) {
     const double eps = 2.220446049250313e-16, nm = cnt * mean * eps;
     const bool constant = var <= cnt * eps * var + nm * nm;
@@ -171,7 +160,7 @@ __global__ void __launch_bounds__(FS_THREADS) feas_solve_kernel(const double* __
       a0 += 1.0;
       a1 += y[i];
     }
-  const double ntr = block_sum(a0, part), npos = block_sum(a1, part);
+  const double ntr = block_sum<FS_WARPS>(a0, part), npos = block_sum<FS_WARPS>(a1, part);
   const int64_t out = (int64_t)p * d;
   if (npos == 0.0 || npos == ntr) {
     for (int c = tid; c < d; c += FS_THREADS) coef[out + c] = 0.0;

@@ -141,15 +141,6 @@ constexpr int KS_TN = 128;  // train points per block (one per thread)
 constexpr int KS_TP = 32;   // candidates per block
 constexpr int KS_DMAX = 64; // input dimensions held in registers
 
-__device__ __forceinline__ double stationary(double s2, int kind) {
-  // s2 = squared scaled distance r^2
-  if (kind == DMO_KERNEL_MATERN52) {
-    double K = sqrt(s2) * 2.23606797749978969641;  // sqrt(5) r
-    return (1.0 + K + K * K / 3.0) * exp(-K);
-  }
-  return exp(-0.5 * s2);
-}
-
 template <bool ISO>
 __global__ void __launch_bounds__(KS_TN) kstar_kernel(const double* __restrict__ Xn, int64_t P, int64_t p_base,
                                                       int64_t Pc, const double* __restrict__ Xt, int64_t N, int d,

@@ -58,6 +58,17 @@ struct dmo_gp {
   int64_t last_refined = 0;       // rows recomputed by the last DMO_GP_AUTO predict
 };
 
+// The float64 covariance at the squared scaled distance s2 = r^2: Matern-5/2 (1 + K + K^2 / 3) exp(-K) with K = sqrt(s2)
+// sqrt(5), or RBF exp(-s2 / 2).  gp_deep_fit.cu keeps its own Matern: it forms sqrt(5 s2), which rounds differently.  The
+// float32 helpers of the tensor paths are not this function either.
+__device__ __forceinline__ double stationary(double s2, int kind) {
+  if (kind == DMO_KERNEL_MATERN52) {
+    const double K = sqrt(s2) * 2.23606797749978969641;
+    return (1.0 + K + K * K / 3.0) * exp(-K);
+  }
+  return exp(-0.5 * s2);
+}
+
 // Candidates per chunk of any predict, whatever its memory budget allows: the K_* producers put chunk / 32 blocks on
 // the grid's y extent (at most 65535), so 2^20 keeps it at 32768.
 constexpr int64_t GP_MAX_CHUNK = (int64_t)1 << 20;

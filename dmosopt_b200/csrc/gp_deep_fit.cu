@@ -105,17 +105,6 @@ __device__ __forceinline__ double df_d2(const double* a, const double* b, int D,
   return s;
 }
 
-// fixed-order sum of one value per thread over a 256-thread block; valid in every thread
-__device__ double df_block_sum(double v, double* red) {
-  v = warp_sum(v);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = 0.0;
-  for (int w = 0; w < 8; ++w) s += red[w];
-  __syncthreads();
-  return s;
-}
-
 // One CTA per unit: Kzz and its Cholesky factor in shared memory (a non-positive pivot is recorded in info[u] and
 // replaced by 1 so that the step stays finite), Lz to global (rows of ZS), and KL_u
 __global__ void __launch_bounds__(256) dgf_factor_kernel(DfLayout L, const double* __restrict__ p, double* __restrict__ Lzg,
@@ -133,6 +122,7 @@ __global__ void __launch_bounds__(256) dgf_factor_kernel(DfLayout L, const doubl
     const int i = e / Z, j = e - i * Z;
     double val = 0.0;
     if (j <= i) {
+      // sqrt(5 d2) rounds differently from gp.cuh's stationary (sqrt(d2) sqrt(5)): the deep GP keeps its own Matern
       const double q = sqrt(5.0 * df_d2(zp + (size_t)i * D, zp + (size_t)j * D, D, il));
       val = s * ((1.0 + q + q * q / 3.0) * exp(-q));
       if (i == j) val += L.jitter;
@@ -176,8 +166,8 @@ __global__ void __launch_bounds__(256) dgf_factor_kernel(DfLayout L, const doubl
     q = fma(mu[k], mu[k], q);
     ld += log(ch[k * Z + k] * ch[k * Z + k]);
   }
-  q = df_block_sum(q, red);
-  ld = df_block_sum(ld, red);
+  q = block_sum<8>(q, red);
+  ld = block_sum<8>(ld, red);
   if (tid == 0) {
     kl[u] = 0.5 * ((q - (double)Z) - ld);
     if (bad) info[u] = bad;
@@ -399,8 +389,8 @@ __global__ void __launch_bounds__(256, 1)
     }
     Bt[e] = w;
   }
-  ks = df_block_sum(ks, red);  // synchronises: the W tile is complete
-  dl = df_block_sum(dl, red);
+  ks = block_sum<8>(ks, red);  // synchronises: the W tile is complete
+  dl = block_sum<8>(dl, red);
   const double il2 = il * il;
   double* pzc = pz + pz_base + (size_t)(u - u0) * pz_unit + (size_t)cta * Z * D;
   for (int e = tid; e < Z * D; e += 256) {
@@ -588,8 +578,8 @@ __global__ void __launch_bounds__(256) dgf_unit_bwd_kernel(DfLayout L, const dou
     dl = fma(w, r2, dl);
     S[e] = w;
   }
-  ks = df_block_sum(ks, red);
-  dl = df_block_sum(dl, red);
+  ks = block_sum<8>(ks, red);
+  dl = block_sum<8>(dl, red);
   const bool hid = u < L.H;
   const int nc = hid ? nc1 : nc2;
   const double* pzu = hid ? pz + (size_t)u * pz_unit1 : pz + pz_base2 + (size_t)(u - L.H) * pz_unit2;
@@ -651,8 +641,8 @@ __global__ void __launch_bounds__(256) dgf_assemble_kernel(DfLayout L, const dou
     a += lterm[(size_t)t * RS + r];
     cb += mbar[(size_t)(H + t) * RS + r];
   }
-  a = df_block_sum(a, red);
-  cb = df_block_sum(cb, red);
+  a = block_sum<8>(a, red);
+  cb = block_sum<8>(cb, red);
   if (tid == 0) {
     double k = 0.0;
     for (int u = 0; u < H + T; ++u) k += kl[u];
@@ -663,14 +653,14 @@ __global__ void __launch_bounds__(256) dgf_assemble_kernel(DfLayout L, const dou
   for (int t = 0; t < T; ++t) {
     double st = 0.0;
     for (int64_t r = tid; r < R2; r += 256) st += sterm[(size_t)t * RS + r];
-    st = df_block_sum(st, red);
+    st = block_sum<8>(st, red);
     if (tid == 0) g[L.otn + t] = st * df_softplus_grad(p[L.otn + t]);
     gsum += st;
   }
   if (tid == 0) g[L.on] = gsum * df_softplus_grad(p[L.on]);
   double bb = 0.0;
   for (int64_t e = tid; e < B * H; e += 256) bb += mbar[(size_t)(e % H) * RS + e / H];
-  bb = df_block_sum(bb, red);
+  bb = block_sum<8>(bb, red);
   if (tid == 0) g[L.ob] = bb;
   for (int c = tid; c < d; c += 256) {
     double acc = 0.0;

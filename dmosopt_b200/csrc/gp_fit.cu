@@ -19,14 +19,6 @@ namespace {
 
 constexpr int CB = 64;  // Cholesky block edge
 
-__device__ __forceinline__ double stationary_fit(double s2, int kind) {
-  if (kind == DMO_KERNEL_MATERN52) {
-    const double K = sqrt(s2) * 2.23606797749978969641;
-    return (1.0 + K + K * K / 3.0) * exp(-K);
-  }
-  return exp(-0.5 * s2);
-}
-
 // lower triangle (and diagonal) of K, row-major with leading dimension ld; the strict upper triangle is zeroed.
 // One CTA per 32 x 32 tile of K: the 64 rows of X it needs are staged in shared memory once (scaled by 1 / l), tiles
 // strictly above the diagonal only write zeros.  Batched over blockIdx.z: problem b has its own inv_ls (d), constant,
@@ -68,7 +60,7 @@ __global__ void __launch_bounds__(256) kernel_matrix_kernel(const double* __rest
           const double t = a[c] - b[c];
           s += t * t;
         }
-        v = constant * stationary_fit(s, kind);
+        v = constant * stationary(s, kind);
         if (i == j) v += diag_add;
       }
     } else if (i == N && j < N) {
@@ -240,25 +232,9 @@ __global__ void __launch_bounds__(SV_T) finish_fit_kernel(const double* __restri
     q += z * z;
     ld_sum += log(L[i * ld + i]);
   }
-  q = warp_sum(q);
-  ld_sum = warp_sum(ld_sum);
-  if ((tid & 31) == 0) red[tid >> 5] = q;
-  __syncthreads();
-  if (tid == 0) {
-    double s = 0.0;
-    for (int w = 0; w < SV_T / 32; ++w) s += red[w];
-    red[0] = s;
-  }
-  __syncthreads();
-  const double quad = red[0];
-  __syncthreads();
-  if ((tid & 31) == 0) red[tid >> 5] = ld_sum;
-  __syncthreads();
-  if (tid == 0) {
-    double s = 0.0;
-    for (int w = 0; w < SV_T / 32; ++w) s += red[w];
-    lml[0] = -0.5 * quad - s - 0.5 * (double)N * 1.8378770664093453;  // log(2 pi)
-  }
+  const double quad = block_sum<SV_T / 32>(q, red);
+  ld_sum = block_sum<SV_T / 32>(ld_sum, red);
+  if (tid == 0) lml[0] = -0.5 * quad - ld_sum - 0.5 * (double)N * 1.8378770664093453;  // log(2 pi)
   if (!want_alpha) return;
   // backward: L' alpha = z over the whole padded matrix with right-hand side (z, 0, 0, ...): the augmented row and the identity
   // tail get alpha = 0 and drop out, the leading N x N block is solved exactly.  Block columns from the last to the first.

@@ -115,6 +115,7 @@ __global__ void __launch_bounds__(PF_TN)
 // point) are written, whatever M.
 constexpr int PT_TN = 128, PT_TP = 32;
 
+// flushes denormal results to zero, unlike gp_tensor.cu's stationary_f (see there); the two are not interchangeable
 __device__ __forceinline__ float matern52_f(float s2) {
   float r, e;
   asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(s2));

@@ -46,18 +46,6 @@ __device__ __forceinline__ void tile_of(int t, int& ti, int& tj) {
   tj = t - ti * (ti + 1) / 2;
 }
 
-// fixed-order block sum of one value per thread (256 threads); the result is valid in thread 0
-__device__ __forceinline__ double block_sum256(double v, double* red) {
-  v = warp_sum(v);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = 0.0;
-  if (threadIdx.x == 0)
-    for (int w = 0; w < 8; ++w) s += red[w];
-  __syncthreads();
-  return s;
-}
-
 // S = sum_j lambda_j L_j^-T L_j^-1 on the tiles ti >= tj (row-major, leading dimension ld = Npad), and per tile and block
 // part[tile][j] = sum_{i,i'} K_x(i,i') A_j^-1(i,i') over the tile's lower triangle (twice off the diagonal) and
 // part[tile][M + j] = its diagonal part of tr(A_j^-1).  Linv: (M, ld, ld), zero above the diagonal and in the padding;
@@ -167,8 +155,8 @@ __global__ void __launch_bounds__(256) mt_ainv_syrk_kernel(const double* __restr
         tka = fma(wk[u][v], acc[u][v], tka);
         if (dg[u][v]) ta += acc[u][v];
       }
-    tka = block_sum256(tka, red);
-    ta = block_sum256(ta, red);
+    tka = block_sum<8>(tka, red);
+    ta = block_sum<8>(ta, red);
     if (tid == 0) {
       part[(size_t)blockIdx.x * 2 * M + jb] = tka;
       part[(size_t)blockIdx.x * 2 * M + M + jb] = ta;

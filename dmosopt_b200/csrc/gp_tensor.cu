@@ -331,7 +331,8 @@ __global__ void split_linv_kernel(const double* __restrict__ Linv, int64_t Npad,
 constexpr int KT_TN = 128, KT_TP = 32;
 
 // c * k(r): hardware approximations (sqrt.approx / ex2.approx, relative error ~2^-22 each) are inside the 2^-22 budget
-// the hi + lo fp16 split of K_* has anyway
+// the hi + lo fp16 split of K_* has anyway.  Not interchangeable with gp_multitask.cu's matern52_f: __expf keeps denormal
+// results, which its ex2.approx.ftz flushes to zero (r past about 39).
 __device__ __forceinline__ float stationary_f(float s2, int kind) {
   if (kind == DMO_KERNEL_MATERN52) {
     float r;

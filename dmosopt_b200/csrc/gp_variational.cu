@@ -78,6 +78,7 @@ __global__ void __launch_bounds__(256)
     }
 }
 
+// a shared-memory tree, not common.cuh's block_sum: the QR's results keep the bits of this order
 __device__ double block_sum_256(double s, double* red) {
   red[threadIdx.x] = s;
   __syncthreads();

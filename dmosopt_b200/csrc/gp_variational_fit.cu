@@ -40,17 +40,6 @@ constexpr int64_t SVF_ZMAX = 8192;
 constexpr double SQRT5 = 2.23606797749978969641;
 constexpr double LOG_2PI = 1.8378770664093453;
 
-// fixed-order sum of one value per thread over a 256-thread block; valid in every thread
-__device__ double svf_block_sum(double v, double* red) {
-  v = warp_sum(v);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = 0.0;
-  for (int w = 0; w < 8; ++w) s += red[w];
-  __syncthreads();
-  return s;
-}
-
 // xs[b][c] = X[idx[b]][c] inv_ls[c]  (idx NULL: row b)
 __global__ void svf_scale_rows_kernel(const double* __restrict__ X, const int64_t* __restrict__ idx, int64_t n, int d,
                                       const double* __restrict__ inv_ls, double* __restrict__ xs) {
@@ -72,8 +61,7 @@ __global__ void svf_cross_kernel(const double* __restrict__ zs, int64_t Z, const
     const double u = zs[i * d + c] - xs[b * d + c];
     s2 = fma(u, u, s2);
   }
-  const double r = sqrt(s2) * SQRT5;
-  K[t] = s * ((1.0 + r + r * r / 3.0) * exp(-r));
+  K[t] = s * stationary(s2, DMO_KERNEL_MATERN52);
 }
 
 // VGP: A[k][b] = Lz[batch[b]][k] (zero above the diagonal), Lz rows of ld
@@ -122,8 +110,8 @@ __global__ void __launch_bounds__(256) svf_kl_kernel(const double* __restrict__ 
     q = fma(m[k], m[k], q);
     ld += log(U[k * Z + k]);
   }
-  q = svf_block_sum(q, red);
-  ld = svf_block_sum(ld, red);
+  q = block_sum<8>(q, red);
+  ld = block_sum<8>(ld, red);
   if (threadIdx.x == 0) kl[blockIdx.x] = 0.5 * (q - (double)Z) - ld;
 }
 
@@ -150,8 +138,8 @@ __global__ void __launch_bounds__(256) svf_ell_kernel(const double* __restrict__
     e_acc += c0 - q / (2.0 * s2);
     g_acc += -0.5 / s2 + q / (2.0 * s2 * s2);
   }
-  e_acc = svf_block_sum(e_acc, red);
-  g_acc = svf_block_sum(g_acc, red);
+  e_acc = block_sum<8>(e_acc, red);
+  g_acc = block_sum<8>(g_acc, red);
   if (threadIdx.x == 0) {
     ell[m] = scale * e_acc;
     gnoise[m] = scale * g_acc;
@@ -178,11 +166,11 @@ __global__ void __launch_bounds__(256) svf_latent_bar_kernel(int M, int L, int64
   if (!gW) return;
   double vs = 0.0;
   for (int64_t b = threadIdx.x; b < B; b += 256) vs += v[l * B + b];
-  vs = svf_block_sum(vs, red);
+  vs = block_sum<8>(vs, red);
   for (int m = 0; m < M; ++m) {
     double s = 0.0;
     for (int64_t b = threadIdx.x; b < B; b += 256) s = fma(r[m * B + b], mu[l * B + b], s);
-    s = svf_block_sum(s, red);
+    s = block_sum<8>(s, red);
     if (threadIdx.x == 0) gW[m * L + l] = scale * (s - W[m * L + l] / noise[m] * vs);
   }
 }
@@ -241,7 +229,7 @@ __global__ void __launch_bounds__(256) svf_grad_pass_kernel(const double* __rest
         const double u = zi[c] - xj[c];
         s2 = fma(u, u, s2);
       }
-      const double r = sqrt(s2) * SQRT5, e = exp(-r);
+      const double r = sqrt(s2) * SQRT5, e = exp(-r);  // stationary()'s Matern, with exp(-r) kept for the derivative factor
       ks = fma(kb, (1.0 + r + r * r / 3.0) * e, ks);
       wv = kb * s * (5.0 / 3.0) * (1.0 + r) * e;
     }
@@ -257,7 +245,7 @@ __global__ void __launch_bounds__(256) svf_grad_pass_kernel(const double* __rest
     }
     __syncthreads();
   }
-  ks = svf_block_sum(ks, red);
+  ks = block_sum<8>(ks, red);
   if (tid < d) part[i * (d + 1) + tid] = acc;
   if (tid == 0) part[i * (d + 1) + d] = ks;
 }

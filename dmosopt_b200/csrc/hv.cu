@@ -55,22 +55,14 @@ __global__ void compact_rows_kernel(const double* __restrict__ F, int64_t n, int
   for (int j = 0; j < M; ++j) out[(int64_t)pos[i] * M + j] = F[i * M + j];
 }
 
-__global__ void col_key_kernel(const double* __restrict__ F, int64_t n, int M, int j, uint64_t* __restrict__ keys,
-                               uint32_t* __restrict__ idx) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) {
-    keys[i] = f64_to_ordered(F[i * M + j]);
-    idx[i] = (uint32_t)i;
-  }
-}
-
 __global__ void invert_perm_kernel(const uint32_t* __restrict__ sidx, int64_t n, uint32_t* __restrict__ inv) {
   int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (p < n) inv[sidx[p]] = (uint32_t)p;
 }
 
+// single block.  This kernel and final_sum_kernel reduce through a shared-memory tree, not block_sum's serial order over
+// the warps: they keep the tree so that their results keep their bits.
 __global__ void min_col_kernel(const double* __restrict__ F, int64_t n, double* out) {
-  // single block
   __shared__ double s[256];
   double m = INFINITY;
   for (int64_t i = threadIdx.x; i < n; i += blockDim.x) m = fmin(m, F[i]);
@@ -132,19 +124,6 @@ __global__ void __launch_bounds__(ND_T) nondominated_flag_kernel(const double* _
   if (blockIdx.x == 0 && threadIdx.x == 0) flag[n] = 0;
 }
 
-// deterministic block sum -> partial[blockIdx.x]
-__device__ __forceinline__ void block_sum_store(double v, double* partial) {
-  __shared__ double ws[32];
-  v = warp_sum(v);
-  if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = v;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double s = 0.0;
-    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += ws[w];
-    partial[blockIdx.x] = s;
-  }
-}
-
 __global__ void final_sum_kernel(const double* __restrict__ partial, int64_t nb, double* out) {
   __shared__ double s[256];
   double a = 0.0;
@@ -170,7 +149,9 @@ __global__ void hv2_kernel(const double* __restrict__ F, const uint32_t* __restr
     const double xn = (p + 1 < n) ? F[(int64_t)sidx[p + 1] * 2] : r0;
     v = (xn - x) * (r1 - ymin[p]);
   }
-  block_sum_store(v, partial);
+  __shared__ double red[256 / 32];
+  const double s = block_sum<256 / 32>(v, red);
+  if (threadIdx.x == 0) partial[blockIdx.x] = s;
 }
 
 // M = 3 (and the innermost level of the M >= 4 recursion).
@@ -223,18 +204,15 @@ __global__ void __launch_bounds__(HV_T) hv3_kernel(const double* __restrict__ xs
     const double excl = (rx - xk) * (ry - yk) - covered;
     v = excl * (rz - zs[k]);
   }
-  block_sum_store(v, partial);
+  __shared__ double red[HV_T / 32];
+  const double s = block_sum<HV_T / 32>(v, red);
+  if (threadIdx.x == 0) partial[blockIdx.x] = s;
 }
 
 __global__ void gather_col_kernel(const double* __restrict__ F, const uint32_t* __restrict__ sidx, int64_t n, int M,
                                   int j, double* __restrict__ out) {
   int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (p < n) out[p] = F[(int64_t)sidx[p] * M + j];
-}
-__global__ void gather_u32_kernel2(const uint32_t* __restrict__ src, const uint32_t* __restrict__ sidx, int64_t n,
-                                   uint32_t* __restrict__ out) {
-  int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p < n) out[p] = src[sidx[p]];
 }
 
 // ---- M = 4, 5: the slicing identity applied recursively ----------------------------------------------------------
@@ -321,16 +299,9 @@ __global__ void __launch_bounds__(HV_T) hv_slice_kernel(HvArrays A, int64_t n, d
       total += hprod * (A.rs[0] - clipz) * excl;
     }
   }
-  // deterministic block partial
-  __shared__ double ws[HV_T / 32];
-  double v = warp_sum(total);
-  if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = v;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double acc = 0.0;
-    for (int w = 0; w < HV_T / 32; ++w) acc += ws[w];
-    partial[(int64_t)blockIdx.x * gridDim.y + blockIdx.y] = acc;
-  }
+  __shared__ double red[HV_T / 32];
+  const double acc = block_sum<HV_T / 32>(total, red);
+  if (threadIdx.x == 0) partial[(int64_t)blockIdx.x * gridDim.y + blockIdx.y] = acc;
 }
 
 // lower-order terms: sum_k1 h1 vol(k1)  [and for M = 5: sum_{k1>k2} h1 h2 vol3(k1,k2)]
@@ -355,9 +326,13 @@ __global__ void hv_volume_terms_kernel(HvArrays A, int64_t n, double* __restrict
       }
     }
   }
-  block_sum_store(ta, partial_a);
-  __syncthreads();
-  if (D == 3) block_sum_store(tb, partial_b);
+  __shared__ double red[256 / 32];
+  const double sa = block_sum<256 / 32>(ta, red);
+  if (threadIdx.x == 0) partial_a[blockIdx.x] = sa;
+  if (D == 3) {
+    const double sb = block_sum<256 / 32>(tb, red);
+    if (threadIdx.x == 0) partial_b[blockIdx.x] = sb;
+  }
 }
 
 // ---- EHVI -----------------------------------------------------------------------------------------------
@@ -462,8 +437,6 @@ int compact_rows(dmo_ctx* ctx, const double* dF, int64_t n, int M, DevBuf<int32_
   return DMO_OK;
 }
 
-int sort_by_column(dmo_ctx* ctx, const double* dF, int64_t n, int M, int j, DevBuf<uint32_t>& sidx);
-
 }  // namespace
 
 // flag[i] = 1 iff row i is rank 0 (identical vectors are mutually non-dominating), flag[n] = 0; flag holds n + 1 entries
@@ -479,7 +452,7 @@ int nondominated_keep_flags(dmo_ctx* ctx, const double* dF, int64_t n, int M, De
     DMO_LAUNCH(rank0_flag_kernel, (unsigned)ceil_div(n + 1, 256), 256, 0, rank.p, n, flag.p);
     return DMO_OK;
   }
-  DMO_TRY(sort_by_column(ctx, dF, n, M, 0, sidx));
+  DMO_TRY(prim_sort_by_column(ctx, dF, n, M, 0, sidx));
   {
     ProfileScope ps(ctx, "nd_filter");
     if (M <= 8)
@@ -505,18 +478,6 @@ int nondominated_subset(dmo_ctx* ctx, const double* dF, int64_t n, int M, DevBuf
 __global__ void dominated_flag_kernel(const int32_t* __restrict__ keep, int64_t n, int32_t* __restrict__ out) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) out[i] = keep[i] ? 0 : 1;
-}
-
-int sort_by_column(dmo_ctx* ctx, const double* dF, int64_t n, int M, int j, DevBuf<uint32_t>& sidx) {
-  DevBuf<uint64_t> k0, k1;
-  DevBuf<uint32_t> i0;
-  DMO_TRY(k0.alloc(ctx, n));
-  DMO_TRY(k1.alloc(ctx, n));
-  DMO_TRY(i0.alloc(ctx, n));
-  DMO_TRY(sidx.alloc(ctx, n));
-  DMO_LAUNCH(col_key_kernel, (unsigned)ceil_div(n, 256), 256, 0, dF, n, M, j, k0.p, i0.p);
-  DMO_TRY(prim_sort_pairs_u64(ctx, k0.p, k1.p, i0.p, sidx.p, n, 0, 64));
-  return DMO_OK;
 }
 
 int sum_partials(dmo_ctx* ctx, DevBuf<double>& partial, int64_t nb, double* h_out) {
@@ -604,11 +565,11 @@ int hypervolume_device_ranked(dmo_ctx* ctx, const double* dF, int64_t n, int M, 
   if (M >= 6 || (M >= 4 && getenv("DMO_HV_WFG") && atoi(getenv("DMO_HV_WFG")))) {
     // 6 .. 8 objectives: limit-set recursion (hv_many.cu); DMO_HV_WFG=1 sends M = 4, 5 there too (cross-check of the chain sums)
     DevBuf<uint32_t> sl;
-    DMO_TRY(sort_by_column(ctx, Fnd.p, n2, M, M - 1, sl));
+    DMO_TRY(prim_sort_by_column(ctx, Fnd.p, n2, M, M - 1, sl));
     return hv_many_device(ctx, Fnd.p, sl.p, n2, M, dref.p, h_out);
   }
   DevBuf<uint32_t> sx;
-  DMO_TRY(sort_by_column(ctx, Fnd.p, n2, M, 0, sx));
+  DMO_TRY(prim_sort_by_column(ctx, Fnd.p, n2, M, 0, sx));
   if (M == 2) {
     const int64_t nb = ceil_div(n2, 256);
     DevBuf<double> partial, ys, ymin;
@@ -645,9 +606,9 @@ int hypervolume_device_ranked(dmo_ctx* ctx, const double* dF, int64_t n, int M, 
     for (int a = 0; a < D; ++a) {
       DMO_TRY(sc[a].alloc(ctx, n2));
       DMO_TRY(so_[a].alloc(ctx, n2));
-      DMO_TRY(sort_by_column(ctx, Fnd.p, n2, M, 2 + a, sidx_a));
+      DMO_TRY(prim_sort_by_column(ctx, Fnd.p, n2, M, 2 + a, sidx_a));
       DMO_LAUNCH(invert_perm_kernel, g4, 256, 0, sidx_a.p, n2, inv_a.p);
-      DMO_LAUNCH(gather_u32_kernel2, g4, 256, 0, inv_a.p, sx.p, n2, so_[a].p);
+      DMO_TRY(prim_gather_u32(ctx, inv_a.p, sx.p, n2, so_[a].p));
       DMO_LAUNCH(gather_col_kernel, g4, 256, 0, Fnd.p, sx.p, n2, M, 2 + a, sc[a].p);
       A.s[a] = sc[a].p;
       A.o[a] = so_[a].p;
@@ -681,7 +642,7 @@ int hypervolume_device_ranked(dmo_ctx* ctx, const double* dF, int64_t n, int M, 
   // M == 3
   DevBuf<uint32_t> sz, zinv, zo;
   DevBuf<double> xs, ys, zs;
-  DMO_TRY(sort_by_column(ctx, Fnd.p, n2, M, 2, sz));
+  DMO_TRY(prim_sort_by_column(ctx, Fnd.p, n2, M, 2, sz));
   DMO_TRY(zinv.alloc(ctx, n2));
   DMO_TRY(zo.alloc(ctx, n2));
   DMO_TRY(xs.alloc(ctx, n2));
@@ -689,7 +650,7 @@ int hypervolume_device_ranked(dmo_ctx* ctx, const double* dF, int64_t n, int M, 
   DMO_TRY(zs.alloc(ctx, n2));
   const unsigned g = (unsigned)ceil_div(n2, 256);
   DMO_LAUNCH(invert_perm_kernel, g, 256, 0, sz.p, n2, zinv.p);     // zinv[i] = position of point i along z
-  DMO_LAUNCH(gather_u32_kernel2, g, 256, 0, zinv.p, sx.p, n2, zo.p);  // ... re-indexed by x-sorted position
+  DMO_TRY(prim_gather_u32(ctx, zinv.p, sx.p, n2, zo.p));            // ... re-indexed by x-sorted position
   DMO_LAUNCH(gather_col_kernel, g, 256, 0, Fnd.p, sx.p, n2, M, 0, xs.p);
   DMO_LAUNCH(gather_col_kernel, g, 256, 0, Fnd.p, sx.p, n2, M, 1, ys.p);
   DMO_LAUNCH(gather_col_kernel, g, 256, 0, Fnd.p, sx.p, n2, M, 2, zs.p);
@@ -791,7 +752,7 @@ int dmo_ehvi_select(dmo_ctx* ctx, const double* F, int64_t nf, const double* mea
       nfr = nf;
   }
   DevBuf<uint32_t> sidx;
-  DMO_TRY(sort_by_column(ctx, front, nfr, M, 0, sidx));
+  DMO_TRY(prim_sort_by_column(ctx, front, nfr, M, 0, sidx));
   DevBuf<int32_t> flag, pos;
   DMO_TRY(flag.alloc(ctx, nfr + 2));
   DMO_TRY(pos.alloc(ctx, nfr + 2));

@@ -210,7 +210,7 @@ __global__ void __launch_bounds__(128) hv3_tree_kernel(Tree T, const double* __r
     }
     v = area * (rz - zs[k]);
   }
-  // deterministic block partial
+  // deterministic block partial: the four warps summed pairwise, not in block_sum's serial order (which would change the bits)
   __shared__ double ws[4];
   v = warp_sum(v);
   if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = v;

@@ -80,3 +80,53 @@ int prim_iota_u32(dmo_ctx* ctx, uint32_t* out, int64_t n) {
   DMO_CHECK_LAUNCH();
   return DMO_OK;
 }
+
+__global__ void gather_u32_kernel(const uint32_t* __restrict__ src, const uint32_t* __restrict__ idx, int64_t n,
+                                  uint32_t* __restrict__ out) {
+  int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p < n) out[p] = src[idx[p]];
+}
+
+int prim_gather_u32(dmo_ctx* ctx, const uint32_t* src, const uint32_t* idx, int64_t n, uint32_t* out) {
+  if (n <= 0) return DMO_OK;
+  DMO_LAUNCH(gather_u32_kernel, (unsigned)ceil_div(n, 256), 256, 0, src, idx, n, out);
+  DMO_CHECK_LAUNCH();
+  return DMO_OK;
+}
+
+__global__ void round_f32_kernel(double* a, int64_t n) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) a[i] = (double)(float)a[i];
+}
+
+int prim_round_f32(dmo_ctx* ctx, double* a, int64_t n) {
+  if (n <= 0) return DMO_OK;
+  DMO_LAUNCH(round_f32_kernel, (unsigned)ceil_div(n, 256), 256, 0, a, n);
+  DMO_CHECK_LAUNCH();
+  return DMO_OK;
+}
+
+__global__ void col_key_kernel(const double* __restrict__ F, int64_t n, int M, int j, uint64_t* __restrict__ keys,
+                               uint32_t* __restrict__ idx) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) {
+    keys[i] = f64_to_ordered(F[i * M + j]);
+    idx[i] = (uint32_t)i;
+  }
+}
+
+int prim_col_keys(dmo_ctx* ctx, const double* dF, int64_t n, int M, int j, uint64_t* keys, uint32_t* idx) {
+  DMO_LAUNCH(col_key_kernel, (unsigned)ceil_div(n, 256), 256, 0, dF, n, M, j, keys, idx);
+  return DMO_OK;
+}
+
+int prim_sort_by_column(dmo_ctx* ctx, const double* dF, int64_t n, int M, int j, DevBuf<uint32_t>& sidx) {
+  DevBuf<uint64_t> k0, k1;
+  DevBuf<uint32_t> i0;
+  DMO_TRY(k0.alloc(ctx, n));
+  DMO_TRY(k1.alloc(ctx, n));
+  DMO_TRY(i0.alloc(ctx, n));
+  DMO_TRY(sidx.alloc(ctx, n));
+  DMO_TRY(prim_col_keys(ctx, dF, n, M, j, k0.p, i0.p));
+  return prim_sort_pairs_u64(ctx, k0.p, k1.p, i0.p, sidx.p, n, 0, 64);
+}

@@ -46,15 +46,6 @@ __device__ __forceinline__ void st_release_gpu(int* p, int v) {
   asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
-__global__ void col_keys_kernel(const double* __restrict__ Y, int64_t n, int M, int j, uint64_t* __restrict__ keys,
-                                uint32_t* __restrict__ idx) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) {
-    keys[i] = f64_to_ordered(Y[i * M + j]);
-    idx[i] = (uint32_t)i;
-  }
-}
-
 __global__ void flag_new_u64_kernel(const uint64_t* __restrict__ skeys, int64_t n, uint32_t* __restrict__ flag) {
   int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (p < n) flag[p] = (p > 0 && skeys[p] != skeys[p - 1]) ? 1u : 0u;
@@ -64,12 +55,6 @@ __global__ void scatter_dense_kernel(const uint32_t* __restrict__ dense, const u
                                      uint32_t* __restrict__ R) {
   int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (p < n) R[sidx[p]] = dense[p];
-}
-
-__global__ void gather_u32_kernel(const uint32_t* __restrict__ src, const uint32_t* __restrict__ perm, int64_t n,
-                                  uint32_t* __restrict__ out) {
-  int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p < n) out[p] = src[perm[p]];
 }
 
 // flag[p] = 1 iff the vector at sorted position p differs from the one at p-1
@@ -1061,7 +1046,7 @@ int build_cell_grid(dmo_ctx* ctx, const GridIds& ids, int64_t n, int gbits, bool
   DMO_TRY(prim_iota_u32(ctx, iota.p, n));
   DMO_TRY(prim_sort_pairs_u32(ctx, key0.p, keyS.p, iota.p, ord0.p, n, 0, bits_for(n)));  // by objective-1 id ...
   for (int pass = 0; pass < 2; ++pass) {                                                // ... then stably by cell
-    DMO_LAUNCH(gather_u32_kernel, g, 256, 0, pass == 0 ? keyA.p : keyB.p, ord0.p, n, keyT.p);
+    DMO_TRY(prim_gather_u32(ctx, pass == 0 ? keyA.p : keyB.p, ord0.p, n, keyT.p));
     DMO_TRY(prim_sort_pairs_u32(ctx, keyT.p, keyS.p, ord0.p, ordS.p, n, 0, 2 * gbits));
     DMO_LAUNCH(grid_gather_kernel, g, 256, 0, ids, ordS.p, n, pass == 0 ? cg.crecA.p : cg.crecB.p, pass == 0 ? cg.slotA.p : cg.slotB.p);
     DMO_LAUNCH(grid_start_kernel, (unsigned)ceil_div(GG + 1, 256), 256, 0, keyS.p, n, GG, pass == 0 ? cg.cstartA.p : cg.cstartB.p);
@@ -1266,7 +1251,7 @@ int dense_ids(dmo_ctx* ctx, const double* dY, int64_t n, int M, DevBuf<uint32_t>
   DMO_TRY(flag.alloc(ctx, n));
   DMO_TRY(dense.alloc(ctx, n));
   for (int j = 0; j < M; ++j) {
-    DMO_LAUNCH(col_keys_kernel, g, 256, 0, dY, n, M, j, k0.p, i0.p);
+    DMO_TRY(prim_col_keys(ctx, dY, n, M, j, k0.p, i0.p));
     DMO_TRY(prim_sort_pairs_u64(ctx, k0.p, k1.p, i0.p, i1.p, n, 0, 64));
     DMO_LAUNCH(flag_new_u64_kernel, g, 256, 0, k1.p, n, flag.p);
     DMO_TRY(prim_inclusive_sum_u32(ctx, flag.p, dense.p, n));
@@ -1295,7 +1280,7 @@ int lex_order(dmo_ctx* ctx, const uint32_t* R, int64_t n, int M, int sshift, Dev
   uint32_t* pout = permB.p;
   auto sort_pass = [&](const uint32_t* col, int shift, int nbits) -> int {
     if (shift == 0) {
-      DMO_LAUNCH(gather_u32_kernel, g, 256, 0, col, pin, n, keyA.p);
+      DMO_TRY(prim_gather_u32(ctx, col, pin, n, keyA.p));
     } else {
       DMO_LAUNCH(seg_key_kernel, g, 256, 0, col, pin, n, shift, keyA.p);
     }

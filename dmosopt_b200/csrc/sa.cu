@@ -75,19 +75,6 @@ __global__ void __launch_bounds__(SA_THREADS) fast_design_kernel(int64_t N, int 
   }
 }
 
-// sum over the CTA in a fixed order: lanes (butterfly), then warps 0..SA_WARPS-1; every thread gets the result
-__device__ __forceinline__ double block_sum(double v, double* part) {
-  v = warp_sum(v);
-  const int w = threadIdx.x >> 5;
-  __syncthreads();  // part may still be read from the previous call
-  if ((threadIdx.x & 31) == 0) part[w] = v;
-  __syncthreads();
-  double s = 0.0;
-#pragma unroll
-  for (int k = 0; k < SA_WARPS; ++k) s += part[k];
-  return s;
-}
-
 // One CTA per (output m, parameter j), blockIdx.x = m d + j.  Stages yb_i = Y[base_i, m] and q2_i = ((Y[pert_ij, m] -
 // yb_i) / (X[pert_ij, j] - X[base_i, j]))^2 (shared memory when they fit, else this CTA's slice of scratch), reduces the
 // full-sample statistics, then each warp runs replicates r = warp, warp + SA_WARPS, ... over the resampled indices.
@@ -120,8 +107,8 @@ __global__ void __launch_bounds__(SA_THREADS) dgsm_stats_kernel(const double* __
     a += q2[i];
     c += yb[i];
   }
-  const double vi = block_sum(a, part) / dN;
-  const double ym = block_sum(c, part) / dN;
+  const double vi = block_sum<SA_WARPS>(a, part) / dN;
+  const double ym = block_sum<SA_WARPS>(c, part) / dN;
   a = 0.0;
   c = 0.0;
   for (int64_t i = threadIdx.x; i < N; i += SA_THREADS) {
@@ -129,8 +116,8 @@ __global__ void __launch_bounds__(SA_THREADS) dgsm_stats_kernel(const double* __
     a += e * e;
     c += f * f;
   }
-  const double vs = sqrt(block_sum(a, part) / dN);
-  const double var = block_sum(c, part) / dN;
+  const double vs = sqrt(block_sum<SA_WARPS>(a, part) / dN);
+  const double var = block_sum<SA_WARPS>(c, part) / dN;
   // replicates: one warp each, lane-strided sums then the butterfly
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int r = warp; r < R; r += SA_WARPS) {

@@ -88,11 +88,6 @@ __global__ void f64_to_f32_kernel(const double* __restrict__ a, int64_t n, float
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) out[i] = (float)a[i];
 }
-__global__ void round_f32_inplace_kernel(double* a, int64_t n) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) a[i] = (double)(float)a[i];
-}
-
 }  // namespace
 
 extern "C" {
@@ -180,8 +175,8 @@ int dmo_smpso_update(dmo_ctx* ctx, double* parm, double* obj, double* vel, const
     if (rc != DMO_OK) return rc;
   }
   // the reference assigns the survivors into float32 state arrays
-  DMO_LAUNCH(round_f32_inplace_kernel, (unsigned)ceil_div(n * d, 256), 256, 0, parm, n * d);
-  DMO_LAUNCH(round_f32_inplace_kernel, (unsigned)ceil_div(n * M, 256), 256, 0, obj, n * M);
+  DMO_TRY(prim_round_f32(ctx, parm, n * d));
+  DMO_TRY(prim_round_f32(ctx, obj, n * M));
   DMO_TRY(orank.finish(ctx));
   DMO_TRY(operm.finish(ctx));
   if (parm_f32) {
