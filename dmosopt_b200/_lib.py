@@ -40,6 +40,7 @@ _SIGNATURES = {
     "dmo_synchronize": (_c_int, [_vp]),
     "dmo_stream": (_vp, [_vp]),
     "dmo_launch_count": (_c_i64, [_vp]),
+    "dmo_wait_count": (_c_i64, [_vp]),
     "dmo_sm_count": (_c_int, [_vp]),
     "dmo_timer_begin": (_c_int, [_vp]),
     "dmo_timer_end": (_c_int, [_vp, ctypes.POINTER(ctypes.c_float)]),
@@ -274,6 +275,12 @@ def stream_ptr():
 def launch_count():
     lib = load_library()
     return int(lib.dmo_launch_count(context())) + sum(int(lib.dmo_launch_count(c)) for c in _worker_ctx)
+
+
+def wait_count():
+    """Times the library has blocked the host on its stream (a stream synchronise or a blocking copy), all contexts."""
+    lib = load_library()
+    return int(lib.dmo_wait_count(context())) + sum(int(lib.dmo_wait_count(c)) for c in _worker_ctx)
 
 
 def sm_count():

@@ -190,7 +190,7 @@ int dmo_benchmark_eval(dmo_ctx* ctx, int problem, const double* X, int64_t n, in
   DMO_LAUNCH(benchmark_kernel, (unsigned)ceil_div(n, 128), 128, 0, problem, x.d, n, n_var, n_obj, alpha, y.d);
   DMO_CHECK_LAUNCH();
   DMO_TRY(y.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 

@@ -20,11 +20,21 @@ struct dmo_ctx {
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   int sm_count = 132;  // H100 SXM; replaced by the device's count in dmo_create
   int64_t launches = 0;
+  int64_t waits = 0;  // times the host blocked on the stream (dmo_wait); dmo_wait_count() reports it
   std::string err;
   void* flush_buf = nullptr;
   size_t flush_bytes = 0;
   int* dev_flag = nullptr;  // device-side error / watchdog flag (int[4])
   uint64_t h2d_bytes = 0, d2h_bytes = 0;  // bytes staged for host buffers (In<> / Out<>)
+  // pinned slots and their events for read-backs the host waits on later than it enqueues them: [0], [1] the front peel's
+  // counts (rank.cu), [2] the fused step's GP read-back (gp.cu); created on first use (dmo_lag_slots), released by
+  // dmo_destroy
+  unsigned long long* lag_host = nullptr;
+  cudaEvent_t lag_ev[3] = {nullptr, nullptr, nullptr};
+  // side streams for independent work of one call (SideStreams below); created on first use, released by dmo_destroy
+  static constexpr int kSide = 4;
+  cudaStream_t side[kSide] = {};
+  cudaEvent_t side_ev[kSide + 1] = {};  // [0]: fork point on the main stream, [1 + s]: end of side stream s
   // optional per-kernel CUDA-event timers (dmo_profile_enable); bench.py reads them for the roofline
   bool profiling = false;
   struct Timer {
@@ -82,6 +92,31 @@ int dmo_fail(dmo_ctx* ctx, int code, const char* fmt, ...);
   } while (0)
 
 #define DMO_CHECK_LAUNCH() DMO_CUDA(cudaGetLastError())
+
+// Independent work issued on side streams of the context: side s waits for everything enqueued on the main stream
+// before the constructor, and the main stream waits for every side stream's work in the destructor.  Inside, on(s)
+// points ctx->stream at side s, so any library function called there enqueues on it (and allocates and frees its own
+// scratch there); back() returns to the main stream.  Scratch shared with the main stream is allocated before the
+// constructor and released after the destructor.  The bits do not depend on the interleaving: the streams write
+// disjoint buffers.
+struct SideStreams {
+  dmo_ctx* ctx;
+  cudaStream_t main;
+  int k = 0;
+  int rc = DMO_OK;
+  SideStreams(dmo_ctx* c, int nside);
+  ~SideStreams();
+  void on(int s) { ctx->stream = ctx->side[s]; }
+  void back() { ctx->stream = main; }
+};
+
+int dmo_lag_slots(dmo_ctx* ctx);
+
+// every host wait of the library on its stream goes through this, so that dmo_wait_count() counts them
+static inline cudaError_t dmo_wait(dmo_ctx* ctx) {
+  ctx->waits++;
+  return cudaStreamSynchronize(ctx->stream);
+}
 
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
@@ -304,6 +339,18 @@ int hypervolume_device(dmo_ctx* ctx, const double* dF, int64_t n, int M, const d
 // the same when the rows carry their non-dominated ranks within a superset (rank > 0 rows are skipped, no filter pass)
 int hypervolume_device_ranked(dmo_ctx* ctx, const double* dF, int64_t n, int M, const double* h_ref, const int32_t* d_rank,
                               double* h_out);
+// device bodies of dmo_tournament, dmo_nsga2_generate and dmo_remove_worst (variation.cu, sortmo.cu) for dmo_nsga2_step:
+// device arrays only, enqueued on the context's stream without the public entry points' trailing wait.  The generate body
+// waits once, for the offspring count it returns in *n_children.
+int tournament_device(dmo_ctx* ctx, const int32_t* d_rank, const double* d_crowd, int64_t pop, int64_t poolsize, uint64_t seed,
+                      uint64_t stream_id, int64_t* d_pool, double* d_u);
+int nsga2_generate_device(dmo_ctx* ctx, const double* d_pop_x, int d, const int64_t* d_pool, int64_t poolsize, int64_t popsize,
+                          double crossover_prob, double mutation_prob, double mutation_rate, const double* d_dic,
+                          const double* d_dim, const double* d_xlb, const double* d_xub, uint64_t seed, uint64_t stream_id,
+                          double* d_x_gen, int32_t* d_kind, int64_t* n_children, double* d_draws);
+int remove_worst_device(dmo_ctx* ctx, const double* dX, const double* dY, int64_t n, int d, int M, int metric,
+                        const double* const* d_extra, int n_extra, int64_t keep, double* dX_out, double* dY_out, int32_t* d_rank_out,
+                        int64_t* d_perm_out);
 // the feasibility model's rank (csrc/feasibility.cu) of n device rows into d_rank, enqueued on the context's stream
 int feas_rank_device(dmo_ctx* ctx, const dmo_feas* m, const double* dX, int64_t n, double* d_rank);
 int feas_model_dim(const dmo_feas* m);

@@ -24,6 +24,35 @@ bool dmo_is_device_ptr(const void* p) {
   return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
 }
 
+int dmo_lag_slots(dmo_ctx* ctx) {
+  if (ctx->lag_host) return DMO_OK;
+  DMO_CUDA(cudaHostAlloc((void**)&ctx->lag_host, 3 * sizeof(unsigned long long), cudaHostAllocDefault));
+  for (cudaEvent_t& e : ctx->lag_ev) DMO_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  return DMO_OK;
+}
+
+SideStreams::SideStreams(dmo_ctx* c, int nside) : ctx(c), main(c->stream) {
+  if (nside > dmo_ctx::kSide) nside = dmo_ctx::kSide;
+  if (!ctx->side[0]) {
+    for (cudaStream_t& st : ctx->side)
+      if (cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess) rc = DMO_ERR_CUDA;
+    for (cudaEvent_t& e : ctx->side_ev)
+      if (cudaEventCreateWithFlags(&e, cudaEventDisableTiming) != cudaSuccess) rc = DMO_ERR_CUDA;
+  }
+  if (rc == DMO_OK && cudaEventRecord(ctx->side_ev[0], main) != cudaSuccess) rc = DMO_ERR_CUDA;
+  for (int s = 0; rc == DMO_OK && s < nside; ++s, ++k)
+    if (cudaStreamWaitEvent(ctx->side[s], ctx->side_ev[0], 0) != cudaSuccess) rc = DMO_ERR_CUDA;
+  if (rc != DMO_OK) dmo_fail(ctx, rc, "could not set up side streams");
+}
+
+SideStreams::~SideStreams() {
+  ctx->stream = main;
+  for (int s = 0; s < k; ++s) {
+    cudaEventRecord(ctx->side_ev[1 + s], ctx->side[s]);
+    cudaStreamWaitEvent(main, ctx->side_ev[1 + s], 0);
+  }
+}
+
 extern "C" {
 
 int dmo_version(void) { return 100; }
@@ -68,9 +97,16 @@ int dmo_create(int device, dmo_ctx** out) {
 int dmo_destroy(dmo_ctx* ctx) {
   if (!ctx) return DMO_OK;
   cudaSetDevice(ctx->device);
-  cudaStreamSynchronize(ctx->stream);
+  dmo_wait(ctx);
   if (ctx->flush_buf) cudaFree(ctx->flush_buf);
   if (ctx->dev_flag) cudaFree(ctx->dev_flag);
+  if (ctx->lag_host) cudaFreeHost(ctx->lag_host);
+  for (cudaEvent_t e : ctx->lag_ev)
+    if (e) cudaEventDestroy(e);
+  for (cudaEvent_t e : ctx->side_ev)
+    if (e) cudaEventDestroy(e);
+  for (cudaStream_t st : ctx->side)
+    if (st) cudaStreamDestroy(st);
   cudaEventDestroy(ctx->ev0);
   cudaEventDestroy(ctx->ev1);
   cudaStreamDestroy(ctx->stream);
@@ -81,12 +117,13 @@ int dmo_destroy(dmo_ctx* ctx) {
 const char* dmo_last_error(dmo_ctx* ctx) { return ctx ? ctx->err.c_str() : "null context"; }
 
 int dmo_synchronize(dmo_ctx* ctx) {
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
 void* dmo_stream(dmo_ctx* ctx) { return (void*)ctx->stream; }
 int64_t dmo_launch_count(dmo_ctx* ctx) { return ctx->launches; }
+int64_t dmo_wait_count(dmo_ctx* ctx) { return ctx->waits; }
 int dmo_sm_count(dmo_ctx* ctx) { return ctx->sm_count; }
 
 int dmo_timer_begin(dmo_ctx* ctx) {
@@ -96,6 +133,7 @@ int dmo_timer_begin(dmo_ctx* ctx) {
 
 int dmo_timer_end(dmo_ctx* ctx, float* ms) {
   DMO_CUDA(cudaEventRecord(ctx->ev1, ctx->stream));
+  ctx->waits++;
   DMO_CUDA(cudaEventSynchronize(ctx->ev1));
   DMO_CUDA(cudaEventElapsedTime(ms, ctx->ev0, ctx->ev1));
   return DMO_OK;
@@ -125,7 +163,7 @@ int dmo_memcpy(dmo_ctx* ctx, void* dst, const void* src, uint64_t bytes) {
   if (!ctx) return DMO_ERR_ARG;
   if (bytes == 0) return DMO_OK;
   DMO_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   const bool sd = dmo_is_device_ptr(src), dd = dmo_is_device_ptr(dst);
   if (!sd && dd) ctx->h2d_bytes += bytes;
   if (sd && !dd) ctx->d2h_bytes += bytes;
@@ -139,7 +177,7 @@ int dmo_transfer_bytes(dmo_ctx* ctx, uint64_t* h2d, uint64_t* d2h) {
 }
 
 int dmo_profile_enable(dmo_ctx* ctx, int on) {
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   for (auto& t : ctx->timers) {
     cudaEventDestroy(t.a);
     cudaEventDestroy(t.b);
@@ -151,7 +189,7 @@ int dmo_profile_enable(dmo_ctx* ctx, int on) {
 
 // "name ms count" lines, one per timer name, summed over the scopes recorded since dmo_profile_enable(1)
 int dmo_profile_report(dmo_ctx* ctx, char* buf, uint64_t cap) {
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   std::vector<std::string> names;
   std::vector<double> ms;
   std::vector<int> cnt;

@@ -201,7 +201,7 @@ int glp_check_multipliers(dmo_ctx* ctx, const int64_t* H, int64_t C, int s, int6
   if (dmo_is_device_ptr(H)) {
     host.resize((size_t)(C * s));
     DMO_CUDA(cudaMemcpyAsync(host.data(), H, host.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+    DMO_CUDA(dmo_wait(ctx));
     p = host.data();
   }
   int bad = 0;
@@ -238,7 +238,7 @@ int dmo_glp_cd2_terms(dmo_ctx* ctx, const int64_t* H, int64_t C, int s, int64_t 
   DMO_TRY((l2_terms<LatticeSrc, CD2>(ctx, src, C, rows, s, o2.d, o3.d)));
   DMO_TRY(o2.finish(ctx));
   DMO_TRY(o3.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -260,7 +260,7 @@ int dmo_glp_cd2_pairs(dmo_ctx* ctx, const int64_t* H, int64_t L, int s, int64_t 
   }
   DMO_CHECK_LAUNCH();
   DMO_TRY(op.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -285,6 +285,6 @@ int dmo_l2_discrepancy_terms(dmo_ctx* ctx, int metric, const double* X, int64_t 
   }
   DMO_TRY(o2.finish(ctx));
   DMO_TRY(o3.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }

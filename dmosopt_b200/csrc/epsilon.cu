@@ -114,7 +114,7 @@ extern "C" int dmo_epsilon_sort(dmo_ctx* ctx, const double* Y, int64_t n, int M,
   EpsArgs ea;
   if (dmo_is_device_ptr(eps)) {
     DMO_CUDA(cudaMemcpyAsync(ea.e, eps, M * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+    DMO_CUDA(dmo_wait(ctx));
   } else {
     for (int j = 0; j < M; ++j) ea.e[j] = eps[j];
   }
@@ -145,7 +145,7 @@ extern "C" int dmo_epsilon_sort(dmo_ctx* ctx, const double* Y, int64_t n, int M,
   DMO_CHECK_LAUNCH();
   unsigned long long first = 0;
   DMO_CUDA(cudaMemcpyAsync(&first, ovf.p, sizeof(first), cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   if (first != ~0ull)
     return dmo_fail(ctx, DMO_ERR_OVERFLOW, "epsilon_sort: y / eps overflows to infinity in row %llu (the reference's math.floor raises OverflowError)", first);
 
@@ -169,7 +169,7 @@ extern "C" int dmo_epsilon_sort(dmo_ctx* ctx, const double* Y, int64_t n, int M,
     DMO_CHECK_LAUNCH();
     DMO_TRY(prim_exclusive_sum_i32(ctx, win.p, wpos.p, n + 1));
     DMO_CUDA(cudaMemcpyAsync(&k, wpos.p + n, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+    DMO_CUDA(dmo_wait(ctx));
   }
 
   // 3. the boxes no other occupied box dominates
@@ -194,9 +194,9 @@ extern "C" int dmo_epsilon_sort(dmo_ctx* ctx, const double* Y, int64_t n, int M,
   DMO_CUDA(cudaMemcpyAsync(&h, kpos.p + n, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
   DMO_LAUNCH(write_rows_kernel, g, 256, 0, kept.p, kpos.p, n, out.d);
   DMO_CHECK_LAUNCH();
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   DMO_TRY(out.finish(ctx, (size_t)h));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   *count = h;
   return DMO_OK;
 }

@@ -513,7 +513,7 @@ int dmo_feas_fit(dmo_ctx* ctx, const double* X, int64_t N, int d, int J, const u
   DMO_TRY(okkt.finish(ctx));
   DMO_TRY(oconv.finish(ctx));
   DMO_TRY(ocor.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -552,7 +552,7 @@ int dmo_feas_create(dmo_ctx* ctx, int d, int J, const int32_t* k, const double* 
   }
   cudaError_t e = cudaMemcpyAsync(m->k.p, k, J * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream);
   if (e == cudaSuccess) e = cudaMemcpyAsync(m->par.p, h.data(), h.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  if (e == cudaSuccess) e = dmo_wait(ctx);
   if (e != cudaSuccess) {
     delete m;
     return dmo_fail(ctx, DMO_ERR_CUDA, "feas_create: upload failed: %s", cudaGetErrorString(e));
@@ -565,7 +565,7 @@ int dmo_feas_destroy(dmo_ctx* ctx, dmo_feas* m) {
   if (!ctx) return DMO_ERR_ARG;
   if (!m) return DMO_OK;
   DMO_CUDA(cudaSetDevice(ctx->device));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   delete m;
   return DMO_OK;
 }
@@ -587,7 +587,7 @@ int dmo_feas_eval(dmo_ctx* ctx, const dmo_feas* m, const double* X, int64_t n, i
   DMO_TRY(orank.finish(ctx));
   DMO_TRY(opr.finish(ctx));
   DMO_TRY(odec.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 

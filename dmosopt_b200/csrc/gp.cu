@@ -399,7 +399,7 @@ int gp_linv_from_factor_batched(dmo_ctx* ctx, const double* L, int64_t ldl, int6
 
 int gp_linv_from_factor(dmo_ctx* ctx, const double* L, int64_t N, int64_t ldo, double* dst) {
   DMO_TRY(gp_linv_from_factor_batched(ctx, L, N, 0, N, 1, ldo, 0, dst));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -571,7 +571,7 @@ int gp_calibrate(dmo_ctx* ctx, dmo_gp* gp) {
   DMO_CUDA(cudaMemcpyAsync(h.data() + (size_t)P * M, v64.p, (size_t)P * M * 8, cudaMemcpyDeviceToHost, ctx->stream));
   DMO_CUDA(cudaMemcpyAsync(h.data() + (size_t)2 * P * M, mt.p, (size_t)P * M * 8, cudaMemcpyDeviceToHost, ctx->stream));
   DMO_CUDA(cudaMemcpyAsync(h.data() + (size_t)3 * P * M, vt.p, (size_t)P * M * 8, cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   const double *a64 = h.data(), *b64 = a64 + (size_t)P * M, *at = b64 + (size_t)P * M, *bt = at + (size_t)P * M;
   double em = 0.0, ev = 0.0, eo = 0.0;
   for (int p = 0; p < P; ++p)
@@ -600,46 +600,108 @@ int gp_calibrate(dmo_ctx* ctx, dmo_gp* gp) {
 }
 
 // AUTO predict on normalised inputs: tensor path where the calibration allows it, float64 for the rest
-int gp_predict_auto(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var) {
+int gp_predict_auto(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var,
+                    GpPending* pending) {
   DMO_TRY(gp_calibrate(ctx, gp));
   gp->last_refined = 0;
   if (d_var ? !gp->auto_var_tensor : !gp->auto_mean_only) {
     gp->last_refined = P;
     return gp_predict_fp64(ctx, gp, dXn, P, d_mean, d_var);
   }
-  DMO_TRY(gp_predict_tensor(ctx, gp, dXn, P, d_mean, d_var));
-  if (!d_var) return DMO_OK;
-  const int M = gp->M, d = gp->d;
-  DevBuf<int32_t> flag, pos;
-  DMO_TRY(flag.alloc(ctx, (size_t)P + 1));
-  DMO_TRY(pos.alloc(ctx, (size_t)P + 1));
-  DMO_CUDA(cudaMemsetAsync(flag.p + P, 0, sizeof(int32_t), ctx->stream));
-  DMO_LAUNCH(flag_small_var_kernel, (unsigned)ceil_div(P, 256), 256, 0, d_var, P, M, gp->constant.p, gp->noise.p, gp->ystd.p,
-             gp->refine_theta, flag.p);
-  DMO_TRY(prim_exclusive_sum_i32(ctx, flag.p, pos.p, P + 1));
-  int32_t n_ref = 0;
-  DMO_CUDA(cudaMemcpyAsync(&n_ref, pos.p + P, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (!d_var) return gp_predict_tensor(ctx, gp, dXn, P, d_mean, nullptr);
+  GpPending own;
+  GpPending& q = pending ? *pending : own;
+  DMO_TRY(q.flag.alloc(ctx, (size_t)P + 1));
+  DMO_TRY(q.pos.alloc(ctx, (size_t)P + 2));  // pos[P]: rows to refine, pos[P + 1]: the contraction's watchdog, read back together
+  DMO_TRY(gp_predict_tensor(ctx, gp, dXn, P, d_mean, d_var, q.pos.p + P + 1));
+  DMO_CUDA(cudaMemsetAsync(q.flag.p + P, 0, sizeof(int32_t), ctx->stream));
+  DMO_LAUNCH(flag_small_var_kernel, (unsigned)ceil_div(P, 256), 256, 0, d_var, P, gp->M, gp->constant.p, gp->noise.p, gp->ystd.p,
+             gp->refine_theta, q.flag.p);
+  DMO_TRY(prim_exclusive_sum_i32(ctx, q.flag.p, q.pos.p, P + 1));
+  DMO_TRY(dmo_lag_slots(ctx));
+  DMO_CUDA(cudaMemcpyAsync(ctx->lag_host + 2, q.pos.p + P, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  DMO_CUDA(cudaEventRecord(ctx->lag_ev[2], ctx->stream));
+  q.active = true;
+  q.P = P;
+  q.dXn = dXn;
+  q.d_mean = d_mean;
+  q.d_var = d_var;
+  if (pending) return DMO_OK;
+  bool refined = false;
+  return gp_predict_finish(ctx, gp, q, &refined);
+}
+
+}  // namespace
+
+// mean[p][m] += y_std[m] * (w_m . xn_p + b_m): the prior mean of a gpytorch ExactGP with LinearMean
+__global__ void linear_mean_add_kernel(const double* __restrict__ Xn, int64_t P, int d, int M,
+                                       const double* __restrict__ w, const double* __restrict__ b,
+                                       const double* __restrict__ ystd, double* __restrict__ mean) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= P * M) return;
+  const int64_t p = t / M;
+  const int m = (int)(t - p * M);
+  double s = b[m];
+  for (int j = 0; j < d; ++j) s = fma(w[m * d + j], Xn[p * d + j], s);
+  mean[t] += ystd[m] * s;
+}
+
+int gp_predict_finish(dmo_ctx* ctx, dmo_gp* gp, GpPending& q, bool* refined) {
+  *refined = false;
+  if (!q.active) return DMO_OK;
+  q.active = false;
+  ctx->waits++;
+  DMO_CUDA(cudaEventSynchronize(ctx->lag_ev[2]));
+  int32_t h[2];
+  memcpy(h, ctx->lag_host + 2, sizeof(h));
+  if (h[1]) return dmo_fail(ctx, DMO_ERR_INTERNAL, "%s", GP_WATCHDOG_MSG);
+  const int32_t n_ref = h[0];
   gp->last_refined = n_ref;
   if (n_ref == 0) return DMO_OK;
+  const int M = gp->M, d = gp->d;
+  const int64_t P = q.P;
   DevBuf<int32_t> idx;
   DevBuf<double> xs, ms, vs;
   DMO_TRY(idx.alloc(ctx, (size_t)n_ref));
   DMO_TRY(xs.alloc(ctx, (size_t)n_ref * d));
   DMO_TRY(ms.alloc(ctx, (size_t)n_ref * M));
   DMO_TRY(vs.alloc(ctx, (size_t)n_ref * M));
-  DMO_LAUNCH(compact_rows_kernel, (unsigned)ceil_div(P, 256), 256, 0, flag.p, pos.p, P, d, dXn, idx.p, xs.p);
+  DMO_LAUNCH(compact_rows_kernel, (unsigned)ceil_div(P, 256), 256, 0, q.flag.p, q.pos.p, P, d, q.dXn, idx.p, xs.p);
   {
     ProfileScope ps(ctx, "gp_refine_fp64");
     DMO_TRY(gp_predict_fp64(ctx, gp, xs.p, n_ref, ms.p, vs.p));
   }
   DMO_LAUNCH(scatter_rows_kernel, (unsigned)ceil_div((int64_t)n_ref * M, 256), 256, 0, idx.p, (int64_t)n_ref, M, ms.p, vs.p,
-             d_mean, d_var);
+             q.d_mean, q.d_var);
   DMO_CHECK_LAUNCH();
+  *refined = true;
   return DMO_OK;
 }
 
-}  // namespace
+int gp_predict_device(dmo_ctx* ctx, dmo_gp* gp, const double* dX, int64_t P, double* d_mean, double* d_var, int precision,
+                      GpPending* pending) {
+  // the read-back is left pending only where nothing of this call comes after the refinement (no linear mean)
+  const bool defer = pending && precision == DMO_GP_AUTO && d_var && !gp->has_linear_mean;
+  DevBuf<double> own;
+  DevBuf<double>& xn = defer ? pending->xn : own;
+  DMO_TRY(xn.alloc(ctx, (size_t)P * gp->d));
+  DMO_LAUNCH(normalise_x_kernel, (unsigned)ceil_div(P * gp->d, 256), 256, 0, dX, P, gp->d, gp->xlb.p, gp->xrg.p, xn.p);
+  if (precision == DMO_GP_FP64) {
+    DMO_TRY(gp_predict_fp64(ctx, gp, xn.p, P, d_mean, d_var));
+  } else if (precision == DMO_GP_TENSOR) {
+    DMO_TRY(gp_predict_tensor(ctx, gp, xn.p, P, d_mean, d_var));
+  } else if (precision == DMO_GP_AUTO) {
+    DMO_TRY(gp_predict_auto(ctx, gp, xn.p, P, d_mean, d_var, defer ? pending : nullptr));
+  } else {
+    return dmo_fail(ctx, DMO_ERR_ARG, "gp_predict: unknown precision %d", precision);
+  }
+  if (gp->has_linear_mean) {
+    DMO_LAUNCH(linear_mean_add_kernel, (unsigned)ceil_div(P * gp->M, 256), 256, 0, xn.p, P, gp->d, gp->M, gp->lin_w.p,
+               gp->lin_b.p, gp->ystd.p, d_mean);
+    DMO_CHECK_LAUNCH();
+  }
+  return DMO_OK;
+}
 
 extern "C" {
 
@@ -724,7 +786,7 @@ int dmo_gp_create(dmo_ctx* ctx, int64_t N, int d, int M, int kernel, const doubl
       const int64_t nb = std::min<int64_t>(ceil_div(n, 256), (int64_t)8 * ctx->sm_count);
       DMO_LAUNCH(factor_diff_kernel, (unsigned)nb, 256, 0, reinterpret_cast<const unsigned long long*>(f.d), n, M, diff.p);
       GP_CUDA(cudaMemcpyAsync(h_diff.data(), diff.p, M * sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));
-      GP_CUDA(cudaStreamSynchronize(ctx->stream));
+      GP_CUDA(dmo_wait(ctx));
     }
     gp->h_cov.assign(M, -1);
     for (int m = 0; m < M; ++m) {
@@ -763,7 +825,7 @@ int dmo_gp_create(dmo_ctx* ctx, int64_t N, int d, int M, int kernel, const doubl
       }
     }
     GP_CUDA(cudaGetLastError());
-    GP_CUDA(cudaStreamSynchronize(ctx->stream));
+    GP_CUDA(dmo_wait(ctx));
   }
   // host copies used by the tensor path's scaling
   gp->h_constant = h_c;
@@ -781,22 +843,9 @@ int dmo_gp_destroy(dmo_ctx* ctx, dmo_gp* gp) {
   if (!ctx) return DMO_ERR_ARG;
   if (!gp) return DMO_OK;
   DMO_CUDA(cudaSetDevice(ctx->device));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   delete gp;
   return DMO_OK;
-}
-
-// mean[p][m] += y_std[m] * (w_m . xn_p + b_m): the prior mean of a gpytorch ExactGP with LinearMean
-__global__ void linear_mean_add_kernel(const double* __restrict__ Xn, int64_t P, int d, int M,
-                                       const double* __restrict__ w, const double* __restrict__ b,
-                                       const double* __restrict__ ystd, double* __restrict__ mean) {
-  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= P * M) return;
-  const int64_t p = t / M;
-  const int m = (int)(t - p * M);
-  double s = b[m];
-  for (int j = 0; j < d; ++j) s = fma(w[m * d + j], Xn[p * d + j], s);
-  mean[t] += ystd[m] * s;
 }
 
 int dmo_gp_set_linear_mean(dmo_ctx* ctx, dmo_gp* gp, const double* weight, const double* bias) {
@@ -815,7 +864,7 @@ int dmo_gp_set_linear_mean(dmo_ctx* ctx, dmo_gp* gp, const double* weight, const
   DMO_TRY(gp->lin_b.alloc(ctx, (size_t)gp->M));
   DMO_CUDA(cudaMemcpyAsync(gp->lin_w.p, w.d, (size_t)gp->M * gp->d * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
   DMO_CUDA(cudaMemcpyAsync(gp->lin_b.p, b.d, (size_t)gp->M * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   gp->has_linear_mean = true;
   return DMO_OK;
 }
@@ -854,26 +903,10 @@ int dmo_gp_predict(dmo_ctx* ctx, dmo_gp* gp, const double* X, int64_t P, double*
   DMO_TRY(x.init(ctx, X, (size_t)P * gp->d));
   DMO_TRY(om.init(ctx, mean, (size_t)P * gp->M));
   DMO_TRY(ov.init(ctx, var, (size_t)P * gp->M));
-  DevBuf<double> xn;
-  DMO_TRY(xn.alloc(ctx, (size_t)P * gp->d));
-  DMO_LAUNCH(normalise_x_kernel, (unsigned)ceil_div(P * gp->d, 256), 256, 0, x.d, P, gp->d, gp->xlb.p, gp->xrg.p, xn.p);
-  if (precision == DMO_GP_FP64) {
-    DMO_TRY(gp_predict_fp64(ctx, gp, xn.p, P, om.d, ov.d));
-  } else if (precision == DMO_GP_TENSOR) {
-    DMO_TRY(gp_predict_tensor(ctx, gp, xn.p, P, om.d, ov.d));
-  } else if (precision == DMO_GP_AUTO) {
-    DMO_TRY(gp_predict_auto(ctx, gp, xn.p, P, om.d, ov.d));
-  } else {
-    return dmo_fail(ctx, DMO_ERR_ARG, "gp_predict: unknown precision %d", precision);
-  }
-  if (gp->has_linear_mean) {
-    DMO_LAUNCH(linear_mean_add_kernel, (unsigned)ceil_div(P * gp->M, 256), 256, 0, xn.p, P, gp->d, gp->M, gp->lin_w.p,
-               gp->lin_b.p, gp->ystd.p, om.d);
-    DMO_CHECK_LAUNCH();
-  }
+  DMO_TRY(gp_predict_device(ctx, gp, x.d, P, om.d, ov.d, precision));
   DMO_TRY(om.finish(ctx));
   DMO_TRY(ov.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 

@@ -105,7 +105,28 @@ constexpr int GP_TC_TILE = 128;
 int gp_tensor_var_planes(int64_t Npad);
 int gp_var_contract_tensor(dmo_ctx* ctx, const GpVarOps& ops, const uint16_t* Kh, const uint16_t* Kl, int64_t k_alloc,
                            int64_t k_rows, int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag);
-int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var);
+// abort_flag null: the call reads the contraction's watchdog back and fails when it tripped.  Otherwise the call zeroes
+// *abort_flag (device) and the watchdog lands there; the caller reads it back and fails the same way (gp_predict_auto folds
+// it into its own read-back).  The mean-only route writes no flag.
+int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var,
+                      int* abort_flag = nullptr);
+extern const char* const GP_WATCHDOG_MSG;
+// An AUTO predict whose one read-back (watchdog, rows to refine) is left pending, so the caller can enqueue work behind it
+// while the GP runs; gp_predict_finish waits for it, fails on a tripped watchdog and refines the rows the check flags
+// (after that work: *refined tells the caller to redo it).  Only the AUTO variance route of models without a linear mean
+// defers; other calls finish inside gp_predict_device and leave `active` false.
+struct GpPending {
+  bool active = false;
+  int64_t P = 0;
+  const double* dXn = nullptr;
+  double *d_mean = nullptr, *d_var = nullptr;
+  DevBuf<double> xn;
+  DevBuf<int32_t> flag, pos;
+};
+// dmo_gp_predict on device arrays: X (P, d) un-normalised, mean / var (P, M); var may be null
+int gp_predict_device(dmo_ctx* ctx, dmo_gp* gp, const double* dX, int64_t P, double* d_mean, double* d_var, int precision,
+                      GpPending* pending = nullptr);
+int gp_predict_finish(dmo_ctx* ctx, dmo_gp* gp, GpPending& pending, bool* refined);
 
 // Candidate chunks and variance scratch of the unit-scale posteriors (MEGP, variational; gp_multitask.cu): one K_* plane
 // per chunk (float64 Ks, or fp16 Kh / Kl) contracted against up to `planes` operator planes, partial sums in vnorm (rows

@@ -231,7 +231,7 @@ int dmo_dgp_destroy(dmo_ctx* ctx, dmo_dgp* g) {
   if (!ctx) return DMO_ERR_ARG;
   if (!g) return DMO_OK;
   DMO_CUDA(cudaSetDevice(ctx->device));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   if (g->hidden) dmo_svgp_destroy(ctx, g->hidden);
   if (g->last) dmo_svgp_destroy(ctx, g->last);
   delete g;
@@ -320,7 +320,7 @@ int dmo_dgp_create(dmo_ctx* ctx, int d, int H, int T, int64_t Z1, int64_t Z2, co
   DMO_TRY(upload(ctx, g->xrg, rg));
   if (quad_sites) DMO_TRY(upload(ctx, g->sites, hq));
   DMO_CHECK_LAUNCH();
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));  // host vectors above are staged from the stack
+  DMO_CUDA(dmo_wait(ctx));  // host vectors above are staged from the stack
   *out = g.release();
   return DMO_OK;
 }
@@ -371,7 +371,7 @@ int dmo_dgp_predict(dmo_ctx* ctx, dmo_dgp* g, const double* X, int64_t P, uint64
   DMO_TRY(om.finish(ctx));
   DMO_TRY(ov.finish(ctx));
   DMO_TRY(oe.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 

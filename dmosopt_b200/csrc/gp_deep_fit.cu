@@ -779,7 +779,7 @@ int dgf_check_info(dmo_ctx* ctx, dmo_dgp_fit* st, const char* who) {
   const int U = st->L.H + st->L.T;
   std::vector<int> h(U);
   DMO_CUDA(cudaMemcpyAsync(h.data(), st->info.p, U * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   for (int u = 0; u < U; ++u)
     if (h[u])
       return dmo_fail(ctx, DMO_ERR_ARG, "%s: K(Z, Z) + jitter I of %s unit %d is not positive definite (pivot %d)", who,
@@ -919,7 +919,7 @@ int dmo_dgp_fit_create(dmo_ctx* ctx, int64_t N, int d, int H, int T, int64_t Z1,
   DMO_CUDA(cudaFuncSetAttribute(dgf_factor_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(DF_ZMAX * DF_ZMAX * sizeof(double))));
   DMO_CUDA(cudaFuncSetAttribute(dgf_unit_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(DF_ZMAX * DF_ZMAX * sizeof(double))));
   DMO_CHECK_LAUNCH();
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   *out = st.release();
   return DMO_OK;
 }
@@ -928,7 +928,7 @@ int dmo_dgp_fit_destroy(dmo_ctx* ctx, dmo_dgp_fit* st) {
   if (!ctx) return DMO_ERR_ARG;
   if (!st) return DMO_OK;
   DMO_CUDA(cudaSetDevice(ctx->device));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   delete st;
   return DMO_OK;
 }
@@ -942,7 +942,7 @@ int dmo_dgp_fit_set_params(dmo_ctx* ctx, dmo_dgp_fit* st, const double* raw, int
   DMO_CUDA(cudaMemcpy(h.data(), raw, n * sizeof(double), cudaMemcpyDefault));
   for (int64_t i = 0; i < n; ++i) DMO_REQUIRE(isfinite(h[i]), "dgp_fit_set_params: raw[%lld] must be finite", (long long)i);
   DMO_CUDA(cudaMemcpyAsync(st->p.p, h.data(), n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -952,7 +952,7 @@ int dmo_dgp_fit_get_params(dmo_ctx* ctx, dmo_dgp_fit* st, double* raw, int64_t n
   DMO_REQUIRE(st && raw, "dgp_fit_get_params: null argument");
   DMO_REQUIRE(n == st->L.P, "dgp_fit_get_params: the raw vector has %lld entries (got %lld)", (long long)st->L.P, (long long)n);
   DMO_CUDA(cudaMemcpyAsync(raw, st->p.p, n * sizeof(double), cudaMemcpyDefault, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -979,7 +979,7 @@ int dmo_dgp_fit_loss_grad(dmo_ctx* ctx, dmo_dgp_fit* st, const int64_t* batch, i
   DMO_CUDA(cudaMemcpyAsync(loss_out, st->losses.p, sizeof(double), cudaMemcpyDefault, ctx->stream));
   if (grad_out) DMO_CUDA(cudaMemcpyAsync(grad_out, st->g.p, st->L.P * sizeof(double), cudaMemcpyDefault, ctx->stream));
   if (eps_out) DMO_CUDA(cudaMemcpyAsync(eps_out, st->eps.p, ne * sizeof(double), cudaMemcpyDefault, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -990,7 +990,7 @@ int dmo_dgp_fit_adam_step(dmo_ctx* ctx, dmo_dgp_fit* st, double lr) {
   DMO_REQUIRE(lr > 0.0 && isfinite(lr), "dgp_fit_adam_step: lr must be finite and > 0 (got %g)", lr);
   DMO_TRY(dgf_adam(ctx, st, lr));
   DMO_CHECK_LAUNCH();
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -1020,7 +1020,7 @@ int dmo_dgp_fit_epoch(dmo_ctx* ctx, dmo_dgp_fit* st, const int64_t* perm, int64_
   DMO_CHECK_LAUNCH();
   DMO_TRY(dgf_check_info(ctx, st, "dgp_fit_epoch"));
   DMO_CUDA(cudaMemcpyAsync(losses_out, st->losses.p, nb * sizeof(double), cudaMemcpyDefault, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 

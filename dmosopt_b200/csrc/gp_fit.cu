@@ -364,12 +364,12 @@ int dmo_gp_fit(dmo_ctx* ctx, int64_t N, int d, int M, int kernel, const double* 
   DMO_CHECK_LAUNCH();
   int h_info = 0;
   DMO_CUDA(cudaMemcpyAsync(&h_info, info.p, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   if (h_info) return dmo_fail(ctx, DMO_ERR_ARG, "gp_fit: the kernel matrix is not positive definite (pivot %d)", h_info - 1);
   DMO_TRY(oL.finish(ctx));
   DMO_TRY(oa.finish(ctx));
   DMO_TRY(ol.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 

@@ -365,7 +365,7 @@ int GpUnitPredict::watchdog(dmo_ctx* ctx) {
   if (!abort_flag.p) return DMO_OK;  // no tensor-core contraction ran
   int h_abort = 0;
   DMO_CUDA(cudaMemcpyAsync(&h_abort, abort_flag.p, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   if (h_abort) return dmo_fail(ctx, DMO_ERR_INTERNAL, "%s(tensor): pipeline watchdog tripped", who);
   return DMO_OK;
 }
@@ -515,7 +515,7 @@ int dmo_mtgp_create(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_train
   DMO_TRY(upload(ctx, mt->ymean, ym));
   DMO_TRY(upload(ctx, mt->ystd, ys));
   DMO_CHECK_LAUNCH();
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));  // host vectors above are staged from the stack
+  DMO_CUDA(dmo_wait(ctx));  // host vectors above are staged from the stack
   if (lml_out) DMO_CUDA(cudaMemcpy(lml_out, &lml, sizeof(double), cudaMemcpyDefault));
   *out = mt.release();
   return DMO_OK;
@@ -525,7 +525,7 @@ int dmo_mtgp_destroy(dmo_ctx* ctx, dmo_mtgp* mt) {
   if (!ctx) return DMO_ERR_ARG;
   if (!mt) return DMO_OK;
   DMO_CUDA(cudaSetDevice(ctx->device));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   delete mt;
   return DMO_OK;
 }
@@ -578,7 +578,7 @@ int dmo_mtgp_predict(dmo_ctx* ctx, dmo_mtgp* mt, const double* X, int64_t P, dou
   DMO_TRY(up.watchdog(ctx));
   DMO_TRY(om.finish(ctx));
   DMO_TRY(ov.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 

@@ -356,7 +356,7 @@ int dmo_mtgp_lml_grad(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_tra
   DMO_CHECK_LAUNCH();
   std::vector<double> hr((size_t)2 * M + nq);
   DMO_CUDA(cudaMemcpyAsync(hr.data(), red.p, hr.size() * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   // host combination: trKA_j = tr(K_x A_j^-1), trA_j = tr(A_j^-1)
   const double* trKA = hr.data();
   const double* trA = hr.data() + M;
@@ -463,7 +463,7 @@ int dmo_gp_lml_grad(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_train
   DMO_CUDA(cudaMemcpyAsync(h_info.data(), info.p, M * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   DMO_CUDA(cudaMemcpyAsync(h_lml.data(), lml_d.p, M * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
   DMO_CUDA(cudaMemcpyAsync(al.data(), alpha_d.p, mn * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   for (int m = 0; m < M; ++m)
     if (h_info[m])
       return dmo_fail(ctx, DMO_ERR_ARG, "gp_lml_grad: the kernel matrix of objective %d is not positive definite (pivot %d)", m,
@@ -509,7 +509,7 @@ int dmo_gp_lml_grad(dmo_ctx* ctx, int64_t N, int d, int M, const double* X_train
   DMO_CHECK_LAUNCH();
   std::vector<double> hr((size_t)M * (2 + nq));
   DMO_CUDA(cudaMemcpyAsync(hr.data(), red.p, hr.size() * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   // per objective: tr(K_x K_m^-1), tr(K_m^-1), then sum W dK_x / dl_k * l_k (k < d) and alpha' K_x alpha
   std::vector<double> gl(md), gs(M), gn(M), gw(md, 0.0), gb(M, 0.0);
   for (int m = 0; m < M; ++m) {

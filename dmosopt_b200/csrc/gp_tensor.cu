@@ -1006,7 +1006,7 @@ int gp_prepare_tensor(dmo_ctx* ctx, GpVarOps& ops) {
   }
   DMO_TRY(ops.Kexp.alloc(ctx, G));
   DMO_CUDA(cudaMemcpyAsync(ops.Kexp.p, kexp.data(), G * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));  // kexp is a stack vector
+  DMO_CUDA(dmo_wait(ctx));  // kexp is a stack vector
   DMO_TRY(ops.Lhi.alloc(ctx, (size_t)G * Npad * Npad));
   DMO_TRY(ops.Llo.alloc(ctx, (size_t)G * Npad * Npad));
   DMO_TRY(ops.Lscale.alloc(ctx, (size_t)G * Npad));
@@ -1048,7 +1048,9 @@ int gp_var_contract_tensor(dmo_ctx* ctx, const GpVarOps& ops, const uint16_t* Kh
   return DMO_OK;
 }
 
-int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var) {
+const char* const GP_WATCHDOG_MSG = "gp_predict(tensor): pipeline watchdog tripped (mbarrier wait timed out)";
+
+int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var, int* abort_flag) {
   const int64_t N = gp->N, Npad = gp->ops.Npad;
   const int M = gp->M, G = gp->ops.G, d = gp->d;
   DMO_REQUIRE(M <= 16, "gp_predict(tensor): at most 16 objectives per model (got %d)", M);
@@ -1067,12 +1069,16 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
   const int n_q = gp_tensor_var_planes(Npad);
   DevBuf<uint16_t> Kh, Kl;
   DevBuf<double> vnorm;
-  DevBuf<int> abort_flag;
+  DevBuf<int> own_flag;
   DMO_TRY(Kh.alloc(ctx, (size_t)G * Pc_alloc * Npad));
   DMO_TRY(Kl.alloc(ctx, (size_t)G * Pc_alloc * Npad));
   DMO_TRY(vnorm.alloc(ctx, (size_t)n_q * G * Pc_alloc));
-  DMO_TRY(abort_flag.alloc(ctx, 1));
-  DMO_CUDA(cudaMemsetAsync(abort_flag.p, 0, sizeof(int), ctx->stream));
+  const bool read_back = abort_flag == nullptr;
+  if (read_back) {
+    DMO_TRY(own_flag.alloc(ctx, 1));
+    abort_flag = own_flag.p;
+  }
+  DMO_CUDA(cudaMemsetAsync(abort_flag, 0, sizeof(int), ctx->stream));
   const int64_t kplane = Pc_alloc * Npad;
   // K_* producer fused with the mean (d <= 32, M <= 6; DMO_GP_FUSED=0 keeps kstar_tensor_kernel + mean_split_kernel)
   // (per-dimension length scales with more than two covariances keep the two-kernel route: a distance pass per covariance)
@@ -1160,16 +1166,17 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
     if (d_var) {
       {
         ProfileScope ps_(ctx, "gp_var");
-        DMO_TRY(gp_var_contract_tensor(ctx, gp->ops, Kh.p, Kl.p, G * Pc_alloc, Pc_alloc, Pcpad, vnorm.p, Pc_alloc, abort_flag.p));
+        DMO_TRY(gp_var_contract_tensor(ctx, gp->ops, Kh.p, Kl.p, G * Pc_alloc, Pc_alloc, Pcpad, vnorm.p, Pc_alloc, abort_flag));
       }
       DMO_LAUNCH(var_finish_tc_kernel, (unsigned)ceil_div(Pc * M, 256), 256, 0, vnorm.p, n_q, Pc, Pc_alloc, M, G,
                  gp->cov.p, gp->constant.p, gp->noise.p, gp->ystd.p, p_base, d_var);
     }
   }
   DMO_CHECK_LAUNCH();
+  if (!read_back) return DMO_OK;
   int h_abort = 0;
-  DMO_CUDA(cudaMemcpyAsync(&h_abort, abort_flag.p, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
-  if (h_abort) return dmo_fail(ctx, DMO_ERR_INTERNAL, "gp_predict(tensor): pipeline watchdog tripped (mbarrier wait timed out)");
+  DMO_CUDA(cudaMemcpyAsync(&h_abort, abort_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
+  if (h_abort) return dmo_fail(ctx, DMO_ERR_INTERNAL, "%s", GP_WATCHDOG_MSG);
   return DMO_OK;
 }

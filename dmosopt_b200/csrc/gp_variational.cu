@@ -440,7 +440,7 @@ int dmo_svgp_create(dmo_ctx* ctx, int L, int M, int64_t Z, int d, const double* 
       ga.s[j] = hs[gr->lat[j]];
     }
     DMO_CHECK_LAUNCH();
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));  // host vectors above are staged from the stack
+    DMO_CUDA(dmo_wait(ctx));  // host vectors above are staged from the stack
     sv->groups.push_back(std::move(gr));
   }
   DMO_TRY(upload(ctx, sv->xlb, lb));
@@ -450,7 +450,7 @@ int dmo_svgp_create(dmo_ctx* ctx, int L, int M, int64_t Z, int d, const double* 
   DMO_TRY(upload(ctx, sv->ystd, ys));
   DMO_TRY(upload(ctx, sv->vscale, vs));
   DMO_CHECK_LAUNCH();
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   *out = sv.release();
   return DMO_OK;
 }
@@ -459,7 +459,7 @@ int dmo_svgp_destroy(dmo_ctx* ctx, dmo_svgp* sv) {
   if (!ctx) return DMO_ERR_ARG;
   if (!sv) return DMO_OK;
   DMO_CUDA(cudaSetDevice(ctx->device));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   delete sv;
   return DMO_OK;
 }
@@ -504,7 +504,7 @@ int dmo_svgp_predict(dmo_ctx* ctx, dmo_svgp* sv, const double* X, int64_t P, dou
   DMO_TRY(up.watchdog(ctx));
   DMO_TRY(om.finish(ctx));
   DMO_TRY(ov.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -586,7 +586,7 @@ int dmo_svgp_optimal_q(dmo_ctx* ctx, int64_t N, int64_t Z, int d, int L, const d
     // A' = s K(X, Z) Lz^-T  (N x Z):  At[p][i] = s sum_k Kxz[p][k] Li[i][k]
     DMO_TRY(sv_gemm(ctx,N, Z, Z, s, Kxz.p, Npad, 1, Li.p, 1, Z, 0.0, At.p, Z));
     DMO_CHECK_LAUNCH();
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));  // xsh / xtT are staged from the stack
+    DMO_CUDA(dmo_wait(ctx));  // xsh / xtT are staged from the stack
     }
     // B = I + A A' / sigma^2 (Z x Z)
     DMO_TRY(sv_gemm(ctx,Z, Z, N, 1.0 / s2, At.p, 1, Z, At.p, Z, 1, 1.0, Bm.p, Z));
@@ -598,7 +598,7 @@ int dmo_svgp_optimal_q(dmo_ctx* ctx, int64_t N, int64_t Z, int d, int L, const d
     DMO_TRY(gp_potrf_batched(ctx, Lci.p, ld, 1, info.p));
     int h_info = 0;
     DMO_CUDA(cudaMemcpyAsync(&h_info, info.p, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+    DMO_CUDA(dmo_wait(ctx));
     if (h_info) return dmo_fail(ctx, DMO_ERR_ARG, "svgp_optimal_q: I + A A' / noise of latent %d is not positive definite", l);
     DMO_CUDA(cudaMemsetAsync(Bm.p, 0, zz * sizeof(double), ctx->stream));
     DMO_TRY(gp_linv_from_factor_batched(ctx, Lci.p, ld, 0, Z, 1, Z, 0, Bm.p));  // Lc: the leading Z x Z block of Lci
@@ -608,11 +608,11 @@ int dmo_svgp_optimal_q(dmo_ctx* ctx, int64_t N, int64_t Z, int d, int L, const d
     DMO_TRY(sv_gemm(ctx,Z, 1, Z, 1.0, U, 1, Z, bvec.p, 1, 0, 0.0, tvec.p, 1));
     DMO_TRY(sv_gemm(ctx,Z, 1, Z, 1.0, U, Z, 1, tvec.p, 1, 0, 0.0, oqm.d + (size_t)l * Z, 1));
     DMO_CHECK_LAUNCH();
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));  // xsh / xtT are staged from the stack
+    DMO_CUDA(dmo_wait(ctx));  // xsh / xtT are staged from the stack
   }
   DMO_TRY(oqm.finish(ctx));
   DMO_TRY(oqs.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 

@@ -417,7 +417,7 @@ int svf_kernels(dmo_ctx* ctx, const char* who, dmo_svgp_fit* st, const SvfParams
                          kk.work.p, nullptr, nullptr));
   std::vector<int> h_info(K);
   DMO_CUDA(cudaMemcpyAsync(h_info.data(), kk.info.p, K * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   for (int k = 0; k < K; ++k)
     if (h_info[k]) return dmo_fail(ctx, DMO_ERR_ARG, "%s: K(Z, Z) + jitter I of latent %d is not positive definite", who, p.lead[k]);
   DMO_TRY(gp_linv_from_factor_batched(ctx, kk.Lf.p, ld, ld * ld, Z, K, Z, zz, kk.Li.p));
@@ -505,7 +505,7 @@ int dmo_svgp_fit_create(dmo_ctx* ctx, int64_t N, int d, int M, int L, int64_t Z,
   DMO_TRY(upload(ctx, st->th1, zero));
   DMO_TRY(upload(ctx, st->m, zero));
   DMO_CHECK_LAUNCH();
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   *out = st.release();
   return DMO_OK;
 }
@@ -514,7 +514,7 @@ int dmo_svgp_fit_destroy(dmo_ctx* ctx, dmo_svgp_fit* st) {
   if (!ctx) return DMO_ERR_ARG;
   if (!st) return DMO_OK;
   DMO_CUDA(cudaSetDevice(ctx->device));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   delete st;
   return DMO_OK;
 }
@@ -557,7 +557,7 @@ int dmo_svgp_fit_natgrad(dmo_ctx* ctx, dmo_svgp_fit* st, const int64_t* batch, i
   DMO_TRY(gp_potrf_batched(ctx, LamJ.p, lc, L, info.p));
   std::vector<int> h_info(L);
   DMO_CUDA(cudaMemcpyAsync(h_info.data(), info.p, L * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   for (int l = 0; l < L; ++l)
     if (h_info[l]) return dmo_fail(ctx, DMO_ERR_ARG, "svgp_fit_natgrad: the precision Lambda of latent %d is not positive definite", l);
   DMO_CUDA(cudaMemsetAsync(Lci.p, 0, (size_t)L * zz * sizeof(double), ctx->stream));
@@ -570,7 +570,7 @@ int dmo_svgp_fit_natgrad(dmo_ctx* ctx, dmo_svgp_fit* st, const int64_t* batch, i
     DMO_TRY(sv_gemm(ctx, Z, 1, Z, 1.0, U, Z, 1, Ar.p, 1, 0, 0.0, st->m.p + (size_t)l * Z, 1));
   }
   DMO_CHECK_LAUNCH();
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -659,7 +659,7 @@ int dmo_svgp_fit_elbo_grad(dmo_ctx* ctx, dmo_svgp_fit* st, const int64_t* batch,
   DMO_TRY(o_gl.finish(ctx));
   DMO_TRY(o_gn.finish(ctx));
   DMO_TRY(o_gw.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -670,7 +670,7 @@ int dmo_svgp_fit_q(dmo_ctx* ctx, dmo_svgp_fit* st, double* q_mu_out, double* q_s
   const size_t zz = (size_t)st->Z * st->Z;
   DMO_CUDA(cudaMemcpyAsync(q_mu_out, st->m.p, (size_t)st->L * st->Z * sizeof(double), cudaMemcpyDefault, ctx->stream));
   DMO_CUDA(cudaMemcpyAsync(q_sqrt_out, st->U.p, st->L * zz * sizeof(double), cudaMemcpyDefault, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 

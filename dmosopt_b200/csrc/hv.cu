@@ -429,7 +429,7 @@ int compact_rows(dmo_ctx* ctx, const double* dF, int64_t n, int M, DevBuf<int32_
   DMO_TRY(prim_exclusive_sum_i32(ctx, flag.p, pos.p, n + 1));
   int32_t h = 0;
   DMO_CUDA(cudaMemcpyAsync(&h, pos.p + n, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   *count = h;
   DMO_TRY(out.alloc(ctx, (size_t)(h > 0 ? h : 1) * M));
   if (h > 0) DMO_LAUNCH(compact_rows_kernel, (unsigned)ceil_div(n, 256), 256, 0, dF, n, M, flag.p, pos.p, out.p);
@@ -486,7 +486,7 @@ int sum_partials(dmo_ctx* ctx, DevBuf<double>& partial, int64_t nb, double* h_ou
   DMO_LAUNCH(final_sum_kernel, 1, 256, 0, partial.p, nb, res.p);
   DMO_CHECK_LAUNCH();
   DMO_CUDA(cudaMemcpyAsync(h_out, res.p, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -548,7 +548,7 @@ int hypervolume_device_ranked(dmo_ctx* ctx, const double* dF, int64_t n, int M, 
     DMO_CHECK_LAUNCH();
     double h = 0.0;
     DMO_CUDA(cudaMemcpyAsync(&h, mn.p, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+    DMO_CUDA(dmo_wait(ctx));
     *h_out = h_ref[0] - h;
     return DMO_OK;
   }
@@ -706,7 +706,7 @@ int dmo_nondominated_flags(dmo_ctx* ctx, const double* Y, int64_t n, int M, int3
   DMO_LAUNCH(dominated_flag_kernel, (unsigned)ceil_div(n, 256), 256, 0, keep.p, n, f.d);
   DMO_CHECK_LAUNCH();
   DMO_TRY(f.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -760,7 +760,7 @@ int dmo_ehvi_select(dmo_ctx* ctx, const double* F, int64_t nf, const double* mea
   DMO_TRY(prim_exclusive_sum_i32(ctx, flag.p, pos.p, nfr + 2));
   int32_t nb = 0;
   DMO_CUDA(cudaMemcpyAsync(&nb, pos.p + nfr + 1, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   DevBuf<double> lower, upper, sc;
   DMO_TRY(lower.alloc(ctx, (size_t)(nb > 0 ? nb : 1) * M));
   DMO_TRY(upper.alloc(ctx, (size_t)(nb > 0 ? nb : 1) * M));
@@ -792,7 +792,7 @@ int dmo_ehvi_select(dmo_ctx* ctx, const double* F, int64_t nf, const double* mea
   DMO_CHECK_LAUNCH();
   DMO_TRY(osel.finish(ctx));
   DMO_TRY(osc.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 

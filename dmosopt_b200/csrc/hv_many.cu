@@ -217,7 +217,7 @@ int run_many(dmo_ctx* ctx, const double* dP, int n, const double* dref, double* 
     // largest limit set decides the arena of a task; the k range is processed in chunks that keep the arena under ~4 GiB
     std::vector<int> hc(n);
     DMO_CUDA(cudaMemcpyAsync(hc.data(), cnt.p, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+    DMO_CUDA(dmo_wait(ctx));
     int n_max = 1;
     for (int k = 0; k < n; ++k) n_max = hc[k] > n_max ? hc[k] : n_max;
     const size_t per_k = (size_t)n_max * arena_doubles(D2, n_max) * sizeof(double);
@@ -235,7 +235,7 @@ int run_many(dmo_ctx* ctx, const double* dP, int n, const double* dref, double* 
   }
   DMO_CHECK_LAUNCH();
   DMO_CUDA(cudaMemcpyAsync(h_out, res.p, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 

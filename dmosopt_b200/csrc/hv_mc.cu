@@ -266,7 +266,7 @@ int run_fpras(dmo_ctx* ctx, const McFront& f, int64_t target, FprasState& st) {
     DMO_CHECK_LAUNCH();
     unsigned long long h[2];
     DMO_CUDA(cudaMemcpyAsync(h, sums.p, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+    DMO_CUDA(dmo_wait(ctx));
     if (h[1] == 0 && (int64_t)h[0] <= R) {  // the whole wave fits the budget
       st.N += S;
       st.sum_xi += (int64_t)h[0];
@@ -279,7 +279,7 @@ int run_fpras(dmo_ctx* ctx, const McFront& f, int64_t target, FprasState& st) {
     // straddles the target: it is discarded, its tests are spent, and the next round starts at the sample after it.
     hxi.resize((size_t)S);
     DMO_CUDA(cudaMemcpyAsync(hxi.data(), xi.p, (size_t)S * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+    DMO_CUDA(dmo_wait(ctx));
     int64_t used = 0, s = 0;
     for (; s < S && used < R; ++s) {
       if (hxi[s] == 0 || used + hxi[s] > R) break;
@@ -321,7 +321,7 @@ int run_mcm2rv(dmo_ctx* ctx, const McFront& f, double eps, double delta, int64_t
     DMO_CHECK_LAUNCH();
     unsigned long long h[3];
     DMO_CUDA(cudaMemcpyAsync(h, sums.p, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+    DMO_CUDA(dmo_wait(ctx));
     if (Ssum + (int64_t)h[1] < R) {
       N += (int64_t)h[0];
       Ssum += (int64_t)h[1];
@@ -332,7 +332,7 @@ int run_mcm2rv(dmo_ctx* ctx, const McFront& f, double eps, double delta, int64_t
     }
     hc.resize((size_t)S);
     DMO_CUDA(cudaMemcpyAsync(hc.data(), code.p, (size_t)S * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+    DMO_CUDA(dmo_wait(ctx));
     for (int64_t s = 0; s < S && Ssum < R; ++s) {
       const uint32_t kind = hc[s] >> 30;
       tests += (int64_t)(hc[s] & 0x3FFFFFFFu);
@@ -377,7 +377,7 @@ extern "C" int dmo_hypervolume_mc(dmo_ctx* ctx, const double* F, int64_t n, int 
   int64_t nf = 0;
   DMO_TRY(hv_inside_nondominated(ctx, f.d, n, M, dref.p, front, &nf));
   if (nf == 0) {
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+    DMO_CUDA(dmo_wait(ctx));
     return DMO_OK;
   }
   DMO_REQUIRE(nf < ((int64_t)1 << 32), "hypervolume_mc: front too large (%lld rows)", (long long)nf);
@@ -387,7 +387,7 @@ extern "C" int dmo_hypervolume_mc(dmo_ctx* ctx, const double* F, int64_t n, int 
   // box volumes, W, the sampling CDF, the ideal point and U: O(n M) once, in row order on the host
   std::vector<double> hF((size_t)nf * M), cdf((size_t)nf), ideal(M);
   DMO_CUDA(cudaMemcpyAsync(hF.data(), front.p, hF.size() * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   double W = 0.0;
   for (int j = 0; j < M; ++j) ideal[j] = hF[j];
   for (int64_t i = 0; i < nf; ++i) {
@@ -460,7 +460,7 @@ extern "C" int dmo_hypervolume_mc(dmo_ctx* ctx, const double* F, int64_t n, int 
       DMO_CHECK_LAUNCH();
       unsigned long long h[3];
       DMO_CUDA(cudaMemcpyAsync(h, sums.p, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
-      DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+      DMO_CUDA(dmo_wait(ctx));
       dom = h[0];
       tests += (int64_t)h[2];
       samples += n_samples;
@@ -491,7 +491,7 @@ extern "C" int dmo_hypervolume_mc(dmo_ctx* ctx, const double* F, int64_t n, int 
       DMO_CHECK_LAUNCH();
       int64_t hp[N_PROBES];
       DMO_CUDA(cudaMemcpyAsync(hp, pxi.p, sizeof(hp), cudaMemcpyDeviceToHost, ctx->stream));
-      DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+      DMO_CUDA(dmo_wait(ctx));
       double mean_xi = 0.0;
       for (int p = 0; p < N_PROBES; ++p) mean_xi += (double)hp[p];
       mean_xi /= N_PROBES;

@@ -348,7 +348,7 @@ int dmo_gather_rows(dmo_ctx* ctx, const double* src, const double* alt, const ui
   DMO_TRY(is.init(ctx, sel, (size_t)n));
   DMO_LAUNCH(gather_rows_kernel, (unsigned)ceil_div(n * row_elems, 256), 256, 0, src, alt, is.d, ii.d, n, row_elems, dst);
   DMO_CHECK_LAUNCH();
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -377,7 +377,7 @@ int dmo_age_survival(dmo_ctx* ctx, const double* yn, const double* nn, int64_t m
   }
   DMO_CHECK_LAUNCH();
   DMO_TRY(oc.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -402,7 +402,7 @@ int dmo_smpso_velocity(dmo_ctx* ctx, const float* position, const double* veloci
              c1 * r1, c2 * r2, chi, ilb.d, iub.d, oo.d);
   DMO_CHECK_LAUNCH();
   DMO_TRY(oo.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -428,7 +428,7 @@ int dmo_mutate_groups(dmo_ctx* ctx, const double* pop_x, int64_t group_size, int
   DMO_CHECK_LAUNCH();
   DMO_TRY(oc.finish(ctx));
   DMO_TRY(opar.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -452,7 +452,7 @@ int dmo_cmaes_sample(dmo_ctx* ctx, const double* parents_x, const double* sigmas
              oo.d);
   DMO_CHECK_LAUNCH();
   DMO_TRY(oo.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -484,7 +484,7 @@ int dmo_cmaes_generate(dmo_ctx* ctx, const double* parents_x, const double* sigm
   DMO_LAUNCH(cmaes_rescale_kernel, (unsigned)ceil_div(n * d, 256), 256, 0, oo.d, n, d, mx.p, ilb.d, iub.d);
   DMO_CHECK_LAUNCH();
   DMO_TRY(oo.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -505,7 +505,7 @@ int dmo_cmaes_step_z(dmo_ctx* ctx, const double* x_gen, const int64_t* cand_idx,
   DMO_TRY(iub.init(ctx, xub, (size_t)d));
   DMO_LAUNCH(cmaes_z_kernel, (unsigned)ceil_div(n * d, 256), 256, 0, x_gen, ici.d, parents_x, ipi.d, ilb.d, iub.d, steps, n, d, z_out);
   DMO_CHECK_LAUNCH();
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -523,7 +523,7 @@ int dmo_scale_rows(dmo_ctx* ctx, double* rows, int64_t row_elems, int64_t n_seg,
   DMO_TRY(ifa.init(ctx, factors, (size_t)n_factors));
   DMO_LAUNCH(scale_rows_kernel, (unsigned)ceil_div(n_seg * row_elems, 256), 256, 0, rows, row_elems, n_seg, isr.d, iss.d, ifa.d);
   DMO_CHECK_LAUNCH();
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -560,7 +560,7 @@ int dmo_cmaes_update_cholesky(dmo_ctx* ctx, double* A, double* Ainv, double* pc,
     DMO_CUDA(cudaMemcpyAsync(pc, ppc, (size_t)n * d * 8, cudaMemcpyDeviceToHost, ctx->stream));
     ctx->d2h_bytes += (uint64_t)n * d * (2 * d + 1) * 8;
   }
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 

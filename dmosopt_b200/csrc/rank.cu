@@ -848,7 +848,7 @@ int launch_chain(dmo_ctx* ctx, uint32_t* rec, int nblocks, int* rankS, int* tick
   if (trace.p) {
     std::vector<long long> h((size_t)nblocks * 32);
     DMO_CUDA(cudaMemcpyAsync(h.data(), trace.p, h.size() * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+    DMO_CUDA(dmo_wait(ctx));
     if (FILE* f = fopen(trace_path, "wb")) {
       fwrite(h.data(), sizeof(long long), h.size(), f);
       fclose(f);
@@ -1023,14 +1023,16 @@ int build_cell_grid(dmo_ctx* ctx, const GridIds& ids, int64_t n, int gbits, bool
   cg.gbits = gbits;
   const int GG = 1 << (2 * gbits);
   const unsigned g = (unsigned)ceil_div(n, 256);
-  DevBuf<uint32_t> key0, keyA, keyB, keyS, keyT, ord0, ordS, iota;
+  DevBuf<uint32_t> key0, keyA, keyB, keyS[2], keyT[2], ord0, ordS[2], iota;
   DMO_TRY(key0.alloc(ctx, n));
   DMO_TRY(keyA.alloc(ctx, n));
   DMO_TRY(keyB.alloc(ctx, n));
-  DMO_TRY(keyS.alloc(ctx, n));
-  DMO_TRY(keyT.alloc(ctx, n));
+  for (int pass = 0; pass < 2; ++pass) {
+    DMO_TRY(keyS[pass].alloc(ctx, n));
+    DMO_TRY(keyT[pass].alloc(ctx, n));
+    DMO_TRY(ordS[pass].alloc(ctx, n));
+  }
   DMO_TRY(ord0.alloc(ctx, n));
-  DMO_TRY(ordS.alloc(ctx, n));
   DMO_TRY(iota.alloc(ctx, n));
   DMO_TRY(cg.cstartA.alloc(ctx, GG + 1));
   DMO_TRY(cg.cstartB.alloc(ctx, GG + 1));
@@ -1044,12 +1046,20 @@ int build_cell_grid(dmo_ctx* ctx, const GridIds& ids, int64_t n, int gbits, bool
   }
   DMO_LAUNCH(grid_key_kernel, g, 256, 0, ids, n, gbits, key0.p, keyA.p, keyB.p);
   DMO_TRY(prim_iota_u32(ctx, iota.p, n));
-  DMO_TRY(prim_sort_pairs_u32(ctx, key0.p, keyS.p, iota.p, ord0.p, n, 0, bits_for(n)));  // by objective-1 id ...
-  for (int pass = 0; pass < 2; ++pass) {                                                // ... then stably by cell
-    DMO_TRY(prim_gather_u32(ctx, pass == 0 ? keyA.p : keyB.p, ord0.p, n, keyT.p));
-    DMO_TRY(prim_sort_pairs_u32(ctx, keyT.p, keyS.p, ord0.p, ordS.p, n, 0, 2 * gbits));
-    DMO_LAUNCH(grid_gather_kernel, g, 256, 0, ids, ordS.p, n, pass == 0 ? cg.crecA.p : cg.crecB.p, pass == 0 ? cg.slotA.p : cg.slotB.p);
-    DMO_LAUNCH(grid_start_kernel, (unsigned)ceil_div(GG + 1, 256), 256, 0, keyS.p, n, GG, pass == 0 ? cg.cstartA.p : cg.cstartB.p);
+  DMO_TRY(prim_sort_pairs_u32(ctx, key0.p, keyS[0].p, iota.p, ord0.p, n, 0, bits_for(n)));  // by objective-1 id ...
+  {  // ... then stably by cell, the two copies side by side
+    SideStreams side(ctx, 2);
+    DMO_TRY(side.rc);
+    for (int pass = 0; pass < 2; ++pass) {
+      side.on(pass);
+      DMO_TRY(prim_gather_u32(ctx, pass == 0 ? keyA.p : keyB.p, ord0.p, n, keyT[pass].p));
+      DMO_TRY(prim_sort_pairs_u32(ctx, keyT[pass].p, keyS[pass].p, ord0.p, ordS[pass].p, n, 0, 2 * gbits));
+      DMO_LAUNCH(grid_gather_kernel, g, 256, 0, ids, ordS[pass].p, n, pass == 0 ? cg.crecA.p : cg.crecB.p,
+                 pass == 0 ? cg.slotA.p : cg.slotB.p);
+      DMO_LAUNCH(grid_start_kernel, (unsigned)ceil_div(GG + 1, 256), 256, 0, keyS[pass].p, n, GG,
+                 pass == 0 ? cg.cstartA.p : cg.cstartB.p);
+    }
+    side.back();
   }
   if (peel) DMO_CUDA(cudaMemcpyAsync(cg.first.p, cg.cstartA.p, (size_t)GG * sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->stream));
   DMO_CHECK_LAUNCH();
@@ -1168,6 +1178,7 @@ int rank_by_peeling(dmo_ctx* ctx, const uint32_t* R, const uint32_t* maxid, int6
   if (const char* e = getenv("DMO_RANK_PEEL")) max_peels = atoi(e);
   if (max_peels <= 0) return DMO_OK;
   ProfileScope ps(ctx, "rank_peel");
+  double front_guess;  // the expected size of the front the host reads next: from the probe for front 0
   {  // probe before building anything: fewer than two undominated probes = a first front below ~1 % of the set
     DevBuf<unsigned> pd;
     DMO_TRY(pd.alloc(ctx, PEEL_PROBE / 32));
@@ -1177,10 +1188,11 @@ int rank_by_peeling(dmo_ctx* ctx, const uint32_t* R, const uint32_t* maxid, int6
     DMO_CHECK_LAUNCH();
     unsigned h[PEEL_PROBE / 32];
     DMO_CUDA(cudaMemcpyAsync(h, pd.p, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+    DMO_CUDA(dmo_wait(ctx));
     int free_probes = PEEL_PROBE;
     for (int w = 0; w < PEEL_PROBE / 32; ++w) free_probes -= __builtin_popcount(h[w]);
     if (free_probes < 2 && !(getenv("DMO_RANK_PEEL_NOPROBE") && atoi(getenv("DMO_RANK_PEEL_NOPROBE")))) return DMO_OK;
+    front_guess = (double)free_probes * (double)n / PEEL_PROBE;
   }
   const int bits = bits_for(n);
   int gbits = (bits + 1) / 2;  // two cells per point at n = 131 072: measured 0.80 ms per bench step against 0.96 ms with 2^8 cells per axis
@@ -1198,33 +1210,56 @@ int rank_by_peeling(dmo_ctx* ctx, const uint32_t* R, const uint32_t* maxid, int6
   DMO_TRY(count.alloc(ctx, 1));
   DMO_LAUNCH(fill_u8_kernel, g, 256, 0, alive.p, n, (uint8_t)1);
   DMO_CUDA(cudaMemsetAsync(count.p, 0, sizeof(unsigned long long), ctx->stream));
+  DMO_TRY(dmo_lag_slots(ctx));
+  // peel front j; the running count of ranked rows lands in lag_host[j & 1], lag_ev[j & 1] marks it
+  auto peel = [&](int j) -> int {
+    DMO_TRY(grid_dominated(ctx, cg, ids, n, alive.p, dom.p));
+    DMO_LAUNCH(peel_mark_kernel, g, 256, 0, n, alive.p, dom.p, j, d_rank, cg.slotA.p, cg.slotB.p, cg.crecA.p, cg.crecB.p, count.p);
+    DMO_CHECK_LAUNCH();
+    DMO_CUDA(cudaMemcpyAsync(ctx->lag_host + (j & 1), count.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
+    DMO_CUDA(cudaEventRecord(ctx->lag_ev[j & 1], ctx->stream));
+    return DMO_OK;
+  };
+  // When front k is not expected to complete the `keep` rows (nor, for the first front, to be small enough to give up on),
+  // front k + 1 is enqueued before the host reads front k's count, so the GPU peels while the host waits and decides.  A guess that turns out
+  // wrong changes no kept rank: if front k completes the `keep` rows, peel k + 1 ranks k + 1 rows peel_rest_kernel would
+  // rank k + 1 anyway; if the forecast gives up, the chain overwrites every rank.  It costs one peel, which is why the
+  // last front is not guessed past.
   unsigned long long ranked = 0, before = 0;
   double prev_front = 0.0;
-  int k = 0;
+  int k = 0, queued = 1;
+  DMO_TRY(peel(0));
   for (;; ++k) {
-    DMO_TRY(grid_dominated(ctx, cg, ids, n, alive.p, dom.p));
-    DMO_LAUNCH(peel_mark_kernel, g, 256, 0, n, alive.p, dom.p, k, d_rank, cg.slotA.p, cg.slotB.p, cg.crecA.p, cg.crecB.p, count.p);
-    DMO_CHECK_LAUNCH();
+    if (queued == k + 1 && (double)ranked + front_guess < (double)keep && (k > 0 || front_guess * 64.0 >= (double)keep)) {
+      DMO_TRY(peel(k + 1));
+      ++queued;
+    }
     before = ranked;
-    DMO_CUDA(cudaMemcpyAsync(&ranked, count.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+    ctx->waits++;
+    DMO_CUDA(cudaEventSynchronize(ctx->lag_ev[k & 1]));
+    ranked = ctx->lag_host[k & 1];
     if ((int64_t)ranked >= keep || (int64_t)ranked >= n) break;
     // Give up when many peels are still ahead.  Fronts usually grow over the first few peels (the bench's sets: 2.4 k,
     // then 5 - 12 k points per front), so the forecast extrapolates the last two front sizes linearly, and the first
     // front only decides when it is tiny (a uniform cloud: 72 of 131 072 points).
     const double last = (double)(ranked - before);
+    const double grow = last > prev_front ? last - prev_front : 0.0;
     bool give_up;
     if (k == 0) {
       give_up = last * 64.0 < (double)keep;
     } else {
       const double rem = (double)(keep - (int64_t)ranked);
-      const double grow = last > prev_front ? last - prev_front : 0.0;
       const double b = last + 0.5 * grow;
       const double ahead = grow > 0.0 ? (-b + sqrt(b * b + 2.0 * grow * rem)) / grow : rem / (last > 0.0 ? last : 1.0);
       give_up = (double)(k + 1) + ahead > (double)max_peels;
     }
     if (give_up) return DMO_OK;  // *done stays false: the chain takes over
     prev_front = last;
+    front_guess = last + grow;
+    if (queued == k + 1) {
+      DMO_TRY(peel(k + 1));
+      ++queued;
+    }
   }
   DMO_LAUNCH(peel_rest_kernel, g, 256, 0, n, alive.p, k + 1, d_rank);
   DMO_CHECK_LAUNCH();
@@ -1242,22 +1277,32 @@ int dense_ids(dmo_ctx* ctx, const double* dY, int64_t n, int M, DevBuf<uint32_t>
   const unsigned g = (unsigned)ceil_div(n, 256);
   DMO_TRY(R.alloc(ctx, (size_t)M * n));
   DMO_TRY(maxid.alloc(ctx, M));
-  DevBuf<uint64_t> k0, k1;
-  DevBuf<uint32_t> i0, i1, flag, dense;
-  DMO_TRY(k0.alloc(ctx, n));
-  DMO_TRY(k1.alloc(ctx, n));
-  DMO_TRY(i0.alloc(ctx, n));
-  DMO_TRY(i1.alloc(ctx, n));
-  DMO_TRY(flag.alloc(ctx, n));
-  DMO_TRY(dense.alloc(ctx, n));
-  for (int j = 0; j < M; ++j) {
-    DMO_TRY(prim_col_keys(ctx, dY, n, M, j, k0.p, i0.p));
-    DMO_TRY(prim_sort_pairs_u64(ctx, k0.p, k1.p, i0.p, i1.p, n, 0, 64));
-    DMO_LAUNCH(flag_new_u64_kernel, g, 256, 0, k1.p, n, flag.p);
-    DMO_TRY(prim_inclusive_sum_u32(ctx, flag.p, dense.p, n));
-    DMO_LAUNCH(scatter_dense_kernel, g, 256, 0, dense.p, i1.p, n, R.p + (size_t)j * n);
-    DMO_CUDA(cudaMemcpyAsync(maxid.p + j, dense.p + (n - 1), sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->stream));
+  // the objectives are independent: each sorts on a side stream of its own (up to four at a time), so the latency-bound
+  // radix passes of the columns overlap instead of queueing one column behind the other
+  const int ns = M < dmo_ctx::kSide ? M : dmo_ctx::kSide;
+  DevBuf<uint64_t> k0[dmo_ctx::kSide], k1[dmo_ctx::kSide];
+  DevBuf<uint32_t> i0[dmo_ctx::kSide], i1[dmo_ctx::kSide], flag[dmo_ctx::kSide], dense[dmo_ctx::kSide];
+  for (int s = 0; s < ns; ++s) {
+    DMO_TRY(k0[s].alloc(ctx, n));
+    DMO_TRY(k1[s].alloc(ctx, n));
+    DMO_TRY(i0[s].alloc(ctx, n));
+    DMO_TRY(i1[s].alloc(ctx, n));
+    DMO_TRY(flag[s].alloc(ctx, n));
+    DMO_TRY(dense[s].alloc(ctx, n));
   }
+  SideStreams side(ctx, ns);
+  DMO_TRY(side.rc);
+  for (int j = 0; j < M; ++j) {
+    const int s = j % ns;
+    side.on(s);
+    DMO_TRY(prim_col_keys(ctx, dY, n, M, j, k0[s].p, i0[s].p));
+    DMO_TRY(prim_sort_pairs_u64(ctx, k0[s].p, k1[s].p, i0[s].p, i1[s].p, n, 0, 64));
+    DMO_LAUNCH(flag_new_u64_kernel, g, 256, 0, k1[s].p, n, flag[s].p);
+    DMO_TRY(prim_inclusive_sum_u32(ctx, flag[s].p, dense[s].p, n));
+    DMO_LAUNCH(scatter_dense_kernel, g, 256, 0, dense[s].p, i1[s].p, n, R.p + (size_t)j * n);
+    DMO_CUDA(cudaMemcpyAsync(maxid.p + j, dense[s].p + (n - 1), sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->stream));
+  }
+  side.back();
   DMO_CHECK_LAUNCH();
   return DMO_OK;
 }
@@ -1390,7 +1435,7 @@ int rank_chain(dmo_ctx* ctx, const uint32_t* R, int64_t n, int M, int sshift, Ra
   DMO_CHECK_LAUNCH();
   int herr = 0;
   DMO_CUDA(cudaMemcpyAsync(&herr, errflag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   if (herr) return dmo_fail(ctx, DMO_ERR_INTERNAL, "rank_nd: chain kernel watchdog tripped");
   return DMO_OK;
 }
@@ -1450,6 +1495,6 @@ extern "C" int dmo_rank_nd(dmo_ctx* ctx, const double* Y, int64_t n, int M, int3
   DMO_TRY(r.init(ctx, rank, (size_t)n));
   DMO_TRY(rank_nd_device(ctx, y.d, n, M, r.d));
   DMO_TRY(r.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }

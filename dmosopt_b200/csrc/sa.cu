@@ -174,7 +174,7 @@ int dmo_sa_dgsm_design(dmo_ctx* ctx, const double* base, int64_t N, int d, const
   }
   DMO_CHECK_LAUNCH();
   DMO_TRY(ox.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -198,7 +198,7 @@ int dmo_sa_fast_design(dmo_ctx* ctx, int64_t N, int d, const double* omega, cons
   }
   DMO_CHECK_LAUNCH();
   DMO_TRY(ox.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -227,7 +227,7 @@ int dmo_sa_dgsm_stats(dmo_ctx* ctx, const double* X, const double* Y, int64_t N,
     if (dmo_is_device_ptr(boot_idx)) {
       host.resize((size_t)R * N);
       DMO_CUDA(cudaMemcpyAsync(host.data(), boot_idx, host.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
-      DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+      DMO_CUDA(dmo_wait(ctx));
       p = host.data();
     }
     int h = 0;
@@ -260,6 +260,6 @@ int dmo_sa_dgsm_stats(dmo_ctx* ctx, const double* X, const double* Y, int64_t N,
   DMO_TRY(o2.finish(ctx));
   DMO_TRY(o3.finish(ctx));
   DMO_TRY(o4.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }

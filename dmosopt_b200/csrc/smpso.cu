@@ -114,7 +114,7 @@ int dmo_smpso_generate(dmo_ctx* ctx, const double* parm, const double* vel, int 
   DMO_CHECK_LAUNCH();
   DMO_TRY(ox.finish(ctx));
   DMO_TRY(ox64.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -137,7 +137,7 @@ int dmo_smpso_update(dmo_ctx* ctx, double* parm, double* obj, double* vel, const
     In<float> xf;
     DMO_TRY(xf.init(ctx, (const float*)x_gen, (size_t)n * d));
     DMO_LAUNCH(f32_to_f64_kernel, (unsigned)ceil_div(n * d, 256), 256, 0, xf.d, n * d, xg.p);
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));  // xf is released at the end of this scope
+    DMO_CUDA(dmo_wait(ctx));  // xf is released at the end of this scope
   } else {
     DMO_CUDA(cudaMemcpyAsync(xg.p, x_gen, (size_t)n * d * sizeof(double), cudaMemcpyDefault, ctx->stream));
     if (!dmo_is_device_ptr(x_gen)) ctx->h2d_bytes += (uint64_t)n * d * sizeof(double);
@@ -184,17 +184,17 @@ int dmo_smpso_update(dmo_ctx* ctx, double* parm, double* obj, double* vel, const
     DMO_TRY(o.init(ctx, parm_f32, (size_t)n * d));
     DMO_LAUNCH(f64_to_f32_kernel, (unsigned)ceil_div(n * d, 256), 256, 0, parm, n * d, o.d);
     DMO_TRY(o.finish(ctx));
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+    DMO_CUDA(dmo_wait(ctx));
   }
   if (obj_f32) {
     Out<float> o;
     DMO_TRY(o.init(ctx, obj_f32, (size_t)n * M));
     DMO_LAUNCH(f64_to_f32_kernel, (unsigned)ceil_div(n * M, 256), 256, 0, obj, n * M, o.d);
     DMO_TRY(o.finish(ctx));
-    DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+    DMO_CUDA(dmo_wait(ctx));
   }
   DMO_CHECK_LAUNCH();
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 

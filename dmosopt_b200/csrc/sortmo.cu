@@ -435,6 +435,22 @@ static int order_mo_device(dmo_ctx* ctx, const double* dY, int64_t n, int M, int
   return DMO_OK;
 }
 
+// dmo_remove_worst on device arrays, keep <= n (any output may be null): no host wait of its own
+int remove_worst_device(dmo_ctx* ctx, const double* dX, const double* dY, int64_t n, int d, int M, int metric,
+                        const double* const* d_extra, int n_extra, int64_t keep, double* dX_out, double* dY_out, int32_t* d_rank_out,
+                        int64_t* d_perm_out) {
+  DevBuf<int32_t> rank;
+  DevBuf<double> dist;
+  DevBuf<uint32_t> p;
+  DMO_TRY(order_mo_device(ctx, dY, n, M, metric, d_extra, n_extra, rank, dist, p, keep));
+  if (dX_out) DMO_LAUNCH(gather_rows_kernel, (unsigned)ceil_div(keep * d, 256), 256, 0, dX, p.p, keep, d, dX_out);
+  if (dY_out) DMO_LAUNCH(gather_rows_kernel, (unsigned)ceil_div(keep * M, 256), 256, 0, dY, p.p, keep, M, dY_out);
+  DMO_LAUNCH(gather_sorted_kernel, (unsigned)ceil_div(keep, 256), 256, 0, rank.p, (const double*)nullptr, p.p, keep,
+             d_perm_out, d_rank_out, (double*)nullptr);
+  DMO_CHECK_LAUNCH();
+  return DMO_OK;
+}
+
 extern "C" {
 
 int dmo_crowding_distance(dmo_ctx* ctx, const double* Y, int64_t n, int M, double* D) {
@@ -448,7 +464,7 @@ int dmo_crowding_distance(dmo_ctx* ctx, const double* Y, int64_t n, int M, doubl
   DMO_TRY(d.init(ctx, D, (size_t)n));
   DMO_TRY(crowding_device(ctx, y.d, n, M, d.d));
   DMO_TRY(d.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -463,7 +479,7 @@ int dmo_euclidean_distance(dmo_ctx* ctx, const double* Y, int64_t n, int M, doub
   DMO_TRY(d.init(ctx, D, (size_t)n));
   DMO_TRY(euclidean_device(ctx, y.d, n, M, d.d));
   DMO_TRY(d.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -497,7 +513,7 @@ int dmo_order_mo(dmo_ctx* ctx, const double* Y, int64_t n, int M, int metric, co
   DMO_TRY(op.finish(ctx));
   DMO_TRY(orank.finish(ctx));
   DMO_TRY(odist.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -519,10 +535,6 @@ int dmo_remove_worst(dmo_ctx* ctx, const double* X, const double* Y, int64_t n, 
     DMO_TRY(ex[k].init(ctx, extra_desc_keys[k], (size_t)n));
     dex[k] = ex[k].d;
   }
-  DevBuf<int32_t> rank;
-  DevBuf<double> dist;
-  DevBuf<uint32_t> p;
-  DMO_TRY(order_mo_device(ctx, y.d, n, M, metric, dex, n_extra, rank, dist, p, keep));
   Out<double> ox, oy;
   Out<int32_t> orank;
   Out<int64_t> op;
@@ -530,16 +542,12 @@ int dmo_remove_worst(dmo_ctx* ctx, const double* X, const double* Y, int64_t n, 
   DMO_TRY(oy.init(ctx, Y_out, (size_t)keep * M));
   DMO_TRY(orank.init(ctx, rank_out, (size_t)keep));
   DMO_TRY(op.init(ctx, perm_out, (size_t)keep));
-  if (ox.d) DMO_LAUNCH(gather_rows_kernel, (unsigned)ceil_div(keep * d, 256), 256, 0, x.d, p.p, keep, d, ox.d);
-  if (oy.d) DMO_LAUNCH(gather_rows_kernel, (unsigned)ceil_div(keep * M, 256), 256, 0, y.d, p.p, keep, M, oy.d);
-  DMO_LAUNCH(gather_sorted_kernel, (unsigned)ceil_div(keep, 256), 256, 0, rank.p, (const double*)nullptr, p.p, keep,
-             op.d, orank.d, (double*)nullptr);
-  DMO_CHECK_LAUNCH();
+  DMO_TRY(remove_worst_device(ctx, x.d, y.d, n, d, M, metric, dex, n_extra, keep, ox.d, oy.d, orank.d, op.d));
   DMO_TRY(ox.finish(ctx));
   DMO_TRY(oy.finish(ctx));
   DMO_TRY(orank.finish(ctx));
   DMO_TRY(op.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -596,7 +604,7 @@ static int remove_worst_pair_impl(dmo_ctx* ctx, const double* Xa, const double* 
   DMO_TRY(oy.finish(ctx));
   DMO_TRY(orank.finish(ctx));
   DMO_TRY(op.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -636,7 +644,7 @@ int dmo_get_duplicates(dmo_ctx* ctx, const double* X, int64_t n, int d, double e
   DMO_LAUNCH(duplicates_kernel, g, 256, 0, x.d, k1.p, i1.p, n, d, eps, o.d);
   DMO_CHECK_LAUNCH();
   DMO_TRY(o.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -664,7 +672,7 @@ int dmo_get_duplicates_pair(dmo_ctx* ctx, const double* X, int64_t n, const doub
   DMO_LAUNCH(duplicates_pair_kernel, g, 256, 0, x.d, n, y.d, ny, k1.p, i1.p, d, eps, o.d);
   DMO_CHECK_LAUNCH();
   DMO_TRY(o.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 

@@ -5,8 +5,13 @@
 //   tournament (NSGA2.py:116-140) -> variation loop (NSGA2.py:142-178) -> GP posterior mean [+ variance]
 //   (model.py:1254-1275) -> children stacked over parents, rank + stable truncation (NSGA2.py:205-214, MOEA.py:398-423)
 //   -> float32 rounding of the stored objectives (NSGA2.py:228-230) -> optional hypervolume of the survivors.
-// It is a composition of the entry points of this library on device buffers (no host round trips except the offspring
-// count and the hypervolume value); bench.py's `value` leg is this call.
+// It is a composition of the device bodies of this library's entry points, without their trailing waits.  The host waits
+// only for values it needs: the offspring count (it sizes the GP launch), one read-back after the GP (watchdog and rows to
+// refine, read once the truncation is enqueued behind it), the rank's (the peel probe and one count per peeled front, mostly read while the next front is peeled; or the
+// chain's watchdog) and the hypervolume's (its route and its value).  bench.py's `value` leg is this call;
+// scripts/step_phases.py times its phases (the step_* profile scopes) and counts the waits.
+#include <string.h>
+
 #include "common.cuh"
 #include "gp.cuh"
 
@@ -18,7 +23,8 @@ int dmo_nsga2_step(dmo_ctx* ctx, dmo_gp* gp, double* pop_x, double* pop_y, int32
                    double* hv_out) {
   if (!ctx) return DMO_ERR_ARG;
   DMO_CUDA(cudaSetDevice(ctx->device));
-  DMO_REQUIRE(gp && pop_x && pop_y && rank && pop >= 2 && d >= 1 && M >= 1, "nsga2_step: bad arguments");
+  DMO_REQUIRE(gp && pop_x && pop_y && rank && pop >= 2 && d >= 1 && M >= 1 && di_crossover && di_mutation && xlb && xub,
+              "nsga2_step: bad arguments");
   DMO_REQUIRE(distance_metric == DMO_METRIC_NONE || distance_metric == DMO_METRIC_CROWDING || distance_metric == DMO_METRIC_EUCLIDEAN,
               "nsga2_step: unknown distance metric %d", distance_metric);
   DMO_REQUIRE(dmo_is_device_ptr(pop_x) && dmo_is_device_ptr(pop_y) && dmo_is_device_ptr(rank),
@@ -35,31 +41,71 @@ int dmo_nsga2_step(dmo_ctx* ctx, dmo_gp* gp, double* pop_x, double* pop_y, int32
   DMO_TRY(Ys.alloc(ctx, (size_t)(cap + pop) * M));
   DMO_TRY(kind.alloc(ctx, cap));
   if (with_variance) DMO_TRY(var.alloc(ctx, (size_t)cap * M));
-  int rc = dmo_tournament(ctx, rank, nullptr, pop, poolsize, seed, stream_id, pool.p, nullptr);
-  if (rc != DMO_OK) return rc;
-  int64_t P = 0;
-  rc = dmo_nsga2_generate(ctx, pop_x, pop, d, pool.p, poolsize, pop, crossover_prob, mutation_prob, mutation_rate,
-                          di_crossover, di_mutation, xlb, xub, seed, stream_id + 1, Xs.p, kind.p, &P, nullptr);
-  if (rc != DMO_OK) return rc;
-  if (n_children) *n_children = P;
-  rc = dmo_gp_predict(ctx, gp, Xs.p, P, Ys.p, with_variance ? var.p : nullptr, precision);
-  if (rc != DMO_OK) return rc;
-  // parents under the children (np.vstack((x_gen, population_parm)), NSGA2.py:205-206)
-  DMO_CUDA(cudaMemcpyAsync(Xs.p + (size_t)P * d, pop_x, (size_t)pop * d * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
-  DMO_CUDA(cudaMemcpyAsync(Ys.p + (size_t)P * M, pop_y, (size_t)pop * M * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
-  rc = dmo_remove_worst(ctx, Xs.p, Ys.p, P + pop, d, M, distance_metric, nullptr, 0, pop, pop_x, pop_y, rank, perm.p);
-  if (rc != DMO_OK) return rc;
-  if (round_to_f32) {
-    rc = dmo_round_f32(ctx, pop_y, pop * M);
-    if (rc != DMO_OK) return rc;
+  In<double> idc, idm, ilb, iub;
+  DMO_TRY(idc.init(ctx, di_crossover, d));
+  DMO_TRY(idm.init(ctx, di_mutation, d));
+  DMO_TRY(ilb.init(ctx, xlb, d));
+  DMO_TRY(iub.init(ctx, xub, d));
+  {
+    ProfileScope ps(ctx, "step_tournament");
+    DMO_TRY(tournament_device(ctx, rank, nullptr, pop, poolsize, seed, stream_id, pool.p, nullptr));
   }
+  int64_t P = 0;
+  {
+    ProfileScope ps(ctx, "step_generate");
+    DMO_TRY(nsga2_generate_device(ctx, pop_x, d, pool.p, poolsize, pop, crossover_prob, mutation_prob, mutation_rate, idc.d, idm.d,
+                                  ilb.d, iub.d, seed, stream_id + 1, Xs.p, kind.p, &P, nullptr));
+  }
+  if (n_children) *n_children = P;
+  {
+    ProfileScope ps(ctx, "step_truncate");
+    // parents under the children (np.vstack((x_gen, population_parm)), NSGA2.py:205-206); the GP reads and writes the rows
+    // above them only, so the copies are enqueued first and the host does not issue them after the GP's read-back
+    DMO_CUDA(cudaMemcpyAsync(Xs.p + (size_t)P * d, pop_x, (size_t)pop * d * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
+    DMO_CUDA(cudaMemcpyAsync(Ys.p + (size_t)P * M, pop_y, (size_t)pop * M * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
+  }
+  // The GP's read-back is left pending and the truncation is enqueued behind it, so the host issues the truncation's first
+  // launches while the GP runs; the truncation's own first wait comes after the GP anyway.  If the GP then fails, the
+  // population is put back (the parents are still in Xs / Ys); if AUTO refines rows, the truncation runs again on them.
+  GpPending gpp;
+  DevBuf<int32_t> rank_in;
+  if (P > 0) {
+    ProfileScope ps(ctx, "step_gp");
+    DMO_TRY(gp_predict_device(ctx, gp, Xs.p, P, Ys.p, with_variance ? var.p : nullptr, precision, &gpp));
+  }
+  if (gpp.active) {
+    DMO_TRY(rank_in.alloc(ctx, pop));
+    DMO_CUDA(cudaMemcpyAsync(rank_in.p, rank, (size_t)pop * sizeof(int32_t), cudaMemcpyDeviceToDevice, ctx->stream));
+  }
+  auto truncate = [&]() -> int {
+    ProfileScope ps(ctx, "step_truncate");
+    DMO_TRY(remove_worst_device(ctx, Xs.p, Ys.p, P + pop, d, M, distance_metric, nullptr, 0, pop, pop_x, pop_y, rank, perm.p));
+    if (round_to_f32) DMO_TRY(prim_round_f32(ctx, pop_y, pop * M));
+    return DMO_OK;
+  };
+  DMO_TRY(truncate());
+  bool refined = false;
+  const int rc = gp_predict_finish(ctx, gp, gpp, &refined);
+  if (rc != DMO_OK) {
+    DMO_CUDA(cudaMemcpyAsync(pop_x, Xs.p + (size_t)P * d, (size_t)pop * d * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
+    DMO_CUDA(cudaMemcpyAsync(pop_y, Ys.p + (size_t)P * M, (size_t)pop * M * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
+    DMO_CUDA(cudaMemcpyAsync(rank, rank_in.p, (size_t)pop * sizeof(int32_t), cudaMemcpyDeviceToDevice, ctx->stream));
+    DMO_CUDA(dmo_wait(ctx));
+    return rc;
+  }
+  if (refined) DMO_TRY(truncate());
   if (hv_ref && hv_out) {
+    ProfileScope ps(ctx, "step_hv");
     // the survivors carry their ranks within the merged set: rows of rank > 0 cannot add volume (hv.cu)
     DMO_REQUIRE(M <= 16, "nsga2_step: too many objectives for the hypervolume");
     double h_ref[16];
-    DMO_CUDA(cudaMemcpy(h_ref, hv_ref, M * sizeof(double), cudaMemcpyDefault));
-    rc = hypervolume_device_ranked(ctx, pop_y, pop, M, h_ref, rank, hv_out);
-    if (rc != DMO_OK) return rc;
+    if (dmo_is_device_ptr(hv_ref)) {
+      ctx->waits++;  // a copy into pageable host memory returns once it has landed: behind the truncation
+      DMO_CUDA(cudaMemcpyAsync(h_ref, hv_ref, M * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    } else {
+      memcpy(h_ref, hv_ref, M * sizeof(double));
+    }
+    DMO_TRY(hypervolume_device_ranked(ctx, pop_y, pop, M, h_ref, rank, hv_out));
   }
   return DMO_OK;
 }

@@ -176,6 +176,63 @@ __global__ void children_kernel(int64_t T, int d, int64_t popsize, const int32_t
 
 }  // namespace
 
+// dmo_tournament on device arrays, enqueued only (crowd and u_out may be null)
+int tournament_device(dmo_ctx* ctx, const int32_t* d_rank, const double* d_crowd, int64_t pop, int64_t poolsize, uint64_t seed,
+                      uint64_t stream_id, int64_t* d_pool, double* d_u) {
+  // candidates in np.lexsort((-crowd, rank)) order (MOEA.py:388-389; AGEMOEA.py:140-142)
+  DevBuf<uint32_t> order, i0, i1;
+  DevBuf<uint64_t> k0, k1;
+  DMO_TRY(order.alloc(ctx, pop));
+  DMO_TRY(i0.alloc(ctx, pop));
+  DMO_TRY(i1.alloc(ctx, pop));
+  DMO_TRY(k0.alloc(ctx, pop));
+  DMO_TRY(k1.alloc(ctx, pop));
+  const double* keys[1] = {d_crowd};
+  DMO_TRY(lexsort_device(ctx, d_rank, keys, d_crowd ? 1 : 0, pop, order.p, false));  // caller ranks: any int32
+  DMO_LAUNCH(gumbel_keys_kernel, (unsigned)ceil_div(pop, 256), 256, 0, pop, seed, stream_id, log(0.5), k0.p, i0.p, d_u);
+  DMO_TRY(prim_sort_pairs_u64(ctx, k0.p, k1.p, i0.p, i1.p, pop, 0, 64));
+  DMO_LAUNCH(pool_gather_kernel, (unsigned)ceil_div(poolsize, 256), 256, 0, order.p, i1.p, poolsize, d_pool);
+  DMO_CHECK_LAUNCH();
+  return DMO_OK;
+}
+
+// dmo_nsga2_generate on device arrays (d_draws may be null).  The one host wait is the read-back of the offspring count,
+// *n_children: the caller sizes what follows by it.
+int nsga2_generate_device(dmo_ctx* ctx, const double* d_pop_x, int d, const int64_t* d_pool, int64_t poolsize, int64_t popsize,
+                          double crossover_prob, double mutation_prob, double mutation_rate, const double* d_dic,
+                          const double* d_dim, const double* d_xlb, const double* d_xub, uint64_t seed, uint64_t stream_id,
+                          double* d_x_gen, int32_t* d_kind, int64_t* n_children, double* d_draws) {
+  DMO_REQUIRE(poolsize >= 2 || crossover_prob <= 0.0, "nsga2_generate: crossover needs a pool of at least 2");
+  DMO_REQUIRE(crossover_prob > 0.0 || mutation_prob > 0.0, "nsga2_generate: both probabilities are zero");
+  const int64_t T = dmo_nsga2_plan_length(popsize, crossover_prob, mutation_prob);
+  DMO_REQUIRE(T > 0, "nsga2_generate: crossover_prob / mutation_prob too small for popsize %lld", (long long)popsize);
+  const int64_t cap = popsize + 1;
+  DevBuf<int32_t> count, start, flags, parents;
+  DevBuf<int64_t> nch;
+  DMO_TRY(count.alloc(ctx, T + 1));
+  DMO_TRY(start.alloc(ctx, T + 1));
+  DMO_TRY(flags.alloc(ctx, T));
+  DMO_TRY(parents.alloc(ctx, 3 * T));
+  DMO_TRY(nch.alloc(ctx, 1));
+  // -1 = loop never finished; popsize 1: `while count < popsize - 1` never runs, no children
+  DMO_CUDA(cudaMemsetAsync(nch.p, popsize > 1 ? 0xFF : 0, sizeof(int64_t), ctx->stream));
+  DMO_CUDA(cudaMemsetAsync(d_kind, 0xFF, cap * sizeof(int32_t), ctx->stream));
+  DMO_LAUNCH(plan_kernel, (unsigned)ceil_div(T + 1, 256), 256, 0, T, poolsize, crossover_prob, mutation_prob, seed,
+             stream_id, count.p, flags.p, parents.p, d_draws);
+  DMO_TRY(prim_exclusive_sum_i32(ctx, count.p, start.p, T + 1));
+  DMO_LAUNCH(children_kernel, (unsigned)ceil_div(T * d, 256), 256, 0, T, d, popsize, start.p, flags.p, parents.p, d_pop_x,
+             d_pool, d_dic, d_dim, d_xlb, d_xub, mutation_rate, seed, stream_id, d_x_gen, d_kind, nch.p, d_draws);
+  DMO_CHECK_LAUNCH();
+  int64_t h_n = -1;
+  DMO_CUDA(cudaMemcpyAsync(&h_n, nch.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
+  if (h_n < 0 || h_n > cap)
+    return dmo_fail(ctx, DMO_ERR_INTERNAL, "nsga2_generate: planned %lld iterations but produced %lld children",
+                    (long long)T, (long long)h_n);
+  *n_children = h_n;
+  return DMO_OK;
+}
+
 extern "C" {
 
 int dmo_mutation_u(dmo_ctx* ctx, const double* parents, const double* u, int64_t n, int d, const double* di_mutation,
@@ -196,7 +253,7 @@ int dmo_mutation_u(dmo_ctx* ctx, const double* parents, const double* u, int64_t
              mutation_rate, oc.d);
   DMO_CHECK_LAUNCH();
   DMO_TRY(oc.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -222,7 +279,7 @@ int dmo_sbx_u(dmo_ctx* ctx, const double* parent1, const double* parent2, const 
   DMO_CHECK_LAUNCH();
   DMO_TRY(o1.finish(ctx));
   DMO_TRY(o2.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -239,24 +296,10 @@ int dmo_tournament(dmo_ctx* ctx, const int32_t* rank, const double* crowd, int64
   DMO_TRY(icr.init(ctx, crowd, (size_t)pop));
   DMO_TRY(op.init(ctx, pool_idx, (size_t)poolsize));
   DMO_TRY(ou.init(ctx, u_out, (size_t)pop));
-  // candidates in np.lexsort((-crowd, rank)) order (MOEA.py:388-389; AGEMOEA.py:140-142)
-  DevBuf<uint32_t> order, i0, i1;
-  DevBuf<uint64_t> k0, k1;
-  DMO_TRY(order.alloc(ctx, pop));
-  DMO_TRY(i0.alloc(ctx, pop));
-  DMO_TRY(i1.alloc(ctx, pop));
-  DMO_TRY(k0.alloc(ctx, pop));
-  DMO_TRY(k1.alloc(ctx, pop));
-  const double* keys[1] = {icr.d};
-  DMO_TRY(lexsort_device(ctx, ir.d, keys, crowd ? 1 : 0, pop, order.p, false));  // caller ranks: any int32
-  DMO_LAUNCH(gumbel_keys_kernel, (unsigned)ceil_div(pop, 256), 256, 0, pop, seed, stream_id, log(0.5), k0.p, i0.p,
-             ou.d);
-  DMO_TRY(prim_sort_pairs_u64(ctx, k0.p, k1.p, i0.p, i1.p, pop, 0, 64));
-  DMO_LAUNCH(pool_gather_kernel, (unsigned)ceil_div(poolsize, 256), 256, 0, order.p, i1.p, poolsize, op.d);
-  DMO_CHECK_LAUNCH();
+  DMO_TRY(tournament_device(ctx, ir.d, icr.d, pop, poolsize, seed, stream_id, op.d, ou.d));
   DMO_TRY(op.finish(ctx));
   DMO_TRY(ou.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 
@@ -288,10 +331,7 @@ int dmo_nsga2_generate(dmo_ctx* ctx, const double* pop_x, int64_t npop, int d, c
   DMO_REQUIRE(npop > 0 && d >= 1 && poolsize >= 1 && popsize >= 1 && pop_x && pool_idx && di_crossover && di_mutation &&
                   xlb && xub && x_gen && child_kind && n_children,
               "nsga2_generate: bad arguments");
-  DMO_REQUIRE(poolsize >= 2 || crossover_prob <= 0.0, "nsga2_generate: crossover needs a pool of at least 2");
-  DMO_REQUIRE(crossover_prob > 0.0 || mutation_prob > 0.0, "nsga2_generate: both probabilities are zero");
   const int64_t T = dmo_nsga2_plan_length(popsize, crossover_prob, mutation_prob);
-  DMO_REQUIRE(T > 0, "nsga2_generate: crossover_prob / mutation_prob too small for popsize %lld", (long long)popsize);
   const int64_t cap = popsize + 1;
   In<double> ipx, idc, idm, ilb, iub;
   In<int64_t> ipool;
@@ -305,34 +345,13 @@ int dmo_nsga2_generate(dmo_ctx* ctx, const double* pop_x, int64_t npop, int d, c
   DMO_TRY(iub.init(ctx, xub, d));
   DMO_TRY(ox.init(ctx, x_gen, (size_t)cap * d));
   DMO_TRY(okind.init(ctx, child_kind, (size_t)cap));
-  DMO_TRY(odraws.init(ctx, draws, (size_t)T * (5 + 2 * d)));
-  DevBuf<int32_t> count, start, flags, parents;
-  DevBuf<int64_t> nch;
-  DMO_TRY(count.alloc(ctx, T + 1));
-  DMO_TRY(start.alloc(ctx, T + 1));
-  DMO_TRY(flags.alloc(ctx, T));
-  DMO_TRY(parents.alloc(ctx, 3 * T));
-  DMO_TRY(nch.alloc(ctx, 1));
-  // -1 = loop never finished; popsize 1: `while count < popsize - 1` never runs, no children
-  DMO_CUDA(cudaMemsetAsync(nch.p, popsize > 1 ? 0xFF : 0, sizeof(int64_t), ctx->stream));
-  DMO_CUDA(cudaMemsetAsync(okind.d, 0xFF, cap * sizeof(int32_t), ctx->stream));
-  DMO_LAUNCH(plan_kernel, (unsigned)ceil_div(T + 1, 256), 256, 0, T, poolsize, crossover_prob, mutation_prob, seed,
-             stream_id, count.p, flags.p, parents.p, odraws.d);
-  DMO_TRY(prim_exclusive_sum_i32(ctx, count.p, start.p, T + 1));
-  DMO_LAUNCH(children_kernel, (unsigned)ceil_div(T * d, 256), 256, 0, T, d, popsize, start.p, flags.p, parents.p, ipx.d,
-             ipool.d, idc.d, idm.d, ilb.d, iub.d, mutation_rate, seed, stream_id, ox.d, okind.d, nch.p, odraws.d);
-  DMO_CHECK_LAUNCH();
-  int64_t h_n = -1;
-  DMO_CUDA(cudaMemcpyAsync(&h_n, nch.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
-  if (h_n < 0 || h_n > cap)
-    return dmo_fail(ctx, DMO_ERR_INTERNAL, "nsga2_generate: planned %lld iterations but produced %lld children",
-                    (long long)T, (long long)h_n);
-  *n_children = h_n;
-  DMO_TRY(ox.finish(ctx, (size_t)h_n * d));
-  DMO_TRY(okind.finish(ctx, (size_t)h_n));
+  DMO_TRY(odraws.init(ctx, T > 0 ? draws : nullptr, (size_t)T * (5 + 2 * d)));
+  DMO_TRY(nsga2_generate_device(ctx, ipx.d, d, ipool.d, poolsize, popsize, crossover_prob, mutation_prob, mutation_rate, idc.d,
+                                idm.d, ilb.d, iub.d, seed, stream_id, ox.d, okind.d, n_children, odraws.d));
+  DMO_TRY(ox.finish(ctx, (size_t)*n_children * d));
+  DMO_TRY(okind.finish(ctx, (size_t)*n_children));
   DMO_TRY(odraws.finish(ctx));
-  DMO_CUDA(cudaStreamSynchronize(ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
 

@@ -71,6 +71,7 @@ const char* dmo_last_error(dmo_ctx* ctx);
 int dmo_synchronize(dmo_ctx* ctx);
 void* dmo_stream(dmo_ctx* ctx);             /* the context's cudaStream_t */
 int64_t dmo_launch_count(dmo_ctx* ctx);     /* kernels launched by this context so far */
+int64_t dmo_wait_count(dmo_ctx* ctx);       /* times this context's host side has blocked on its stream so far */
 int dmo_sm_count(dmo_ctx* ctx);
 /* CUDA-event stopwatch on the context's stream (bench.py times kernels with it) */
 int dmo_timer_begin(dmo_ctx* ctx);

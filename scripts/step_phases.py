@@ -1,0 +1,118 @@
+"""Where the resident NSGA-II generation step (dmo_nsga2_step, bench.py's `value`) spends its time, phase by phase.
+
+Builds bench.py's workload (bench.workload, same seed, same GP model, pop 65 536, d 30, M 3, N_train 4096 by default),
+runs the fused step for --warmup generations, then times --steps generations with the library's per-scope CUDA-event
+timers on and prints, per generation:
+  * device-timer ms of each phase (step_tournament, step_generate, step_gp, step_truncate, step_hv) and of the kernels
+    inside them that have scopes of their own (gp_kstar, gp_var, rank_peel, ...);
+  * the whole step, by device events around the timed window and by the host clock;
+  * host waits (stream synchronises and blocking copies, dmo_wait_count) and kernel launches (dmo_launch_count);
+  * the card's name, its power limit and the median SM clock sampled during the timed window.
+Usage: python scripts/step_phases.py [--steps 100] [--warmup 20] [--json OUT.json]
+"""
+
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+
+PHASES = ("step_tournament", "step_generate", "step_gp", "step_truncate", "step_hv")
+
+
+def card(device):
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits", "-i", str(device)],
+                           capture_output=True, text=True, timeout=30).stdout.strip().split(",")
+        return q[0].strip(), float(q[1])
+    except Exception:
+        return None, None
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=100)
+    ap.add_argument("--warmup", type=int, default=20)
+    ap.add_argument("--pop", type=int, default=65536)
+    ap.add_argument("--dim", type=int, default=30)
+    ap.add_argument("--obj", type=int, default=3)
+    ap.add_argument("--ntrain", type=int, default=4096)
+    ap.add_argument("--seed", type=int, default=1234)
+    ap.add_argument("--json", default=None, help="also write the result to this file")
+    args = ap.parse_args()
+
+    import bench
+    import dmosopt_b200 as b2
+    from dmosopt_b200 import _lib as L
+
+    L.context(0)
+    clocks = bench.ClockSampler(0)
+    clocks.start()
+    pop, d, M, N = args.pop, args.dim, args.obj, args.ntrain
+    w = bench.workload(pop, d, M, N)
+    sm = b2.GPR_Matern(w["Xtr"], w["Ytr"], d, M, w["xlb"], w["xub"], optimizer=None, precision="auto")
+    y0 = sm.evaluate(w["X0"]).astype(np.float32)
+    ref = y0.max(axis=0).astype(np.float64) + 0.1 * (y0.max(axis=0) - y0.min(axis=0))
+    opt = b2.NSGA2(popsize=pop, nInput=d, nOutput=M, model=b2.Model(objective=sm), distance_metric=None)
+    opt.initialize_strategy(w["X0"], y0, np.column_stack((w["xlb"], w["xub"])), np.random.default_rng(args.seed))
+    rs = bench.ResidentStep(L, sm._gp, pop, d, M, w["xlb"], w["xub"], opt.state.population_parm,
+                            opt.state.population_obj.astype(np.float64), opt.state.rank.copy(), ref, args.seed)
+    rs.precision, rs.metric = L.GP_AUTO, L.METRIC_NONE
+    for _ in range(args.warmup):
+        rs.step()
+    L.synchronize()
+
+    clocks.mark_begin()
+    L.profile_enable(True)
+    w0, l0 = L.wait_count(), L.launch_count()
+    t0 = time.perf_counter()
+    L.timer_begin()
+    for _ in range(args.steps):
+        rs.step()
+    ms_dev = L.timer_end()
+    t_host = time.perf_counter() - t0
+    waits, launches = L.wait_count() - w0 - 1, L.launch_count() - l0  # - 1: timer_end's own wait
+    prof = L.profile_report()
+    L.profile_enable(False)
+    clocks.mark_end()
+    clk = clocks.stop()
+    name, plimit = card(0)
+
+    K = args.steps
+    out = {
+        "card": name, "power_limit_w": plimit, "sm_mhz_median": clk.get("sm_mhz"), "clock_reasons": clk.get("reasons"),
+        "steps": K, "pop": pop, "dim": d, "obj": M, "ntrain": N,
+        "step_ms_device": ms_dev / K, "step_ms_host": t_host * 1e3 / K,
+        "waits_per_step": waits / K, "launches_per_step": launches / K,
+        "phases_ms": {k: prof[k][0] / K for k in PHASES if k in prof},
+        "scopes_ms": {k: v[0] / K for k, v in sorted(prof.items()) if k not in PHASES},
+        "scope_counts_per_step": {k: v[1] / K for k, v in sorted(prof.items())},
+    }
+    ph = out["phases_ms"]
+    out["outside_gp_ms"] = out["step_ms_device"] - ph.get("step_gp", 0.0)
+    print(f"{name}, power limit {plimit} W, median SM clock {clk.get('sm_mhz')} MHz, {K} generations")
+    print(f"{'phase':<18}{'ms / generation':>16}")
+    for k in PHASES:
+        if k in ph:
+            print(f"{k:<18}{ph[k]:>16.3f}")
+    for k, v in out["scopes_ms"].items():
+        print(f"  {k:<16}{v:>16.3f}")
+    print(f"{'step (events)':<18}{out['step_ms_device']:>16.3f}")
+    print(f"{'step (host)':<18}{out['step_ms_host']:>16.3f}")
+    print(f"{'outside step_gp':<18}{out['outside_gp_ms']:>16.3f}")
+    print(f"host waits / generation {out['waits_per_step']:.2f}, launches / generation {out['launches_per_step']:.1f}")
+    print(json.dumps(out), flush=True)
+    if args.json:
+        with open(args.json, "w") as f:
+            json.dump(out, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
