@@ -35,6 +35,12 @@ struct dmo_ctx {
   static constexpr int kSide = 4;
   cudaStream_t side[kSide] = {};
   cudaEvent_t side_ev[kSide + 1] = {};  // [0]: fork point on the main stream, [1 + s]: end of side stream s
+  // the fused step's concurrent lane (step.cu): `lane` runs the truncation beside the GP variance contraction, which runs on
+  // `gp_hi`, a stream of the device's greatest priority, so that its CTAs take their SMs before the lane's kernels fill
+  // the card.  lane_ev: [0] every mean written, [1] / [2] fork to / join from gp_hi, [3] end of the lane.  Created on
+  // first use (dmo_lane_streams), released by dmo_destroy
+  cudaStream_t lane = nullptr, gp_hi = nullptr;
+  cudaEvent_t lane_ev[4] = {};
   // optional per-kernel CUDA-event timers (dmo_profile_enable); bench.py reads them for the roofline
   bool profiling = false;
   struct Timer {
@@ -111,6 +117,7 @@ struct SideStreams {
 };
 
 int dmo_lag_slots(dmo_ctx* ctx);
+int dmo_lane_streams(dmo_ctx* ctx);
 
 // every host wait of the library on its stream goes through this, so that dmo_wait_count() counts them
 static inline cudaError_t dmo_wait(dmo_ctx* ctx) {

@@ -31,6 +31,17 @@ int dmo_lag_slots(dmo_ctx* ctx) {
   return DMO_OK;
 }
 
+int dmo_lane_streams(dmo_ctx* ctx) {
+  if (ctx->gp_hi) return DMO_OK;
+  int least = 0, greatest = 0;
+  DMO_CUDA(cudaDeviceGetStreamPriorityRange(&least, &greatest));
+  for (cudaEvent_t& e : ctx->lane_ev)
+    if (!e) DMO_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  if (!ctx->lane) DMO_CUDA(cudaStreamCreateWithFlags(&ctx->lane, cudaStreamNonBlocking));
+  DMO_CUDA(cudaStreamCreateWithPriority(&ctx->gp_hi, cudaStreamNonBlocking, greatest));
+  return DMO_OK;
+}
+
 SideStreams::SideStreams(dmo_ctx* c, int nside) : ctx(c), main(c->stream) {
   if (nside > dmo_ctx::kSide) nside = dmo_ctx::kSide;
   if (!ctx->side[0]) {
@@ -107,6 +118,10 @@ int dmo_destroy(dmo_ctx* ctx) {
     if (e) cudaEventDestroy(e);
   for (cudaStream_t st : ctx->side)
     if (st) cudaStreamDestroy(st);
+  for (cudaEvent_t e : ctx->lane_ev)
+    if (e) cudaEventDestroy(e);
+  if (ctx->lane) cudaStreamDestroy(ctx->lane);
+  if (ctx->gp_hi) cudaStreamDestroy(ctx->gp_hi);
   cudaEventDestroy(ctx->ev0);
   cudaEventDestroy(ctx->ev1);
   cudaStreamDestroy(ctx->stream);

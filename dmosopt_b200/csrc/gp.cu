@@ -613,7 +613,7 @@ int gp_predict_auto(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, doub
   GpPending& q = pending ? *pending : own;
   DMO_TRY(q.flag.alloc(ctx, (size_t)P + 1));
   DMO_TRY(q.pos.alloc(ctx, (size_t)P + 2));  // pos[P]: rows to refine, pos[P + 1]: the contraction's watchdog, read back together
-  DMO_TRY(gp_predict_tensor(ctx, gp, dXn, P, d_mean, d_var, q.pos.p + P + 1));
+  DMO_TRY(gp_predict_tensor(ctx, gp, dXn, P, d_mean, d_var, q.pos.p + P + 1, q.ov.mean_ready ? &q.ov : nullptr));
   DMO_CUDA(cudaMemsetAsync(q.flag.p + P, 0, sizeof(int32_t), ctx->stream));
   DMO_LAUNCH(flag_small_var_kernel, (unsigned)ceil_div(P, 256), 256, 0, d_var, P, gp->M, gp->constant.p, gp->noise.p, gp->ystd.p,
              gp->refine_theta, q.flag.p);

@@ -100,22 +100,34 @@ int gp_prepare_tensor(dmo_ctx* ctx, GpVarOps& ops);
 // wgmma variance contraction (gp_var_wgmma_kernel, paired schedule) over K_* hi / lo rows of ops.Npad fp16 values:
 // k_alloc rows are allocated, plane g < ops.G reads rows g * k_rows + [0, Pcpad) (k_rows = 0: one K_* plane for every
 // g); Pcpad is a multiple of GP_TC_TILE.  vnorm[q][g][p], q < gp_tensor_var_planes(ops.Npad), holds the partial sums.
-// abort_flag (device int, zeroed by the caller) is set when the pipeline watchdog trips.
+// abort_flag (device int, zeroed by the caller) is set when the pipeline watchdog trips.  The grid is the smallest one
+// with as many work items per CTA as sm_count CTAs would take, less `reserve` further CTAs; every item writes its own
+// vnorm slot, so the grid does not change a bit.
 constexpr int GP_TC_TILE = 128;
 int gp_tensor_var_planes(int64_t Npad);
 int gp_var_contract_tensor(dmo_ctx* ctx, const GpVarOps& ops, const uint16_t* Kh, const uint16_t* Kl, int64_t k_alloc,
-                           int64_t k_rows, int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag);
+                           int64_t k_rows, int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag, int reserve = 0);
+// A caller that runs its own work beside the variance contraction (the fused step's lane, step.cu) passes this to the
+// tensor route: mean_ready is recorded on the stream once the last chunk's mean is written, the contraction runs on the
+// context's high-priority stream (joined back before var_finish_tc_kernel), and `reserve` SMs are kept out of its grid.
+// The caller creates those streams first (dmo_lane_streams).
+struct GpOverlap {
+  cudaEvent_t mean_ready = nullptr;
+  int reserve = 0;
+};
 // abort_flag null: the call reads the contraction's watchdog back and fails when it tripped.  Otherwise the call zeroes
 // *abort_flag (device) and the watchdog lands there; the caller reads it back and fails the same way (gp_predict_auto folds
 // it into its own read-back).  The mean-only route writes no flag.
 int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var,
-                      int* abort_flag = nullptr);
+                      int* abort_flag = nullptr, const GpOverlap* ov = nullptr);
 extern const char* const GP_WATCHDOG_MSG;
 // An AUTO predict whose one read-back (watchdog, rows to refine) is left pending, so the caller can enqueue work behind it
 // while the GP runs; gp_predict_finish waits for it, fails on a tripped watchdog and refines the rows the check flags
 // (after that work: *refined tells the caller to redo it).  Only the AUTO variance route of models without a linear mean
-// defers; other calls finish inside gp_predict_device and leave `active` false.
+// defers; other calls finish inside gp_predict_device and leave `active` false.  A caller that sets ov.mean_ready before
+// the call gets the overlapped contraction of GpOverlap; once `active`, the event has been recorded.
 struct GpPending {
+  GpOverlap ov;
   bool active = false;
   int64_t P = 0;
   const double* dXn = nullptr;

@@ -1022,7 +1022,7 @@ static_assert(TMV == GP_TC_TILE, "gp.cuh exports the wgmma candidate tile");
 int gp_tensor_var_planes(int64_t Npad) { return (int)((Npad / TN + 1) / 2); }
 
 int gp_var_contract_tensor(dmo_ctx* ctx, const GpVarOps& ops, const uint16_t* Kh, const uint16_t* Kl, int64_t k_alloc,
-                           int64_t k_rows, int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag) {
+                           int64_t k_rows, int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag, int reserve) {
   const int64_t Npad = ops.Npad;
   DMO_REQUIRE(Npad % TN == 0 && Pcpad % TMV == 0, "gp_var_contract_tensor: internal padding error");
   CUtensorMap map_kh, map_kl, map_lh, map_ll;
@@ -1042,15 +1042,23 @@ int gp_var_contract_tensor(dmo_ctx* ctx, const GpVarOps& ops, const uint16_t* Kh
   prm.vnorm = vnorm;
   prm.vn_ld = vn_ld;
   prm.abort_flag = abort_flag;
+  // static round-robin: the makespan is ceil(n_work / grid) items, so the smallest grid with that many items per CTA
+  // finishes with it and leaves the other SMs free (at the bench shape 4096 items take 128 CTAs, not 132)
   const int n_work = prm.M * prm.n_pb * prm.n_q;
-  const int grid = n_work < ctx->sm_count ? n_work : ctx->sm_count;
+  int per_cta = (int)ceil_div(n_work, ctx->sm_count);
+  int grid = (int)ceil_div(n_work, per_cta);
+  if (reserve > 0) {  // `reserve` SMs more kept free, at a longer makespan; at least one CTA
+    per_cta = (int)ceil_div(n_work, reserve < grid ? grid - reserve : 1);
+    grid = (int)ceil_div(n_work, per_cta);
+  }
   DMO_LAUNCH(gp_var_wgmma_kernel, grid, NTHREADS, GEMM_SMEM, map_kh, map_kl, map_lh, map_ll, prm);
   return DMO_OK;
 }
 
 const char* const GP_WATCHDOG_MSG = "gp_predict(tensor): pipeline watchdog tripped (mbarrier wait timed out)";
 
-int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var, int* abort_flag) {
+int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var, int* abort_flag,
+                      const GpOverlap* ov) {
   const int64_t N = gp->N, Npad = gp->ops.Npad;
   const int M = gp->M, G = gp->ops.G, d = gp->d;
   DMO_REQUIRE(M <= 16, "gp_predict(tensor): at most 16 objectives per model (got %d)", M);
@@ -1163,10 +1171,24 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
                    gp->cov.p, gp->ops.Kexp.p, gp->alpha.p, gp->ymean.p, gp->ystd.p, p_base, d_mean);
       }
     }
+    if (ov && p_base + Pc_alloc >= P) DMO_CUDA(cudaEventRecord(ov->mean_ready, ctx->stream));
     if (d_var) {
       {
         ProfileScope ps_(ctx, "gp_var");
-        DMO_TRY(gp_var_contract_tensor(ctx, gp->ops, Kh.p, Kl.p, G * Pc_alloc, Pc_alloc, Pcpad, vnorm.p, Pc_alloc, abort_flag));
+        cudaStream_t main = ctx->stream;
+        if (ov) {
+          DMO_CUDA(cudaEventRecord(ctx->lane_ev[1], main));
+          DMO_CUDA(cudaStreamWaitEvent(ctx->gp_hi, ctx->lane_ev[1], 0));
+          ctx->stream = ctx->gp_hi;
+        }
+        const int rc = gp_var_contract_tensor(ctx, gp->ops, Kh.p, Kl.p, G * Pc_alloc, Pc_alloc, Pcpad, vnorm.p, Pc_alloc, abort_flag,
+                                              ov ? ov->reserve : 0);
+        if (ov) {
+          ctx->stream = main;
+          DMO_CUDA(cudaEventRecord(ctx->lane_ev[2], ctx->gp_hi));
+          DMO_CUDA(cudaStreamWaitEvent(main, ctx->lane_ev[2], 0));
+        }
+        DMO_TRY(rc);
       }
       DMO_LAUNCH(var_finish_tc_kernel, (unsigned)ceil_div(Pc * M, 256), 256, 0, vnorm.p, n_q, Pc, Pc_alloc, M, G,
                  gp->cov.p, gp->constant.p, gp->noise.p, gp->ystd.p, p_base, d_var);

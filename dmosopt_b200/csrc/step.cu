@@ -8,8 +8,10 @@
 // It is a composition of the device bodies of this library's entry points, without their trailing waits.  The host waits
 // only for values it needs: the offspring count (it sizes the GP launch), one read-back after the GP (watchdog and rows to
 // refine, read once the truncation is enqueued behind it), the rank's (the peel probe and one count per peeled front, mostly read while the next front is peeled; or the
-// chain's watchdog) and the hypervolume's (its route and its value).  bench.py's `value` leg is this call;
-// scripts/step_phases.py times its phases (the step_* profile scopes) and counts the waits.
+// chain's watchdog) and the hypervolume's (its route and its value).  The truncation runs beside the GP's variance
+// contraction, on a stream of its own (below).  bench.py's `value` leg is this call; scripts/step_phases.py times its
+// phases (the step_* profile scopes) and counts the waits.
+#include <stdlib.h>
 #include <string.h>
 
 #include "common.cuh"
@@ -64,18 +66,30 @@ int dmo_nsga2_step(dmo_ctx* ctx, dmo_gp* gp, double* pop_x, double* pop_y, int32
     DMO_CUDA(cudaMemcpyAsync(Xs.p + (size_t)P * d, pop_x, (size_t)pop * d * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
     DMO_CUDA(cudaMemcpyAsync(Ys.p + (size_t)P * M, pop_y, (size_t)pop * M * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
   }
-  // The GP's read-back is left pending and the truncation is enqueued behind it, so the host issues the truncation's first
-  // launches while the GP runs; the truncation's own first wait comes after the GP anyway.  If the GP then fails, the
-  // population is put back (the parents are still in Xs / Ys); if AUTO refines rows, the truncation runs again on them.
+  // The GP's read-back is left pending and the truncation is enqueued before the host waits for it.  The truncation needs
+  // the posterior mean only, which the tensor route writes before its variance contraction: by default (DMO_STEP_OVERLAP
+  // unset or not 0) the truncation runs on the context's lane stream from that point on, beside the contraction, which
+  // runs on a higher-priority stream on the SMs its grid leaves free (DMO_GP_VAR_RESERVE=r keeps r more from it).  With
+  // DMO_STEP_OVERLAP=0 it queues behind the whole GP on the main stream.  Either way its host waits (peel probe, peel
+  // counts) wait for its own stream only.  If the GP then fails, the population is put back (the parents are still in
+  // Xs / Ys); if AUTO refines rows, the truncation runs again on them.  Every buffer the two streams share is allocated
+  // on the main stream before the fork and released after the join.
+  const char* ov_env = getenv("DMO_STEP_OVERLAP");
+  const bool overlap = !(ov_env && atoi(ov_env) == 0);
+  int var_reserve = 0;
+  if (const char* e = getenv("DMO_GP_VAR_RESERVE")) var_reserve = atoi(e);
+  DMO_REQUIRE(var_reserve >= 0, "nsga2_step: DMO_GP_VAR_RESERVE must not be negative");
   GpPending gpp;
-  DevBuf<int32_t> rank_in;
+  DevBuf<int32_t> rank_in;  // the ranks before the truncation, for the failure path
   if (P > 0) {
+    DMO_TRY(rank_in.alloc(ctx, pop));
+    if (overlap) {
+      DMO_TRY(dmo_lane_streams(ctx));
+      gpp.ov.mean_ready = ctx->lane_ev[0];
+      gpp.ov.reserve = var_reserve;
+    }
     ProfileScope ps(ctx, "step_gp");
     DMO_TRY(gp_predict_device(ctx, gp, Xs.p, P, Ys.p, with_variance ? var.p : nullptr, precision, &gpp));
-  }
-  if (gpp.active) {
-    DMO_TRY(rank_in.alloc(ctx, pop));
-    DMO_CUDA(cudaMemcpyAsync(rank_in.p, rank, (size_t)pop * sizeof(int32_t), cudaMemcpyDeviceToDevice, ctx->stream));
   }
   auto truncate = [&]() -> int {
     ProfileScope ps(ctx, "step_truncate");
@@ -83,7 +97,33 @@ int dmo_nsga2_step(dmo_ctx* ctx, dmo_gp* gp, double* pop_x, double* pop_y, int32
     if (round_to_f32) DMO_TRY(prim_round_f32(ctx, pop_y, pop * M));
     return DMO_OK;
   };
-  DMO_TRY(truncate());
+  auto first_truncate = [&]() -> int {
+    if (gpp.active) DMO_CUDA(cudaMemcpyAsync(rank_in.p, rank, (size_t)pop * sizeof(int32_t), cudaMemcpyDeviceToDevice, ctx->stream));
+    return truncate();
+  };
+  if (gpp.active && gpp.ov.mean_ready) {
+    // The lane reads Xs, Ys (the mean rows and the parents) and writes pop_x, pop_y, rank, rank_in and its own scratch; the
+    // GP's work after the fork point writes the variance and its own scratch only.  The lane may run on a few SMs while
+    // the contraction holds the rest, so nothing in it may need all of its CTAs resident at once.  Every kernel
+    // remove_worst_device reaches (metric none, crowding or euclidean) was checked for that: the dense-id, lexicographic,
+    // cell and key radix sorts are CUB's (onesweep passes take their tile from an atomic counter and look back only at
+    // tiles taken before; small sorts run as one tile, or as separate upsweep / scan / downsweep kernels); CUB's scans
+    // look back only at lower block indices, which are dispatched first; the peel probe
+    // is a grid-stride loop with atomicOr; the chain kernel (rank.cu) takes its blocks from an atomic ticket and waits
+    // only for blocks taken before; everything else (keys, gathers, cell grid, prefix minima, peel marks, column min / max,
+    // crowding, euclidean, round_f32) is one pass per element or per block, with atomics at most, and no grid-wide barrier.
+    cudaStream_t main = ctx->stream;
+    DMO_CUDA(cudaStreamWaitEvent(ctx->lane, gpp.ov.mean_ready, 0));
+    ctx->stream = ctx->lane;
+    const int rc = first_truncate();
+    ctx->stream = main;
+    // joined before gp_predict_finish: its refinement, the failure path and the second truncation come after the lane
+    DMO_CUDA(cudaEventRecord(ctx->lane_ev[3], ctx->lane));
+    DMO_CUDA(cudaStreamWaitEvent(main, ctx->lane_ev[3], 0));
+    DMO_TRY(rc);
+  } else {
+    DMO_TRY(first_truncate());
+  }
   bool refined = false;
   const int rc = gp_predict_finish(ctx, gp, gpp, &refined);
   if (rc != DMO_OK) {
