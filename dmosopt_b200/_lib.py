@@ -108,6 +108,8 @@ _SIGNATURES = {
     "dmo_gp_lml_grad": (_c_int, [_vp, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dmo_nsga2_step": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_i64, _c_int, _c_int, _c_dbl, _c_dbl, _c_dbl, _vp, _vp, _vp, _vp, _c_u64, _c_u64,
                                 _c_int, _c_int, _c_int, _c_int, _vp, _vp, _vp]),
+    "dmo_nsga2_step_record": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_i64, _c_int, _c_int, _c_dbl, _c_dbl, _c_dbl, _vp, _vp, _vp, _vp,
+                                       _c_u64, _c_u64, _c_int, _c_int, _c_int, _vp, _vp, _vp, _vp]),
     "dmo_hypervolume": (_c_int, [_vp, _vp, _c_i64, _c_int, _vp, ctypes.POINTER(_c_dbl)]),
     "dmo_hypervolume_ranked": (_c_int, [_vp, _vp, _c_i64, _c_int, _vp, _vp, ctypes.POINTER(_c_dbl)]),
     "dmo_nondominated_flags": (_c_int, [_vp, _vp, _c_i64, _c_int, _vp]),
@@ -491,6 +493,16 @@ def mirror_ptr(a, require_readonly=True):
     return dev.ptr + off if dev.ptr and off + a.nbytes <= nbytes else None
 
 
+def mirror_array(a):
+    """The DeviceArray mirroring all of the host array ``a`` (same start, same size), else None."""
+    if not isinstance(a, np.ndarray):
+        return None
+    ent = _mirrors.get(a.ctypes.data)
+    if ent is None or ent[0] != a.nbytes or not ent[1].ptr:
+        return None
+    return ent[1]
+
+
 def _in(a):
     """Pointer for an input array: the device mirror when the library holds one, else the host address."""
     if a is None:
@@ -735,6 +747,34 @@ def nsga2_generate(pop_x, pool_idx, popsize, crossover_prob, mutation_prob, muta
         "u_genes": draws[5 * T :].reshape(T, 2, d),
     }
     return x_gen[:P], kind[:P], dd
+
+
+def nsga2_step_record(gp, pop_x, pop_y, rank, crossover_prob, mutation_prob, mutation_rate, di_crossover, di_mutation, xlb, xub,
+                      seed, stream_id, precision, metric, round_to_f32, x_gen, y_gen, counts, key=None):
+    """One resident NSGA-II generation, recorded (dmo_nsga2_step_record).  Returns the offspring count P.
+
+    ``gp`` a GPHandle; ``pop_x`` (pop, d) float64, ``pop_y`` (pop, M) float64 and ``rank`` (pop,) int32 are device
+    buffers (DeviceArray, a device address or a CUDA tensor), updated in place.  ``x_gen`` (pop+1, d), ``y_gen`` (pop+1, M)
+    float64 and ``counts`` (4,) int64 receive the offspring, their posterior mean and the operator counts; into device or
+    page-locked memory they are complete only after ``synchronize()``.  ``key`` (optional FeasModel): its rank of
+    [children; parents] is the truncation's last key."""
+    pop, d = int(pop_x.shape[0]), int(pop_x.shape[1])
+    M = int(pop_y.shape[1])
+    for name, a, shape, dt in (("x_gen", x_gen, (pop + 1, d), np.float64), ("y_gen", y_gen, (pop + 1, M), np.float64), ("counts", counts, (4,), np.int64)):
+        if isinstance(a, np.ndarray) and (a.shape != shape or a.dtype != dt or not a.flags.c_contiguous or not a.flags.writeable):
+            raise ValueError(f"nsga2_step_record: {name} must be a writable C-contiguous {np.dtype(dt).name} array of shape {shape}")
+    dic, dim = _per_dim(di_crossover, d), _per_dim(di_mutation, d)
+    lb, ub = _f64(xlb), _f64(xub)
+    nch = np.zeros(1, dtype=np.int64)
+    _check(
+        load_library().dmo_nsga2_step_record(
+            context(), gp._h, None if key is None else key._h, _ptr(pop_x), _ptr(pop_y), _ptr(rank), pop, d, M, float(crossover_prob),
+            float(mutation_prob), float(mutation_rate), _ptr(dic), _ptr(dim), _ptr(lb), _ptr(ub), _seed(seed), int(stream_id), int(precision),
+            int(metric), 1 if round_to_f32 else 0, _ptr(x_gen), _ptr(y_gen), _ptr(counts), _ptr(nch),
+        ),
+        "dmo_nsga2_step_record",
+    )
+    return int(nch[0])
 
 
 # --------------------------------------------------------------------------- N1: exact-GP fit for given hyper-parameters

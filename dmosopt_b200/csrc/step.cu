@@ -11,18 +11,72 @@
 // chain's watchdog) and the hypervolume's (its route and its value).  The truncation runs beside the GP's variance
 // contraction, on a stream of its own (below).  bench.py's `value` leg is this call; scripts/step_phases.py times its
 // phases (the step_* profile scopes) and counts the waits.
+// dmo_nsga2_step_record runs the same body for MOASMO.optimize's resident epoch (dmosopt_b200/MOASMO.py): the mean only,
+// optionally a feasibility rank as the truncation's last key, and the generation's offspring, their mean and operator
+// counts copied out without a host wait.
 #include <stdlib.h>
 #include <string.h>
+
+#include <algorithm>
 
 #include "common.cuh"
 #include "gp.cuh"
 
-extern "C" {
-int dmo_nsga2_step(dmo_ctx* ctx, dmo_gp* gp, double* pop_x, double* pop_y, int32_t* rank, int64_t pop, int d, int M,
-                   double crossover_prob, double mutation_prob, double mutation_rate, const double* di_crossover,
-                   const double* di_mutation, const double* xlb, const double* xub, uint64_t seed, uint64_t stream_id,
-                   int precision, int distance_metric, int with_variance, int round_to_f32, const double* hv_ref, int64_t* n_children,
-                   double* hv_out) {
+// counts[0..3] += children from crossover (kind < 2), mutants (kind == 2), and the same two among the survivors (the
+// rows of perm below P): the values NSGA2.update_strategy derives its success counters from (NSGA2.py:216-222).  Sums of
+// ones stay far below 2^53, so block_sum is exact; one integer atomic per CTA and counter.
+constexpr int kCountWarps = 8;
+__global__ void __launch_bounds__(kCountWarps * 32) step_counts_kernel(const int32_t* __restrict__ kind, int64_t P,
+                                                                        const int64_t* __restrict__ perm, int64_t pop,
+                                                                        unsigned long long* counts) {
+  __shared__ double red[kCountWarps];
+  double c[4] = {0.0, 0.0, 0.0, 0.0};
+  const int64_t n = P > pop ? P : pop;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    if (i < P) {
+      const int32_t k = kind[i];
+      c[0] += k < 2 ? 1.0 : 0.0;
+      c[1] += k == 2 ? 1.0 : 0.0;
+    }
+    if (i < pop) {
+      const int64_t j = perm[i];
+      if (j < P) {
+        const int32_t k = kind[j];
+        c[2] += k < 2 ? 1.0 : 0.0;
+        c[3] += k == 2 ? 1.0 : 0.0;
+      }
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const double s = block_sum<kCountWarps>(c[k], red);
+    if (threadIdx.x == 0 && s > 0.0) atomicAdd(&counts[k], (unsigned long long)s);
+  }
+}
+
+// An output the caller may hand in as device, page-locked or pageable host memory.  The copy is enqueued on the stream;
+// into pageable memory cudaMemcpyAsync returns only once it has landed, which is a host wait and counted as one.
+static int copy_out(dmo_ctx* ctx, void* dst, const void* src, size_t bytes) {
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, dst) != cudaSuccess) {
+    cudaGetLastError();  // clear
+    a.type = cudaMemoryTypeUnregistered;
+  }
+  if (a.type == cudaMemoryTypeUnregistered) ctx->waits++;
+  if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) ctx->d2h_bytes += bytes;
+  DMO_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, ctx->stream));
+  return DMO_OK;
+}
+
+// The body of both entry points.  key (may be null): the feasibility rank of [children; parents] as the truncation's least
+// significant descending key.  x_gen / y_gen / counts (all null, or all set): the offspring, their posterior mean and the
+// operator counts of step_counts_kernel, copied out once the GP is final.
+static int nsga2_step_body(dmo_ctx* ctx, dmo_gp* gp, const dmo_feas* key, double* pop_x, double* pop_y, int32_t* rank,
+                           int64_t pop, int d, int M, double crossover_prob, double mutation_prob, double mutation_rate,
+                           const double* di_crossover, const double* di_mutation, const double* xlb, const double* xub,
+                           uint64_t seed, uint64_t stream_id, int precision, int distance_metric, int with_variance,
+                           int round_to_f32, const double* hv_ref, int64_t* n_children, double* hv_out, double* x_gen,
+                           double* y_gen, int64_t* counts) {
   if (!ctx) return DMO_ERR_ARG;
   DMO_CUDA(cudaSetDevice(ctx->device));
   DMO_REQUIRE(gp && pop_x && pop_y && rank && pop >= 2 && d >= 1 && M >= 1 && di_crossover && di_mutation && xlb && xub,
@@ -66,6 +120,15 @@ int dmo_nsga2_step(dmo_ctx* ctx, dmo_gp* gp, double* pop_x, double* pop_y, int32
     DMO_CUDA(cudaMemcpyAsync(Xs.p + (size_t)P * d, pop_x, (size_t)pop * d * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
     DMO_CUDA(cudaMemcpyAsync(Ys.p + (size_t)P * M, pop_y, (size_t)pop * M * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
   }
+  // the feasibility rank of the merged rows (the key of dmo_remove_worst_pair_keys), on the main stream before the GP forks
+  DevBuf<double> kx;
+  const double* kp[1] = {nullptr};
+  if (key) {
+    ProfileScope ps(ctx, "step_truncate");
+    DMO_TRY(kx.alloc(ctx, (size_t)(P + pop)));
+    DMO_TRY(feas_rank_device(ctx, key, Xs.p, P + pop, kx.p));
+    kp[0] = kx.p;
+  }
   // The GP's read-back is left pending and the truncation is enqueued before the host waits for it.  The truncation needs
   // the posterior mean only, which the tensor route writes before its variance contraction: by default (DMO_STEP_OVERLAP
   // unset or not 0) the truncation runs on the context's lane stream from that point on, beside the contraction, which
@@ -93,7 +156,8 @@ int dmo_nsga2_step(dmo_ctx* ctx, dmo_gp* gp, double* pop_x, double* pop_y, int32
   }
   auto truncate = [&]() -> int {
     ProfileScope ps(ctx, "step_truncate");
-    DMO_TRY(remove_worst_device(ctx, Xs.p, Ys.p, P + pop, d, M, distance_metric, nullptr, 0, pop, pop_x, pop_y, rank, perm.p));
+    DMO_TRY(remove_worst_device(ctx, Xs.p, Ys.p, P + pop, d, M, distance_metric, key ? kp : nullptr, key ? 1 : 0, pop, pop_x, pop_y,
+                                rank, perm.p));
     if (round_to_f32) DMO_TRY(prim_round_f32(ctx, pop_y, pop * M));
     return DMO_OK;
   };
@@ -134,6 +198,19 @@ int dmo_nsga2_step(dmo_ctx* ctx, dmo_gp* gp, double* pop_x, double* pop_y, int32
     return rc;
   }
   if (refined) DMO_TRY(truncate());
+  if (x_gen) {
+    ProfileScope ps(ctx, "step_record");
+    DevBuf<unsigned long long> cnt;
+    DMO_TRY(cnt.alloc(ctx, 4));
+    DMO_CUDA(cudaMemsetAsync(cnt.p, 0, 4 * sizeof(unsigned long long), ctx->stream));
+    const int64_t n = P > pop ? P : pop;
+    const unsigned grid = (unsigned)std::min<int64_t>(ceil_div(n, kCountWarps * 32), 4 * (int64_t)ctx->sm_count);
+    DMO_LAUNCH(step_counts_kernel, grid, kCountWarps * 32, 0, kind.p, P, perm.p, pop, cnt.p);
+    DMO_CHECK_LAUNCH();
+    DMO_TRY(copy_out(ctx, x_gen, Xs.p, (size_t)P * d * sizeof(double)));
+    DMO_TRY(copy_out(ctx, y_gen, Ys.p, (size_t)P * M * sizeof(double)));
+    DMO_TRY(copy_out(ctx, counts, cnt.p, 4 * sizeof(int64_t)));
+  }
   if (hv_ref && hv_out) {
     ProfileScope ps(ctx, "step_hv");
     // the survivors carry their ranks within the merged set: rows of rank > 0 cannot add volume (hv.cu)
@@ -148,5 +225,30 @@ int dmo_nsga2_step(dmo_ctx* ctx, dmo_gp* gp, double* pop_x, double* pop_y, int32
     DMO_TRY(hypervolume_device_ranked(ctx, pop_y, pop, M, h_ref, rank, hv_out));
   }
   return DMO_OK;
+}
+
+extern "C" {
+int dmo_nsga2_step(dmo_ctx* ctx, dmo_gp* gp, double* pop_x, double* pop_y, int32_t* rank, int64_t pop, int d, int M,
+                   double crossover_prob, double mutation_prob, double mutation_rate, const double* di_crossover,
+                   const double* di_mutation, const double* xlb, const double* xub, uint64_t seed, uint64_t stream_id,
+                   int precision, int distance_metric, int with_variance, int round_to_f32, const double* hv_ref, int64_t* n_children,
+                   double* hv_out) {
+  return nsga2_step_body(ctx, gp, nullptr, pop_x, pop_y, rank, pop, d, M, crossover_prob, mutation_prob, mutation_rate,
+                         di_crossover, di_mutation, xlb, xub, seed, stream_id, precision, distance_metric, with_variance,
+                         round_to_f32, hv_ref, n_children, hv_out, nullptr, nullptr, nullptr);
+}
+
+int dmo_nsga2_step_record(dmo_ctx* ctx, dmo_gp* gp, const dmo_feas* key, double* pop_x, double* pop_y, int32_t* rank,
+                          int64_t pop, int d, int M, double crossover_prob, double mutation_prob, double mutation_rate,
+                          const double* di_crossover, const double* di_mutation, const double* xlb, const double* xub,
+                          uint64_t seed, uint64_t stream_id, int precision, int distance_metric, int round_to_f32,
+                          double* x_gen, double* y_gen, int64_t* counts, int64_t* n_children) {
+  if (!ctx) return DMO_ERR_ARG;
+  DMO_REQUIRE(x_gen && y_gen && counts, "nsga2_step_record: x_gen, y_gen and counts are required");
+  DMO_REQUIRE(!key || feas_model_dim(key) == d, "nsga2_step_record: the key model takes %d columns, the population has %d",
+              feas_model_dim(key), d);
+  return nsga2_step_body(ctx, gp, key, pop_x, pop_y, rank, pop, d, M, crossover_prob, mutation_prob, mutation_rate,
+                         di_crossover, di_mutation, xlb, xub, seed, stream_id, precision, distance_metric, 0, round_to_f32,
+                         nullptr, n_children, nullptr, x_gen, y_gen, counts);
 }
 }

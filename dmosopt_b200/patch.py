@@ -19,10 +19,15 @@ called by the reference's controller code directly on its own modules, so swappi
 
 ``install()`` rebinds exactly those module attributes of an already importable ``dmosopt`` package to the functions of
 this package (same signatures, same results: see tests/test_gpu_reference_loop.py) and ``uninstall()`` restores them.
+``install(resident_epoch=True)`` also rebinds ``MOASMO.optimize``, the surrogate epoch of ``MOASMO.epoch``: an epoch
+that ``dmosopt_b200.MOASMO.resident_eligible`` accepts (this package's NSGA2 with a GPR_Matern / GPR_RBF surrogate) runs
+on the resident generation step, with the per-generation loop's results; every other epoch runs the reference's own
+``optimize`` unchanged, including the yield / send protocol of an epoch without a surrogate.
 Nothing is patched implicitly; importing dmosopt_b200 never touches dmosopt.
 """
 
 import importlib
+import inspect
 
 import numpy as np
 
@@ -45,10 +50,35 @@ def _dda_ens(Y, return_dom=False):
     return _lib.rank_nd(np.asarray(Y, dtype=np.float64))
 
 
-def install(package="dmosopt"):
-    """Route the helpers listed in the module docstring to the GPU.  Returns the list of patched names."""
-    if _saved:
-        return [f"{o.__name__}.{n}" for o, n, _ in _saved]
+def install(package="dmosopt", resident_epoch=False):
+    """Route the helpers listed in the module docstring to the GPU (and, with ``resident_epoch``, eligible surrogate
+    epochs to the resident generation step).  Returns the list of patched names."""
+    if not _saved:
+        _install_helpers(package)
+    if resident_epoch and not any(name == "optimize" for _, name, _ in _saved):
+        _install_resident_epoch(package)
+    return [f"{getattr(o, '__name__', o)}.{n}" for o, n, _ in _saved]
+
+
+def _install_resident_epoch(package):
+    from . import MOASMO as _moasmo
+
+    moasmo = importlib.import_module(f"{package}.MOASMO")
+    original = moasmo.optimize
+    signature = inspect.signature(original)
+
+    def optimize(*args, **kwargs):
+        a = signature.bind(*args, **kwargs)
+        a.apply_defaults()
+        if _moasmo.resident_eligible(a.arguments["optimizer"], a.arguments["model"], a.arguments["optimize_mean_variance"]):
+            return (yield from _moasmo.optimize(*args, **kwargs))
+        return (yield from original(*args, **kwargs))
+
+    optimize.__doc__ = original.__doc__
+    _set(moasmo, "optimize", optimize)
+
+
+def _install_helpers(package):
     moea = importlib.import_module(f"{package}.MOEA")
     ind = importlib.import_module(f"{package}.indicators")
     dda = importlib.import_module(f"{package}.dda")
@@ -99,7 +129,6 @@ def install(package="dmosopt"):
         return original(self, pareto_front, algorithm, verbose)
 
     _set(hv.AdaptiveHyperVolume, "compute_hypervolume", compute_hypervolume)
-    return [f"{getattr(o, '__name__', o)}.{n}" for o, n, _ in _saved]
 
 
 def uninstall():

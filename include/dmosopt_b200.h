@@ -194,6 +194,26 @@ int dmo_nsga2_step(dmo_ctx* ctx, dmo_gp* gp, double* pop_x, double* pop_y, int32
                    int distance_metric, int with_variance, int round_to_f32, const double* hv_ref,
                    int64_t* n_children, double* hv_out);
 
+/* One generation of dmo_nsga2_step with the posterior mean only and no hypervolume, recorded for MOASMO.optimize's
+ * epoch results (dmosopt/MOASMO.py:105-122): the resident epoch of dmosopt_b200.MOASMO.optimize.
+ * key (may be NULL): a feasibility model (dmo_feas_create) whose rank over [children; parents] is the truncation's
+ *   least significant descending key, as in dmo_remove_worst_pair_keys; its d must equal d.
+ * x_gen (pop+1, d), y_gen (pop+1, M): the first n_children rows receive the offspring (NSGA2.generate) and their
+ *   posterior mean (GPR_Matern.evaluate), after AUTO has refined its rows.
+ * counts (4,): children from crossover, mutants, crossover children among the survivors, mutants among the survivors
+ *   (what NSGA2.update_strategy counts, NSGA2.py:216-222).
+ * x_gen, y_gen and counts are required.  Unlike the other entry points, the call may return before they are written:
+ * into device or page-locked host memory the copies are enqueued without a host wait, and they are complete after
+ * dmo_synchronize(ctx).  Pageable host memory is accepted; the copy into it blocks the host (one counted wait each).
+ * n_children (host, may be NULL) is written before the call returns.  With key == NULL the population, objectives,
+ * ranks and n_children are those of dmo_nsga2_step(..., with_variance = 0, ..., hv_ref = NULL, ...), bit for bit. */
+int dmo_nsga2_step_record(dmo_ctx* ctx, dmo_gp* gp, const dmo_feas* key, double* pop_x, double* pop_y,
+                          int32_t* rank, int64_t pop, int d, int M, double crossover_prob,
+                          double mutation_prob, double mutation_rate, const double* di_crossover,
+                          const double* di_mutation, const double* xlb, const double* xub, uint64_t seed,
+                          uint64_t stream_id, int precision, int distance_metric, int round_to_f32,
+                          double* x_gen, double* y_gen, int64_t* counts, int64_t* n_children);
+
 /* ---- A18: exact-GP posterior (GPR_Matern / GPR_RBF predict) -------------------
  * replaces GPR_Matern.predict / .evaluate (dmosopt/model.py:1254-1275; GPR_RBF :1343-1364),
  * i.e. per objective sklearn GaussianProcessRegressor.predict(return_std=True) ** 2.
