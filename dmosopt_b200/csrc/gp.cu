@@ -593,9 +593,6 @@ int gp_calibrate(dmo_ctx* ctx, dmo_gp* gp) {
   gp->auto_var_tensor = gp->auto_mean_tensor && ev <= 4.5e-6;
   gp->refine_theta = fmax(0.02, 2.0 * ev / 1e-5);
   gp->calibrated = true;
-  if (getenv("DMO_GP_VERBOSE"))
-    fprintf(stderr, "dmosopt_b200: GP calibration (N=%lld d=%d M=%d): mean err K*alpha %.3e, mean-only kernel %.3e, var err/prior %.3e -> mean %s, var %s, theta %.3f\n",
-            (long long)gp->N, d, M, em, eo, ev, gp->auto_mean_tensor ? "K*alpha pass" : "float64", gp->auto_var_tensor ? "tensor" : "float64", gp->refine_theta);
   return DMO_OK;
 }
 

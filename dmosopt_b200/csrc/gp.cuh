@@ -101,19 +101,18 @@ int gp_prepare_tensor(dmo_ctx* ctx, GpVarOps& ops);
 // k_alloc rows are allocated, plane g < ops.G reads rows g * k_rows + [0, Pcpad) (k_rows = 0: one K_* plane for every
 // g); Pcpad is a multiple of GP_TC_TILE.  vnorm[q][g][p], q < gp_tensor_var_planes(ops.Npad), holds the partial sums.
 // abort_flag (device int, zeroed by the caller) is set when the pipeline watchdog trips.  The grid is the smallest one
-// with as many work items per CTA as sm_count CTAs would take, less `reserve` further CTAs; every item writes its own
-// vnorm slot, so the grid does not change a bit.
+// with as many work items per CTA as sm_count CTAs would take; every item writes its own vnorm slot, so the grid does
+// not change a bit.
 constexpr int GP_TC_TILE = 128;
 int gp_tensor_var_planes(int64_t Npad);
 int gp_var_contract_tensor(dmo_ctx* ctx, const GpVarOps& ops, const uint16_t* Kh, const uint16_t* Kl, int64_t k_alloc,
-                           int64_t k_rows, int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag, int reserve = 0);
+                           int64_t k_rows, int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag);
 // A caller that runs its own work beside the variance contraction (the fused step's lane, step.cu) passes this to the
-// tensor route: mean_ready is recorded on the stream once the last chunk's mean is written, the contraction runs on the
-// context's high-priority stream (joined back before var_finish_tc_kernel), and `reserve` SMs are kept out of its grid.
-// The caller creates those streams first (dmo_lane_streams).
+// tensor route: mean_ready is recorded on the stream once the last chunk's mean is written, and the contraction runs on
+// the context's high-priority stream (joined back before var_finish_tc_kernel); the caller's work has the SMs the
+// contraction's grid leaves free.  The caller creates those streams first (dmo_lane_streams).
 struct GpOverlap {
   cudaEvent_t mean_ready = nullptr;
-  int reserve = 0;
 };
 // abort_flag null: the call reads the contraction's watchdog back and fails when it tripped.  Otherwise the call zeroes
 // *abort_flag (device) and the watchdog lands there; the caller reads it back and fails the same way (gp_predict_auto folds

@@ -1022,7 +1022,7 @@ static_assert(TMV == GP_TC_TILE, "gp.cuh exports the wgmma candidate tile");
 int gp_tensor_var_planes(int64_t Npad) { return (int)((Npad / TN + 1) / 2); }
 
 int gp_var_contract_tensor(dmo_ctx* ctx, const GpVarOps& ops, const uint16_t* Kh, const uint16_t* Kl, int64_t k_alloc,
-                           int64_t k_rows, int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag, int reserve) {
+                           int64_t k_rows, int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag) {
   const int64_t Npad = ops.Npad;
   DMO_REQUIRE(Npad % TN == 0 && Pcpad % TMV == 0, "gp_var_contract_tensor: internal padding error");
   CUtensorMap map_kh, map_kl, map_lh, map_ll;
@@ -1045,12 +1045,8 @@ int gp_var_contract_tensor(dmo_ctx* ctx, const GpVarOps& ops, const uint16_t* Kh
   // static round-robin: the makespan is ceil(n_work / grid) items, so the smallest grid with that many items per CTA
   // finishes with it and leaves the other SMs free (at the bench shape 4096 items take 128 CTAs, not 132)
   const int n_work = prm.M * prm.n_pb * prm.n_q;
-  int per_cta = (int)ceil_div(n_work, ctx->sm_count);
-  int grid = (int)ceil_div(n_work, per_cta);
-  if (reserve > 0) {  // `reserve` SMs more kept free, at a longer makespan; at least one CTA
-    per_cta = (int)ceil_div(n_work, reserve < grid ? grid - reserve : 1);
-    grid = (int)ceil_div(n_work, per_cta);
-  }
+  const int per_cta = (int)ceil_div(n_work, ctx->sm_count);
+  const int grid = (int)ceil_div(n_work, per_cta);
   DMO_LAUNCH(gp_var_wgmma_kernel, grid, NTHREADS, GEMM_SMEM, map_kh, map_kl, map_lh, map_ll, prm);
   return DMO_OK;
 }
@@ -1181,8 +1177,7 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
           DMO_CUDA(cudaStreamWaitEvent(ctx->gp_hi, ctx->lane_ev[1], 0));
           ctx->stream = ctx->gp_hi;
         }
-        const int rc = gp_var_contract_tensor(ctx, gp->ops, Kh.p, Kl.p, G * Pc_alloc, Pc_alloc, Pcpad, vnorm.p, Pc_alloc, abort_flag,
-                                              ov ? ov->reserve : 0);
+        const int rc = gp_var_contract_tensor(ctx, gp->ops, Kh.p, Kl.p, G * Pc_alloc, Pc_alloc, Pcpad, vnorm.p, Pc_alloc, abort_flag);
         if (ov) {
           ctx->stream = main;
           DMO_CUDA(cudaEventRecord(ctx->lane_ev[2], ctx->gp_hi));

@@ -27,9 +27,7 @@
 // Algorithmic bytes: 8 n M read + 4 n written; pair tests <= n^2 / 2 (compare / latency bound, see DESIGN.md section 4.2).
 #include <stdlib.h>
 
-#include <cstdio>
 #include <type_traits>
-#include <vector>
 
 #include "common.cuh"
 
@@ -311,15 +309,7 @@ __device__ __forceinline__ int maxplus_packed(const int8_t* row, const int16_t* 
 // Above eight objectives the shared memory alone limits a CTA to four per SM, so the register cap follows that.
 template <int M, int T, bool SEG>
 __global__ void __launch_bounds__(T, (SEG || M > 8) ? 4 : 5) rank_chain_kernel(uint32_t* rec, int nblocks, int* __restrict__ rankS, int* ticket,
-                                                                 int* errflag, long long* trace, RankSeg sg) {
-  // optional per-block time stamps (DMO_RANK_TRACE=<file>): 16 x globaltimer ns, then 16 x clock64, see scripts/rank_trace.py
-#define RANK_TRACE(slot)                                                         \
-  if (trace != nullptr && tid == 0) {                                            \
-    long long gt_;                                                               \
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt_));                     \
-    trace[(int64_t)b * 32 + (slot)] = gt_;                                       \
-    trace[(int64_t)b * 32 + 16 + (slot)] = clock64();                             \
-  }
+                                                                 int* errflag, RankSeg sg) {
   constexpr int W = 4 * ((M + 1 + 3) / 4);
   constexpr int NV = W / 4;
   constexpr int NW = T / 32;
@@ -360,12 +350,6 @@ __global__ void __launch_bounds__(T, (SEG || M > 8) ? 4 : 5) rank_chain_kernel(u
     __syncthreads();
     if (b >= nblocks) return;
     const int64_t i = (int64_t)b * T + tid;
-    RANK_TRACE(0);
-    if (trace != nullptr && tid == 0) {
-      unsigned smid_;
-      asm volatile("mov.u32 %0, %%smid;" : "=r"(smid_));
-      trace[(int64_t)b * 32 + 7] = smid_;
-    }
 
     // ---- own record -> registers and shared tile
     uint32_t v[W];
@@ -536,7 +520,6 @@ __global__ void __launch_bounds__(T, (SEG || M > 8) ? 4 : 5) rank_chain_kernel(u
     }
 
     // ---- stream every earlier block except the predecessor: best = max over dominators of (rank + 1)
-    RANK_TRACE(1);
     // Software pipelined: the data of the next tile (static words and, speculatively, its rank word -- or its staircase
     // entry) is requested before the current tile is evaluated, and the shared tile is double buffered, so a block that is
     // behind the wavefront pays one barrier and the evaluation per tile, not an L2 round trip on top; a block at the
@@ -576,7 +559,6 @@ __global__ void __launch_bounds__(T, (SEG || M > 8) ? 4 : 5) rank_chain_kernel(u
       if (k < b - 1) request(k, kind);
       int pb = 0;  // stream buffer parity
       while (k < b - 1) {
-        if (k == b - 2) RANK_TRACE(2);
         {
           unsigned spins = 0;
           if (SEG && kind == 2) {
@@ -619,7 +601,6 @@ __global__ void __launch_bounds__(T, (SEG || M > 8) ? 4 : 5) rank_chain_kernel(u
         if (kn < b - 1) request(kn, kind_n);  // consumed after this tile's evaluation
         // one barrier per tile: a stream buffer is rewritten two tiles later, after the next tile's barrier
         const bool may_share_group = __syncthreads_or(last_shares ? 1 : 0) != 0;
-        if (k == b - 2) RANK_TRACE(3);
         const uint32_t* c1tb = c1t + (SEG ? pb * T : 0);
         if (SEG && kind == 2) {
           const uint2* st = reinterpret_cast<const uint2*>(tb);  // .x = key (ascending), .y = running max of rank + 1
@@ -692,7 +673,6 @@ __global__ void __launch_bounds__(T, (SEG || M > 8) ? 4 : 5) rank_chain_kernel(u
     if (b > 0) {
       const int k = b - 1;
       // ---- critical section starts here
-      RANK_TRACE(4);
       bool big;
       {
         const uint32_t* rw = rec + ((int64_t)k * T + tid) * W + M;
@@ -710,7 +690,6 @@ __global__ void __launch_bounds__(T, (SEG || M > 8) ? 4 : 5) rank_chain_kernel(u
         big = (int)r1 > PACK_LIMIT || r > PACK_LIMIT;
       }
       const int any_big = __syncthreads_or(big ? 1 : 0);
-      RANK_TRACE(5);
       if (!any_big) {
         r = maxplus_packed<T>(sE + tid * DLD, sh_h16, r);
       } else {
@@ -722,7 +701,6 @@ __global__ void __launch_bounds__(T, (SEG || M > 8) ? 4 : 5) rank_chain_kernel(u
     }
     st_relaxed_u32(rec + i * W + M, (uint32_t)(r + 1));  // publish: the rank word doubles as the ready flag
     rankS[i] = r;
-    RANK_TRACE(6);
     if (SEG) {
       // staircase of this tile for the blocks of later segments (off the critical path: they are at least a segment
       // away): running maximum of rank + 1 in ascending order of the last compare word; key and value travel in one
@@ -743,7 +721,6 @@ __global__ void __launch_bounds__(T, (SEG || M > 8) ? 4 : 5) rank_chain_kernel(u
     }
     __syncthreads();
   }
-#undef RANK_TRACE
 }
 
 // Rank-0 test only (filter for the hypervolume / EHVI routines): "is some point dominating me" has no dependency chain,
@@ -820,13 +797,6 @@ __global__ void copy_u32_to_i32_kernel(const uint32_t* __restrict__ a, int64_t n
 
 template <int M, bool SEG>
 int launch_chain(dmo_ctx* ctx, uint32_t* rec, int nblocks, int* rankS, int* ticket, int* errflag, const RankSeg& sg) {
-  // debugging aid: DMO_RANK_TRACE=<file> dumps 32 int64 time stamps per block of the chain kernel
-  DevBuf<long long> trace;
-  const char* trace_path = getenv("DMO_RANK_TRACE");
-  if (trace_path && *trace_path) {
-    DMO_TRY(trace.alloc(ctx, (size_t)nblocks * 32));
-    DMO_CUDA(cudaMemsetAsync(trace.p, 0, (size_t)nblocks * 32 * sizeof(long long), ctx->stream));
-  }
   constexpr int NV = (M + 1 + 3) / 4;
   const size_t dyn = NV > 4 ? (size_t)RANK_T * NV * sizeof(uint4) : 0;  // the kernel's DYN_TILE
   if (dyn > 0)
@@ -842,17 +812,8 @@ int launch_chain(dmo_ctx* ctx, uint32_t* rec, int nblocks, int* rankS, int* tick
   int nctas = nblocks < occ * ctx->sm_count ? nblocks : occ * ctx->sm_count;
   {
     ProfileScope ps(ctx, "rank_chain");
-    DMO_LAUNCH((rank_chain_kernel<M, RANK_T, SEG>), nctas, RANK_T, dyn, rec, nblocks, rankS, ticket, errflag, trace.p, sg);
+    DMO_LAUNCH((rank_chain_kernel<M, RANK_T, SEG>), nctas, RANK_T, dyn, rec, nblocks, rankS, ticket, errflag, sg);
     DMO_CHECK_LAUNCH();
-  }
-  if (trace.p) {
-    std::vector<long long> h((size_t)nblocks * 32);
-    DMO_CUDA(cudaMemcpyAsync(h.data(), trace.p, h.size() * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
-    DMO_CUDA(dmo_wait(ctx));
-    if (FILE* f = fopen(trace_path, "wb")) {
-      fwrite(h.data(), sizeof(long long), h.size(), f);
-      fclose(f);
-    }
   }
   return DMO_OK;
 }

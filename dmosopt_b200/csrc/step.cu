@@ -14,7 +14,6 @@
 // dmo_nsga2_step_record runs the same body for MOASMO.optimize's resident epoch (dmosopt_b200/MOASMO.py): the mean only,
 // optionally a feasibility rank as the truncation's last key, and the generation's offspring, their mean and operator
 // counts copied out without a host wait.
-#include <stdlib.h>
 #include <string.h>
 
 #include <algorithm>
@@ -130,27 +129,19 @@ static int nsga2_step_body(dmo_ctx* ctx, dmo_gp* gp, const dmo_feas* key, double
     kp[0] = kx.p;
   }
   // The GP's read-back is left pending and the truncation is enqueued before the host waits for it.  The truncation needs
-  // the posterior mean only, which the tensor route writes before its variance contraction: by default (DMO_STEP_OVERLAP
-  // unset or not 0) the truncation runs on the context's lane stream from that point on, beside the contraction, which
-  // runs on a higher-priority stream on the SMs its grid leaves free (DMO_GP_VAR_RESERVE=r keeps r more from it).  With
-  // DMO_STEP_OVERLAP=0 it queues behind the whole GP on the main stream.  Either way its host waits (peel probe, peel
-  // counts) wait for its own stream only.  If the GP then fails, the population is put back (the parents are still in
-  // Xs / Ys); if AUTO refines rows, the truncation runs again on them.  Every buffer the two streams share is allocated
-  // on the main stream before the fork and released after the join.
-  const char* ov_env = getenv("DMO_STEP_OVERLAP");
-  const bool overlap = !(ov_env && atoi(ov_env) == 0);
-  int var_reserve = 0;
-  if (const char* e = getenv("DMO_GP_VAR_RESERVE")) var_reserve = atoi(e);
-  DMO_REQUIRE(var_reserve >= 0, "nsga2_step: DMO_GP_VAR_RESERVE must not be negative");
+  // the posterior mean only, which the tensor route writes before its variance contraction: when the GP defers its
+  // read-back, the truncation runs on the context's lane stream from that point on, beside the contraction, which runs on
+  // a higher-priority stream on the SMs its grid leaves free.  Otherwise (float64 or tensor precision, a linear mean, a
+  // non-tensor AUTO route) the GP has finished inside the call and the truncation follows it on the main stream.  Either
+  // way its host waits (peel probe, peel counts) wait for its own stream only.  If the GP then fails, the population is
+  // put back (the parents are still in Xs / Ys); if AUTO refines rows, the truncation runs again on them.  Every buffer
+  // the two streams share is allocated on the main stream before the fork and released after the join.
   GpPending gpp;
   DevBuf<int32_t> rank_in;  // the ranks before the truncation, for the failure path
   if (P > 0) {
     DMO_TRY(rank_in.alloc(ctx, pop));
-    if (overlap) {
-      DMO_TRY(dmo_lane_streams(ctx));
-      gpp.ov.mean_ready = ctx->lane_ev[0];
-      gpp.ov.reserve = var_reserve;
-    }
+    DMO_TRY(dmo_lane_streams(ctx));
+    gpp.ov.mean_ready = ctx->lane_ev[0];
     ProfileScope ps(ctx, "step_gp");
     DMO_TRY(gp_predict_device(ctx, gp, Xs.p, P, Ys.p, with_variance ? var.p : nullptr, precision, &gpp));
   }

@@ -37,25 +37,3 @@ for g in range(int(sys.argv[1]) if len(sys.argv) > 1 else 4):
     os.environ.pop("DMO_RANK_NOSEG", None)
     opt.update(x_gen, y_gen, st)
 
-# optional: timeline of the last generation's merged set (DMO_RANK_TRACE must be set before the library launches)
-if os.environ.get("RANK_REAL_TRACE"):
-    import tempfile
-    path = os.path.join(tempfile.gettempdir(), "rank_trace_real.bin")
-    os.environ["DMO_RANK_TRACE"] = path
-    L._check(lib.dmo_rank_nd(ctx, dY.ptr, Y.shape[0], M, r.ptr), "rank")
-    t = np.fromfile(path, dtype=np.int64).reshape(-1, 32)
-    c = t[:, 16:32].astype(np.float64)
-    g = t[:, :16].astype(np.float64)
-    pub = g[:, 6] - g[:, 0].min()
-    print("span us", pub.max() / 1e3, "link mean/median ns", np.diff(pub).mean(), np.median(np.diff(pub)))
-    for nm, a, b in [("tables", 0, 1), ("bulk", 1, 2), ("wait b-2", 2, 3), ("tile b-2 + fold", 3, 4), ("wait pred", 4, 5), ("resolve", 5, 6)]:
-        ok = (t[:, a] > 0) & (t[:, b] > 0)
-        dd = (c[:, b] - c[:, a])[ok]
-        print(f"  {nm:16s} cycles mean {dd.mean():10.0f} median {np.median(dd):10.0f} p90 {np.percentile(dd, 90):10.0f}")
-    sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-    import rank_trace
-    gg = g - g[:, 0].min()
-    rank_trace.dump_gaps(gg, pub, k=24)
-    link = np.diff(pub)
-    big = link > 8000
-    print("links > 8 us:", int(big.sum()), "of", len(link), "sum", link[big].sum() / 1e3, "us; blocks:", np.flatnonzero(big)[:40] + 1)

@@ -1,19 +1,16 @@
 """Where the resident NSGA-II generation step (dmo_nsga2_step, bench.py's `value`) spends its time, phase by phase.
 
 Builds bench.py's workload (bench.workload, same seed, same GP model, pop 65 536, d 30, M 3, N_train 4096 by default)
-and measures the fused step under a list of settings, one after the other in the same process (--rounds times over):
-  * serial:  DMO_STEP_OVERLAP=0, the truncation queued behind the whole GP on one stream;
-  * r=<r>:   the truncation on its own stream beside the GP's variance contraction, with DMO_GP_VAR_RESERVE=r SMs kept
-             from the contraction beyond those its grid leaves free (--reserves, default 0,4,8,12).
-Each setting runs --warmup generations, then --steps timed generations with the profile timers off (the whole step, by
-device events around the window and by the host clock; host waits and kernel launches per generation), then --steps
-generations with the library's per-scope CUDA-event timers on, and prints per generation:
+and measures the fused step --rounds times in the same process.  Each round runs --warmup generations, then --steps
+timed generations with the profile timers off (the whole step, by device events around the window and by the host
+clock; host waits and kernel launches per generation), then --steps generations with the library's per-scope
+CUDA-event timers on, and prints per generation:
   * device-timer ms of each phase (step_tournament, step_generate, step_gp, step_truncate, step_hv) and of the kernels
     inside them that have scopes of their own (gp_kstar, gp_var, rank_peel, ...);
   * beside the contraction: the lane's wall time (step_truncate) against the contraction's window (gp_var), both from the
     point the mean is written, and the slack between them (positive: the lane finished inside the window);
   * the card's name, its power limit and the median SM clock sampled during the timed window.
-Usage: python scripts/step_phases.py [--steps 100] [--warmup 20] [--reserves 0,4,8,12] [--rounds 1] [--json OUT.json]
+Usage: python scripts/step_phases.py [--steps 100] [--warmup 20] [--rounds 1] [--json OUT.json]
 """
 
 import argparse
@@ -83,8 +80,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--warmup", type=int, default=20)
-    ap.add_argument("--reserves", default="0,4,8,12", help="DMO_GP_VAR_RESERVE values to run with the overlapped step")
-    ap.add_argument("--rounds", type=int, default=1, help="times the whole list of settings is run, alternating")
+    ap.add_argument("--rounds", type=int, default=1, help="times the step is measured, one after the other")
     ap.add_argument("--pop", type=int, default=65536)
     ap.add_argument("--dim", type=int, default=30)
     ap.add_argument("--obj", type=int, default=3)
@@ -110,45 +106,38 @@ def main():
     rs.precision, rs.metric = L.GP_AUTO, L.METRIC_NONE
     name, plimit = card(0)
 
-    settings = [("serial", {"DMO_STEP_OVERLAP": "0"})]
-    settings += [(f"r={r}", {"DMO_STEP_OVERLAP": "1", "DMO_GP_VAR_RESERVE": r}) for r in args.reserves.split(",") if r.strip()]
     results = []
     for rnd in range(args.rounds):
-        for label, env in settings:
-            os.environ.pop("DMO_GP_VAR_RESERVE", None)
-            os.environ.update(env)
-            out = measure(L, bench, rs, args.steps, args.warmup)
-            out.update(setting=label, round=rnd)
-            results.append(out)
-            ph, sc = out["phases_ms"], out["scopes_ms"]
-            print(f"--- {label} (round {rnd}): {name}, power limit {plimit} W, median SM clock {out['sm_mhz_median']} MHz, "
-                  f"{args.steps} generations")
-            print(f"{'phase':<18}{'ms / generation':>16}")
-            for k in PHASES:
-                if k in ph:
-                    print(f"{k:<18}{ph[k]:>16.3f}")
-            for k, v in sc.items():
-                print(f"  {k:<16}{v:>16.3f}")
-            print(f"{'step (events)':<18}{out['step_ms_device']:>16.3f}")
-            print(f"{'step (host)':<18}{out['step_ms_host']:>16.3f}")
-            print(f"{'outside step_gp':<18}{out['outside_gp_ms']:>16.3f}")
-            if label != "serial" and "lane_slack_ms" in out:
-                print(f"lane {ph['step_truncate']:.3f} ms against the contraction's window {sc['gp_var']:.3f} ms: "
-                      f"slack {out['lane_slack_ms']:+.3f} ms")
-            print(f"host waits / generation {out['waits_per_step']:.2f}, launches / generation {out['launches_per_step']:.1f}", flush=True)
-    for k in ("DMO_STEP_OVERLAP", "DMO_GP_VAR_RESERVE"):
-        os.environ.pop(k, None)
+        out = measure(L, bench, rs, args.steps, args.warmup)
+        out.update(round=rnd)
+        results.append(out)
+        ph, sc = out["phases_ms"], out["scopes_ms"]
+        print(f"--- round {rnd}: {name}, power limit {plimit} W, median SM clock {out['sm_mhz_median']} MHz, "
+              f"{args.steps} generations")
+        print(f"{'phase':<18}{'ms / generation':>16}")
+        for k in PHASES:
+            if k in ph:
+                print(f"{k:<18}{ph[k]:>16.3f}")
+        for k, v in sc.items():
+            print(f"  {k:<16}{v:>16.3f}")
+        print(f"{'step (events)':<18}{out['step_ms_device']:>16.3f}")
+        print(f"{'step (host)':<18}{out['step_ms_host']:>16.3f}")
+        print(f"{'outside step_gp':<18}{out['outside_gp_ms']:>16.3f}")
+        if "lane_slack_ms" in out:
+            print(f"lane {ph['step_truncate']:.3f} ms against the contraction's window {sc['gp_var']:.3f} ms: "
+                  f"slack {out['lane_slack_ms']:+.3f} ms")
+        print(f"host waits / generation {out['waits_per_step']:.2f}, launches / generation {out['launches_per_step']:.1f}", flush=True)
 
     print(f"\n{name}, power limit {plimit} W, pop {pop}, dim {d}, {M} objectives, N_train {N}")
-    print(f"{'setting':<10}{'round':>6}{'step ms':>10}{'gp_var':>9}{'lane':>9}{'slack':>9}{'SM MHz':>9}")
+    print(f"{'round':>6}{'step ms':>10}{'gp_var':>9}{'lane':>9}{'slack':>9}{'SM MHz':>9}")
     for r in results:
         ph, sc = r["phases_ms"], r["scopes_ms"]
-        slack = r.get("lane_slack_ms") if r["setting"] != "serial" else None
-        print(f"{r['setting']:<10}{r['round']:>6}{r['step_ms_device']:>10.3f}{sc.get('gp_var', float('nan')):>9.3f}"
+        slack = r.get("lane_slack_ms")
+        print(f"{r['round']:>6}{r['step_ms_device']:>10.3f}{sc.get('gp_var', float('nan')):>9.3f}"
               f"{ph.get('step_truncate', float('nan')):>9.3f}{(f'{slack:+.3f}' if slack is not None else '-'):>9}"
               f"{(r['sm_mhz_median'] or float('nan')):>9.0f}")
     summary = {"card": name, "power_limit_w": plimit, "steps": args.steps, "pop": pop, "dim": d, "obj": M, "ntrain": N,
-               "settings": results}
+               "rounds": results}
     print(json.dumps(summary), flush=True)
     if args.json:
         with open(args.json, "w") as f:

@@ -26,7 +26,7 @@ from oracle import dda, indicators
 pytestmark = pytest.mark.gpu
 
 ROUTE_VARS = ("DMO_RANK_SEGBITS", "DMO_RANK_NOSEG", "DMO_RANK_OCC", "DMO_ND_BRUTE", "DMO_RANK_PEEL", "DMO_RANK_PEEL_NOPROBE",
-              "DMO_PEEL_GBITS", "DMO_RANK_TRACE")
+              "DMO_PEEL_GBITS")
 
 
 @pytest.fixture(scope="module")

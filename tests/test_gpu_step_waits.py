@@ -1,6 +1,7 @@
-"""dmo_nsga2_step composes the device bodies of the entry points it uses, without their trailing host waits.  For several
-generations the fused step runs beside the same generation composed from the public entry points on device buffers (as
-bench.py's multi-GPU branch composes it), from the same population and Philox streams: population, objectives, ranks,
+"""dmo_nsga2_step composes the device bodies of the entry points it uses, without their trailing host waits, and on the
+tensor route truncates on a stream of its own beside the GP's variance contraction.  For several generations the fused
+step runs beside the same generation composed serially from the public entry points on device buffers (as bench.py's
+multi-GPU branch composes it), from the same population and Philox streams: population, objectives, ranks,
 offspring count and hypervolume must be bit-identical, and the fused step must wait on the host only where it needs a
 value (the offspring count, one read-back after the GP, one per peeled front and the hypervolume's route and value), i.e.
 exactly the composed calls' waits minus the trailing wait of each of the four wrappers (plus a second truncation's when
@@ -47,6 +48,8 @@ CASES = {
     "odd_pop": (30, 1024, 8193, "dtlz2", 0, None),
     # merged set below the peel threshold (n < 8192): the chain, no peel
     "small_chain": (30, 1024, 4095, "dtlz2", 0, "chain_only"),
+    # the same with crowding: the chain and the crowding distance on the lane beside the variance contraction
+    "chain_crowding": (30, 1024, 4095, "dtlz2", 1, "chain_only"),
 }
 
 
@@ -139,5 +142,5 @@ def test_fused_step_equals_composed_entry_points_with_fewer_waits(L, case):
             assert "rank_chain" in prof and "rank_peel" not in prof, (msg, sorted(prof))
     if case == "refined":
         assert tensor and max(refined) > 0, refined
-    elif case in ("bench_peel", "crowding", "euclidean", "odd_pop"):
+    elif case in ("bench_peel", "crowding", "euclidean", "odd_pop", "chain_crowding"):
         assert tensor, case
