@@ -346,6 +346,18 @@ int hypervolume_device(dmo_ctx* ctx, const double* dF, int64_t n, int M, const d
 // the same when the rows carry their non-dominated ranks within a superset (rank > 0 rows are skipped, no filter pass)
 int hypervolume_device_ranked(dmo_ctx* ctx, const double* dF, int64_t n, int M, const double* h_ref, const int32_t* d_rank,
                               double* h_out);
+// its M = 3 route in two halves (hv.cu): the device work, with no host read, then the route's reads and the volume.
+// h_ref must be finite.  The buffers are released by the destructor, on the stream current at that point.
+struct Hv3Ranked {
+  int64_t n = 0;
+  double ref[3] = {0.0, 0.0, 0.0};
+  bool tree = false;
+  DevBuf<int32_t> pos;
+  DevBuf<double> xs, ys, zs, res;
+  DevBuf<uint32_t> zo;
+};
+int hv3_ranked_enqueue(dmo_ctx* ctx, const double* dF, int64_t n, const double* h_ref, const int32_t* d_rank, Hv3Ranked& s);
+int hv3_ranked_finish(dmo_ctx* ctx, Hv3Ranked& s, double* h_out);
 // device bodies of dmo_tournament, dmo_nsga2_generate and dmo_remove_worst (variation.cu, sortmo.cu) for dmo_nsga2_step:
 // device arrays only, enqueued on the context's stream without the public entry points' trailing wait.  The generate body
 // waits once, for the offspring count it returns in *n_children.

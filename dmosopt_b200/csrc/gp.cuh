@@ -101,16 +101,23 @@ int gp_prepare_tensor(dmo_ctx* ctx, GpVarOps& ops);
 // k_alloc rows are allocated, plane g < ops.G reads rows g * k_rows + [0, Pcpad) (k_rows = 0: one K_* plane for every
 // g); Pcpad is a multiple of GP_TC_TILE.  vnorm[q][g][p], q < gp_tensor_var_planes(ops.Npad), holds the partial sums.
 // abort_flag (device int, zeroed by the caller) is set when the pipeline watchdog trips.  The grid is the smallest one
-// with as many work items per CTA as sm_count CTAs would take; every item writes its own vnorm slot, so the grid does
-// not change a bit.
+// with as many work items per CTA as sm_count - free_sms CTAs would take; every item writes its own vnorm slot, so the
+// grid does not change a bit.
 constexpr int GP_TC_TILE = 128;
 int gp_tensor_var_planes(int64_t Npad);
 int gp_var_contract_tensor(dmo_ctx* ctx, const GpVarOps& ops, const uint16_t* Kh, const uint16_t* Kl, int64_t k_alloc,
-                           int64_t k_rows, int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag);
+                           int64_t k_rows, int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag, int free_sms = 0);
+// SMs the overlapped contraction leaves to the fused step's lane (the truncation and the hypervolume, step.cu).  Each SM
+// taken from the contraction costs it about 0.034 ms at the bench shape (H100 80GB HBM3, 700 W); the value is the one
+// scripts/step_phases.py --free-sms picked (README, "Resident step by phase").  -DDMO_GP_LANE_SMS=F builds another.
+#ifndef DMO_GP_LANE_SMS
+#define DMO_GP_LANE_SMS 14
+#endif
+constexpr int GP_LANE_SMS = DMO_GP_LANE_SMS;
 // A caller that runs its own work beside the variance contraction (the fused step's lane, step.cu) passes this to the
 // tensor route: mean_ready is recorded on the stream once the last chunk's mean is written, and the contraction runs on
-// the context's high-priority stream (joined back before var_finish_tc_kernel); the caller's work has the SMs the
-// contraction's grid leaves free.  The caller creates those streams first (dmo_lane_streams).
+// the context's high-priority stream (joined back before var_finish_tc_kernel) with a grid that leaves at least
+// GP_LANE_SMS SMs to the caller's work.  The caller creates those streams first (dmo_lane_streams).
 struct GpOverlap {
   cudaEvent_t mean_ready = nullptr;
 };

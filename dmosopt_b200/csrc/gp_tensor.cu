@@ -1022,7 +1022,7 @@ static_assert(TMV == GP_TC_TILE, "gp.cuh exports the wgmma candidate tile");
 int gp_tensor_var_planes(int64_t Npad) { return (int)((Npad / TN + 1) / 2); }
 
 int gp_var_contract_tensor(dmo_ctx* ctx, const GpVarOps& ops, const uint16_t* Kh, const uint16_t* Kl, int64_t k_alloc,
-                           int64_t k_rows, int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag) {
+                           int64_t k_rows, int64_t Pcpad, double* vnorm, int64_t vn_ld, int* abort_flag, int free_sms) {
   const int64_t Npad = ops.Npad;
   DMO_REQUIRE(Npad % TN == 0 && Pcpad % TMV == 0, "gp_var_contract_tensor: internal padding error");
   CUtensorMap map_kh, map_kl, map_lh, map_ll;
@@ -1043,9 +1043,10 @@ int gp_var_contract_tensor(dmo_ctx* ctx, const GpVarOps& ops, const uint16_t* Kh
   prm.vn_ld = vn_ld;
   prm.abort_flag = abort_flag;
   // static round-robin: the makespan is ceil(n_work / grid) items, so the smallest grid with that many items per CTA
-  // finishes with it and leaves the other SMs free (at the bench shape 4096 items take 128 CTAs, not 132)
+  // finishes with it and leaves the other SMs free (at the bench shape 4096 items take 128 CTAs, not 132).  free_sms > 0
+  // caps the grid at sm_count - free_sms CTAs' worth of items per CTA (4096 items on 118 CTAs for 14 free SMs)
   const int n_work = prm.M * prm.n_pb * prm.n_q;
-  const int per_cta = (int)ceil_div(n_work, ctx->sm_count);
+  const int per_cta = (int)ceil_div(n_work, ctx->sm_count - free_sms > 1 ? ctx->sm_count - free_sms : 1);
   const int grid = (int)ceil_div(n_work, per_cta);
   DMO_LAUNCH(gp_var_wgmma_kernel, grid, NTHREADS, GEMM_SMEM, map_kh, map_kl, map_lh, map_ll, prm);
   return DMO_OK;
@@ -1177,7 +1178,8 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
           DMO_CUDA(cudaStreamWaitEvent(ctx->gp_hi, ctx->lane_ev[1], 0));
           ctx->stream = ctx->gp_hi;
         }
-        const int rc = gp_var_contract_tensor(ctx, gp->ops, Kh.p, Kl.p, G * Pc_alloc, Pc_alloc, Pcpad, vnorm.p, Pc_alloc, abort_flag);
+        const int rc = gp_var_contract_tensor(ctx, gp->ops, Kh.p, Kl.p, G * Pc_alloc, Pc_alloc, Pcpad, vnorm.p, Pc_alloc, abort_flag,
+                                              ov ? GP_LANE_SMS : 0);
         if (ov) {
           ctx->stream = main;
           DMO_CUDA(cudaEventRecord(ctx->lane_ev[2], ctx->gp_hi));

@@ -16,6 +16,7 @@
 //   M = 6 .. 8: the identity with non-dominated limit sets at every level (hv_many.cu).
 // All arithmetic is float64; block partial sums are combined in a fixed order (deterministic result).
 #include <stdlib.h>
+#include <string.h>
 
 #include "common.cuh"
 
@@ -480,6 +481,24 @@ __global__ void dominated_flag_kernel(const int32_t* __restrict__ keep, int64_t 
   if (i < n) out[i] = keep[i] ? 0 : 1;
 }
 
+// M = 3, small fronts: one O(n) sweep per point (n^2 / 2 cheap tests, no set-up); large fronts: the merge-sort-tree walks
+// of hv3_tree.cu (O(n log^2 n)).  DMO_HV3_TREE = 0 / 1 forces one or the other, any larger value moves the threshold.
+int64_t hv3_tree_min() {
+  if (const char* e = getenv("DMO_HV3_TREE")) {
+    const long v = atol(e);
+    return v == 0 ? INT64_MAX : (v == 1 ? 0 : v);
+  }
+  return 4096;
+}
+
+// rows [*count, n) of the row-major (n, M) F := ref
+__global__ void pad_rows_kernel(double* __restrict__ F, int64_t n, int M, const int32_t* __restrict__ count,
+                                const double* __restrict__ ref) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= *count && i < n)
+    for (int j = 0; j < M; ++j) F[i * M + j] = ref[j];
+}
+
 int sum_partials(dmo_ctx* ctx, DevBuf<double>& partial, int64_t nb, double* h_out) {
   DevBuf<double> res;
   DMO_TRY(res.alloc(ctx, 1));
@@ -657,14 +676,7 @@ int hypervolume_device_ranked(dmo_ctx* ctx, const double* dF, int64_t n, int M, 
   int64_t nb = ceil_div(n2, HV_T);
   DevBuf<double> partial;
   DMO_TRY(partial.alloc(ctx, nb));
-  // small fronts: one O(n) sweep per point (n^2 / 2 cheap tests, no set-up); large fronts: the merge-sort-tree walks of
-  // hv3_tree.cu (O(n log^2 n)).  DMO_HV3_TREE = 0 / 1 forces one or the other, any larger value moves the threshold.
-  int64_t tree_min = 4096;
-  if (const char* e = getenv("DMO_HV3_TREE")) {
-    const long v = atol(e);
-    tree_min = v == 0 ? INT64_MAX : (v == 1 ? 0 : v);
-  }
-  if (n2 >= tree_min) {
+  if (n2 >= hv3_tree_min()) {
     DMO_TRY(hv3_tree_device(ctx, xs.p, ys.p, zs.p, zo.p, n2, h_ref[0], h_ref[1], h_ref[2], partial.p, &nb));
   } else {
     ProfileScope ps(ctx, "hv3");
@@ -672,6 +684,79 @@ int hypervolume_device_ranked(dmo_ctx* ctx, const double* dF, int64_t n, int M, 
   }
   DMO_TRY(sum_partials(ctx, partial, nb, h_out));
   return DMO_OK;
+}
+
+// The M = 3 route of hypervolume_device_ranked for the fused step's lane (step.cu): hv3_ranked_enqueue issues no host
+// read, so a caller can enqueue it beside other work and drop it unread.  The n1 rows it keeps (rank 0, strictly inside
+// ref) are compacted into n rows and rows n1 .. n-1 are set to ref itself, which is greater than every kept row on every
+// axis: the stable column sorts put those rows last, so the first n1 entries of the sorted orders, the z-order ids and
+// the gathered coordinates are exactly those of the n1-row route.  A padding row adds no volume (its staircase is
+// already below it and its z slab is empty), and in the tree it is never a drop for a kept row (its z-order id is >= n1);
+// the walk over n rows therefore finds the same drops as the walk over n1, and blocks past n1 add exact zeros to the
+// fixed-order final sum.  The tree is built and walked on the lane when n reaches the tree threshold; hv3_ranked_finish
+// reads n1 (the route, as the n1-row route does) and then the tree's volume, or runs the sweep on the first n1 entries
+// when n1 is below the threshold.  The volume has the bits of hypervolume_device_ranked's (tests/test_gpu_steps_hv_lane.py).
+int hv3_ranked_enqueue(dmo_ctx* ctx, const double* dF, int64_t n, const double* h_ref, const int32_t* d_rank, Hv3Ranked& s) {
+  s.n = n;
+  memcpy(s.ref, h_ref, sizeof(s.ref));
+  s.tree = n >= hv3_tree_min();
+  DevBuf<double> dref, Fin;
+  DevBuf<int32_t> flag;
+  DevBuf<uint32_t> sx, sz, zinv;
+  DMO_TRY(dref.alloc(ctx, 3));
+  DMO_CUDA(cudaMemcpyAsync(dref.p, h_ref, 3 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  DMO_TRY(flag.alloc(ctx, n + 1));
+  DMO_TRY(s.pos.alloc(ctx, n + 1));
+  DMO_TRY(Fin.alloc(ctx, (size_t)n * 3));
+  const unsigned g = (unsigned)ceil_div(n, 256);
+  DMO_LAUNCH(inside_flag_kernel, (unsigned)ceil_div(n + 1, 256), 256, 0, dF, n, 3, dref.p, d_rank, flag.p);
+  DMO_TRY(prim_exclusive_sum_i32(ctx, flag.p, s.pos.p, n + 1));
+  DMO_LAUNCH(compact_rows_kernel, g, 256, 0, dF, n, 3, flag.p, s.pos.p, Fin.p);
+  DMO_LAUNCH(pad_rows_kernel, g, 256, 0, Fin.p, n, 3, s.pos.p + n, dref.p);
+  DMO_TRY(prim_sort_by_column(ctx, Fin.p, n, 3, 0, sx));
+  DMO_TRY(prim_sort_by_column(ctx, Fin.p, n, 3, 2, sz));
+  DMO_TRY(zinv.alloc(ctx, n));
+  DMO_TRY(s.zo.alloc(ctx, n));
+  DMO_TRY(s.xs.alloc(ctx, n));
+  DMO_TRY(s.ys.alloc(ctx, n));
+  DMO_TRY(s.zs.alloc(ctx, n));
+  DMO_LAUNCH(invert_perm_kernel, g, 256, 0, sz.p, n, zinv.p);
+  DMO_TRY(prim_gather_u32(ctx, zinv.p, sx.p, n, s.zo.p));
+  DMO_LAUNCH(gather_col_kernel, g, 256, 0, Fin.p, sx.p, n, 3, 0, s.xs.p);
+  DMO_LAUNCH(gather_col_kernel, g, 256, 0, Fin.p, sx.p, n, 3, 1, s.ys.p);
+  DMO_LAUNCH(gather_col_kernel, g, 256, 0, Fin.p, sx.p, n, 3, 2, s.zs.p);
+  if (s.tree) {
+    DevBuf<double> partial;
+    int64_t nb = ceil_div(n, HV_T);
+    DMO_TRY(partial.alloc(ctx, nb));
+    DMO_TRY(hv3_tree_device(ctx, s.xs.p, s.ys.p, s.zs.p, s.zo.p, n, h_ref[0], h_ref[1], h_ref[2], partial.p, &nb));
+    DMO_TRY(s.res.alloc(ctx, 1));
+    DMO_LAUNCH(final_sum_kernel, 1, 256, 0, partial.p, nb, s.res.p);
+  }
+  DMO_CHECK_LAUNCH();
+  return DMO_OK;
+}
+
+int hv3_ranked_finish(dmo_ctx* ctx, Hv3Ranked& s, double* h_out) {
+  *h_out = 0.0;
+  int32_t n1 = 0;
+  DMO_CUDA(cudaMemcpyAsync(&n1, s.pos.p + s.n, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
+  if (n1 == 0) return DMO_OK;
+  if (s.tree && n1 >= hv3_tree_min()) {
+    DMO_CUDA(cudaMemcpyAsync(h_out, s.res.p, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    DMO_CUDA(dmo_wait(ctx));
+    return DMO_OK;
+  }
+  const int64_t nb = ceil_div(n1, HV_T);
+  DevBuf<double> partial;
+  DMO_TRY(partial.alloc(ctx, nb));
+  {
+    ProfileScope ps(ctx, "hv3");
+    DMO_LAUNCH(hv3_kernel, (unsigned)nb, HV_T, 0, s.xs.p, s.ys.p, s.zs.p, s.zo.p, (int64_t)n1, s.ref[0], s.ref[1], s.ref[2],
+               partial.p);
+  }
+  return sum_partials(ctx, partial, nb, h_out);
 }
 
 extern "C" {

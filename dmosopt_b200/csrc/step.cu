@@ -8,8 +8,8 @@
 // It is a composition of the device bodies of this library's entry points, without their trailing waits.  The host waits
 // only for values it needs: the offspring count (it sizes the GP launch), one read-back after the GP (watchdog and rows to
 // refine, read once the truncation is enqueued behind it), the rank's (the peel probe and one count per peeled front, mostly read while the next front is peeled; or the
-// chain's watchdog) and the hypervolume's (its route and its value).  The truncation runs beside the GP's variance
-// contraction, on a stream of its own (below).  bench.py's `value` leg is this call; scripts/step_phases.py times its
+// chain's watchdog) and the hypervolume's (its route and its value).  The truncation and the hypervolume run beside the
+// GP's variance contraction, on a stream of its own (below).  bench.py's `value` leg is this call; scripts/step_phases.py times its
 // phases (the step_* profile scopes) and counts the waits.
 // dmo_nsga2_step_record runs the same body for MOASMO.optimize's resident epoch (dmosopt_b200/MOASMO.py): the mean only,
 // optionally a feasibility rank as the truncation's last key, and the generation's offspring, their mean and operator
@@ -17,6 +17,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 
 #include "common.cuh"
 #include "gp.cuh"
@@ -128,14 +129,26 @@ static int nsga2_step_body(dmo_ctx* ctx, dmo_gp* gp, const dmo_feas* key, double
     DMO_TRY(feas_rank_device(ctx, key, Xs.p, P + pop, kx.p));
     kp[0] = kx.p;
   }
-  // The GP's read-back is left pending and the truncation is enqueued before the host waits for it.  The truncation needs
-  // the posterior mean only, which the tensor route writes before its variance contraction: when the GP defers its
-  // read-back, the truncation runs on the context's lane stream from that point on, beside the contraction, which runs on
-  // a higher-priority stream on the SMs its grid leaves free.  Otherwise (float64 or tensor precision, a linear mean, a
-  // non-tensor AUTO route) the GP has finished inside the call and the truncation follows it on the main stream.  Either
-  // way its host waits (peel probe, peel counts) wait for its own stream only.  If the GP then fails, the population is
-  // put back (the parents are still in Xs / Ys); if AUTO refines rows, the truncation runs again on them.  Every buffer
-  // the two streams share is allocated on the main stream before the fork and released after the join.
+  // The GP's read-back is left pending and the truncation is enqueued before the host waits for it.  The truncation and
+  // the hypervolume of its survivors need the posterior mean only, which the tensor route writes before its variance
+  // contraction: when the GP defers its read-back, both run on the context's lane stream from that point on, beside the
+  // contraction, which runs on a higher-priority stream on the SMs its grid leaves free.  Otherwise (float64 or tensor
+  // precision, a linear mean, a non-tensor AUTO route) the GP has finished inside the call and both follow it on the
+  // main stream.  Either way the truncation's host waits (peel probe, peel counts) wait for its own stream only, and the
+  // hypervolume's reads come after the GP's read-back.  If the GP then fails, the population is put back (the parents are
+  // still in Xs / Ys) and hv_out is left alone; if AUTO refines rows, the truncation and the hypervolume run again on
+  // them.  Every buffer the two streams share is allocated on the main stream before the fork and released after the join.
+  // The hypervolume's reference point is staged before the fork, so that the lane can use it.
+  const bool want_hv = hv_ref && hv_out;
+  double h_ref[16] = {};
+  if (want_hv && M <= 16) {
+    if (dmo_is_device_ptr(hv_ref)) {
+      ctx->waits++;  // a copy into pageable host memory returns once it has landed
+      DMO_CUDA(cudaMemcpyAsync(h_ref, hv_ref, M * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    } else {
+      memcpy(h_ref, hv_ref, M * sizeof(double));
+    }
+  }
   GpPending gpp;
   DevBuf<int32_t> rank_in;  // the ranks before the truncation, for the failure path
   if (P > 0) {
@@ -156,21 +169,43 @@ static int nsga2_step_body(dmo_ctx* ctx, dmo_gp* gp, const dmo_feas* key, double
     if (gpp.active) DMO_CUDA(cudaMemcpyAsync(rank_in.p, rank, (size_t)pop * sizeof(int32_t), cudaMemcpyDeviceToDevice, ctx->stream));
     return truncate();
   };
+  // the survivors carry their ranks within the merged set: rows of rank > 0 cannot add volume (hv.cu)
+  auto hypervolume = [&](double* h) -> int {
+    ProfileScope ps(ctx, "step_hv");
+    return hypervolume_device_ranked(ctx, pop_y, pop, M, h_ref, rank, h);
+  };
+  // With three objectives and a finite reference point the lane also enqueues the device work of the hypervolume, which
+  // has no host read (hv3_ranked_enqueue); its reads and the volume follow gp_predict_finish, unless the GP fails (the
+  // population is put back, hv_out is left alone) or refines rows (the lane's work is dropped unread, and the truncation
+  // and the hypervolume run again).  So the step's host waits are the serial composition's whether or not AUTO refines.
+  // The other routes read counts back from the device before their last kernels, and run after the join.
+  Hv3Ranked hv_lane;
+  const bool hv_on_lane = want_hv && M == 3 && std::isfinite(h_ref[0]) && std::isfinite(h_ref[1]) && std::isfinite(h_ref[2]);
+  bool hv_enqueued = false;
   if (gpp.active && gpp.ov.mean_ready) {
     // The lane reads Xs, Ys (the mean rows and the parents) and writes pop_x, pop_y, rank, rank_in and its own scratch; the
     // GP's work after the fork point writes the variance and its own scratch only.  The lane may run on a few SMs while
-    // the contraction holds the rest, so nothing in it may need all of its CTAs resident at once.  Every kernel
-    // remove_worst_device reaches (metric none, crowding or euclidean) was checked for that: the dense-id, lexicographic,
-    // cell and key radix sorts are CUB's (onesweep passes take their tile from an atomic counter and look back only at
-    // tiles taken before; small sorts run as one tile, or as separate upsweep / scan / downsweep kernels); CUB's scans
-    // look back only at lower block indices, which are dispatched first; the peel probe
+    // the contraction holds the rest (it leaves GP_LANE_SMS free), so nothing in it may need all of its CTAs resident at
+    // once.  Every kernel remove_worst_device reaches (metric none, crowding or euclidean) was checked for that: the
+    // dense-id, lexicographic, cell and key radix sorts are CUB's (onesweep passes take their tile from an atomic counter
+    // and look back only at tiles taken before; small sorts run as one tile, or as separate upsweep / scan / downsweep
+    // kernels); CUB's scans look back only at lower block indices, which are dispatched first; the peel probe
     // is a grid-stride loop with atomicOr; the chain kernel (rank.cu) takes its blocks from an atomic ticket and waits
     // only for blocks taken before; everything else (keys, gathers, cell grid, prefix minima, peel marks, column min / max,
     // crowding, euclidean, round_f32) is one pass per element or per block, with atomics at most, and no grid-wide barrier.
+    // So was every kernel hv3_ranked_enqueue reaches: the column sorts (prim_sort_by_column) and the compaction scan are
+    // the CUB sorts and scans above; the inside / rank-0 flags, compaction, padding, inverse permutation and gathers, and
+    // the tree's y_by_t, build_low, per-level build_high and carry kernels and its walks (hv3_tree.cu) are one pass per
+    // element or per block, each block reading only what earlier launches wrote; final_sum_kernel is a single block.
     cudaStream_t main = ctx->stream;
     DMO_CUDA(cudaStreamWaitEvent(ctx->lane, gpp.ov.mean_ready, 0));
     ctx->stream = ctx->lane;
-    const int rc = first_truncate();
+    int rc = first_truncate();
+    if (rc == DMO_OK && hv_on_lane) {
+      ProfileScope ps(ctx, "step_hv");
+      rc = hv3_ranked_enqueue(ctx, pop_y, pop, h_ref, rank, hv_lane);
+      hv_enqueued = rc == DMO_OK;
+    }
     ctx->stream = main;
     // joined before gp_predict_finish: its refinement, the failure path and the second truncation come after the lane
     DMO_CUDA(cudaEventRecord(ctx->lane_ev[3], ctx->lane));
@@ -188,7 +223,10 @@ static int nsga2_step_body(dmo_ctx* ctx, dmo_gp* gp, const dmo_feas* key, double
     DMO_CUDA(dmo_wait(ctx));
     return rc;
   }
-  if (refined) DMO_TRY(truncate());
+  if (refined) {
+    DMO_TRY(truncate());
+    hv_enqueued = false;
+  }
   if (x_gen) {
     ProfileScope ps(ctx, "step_record");
     DevBuf<unsigned long long> cnt;
@@ -202,18 +240,16 @@ static int nsga2_step_body(dmo_ctx* ctx, dmo_gp* gp, const dmo_feas* key, double
     DMO_TRY(copy_out(ctx, y_gen, Ys.p, (size_t)P * M * sizeof(double)));
     DMO_TRY(copy_out(ctx, counts, cnt.p, 4 * sizeof(int64_t)));
   }
-  if (hv_ref && hv_out) {
-    ProfileScope ps(ctx, "step_hv");
-    // the survivors carry their ranks within the merged set: rows of rank > 0 cannot add volume (hv.cu)
-    DMO_REQUIRE(M <= 16, "nsga2_step: too many objectives for the hypervolume");
-    double h_ref[16];
-    if (dmo_is_device_ptr(hv_ref)) {
-      ctx->waits++;  // a copy into pageable host memory returns once it has landed: behind the truncation
-      DMO_CUDA(cudaMemcpyAsync(h_ref, hv_ref, M * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    } else {
-      memcpy(h_ref, hv_ref, M * sizeof(double));
+  if (want_hv) {
+    if (hv_enqueued) {
+      ProfileScope ps(ctx, "step_hv");
+      double h = 0.0;
+      DMO_TRY(hv3_ranked_finish(ctx, hv_lane, &h));
+      *hv_out = h;
+      return DMO_OK;
     }
-    DMO_TRY(hypervolume_device_ranked(ctx, pop_y, pop, M, h_ref, rank, hv_out));
+    DMO_REQUIRE(M <= 16, "nsga2_step: too many objectives for the hypervolume");
+    DMO_TRY(hypervolume(hv_out));
   }
   return DMO_OK;
 }

@@ -7,10 +7,14 @@ clock; host waits and kernel launches per generation), then --steps generations 
 CUDA-event timers on, and prints per generation:
   * device-timer ms of each phase (step_tournament, step_generate, step_gp, step_truncate, step_hv) and of the kernels
     inside them that have scopes of their own (gp_kstar, gp_var, rank_peel, ...);
-  * beside the contraction: the lane's wall time (step_truncate) against the contraction's window (gp_var), both from the
-    point the mean is written, and the slack between them (positive: the lane finished inside the window);
+  * beside the contraction: the lane's time (step_truncate + step_hv) against the contraction's window (gp_var), both from
+    the point the mean is written, and the slack between them (positive: the lane finished inside the window);
   * the card's name, its power limit and the median SM clock sampled during the timed window.
-Usage: python scripts/step_phases.py [--steps 100] [--warmup 20] [--rounds 1] [--json OUT.json]
+--free-sms F1,F2,... sweeps the SMs the overlapped contraction leaves to the lane (GP_LANE_SMS, gp.cuh): it builds one
+library per value into a temporary directory (gp_tensor.cu, the one source that reads the constant, compiled with
+-DDMO_GP_LANE_SMS=F and linked with the tree's other objects) and measures each in a process of its own, the values
+alternating within every round.
+Usage: python scripts/step_phases.py [--steps 100] [--warmup 20] [--rounds 1] [--free-sms 4,11,14,18] [--json OUT.json]
 """
 
 import argparse
@@ -18,6 +22,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import time
 
 import numpy as np
@@ -72,8 +77,57 @@ def measure(L, bench, rs, steps, warmup):
     ph = out["phases_ms"]
     out["outside_gp_ms"] = out["step_ms_device"] - ph.get("step_gp", 0.0)
     if "gp_var" in out["scopes_ms"] and "step_truncate" in ph:
-        out["lane_slack_ms"] = out["scopes_ms"]["gp_var"] - ph["step_truncate"]
+        out["lane_ms"] = ph["step_truncate"] + ph.get("step_hv", 0.0)
+        out["lane_slack_ms"] = out["scopes_ms"]["gp_var"] - out["lane_ms"]
     return out
+
+
+def build_free_sms(values, out_dir):
+    """One library per GP_LANE_SMS value: gp_tensor.cu compiled with -DDMO_GP_LANE_SMS=F, the tree's other objects."""
+    from dmosopt_b200 import build as b
+
+    b.build(verbose=False)
+    others = [os.path.join(b.OBJ, s.replace(".cu", ".o")) for s in b.SOURCES if s != "gp_tensor.cu"]
+    libs = {}
+    for f in values:
+        obj = os.path.join(out_dir, f"gp_tensor_{f}.o")
+        lib = os.path.join(out_dir, f"libdmosopt_b200_free{f}.so")
+        subprocess.run([b._nvcc()] + [x for x in b.NVCC_FLAGS if x not in ("-Xptxas", "-v")] + [f"-DDMO_GP_LANE_SMS={f}", "-c",
+                       os.path.join(b.CSRC, "gp_tensor.cu"), "-o", obj], check=True)
+        subprocess.run([b._nvcc(), "-shared", "-o", lib, obj] + others + ["-gencode", "arch=compute_90a,code=sm_90a"], check=True)
+        libs[f] = lib
+    return libs
+
+
+def sweep(args):
+    values = [int(v) for v in args.free_sms.split(",")]
+    rows = []
+    with tempfile.TemporaryDirectory(prefix="dmo_free_sms_") as tmp:
+        libs = build_free_sms(values, tmp)
+        for rnd in range(args.rounds):
+            for f in values:
+                js = os.path.join(tmp, f"r{rnd}_f{f}.json")
+                cmd = [sys.executable, os.path.abspath(__file__), "--lib", libs[f], "--json", js] + [
+                    f"--{k}={getattr(args, k)}" for k in ("steps", "warmup", "pop", "dim", "obj", "ntrain", "seed")]
+                subprocess.run(cmd, check=True, stdout=sys.stderr)
+                with open(js) as fh:
+                    res = json.load(fh)
+                r = res["rounds"][0]
+                rows.append({**r, "free_sms": f, "round": rnd, "card": res["card"], "power_limit_w": res["power_limit_w"]})
+    print(f"\n{rows[0]['card']}, power limit {rows[0]['power_limit_w']} W, pop {args.pop}, dim {args.dim}, {args.obj} objectives, "
+          f"N_train {args.ntrain}, {args.steps} generations")
+    print(f"{'free SMs':>9}{'round':>6}{'step ms':>10}{'gp_var':>9}{'truncate':>9}{'hv':>8}{'slack':>9}{'SM MHz':>9}")
+    for r in rows:
+        ph, sc = r["phases_ms"], r["scopes_ms"]
+        slack = r.get("lane_slack_ms")
+        print(f"{r['free_sms']:>9}{r['round']:>6}{r['step_ms_device']:>10.3f}{sc.get('gp_var', float('nan')):>9.3f}"
+              f"{ph.get('step_truncate', float('nan')):>9.3f}{ph.get('step_hv', float('nan')):>8.3f}"
+              f"{(f'{slack:+.3f}' if slack is not None else '-'):>9}{(r['sm_mhz_median'] or float('nan')):>9.0f}")
+    summary = {"steps": args.steps, "pop": args.pop, "dim": args.dim, "obj": args.obj, "ntrain": args.ntrain, "sweep": rows}
+    print(json.dumps(summary), flush=True)
+    if args.json:
+        with open(args.json, "w") as f:
+            json.dump(summary, f, indent=1)
 
 
 def main():
@@ -87,12 +141,18 @@ def main():
     ap.add_argument("--ntrain", type=int, default=4096)
     ap.add_argument("--seed", type=int, default=1234)
     ap.add_argument("--json", default=None, help="also write the result to this file")
+    ap.add_argument("--free-sms", default=None, help="comma-separated GP_LANE_SMS values to sweep, one library each")
+    ap.add_argument("--lib", default=None, help=argparse.SUPPRESS)  # the library a --free-sms child measures
     args = ap.parse_args()
+    if args.free_sms:
+        return sweep(args)
 
     import bench
     import dmosopt_b200 as b2
     from dmosopt_b200 import _lib as L
 
+    if args.lib:
+        L.load_library(args.lib)
     L.context(0)
     pop, d, M, N = args.pop, args.dim, args.obj, args.ntrain
     w = bench.workload(pop, d, M, N)
@@ -124,18 +184,18 @@ def main():
         print(f"{'step (host)':<18}{out['step_ms_host']:>16.3f}")
         print(f"{'outside step_gp':<18}{out['outside_gp_ms']:>16.3f}")
         if "lane_slack_ms" in out:
-            print(f"lane {ph['step_truncate']:.3f} ms against the contraction's window {sc['gp_var']:.3f} ms: "
-                  f"slack {out['lane_slack_ms']:+.3f} ms")
+            print(f"lane {out['lane_ms']:.3f} ms (truncation {ph['step_truncate']:.3f}, hypervolume {ph.get('step_hv', 0.0):.3f}) "
+                  f"against the contraction's window {sc['gp_var']:.3f} ms: slack {out['lane_slack_ms']:+.3f} ms")
         print(f"host waits / generation {out['waits_per_step']:.2f}, launches / generation {out['launches_per_step']:.1f}", flush=True)
 
     print(f"\n{name}, power limit {plimit} W, pop {pop}, dim {d}, {M} objectives, N_train {N}")
-    print(f"{'round':>6}{'step ms':>10}{'gp_var':>9}{'lane':>9}{'slack':>9}{'SM MHz':>9}")
+    print(f"{'round':>6}{'step ms':>10}{'gp_var':>9}{'truncate':>9}{'hv':>8}{'slack':>9}{'SM MHz':>9}")
     for r in results:
         ph, sc = r["phases_ms"], r["scopes_ms"]
         slack = r.get("lane_slack_ms")
         print(f"{r['round']:>6}{r['step_ms_device']:>10.3f}{sc.get('gp_var', float('nan')):>9.3f}"
-              f"{ph.get('step_truncate', float('nan')):>9.3f}{(f'{slack:+.3f}' if slack is not None else '-'):>9}"
-              f"{(r['sm_mhz_median'] or float('nan')):>9.0f}")
+              f"{ph.get('step_truncate', float('nan')):>9.3f}{ph.get('step_hv', float('nan')):>8.3f}"
+              f"{(f'{slack:+.3f}' if slack is not None else '-'):>9}{(r['sm_mhz_median'] or float('nan')):>9.0f}")
     summary = {"card": name, "power_limit_w": plimit, "steps": args.steps, "pop": pop, "dim": d, "obj": M, "ntrain": N,
                "rounds": results}
     print(json.dumps(summary), flush=True)
