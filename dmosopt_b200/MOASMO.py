@@ -2,8 +2,10 @@
 
   * ``optimize``           MOASMO.py:21-131, the surrogate epoch: a drop-in with the same signature and generator
                            protocol.  An eligible epoch (``resident_eligible``) keeps the population in HBM and runs
-                           each generation as one ``dmo_nsga2_step_record`` call; any other runs the reference's
-                           per-generation plugin loop (``optimize_per_generation``).  Both return the same results.
+                           each generation as one ``dmo_nsga2_step_record`` call (GPR_Matern, GPR_RBF) or one
+                           ``dmo_nsga2_step_record_posterior`` call (EGP, the variational and the deep-GP surrogates); any
+                           other runs the reference's per-generation plugin loop (``optimize_per_generation``).  Both
+                           return the same results.
   * ``epsilon_get_best``   MOASMO.py:703-758 -> MOEA.get_duplicates (dmo_get_duplicates) + dmo_epsilon_sort
 """
 
@@ -29,16 +31,30 @@ def _datatypes():
     return OptHistory, EpochResults
 
 
+def _posterior_types():
+    """The surrogate types whose epochs step on ``dmo_nsga2_step_record_posterior`` (by exact type)."""
+    from .model_gpflow import CRV_Matern, SIV_Matern, SPV_Matern, SVGP_Matern, VGP_Matern
+    from .model_gpytorch import EGP_Matern, MDGP_Matern, MDSPP_Matern
+
+    return (EGP_Matern, SVGP_Matern, VGP_Matern, SIV_Matern, SPV_Matern, CRV_Matern, MDSPP_Matern, MDGP_Matern)
+
+
 def resident_eligible(optimizer, model, optimize_mean_variance=False):
     """True when ``optimize`` runs this epoch on the resident generation step: the optimizer is exactly
-    ``dmosopt_b200.NSGA2``, the surrogate exactly ``GPR_Matern`` or ``GPR_RBF`` returning the mean only, no mean-variance
-    objectives, no adaptive population size, a y-metric of None, "crowding" or "euclidean", and an x-metric of None or
-    the rank of a GPU ``LogisticFeasibilityModel``."""
+    ``dmosopt_b200.NSGA2``, the surrogate exactly ``GPR_Matern``, ``GPR_RBF``, ``EGP_Matern``, one of the five
+    variational classes or one of the two deep GPs, with its device posterior and returning the mean only, no
+    mean-variance objectives, no adaptive population size, a y-metric of None, "crowding" or "euclidean", and an x-metric
+    of None or the rank of a GPU ``LogisticFeasibilityModel``."""
     from .model import GPR_Matern, GPR_RBF
     from .NSGA2 import NSGA2, _device_feasibility_key
 
     sm = getattr(model, "objective", None)
-    if type(optimizer) is not NSGA2 or type(sm) not in (GPR_Matern, GPR_RBF) or getattr(sm, "_gp", None) is None:
+    if type(optimizer) is not NSGA2:
+        return False
+    if type(sm) in (GPR_Matern, GPR_RBF):
+        if getattr(sm, "_gp", None) is None:
+            return False
+    elif type(sm) not in _posterior_types() or sm.resident_posterior()[1] is None:
         return False
     if optimize_mean_variance or optimizer.optimize_mean_variance or sm.return_mean_variance:
         return False
@@ -65,7 +81,8 @@ def optimize(num_generations, optimizer, model, nInput, nOutput, xlb, xub, popsi
     """dmosopt.MOASMO.optimize (MOASMO.py:21-131): a generator that returns the EpochResults through StopIteration.
 
     Eligible epochs (``resident_eligible``) never yield: the host steps before the loop are the reference's, then each
-    generation is one ``dmo_nsga2_step_record`` call on the population kept in HBM, with the same Philox streams,
+    generation is one ``dmo_nsga2_step_record`` (or, for EGP, the variational and the deep-GP surrogates,
+    ``dmo_nsga2_step_record_posterior``) call on the population kept in HBM, with the same Philox streams,
     results and optimizer state as the per-generation loop.  The host waits only for the offspring count of each
     generation; with ``termination`` it also reads the population back before every ``has_terminated``, and with
     ``adaptive_operator_rates`` the operator counts before every ``update_operator_rates``.  The offspring and their
@@ -184,7 +201,11 @@ def _resident_generations(num_generations, optimizer, model, termination, logger
     rows are views of the page-locked record) and leaves the optimizer's state as the per-generation loop leaves it."""
     from .NSGA2 import _device_feasibility_key
 
+    from .model import GPR_Matern, GPR_RBF
+
     p, st, sm = optimizer.opt_params, optimizer.state, model.objective
+    # (kind, handle, precision, mean dtype) of the surrogates that step on dmo_nsga2_step_record_posterior
+    post = None if type(sm) in (GPR_Matern, GPR_RBF) else sm.resident_posterior()
     pop, d = st.population_parm.shape
     M = st.population_obj.shape[1]
     key = _device_feasibility_key(optimizer.x_distance_metrics)
@@ -240,8 +261,16 @@ def _resident_generations(num_generations, optimizer, model, termination, logger
         stream = optimizer._next_stream()  # the tournament's stream; the variation takes the next one
         optimizer._next_stream()
         x_gen, y_gen, counts = hist.next()
-        P = _lib.nsga2_step_record(sm._gp, dev_x, dev_y, dev_r, p.crossover_prob, p.mutation_prob, p.mutation_rate, p.di_crossover,
-                                   p.di_mutation, xlb, xub, seed, stream, sm.precision, metric, round_f32, x_gen, y_gen, counts, key=key)
+        if post is None:
+            P = _lib.nsga2_step_record(sm._gp, dev_x, dev_y, dev_r, p.crossover_prob, p.mutation_prob, p.mutation_rate, p.di_crossover,
+                                       p.di_mutation, xlb, xub, seed, stream, sm.precision, metric, round_f32, x_gen, y_gen, counts, key=key)
+        else:
+            kind, handle, precision, mean_dtype = post
+            # a deep GP draws its key as each predict does: MDGP's call counter advances once per generation, in order
+            draw = sm._draw_key() if kind == _lib.POSTERIOR_DGP else (0, 0)
+            P = _lib.nsga2_step_record_posterior(kind, handle, draw, dev_x, dev_y, dev_r, p.crossover_prob, p.mutation_prob, p.mutation_rate,
+                                                 p.di_crossover, p.di_mutation, xlb, xub, seed, stream, precision, metric,
+                                                 mean_dtype == np.float32, round_f32, x_gen, y_gen, counts, key=key)
         pending.append(counts)
         n_eval += P
         done.append((i, x_gen[:P], y_gen[:P]))
@@ -250,6 +279,9 @@ def _resident_generations(num_generations, optimizer, model, termination, logger
             optimizer.update_operator_rates()
     add_counts()
     sync_state()
+    if post is not None and post[3] == np.float32:
+        # evaluate's float32 means (the record holds them exactly); read once the copies have landed (add_counts synchronised)
+        done = [(i, x, y.astype(np.float32)) for i, x, y in done]
     yield from done
 
 

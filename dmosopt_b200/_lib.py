@@ -21,6 +21,7 @@ LIB_PATH = os.path.join(_HERE, "libdmosopt_b200.so")
 METRIC_NONE, METRIC_CROWDING, METRIC_EUCLIDEAN = 0, 1, 2
 KERNEL_MATERN52, KERNEL_RBF = 0, 1
 GP_FP64, GP_TENSOR, GP_AUTO = 0, 1, 2
+POSTERIOR_GP, POSTERIOR_SVGP, POSTERIOR_DGP = 0, 1, 2  # dmo_nsga2_step_record_posterior: dmo_gp, dmo_svgp, dmo_dgp
 GP_PREDICT_MAX_D = 64  # input dimensions of dmo_gp_create (csrc/gp.cu KS_DMAX) and of every tensor-core predict
 GP_PREDICT_MAX_M = 16  # objectives of dmo_gp_create (csrc/gp.cu GP_MAX_M)
 HV_MAX_OBJECTIVES = 8  # dmo_hypervolume: exact, chain sums for M <= 5 (csrc/hv.cu), limit-set recursion for 6 .. 8 (csrc/hv_many.cu)
@@ -110,6 +111,9 @@ _SIGNATURES = {
                                 _c_int, _c_int, _c_int, _c_int, _vp, _vp, _vp]),
     "dmo_nsga2_step_record": (_c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_i64, _c_int, _c_int, _c_dbl, _c_dbl, _c_dbl, _vp, _vp, _vp, _vp,
                                        _c_u64, _c_u64, _c_int, _c_int, _c_int, _vp, _vp, _vp, _vp]),
+    "dmo_nsga2_step_record_posterior": (_c_int, [_vp, _c_int, _vp, _c_u64, _c_u64, _vp, _vp, _vp, _vp, _c_i64, _c_int, _c_int, _c_dbl, _c_dbl,
+                                                 _c_dbl, _vp, _vp, _vp, _vp, _c_u64, _c_u64, _c_int, _c_int, _c_int, _c_int, _vp, _vp, _vp,
+                                                 _vp]),
     "dmo_hypervolume": (_c_int, [_vp, _vp, _c_i64, _c_int, _vp, ctypes.POINTER(_c_dbl)]),
     "dmo_hypervolume_ranked": (_c_int, [_vp, _vp, _c_i64, _c_int, _vp, _vp, ctypes.POINTER(_c_dbl)]),
     "dmo_nondominated_flags": (_c_int, [_vp, _vp, _c_i64, _c_int, _vp]),
@@ -758,14 +762,8 @@ def nsga2_step_record(gp, pop_x, pop_y, rank, crossover_prob, mutation_prob, mut
     float64 and ``counts`` (4,) int64 receive the offspring, their posterior mean and the operator counts; into device or
     page-locked memory they are complete only after ``synchronize()``.  ``key`` (optional FeasModel): its rank of
     [children; parents] is the truncation's last key."""
-    pop, d = int(pop_x.shape[0]), int(pop_x.shape[1])
-    M = int(pop_y.shape[1])
-    for name, a, shape, dt in (("x_gen", x_gen, (pop + 1, d), np.float64), ("y_gen", y_gen, (pop + 1, M), np.float64), ("counts", counts, (4,), np.int64)):
-        if isinstance(a, np.ndarray) and (a.shape != shape or a.dtype != dt or not a.flags.c_contiguous or not a.flags.writeable):
-            raise ValueError(f"nsga2_step_record: {name} must be a writable C-contiguous {np.dtype(dt).name} array of shape {shape}")
-    dic, dim = _per_dim(di_crossover, d), _per_dim(di_mutation, d)
-    lb, ub = _f64(xlb), _f64(xub)
-    nch = np.zeros(1, dtype=np.int64)
+    pop, d, M, dic, dim, lb, ub, nch = _step_record_args("nsga2_step_record", pop_x, pop_y, di_crossover, di_mutation, xlb, xub, x_gen,
+                                                         y_gen, counts)
     _check(
         load_library().dmo_nsga2_step_record(
             context(), gp._h, None if key is None else key._h, _ptr(pop_x), _ptr(pop_y), _ptr(rank), pop, d, M, float(crossover_prob),
@@ -775,6 +773,38 @@ def nsga2_step_record(gp, pop_x, pop_y, rank, crossover_prob, mutation_prob, mut
         "dmo_nsga2_step_record",
     )
     return int(nch[0])
+
+
+def nsga2_step_record_posterior(kind, posterior, draw_key, pop_x, pop_y, rank, crossover_prob, mutation_prob, mutation_rate, di_crossover,
+                                di_mutation, xlb, xub, seed, stream_id, precision, metric, mean_f32, round_to_f32, x_gen, y_gen, counts,
+                                key=None):
+    """``nsga2_step_record`` on another posterior (dmo_nsga2_step_record_posterior): ``kind`` POSTERIOR_GP, _SVGP or _DGP and
+    ``posterior`` the GPHandle, SVGPHandle or DGPHandle.  The offspring's objectives are the mean that handle's predict
+    writes with return_var=True, rounded to float32 first when ``mean_f32``; ``draw_key`` (seed, stream_id) keys a deep
+    GP's Monte Carlo draws.  Returns the offspring count P."""
+    pop, d, M, dic, dim, lb, ub, nch = _step_record_args("nsga2_step_record_posterior", pop_x, pop_y, di_crossover, di_mutation, xlb, xub,
+                                                         x_gen, y_gen, counts)
+    draw_seed, draw_stream = draw_key
+    _check(
+        load_library().dmo_nsga2_step_record_posterior(
+            context(), int(kind), posterior._h, _seed(draw_seed), int(draw_stream), None if key is None else key._h, _ptr(pop_x), _ptr(pop_y),
+            _ptr(rank), pop, d, M, float(crossover_prob), float(mutation_prob), float(mutation_rate), _ptr(dic), _ptr(dim), _ptr(lb), _ptr(ub),
+            _seed(seed), int(stream_id), int(precision), int(metric), 1 if mean_f32 else 0, 1 if round_to_f32 else 0, _ptr(x_gen), _ptr(y_gen),
+            _ptr(counts), _ptr(nch),
+        ),
+        "dmo_nsga2_step_record_posterior",
+    )
+    return int(nch[0])
+
+
+def _step_record_args(who, pop_x, pop_y, di_crossover, di_mutation, xlb, xub, x_gen, y_gen, counts):
+    """(pop, d, M, di_crossover, di_mutation, xlb, xub, n_children buffer) of a recorded step, its host record checked."""
+    pop, d = int(pop_x.shape[0]), int(pop_x.shape[1])
+    M = int(pop_y.shape[1])
+    for name, a, shape, dt in (("x_gen", x_gen, (pop + 1, d), np.float64), ("y_gen", y_gen, (pop + 1, M), np.float64), ("counts", counts, (4,), np.int64)):
+        if isinstance(a, np.ndarray) and (a.shape != shape or a.dtype != dt or not a.flags.c_contiguous or not a.flags.writeable):
+            raise ValueError(f"{who}: {name} must be a writable C-contiguous {np.dtype(dt).name} array of shape {shape}")
+    return pop, d, M, _per_dim(di_crossover, d), _per_dim(di_mutation, d), _f64(xlb), _f64(xub), np.zeros(1, dtype=np.int64)
 
 
 # --------------------------------------------------------------------------- N1: exact-GP fit for given hyper-parameters

@@ -676,7 +676,7 @@ int gp_predict_finish(dmo_ctx* ctx, dmo_gp* gp, GpPending& q, bool* refined) {
 }
 
 int gp_predict_device(dmo_ctx* ctx, dmo_gp* gp, const double* dX, int64_t P, double* d_mean, double* d_var, int precision,
-                      GpPending* pending) {
+                      GpPending* pending, bool var_route_mean) {
   // the read-back is left pending only where nothing of this call comes after the refinement (no linear mean)
   const bool defer = pending && precision == DMO_GP_AUTO && d_var && !gp->has_linear_mean;
   DevBuf<double> own;
@@ -686,7 +686,7 @@ int gp_predict_device(dmo_ctx* ctx, dmo_gp* gp, const double* dX, int64_t P, dou
   if (precision == DMO_GP_FP64) {
     DMO_TRY(gp_predict_fp64(ctx, gp, xn.p, P, d_mean, d_var));
   } else if (precision == DMO_GP_TENSOR) {
-    DMO_TRY(gp_predict_tensor(ctx, gp, xn.p, P, d_mean, d_var));
+    DMO_TRY(gp_predict_tensor(ctx, gp, xn.p, P, d_mean, d_var, nullptr, nullptr, var_route_mean));
   } else if (precision == DMO_GP_AUTO) {
     DMO_TRY(gp_predict_auto(ctx, gp, xn.p, P, d_mean, d_var, defer ? pending : nullptr));
   } else {

@@ -123,9 +123,10 @@ struct GpOverlap {
 };
 // abort_flag null: the call reads the contraction's watchdog back and fails when it tripped.  Otherwise the call zeroes
 // *abort_flag (device) and the watchdog lands there; the caller reads it back and fails the same way (gp_predict_auto folds
-// it into its own read-back).  The mean-only route writes no flag.
+// it into its own read-back).  The mean-only route writes no flag.  var_route_mean (d_var null): the mean is the one a
+// call with d_var writes, bit for bit, without the variance contraction and with no read-back.
 int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var,
-                      int* abort_flag = nullptr, const GpOverlap* ov = nullptr);
+                      int* abort_flag = nullptr, const GpOverlap* ov = nullptr, bool var_route_mean = false);
 extern const char* const GP_WATCHDOG_MSG;
 // An AUTO predict whose one read-back (watchdog, rows to refine) is left pending, so the caller can enqueue work behind it
 // while the GP runs; gp_predict_finish waits for it, fails on a tripped watchdog and refines the rows the check flags
@@ -141,9 +142,11 @@ struct GpPending {
   DevBuf<double> xn;
   DevBuf<int32_t> flag, pos;
 };
-// dmo_gp_predict on device arrays: X (P, d) un-normalised, mean / var (P, M); var may be null
+// dmo_gp_predict on device arrays: X (P, d) un-normalised, mean / var (P, M); var may be null.  var_route_mean (var null,
+// DMO_GP_FP64 or DMO_GP_TENSOR): the mean of dmo_gp_predict with a variance buffer, bit for bit, without its variance
+// (float64: the mean never depends on it; tensor: gp_predict_tensor's var_route_mean).
 int gp_predict_device(dmo_ctx* ctx, dmo_gp* gp, const double* dX, int64_t P, double* d_mean, double* d_var, int precision,
-                      GpPending* pending = nullptr);
+                      GpPending* pending = nullptr, bool var_route_mean = false);
 int gp_predict_finish(dmo_ctx* ctx, dmo_gp* gp, GpPending& pending, bool* refined);
 
 // Candidate chunks and variance scratch of the unit-scale posteriors (MEGP, variational; gp_multitask.cu): one K_* plane
@@ -185,6 +188,17 @@ int sv_flip(dmo_ctx* ctx, const double* C, int64_t n, double s, double* O, int64
 // dmo_svgp_predict before its output mix: the latent moments fm (L,P) and fv (L,P) (fv NULL: means only) of the DEVICE
 // inputs X (P,d), with up checked by the caller (GpUnitPredict::check).  Not synchronised; the caller runs up.watchdog.
 int svgp_latent_moments(dmo_ctx* ctx, dmo_svgp* sv, GpUnitPredict& up, const double* X, int64_t P, double* fm, double* fv);
+// dmo_svgp_predict on DEVICE arrays without its trailing waits: X (P, d), mean / var (P, M), var may be null.  The mean
+// does not depend on whether var is given.  up checked by the caller, which runs up.watchdog.
+int svgp_predict_device(dmo_ctx* ctx, dmo_svgp* sv, GpUnitPredict& up, const double* X, int64_t P, double* mean, double* var);
+// input dimensions and outputs of a variational or deep-GP posterior
+void svgp_dims(const dmo_svgp* sv, int* d, int* M);
+void dgp_dims(const dmo_dgp* g, int* d, int* T);
+// dmo_dgp_predict on DEVICE arrays without its trailing waits (eps / var may be null; the mean does not depend on var:
+// the last layer's mean-only kernel accumulates it in the same order).  up checked by the caller, which runs
+// up.watchdog; stream_id < 2^54 checked by the caller.
+int dgp_predict_device(dmo_ctx* ctx, dmo_dgp* g, GpUnitPredict& up, const double* X, int64_t P, uint64_t seed, uint64_t stream_id,
+                       double* eps, double* mean, double* var);
 // Latent l's device operands, for a caller that forms its own K_*: the operator planes O0 = s Lz^-1 and O1 = s T (rows
 // of Npad, zero padded), the mean vector a_l (Npad,), the scaled inducing points XtT (d, Npad) and 1 / ell (d,).
 struct SvLatentView {

@@ -225,6 +225,43 @@ struct dmo_dgp {
   DevBuf<double> w1, xlb, xrg, sites;
 };
 
+void dgp_dims(const dmo_dgp* g, int* d, int* T) {
+  *d = g->d;
+  *T = g->T;
+}
+
+int dgp_predict_device(dmo_ctx* ctx, dmo_dgp* g, GpUnitPredict& up, const double* X, int64_t P, uint64_t seed, uint64_t stream_id,
+                       double* eps, double* mean, double* var) {
+  const int d = g->d, H = g->H, T = g->T, J = g->J;
+  DevBuf<double> m1, s1;
+  DMO_TRY(m1.alloc(ctx, (size_t)H * P));
+  DMO_TRY(s1.alloc(ctx, (size_t)H * P));
+  {
+    // the hidden layer's variance is not optional: its standard deviation places the last layer's inputs
+    ProfileScope ps(ctx, "dgp_hidden");
+    DMO_TRY(svgp_latent_moments(ctx, g->hidden, up, X, P, m1.p, s1.p));
+    DMO_LAUNCH(dgp_hidden_epilogue_kernel, (unsigned)ceil_div(P, 256), 256, 0, X, P, d, H, g->xlb.p, g->xrg.p, g->w1.p, g->b1,
+               g->jitter, g->min_var, m1.p, s1.p);
+  }
+  {
+    ProfileScope ps(ctx, "dgp_layer2");
+    const int PT = DG_ROWS / J;
+    dim3 grid((unsigned)ceil_div(P, PT), (unsigned)T);
+    const double* sites = g->quadrature ? g->sites.p : nullptr;
+    if (var) {
+      DMO_CUDA(cudaFuncSetAttribute(dgp_layer2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DG_SMEM));
+      DMO_LAUNCH(dgp_layer2_kernel<true>, grid, 256, DG_SMEM, g->tasks, T, P, H, J, PT, g->Z2, g->Npad2, m1.p, s1.p, sites, seed,
+                 stream_id, g->c2, g->min_var, eps, mean, var);
+    } else {
+      DMO_CUDA(cudaFuncSetAttribute(dgp_layer2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DG_SMEM));
+      DMO_LAUNCH(dgp_layer2_kernel<false>, grid, 256, DG_SMEM, g->tasks, T, P, H, J, PT, g->Z2, g->Npad2, m1.p, s1.p, sites, seed,
+                 stream_id, g->c2, g->min_var, eps, mean, nullptr);
+    }
+  }
+  DMO_CHECK_LAUNCH();
+  return DMO_OK;
+}
+
 extern "C" {
 
 int dmo_dgp_destroy(dmo_ctx* ctx, dmo_dgp* g) {
@@ -342,31 +379,7 @@ int dmo_dgp_predict(dmo_ctx* ctx, dmo_dgp* g, const double* X, int64_t P, uint64
   DMO_TRY(om.init(ctx, mean, (size_t)P * T));
   DMO_TRY(ov.init(ctx, var, (size_t)P * T));
   DMO_TRY(oe.init(ctx, eps_out, (size_t)J * P * H));
-  DevBuf<double> m1, s1;
-  DMO_TRY(m1.alloc(ctx, (size_t)H * P));
-  DMO_TRY(s1.alloc(ctx, (size_t)H * P));
-  {
-    ProfileScope ps(ctx, "dgp_hidden");
-    DMO_TRY(svgp_latent_moments(ctx, g->hidden, up, x.d, P, m1.p, s1.p));
-    DMO_LAUNCH(dgp_hidden_epilogue_kernel, (unsigned)ceil_div(P, 256), 256, 0, x.d, P, d, H, g->xlb.p, g->xrg.p, g->w1.p, g->b1,
-               g->jitter, g->min_var, m1.p, s1.p);
-  }
-  {
-    ProfileScope ps(ctx, "dgp_layer2");
-    const int PT = DG_ROWS / J;
-    dim3 grid((unsigned)ceil_div(P, PT), (unsigned)T);
-    const double* sites = g->quadrature ? g->sites.p : nullptr;
-    if (ov.d) {
-      DMO_CUDA(cudaFuncSetAttribute(dgp_layer2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DG_SMEM));
-      DMO_LAUNCH(dgp_layer2_kernel<true>, grid, 256, DG_SMEM, g->tasks, T, P, H, J, PT, g->Z2, g->Npad2, m1.p, s1.p, sites, seed,
-                 stream_id, g->c2, g->min_var, oe.d, om.d, ov.d);
-    } else {
-      DMO_CUDA(cudaFuncSetAttribute(dgp_layer2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DG_SMEM));
-      DMO_LAUNCH(dgp_layer2_kernel<false>, grid, 256, DG_SMEM, g->tasks, T, P, H, J, PT, g->Z2, g->Npad2, m1.p, s1.p, sites, seed,
-                 stream_id, g->c2, g->min_var, oe.d, om.d, nullptr);
-    }
-  }
-  DMO_CHECK_LAUNCH();
+  DMO_TRY(dgp_predict_device(ctx, g, up, x.d, P, seed, stream_id, oe.d, om.d, ov.d));
   DMO_TRY(up.watchdog(ctx));
   DMO_TRY(om.finish(ctx));
   DMO_TRY(ov.finish(ctx));

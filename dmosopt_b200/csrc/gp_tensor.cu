@@ -628,7 +628,8 @@ __global__ void __launch_bounds__(KM_T, 4)
 // float64 in ascending order over the slice; the slices are those of pick_slices(.., KF_NS, 3 x SMs, ..).  The chains
 // run after each batch of 8 candidates from the unscaled kernel values the batch left in shared memory (one lane per
 // (candidate, 16-point group)); after each chunk, lane l of a warp folds the chunk's group sums of the warp's candidate
-// l into float64.
+// l into float64.  STORE = false writes the same mean and no K_* (the mean of a predict with variance, wanted without
+// its variance: the resident step of the surrogates whose evaluate returns that mean, step.cu).
 constexpr int KF_NS = 16;                         // training points per fp32 partial sum of the mean
 constexpr int KS_T = 128, KS_QW = 32, KS_Q = 4 * KS_QW;  // threads, candidates per warp, candidates per block
 constexpr int KS_C = 64;                          // training points per chunk: two per lane
@@ -643,7 +644,7 @@ constexpr size_t kstar_mean_smem(int MT) {
   return (size_t)(KS_Q * KM_D + 4 * ks_warp_floats(MT)) * sizeof(float) + (size_t)4 * MT * KS_QW * sizeof(double);
 }
 
-template <bool ISO, int MT, bool GROUPED>
+template <bool ISO, int MT, bool GROUPED, bool STORE>
 __global__ void __launch_bounds__(KS_T, MT <= 3 ? 4 : 3)  // 4 blocks / SM up to M = 3 (registers and shared memory)
     kstar_mean_kernel(const double* __restrict__ Xn, int64_t P, int64_t p_base, const float* __restrict__ Xtf, int64_t N,
                       int64_t Npad, int64_t n_per_block, int d, int kind, int G, const int* __restrict__ cov,
@@ -672,7 +673,7 @@ __global__ void __launch_bounds__(KS_T, MT <= 3 ? 4 : 3)  // 4 blocks / SM up to
     const int g = i / KM_D, j = i % KM_D;
     s_il[i] = j < d ? (float)inv_ls[g * d + j] : 0.f;
   }
-  if (t < NG) s_c[t] = scalbnf((float)constant[t], k_exp[t]);
+  if (STORE && t < NG) s_c[t] = scalbnf((float)constant[t], k_exp[t]);
   if (GROUPED && t < MT) s_cov[t] = cov[t];
   __syncthreads();
   const int64_t lo = (int64_t)blockIdx.x * n_per_block;  // slice [lo, hi): multiples of KF_NS
@@ -767,13 +768,15 @@ __global__ void __launch_bounds__(KS_T, MT <= 3 ? 4 : 3)  // 4 blocks / SM up to
           }
           const float2 k0 = stationary2_f(rr, kind);  // (point a, point b)
           *reinterpret_cast<float2*>(s_k + (m * KS_B + v) * KS_LD + 2 * lane) = k0;
-          const float2 kv = fmul2(k0, make_float2(s_c[m] * live_a, s_c[m] * live_b));  // c * k(r) * 2^kexp (exact)
-          const __half2 h = __floats2half2_rn(kv.x, kv.y);
-          const float2 hf = __half22float2(h);
-          const __half2 l = __floats2half2_rn(kv.x - hf.x, kv.y - hf.y);
-          if (mine) {
-            ph[m * hplane] = *reinterpret_cast<const uint32_t*>(&h);
-            pl[m * hplane] = *reinterpret_cast<const uint32_t*>(&l);
+          if constexpr (STORE) {
+            const float2 kv = fmul2(k0, make_float2(s_c[m] * live_a, s_c[m] * live_b));  // c * k(r) * 2^kexp (exact)
+            const __half2 h = __floats2half2_rn(kv.x, kv.y);
+            const float2 hf = __half22float2(h);
+            const __half2 l = __floats2half2_rn(kv.x - hf.x, kv.y - hf.y);
+            if (mine) {
+              ph[m * hplane] = *reinterpret_cast<const uint32_t*>(&h);
+              pl[m * hplane] = *reinterpret_cast<const uint32_t*>(&l);
+            }
           }
         };
         if (ISO) {
@@ -1055,15 +1058,21 @@ int gp_var_contract_tensor(dmo_ctx* ctx, const GpVarOps& ops, const uint16_t* Kh
 const char* const GP_WATCHDOG_MSG = "gp_predict(tensor): pipeline watchdog tripped (mbarrier wait timed out)";
 
 int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, double* d_mean, double* d_var, int* abort_flag,
-                      const GpOverlap* ov) {
+                      const GpOverlap* ov, bool var_route_mean) {
   const int64_t N = gp->N, Npad = gp->ops.Npad;
   const int M = gp->M, G = gp->ops.G, d = gp->d;
   DMO_REQUIRE(M <= 16, "gp_predict(tensor): at most 16 objectives per model (got %d)", M);
   DMO_REQUIRE(d <= 64, "gp_predict(tensor): at most 64 input dimensions (got %d); use DMO_GP_FP64", d);
   DMO_REQUIRE(Npad % TN == 0, "gp_predict(tensor): internal padding error");
-  if (!d_var && d <= KM_D && M <= 6)
+  // var_route_mean: the mean of the route below without its contraction (same chunks, slices and kernels, so the same
+  // bits); the fused producer then stores no K_*, the two-kernel route still needs it for mean_split_kernel
+  const bool mean_only = !d_var && var_route_mean;
+  if (!d_var && !mean_only && d <= KM_D && M <= 6)
     return gp_mean_direct(ctx, gp, dXn, P, d_mean);  // nothing but the mean is wanted: K_* stays in registers
-  DMO_TRY(gp_prepare_tensor(ctx, gp->ops));
+  const bool fused = d <= KM_D && M <= 6 && (gp->isotropic || G <= 2) &&
+                     !(getenv("DMO_GP_FUSED") && atoi(getenv("DMO_GP_FUSED")) == 0);
+  const bool store = !(mean_only && fused);
+  if (store) DMO_TRY(gp_prepare_tensor(ctx, gp->ops));
   constexpr int64_t TMv = KM_Q;  // candidate padding: the K_* producers write 256-candidate blocks
   // candidate chunk: K_* hi/lo (2 x G x Pc x Npad fp16) within ~6 GiB, and the producers' grids within their limit
   int64_t Pc_max = ((int64_t)6 << 30) / ((int64_t)G * Npad * 4);
@@ -1075,20 +1084,23 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
   DevBuf<uint16_t> Kh, Kl;
   DevBuf<double> vnorm;
   DevBuf<int> own_flag;
-  DMO_TRY(Kh.alloc(ctx, (size_t)G * Pc_alloc * Npad));
-  DMO_TRY(Kl.alloc(ctx, (size_t)G * Pc_alloc * Npad));
-  DMO_TRY(vnorm.alloc(ctx, (size_t)n_q * G * Pc_alloc));
-  const bool read_back = abort_flag == nullptr;
-  if (read_back) {
-    DMO_TRY(own_flag.alloc(ctx, 1));
-    abort_flag = own_flag.p;
+  if (store) {
+    DMO_TRY(Kh.alloc(ctx, (size_t)G * Pc_alloc * Npad));
+    DMO_TRY(Kl.alloc(ctx, (size_t)G * Pc_alloc * Npad));
   }
-  DMO_CUDA(cudaMemsetAsync(abort_flag, 0, sizeof(int), ctx->stream));
+  // without the contraction there is no watchdog to read back
+  const bool read_back = abort_flag == nullptr && !mean_only;
+  if (!mean_only) {
+    DMO_TRY(vnorm.alloc(ctx, (size_t)n_q * G * Pc_alloc));
+    if (read_back) {
+      DMO_TRY(own_flag.alloc(ctx, 1));
+      abort_flag = own_flag.p;
+    }
+    DMO_CUDA(cudaMemsetAsync(abort_flag, 0, sizeof(int), ctx->stream));
+  }
   const int64_t kplane = Pc_alloc * Npad;
   // K_* producer fused with the mean (d <= 32, M <= 6; DMO_GP_FUSED=0 keeps kstar_tensor_kernel + mean_split_kernel)
   // (per-dimension length scales with more than two covariances keep the two-kernel route: a distance pass per covariance)
-  const bool fused = d <= KM_D && M <= 6 && (gp->isotropic || G <= 2) &&
-                     !(getenv("DMO_GP_FUSED") && atoi(getenv("DMO_GP_FUSED")) == 0);
   DevBuf<double> mpart;
   if (fused) DMO_TRY(prepare_direct_state(ctx, gp));
   for (int64_t p_base = 0; p_base < P; p_base += Pc_alloc) {
@@ -1104,12 +1116,19 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
       const size_t smem = kstar_mean_smem(M);
       {
         ProfileScope ps_(ctx, "gp_kstar");
-#define KF_LAUNCH(ISO_, MT_, GR_)                                                                                          \
-  do {                                                                                                                     \
-    DMO_CUDA(cudaFuncSetAttribute(kstar_mean_kernel<ISO_, MT_, GR_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    DMO_LAUNCH((kstar_mean_kernel<ISO_, MT_, GR_>), gf, KS_T, smem, dXn, P, p_base, gp->Xtf.p, N, Npad, n_per_block, d,          \
-               gp->kernel, G, gp->cov.p, gp->g_inv_ls.p, gp->g_constant.p, gp->ops.Kexp.p, gp->CAf.p, kplane, Kh.p, Kl.p,   \
-               mpart.p, Pcpad);                                                                                            \
+#define KF_LAUNCH_ST(ISO_, MT_, GR_, ST_)                                                                                      \
+  do {                                                                                                                          \
+    DMO_CUDA(cudaFuncSetAttribute(kstar_mean_kernel<ISO_, MT_, GR_, ST_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+    DMO_LAUNCH((kstar_mean_kernel<ISO_, MT_, GR_, ST_>), gf, KS_T, smem, dXn, P, p_base, gp->Xtf.p, N, Npad, n_per_block, d,          \
+               gp->kernel, G, gp->cov.p, gp->g_inv_ls.p, gp->g_constant.p, gp->ops.Kexp.p, gp->CAf.p, kplane, Kh.p, Kl.p,        \
+               mpart.p, Pcpad);                                                                                                 \
+  } while (0)
+#define KF_LAUNCH(ISO_, MT_, GR_)            \
+  do {                                       \
+    if (store)                               \
+      KF_LAUNCH_ST(ISO_, MT_, GR_, true);    \
+    else                                     \
+      KF_LAUNCH_ST(ISO_, MT_, GR_, false);   \
   } while (0)
 #define KF_SWITCH(ISO_)                                         \
   if (G < M) {                                                  \
@@ -1137,6 +1156,7 @@ int gp_predict_tensor(dmo_ctx* ctx, dmo_gp* gp, const double* dXn, int64_t P, do
         }
 #undef KF_SWITCH
 #undef KF_LAUNCH
+#undef KF_LAUNCH_ST
       }
       DMO_LAUNCH(mean_finish_tc_kernel, (unsigned)ceil_div(Pc * M, 256), 256, 0, mpart.p, (int)nsplit, Pc, Pcpad, M, gp->ymean.p,
                  gp->ystd.p, p_base, d_mean);

@@ -292,6 +292,26 @@ int svgp_latent_moments(dmo_ctx* ctx, dmo_svgp* sv, GpUnitPredict& up, const dou
   return DMO_OK;
 }
 
+int svgp_predict_device(dmo_ctx* ctx, dmo_svgp* sv, GpUnitPredict& up, const double* X, int64_t P, double* mean, double* var) {
+  const int M = sv->M, L = sv->L;
+  DevBuf<double> fm, fv;
+  DMO_TRY(fm.alloc(ctx, (size_t)L * P));
+  if (var) DMO_TRY(fv.alloc(ctx, (size_t)L * P));
+  DMO_TRY(svgp_latent_moments(ctx, sv, up, X, P, fm.p, var ? fv.p : nullptr));
+  {
+    ProfileScope ps(ctx, "svgp_mix");
+    DMO_LAUNCH(sv_mix_kernel, (unsigned)ceil_div(P * M, 256), 256, 0, P, L, M, fm.p, fv.p, sv->W.p, sv->ymean.p, sv->ystd.p,
+               sv->vscale.p, mean, var);
+  }
+  DMO_CHECK_LAUNCH();
+  return DMO_OK;
+}
+
+void svgp_dims(const dmo_svgp* sv, int* d, int* M) {
+  *d = sv->d;
+  *M = sv->M;
+}
+
 int svgp_latent_view(const dmo_svgp* sv, int l, SvLatentView* v) {
   for (auto& gp_ : sv->groups) {
     const SvGroup& gr = *gp_;
@@ -480,7 +500,7 @@ int dmo_svgp_predict(dmo_ctx* ctx, dmo_svgp* sv, const double* X, int64_t P, dou
   if (!ctx) return DMO_ERR_ARG;
   DMO_CUDA(cudaSetDevice(ctx->device));
   DMO_REQUIRE(sv, "svgp_predict: null model");
-  const int M = sv->M, L = sv->L, d = sv->d;
+  const int M = sv->M, d = sv->d;
   GpUnitPredict up;
   DMO_TRY(up.check(ctx, "svgp_predict", precision, d));
   if (P == 0) return DMO_OK;
@@ -490,17 +510,7 @@ int dmo_svgp_predict(dmo_ctx* ctx, dmo_svgp* sv, const double* X, int64_t P, dou
   DMO_TRY(x.init(ctx, X, (size_t)P * d));
   DMO_TRY(om.init(ctx, mean, (size_t)P * M));
   DMO_TRY(ov.init(ctx, var, (size_t)P * M));
-  const bool want_var = ov.d != nullptr;
-  DevBuf<double> fm, fv;
-  DMO_TRY(fm.alloc(ctx, (size_t)L * P));
-  if (want_var) DMO_TRY(fv.alloc(ctx, (size_t)L * P));
-  DMO_TRY(svgp_latent_moments(ctx, sv, up, x.d, P, fm.p, want_var ? fv.p : nullptr));
-  {
-    ProfileScope ps(ctx, "svgp_mix");
-    DMO_LAUNCH(sv_mix_kernel, (unsigned)ceil_div(P * M, 256), 256, 0, P, L, M, fm.p, fv.p, sv->W.p, sv->ymean.p, sv->ystd.p,
-               sv->vscale.p, om.d, ov.d);
-  }
-  DMO_CHECK_LAUNCH();
+  DMO_TRY(svgp_predict_device(ctx, sv, up, x.d, P, om.d, ov.d));
   DMO_TRY(up.watchdog(ctx));
   DMO_TRY(om.finish(ctx));
   DMO_TRY(ov.finish(ctx));

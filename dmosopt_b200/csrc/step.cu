@@ -13,7 +13,10 @@
 // phases (the step_* profile scopes) and counts the waits.
 // dmo_nsga2_step_record runs the same body for MOASMO.optimize's resident epoch (dmosopt_b200/MOASMO.py): the mean only,
 // optionally a feasibility rank as the truncation's last key, and the generation's offspring, their mean and operator
-// counts copied out without a host wait.
+// counts copied out without a host wait.  dmo_nsga2_step_record_posterior runs it with the other posteriors the resident
+// epoch serves: the exact GP (EGP_Matern's linear-mean model), the variational posterior and the deep GPs, each giving
+// the mean its public predict writes when the variance is requested too (what those surrogates' evaluate returns),
+// optionally rounded to float32 before the truncation.
 #include <string.h>
 
 #include <algorithm>
@@ -68,10 +71,45 @@ static int copy_out(dmo_ctx* ctx, void* dst, const void* src, size_t bytes) {
   return DMO_OK;
 }
 
-// The body of both entry points.  key (may be null): the feasibility rank of [children; parents] as the truncation's least
+// The surrogate posterior of a step.  DMO_POSTERIOR_GP with var_route_mean: the mean of the predict with variance,
+// without the variance (gp_predict_device); the variational and deep-GP means never depend on the variance, which these
+// steps do not form (the deep GP's hidden layer still contracts its own: its spread places the last layer's inputs).
+// mean_f32: the offspring's mean is rounded to float32 before the truncation and the record.
+struct StepPosterior {
+  int kind = DMO_POSTERIOR_GP;
+  dmo_gp* gp = nullptr;
+  dmo_svgp* sv = nullptr;
+  dmo_dgp* dg = nullptr;
+  uint64_t draw_seed = 0, draw_stream = 0;  // the deep GP's Philox key (Monte Carlo draws)
+  bool var_route_mean = false;
+  bool mean_f32 = false;
+};
+
+// the posterior mean (and, for the exact GP only, variance) of the P offspring rows of X; only the exact GP's AUTO route
+// with a variance may leave its read-back pending in gpp.  The variational and deep-GP routes wait only for the tensor
+// pipeline's watchdog, when a contraction ran.
+static int step_predict(dmo_ctx* ctx, const StepPosterior& post, const double* X, int64_t P, double* mean, double* var, int precision,
+                        GpPending* gpp) {
+  if (post.kind == DMO_POSTERIOR_GP) return gp_predict_device(ctx, post.gp, X, P, mean, var, precision, gpp, post.var_route_mean);
+  GpUnitPredict up;
+  if (post.kind == DMO_POSTERIOR_SVGP) {
+    int dd = 0, mm = 0;
+    svgp_dims(post.sv, &dd, &mm);
+    DMO_TRY(up.check(ctx, "nsga2_step", precision, dd));
+    DMO_TRY(svgp_predict_device(ctx, post.sv, up, X, P, mean, nullptr));
+  } else {
+    int dd = 0, tt = 0;
+    dgp_dims(post.dg, &dd, &tt);
+    DMO_TRY(up.check(ctx, "nsga2_step", precision, dd));
+    DMO_TRY(dgp_predict_device(ctx, post.dg, up, X, P, post.draw_seed, post.draw_stream, nullptr, mean, nullptr));
+  }
+  return up.watchdog(ctx);
+}
+
+// The body of the entry points.  key (may be null): the feasibility rank of [children; parents] as the truncation's least
 // significant descending key.  x_gen / y_gen / counts (all null, or all set): the offspring, their posterior mean and the
 // operator counts of step_counts_kernel, copied out once the GP is final.
-static int nsga2_step_body(dmo_ctx* ctx, dmo_gp* gp, const dmo_feas* key, double* pop_x, double* pop_y, int32_t* rank,
+static int nsga2_step_body(dmo_ctx* ctx, const StepPosterior& post, const dmo_feas* key, double* pop_x, double* pop_y, int32_t* rank,
                            int64_t pop, int d, int M, double crossover_prob, double mutation_prob, double mutation_rate,
                            const double* di_crossover, const double* di_mutation, const double* xlb, const double* xub,
                            uint64_t seed, uint64_t stream_id, int precision, int distance_metric, int with_variance,
@@ -79,7 +117,7 @@ static int nsga2_step_body(dmo_ctx* ctx, dmo_gp* gp, const dmo_feas* key, double
                            double* y_gen, int64_t* counts) {
   if (!ctx) return DMO_ERR_ARG;
   DMO_CUDA(cudaSetDevice(ctx->device));
-  DMO_REQUIRE(gp && pop_x && pop_y && rank && pop >= 2 && d >= 1 && M >= 1 && di_crossover && di_mutation && xlb && xub,
+  DMO_REQUIRE((post.gp || post.sv || post.dg) && pop_x && pop_y && rank && pop >= 2 && d >= 1 && M >= 1 && di_crossover && di_mutation && xlb && xub,
               "nsga2_step: bad arguments");
   DMO_REQUIRE(distance_metric == DMO_METRIC_NONE || distance_metric == DMO_METRIC_CROWDING || distance_metric == DMO_METRIC_EUCLIDEAN,
               "nsga2_step: unknown distance metric %d", distance_metric);
@@ -156,7 +194,9 @@ static int nsga2_step_body(dmo_ctx* ctx, dmo_gp* gp, const dmo_feas* key, double
     DMO_TRY(dmo_lane_streams(ctx));
     gpp.ov.mean_ready = ctx->lane_ev[0];
     ProfileScope ps(ctx, "step_gp");
-    DMO_TRY(gp_predict_device(ctx, gp, Xs.p, P, Ys.p, with_variance ? var.p : nullptr, precision, &gpp));
+    DMO_TRY(step_predict(ctx, post, Xs.p, P, Ys.p, with_variance ? var.p : nullptr, precision, &gpp));
+    // evaluate's float32 cast; the routes that round have finished their predict here (no pending read-back)
+    if (post.mean_f32) DMO_TRY(prim_round_f32(ctx, Ys.p, P * M));
   }
   auto truncate = [&]() -> int {
     ProfileScope ps(ctx, "step_truncate");
@@ -215,7 +255,7 @@ static int nsga2_step_body(dmo_ctx* ctx, dmo_gp* gp, const dmo_feas* key, double
     DMO_TRY(first_truncate());
   }
   bool refined = false;
-  const int rc = gp_predict_finish(ctx, gp, gpp, &refined);
+  const int rc = gp_predict_finish(ctx, post.gp, gpp, &refined);
   if (rc != DMO_OK) {
     DMO_CUDA(cudaMemcpyAsync(pop_x, Xs.p + (size_t)P * d, (size_t)pop * d * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
     DMO_CUDA(cudaMemcpyAsync(pop_y, Ys.p + (size_t)P * M, (size_t)pop * M * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
@@ -260,7 +300,9 @@ int dmo_nsga2_step(dmo_ctx* ctx, dmo_gp* gp, double* pop_x, double* pop_y, int32
                    const double* di_mutation, const double* xlb, const double* xub, uint64_t seed, uint64_t stream_id,
                    int precision, int distance_metric, int with_variance, int round_to_f32, const double* hv_ref, int64_t* n_children,
                    double* hv_out) {
-  return nsga2_step_body(ctx, gp, nullptr, pop_x, pop_y, rank, pop, d, M, crossover_prob, mutation_prob, mutation_rate,
+  StepPosterior post;
+  post.gp = gp;
+  return nsga2_step_body(ctx, post, nullptr, pop_x, pop_y, rank, pop, d, M, crossover_prob, mutation_prob, mutation_rate,
                          di_crossover, di_mutation, xlb, xub, seed, stream_id, precision, distance_metric, with_variance,
                          round_to_f32, hv_ref, n_children, hv_out, nullptr, nullptr, nullptr);
 }
@@ -274,7 +316,57 @@ int dmo_nsga2_step_record(dmo_ctx* ctx, dmo_gp* gp, const dmo_feas* key, double*
   DMO_REQUIRE(x_gen && y_gen && counts, "nsga2_step_record: x_gen, y_gen and counts are required");
   DMO_REQUIRE(!key || feas_model_dim(key) == d, "nsga2_step_record: the key model takes %d columns, the population has %d",
               feas_model_dim(key), d);
-  return nsga2_step_body(ctx, gp, key, pop_x, pop_y, rank, pop, d, M, crossover_prob, mutation_prob, mutation_rate,
+  StepPosterior post;
+  post.gp = gp;
+  return nsga2_step_body(ctx, post, key, pop_x, pop_y, rank, pop, d, M, crossover_prob, mutation_prob, mutation_rate,
+                         di_crossover, di_mutation, xlb, xub, seed, stream_id, precision, distance_metric, 0, round_to_f32,
+                         nullptr, n_children, nullptr, x_gen, y_gen, counts);
+}
+
+int dmo_nsga2_step_record_posterior(dmo_ctx* ctx, int kind, void* posterior, uint64_t draw_seed, uint64_t draw_stream,
+                                    const dmo_feas* key, double* pop_x, double* pop_y, int32_t* rank, int64_t pop, int d, int M,
+                                    double crossover_prob, double mutation_prob, double mutation_rate, const double* di_crossover,
+                                    const double* di_mutation, const double* xlb, const double* xub, uint64_t seed,
+                                    uint64_t stream_id, int precision, int distance_metric, int mean_f32, int round_to_f32,
+                                    double* x_gen, double* y_gen, int64_t* counts, int64_t* n_children) {
+  if (!ctx) return DMO_ERR_ARG;
+  DMO_CUDA(cudaSetDevice(ctx->device));
+  const char* who = "nsga2_step_record_posterior";
+  DMO_REQUIRE(kind == DMO_POSTERIOR_GP || kind == DMO_POSTERIOR_SVGP || kind == DMO_POSTERIOR_DGP, "%s: unknown posterior kind %d", who,
+              kind);
+  DMO_REQUIRE(posterior, "%s: null posterior", who);
+  DMO_REQUIRE(x_gen && y_gen && counts, "%s: x_gen, y_gen and counts are required", who);
+  DMO_REQUIRE(pop >= 2, "%s: pop must be at least 2 (got %lld)", who, (long long)pop);
+  // AUTO refines the rows its variance flags, so its mean cannot be had without the variance; the exact GP's surrogates
+  // that evaluate on this route predict in float64 or on the tensor path
+  DMO_REQUIRE(precision == DMO_GP_FP64 || precision == DMO_GP_TENSOR, "%s: precision must be DMO_GP_FP64 or DMO_GP_TENSOR (got %d)", who,
+              precision);
+  StepPosterior post;
+  post.kind = kind;
+  post.var_route_mean = true;
+  post.mean_f32 = mean_f32 != 0;
+  int md = 0, mM = 0;
+  if (kind == DMO_POSTERIOR_GP) {
+    post.gp = static_cast<dmo_gp*>(posterior);
+    md = post.gp->d;
+    mM = post.gp->M;
+  } else if (kind == DMO_POSTERIOR_SVGP) {
+    post.sv = static_cast<dmo_svgp*>(posterior);
+    svgp_dims(post.sv, &md, &mM);
+  } else {
+    post.dg = static_cast<dmo_dgp*>(posterior);
+    dgp_dims(post.dg, &md, &mM);
+    DMO_REQUIRE(draw_stream < ((uint64_t)1 << 54), "%s: the draw stream must be below 2^54", who);
+    post.draw_seed = draw_seed;
+    post.draw_stream = draw_stream;
+  }
+  DMO_REQUIRE(md == d && mM == M, "%s: the posterior takes %d inputs and has %d outputs, the population has %d and %d", who, md, mM, d, M);
+  if (kind != DMO_POSTERIOR_GP) {  // the exact GP's d fits every route (dmo_gp_create)
+    GpUnitPredict up;
+    DMO_TRY(up.check(ctx, who, precision, d));
+  }
+  DMO_REQUIRE(!key || feas_model_dim(key) == d, "%s: the key model takes %d columns, the population has %d", who, feas_model_dim(key), d);
+  return nsga2_step_body(ctx, post, key, pop_x, pop_y, rank, pop, d, M, crossover_prob, mutation_prob, mutation_rate,
                          di_crossover, di_mutation, xlb, xub, seed, stream_id, precision, distance_metric, 0, round_to_f32,
                          nullptr, n_children, nullptr, x_gen, y_gen, counts);
 }

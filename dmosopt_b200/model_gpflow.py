@@ -433,6 +433,11 @@ class _VariationalGP:
             return mean, var
         return mean
 
+    def resident_posterior(self):
+        """(kind, handle, precision, mean dtype) of the posterior MOASMO's resident epoch steps on: ``evaluate`` returns
+        this handle's mean with the variance requested, as float32."""
+        return _lib.POSTERIOR_SVGP, getattr(self, "_h", None), self.precision, np.float32
+
 
 class SVGP_Matern(_VariationalGP):
     """dmosopt/model.py:769-988: one SVGP per output, each with its own inducing points."""

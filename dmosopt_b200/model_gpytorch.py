@@ -157,6 +157,11 @@ class EGP_Matern:
         mean, var = self.predict(x)
         return (mean, var) if self.return_mean_variance else mean
 
+    def resident_posterior(self):
+        """(kind, handle, precision, mean dtype) of the posterior MOASMO's resident epoch steps on: ``evaluate`` returns
+        this handle's mean with the variance requested, as float32."""
+        return _lib.POSTERIOR_GP, getattr(self, "_gp", None), self.precision, np.float32
+
 
 # ----------------------------------------------------------------------------------------------------------- MEGP
 def filter_samples(y, x, nan="remove"):
@@ -1002,6 +1007,12 @@ class _DeepGP:
     def evaluate(self, x):
         mean, var = self.predict(x)
         return (mean, var) if self.return_mean_variance else mean
+
+    def resident_posterior(self):
+        """(kind, handle, precision, mean dtype) of the posterior MOASMO's resident epoch steps on: ``evaluate`` returns
+        this handle's mean with the variance requested, as float64.  Each step takes its draw key from ``_draw_key``, as
+        each predict does."""
+        return _lib.POSTERIOR_DGP, getattr(self, "_gp", None), self.precision, np.float64
 
 
 class MDSPP_Matern(_DeepGP):

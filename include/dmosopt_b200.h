@@ -214,6 +214,33 @@ int dmo_nsga2_step_record(dmo_ctx* ctx, dmo_gp* gp, const dmo_feas* key, double*
                           uint64_t stream_id, int precision, int distance_metric, int round_to_f32,
                           double* x_gen, double* y_gen, int64_t* counts, int64_t* n_children);
 
+/* dmo_nsga2_step_record for the other surrogates of the resident epoch: the posterior is given by kind and handle.
+ *   DMO_POSTERIOR_GP    posterior is a dmo_gp* (EGP_Matern: the exact GP with a linear mean)
+ *   DMO_POSTERIOR_SVGP  posterior is a dmo_svgp* (SVGP / VGP / SIV / SPV / CRV_Matern)
+ *   DMO_POSTERIOR_DGP   posterior is a dmo_dgp* (MDSPP / MDGP_Matern); (draw_seed, draw_stream) is the Philox key of
+ *                       its Monte Carlo draws, as dmo_dgp_predict's (seed, stream_id); draw_stream < 2^54
+ * The offspring's objectives are the mean the posterior's predict writes when a variance buffer is passed too, bit for
+ * bit, formed without that variance where the route allows it: the exact GP in float64 and on the tensor path (the
+ * fused K* + mean producer without its K* stores, or K* and the split mean without the contraction), the variational
+ * posterior always; the deep GP forms its hidden layer's variance (it places the last layer's inputs) but not the last
+ * layer's.  mean_f32: that mean is rounded to float32 before the truncation (the surrogates whose evaluate casts to
+ * float32); y_gen receives the rounded values.  precision: DMO_GP_FP64 or DMO_GP_TENSOR (AUTO's refinement follows the
+ * variance).  The host waits for the offspring count, the tensor pipeline's watchdog when a contraction runs (the deep
+ * GP's hidden layer on the tensor path) and the truncation's own reads.  Refused with DMO_ERR_ARG before any launch: an
+ * unknown kind or null posterior, a posterior whose d or M differs from the population's, a key of another width,
+ * missing x_gen / y_gen / counts, pop < 2, draw_stream >= 2^54.  Everything else as dmo_nsga2_step_record. */
+#define DMO_POSTERIOR_GP 0
+#define DMO_POSTERIOR_SVGP 1
+#define DMO_POSTERIOR_DGP 2
+int dmo_nsga2_step_record_posterior(dmo_ctx* ctx, int kind, void* posterior, uint64_t draw_seed,
+                                    uint64_t draw_stream, const dmo_feas* key, double* pop_x, double* pop_y,
+                                    int32_t* rank, int64_t pop, int d, int M, double crossover_prob,
+                                    double mutation_prob, double mutation_rate, const double* di_crossover,
+                                    const double* di_mutation, const double* xlb, const double* xub,
+                                    uint64_t seed, uint64_t stream_id, int precision, int distance_metric,
+                                    int mean_f32, int round_to_f32, double* x_gen, double* y_gen, int64_t* counts,
+                                    int64_t* n_children);
+
 /* ---- A18: exact-GP posterior (GPR_Matern / GPR_RBF predict) -------------------
  * replaces GPR_Matern.predict / .evaluate (dmosopt/model.py:1254-1275; GPR_RBF :1343-1364),
  * i.e. per objective sklearn GaussianProcessRegressor.predict(return_std=True) ** 2.
