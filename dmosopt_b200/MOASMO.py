@@ -2,10 +2,11 @@
 
   * ``optimize``           MOASMO.py:21-131, the surrogate epoch: a drop-in with the same signature and generator
                            protocol.  An eligible epoch (``resident_eligible``) keeps the population in HBM and runs
-                           each generation as one ``dmo_nsga2_step_record`` call (GPR_Matern, GPR_RBF) or one
-                           ``dmo_nsga2_step_record_posterior`` call (EGP, the variational and the deep-GP surrogates); any
-                           other runs the reference's per-generation plugin loop (``optimize_per_generation``).  Both
-                           return the same results.
+                           each generation as one C call: for NSGA2, ``dmo_nsga2_step_record`` (GPR_Matern, GPR_RBF) or
+                           ``dmo_nsga2_step_record_posterior`` (EGP, the variational and the deep-GP surrogates); for
+                           SMPSO, ``dmo_smpso_step_record`` on the resident swarms (every one of those surrogates).  Any
+                           other epoch runs the reference's per-generation plugin loop (``optimize_per_generation``).
+                           Both return the same results.
   * ``epsilon_get_best``   MOASMO.py:703-758 -> MOEA.get_duplicates (dmo_get_duplicates) + dmo_epsilon_sort
 """
 
@@ -40,16 +41,18 @@ def _posterior_types():
 
 
 def resident_eligible(optimizer, model, optimize_mean_variance=False):
-    """True when ``optimize`` runs this epoch on the resident generation step: the optimizer is exactly
-    ``dmosopt_b200.NSGA2``, the surrogate exactly ``GPR_Matern``, ``GPR_RBF``, ``EGP_Matern``, one of the five
-    variational classes or one of the two deep GPs, with its device posterior and returning the mean only, no
-    mean-variance objectives, no adaptive population size, a y-metric of None, "crowding" or "euclidean", and an x-metric
-    of None or the rank of a GPU ``LogisticFeasibilityModel``."""
+    """True when ``optimize`` runs this epoch on a resident generation step: the optimizer is exactly
+    ``dmosopt_b200.NSGA2`` or ``dmosopt_b200.SMPSO``, the surrogate exactly ``GPR_Matern``, ``GPR_RBF``, ``EGP_Matern``,
+    one of the five variational classes or one of the two deep GPs, with its device posterior and returning the mean
+    only, no mean-variance objectives, no adaptive population size, a y-metric of None, "crowding" or "euclidean", and
+    for NSGA2 an x-metric of None or the rank of a GPU ``LogisticFeasibilityModel``, for SMPSO its resident swarm state
+    (``SMPSO._resident``)."""
     from .model import GPR_Matern, GPR_RBF
     from .NSGA2 import NSGA2, _device_feasibility_key
+    from .SMPSO import SMPSO
 
     sm = getattr(model, "objective", None)
-    if type(optimizer) is not NSGA2:
+    if type(optimizer) not in (NSGA2, SMPSO):
         return False
     if type(sm) in (GPR_Matern, GPR_RBF):
         if getattr(sm, "_gp", None) is None:
@@ -63,15 +66,26 @@ def resident_eligible(optimizer, model, optimize_mean_variance=False):
     ym = optimizer.y_distance_metrics
     if ym is not None and (len(ym) != 1 or not isinstance(ym[0], str) or ym[0] not in ("crowding", "euclidean")):
         return False
+    if type(optimizer) is SMPSO:
+        return optimizer._resident_available()
     return optimizer.x_distance_metrics is None or _device_feasibility_key(optimizer.x_distance_metrics) is not None
 
 
 def _state_fits(optimizer, model):
-    """The initialized state has the shapes and dtypes of the resident step: pop (>= 2) rows of float64 parameters,
-    float32 or float64 objectives, ranks."""
+    """The initialized state has the shapes and dtypes of the resident step.  NSGA2: pop (>= 2) rows of float64
+    parameters, float32 or float64 objectives, ranks.  SMPSO: swarm_size * pop rows of float32 positions, float32
+    objectives and float64 velocities, one rank array per swarm."""
+    from .SMPSO import SMPSO
+
     st, sm = optimizer.state, model.objective
-    x, y, r = st.population_parm, st.population_obj, np.asarray(st.rank)
     pop = optimizer.opt_params.popsize
+    if type(optimizer) is SMPSO:
+        n = optimizer.opt_params.swarm_size * pop
+        x, y, v = st.population_parm, st.population_obj, st.velocity
+        return (all(isinstance(a, np.ndarray) for a in (x, y, v)) and x.dtype == np.float32 and y.dtype == np.float32
+                and v.dtype == np.float64 and x.shape == (n, sm.nInput) and y.shape == (n, sm.nOutput) and v.shape == (n, sm.nInput)
+                and len(st.ranks) == optimizer.opt_params.swarm_size and optimizer._resident() is not None)
+    x, y, r = st.population_parm, st.population_obj, np.asarray(st.rank)
     return (isinstance(x, np.ndarray) and isinstance(y, np.ndarray) and x.dtype == np.float64 and y.dtype in (np.float32, np.float64)
             and pop >= 2 and x.shape == (pop, sm.nInput) and y.shape == (pop, sm.nOutput) and r.shape == (pop,))
 
@@ -81,13 +95,15 @@ def optimize(num_generations, optimizer, model, nInput, nOutput, xlb, xub, popsi
     """dmosopt.MOASMO.optimize (MOASMO.py:21-131): a generator that returns the EpochResults through StopIteration.
 
     Eligible epochs (``resident_eligible``) never yield: the host steps before the loop are the reference's, then each
-    generation is one ``dmo_nsga2_step_record`` (or, for EGP, the variational and the deep-GP surrogates,
-    ``dmo_nsga2_step_record_posterior``) call on the population kept in HBM, with the same Philox streams,
-    results and optimizer state as the per-generation loop.  The host waits only for the offspring count of each
-    generation; with ``termination`` it also reads the population back before every ``has_terminated``, and with
-    ``adaptive_operator_rates`` the operator counts before every ``update_operator_rates``.  The offspring and their
-    mean are recorded in page-locked memory, G * (pop + 1) * (d + M) * 8 bytes for G generations.  Other epochs run
-    ``optimize_per_generation``."""
+    generation is one C call on the population kept in HBM, with the same Philox streams, host draws, results and
+    optimizer state as the per-generation loop.  NSGA2 steps on ``dmo_nsga2_step_record`` (or, for EGP, the variational
+    and the deep-GP surrogates, ``dmo_nsga2_step_record_posterior``); the host waits for the offspring count of each
+    generation, and with ``adaptive_operator_rates`` reads the operator counts before every ``update_operator_rates``.
+    SMPSO steps on ``dmo_smpso_step_record`` with the swarms' velocity draws taken on the host; its success counter and
+    operator rates need nothing from the device, and the host waits only inside the predict and the swarm truncations.
+    With ``termination`` the state is read back before every ``has_terminated``.  The offspring and their mean are
+    recorded in page-locked memory, G * R * (d + M) * 8 bytes for G generations of R offspring rows (NSGA2: pop + 1,
+    SMPSO: 2 * swarm_size * pop).  Other epochs run ``optimize_per_generation``."""
     return _optimize(True, num_generations, optimizer, model, nInput, nOutput, xlb, xub, popsize, initial, termination,
                      local_random, logger, optimize_mean_variance, kwargs)
 
@@ -176,12 +192,12 @@ def _log_generation(logger, optimizer, i, num_generations, termination):
 
 
 class _History:
-    """Page-locked rows the resident generations are recorded into: (pop + 1) offspring rows, their means and four
-    operator counts per generation, allocated in blocks of ``per_block`` generations as the epoch goes (its length is
-    open with a termination criterion; page-locked blocks of a bounded size are also recycled by the pool)."""
+    """Page-locked rows the resident generations are recorded into: ``rows`` offspring rows, their means and
+    ``n_counts`` operator counts per generation, allocated in blocks of ``per_block`` generations as the epoch goes (its
+    length is open with a termination criterion; page-locked blocks of a bounded size are also recycled by the pool)."""
 
-    def __init__(self, pop, d, M, per_block):
-        self.pop, self.d, self.M, self.per_block = pop, d, M, max(int(per_block), 1)
+    def __init__(self, rows, d, M, per_block, n_counts):
+        self.rows, self.d, self.M, self.per_block, self.n_counts = rows, d, M, max(int(per_block), 1), n_counts
         self.blocks = []
         self.n = 0
 
@@ -189,98 +205,177 @@ class _History:
         k, j = divmod(self.n, self.per_block)
         if k == len(self.blocks):
             b = self.per_block
-            self.blocks.append((_lib.pinned_empty((b, self.pop + 1, self.d)), _lib.pinned_empty((b, self.pop + 1, self.M)),
-                                _lib.pinned_empty((b, 4), np.int64)))
+            self.blocks.append((_lib.pinned_empty((b, self.rows, self.d)), _lib.pinned_empty((b, self.rows, self.M)),
+                                _lib.pinned_empty((b, self.n_counts), np.int64) if self.n_counts else None))
         self.n += 1
         xb, yb, cb = self.blocks[k]
-        return xb[j], yb[j], cb[j]
+        return xb[j], yb[j], None if cb is None else cb[j]
 
 
-def _resident_generations(num_generations, optimizer, model, termination, logger, OptHistory):
-    """The generations of an eligible epoch on the resident step; yields (i, x_gen, y_gen) once the epoch is done (the
-    rows are views of the page-locked record) and leaves the optimizer's state as the per-generation loop leaves it."""
-    from .NSGA2 import _device_feasibility_key
-
+def _resident_posterior(sm):
+    """(kind, handle, precision, mean dtype, var_route_mean) of the surrogate's device posterior: the exact GP's mean-only
+    predict for GPR_Matern / GPR_RBF, else the mean of the predict with variance (``resident_posterior``)."""
     from .model import GPR_Matern, GPR_RBF
 
-    p, st, sm = optimizer.opt_params, optimizer.state, model.objective
-    # (kind, handle, precision, mean dtype) of the surrogates that step on dmo_nsga2_step_record_posterior
-    post = None if type(sm) in (GPR_Matern, GPR_RBF) else sm.resident_posterior()
-    pop, d = st.population_parm.shape
-    M = st.population_obj.shape[1]
-    key = _device_feasibility_key(optimizer.x_distance_metrics)
-    ym = optimizer.y_distance_metrics
-    metric = {None: _lib.METRIC_NONE, "crowding": _lib.METRIC_CROWDING, "euclidean": _lib.METRIC_EUCLIDEAN}[None if ym is None else ym[0]]
-    round_f32 = st.population_obj.dtype == np.float32
-    xlb, xub = st.bounds[:, 0], st.bounds[:, 1]
+    if type(sm) in (GPR_Matern, GPR_RBF):
+        return _lib.POSTERIOR_GP, sm._gp, sm.precision, np.float64, False
+    return tuple(sm.resident_posterior()) + (True,)
 
-    # the population in HBM: the state's own device mirror when it has one (NSGA2.initialize_state), else a copy
-    base = getattr(optimizer, "_pop_base", None)
-    if base is not None and (st.population_parm.ctypes.data != base.ctypes.data or st.population_parm.shape != base.shape):
-        base = None
-    dev_x = _lib.mirror_array(base) if base is not None else None
-    if dev_x is None:
-        base = None
-        dev_x = _lib.DeviceArray((pop, d), np.float64).upload(st.population_parm)
-    dev_y = _lib.DeviceArray((pop, M), np.float64).upload(np.asarray(st.population_obj, dtype=np.float64))
-    dev_r = _lib.DeviceArray((pop,), np.int32).upload(np.asarray(st.rank, dtype=np.int32))
 
-    def sync_state():
-        if base is not None:
-            _lib.memcpy(base, dev_x.ptr, base.nbytes)  # the read-only state view shows the survivors
+class _Nsga2Step:
+    """NSGA2's generation on the population in HBM: ``dmo_nsga2_step_record`` (GPR_Matern, GPR_RBF) or
+    ``dmo_nsga2_step_record_posterior``; the operator counts are added to the success counters once read."""
+
+    n_counts = 4
+
+    def __init__(self, optimizer, model, post):
+        from .NSGA2 import _device_feasibility_key
+
+        self.opt, self.sm, self.post = optimizer, model.objective, post
+        st = optimizer.state
+        pop, d = st.population_parm.shape
+        M = st.population_obj.shape[1]
+        self.rows = pop + 1
+        self.key = _device_feasibility_key(optimizer.x_distance_metrics)
+        ym = optimizer.y_distance_metrics
+        self.metric = {None: _lib.METRIC_NONE, "crowding": _lib.METRIC_CROWDING, "euclidean": _lib.METRIC_EUCLIDEAN}[None if ym is None else ym[0]]
+        self.round_f32 = st.population_obj.dtype == np.float32
+        # the population in HBM: the state's own device mirror when it has one (NSGA2.initialize_state), else a copy
+        base = getattr(optimizer, "_pop_base", None)
+        if base is not None and (st.population_parm.ctypes.data != base.ctypes.data or st.population_parm.shape != base.shape):
+            base = None
+        self.dev_x = _lib.mirror_array(base) if base is not None else None
+        if self.dev_x is None:
+            base = None
+            self.dev_x = _lib.DeviceArray((pop, d), np.float64).upload(st.population_parm)
+        self.base = base
+        self.dev_y = _lib.DeviceArray((pop, M), np.float64).upload(np.asarray(st.population_obj, dtype=np.float64))
+        self.dev_r = _lib.DeviceArray((pop,), np.int32).upload(np.asarray(st.rank, dtype=np.int32))
+        self.pending = []  # operator counts of generations not yet added to the success counters
+
+    def __call__(self, x_gen, y_gen, counts, draw):
+        opt, p, st = self.opt, self.opt.opt_params, self.opt.state
+        xlb, xub = st.bounds[:, 0], st.bounds[:, 1]
+        seed = opt._rng_seed()
+        stream = opt._next_stream()  # the tournament's stream; the variation takes the next one
+        opt._next_stream()
+        kind, handle, precision, mean_dtype, var_route_mean = self.post
+        if not var_route_mean:
+            P = _lib.nsga2_step_record(handle, self.dev_x, self.dev_y, self.dev_r, p.crossover_prob, p.mutation_prob, p.mutation_rate,
+                                       p.di_crossover, p.di_mutation, xlb, xub, seed, stream, precision, self.metric, self.round_f32, x_gen,
+                                       y_gen, counts, key=self.key)
         else:
-            optimizer._store_population(dev_x.download())
-        st.population_obj[:] = dev_y.download()
-        st.rank[:] = dev_r.download()
+            P = _lib.nsga2_step_record_posterior(kind, handle, draw, self.dev_x, self.dev_y, self.dev_r, p.crossover_prob, p.mutation_prob,
+                                                 p.mutation_rate, p.di_crossover, p.di_mutation, xlb, xub, seed, stream, precision,
+                                                 self.metric, mean_dtype == np.float32, self.round_f32, x_gen, y_gen, counts, key=self.key)
+        self.pending.append(counts)
+        if p.adaptive_operator_rates:
+            self._add_counts()  # the rates of the next generation depend on this one's counts
+            opt.update_operator_rates()
+        return P
 
-    pending = []  # operator counts of generations not yet added to the success counters
-
-    def add_counts():
+    def _add_counts(self):
         _lib.synchronize()
-        for c in pending:
+        st = self.opt.state
+        for c in self.pending:
             # with the plugin's types: len() of the index arrays, np.count_nonzero (an np.intp) of the survivors
             st.total_crossovers += int(c[0]) // 2  # NSGA2.py:159, 176
             st.total_mutations += int(c[1])
             st.successful_crossovers += np.intp(c[2]) / 2  # NSGA2.py:216-222
             st.successful_mutations += np.intp(c[3])
-        pending.clear()
+        self.pending.clear()
 
-    hist = _History(pop, d, M, 8)
+    def sync(self):
+        """The host state as the plugin loop leaves it; every recorded row has landed."""
+        self._add_counts()
+        st = self.opt.state
+        if self.base is not None:
+            _lib.memcpy(self.base, self.dev_x.ptr, self.base.nbytes)  # the read-only state view shows the survivors
+        else:
+            self.opt._store_population(self.dev_x.download())
+        st.population_obj[:] = self.dev_y.download()
+        st.rank[:] = self.dev_r.download()
+
+
+class _SmpsoStep:
+    """SMPSO's generation on its resident swarms (``SMPSO._resident``): ``dmo_smpso_step_record`` with the velocity
+    scalars drawn on the host.  Every swarm keeps pop of its 2 * pop stacked rows, all of them offspring indices below
+    2 * swarm_size * pop, so the plugin's success count (np.isin over the survivors' indices) is swarm_size * pop per
+    generation, known without the device."""
+
+    n_counts = 0
+
+    def __init__(self, optimizer, model, post):
+        self.opt, self.post = optimizer, post
+        self.sw = optimizer._resident()
+        p = optimizer.opt_params
+        self.n = p.swarm_size * p.popsize
+        self.rows = 2 * self.n
+        self.metric = optimizer._metric_code()
+        self.dev_r = _lib.DeviceArray((self.n,), np.int32)  # written by every step; read only once one has run
+        self.stepped = False
+
+    def __call__(self, x_gen, y_gen, counts, draw):
+        opt, p, st = self.opt, self.opt.opt_params, self.opt.state
+        xlb, xub = st.bounds[:, 0], st.bounds[:, 1]
+        seed = opt._rng_seed()  # generate_strategy's order: the seed, then the stream
+        stream = opt._next_stream()
+        sc = opt._velocity_scalars()  # update_strategy's draws
+        kind, handle, precision, mean_dtype, var_route_mean = self.post
+        self.sw.step_record(kind, handle, draw, var_route_mean, p.di_mutation, xlb, xub, p.mutation_rate, seed, stream, precision,
+                            mean_dtype == np.float32, self.metric, sc, self.dev_r, x_gen, y_gen)
+        self.stepped = True
+        st.successful_children += self.n
+        if p.adaptive_operator_rates:
+            opt.update_operator_rates()
+        return self.rows
+
+    def sync(self):
+        """The host state as the plugin loop leaves it, written into the state's own arrays (so the resident copy stays
+        keyed to them); every recorded row has landed.  Before the first step the host state is already the plugin's."""
+        _lib.synchronize()
+        if not self.stepped:
+            return
+        st, sw = self.opt.state, self.sw
+        st.population_parm[...] = sw.parm.download()  # float32 values: the casts are exact
+        st.population_obj[...] = sw.obj.download()
+        sw.velocity_into(st.velocity)
+        r = self.dev_r.download().astype(np.intp).reshape(self.opt.opt_params.swarm_size, -1)
+        for k in range(r.shape[0]):
+            st.ranks[k] = r[k]
+
+
+def _resident_generations(num_generations, optimizer, model, termination, logger, OptHistory):
+    """The generations of an eligible epoch on the resident step; yields (i, x_gen, y_gen) once the epoch is done (the
+    rows are views of the page-locked record) and leaves the optimizer's state as the per-generation loop leaves it."""
+    from .SMPSO import SMPSO
+
+    sm = model.objective
+    post = _resident_posterior(sm)
+    step = (_SmpsoStep if type(optimizer) is SMPSO else _Nsga2Step)(optimizer, model, post)
+    st = optimizer.state
+    # blocks of 8 generations, or of the whole epoch when it is shorter and its length is known
+    per_block = 8 if termination is not None else min(8, num_generations)
+    hist = _History(step.rows, st.population_parm.shape[1], st.population_obj.shape[1], per_block, step.n_counts)
     done = []
     n_eval = 0
     it = range(1, num_generations + 1) if termination is None else itertools.count(1)
     for i in it:
         if termination is not None:
-            add_counts()
-            sync_state()
+            step.sync()
             pop_x, pop_y = optimizer.population_objectives
             if termination.has_terminated(OptHistory(i, n_eval, pop_x, pop_y, None)):
                 break
         _log_generation(logger, optimizer, i, num_generations, termination)
-        seed = optimizer._rng_seed()
-        stream = optimizer._next_stream()  # the tournament's stream; the variation takes the next one
-        optimizer._next_stream()
         x_gen, y_gen, counts = hist.next()
-        if post is None:
-            P = _lib.nsga2_step_record(sm._gp, dev_x, dev_y, dev_r, p.crossover_prob, p.mutation_prob, p.mutation_rate, p.di_crossover,
-                                       p.di_mutation, xlb, xub, seed, stream, sm.precision, metric, round_f32, x_gen, y_gen, counts, key=key)
-        else:
-            kind, handle, precision, mean_dtype = post
-            # a deep GP draws its key as each predict does: MDGP's call counter advances once per generation, in order
-            draw = sm._draw_key() if kind == _lib.POSTERIOR_DGP else (0, 0)
-            P = _lib.nsga2_step_record_posterior(kind, handle, draw, dev_x, dev_y, dev_r, p.crossover_prob, p.mutation_prob, p.mutation_rate,
-                                                 p.di_crossover, p.di_mutation, xlb, xub, seed, stream, precision, metric,
-                                                 mean_dtype == np.float32, round_f32, x_gen, y_gen, counts, key=key)
-        pending.append(counts)
+        # a deep GP draws its key as each predict does: MDGP's call counter advances once per generation, in order
+        draw = sm._draw_key() if post[0] == _lib.POSTERIOR_DGP else (0, 0)
+        P = step(x_gen, y_gen, counts, draw)
         n_eval += P
         done.append((i, x_gen[:P], y_gen[:P]))
-        if p.adaptive_operator_rates:
-            add_counts()  # the rates of the next generation depend on this one's counts
-            optimizer.update_operator_rates()
-    add_counts()
-    sync_state()
-    if post is not None and post[3] == np.float32:
-        # evaluate's float32 means (the record holds them exactly); read once the copies have landed (add_counts synchronised)
+    step.sync()
+    if post[3] == np.float32:
+        # evaluate's float32 means (the record holds them exactly); read once the copies have landed (sync synchronised)
         done = [(i, x, y.astype(np.float32)) for i, x, y in done]
     yield from done
 

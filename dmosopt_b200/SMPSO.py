@@ -116,11 +116,16 @@ class SMPSO(MOEA):
 
     # ---- resident swarm state (csrc/smpso.cu).  The NumPy state arrays stay the interface (dmosopt reads and saves
     # them); the device copy is rebuilt whenever the caller has replaced or resized them.
+    def _resident_available(self):
+        """Whether the swarm state can be kept in HBM: the library has it and the options allow it."""
+        p = self.opt_params
+        if p.adaptive_population_size or getattr(_lib, "SmpsoSwarms", None) is None or self.x_distance_metrics is not None:
+            return False
+        return self.y_distance_metrics is None or self.y_distance_metrics[0] in ("crowding", "euclidean")
+
     def _resident(self):
         st, p = self.state, self.opt_params
-        if p.adaptive_population_size or getattr(_lib, "SmpsoSwarms", None) is None or self.x_distance_metrics is not None:
-            return None
-        if self.y_distance_metrics is not None and self.y_distance_metrics[0] not in ("crowding", "euclidean"):
+        if not self._resident_available():
             return None
         sw = getattr(self, "_swarms", None)
         key = (id(st.population_parm), id(st.population_obj), id(st.velocity), st.population_parm.shape)
@@ -179,25 +184,8 @@ class SMPSO(MOEA):
         """update_strategy with the swarm state in HBM: the scalar draws of velocity_vector are taken from the caller's
         generator in the reference's order (SMPSO.py:317-331, one swarm after the other), everything else is one call."""
         st, p = self.state, self.opt_params
-        S, popsize = p.swarm_size, p.popsize
-        rng = self.local_random
-        sc = np.zeros((S, 8))
-        for k in range(S):
-            r1 = rng.uniform(low=0.0, high=1.0, size=1)[0]
-            r2 = rng.uniform(low=0.0, high=1.0, size=1)[0]
-            w = rng.uniform(low=0.1, high=0.5, size=1)[0]
-            c1 = rng.uniform(low=1.5, high=2.5, size=1)[0]
-            c2 = rng.uniform(low=1.5, high=2.5, size=1)[0]
-            phi = c1 + c2 if c1 + c2 > 4 else 0
-            chi = 2 / (2 - phi - ((phi**2) - 4 * phi) ** (1 / 2))
-            if popsize > 2:
-                ind_1, ind_2 = rng.integers(low=0, high=popsize, size=2)
-            else:
-                ind_1 = ind_2 = -1
-            sc[k] = (w, c1, r1, c2, r2, chi, ind_1, ind_2)
-        code = {None: _lib.METRIC_NONE, "crowding": _lib.METRIC_CROWDING, "euclidean": _lib.METRIC_EUCLIDEAN}[
-            None if self.y_distance_metrics is None else self.y_distance_metrics[0]]
-        ranks, perm = sw.update(x_gen, y_gen, sc, xlb, xub, code, st.population_parm, st.population_obj)
+        S = p.swarm_size
+        ranks, perm = sw.update(x_gen, y_gen, self._velocity_scalars(), xlb, xub, self._metric_code(), st.population_parm, st.population_obj)
         sw.velocity_into(st.velocity)
         _lib.mirror_drop(x_gen)  # consumed: the HBM copy of the offspring matrix is released
         total_children = np.asarray(x_gen).shape[0]
@@ -206,6 +194,32 @@ class SMPSO(MOEA):
             # np.isin(arange(total_children), perm): how many of the kept rows are indices below total_children -- all of them
             # (perm indexes the swarm's 2 * popsize stacked rows and total_children = 2 * swarm_size * popsize), as in SMPSO.py:231-233
             st.successful_children += int(np.count_nonzero(np.isin(np.arange(total_children), perm[k], assume_unique=True)))
+
+    def _velocity_scalars(self):
+        """(swarm_size, 8) float64: w, c1, r1, c2, r2, chi and the two leader indices of each swarm's velocity_vector, drawn
+        from the caller's generator in the reference's order (SMPSO.py:317-331, one swarm after the other); the indices
+        are -1 where the reference draws none (an archive of at most two rows)."""
+        p, rng = self.opt_params, self.local_random
+        sc = np.zeros((p.swarm_size, 8))
+        for k in range(p.swarm_size):
+            r1 = rng.uniform(low=0.0, high=1.0, size=1)[0]
+            r2 = rng.uniform(low=0.0, high=1.0, size=1)[0]
+            w = rng.uniform(low=0.1, high=0.5, size=1)[0]
+            c1 = rng.uniform(low=1.5, high=2.5, size=1)[0]
+            c2 = rng.uniform(low=1.5, high=2.5, size=1)[0]
+            phi = c1 + c2 if c1 + c2 > 4 else 0
+            chi = 2 / (2 - phi - ((phi**2) - 4 * phi) ** (1 / 2))
+            if p.popsize > 2:
+                ind_1, ind_2 = rng.integers(low=0, high=p.popsize, size=2)
+            else:
+                ind_1 = ind_2 = -1
+            sc[k] = (w, c1, r1, c2, r2, chi, ind_1, ind_2)
+        return sc
+
+    def _metric_code(self):
+        """The library's code of the y-metric (None, "crowding" or "euclidean")."""
+        return {None: _lib.METRIC_NONE, "crowding": _lib.METRIC_CROWDING, "euclidean": _lib.METRIC_EUCLIDEAN}[
+            None if self.y_distance_metrics is None else self.y_distance_metrics[0]]
 
     def get_population_strategy(self):
         """SMPSO.py:240-258 (the reference returns the de-duplicated population, not the truncated one)."""

@@ -11,7 +11,7 @@ Plugin import paths (dmosopt resolves them with ``config.import_object_by_path``
 ``dmosopt_b200.install()`` additionally routes the controller-side helpers that dmosopt calls on its own modules
 (resample / get_best duplicates + sort, per-generation termination hypervolume, the epsilon-nondominated archive of
 epsilon_get_best) to the same kernels; ``install(resident_epoch=True)`` also runs eligible surrogate epochs
-(``dmosopt_b200.MOASMO.optimize``: NSGA2 with GPR_Matern / GPR_RBF) on the resident generation step.
+(``dmosopt_b200.MOASMO.optimize``: NSGA2 or SMPSO with one of the GPU surrogates) on the resident generation step.
 ``dmosopt_b200.MOEA.EpsilonSort`` and ``dmosopt_b200.MOASMO.epsilon_get_best`` are the GPU archive's own mirrors of the
 reference's.
 
@@ -36,7 +36,8 @@ from .feasibility import LogisticFeasibilityModel, train_with_feasibility  # noq
 def install(package="dmosopt", resident_epoch=False):
     """Route the reference controller's own hot helpers (resample duplicates / crowding, get_best, termination
     hypervolume, dda_ens, EpsilonSort) to the GPU library; with ``resident_epoch=True``, also run eligible surrogate
-    epochs of ``MOASMO.optimize`` on the resident generation step: see dmosopt_b200/patch.py.  Opt-in; nothing is
+    epochs of ``MOASMO.optimize`` (NSGA2 or SMPSO with a GPU surrogate) on the resident generation step: see
+    dmosopt_b200/patch.py.  Opt-in; nothing is
     patched on import."""
     from . import patch
 

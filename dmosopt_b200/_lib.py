@@ -21,7 +21,7 @@ LIB_PATH = os.path.join(_HERE, "libdmosopt_b200.so")
 METRIC_NONE, METRIC_CROWDING, METRIC_EUCLIDEAN = 0, 1, 2
 KERNEL_MATERN52, KERNEL_RBF = 0, 1
 GP_FP64, GP_TENSOR, GP_AUTO = 0, 1, 2
-POSTERIOR_GP, POSTERIOR_SVGP, POSTERIOR_DGP = 0, 1, 2  # dmo_nsga2_step_record_posterior: dmo_gp, dmo_svgp, dmo_dgp
+POSTERIOR_GP, POSTERIOR_SVGP, POSTERIOR_DGP = 0, 1, 2  # dmo_nsga2_step_record_posterior, dmo_smpso_step_record: dmo_gp, dmo_svgp, dmo_dgp
 GP_PREDICT_MAX_D = 64  # input dimensions of dmo_gp_create (csrc/gp.cu KS_DMAX) and of every tensor-core predict
 GP_PREDICT_MAX_M = 16  # objectives of dmo_gp_create (csrc/gp.cu GP_MAX_M)
 HV_MAX_OBJECTIVES = 8  # dmo_hypervolume: exact, chain sums for M <= 5 (csrc/hv.cu), limit-set recursion for 6 .. 8 (csrc/hv_many.cu)
@@ -146,6 +146,8 @@ _SIGNATURES = {
     "dmo_feas_eval": (_c_int, [_vp, _vp, _vp, _c_i64, _c_int, _vp, _vp, _vp]),
     "dmo_smpso_generate": (_c_int, [_vp, _vp, _vp, _c_int, _c_i64, _c_int, _vp, _vp, _vp, _c_dbl, _c_u64, _c_u64, _vp, _vp]),
     "dmo_smpso_update": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_int, _vp, _c_int, _c_i64, _c_int, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "dmo_smpso_step_record": (_c_int, [_vp, _c_int, _vp, _c_u64, _c_u64, _c_int, _vp, _vp, _vp, _c_int, _c_i64, _c_int, _c_int, _vp, _vp, _vp,
+                                       _c_dbl, _c_u64, _c_u64, _c_int, _c_int, _c_int, _vp, _vp, _vp, _vp]),
 }
 
 _lib = None
@@ -1460,6 +1462,29 @@ class SmpsoSwarms:
         if oo is not obj_out:
             obj_out[...] = oo
         return ranks.astype(np.intp).reshape(self.swarms, self.pop), perm.reshape(self.swarms, self.pop)
+
+    def step_record(self, kind, posterior, draw_key, var_route_mean, di_mutation, xlb, xub, mutation_rate, seed, stream_id, precision,
+                    mean_f32, metric, scalars, ranks, x_gen, y_gen):
+        """One resident SMPSO generation of MOASMO.optimize, recorded (dmo_smpso_step_record): generate, the posterior mean
+        of every offspring row, update.  ``kind`` POSTERIOR_GP, _SVGP or _DGP and ``posterior`` its handle; ``draw_key``
+        (seed, stream_id) keys a deep GP's draws.  ``var_route_mean`` False: the exact GP's mean-only predict (any
+        precision); True: the mean its predict writes with return_var=True, rounded to float32 first when ``mean_f32``.
+        ``scalars`` (swarms, 8) the host draws of the velocity update; ``ranks`` a (swarms * pop,) int32 DeviceArray that
+        receives the survivors' ranks.  ``x_gen`` (2 * swarms * pop, d) and ``y_gen`` (2 * swarms * pop, M) float64
+        receive the offspring and their mean; into page-locked memory they are complete only after ``synchronize()``."""
+        P = 2 * self.swarms * self.pop
+        for name, a, shape in (("x_gen", x_gen, (P, self.d)), ("y_gen", y_gen, (P, self.M))):
+            if isinstance(a, np.ndarray) and (a.shape != shape or a.dtype != np.float64 or not a.flags.c_contiguous or not a.flags.writeable):
+                raise ValueError(f"smpso_step_record: {name} must be a writable C-contiguous float64 array of shape {shape}")
+        sc = _f64(scalars)
+        if sc.shape != (self.swarms, 8):
+            raise ValueError(f"smpso_step_record: scalars must have shape {(self.swarms, 8)}")
+        draw_seed, draw_stream = draw_key
+        di, lb, ub = _per_dim(di_mutation, self.d), _f64(xlb), _f64(xub)  # alive until the call returns
+        _check(load_library().dmo_smpso_step_record(
+            context(), int(kind), posterior._h, _seed(draw_seed), int(draw_stream), 1 if var_route_mean else 0, self.parm.ptr, self.obj.ptr,
+            self.vel.ptr, self.swarms, self.pop, self.d, self.M, _ptr(di), _ptr(lb), _ptr(ub), float(mutation_rate), _seed(seed), int(stream_id),
+            int(precision), 1 if mean_f32 else 0, int(metric), _ptr(sc), _ptr(ranks), _ptr(x_gen), _ptr(y_gen)), "dmo_smpso_step_record")
 
     def velocity_into(self, out):
         """Copy the resident velocities into ``out`` (float64, C-contiguous; page-locked state arrays take the DMA path)."""

@@ -213,6 +213,10 @@ struct Out {
   }
 };
 
+// An output the caller may hand in as device, page-locked or pageable host memory (ctx.cu).  The copy is enqueued on the
+// stream; into pageable memory cudaMemcpyAsync returns only once it has landed, which is a host wait and counted as one.
+int copy_out(dmo_ctx* ctx, void* dst, const void* src, size_t bytes);
+
 // ---------------------------------------------------------------------------
 // device helpers
 #ifdef __CUDACC__

@@ -24,6 +24,18 @@ bool dmo_is_device_ptr(const void* p) {
   return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
 }
 
+int copy_out(dmo_ctx* ctx, void* dst, const void* src, size_t bytes) {
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, dst) != cudaSuccess) {
+    cudaGetLastError();  // clear
+    a.type = cudaMemoryTypeUnregistered;
+  }
+  if (a.type == cudaMemoryTypeUnregistered) ctx->waits++;
+  if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) ctx->d2h_bytes += bytes;
+  DMO_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, ctx->stream));
+  return DMO_OK;
+}
+
 int dmo_lag_slots(dmo_ctx* ctx) {
   if (ctx->lag_host) return DMO_OK;
   DMO_CUDA(cudaHostAlloc((void**)&ctx->lag_host, 3 * sizeof(unsigned long long), cudaHostAllocDefault));

@@ -199,6 +199,31 @@ void dgp_dims(const dmo_dgp* g, int* d, int* T);
 // up.watchdog; stream_id < 2^54 checked by the caller.
 int dgp_predict_device(dmo_ctx* ctx, dmo_dgp* g, GpUnitPredict& up, const double* X, int64_t P, uint64_t seed, uint64_t stream_id,
                        double* eps, double* mean, double* var);
+
+// The surrogate posterior of a resident step (step.cu, smpso.cu).  DMO_POSTERIOR_GP with var_route_mean: the mean of the
+// predict with variance, without the variance (gp_predict_device); the variational and deep-GP means never depend on the
+// variance, which these steps do not form (the deep GP's hidden layer still contracts its own: its spread places the last
+// layer's inputs).  mean_f32: the offspring's mean is rounded to float32 before the truncation and the record.
+struct StepPosterior {
+  int kind = DMO_POSTERIOR_GP;
+  dmo_gp* gp = nullptr;
+  dmo_svgp* sv = nullptr;
+  dmo_dgp* dg = nullptr;
+  uint64_t draw_seed = 0, draw_stream = 0;  // the deep GP's Philox key (Monte Carlo draws)
+  bool var_route_mean = false;
+  bool mean_f32 = false;
+};
+// The posterior given by kind and handle to a recorded step, checked against the population's d and M: an unknown kind, a
+// null handle, a precision other than DMO_GP_FP64 / DMO_GP_TENSOR when var_route_mean (AUTO's refinement follows the
+// variance), a posterior of other dimensions and a deep GP's draw_stream >= 2^54 are refused with DMO_ERR_ARG.  Messages
+// are prefixed by `who`.
+int step_posterior(dmo_ctx* ctx, const char* who, int kind, void* posterior, uint64_t draw_seed, uint64_t draw_stream, bool var_route_mean,
+                   bool mean_f32, int precision, int d, int M, StepPosterior* post);
+// the posterior mean (and, for the exact GP only, variance) of the P rows of the device array X; only the exact GP's AUTO
+// route with a variance may leave its read-back pending in gpp.  The variational and deep-GP routes wait only for the
+// tensor pipeline's watchdog, when a contraction ran.  Messages are prefixed by `who`.
+int step_predict(dmo_ctx* ctx, const char* who, const StepPosterior& post, const double* X, int64_t P, double* mean, double* var,
+                 int precision, GpPending* gpp);
 // Latent l's device operands, for a caller that forms its own K_*: the operator planes O0 = s Lz^-1 and O1 = s T (rows
 // of Npad, zero padded), the mean vector a_l (Npad,), the scaled inducing points XtT (d, Npad) and 1 / ell (d,).
 struct SvLatentView {

@@ -57,50 +57,55 @@ __global__ void __launch_bounds__(kCountWarps * 32) step_counts_kernel(const int
   }
 }
 
-// An output the caller may hand in as device, page-locked or pageable host memory.  The copy is enqueued on the stream;
-// into pageable memory cudaMemcpyAsync returns only once it has landed, which is a host wait and counted as one.
-static int copy_out(dmo_ctx* ctx, void* dst, const void* src, size_t bytes) {
-  cudaPointerAttributes a;
-  if (cudaPointerGetAttributes(&a, dst) != cudaSuccess) {
-    cudaGetLastError();  // clear
-    a.type = cudaMemoryTypeUnregistered;
+int step_posterior(dmo_ctx* ctx, const char* who, int kind, void* posterior, uint64_t draw_seed, uint64_t draw_stream, bool var_route_mean,
+                   bool mean_f32, int precision, int d, int M, StepPosterior* post) {
+  DMO_REQUIRE(kind == DMO_POSTERIOR_GP || kind == DMO_POSTERIOR_SVGP || kind == DMO_POSTERIOR_DGP, "%s: unknown posterior kind %d", who,
+              kind);
+  DMO_REQUIRE(posterior, "%s: null posterior", who);
+  // AUTO refines the rows its variance flags, so its mean cannot be had without the variance; the exact GP's surrogates
+  // that evaluate on this route predict in float64 or on the tensor path
+  if (var_route_mean)
+    DMO_REQUIRE(precision == DMO_GP_FP64 || precision == DMO_GP_TENSOR, "%s: precision must be DMO_GP_FP64 or DMO_GP_TENSOR (got %d)", who,
+                precision);
+  post->kind = kind;
+  post->var_route_mean = var_route_mean;
+  post->mean_f32 = mean_f32;
+  int md = 0, mM = 0;
+  if (kind == DMO_POSTERIOR_GP) {
+    post->gp = static_cast<dmo_gp*>(posterior);
+    md = post->gp->d;
+    mM = post->gp->M;
+  } else if (kind == DMO_POSTERIOR_SVGP) {
+    post->sv = static_cast<dmo_svgp*>(posterior);
+    svgp_dims(post->sv, &md, &mM);
+  } else {
+    post->dg = static_cast<dmo_dgp*>(posterior);
+    dgp_dims(post->dg, &md, &mM);
+    DMO_REQUIRE(draw_stream < ((uint64_t)1 << 54), "%s: the draw stream must be below 2^54", who);
+    post->draw_seed = draw_seed;
+    post->draw_stream = draw_stream;
   }
-  if (a.type == cudaMemoryTypeUnregistered) ctx->waits++;
-  if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) ctx->d2h_bytes += bytes;
-  DMO_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, ctx->stream));
+  DMO_REQUIRE(md == d && mM == M, "%s: the posterior takes %d inputs and has %d outputs, the population has %d and %d", who, md, mM, d, M);
+  if (kind != DMO_POSTERIOR_GP) {  // the exact GP's d fits every route (dmo_gp_create)
+    GpUnitPredict up;
+    DMO_TRY(up.check(ctx, who, precision, d));
+  }
   return DMO_OK;
 }
 
-// The surrogate posterior of a step.  DMO_POSTERIOR_GP with var_route_mean: the mean of the predict with variance,
-// without the variance (gp_predict_device); the variational and deep-GP means never depend on the variance, which these
-// steps do not form (the deep GP's hidden layer still contracts its own: its spread places the last layer's inputs).
-// mean_f32: the offspring's mean is rounded to float32 before the truncation and the record.
-struct StepPosterior {
-  int kind = DMO_POSTERIOR_GP;
-  dmo_gp* gp = nullptr;
-  dmo_svgp* sv = nullptr;
-  dmo_dgp* dg = nullptr;
-  uint64_t draw_seed = 0, draw_stream = 0;  // the deep GP's Philox key (Monte Carlo draws)
-  bool var_route_mean = false;
-  bool mean_f32 = false;
-};
-
-// the posterior mean (and, for the exact GP only, variance) of the P offspring rows of X; only the exact GP's AUTO route
-// with a variance may leave its read-back pending in gpp.  The variational and deep-GP routes wait only for the tensor
-// pipeline's watchdog, when a contraction ran.
-static int step_predict(dmo_ctx* ctx, const StepPosterior& post, const double* X, int64_t P, double* mean, double* var, int precision,
-                        GpPending* gpp) {
+int step_predict(dmo_ctx* ctx, const char* who, const StepPosterior& post, const double* X, int64_t P, double* mean, double* var,
+                 int precision, GpPending* gpp) {
   if (post.kind == DMO_POSTERIOR_GP) return gp_predict_device(ctx, post.gp, X, P, mean, var, precision, gpp, post.var_route_mean);
   GpUnitPredict up;
   if (post.kind == DMO_POSTERIOR_SVGP) {
     int dd = 0, mm = 0;
     svgp_dims(post.sv, &dd, &mm);
-    DMO_TRY(up.check(ctx, "nsga2_step", precision, dd));
+    DMO_TRY(up.check(ctx, who, precision, dd));
     DMO_TRY(svgp_predict_device(ctx, post.sv, up, X, P, mean, nullptr));
   } else {
     int dd = 0, tt = 0;
     dgp_dims(post.dg, &dd, &tt);
-    DMO_TRY(up.check(ctx, "nsga2_step", precision, dd));
+    DMO_TRY(up.check(ctx, who, precision, dd));
     DMO_TRY(dgp_predict_device(ctx, post.dg, up, X, P, post.draw_seed, post.draw_stream, nullptr, mean, nullptr));
   }
   return up.watchdog(ctx);
@@ -194,7 +199,7 @@ static int nsga2_step_body(dmo_ctx* ctx, const StepPosterior& post, const dmo_fe
     DMO_TRY(dmo_lane_streams(ctx));
     gpp.ov.mean_ready = ctx->lane_ev[0];
     ProfileScope ps(ctx, "step_gp");
-    DMO_TRY(step_predict(ctx, post, Xs.p, P, Ys.p, with_variance ? var.p : nullptr, precision, &gpp));
+    DMO_TRY(step_predict(ctx, "nsga2_step", post, Xs.p, P, Ys.p, with_variance ? var.p : nullptr, precision, &gpp));
     // evaluate's float32 cast; the routes that round have finished their predict here (no pending read-back)
     if (post.mean_f32) DMO_TRY(prim_round_f32(ctx, Ys.p, P * M));
   }
@@ -337,34 +342,8 @@ int dmo_nsga2_step_record_posterior(dmo_ctx* ctx, int kind, void* posterior, uin
   DMO_REQUIRE(posterior, "%s: null posterior", who);
   DMO_REQUIRE(x_gen && y_gen && counts, "%s: x_gen, y_gen and counts are required", who);
   DMO_REQUIRE(pop >= 2, "%s: pop must be at least 2 (got %lld)", who, (long long)pop);
-  // AUTO refines the rows its variance flags, so its mean cannot be had without the variance; the exact GP's surrogates
-  // that evaluate on this route predict in float64 or on the tensor path
-  DMO_REQUIRE(precision == DMO_GP_FP64 || precision == DMO_GP_TENSOR, "%s: precision must be DMO_GP_FP64 or DMO_GP_TENSOR (got %d)", who,
-              precision);
   StepPosterior post;
-  post.kind = kind;
-  post.var_route_mean = true;
-  post.mean_f32 = mean_f32 != 0;
-  int md = 0, mM = 0;
-  if (kind == DMO_POSTERIOR_GP) {
-    post.gp = static_cast<dmo_gp*>(posterior);
-    md = post.gp->d;
-    mM = post.gp->M;
-  } else if (kind == DMO_POSTERIOR_SVGP) {
-    post.sv = static_cast<dmo_svgp*>(posterior);
-    svgp_dims(post.sv, &md, &mM);
-  } else {
-    post.dg = static_cast<dmo_dgp*>(posterior);
-    dgp_dims(post.dg, &md, &mM);
-    DMO_REQUIRE(draw_stream < ((uint64_t)1 << 54), "%s: the draw stream must be below 2^54", who);
-    post.draw_seed = draw_seed;
-    post.draw_stream = draw_stream;
-  }
-  DMO_REQUIRE(md == d && mM == M, "%s: the posterior takes %d inputs and has %d outputs, the population has %d and %d", who, md, mM, d, M);
-  if (kind != DMO_POSTERIOR_GP) {  // the exact GP's d fits every route (dmo_gp_create)
-    GpUnitPredict up;
-    DMO_TRY(up.check(ctx, who, precision, d));
-  }
+  DMO_TRY(step_posterior(ctx, who, kind, posterior, draw_seed, draw_stream, true, mean_f32 != 0, precision, d, M, &post));
   DMO_REQUIRE(!key || feas_model_dim(key) == d, "%s: the key model takes %d columns, the population has %d", who, feas_model_dim(key), d);
   return nsga2_step_body(ctx, post, key, pop_x, pop_y, rank, pop, d, M, crossover_prob, mutation_prob, mutation_rate,
                          di_crossover, di_mutation, xlb, xub, seed, stream_id, precision, distance_metric, 0, round_to_f32,

@@ -20,8 +20,8 @@ called by the reference's controller code directly on its own modules, so swappi
 ``install()`` rebinds exactly those module attributes of an already importable ``dmosopt`` package to the functions of
 this package (same signatures, same results: see tests/test_gpu_reference_loop.py) and ``uninstall()`` restores them.
 ``install(resident_epoch=True)`` also rebinds ``MOASMO.optimize``, the surrogate epoch of ``MOASMO.epoch``: an epoch
-that ``dmosopt_b200.MOASMO.resident_eligible`` accepts (this package's NSGA2 with a GPR_Matern / GPR_RBF surrogate) runs
-on the resident generation step, with the per-generation loop's results; every other epoch runs the reference's own
+that ``dmosopt_b200.MOASMO.resident_eligible`` accepts (this package's NSGA2 or SMPSO with one of its GPU surrogates)
+runs on the resident generation step, with the per-generation loop's results; every other epoch runs the reference's own
 ``optimize`` unchanged, including the yield / send protocol of an epoch without a surrogate.
 Nothing is patched implicitly; importing dmosopt_b200 never touches dmosopt.
 """

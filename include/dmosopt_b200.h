@@ -581,6 +581,27 @@ int dmo_smpso_update(dmo_ctx* ctx, double* parm, double* obj, double* vel, const
                      const double* y_gen, int swarms, int64_t pop, int d, int M, int metric, const double* scalars,
                      const double* xlb, const double* xub, int32_t* ranks, int64_t* perm, float* parm_f32,
                      float* obj_f32);
+/* dmo_smpso_step_record: one generation of MOASMO.optimize's surrogate epoch for SMPSO (dmosopt/MOASMO.py:105-122) on the
+ * resident swarm state, as dmo_smpso_generate -> the posterior's predict -> dmo_smpso_update give it, bit for bit:
+ *   1. the offspring of dmo_smpso_generate (seed, stream_id), P = 2*swarms*pop rows, kept on the device as float64;
+ *   2. their posterior mean, given by kind and handle as in dmo_nsga2_step_record_posterior (draw_seed / draw_stream
+ *      key a deep GP's draws, draw_stream < 2^54).  var_route_mean = 0: the exact GP's mean-only predict
+ *      (GPR_Matern / GPR_RBF evaluate; kind DMO_POSTERIOR_GP, any precision including AUTO).  var_route_mean = 1: the
+ *      mean the predict writes when a variance buffer is passed too (EGP, the variational and the deep-GP evaluate;
+ *      precision DMO_GP_FP64 or DMO_GP_TENSOR).  mean_f32: that mean rounded to float32 (the float32 surrogates' cast);
+ *   3. dmo_smpso_update on rows [0, swarms*pop) of the offspring (float64, x_is_f32 = 0) and their mean, with the host
+ *      scalars (swarms, 8); ranks (swarms*pop,) int32 DEVICE receives the survivors' ranks;
+ *   4. x_gen (P, d) and y_gen (P, M) float64 receive the offspring and their mean.  Into device or page-locked memory
+ *      the copies are enqueued without a host wait and are complete after dmo_synchronize(ctx).
+ * The host waits inside the predict (a tensor watchdog) and inside each swarm's truncation only.  Refused with
+ * DMO_ERR_ARG before any launch: an unknown kind or null posterior, var_route_mean = 0 with another kind than the exact
+ * GP, AUTO with var_route_mean = 1, a posterior whose d or M differs from the state's, swarm state or ranks not on the
+ * device, scalars on the device, a null x_gen or y_gen, a leader index >= pop, draw_stream >= 2^54. */
+int dmo_smpso_step_record(dmo_ctx* ctx, int kind, void* posterior, uint64_t draw_seed, uint64_t draw_stream,
+                          int var_route_mean, double* parm, double* obj, double* vel, int swarms, int64_t pop, int d,
+                          int M, const double* di_mutation, const double* xlb, const double* xub,
+                          double mutation_rate, uint64_t seed, uint64_t stream_id, int precision, int mean_f32,
+                          int metric, const double* scalars, int32_t* ranks, double* x_gen, double* y_gen);
 
 /* ---- A13 / A15: MO-CMA-ES ----------------------------------------------------------------
  * dmo_cmaes_sample: individuals[i] = x_p + sigma_p * (A_p @ z_i), p = p_idx[i] (dmosopt/CMAES.py:263-267);

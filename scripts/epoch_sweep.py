@@ -2,10 +2,11 @@
 """One MOASMO.optimize surrogate epoch, resident against the per-generation plugin loop, at bench.py's shape.
 
     python scripts/epoch_sweep.py [--pop 65536] [--d 30] [--M 3] [--train 4096] [--gens 50] [--rounds 3]
-                                  [--surrogate GPR_Matern] [--precision auto]
+                                  [--surrogate GPR_Matern] [--precision auto] [--optimizer NSGA2] [--swarm-size 5]
 
 NSGA2 (distance_metric=None, as MOASMO.epoch builds it) with a GPR_Matern surrogate (precision "auto", the
-hyper-parameters kept at their initial values) fitted on DTLZ2 data; the training set is the epoch's ``initial`` rows, as
+hyper-parameters kept at their initial values) fitted on DTLZ2 data; --optimizer SMPSO runs SMPSO with --swarm-size
+swarms of --pop particles instead (2 * swarm_size * pop candidates per generation); the training set is the epoch's ``initial`` rows, as
 MOASMO.epoch passes it.  --surrogate EGP_Matern, SVGP_Matern, VGP_Matern, SIV_Matern, SPV_Matern, MDSPP_Matern or
 MDGP_Matern (--precision fp64 or tensor) builds that class from seeded hyper-parameters instead, with no training: EGP
 with one length scale per objective, the variational classes with their own inducing-point rule (SVGP: 0.2 N points per
@@ -131,7 +132,10 @@ def epoch(fn, sm, X, Y, a, evaluate=None):
     if evaluate is not None:
         sm.evaluate = evaluate
     model = b2.Model(objective=sm)
-    opt = b2.NSGA2(popsize=a.pop, nInput=a.d, nOutput=a.M, model=model, distance_metric=None)
+    if a.optimizer == "SMPSO":
+        opt = b2.SMPSO(popsize=a.pop, nInput=a.d, nOutput=a.M, model=model, distance_metric=None, swarm_size=a.swarm_size)
+    else:
+        opt = b2.NSGA2(popsize=a.pop, nInput=a.d, nOutput=a.M, model=model, distance_metric=None)
     xlb, xub = np.zeros(a.d), np.ones(a.d)
     clock = GenerationClock()
     _lib.synchronize()
@@ -171,13 +175,16 @@ def main():
     ap.add_argument("--seed", type=int, default=2026)
     ap.add_argument("--surrogate", default="GPR_Matern")
     ap.add_argument("--precision", default="auto")
+    ap.add_argument("--optimizer", default="NSGA2", choices=("NSGA2", "SMPSO"))
+    ap.add_argument("--swarm-size", type=int, default=5)
     a = ap.parse_args()
 
     import dmosopt_b200 as b2
     from dmosopt_b200 import MOASMO
 
     print(json.dumps({"card": card(), "pop": a.pop, "d": a.d, "M": a.M, "train": a.train, "gens": a.gens, "rounds": a.rounds,
-                      "surrogate": a.surrogate, "precision": a.precision}), flush=True)
+                      "surrogate": a.surrogate, "precision": a.precision, "optimizer": a.optimizer,
+                      "swarm_size": a.swarm_size if a.optimizer == "SMPSO" else None}), flush=True)
     rng = np.random.default_rng(a.seed)
     X = rng.random((a.train, a.d))
     Y = dtlz2(X, a.M)
