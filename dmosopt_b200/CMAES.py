@@ -59,6 +59,64 @@ def _stable_order(rank):
     return np.argsort(rank, kind="stable")
 
 
+def _strategy_scalars(p, psucc, pidx, C, chosen, not_chosen):
+    """The host arithmetic of update_strategy (CMAES.py:273-411), shared by the plugin and MOASMO's resident generation:
+    the success rates and step-size factors are NumPy's (its float64 ``exp`` is not CUDA's), everything they scale stays
+    on the device.  ``p`` the optimizer parameters, ``psucc`` the parents' success rates, ``pidx`` the parent of each of
+    the C + P candidates (offspring first), ``chosen`` / ``not_chosen`` the selection masks.  Returns a Struct of
+      ch_off, par, off_psucc, off_fac   the chosen offspring (candidate rows), their parents, success rates and step-size
+                                        factors;
+      seg_row, seg_start, ev_fac        the parents' success / failure events: one segment per parent, its factors in
+                                        order (dmo_scale_rows);
+      ch, src_idx, psucc                the next parent set: candidate rows, the strategy rows each takes (an index into
+                                        the chosen offspring when ch < C, else into the parents) and its success rates."""
+    cp, d, ptarg = p.cp, p.d, p.ptarg
+    fac = lambda ps: np.exp((ps - ptarg) / (d * (1.0 - ptarg)))  # noqa: E731
+
+    # chosen offspring: their success rate advances from the parent's
+    ch_off = np.flatnonzero(chosen[:C])  # offspring are the first C candidates
+    par = pidx[ch_off]
+    off_psucc = (1.0 - cp) * psucc[par] + cp
+    off_fac = fac(off_psucc)
+
+    # parents: one success event per chosen offspring (ascending candidate index), then one failure event per not-chosen
+    # offspring; the recurrences are sequential per parent: the scalar success rates are advanced event rank by event rank
+    # here, the step-size rows take their factors in the same order on the device
+    new_psucc = psucc.copy()
+    nc_off = np.flatnonzero(not_chosen[:C])
+    ev_parent = np.concatenate((par, pidx[nc_off]))
+    ev_success = np.concatenate((np.ones(len(par), dtype=bool), np.zeros(len(nc_off), dtype=bool)))
+    seg_row, seg_start, f_ev = np.zeros(0, dtype=np.int64), np.zeros(0, dtype=np.int64), np.zeros(0)
+    if len(ev_parent) > 0:
+        order = _stable_order(ev_parent)
+        ep, es = ev_parent[order], ev_success[order]
+        first = np.r_[True, ep[1:] != ep[:-1]]
+        seg_start = np.flatnonzero(first)
+        k_in_parent = np.arange(len(ep)) - np.repeat(seg_start, np.diff(np.r_[seg_start, len(ep)]))
+        f_ev = np.empty(len(ep))
+        for k in range(int(k_in_parent.max()) + 1):
+            sel = np.flatnonzero(k_in_parent == k)
+            q = ep[sel]
+            new_psucc[q] = (1.0 - cp) * new_psucc[q] + np.where(es[sel], cp, 0.0)
+            f_ev[sel] = fac(new_psucc[q])
+        seg_row, seg_start = ep[seg_start], np.r_[seg_start, len(ep)]
+
+    # the next parent set (CMAES.py:385-411)
+    ch = np.flatnonzero(chosen)
+    ch_is_off = ch < C
+    slot = np.full(len(chosen), -1, dtype=np.int64)
+    slot[ch_off] = np.arange(len(ch_off))
+    src_par = pidx[ch]
+    psucc_n = new_psucc[src_par]
+    src_idx = src_par.astype(np.int64)
+    if len(ch_off) > 0:
+        o = slot[ch[ch_is_off]]
+        psucc_n[ch_is_off] = off_psucc[o]
+        src_idx[ch_is_off] = o  # these rows come from the updated offspring arrays
+    return Struct(ch_off=ch_off, par=par, off_psucc=off_psucc, off_fac=off_fac, seg_row=seg_row, seg_start=seg_start, ev_fac=f_ev, ch=ch,
+                  src_idx=src_idx, psucc=psucc_n)
+
+
 class CMAES(MOEA):
     def __init__(
         self,
@@ -201,56 +259,24 @@ class CMAES(MOEA):
         is_off = np.concatenate((np.ones(C, dtype=bool), np.zeros(P, dtype=bool)))
         pidx = np.concatenate((p_idxs, np.arange(P, dtype=np.int_)))
         chosen, not_chosen, rank = self._select(candidates_x, candidates_y, is_off, pidx)
-        cp, cc, ccov, d, ptarg, pthresh = p.cp, p.cc, p.ccov, p.d, p.ptarg, p.pthresh
-        fac = lambda ps: np.exp((ps - ptarg) / (d * (1.0 - ptarg)))  # noqa: E731
+        h = _strategy_scalars(p, st.psucc, pidx, C, chosen, not_chosen)
 
         # ---- chosen offspring: their own strategy parameters start from the parent's (copied before any update)
-        ch_off = np.flatnonzero(chosen[:C])  # offspring are the first C candidates
-        par = pidx[ch_off]
-        off_psucc = (1.0 - cp) * st.psucc[par] + cp
-        last_steps = _lib.gather_rows(sig_d, par)
-        off_sigmas = _lib.scale_rows(_lib.gather_rows(sig_d, par), fac(off_psucc))
-        off_A, off_Ainv, off_pc = _lib.gather_rows(A_d, par), _lib.gather_rows(Ainv_d, par), _lib.gather_rows(pc_d, par)
-        if len(ch_off) > 0:
-            z = _lib.cmaes_step_z(xg_d, ch_off, px_d, par, xlb, xub, last_steps)
-            off_A, off_Ainv, off_pc = _lib.cmaes_update_cholesky(off_A, off_Ainv, off_pc, z, off_psucc, cc, ccov, pthresh)
+        last_steps = _lib.gather_rows(sig_d, h.par)
+        off_sigmas = _lib.scale_rows(_lib.gather_rows(sig_d, h.par), h.off_fac)
+        off_A, off_Ainv, off_pc = _lib.gather_rows(A_d, h.par), _lib.gather_rows(Ainv_d, h.par), _lib.gather_rows(pc_d, h.par)
+        if len(h.ch_off) > 0:
+            z = _lib.cmaes_step_z(xg_d, h.ch_off, px_d, h.par, xlb, xub, last_steps)
+            off_A, off_Ainv, off_pc = _lib.cmaes_update_cholesky(off_A, off_Ainv, off_pc, z, h.off_psucc, p.cc, p.ccov, p.pthresh)
+        # ---- parents: the step-size rows take their event factors in order, in place (the old rows were copied above)
+        if len(h.seg_row) > 0:
+            _lib.scale_rows(sig_d, h.ev_fac, seg_row=h.seg_row, seg_start=h.seg_start)
 
-        # ---- parents: one success event per chosen offspring (ascending candidate index), then one failure event per
-        # not-chosen offspring; the recurrences are sequential per parent: the scalar success rates are advanced event
-        # rank by event rank here, the step-size rows take their factors in the same order on the device
-        new_psucc = st.psucc.copy()
-        nc_off = np.flatnonzero(not_chosen[:C])
-        ev_parent = np.concatenate((par, pidx[nc_off]))
-        ev_success = np.concatenate((np.ones(len(par), dtype=bool), np.zeros(len(nc_off), dtype=bool)))
-        if len(ev_parent) > 0:
-            order = _stable_order(ev_parent)
-            ep, es = ev_parent[order], ev_success[order]
-            first = np.r_[True, ep[1:] != ep[:-1]]
-            seg_start = np.flatnonzero(first)
-            k_in_parent = np.arange(len(ep)) - np.repeat(seg_start, np.diff(np.r_[seg_start, len(ep)]))
-            f_ev = np.empty(len(ep))
-            for k in range(int(k_in_parent.max()) + 1):
-                sel = np.flatnonzero(k_in_parent == k)
-                q = ep[sel]
-                new_psucc[q] = (1.0 - cp) * new_psucc[q] + np.where(es[sel], cp, 0.0)
-                f_ev[sel] = fac(new_psucc[q])
-            _lib.scale_rows(sig_d, f_ev, seg_row=ep[seg_start], seg_start=np.r_[seg_start, len(ep)])  # in place: the old rows were copied above
-        st.psucc = new_psucc
-
-        # ---- assemble the next parent set (CMAES.py:385-411)
-        ch = np.flatnonzero(chosen)
+        # ---- assemble the next parent set (CMAES.py:385-411): one device-side gather per state array, a surviving
+        # parent keeps its rows, a chosen offspring brings its own
+        ch, src_idx = h.ch, h.src_idx
         ch_is_off = ch < C
-        slot = np.full(C + P, -1, dtype=np.int64)
-        slot[ch_off] = np.arange(len(ch_off))
-        src_par = pidx[ch]
-        psucc_n = st.psucc[src_par]
-        src_idx = src_par.astype(np.int64)
-        if len(ch_off) > 0:
-            o = slot[ch[ch_is_off]]
-            psucc_n[ch_is_off] = off_psucc[o]
-            src_idx[ch_is_off] = o  # these rows come from the updated offspring arrays
-        # one device-side gather per state array: a surviving parent keeps its rows, a chosen offspring brings its own
-        sel = ch_is_off if len(ch_off) > 0 else None
+        sel = ch_is_off if len(h.ch_off) > 0 else None
         alt = (lambda a: a) if sel is not None else (lambda a: None)
         sigmas_n = _lib.gather_rows(sig_d, src_idx, alt=alt(off_sigmas), sel=sel)
         A_n = _lib.gather_rows(A_d, src_idx, alt=alt(off_A), sel=sel)
@@ -260,7 +286,7 @@ class CMAES(MOEA):
         st.parents_x = _lib.gather_rows(px_d, x_idx, alt=alt(xg_d), sel=sel)
         st.parents_y = candidates_y[ch]
         st.rank = rank[ch]
-        st.sigmas, st.A, st.Ainv, st.pc, st.psucc = sigmas_n, A_n, Ainv_n, pc_n, psucc_n
+        st.sigmas, st.A, st.Ainv, st.pc, st.psucc = sigmas_n, A_n, Ainv_n, pc_n, h.psucc
         _lib.mirror_drop(x_gen)  # the offspring matrix has been consumed: callers that keep it hold host memory only
         if p.adaptive_population_size:
             self.update_population_size()

@@ -4,8 +4,9 @@
                            protocol.  An eligible epoch (``resident_eligible``) keeps the population in HBM and runs
                            each generation as one C call: for NSGA2, ``dmo_nsga2_step_record`` (GPR_Matern, GPR_RBF) or
                            ``dmo_nsga2_step_record_posterior`` (EGP, the variational and the deep-GP surrogates); for
-                           SMPSO, ``dmo_smpso_step_record`` on the resident swarms (every one of those surrogates).  Any
-                           other epoch runs the reference's per-generation plugin loop (``optimize_per_generation``).
+                           SMPSO, ``dmo_smpso_step_record`` on the resident swarms (every one of those surrogates); for
+                           CMAES, ``dmo_cmaes_step_record`` and ``dmo_cmaes_step_apply`` on the resident parent state.
+                           Any other epoch runs the reference's per-generation plugin loop (``optimize_per_generation``).
                            Both return the same results.
   * ``epsilon_get_best``   MOASMO.py:703-758 -> MOEA.get_duplicates (dmo_get_duplicates) + dmo_epsilon_sort
 """
@@ -42,17 +43,20 @@ def _posterior_types():
 
 def resident_eligible(optimizer, model, optimize_mean_variance=False):
     """True when ``optimize`` runs this epoch on a resident generation step: the optimizer is exactly
-    ``dmosopt_b200.NSGA2`` or ``dmosopt_b200.SMPSO``, the surrogate exactly ``GPR_Matern``, ``GPR_RBF``, ``EGP_Matern``,
-    one of the five variational classes or one of the two deep GPs, with its device posterior and returning the mean
-    only, no mean-variance objectives, no adaptive population size, a y-metric of None, "crowding" or "euclidean", and
-    for NSGA2 an x-metric of None or the rank of a GPU ``LogisticFeasibilityModel``, for SMPSO its resident swarm state
-    (``SMPSO._resident``)."""
+    ``dmosopt_b200.NSGA2``, ``dmosopt_b200.SMPSO`` or ``dmosopt_b200.CMAES``, the surrogate exactly ``GPR_Matern``,
+    ``GPR_RBF``, ``EGP_Matern``, one of the five variational classes or one of the two deep GPs, with its device posterior
+    and returning the mean only, no mean-variance objectives, no adaptive population size, and
+      NSGA2: a y-metric of None, "crowding" or "euclidean", an x-metric of None or the rank of a GPU
+             ``LogisticFeasibilityModel``;
+      SMPSO: the same y-metrics and its resident swarm state (``SMPSO._resident``);
+      CMAES: no x-metric (no ``model.feasibility``); its sortMO never reads the y-metric."""
+    from .CMAES import CMAES
     from .model import GPR_Matern, GPR_RBF
     from .NSGA2 import NSGA2, _device_feasibility_key
     from .SMPSO import SMPSO
 
     sm = getattr(model, "objective", None)
-    if type(optimizer) not in (NSGA2, SMPSO):
+    if type(optimizer) not in (NSGA2, SMPSO, CMAES):
         return False
     if type(sm) in (GPR_Matern, GPR_RBF):
         if getattr(sm, "_gp", None) is None:
@@ -63,6 +67,8 @@ def resident_eligible(optimizer, model, optimize_mean_variance=False):
         return False
     if optimizer.opt_params.adaptive_population_size:
         return False
+    if type(optimizer) is CMAES:
+        return optimizer.x_distance_metrics is None
     ym = optimizer.y_distance_metrics
     if ym is not None and (len(ym) != 1 or not isinstance(ym[0], str) or ym[0] not in ("crowding", "euclidean")):
         return False
@@ -74,11 +80,22 @@ def resident_eligible(optimizer, model, optimize_mean_variance=False):
 def _state_fits(optimizer, model):
     """The initialized state has the shapes and dtypes of the resident step.  NSGA2: pop (>= 2) rows of float64
     parameters, float32 or float64 objectives, ranks.  SMPSO: swarm_size * pop rows of float32 positions, float32
-    objectives and float64 velocities, one rank array per swarm."""
+    objectives and float64 velocities, one rank array per swarm.  CMAES: pop (>= 2) resident rows of parameters, step
+    sizes (one or d per row), Cholesky factors, their inverses and paths, float32 or float64 objectives, success rates
+    and ranks, and at least one offspring per generation."""
+    from .CMAES import CMAES
     from .SMPSO import SMPSO
 
     st, sm = optimizer.state, model.objective
     pop = optimizer.opt_params.popsize
+    if type(optimizer) is CMAES:
+        p, d, M = optimizer.opt_params, sm.nInput, sm.nOutput
+        rows = (st.parents_x, st.sigmas, st.A, st.Ainv, st.pc)
+        y, ps, r = st.parents_y, st.psucc, np.asarray(st.rank)
+        return (all(isinstance(a, _lib.ResidentRows) for a in rows) and st.parents_x.shape == (pop, d) and st.sigmas.shape in ((pop,), (pop, d))
+                and st.A.shape == (pop, d, d) and st.Ainv.shape == (pop, d, d) and st.pc.shape == (pop, d) and isinstance(y, np.ndarray)
+                and y.dtype in (np.float32, np.float64) and y.shape == (pop, M) and isinstance(ps, np.ndarray) and ps.dtype == np.float64
+                and ps.shape == (pop,) and r.shape == (pop,) and pop >= 2 and int(p.mu) >= 1 and int(p.lambda_) >= 1 and d <= 512 and M <= 16)
     if type(optimizer) is SMPSO:
         n = optimizer.opt_params.swarm_size * pop
         x, y, v = st.population_parm, st.population_obj, st.velocity
@@ -101,9 +118,12 @@ def optimize(num_generations, optimizer, model, nInput, nOutput, xlb, xub, popsi
     generation, and with ``adaptive_operator_rates`` reads the operator counts before every ``update_operator_rates``.
     SMPSO steps on ``dmo_smpso_step_record`` with the swarms' velocity draws taken on the host; its success counter and
     operator rates need nothing from the device, and the host waits only inside the predict and the swarm truncations.
+    CMAES steps on ``dmo_cmaes_step_record`` (with the normals and parent draws taken on the host first), one wait for
+    the candidates' selection and the offspring's parents, its success rates and step-size factors on the host
+    (``CMAES._strategy_scalars``), then ``dmo_cmaes_step_apply``.
     With ``termination`` the state is read back before every ``has_terminated``.  The offspring and their mean are
     recorded in page-locked memory, G * R * (d + M) * 8 bytes for G generations of R offspring rows (NSGA2: pop + 1,
-    SMPSO: 2 * swarm_size * pop).  Other epochs run ``optimize_per_generation``."""
+    SMPSO: 2 * swarm_size * pop, CMAES: lambda_ * mu).  Other epochs run ``optimize_per_generation``."""
     return _optimize(True, num_generations, optimizer, model, nInput, nOutput, xlb, xub, popsize, initial, termination,
                      local_random, logger, optimize_mean_variance, kwargs)
 
@@ -345,18 +365,69 @@ class _SmpsoStep:
             st.ranks[k] = r[k]
 
 
+class _CmaesStep:
+    """CMAES's generation on its resident parent state (``_lib.CmaesResident``): the normals and parent draws of
+    generate_strategy from ``local_random`` in its order, ``dmo_cmaes_step_record``, one wait, the host arithmetic of
+    update_strategy (``CMAES._strategy_scalars``), ``dmo_cmaes_step_apply``."""
+
+    n_counts = 0
+
+    def __init__(self, optimizer, model, post):
+        self.opt, self.post = optimizer, post
+        st, p = optimizer.state, optimizer.opt_params
+        self.mu, self.lambda_ = int(p.mu), int(p.lambda_)
+        self.rows = self.lambda_ * self.mu
+        # vstack((y_gen, parents_y)) stays float32 only when both are
+        self.cand_f32 = post[3] == np.float32 and st.parents_y.dtype == np.float32
+        self.res = _lib.CmaesResident(st.parents_x, st.sigmas, st.A, st.Ainv, st.pc, st.parents_y, self.rows)
+        self.psucc = st.psucc
+        self.stepped = False
+
+    def __call__(self, x_gen, y_gen, counts, draw):
+        from .CMAES import _strategy_scalars
+
+        opt, p, res = self.opt, self.opt.opt_params, self.res
+        rng = opt.local_random
+        xlb, xub = opt.bounds[:, 0], opt.bounds[:, 1]
+        arz = rng.normal(size=(self.rows, res.d))  # generate_strategy's draws, in its order
+        js = rng.choice(min(self.mu, res.pop), size=self.rows)
+        kind, handle, precision, mean_dtype, var_route_mean = self.post
+        res.step_record(kind, handle, draw, var_route_mean, precision, mean_dtype == np.float32, self.cand_f32, arz, js, self.mu, xlb, xub,
+                        x_gen, y_gen)
+        _lib.synchronize()
+        chosen = res.codes.astype(bool)
+        pidx = np.concatenate((res.p_idx, np.arange(res.pop, dtype=np.int_)))
+        h = _strategy_scalars(p, self.psucc, pidx, self.rows, chosen, ~chosen)
+        res.step_apply(h, xlb, xub, p.cc, p.ccov, p.pthresh)
+        self.psucc = h.psucc
+        self.stepped = True
+        return self.rows
+
+    def sync(self):
+        """The host state as the plugin loop leaves it: the current half of the double buffer becomes the state's
+        ResidentRows.  Before the first step the host state is already the plugin's."""
+        _lib.synchronize()
+        if not self.stepped:
+            return
+        st = self.opt.state
+        st.parents_x, st.sigmas, st.A, st.Ainv, st.pc, py, rank = self.res.state
+        st.parents_y = py.download().astype(np.float32 if self.cand_f32 else np.float64)
+        st.rank = rank.download().astype(np.intp)
+        st.psucc = self.psucc
+
+
 def _resident_generations(num_generations, optimizer, model, termination, logger, OptHistory):
     """The generations of an eligible epoch on the resident step; yields (i, x_gen, y_gen) once the epoch is done (the
     rows are views of the page-locked record) and leaves the optimizer's state as the per-generation loop leaves it."""
+    from .CMAES import CMAES
     from .SMPSO import SMPSO
 
     sm = model.objective
     post = _resident_posterior(sm)
-    step = (_SmpsoStep if type(optimizer) is SMPSO else _Nsga2Step)(optimizer, model, post)
-    st = optimizer.state
+    step = {SMPSO: _SmpsoStep, CMAES: _CmaesStep}.get(type(optimizer), _Nsga2Step)(optimizer, model, post)
     # blocks of 8 generations, or of the whole epoch when it is shorter and its length is known
     per_block = 8 if termination is not None else min(8, num_generations)
-    hist = _History(step.rows, st.population_parm.shape[1], st.population_obj.shape[1], per_block, step.n_counts)
+    hist = _History(step.rows, sm.nInput, sm.nOutput, per_block, step.n_counts)
     done = []
     n_eval = 0
     it = range(1, num_generations + 1) if termination is None else itertools.count(1)

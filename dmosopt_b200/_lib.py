@@ -148,6 +148,11 @@ _SIGNATURES = {
     "dmo_smpso_update": (_c_int, [_vp, _vp, _vp, _vp, _vp, _c_int, _vp, _c_int, _c_i64, _c_int, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dmo_smpso_step_record": (_c_int, [_vp, _c_int, _vp, _c_u64, _c_u64, _c_int, _vp, _vp, _vp, _c_int, _c_i64, _c_int, _c_int, _vp, _vp, _vp,
                                        _c_dbl, _c_u64, _c_u64, _c_int, _c_int, _c_int, _vp, _vp, _vp, _vp]),
+    "dmo_cmaes_step_record": (_c_int, [_vp, _c_int, _vp, _c_u64, _c_u64, _c_int, _c_int, _c_int, _c_int, _vp, _vp, _c_int, _vp, _vp, _c_i64,
+                                       _c_int, _c_int, _vp, _vp, _c_i64, _c_i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "dmo_cmaes_step_apply": (_c_int, [_vp, _vp, _vp, _c_int, _vp, _vp, _vp, _c_i64, _c_int, _c_int, _vp, _vp, _vp, _c_i64, _c_i64, _vp, _vp,
+                                      _vp, _vp, _c_i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_dbl, _c_dbl, _c_dbl, _vp, _vp, _vp, _vp, _vp,
+                                      _vp, _vp]),
 }
 
 _lib = None
@@ -1654,6 +1659,66 @@ def cmaes_update_cholesky(A, Ainv, pc, z, psucc, cc, ccov, pthresh):
     _check(load_library().dmo_cmaes_update_cholesky(context(), _ptr(A), _ptr(Ainv), _ptr(pc), _ptr(z), _ptr(ps), n, d, float(cc), float(ccov), float(pthresh)),
            "dmo_cmaes_update_cholesky")
     return A, Ainv, pc
+
+
+class CmaesResident:
+    """The device buffers of MOASMO's resident MO-CMA-ES generation (dmo_cmaes_step_record / dmo_cmaes_step_apply): the
+    parent state in two halves, each (parents_x, sigmas, A, Ainv, pc) ResidentRows plus the float64 objectives and int32
+    ranks, and the candidates of the current generation (offspring x, [y_gen; parents_y], their ranks).  ``cur`` is the
+    half that holds the state; ``apply`` writes the other one and flips."""
+
+    def __init__(self, parents_x, sigmas, A, Ainv, pc, parents_y, n_off):
+        self.pop, self.d = parents_x.shape
+        self.M = parents_y.shape[1]
+        self.C = int(n_off)
+        rows = (parents_x, sigmas, A, Ainv, pc)
+        # half 0 is the plugin's own state (no copy), half 1 is allocated here
+        self.halves = [rows + (DeviceArray((self.pop, self.M)).upload(_f64(parents_y)), DeviceArray((self.pop,), np.int32)),
+                       tuple(ResidentRows(DeviceArray(r.shape, np.float64), r.shape) for r in rows)
+                       + (DeviceArray((self.pop, self.M)), DeviceArray((self.pop,), np.int32))]
+        self.cur = 0
+        n = self.C + self.pop
+        self.cand_x = DeviceArray((self.C, self.d))
+        self.cand_y = DeviceArray((n, self.M))
+        self.cand_rank = DeviceArray((n,), np.int32)
+        self.codes = pinned_empty((n,), np.uint8)
+        self.p_idx = pinned_empty((self.C,), np.int64)
+
+    @property
+    def state(self):
+        """(parents_x, sigmas, A, Ainv, pc, parents_y, rank) of the current half."""
+        return self.halves[self.cur]
+
+    def step_record(self, kind, posterior, draw_key, var_route_mean, precision, mean_f32, cand_f32, arz, js, mu, xlb, xub, x_gen, y_gen):
+        """The first half of a generation (dmo_cmaes_step_record): ``arz`` (C, d) normals and ``js`` (C,) parent draws from
+        the host.  x_gen / y_gen (C, d) / (C, M) float64, ``self.codes`` and ``self.p_idx`` are complete after
+        ``synchronize()``."""
+        px, sg, A, _, _, py, _ = self.state
+        z, j = _f64(arz), np.ascontiguousarray(js, dtype=np.int64)
+        lb, ub = _f64(xlb), _f64(xub)
+        if z.shape != (self.C, self.d) or j.shape != (self.C,):
+            raise ValueError(f"cmaes_step_record: arz must have shape {(self.C, self.d)} and js {(self.C,)}")
+        draw_seed, draw_stream = draw_key
+        _check(load_library().dmo_cmaes_step_record(
+            context(), int(kind), posterior._h, _seed(draw_seed), int(draw_stream), 1 if var_route_mean else 0, int(precision), 1 if mean_f32 else 0,
+            1 if cand_f32 else 0, px.ptr, sg.ptr, sg.row_elems, A.ptr, py.ptr, self.pop, self.d, self.M, _ptr(z), _ptr(j), self.C, int(mu), _ptr(lb),
+            _ptr(ub), self.cand_x.ptr, self.cand_y.ptr, self.cand_rank.ptr, _ptr(x_gen), _ptr(y_gen), _ptr(self.codes), _ptr(self.p_idx)),
+            "dmo_cmaes_step_record")
+
+    def step_apply(self, h, xlb, xub, cc, ccov, pthresh):
+        """The second half (dmo_cmaes_step_apply) with the host's update arithmetic ``h`` (CMAES._strategy_scalars);
+        the next parent set goes to the other half, which becomes the current one."""
+        px, sg, A, Ainv, pc, _, _ = self.state
+        out = self.halves[1 - self.cur]
+        i64 = lambda a: np.ascontiguousarray(a, dtype=np.int64)  # noqa: E731
+        oc, op, sr, ss, nc, ns = i64(h.ch_off), i64(h.par), i64(h.seg_row), i64(h.seg_start), i64(h.ch), i64(h.src_idx)
+        ps, of, ef = _f64(h.off_psucc), _f64(h.off_fac), _f64(h.ev_fac)
+        lb, ub = _f64(xlb), _f64(xub)
+        _check(load_library().dmo_cmaes_step_apply(
+            context(), px.ptr, sg.ptr, sg.row_elems, A.ptr, Ainv.ptr, pc.ptr, self.pop, self.d, self.M, self.cand_x.ptr, self.cand_y.ptr,
+            self.cand_rank.ptr, self.C, oc.shape[0], _ptr(oc), _ptr(op), _ptr(ps), _ptr(of), sr.shape[0], _ptr(sr), _ptr(ss), _ptr(ef), _ptr(nc),
+            _ptr(ns), _ptr(lb), _ptr(ub), float(cc), float(ccov), float(pthresh), *(a.ptr for a in out)), "dmo_cmaes_step_apply")
+        self.cur = 1 - self.cur
 
 
 # --------------------------------------------------------------------------- sensitivity analysis (SA_DGSM / SA_FAST)

@@ -17,7 +17,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(CSRC, "build")
 LIB = os.path.join(HERE, "libdmosopt_b200.so")
 
-SOURCES = ["ctx.cu", "prims.cu", "rank.cu", "sortmo.cu", "variation.cu", "gp.cu", "gp_fit.cu", "gp_tensor.cu", "gp_multitask.cu", "gp_multitask_fit.cu", "gp_variational.cu", "gp_variational_fit.cu", "gp_deep.cu", "gp_deep_fit.cu", "hv.cu", "hv3_tree.cu", "hv_many.cu", "hv_mc.cu", "epsilon.cu", "sa.cu", "design.cu", "feasibility.cu", "moea_ext.cu", "smpso.cu", "benchmarks.cu", "step.cu"]
+SOURCES = ["ctx.cu", "prims.cu", "rank.cu", "sortmo.cu", "variation.cu", "gp.cu", "gp_fit.cu", "gp_tensor.cu", "gp_multitask.cu", "gp_multitask_fit.cu", "gp_variational.cu", "gp_variational_fit.cu", "gp_deep.cu", "gp_deep_fit.cu", "hv.cu", "hv3_tree.cu", "hv_many.cu", "hv_mc.cu", "epsilon.cu", "sa.cu", "design.cu", "feasibility.cu", "moea_ext.cu", "smpso.cu", "cmaes_step.cu", "benchmarks.cu", "step.cu"]
 
 NVCC_FLAGS = [
     "-gencode",

@@ -374,6 +374,21 @@ int nsga2_generate_device(dmo_ctx* ctx, const double* d_pop_x, int d, const int6
 int remove_worst_device(dmo_ctx* ctx, const double* dX, const double* dY, int64_t n, int d, int M, int metric,
                         const double* const* d_extra, int n_extra, int64_t keep, double* dX_out, double* dY_out, int32_t* d_rank_out,
                         int64_t* d_perm_out);
+// device bodies of dmo_gather_rows, dmo_cmaes_generate, dmo_cmaes_step_z, dmo_scale_rows, dmo_cmaes_update_cholesky
+// (moea_ext.cu) and dmo_ehvi_select (hv.cu) for the resident CMA-ES step (cmaes_step.cu): device arrays only, without the
+// entry points' trailing waits.  ehvi_select_device takes 1 <= k <= nc and waits once, for its box count.
+int gather_rows_device(dmo_ctx* ctx, const double* src, const double* alt, const uint8_t* sel, const int64_t* idx, int64_t n,
+                       int64_t row_elems, double* dst);
+int cmaes_generate_device(dmo_ctx* ctx, const double* parents_x, const double* sigmas, int sigma_cols, const double* A,
+                          const int64_t* p_idx, const double* z, int64_t n, int d, const double* xlb, const double* xub, double* x_out);
+int cmaes_step_z_device(dmo_ctx* ctx, const double* x_gen, const int64_t* cand_idx, const double* parents_x, const int64_t* par_idx,
+                        const double* xlb, const double* xub, const double* steps, int64_t n, int d, double* z_out);
+int scale_rows_device(dmo_ctx* ctx, double* rows, int64_t row_elems, int64_t n_seg, const int64_t* seg_row, const int64_t* seg_start,
+                      const double* factors);
+int cmaes_update_cholesky_device(dmo_ctx* ctx, double* A, double* Ainv, double* pc, const double* z, const double* psucc, int64_t n, int d,
+                                 double cc, double ccov, double pthresh);
+int ehvi_select_device(dmo_ctx* ctx, const double* F, int64_t nf, const double* means, const double* variances, int64_t nc, int M,
+                       const double* ref, int nds, int64_t k, int64_t* sel, double* score);
 // the feasibility model's rank (csrc/feasibility.cu) of n device rows into d_rank, enqueued on the context's stream
 int feas_rank_device(dmo_ctx* ctx, const dmo_feas* m, const double* dX, int64_t n, double* d_rank);
 int feas_model_dim(const dmo_feas* m);

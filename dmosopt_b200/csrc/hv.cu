@@ -759,6 +759,59 @@ int hv3_ranked_finish(dmo_ctx* ctx, Hv3Ranked& s, double* h_out) {
   return sum_partials(ctx, partial, nb, h_out);
 }
 
+// The body of dmo_ehvi_select on device arrays (1 <= k <= nc), without its trailing wait: it waits once, for the box count
+int ehvi_select_device(dmo_ctx* ctx, const double* F, int64_t nf, const double* means, const double* variances, int64_t nc, int M,
+                       const double* ref, int nds, int64_t k, int64_t* sel, double* score) {
+  // rank-0 subset of the chosen set (indicators.py:299-303)
+  DevBuf<double> front_buf;
+  const double* front = F;
+  int64_t nfr = nf;
+  if (nds) {
+    DMO_TRY(nondominated_subset(ctx, F, nf, M, front_buf, &nfr));
+    if (nfr > 0)
+      front = front_buf.p;
+    else
+      nfr = nf;
+  }
+  DevBuf<uint32_t> sidx;
+  DMO_TRY(prim_sort_by_column(ctx, front, nfr, M, 0, sidx));
+  DevBuf<int32_t> flag, pos;
+  DMO_TRY(flag.alloc(ctx, nfr + 2));
+  DMO_TRY(pos.alloc(ctx, nfr + 2));
+  DMO_LAUNCH(box_flag_kernel, (unsigned)ceil_div(nfr + 2, 256), 256, 0, front, sidx.p, nfr, M, ref, flag.p);
+  DMO_TRY(prim_exclusive_sum_i32(ctx, flag.p, pos.p, nfr + 2));
+  int32_t nb = 0;
+  DMO_CUDA(cudaMemcpyAsync(&nb, pos.p + nfr + 1, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  DMO_CUDA(dmo_wait(ctx));
+  DevBuf<double> lower, upper, sc;
+  DMO_TRY(lower.alloc(ctx, (size_t)(nb > 0 ? nb : 1) * M));
+  DMO_TRY(upper.alloc(ctx, (size_t)(nb > 0 ? nb : 1) * M));
+  DMO_TRY(sc.alloc(ctx, nc));
+  if (nb > 0)
+    DMO_LAUNCH(box_write_kernel, (unsigned)ceil_div(nfr + 1, 256), 256, 0, front, sidx.p, nfr, M, ref, flag.p, pos.p,
+               lower.p, upper.p);
+  if (M <= 8)
+    DMO_LAUNCH(ehvi_kernel<8>, (unsigned)ceil_div(nc, 128), 128, 2 * 64 * M * sizeof(double), lower.p, upper.p, (int64_t)nb,
+               M, means, variances, nc, sc.p);
+  else
+    DMO_LAUNCH(ehvi_kernel<16>, (unsigned)ceil_div(nc, 128), 128, 2 * 64 * M * sizeof(double), lower.p, upper.p, (int64_t)nb,
+               M, means, variances, nc, sc.p);
+  // k largest scores, ties by candidate index
+  DevBuf<uint64_t> k0, k1;
+  DevBuf<uint32_t> i0, i1;
+  DMO_TRY(k0.alloc(ctx, nc));
+  DMO_TRY(k1.alloc(ctx, nc));
+  DMO_TRY(i0.alloc(ctx, nc));
+  DMO_TRY(i1.alloc(ctx, nc));
+  DMO_LAUNCH(neg_key_kernel, (unsigned)ceil_div(nc, 256), 256, 0, sc.p, nc, k0.p, i0.p);
+  DMO_TRY(prim_sort_pairs_u64(ctx, k0.p, k1.p, i0.p, i1.p, nc, 0, 64));
+  DMO_LAUNCH(widen_idx_kernel, (unsigned)ceil_div(k, 256), 256, 0, i1.p, k, sel);
+  if (score) DMO_CUDA(cudaMemcpyAsync(score, sc.p, nc * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
+  DMO_CHECK_LAUNCH();
+  return DMO_OK;
+}
+
+
 extern "C" {
 
 int dmo_hypervolume(dmo_ctx* ctx, const double* F, int64_t n, int M, const double* ref, double* out) {
@@ -825,56 +878,11 @@ int dmo_ehvi_select(dmo_ctx* ctx, const double* F, int64_t nf, const double* mea
   DMO_TRY(mu.init(ctx, means, (size_t)nc * M));
   DMO_TRY(var.init(ctx, variances, (size_t)nc * M));
   DMO_TRY(r.init(ctx, ref, (size_t)M));
-  // rank-0 subset of the chosen set (indicators.py:299-303)
-  DevBuf<double> front_buf;
-  const double* front = f.d;
-  int64_t nfr = nf;
-  if (nds) {
-    DMO_TRY(nondominated_subset(ctx, f.d, nf, M, front_buf, &nfr));
-    if (nfr > 0)
-      front = front_buf.p;
-    else
-      nfr = nf;
-  }
-  DevBuf<uint32_t> sidx;
-  DMO_TRY(prim_sort_by_column(ctx, front, nfr, M, 0, sidx));
-  DevBuf<int32_t> flag, pos;
-  DMO_TRY(flag.alloc(ctx, nfr + 2));
-  DMO_TRY(pos.alloc(ctx, nfr + 2));
-  DMO_LAUNCH(box_flag_kernel, (unsigned)ceil_div(nfr + 2, 256), 256, 0, front, sidx.p, nfr, M, r.d, flag.p);
-  DMO_TRY(prim_exclusive_sum_i32(ctx, flag.p, pos.p, nfr + 2));
-  int32_t nb = 0;
-  DMO_CUDA(cudaMemcpyAsync(&nb, pos.p + nfr + 1, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
-  DMO_CUDA(dmo_wait(ctx));
-  DevBuf<double> lower, upper, sc;
-  DMO_TRY(lower.alloc(ctx, (size_t)(nb > 0 ? nb : 1) * M));
-  DMO_TRY(upper.alloc(ctx, (size_t)(nb > 0 ? nb : 1) * M));
-  DMO_TRY(sc.alloc(ctx, nc));
-  if (nb > 0)
-    DMO_LAUNCH(box_write_kernel, (unsigned)ceil_div(nfr + 1, 256), 256, 0, front, sidx.p, nfr, M, r.d, flag.p, pos.p,
-               lower.p, upper.p);
-  if (M <= 8)
-    DMO_LAUNCH(ehvi_kernel<8>, (unsigned)ceil_div(nc, 128), 128, 2 * 64 * M * sizeof(double), lower.p, upper.p, (int64_t)nb,
-               M, mu.d, var.d, nc, sc.p);
-  else
-    DMO_LAUNCH(ehvi_kernel<16>, (unsigned)ceil_div(nc, 128), 128, 2 * 64 * M * sizeof(double), lower.p, upper.p, (int64_t)nb,
-               M, mu.d, var.d, nc, sc.p);
-  // k largest scores, ties by candidate index
-  DevBuf<uint64_t> k0, k1;
-  DevBuf<uint32_t> i0, i1;
-  DMO_TRY(k0.alloc(ctx, nc));
-  DMO_TRY(k1.alloc(ctx, nc));
-  DMO_TRY(i0.alloc(ctx, nc));
-  DMO_TRY(i1.alloc(ctx, nc));
-  DMO_LAUNCH(neg_key_kernel, (unsigned)ceil_div(nc, 256), 256, 0, sc.p, nc, k0.p, i0.p);
-  DMO_TRY(prim_sort_pairs_u64(ctx, k0.p, k1.p, i0.p, i1.p, nc, 0, 64));
   Out<int64_t> osel;
   Out<double> osc;
   DMO_TRY(osel.init(ctx, sel, (size_t)k));
   DMO_TRY(osc.init(ctx, score, (size_t)nc));
-  DMO_LAUNCH(widen_idx_kernel, (unsigned)ceil_div(k, 256), 256, 0, i1.p, k, osel.d);
-  if (osc.d) DMO_CUDA(cudaMemcpyAsync(osc.d, sc.p, nc * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
-  DMO_CHECK_LAUNCH();
+  DMO_TRY(ehvi_select_device(ctx, f.d, nf, mu.d, var.d, nc, M, r.d, nds, k, osel.d, osc.d));
   DMO_TRY(osel.finish(ctx));
   DMO_TRY(osc.finish(ctx));
   DMO_CUDA(dmo_wait(ctx));

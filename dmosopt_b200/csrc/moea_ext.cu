@@ -332,6 +332,52 @@ __global__ void scale_rows_kernel(double* __restrict__ rows, int64_t row, int64_
 
 }  // namespace
 
+// The bodies of the CMA-ES entry points and of dmo_gather_rows / dmo_scale_rows on device arrays, without their trailing
+// waits; the resident CMA-ES step (cmaes_step.cu) composes them.
+int gather_rows_device(dmo_ctx* ctx, const double* src, const double* alt, const uint8_t* sel, const int64_t* idx, int64_t n,
+                       int64_t row_elems, double* dst) {
+  if (n == 0) return DMO_OK;
+  DMO_LAUNCH(gather_rows_kernel, (unsigned)ceil_div(n * row_elems, 256), 256, 0, src, alt, sel, idx, n, row_elems, dst);
+  DMO_CHECK_LAUNCH();
+  return DMO_OK;
+}
+
+int cmaes_generate_device(dmo_ctx* ctx, const double* parents_x, const double* sigmas, int sigma_cols, const double* A,
+                          const int64_t* p_idx, const double* z, int64_t n, int d, const double* xlb, const double* xub, double* x_out) {
+  DevBuf<unsigned long long> mx;
+  DMO_TRY(mx.alloc(ctx, 1));
+  DMO_CUDA(cudaMemsetAsync(mx.p, 0, sizeof(unsigned long long), ctx->stream));
+  DMO_LAUNCH(cmaes_sample_kernel, (unsigned)ceil_div(n * d, 256), 256, 0, parents_x, sigmas, sigma_cols, A, p_idx, z, n, d, x_out);
+  DMO_LAUNCH(absmax_kernel, (unsigned)std::min<int64_t>(ceil_div(n * d, 256), 4 * (int64_t)ctx->sm_count), 256, 0, x_out, n * d, mx.p);
+  DMO_LAUNCH(cmaes_rescale_kernel, (unsigned)ceil_div(n * d, 256), 256, 0, x_out, n, d, mx.p, xlb, xub);
+  DMO_CHECK_LAUNCH();
+  return DMO_OK;
+}
+
+int cmaes_step_z_device(dmo_ctx* ctx, const double* x_gen, const int64_t* cand_idx, const double* parents_x, const int64_t* par_idx,
+                        const double* xlb, const double* xub, const double* steps, int64_t n, int d, double* z_out) {
+  if (n == 0) return DMO_OK;
+  DMO_LAUNCH(cmaes_z_kernel, (unsigned)ceil_div(n * d, 256), 256, 0, x_gen, cand_idx, parents_x, par_idx, xlb, xub, steps, n, d, z_out);
+  DMO_CHECK_LAUNCH();
+  return DMO_OK;
+}
+
+int scale_rows_device(dmo_ctx* ctx, double* rows, int64_t row_elems, int64_t n_seg, const int64_t* seg_row, const int64_t* seg_start,
+                      const double* factors) {
+  if (n_seg == 0) return DMO_OK;
+  DMO_LAUNCH(scale_rows_kernel, (unsigned)ceil_div(n_seg * row_elems, 256), 256, 0, rows, row_elems, n_seg, seg_row, seg_start, factors);
+  DMO_CHECK_LAUNCH();
+  return DMO_OK;
+}
+
+int cmaes_update_cholesky_device(dmo_ctx* ctx, double* A, double* Ainv, double* pc, const double* z, const double* psucc, int64_t n, int d,
+                                 double cc, double ccov, double pthresh) {
+  if (n == 0) return DMO_OK;
+  DMO_LAUNCH(cmaes_cholesky_kernel, (unsigned)n, 64, 3 * d * sizeof(double), A, Ainv, pc, z, psucc, n, d, cc, ccov, pthresh);
+  DMO_CHECK_LAUNCH();
+  return DMO_OK;
+}
+
 extern "C" {
 
 int dmo_gather_rows(dmo_ctx* ctx, const double* src, const double* alt, const uint8_t* sel, const int64_t* idx, int64_t n,
@@ -346,8 +392,7 @@ int dmo_gather_rows(dmo_ctx* ctx, const double* src, const double* alt, const ui
   In<uint8_t> is;
   DMO_TRY(ii.init(ctx, idx, (size_t)n));
   DMO_TRY(is.init(ctx, sel, (size_t)n));
-  DMO_LAUNCH(gather_rows_kernel, (unsigned)ceil_div(n * row_elems, 256), 256, 0, src, alt, is.d, ii.d, n, row_elems, dst);
-  DMO_CHECK_LAUNCH();
+  DMO_TRY(gather_rows_device(ctx, src, alt, is.d, ii.d, n, row_elems, dst));
   DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
@@ -467,7 +512,6 @@ int dmo_cmaes_generate(dmo_ctx* ctx, const double* parents_x, const double* sigm
   In<double> ipx, isg, iA, iz, ilb, iub;
   In<int64_t> ipi;
   Out<double> oo;
-  DevBuf<unsigned long long> mx;
   DMO_TRY(ipx.init(ctx, parents_x, (size_t)n_parents * d));
   DMO_TRY(isg.init(ctx, sigmas, (size_t)n_parents * sigma_cols));
   DMO_TRY(iA.init(ctx, A, (size_t)n_parents * d * d));
@@ -476,13 +520,7 @@ int dmo_cmaes_generate(dmo_ctx* ctx, const double* parents_x, const double* sigm
   DMO_TRY(ilb.init(ctx, xlb, (size_t)d));
   DMO_TRY(iub.init(ctx, xub, (size_t)d));
   DMO_TRY(oo.init(ctx, x_out, (size_t)n * d));
-  DMO_TRY(mx.alloc(ctx, 1));
-  DMO_CUDA(cudaMemsetAsync(mx.p, 0, sizeof(unsigned long long), ctx->stream));
-  DMO_LAUNCH(cmaes_sample_kernel, (unsigned)ceil_div(n * d, 256), 256, 0, ipx.d, isg.d, sigma_cols, iA.d, ipi.d, iz.d, n, d,
-             oo.d);
-  DMO_LAUNCH(absmax_kernel, (unsigned)std::min<int64_t>(ceil_div(n * d, 256), 4 * (int64_t)ctx->sm_count), 256, 0, oo.d, n * d, mx.p);
-  DMO_LAUNCH(cmaes_rescale_kernel, (unsigned)ceil_div(n * d, 256), 256, 0, oo.d, n, d, mx.p, ilb.d, iub.d);
-  DMO_CHECK_LAUNCH();
+  DMO_TRY(cmaes_generate_device(ctx, ipx.d, isg.d, sigma_cols, iA.d, ipi.d, iz.d, n, d, ilb.d, iub.d, oo.d));
   DMO_TRY(oo.finish(ctx));
   DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
@@ -503,8 +541,7 @@ int dmo_cmaes_step_z(dmo_ctx* ctx, const double* x_gen, const int64_t* cand_idx,
   DMO_TRY(ipi.init(ctx, par_idx, (size_t)n));
   DMO_TRY(ilb.init(ctx, xlb, (size_t)d));
   DMO_TRY(iub.init(ctx, xub, (size_t)d));
-  DMO_LAUNCH(cmaes_z_kernel, (unsigned)ceil_div(n * d, 256), 256, 0, x_gen, ici.d, parents_x, ipi.d, ilb.d, iub.d, steps, n, d, z_out);
-  DMO_CHECK_LAUNCH();
+  DMO_TRY(cmaes_step_z_device(ctx, x_gen, ici.d, parents_x, ipi.d, ilb.d, iub.d, steps, n, d, z_out));
   DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
@@ -521,8 +558,7 @@ int dmo_scale_rows(dmo_ctx* ctx, double* rows, int64_t row_elems, int64_t n_seg,
   DMO_TRY(isr.init(ctx, seg_row, (size_t)n_seg));
   DMO_TRY(iss.init(ctx, seg_start, (size_t)n_seg + 1));
   DMO_TRY(ifa.init(ctx, factors, (size_t)n_factors));
-  DMO_LAUNCH(scale_rows_kernel, (unsigned)ceil_div(n_seg * row_elems, 256), 256, 0, rows, row_elems, n_seg, isr.d, iss.d, ifa.d);
-  DMO_CHECK_LAUNCH();
+  DMO_TRY(scale_rows_device(ctx, rows, row_elems, n_seg, isr.d, iss.d, ifa.d));
   DMO_CUDA(dmo_wait(ctx));
   return DMO_OK;
 }
@@ -551,9 +587,7 @@ int dmo_cmaes_update_cholesky(dmo_ctx* ctx, double* A, double* Ainv, double* pc,
   In<double> iz, ips;
   DMO_TRY(iz.init(ctx, z, (size_t)n * d));
   DMO_TRY(ips.init(ctx, psucc, (size_t)n));
-  DMO_LAUNCH(cmaes_cholesky_kernel, (unsigned)n, 64, 3 * d * sizeof(double), pA, pB, ppc, iz.d, ips.d, n, d, cc, ccov,
-             pthresh);
-  DMO_CHECK_LAUNCH();
+  DMO_TRY(cmaes_update_cholesky_device(ctx, pA, pB, ppc, iz.d, ips.d, n, d, cc, ccov, pthresh));
   if (hostA) {
     DMO_CUDA(cudaMemcpyAsync(A, pA, (size_t)n * d * d * 8, cudaMemcpyDeviceToHost, ctx->stream));
     DMO_CUDA(cudaMemcpyAsync(Ainv, pB, (size_t)n * d * d * 8, cudaMemcpyDeviceToHost, ctx->stream));

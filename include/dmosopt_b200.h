@@ -636,6 +636,47 @@ int dmo_scale_rows(dmo_ctx* ctx, double* rows, int64_t row_elems, int64_t n_seg,
  * sel (n,) uint8 (may be NULL, then alt is ignored) may be host arrays. */
 int dmo_gather_rows(dmo_ctx* ctx, const double* src, const double* alt, const uint8_t* sel, const int64_t* idx,
                     int64_t n, int64_t row_elems, double* dst);
+/* One generation of MOASMO.optimize's surrogate epoch for MO-CMA-ES (dmosopt/MOASMO.py:105-116) on the resident parent
+ * state, in two calls with the host's scalar arithmetic between them; together they give the plugin's generate ->
+ * evaluate -> update bit for bit.  C = n_off = lambda*mu offspring, pop parents, n = C + pop candidates.
+ * dmo_cmaes_step_record:
+ *   1. the parents' non-dominated rank (dmo_rank_nd of parents_y), its stable order, and p_idx[i] = order[js[i]]
+ *      (CMAES.py:241-262); js (C,) int64 HOST, each in [0, min(mu, pop));
+ *   2. the offspring of dmo_cmaes_generate from the host's normals arz (C, d), into cand_x (C, d) DEVICE;
+ *   3. their posterior mean, given by kind and handle as in dmo_smpso_step_record (var_route_mean, mean_f32, draw_seed /
+ *      draw_stream), into rows [0, C) of cand_y (n, M) DEVICE; rows [C, n) receive parents_y (pop, M) DEVICE;
+ *   4. x_gen (C, d) and y_gen (C, M) receive the offspring and their mean (the record);
+ *   5. the candidates' rank into cand_rank (n,) int32 DEVICE and CMAES._select: the whole fronts that fit in pop, in
+ *      candidate order (the reference's order_inv mapping, CMAES.py:190, makes front r the rows [b_r, b_r+1) of the
+ *      cumulative front sizes b), then k more rows of the mid front by hypervolume improvement against the chosen rows
+ *      with ref = max(candidates) + 1 (rounded to float32 when cand_f32, the plugin's float32 candidates), or its
+ *      first k rows when nothing was chosen before it;
+ *   6. codes (n,) uint8 (1 chosen, 0 not chosen) and p_idx (C,) int64.
+ *   The host waits inside the ranks and the predict, once for the front cut and once inside the selection.  Into device
+ *   or page-locked memory the outputs are enqueued without a wait and are complete after dmo_synchronize(ctx).
+ * dmo_cmaes_step_apply: update_strategy's device work (CMAES.py:300-411), without a host wait:
+ *   the n_off chosen offspring (candidate rows off_cand < C, parents off_par) take their parent's strategy rows, step
+ *   sizes scaled by off_fac, and updateCholesky with z of dmo_cmaes_step_z and off_psucc; the parents' step sizes take
+ *   the event factors ev_fac in segments (seg_row, seg_start) as dmo_scale_rows does, in place on sigmas; row i of the
+ *   next parent set is candidate next_cand[i]: an offspring brings its x_gen row and its updated strategy rows
+ *   next_src[i] < n_off, a parent its own rows (strategy rows next_src[i] < pop); parents_y and rank are the candidates'.
+ *   The outputs are DEVICE arrays distinct from the inputs (the other half of a double buffer); the index and factor
+ *   arrays are HOST arrays.
+ * Refused with DMO_ERR_ARG before any launch: a posterior as dmo_smpso_step_record refuses it, state, candidates or
+ * outputs off the device, js or the index arrays on the device, an index out of range, outputs aliasing the state,
+ * a null required pointer, a bad shape (pop < 2, C < 1, d > 512, M > 16, sigma_cols other than 1 or d). */
+int dmo_cmaes_step_record(dmo_ctx* ctx, int kind, void* posterior, uint64_t draw_seed, uint64_t draw_stream, int var_route_mean,
+                          int precision, int mean_f32, int cand_f32, const double* parents_x, const double* sigmas, int sigma_cols,
+                          const double* A, const double* parents_y, int64_t pop, int d, int M, const double* arz, const int64_t* js,
+                          int64_t n_off, int64_t mu, const double* xlb, const double* xub, double* cand_x, double* cand_y,
+                          int32_t* cand_rank, double* x_gen, double* y_gen, uint8_t* codes, int64_t* p_idx);
+int dmo_cmaes_step_apply(dmo_ctx* ctx, const double* parents_x, double* sigmas, int sigma_cols, const double* A, const double* Ainv,
+                         const double* pc, int64_t pop, int d, int M, const double* cand_x, const double* cand_y, const int32_t* cand_rank,
+                         int64_t n_cand_off, int64_t n_off, const int64_t* off_cand, const int64_t* off_par, const double* off_psucc,
+                         const double* off_fac, int64_t n_seg, const int64_t* seg_row, const int64_t* seg_start, const double* ev_fac,
+                         const int64_t* next_cand, const int64_t* next_src, const double* xlb, const double* xub, double cc, double ccov,
+                         double pthresh, double* parents_x_out, double* sigmas_out, double* A_out, double* Ainv_out, double* pc_out,
+                         double* parents_y_out, int32_t* rank_out);
 
 /* ---- N4: vectorised benchmark objective functions --------------------------------------------
  * replaces the row-at-a-time Python functions of dmosopt/benchmarks/moo_benchmarks.py (dtlz1 :21, dtlz2 :59,

@@ -6,7 +6,8 @@
 
 NSGA2 (distance_metric=None, as MOASMO.epoch builds it) with a GPR_Matern surrogate (precision "auto", the
 hyper-parameters kept at their initial values) fitted on DTLZ2 data; --optimizer SMPSO runs SMPSO with --swarm-size
-swarms of --pop particles instead (2 * swarm_size * pop candidates per generation); the training set is the epoch's ``initial`` rows, as
+swarms of --pop particles instead (2 * swarm_size * pop candidates per generation), --optimizer CMAES runs MO-CMA-ES with
+its default parameters (mu = pop // 2, lambda_ = 1: pop // 2 offspring per generation); the training set is the epoch's ``initial`` rows, as
 MOASMO.epoch passes it.  --surrogate EGP_Matern, SVGP_Matern, VGP_Matern, SIV_Matern, SPV_Matern, MDSPP_Matern or
 MDGP_Matern (--precision fp64 or tensor) builds that class from seeded hyper-parameters instead, with no training: EGP
 with one length scale per objective, the variational classes with their own inducing-point rule (SVGP: 0.2 N points per
@@ -134,6 +135,8 @@ def epoch(fn, sm, X, Y, a, evaluate=None):
     model = b2.Model(objective=sm)
     if a.optimizer == "SMPSO":
         opt = b2.SMPSO(popsize=a.pop, nInput=a.d, nOutput=a.M, model=model, distance_metric=None, swarm_size=a.swarm_size)
+    elif a.optimizer == "CMAES":
+        opt = b2.CMAES(popsize=a.pop, nInput=a.d, nOutput=a.M, model=model, distance_metric=None)
     else:
         opt = b2.NSGA2(popsize=a.pop, nInput=a.d, nOutput=a.M, model=model, distance_metric=None)
     xlb, xub = np.zeros(a.d), np.ones(a.d)
@@ -175,7 +178,7 @@ def main():
     ap.add_argument("--seed", type=int, default=2026)
     ap.add_argument("--surrogate", default="GPR_Matern")
     ap.add_argument("--precision", default="auto")
-    ap.add_argument("--optimizer", default="NSGA2", choices=("NSGA2", "SMPSO"))
+    ap.add_argument("--optimizer", default="NSGA2", choices=("NSGA2", "SMPSO", "CMAES"))
     ap.add_argument("--swarm-size", type=int, default=5)
     a = ap.parse_args()
 
